@@ -252,21 +252,32 @@ def test_specialised_functions_agree():
 
 
 def test_ragged_ts_interpolation_and_reuse():
-    """Output times that are not multiples of dt (linear_interp, interp.py:15-18) and a second
-    solve on the same bm with a coarser, nested grid."""
+    """Output times that are not multiples of dt (linear_interp, interp.py:15-18) and later solves on the same bm
+    with a coarser, nested grid: each coarse step merges 8 bound cells in the kernel (n_cells > 1, cell lengths read
+    from the device, and for SRK the H-merge rule).  Both against the oracle, which merges the same cells."""
     tsde = _tsde()
     dev = torch.device('cuda')
     B, D = 16, 4
     sde = problems.GBMDiagonal(D, 'ito', seed=4, dtype=torch.float64).to(dev)
+    sde_cpu = problems.GBMDiagonal(D, 'ito', seed=4, dtype=torch.float64)
     y0 = torch.full((B, D), 0.5, dtype=torch.float64, device=dev)
-    bm = tsde.BrownianInterval(0., 1., size=(B, D), dtype=torch.float64, device=dev, entropy=3)
-    fine = tsde.sdeint(sde, y0, torch.linspace(0, 1, 7, dtype=torch.float64, device=dev), bm=bm, method='euler',
-                       dt=2.0 ** -6)
-    assert fine.shape == (7, B, D) and torch.isfinite(fine).all()
+    bm = tsde.BrownianInterval(0., 1., size=(B, D), dtype=torch.float64, device=dev, entropy=3,
+                               levy_area_approximation='space-time')
+    ts = np.linspace(0, 1, 7)
+    fine = tsde.sdeint(sde, y0, torch.from_numpy(ts).to(dev), bm=bm, method='euler', dt=2.0 ** -6)
+    assert fine.shape == (7, B, D)
+    oracle_bm = _oracle_bm_from(bm, B, D, np.float64, True)
+    ref, _ = solvers.make('euler', problems.NumpySDE(sde_cpu), oracle_bm, 2.0 ** -6).integrate(y0.cpu().numpy(), ts)
+    np.testing.assert_allclose(fine.cpu().numpy(), ref, rtol=1e-11, atol=1e-12)
     # coarser nested grid re-uses the same cells (merged): the Brownian path is the same object
     w_all = bm(0.0, 1.0)
-    coarse = tsde.sdeint(sde, y0, [0.0, 1.0], bm=bm, method='euler', dt=2.0 ** -3)
-    assert torch.isfinite(coarse).all()
+    ts = np.array([0.0, 0.3, 0.55, 0.8, 1.0])
+    for method in ('euler', 'srk'):
+        with torch.no_grad():  # the fused step kernels
+            coarse = tsde.sdeint(sde, y0, torch.from_numpy(ts).to(dev), bm=bm, method=method, dt=2.0 ** -3)
+        ref, _ = solvers.make(method, problems.NumpySDE(sde_cpu), oracle_bm, 2.0 ** -3).integrate(
+            y0.cpu().numpy(), ts)
+        np.testing.assert_allclose(coarse.cpu().numpy(), ref, rtol=1e-11, atol=1e-12, err_msg=method)
     s = sum(bm(k / 8, (k + 1) / 8) for k in range(8))
     torch.testing.assert_close(s, w_all, rtol=1e-12, atol=1e-13)
 

@@ -451,6 +451,24 @@ def test_c_client_of_the_abi(tmp_path):
     assert r.returncode == 0 and 'c client ok, abi 1' in r.stdout, (r.returncode, r.stdout, r.stderr)
 
 
+def test_fast_kernel_row_division_is_exact(tmp_path):
+    """The row-wise fast kernel finds the row of quad Q as Q / qpr by a multiply-high with a 64-bit reciprocal
+    (csrc/rowdiv.cuh) when quads per row is not a power of two.  tests/c/rowdiv_check.cu compiles that same helper
+    for the host and checks row and quad against plain division: every qpr in 3..4096 and a sample up to 2^31, at the
+    row boundaries around 2^24 (where a 2^40 reciprocal wraps 64 bits), 2^31 / qpr and the last row of 32-bit Q."""
+    import shutil
+    import subprocess
+    nvcc = next((c for c in (os.environ.get('NVCC'), '/usr/local/cuda/bin/nvcc', shutil.which('nvcc'))
+                 if c and os.path.exists(c)), None)
+    if nvcc is None:
+        pytest.skip("no nvcc")
+    exe = str(tmp_path / 'rowdiv_check')
+    subprocess.run([nvcc, '-std=c++17', '-O2', '-Wno-deprecated-gpu-targets',
+                    os.path.join(ROOT, 'tests', 'c', 'rowdiv_check.cu'), '-o', exe], check=True)
+    r = subprocess.run([exe], capture_output=True, text=True)
+    assert r.returncode == 0 and ' 0 mismatches' in r.stdout, (r.returncode, r.stdout[-2000:], r.stderr[-600:])
+
+
 def test_bench_clock_sampler_reports_the_timed_window_only():
     """bench.py starts `nvidia-smi -lms` before the warm-up (so that its start-up does not run against the first timed
     steps) and reports only samples taken after `mark()`; throttle reasons outside the window do not count, an empty

@@ -19,6 +19,7 @@
 
 #include "../../include/torchsde_b200.h"
 #include "philox.cuh"
+#include "rowdiv.cuh"
 
 namespace tsde {
 
@@ -111,7 +112,7 @@ struct EwP {
   int32_t vec;     // all pointers 16B-aligned and d % 4 == 0
   int32_t qshift;  // log2(qpr) if qpr is a power of two, else -1
   int32_t small;   // nquads < 2^31: 32-bit index arithmetic
-  uint64_t qmagic; // ceil(2^40 / qpr): row = (Q * qmagic) >> 40, exact while Q * qpr < 2^40
+  uint64_t qmagic; // rowdiv_magic(qpr) = ceil(2^64 / qpr): row = umulhi(Q, qmagic), exact for every 32-bit Q
 };
 
 // ---- vector load / store helpers ---------------------------------------------------------
@@ -332,7 +333,8 @@ ew_kernel(const EwP<Op::NIN, Op::NOUT> p, const NoiseP<T> nz, const Op op) {
 
 // ---- fast variant: the shapes the headline path uses -------------------------------------------
 // Preconditions checked on the host: 128-bit aligned tensors with d % 4 == 0 (vector path), noise not
-// broadcast, quads-per-row a power of two (or divisible by multiply-shift), fewer than 2^31 quads.
+// broadcast, fewer than 2^31 quads.  The row of a quad is a shift when quads-per-row is a power of two, else a
+// multiply-high by a 64-bit reciprocal (rowdiv.cuh), exact for every 32-bit quad index.
 // Everything is 32-bit index arithmetic and there is no per-quad branching.
 //
 // (Tried and rejected: software-pipelining the integer half of iteration i+1's noise (Philox) next to the float
@@ -358,10 +360,10 @@ struct FastCtx {
   uint64_t qmagic;
   bool pow2, stream_hint;
   __device__ __forceinline__ uint32_t row_of(uint32_t Q) const {
-    return pow2 ? (Q >> qshift) : (uint32_t)(((uint64_t)Q * qmagic) >> 40);
+    return pow2 ? (Q >> qshift) : rowdiv_row(Q, qmagic);
   }
   __device__ __forceinline__ uint32_t quad_of(uint32_t Q, uint32_t row) const {
-    return pow2 ? (Q & qmask) : (Q - row * qpr32);
+    return pow2 ? (Q & qmask) : rowdiv_quad(Q, row, qpr32);
   }
   __device__ __forceinline__ void rng(uint32_t Q, T (&w)[4], T (&u)[4]) const {
     const uint32_t r = row_of(Q);
@@ -533,7 +535,7 @@ inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
     p.qshift = sh;
   }
   p.small = p.nquads < (1ll << 31) ? 1 : 0;
-  p.qmagic = ((1ull << 40) + (uint64_t)p.qpr - 1) / (uint64_t)p.qpr;
+  p.qmagic = p.qshift < 0 ? rowdiv_magic((uint64_t)p.qpr) : 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
   bool pdl = false;
   auto go = [&](auto kernel) -> int {
@@ -559,8 +561,8 @@ inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
     kernel<<<(unsigned)blocks, kThreads, 0, st>>>(p, np, op);
     return (int)cudaGetLastError();
   };
-  const bool divisible = p.qshift >= 0 || (p.nquads * p.qpr < (1ll << 40) && p.qpr < (1ll << 20));
-  const bool fast = p.vec && !bcast && divisible && p.small && np.n_cells == 1 &&
+  // (every quads-per-row divides exactly on the fast path: its quad indices are 32-bit, see rowdiv.cuh)
+  const bool fast = p.vec && !bcast && p.small && np.n_cells == 1 &&
                     (L->rows + (nz ? nz->row_offset : 0)) < 0xFFFFFFFFll;
   pdl = fast && pdl_enabled();
   if constexpr (!Op::USES_NOISE) {
