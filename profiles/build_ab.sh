@@ -4,7 +4,7 @@
 # at run time with TORCHSDE_B200_LIB.
 set -e
 cd "$(dirname "$0")/.."
-F="-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -fmad=false -Xcompiler -fPIC"
+F="-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -fmad=false -Xcompiler -fPIC -Xcompiler -fvisibility=hidden"
 mkdir -p /tmp/ab profiles/_ab
 rm -f profiles/_ab/*.so
 for s in cabi tableau_diag tableau_general logode; do nvcc $F -c torchsde_b200/csrc/$s.cu -o /tmp/ab/$s.o & done

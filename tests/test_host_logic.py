@@ -36,6 +36,21 @@ def test_cabi_loads_and_exports_every_declared_symbol():
     assert _cabi.lib().tsde_abi_version() == 1
 
 
+def test_cabi_exports_only_the_declared_symbols():
+    """The library is compiled with hidden visibility: its dynamic symbol table holds the functions of
+    include/torchsde_b200.h and nothing else (no kernel stubs, internal C++ functions or template instantiations)."""
+    import shutil
+    import subprocess
+    nm = shutil.which('nm')
+    if nm is None:
+        pytest.skip("no nm")
+    _cabi.lib()  # make sure the library is built
+    out = subprocess.run([nm, '-D', '--defined-only', _cabi.LIB_PATH], capture_output=True, text=True,
+                         check=True).stdout
+    exported = sorted(line.split()[-1] for line in out.splitlines() if line.strip())
+    assert exported == _declared_symbols()
+
+
 def test_struct_layout_matches_header():
     assert ctypes.sizeof(_cabi.Launch) == 40
     assert ctypes.sizeof(_cabi.Noise) == 80

@@ -81,40 +81,36 @@ struct CellsOp {
   }
 };
 
-static inline unsigned grid_for(int64_t nquads) {
-  int64_t blocks = (nquads + kThreads - 1) / kThreads;
-  const int64_t cap = (int64_t)sm_count() * kBlocksPerSM;
-  return (unsigned)(blocks > cap ? cap : blocks);
+// The Brownian tensors are (rows, m); reuse the row-wise framework with d := m.
+static tsde_launch as_rows_m(const tsde_launch* L) {
+  tsde_launch r = *L;
+  r.d = L->m;
+  r.noise_type = TSDE_NOISE_DIAGONAL;
+  return r;
 }
 
 template <typename T>
 static int cells_impl(const tsde_launch* L, const tsde_noise* nz, void* out_w, void* out_u,
                       void* out_h) {
   if (!nz || nz->source != TSDE_SRC_COUNTER || !out_w) return TSDE_EINVAL;
+  if (!out_h) {
+    const tsde_launch r = as_rows_m(L);
+    tsde_noise z = *nz;
+    if (out_u) {
+      z.want_u = 1;
+      void* outs[2] = {out_w, out_u};
+      return launch_ew<T>(&r, &z, false, nullptr, outs, CellsOp<T, true>{});
+    }
+    void* outs[1] = {out_w};
+    return launch_ew<T>(&r, &z, false, nullptr, outs, CellsOp<T, false>{});
+  }
   NoiseP<T> np;
   if (int e = fill_noise<T>(L, nz, false, np)) return e;
   const int64_t m = L->m, rows = L->rows, qpr = (m + 3) / 4, nquads = rows * qpr;
-  if (nquads == 0) return 0;
-  if (rows + nz->row_offset > 0xFFFFFFFFll) return TSDE_EINVAL;
-  const bool vec = (m % 4 == 0) && aligned16(out_w) && (!out_u || aligned16(out_u)) &&
-                   (!out_h || aligned16(out_h));
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
-  if (out_h) {
-    cells_wh_kernel<T><<<grid_for(nquads), kThreads, 0, st>>>(np, rows, m, qpr, vec, (T*)out_w,
-                                                             (T*)out_u, (T*)out_h);
-    return (int)cudaGetLastError();
-  }
-  tsde_launch r = *L;
-  r.d = m;
-  r.noise_type = TSDE_NOISE_DIAGONAL;
-  tsde_noise z = *nz;
-  if (out_u) {
-    z.want_u = 1;
-    void* outs[2] = {out_w, out_u};
-    return launch_ew<T, CellsOp<T, true>>(&r, &z, false, nullptr, outs, CellsOp<T, true>{});
-  }
-  void* outs[1] = {out_w};
-  return launch_ew<T, CellsOp<T, false>>(&r, &z, false, nullptr, outs, CellsOp<T, false>{});
+  const bool vec = (m % 4 == 0) && aligned16(out_w) && (!out_u || aligned16(out_u)) && aligned16(out_h);
+  return launch_kernel(cells_wh_kernel<T>, capped_grid(nquads, kThreads, kBlocksPerSM), kThreads, 0,
+                       reinterpret_cast<cudaStream_t>(L->stream), false, np, rows, m, qpr, vec, (T*)out_w,
+                       (T*)out_u, (T*)out_h);
 }
 
 // ---- Brownian bridge descent ------------------------------------------------------------------
@@ -188,11 +184,11 @@ static int bridge_impl(const tsde_launch* L, const void* key, int64_t row_offset
   const bool have_h = in_h != nullptr;
   if (have_h && !out_h) return TSDE_EINVAL;
   const int64_t m = L->m, rows = L->rows, qpr = (m + 3) / 4, nquads = rows * qpr;
-  if (nquads == 0) return 0;
-  if (rows + row_offset > 0xFFFFFFFFll) return TSDE_EINVAL;
+  if (rows + row_offset > kMaxGlobalRows) return TSDE_EINVAL;
   const bool vec = (m % 4 == 0) && aligned16(in_w) && aligned16(out_w) &&
                    (!have_h || (aligned16(in_h) && aligned16(out_h)));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
+  const auto kernel = have_h ? bridge_kernel<T, true> : bridge_kernel<T, false>;
   const void* cur_w = in_w;
   const void* cur_h = in_h;
   int done = 0;
@@ -232,19 +228,15 @@ static int bridge_impl(const tsde_launch* L, const void* key, int64_t row_offset
         lv.k[3] = is_left[i] ? 1.0 : 0.0;
       }
     }
-    if (have_h) {
-      bridge_kernel<T, true><<<grid_for(nquads), kThreads, 0, st>>>(
-          bp, key, row_offset, rows, m, qpr, vec, (const T*)cur_w, (const T*)cur_h, (T*)out_w,
-          (T*)out_h);
-    } else {
-      bridge_kernel<T, false><<<grid_for(nquads), kThreads, 0, st>>>(
-          bp, key, row_offset, rows, m, qpr, vec, (const T*)cur_w, nullptr, (T*)out_w, nullptr);
-    }
+    if (int e = launch_kernel(kernel, capped_grid(nquads, kThreads, kBlocksPerSM), kThreads, 0, st, false, bp, key,
+                              row_offset, rows, m, qpr, vec, (const T*)cur_w, (const T*)cur_h, (T*)out_w,
+                              (T*)out_h))
+      return e;
     done += n;
     cur_w = out_w;  // further chunks continue in place
     cur_h = out_h;
   } while (done < depth);
-  return (int)cudaGetLastError();
+  return 0;
 }
 
 // ---- merges ------------------------------------------------------------------------------------
@@ -633,24 +625,17 @@ static int launch_levy_tiles(const tsde_launch* L, const void* key, int64_t row_
   if (warps < 1) return kLevyNoTile;
   const size_t smem = table + (size_t)warps * tile;
   const int vec = (m % 4 == 0 && aligned16(out_a)) ? 1 : 0;   // groups of 4 consecutive columns of one row
+  const auto kernel = m == 16 ? levy_tile_kernel<T, GEN, 16>
+                      : m == 8 ? levy_tile_kernel<T, GEN, 8>
+                               : levy_tile_kernel<T, GEN, 0>;
   // persistent: exactly the CTAs that are resident at once (one wave), rows strided over them
-#define TSDE_LEVY_LAUNCH(MT)                                                                                         \
-  int per_sm = 0;                                                                                                    \
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, levy_tile_kernel<T, GEN, MT>, kLevyWarps * 32, smem) != \
-          cudaSuccess || per_sm < 1)                                                                                 \
-    per_sm = 1;                                                                                                      \
-  const int64_t per_cta = (int64_t)warps * levy_group_rows((int)m, GEN);                                             \
-  int64_t blocks = (L->rows + per_cta - 1) / per_cta;                                                                \
-  if (blocks > (int64_t)sm_count() * per_sm) blocks = (int64_t)sm_count() * per_sm;                                  \
-  levy_tile_kernel<T, GEN, MT><<<(unsigned)blocks, kLevyWarps * 32, smem, st>>>(                                     \
-      key, row_offset, a_id, L->rows, (int)m, warps, (const T*)w, (const T*)hh, (T)(0.1 * h),                        \
-      (T)sqrt((1.0 / 12.0) * h * h), foster, (T*)out_a, vec, cell_id, (T)sqrt(h), (T)sqrt(h / 12.0), (T)h,           \
-      (T*)out_w, (T*)out_u)
-  if (m == 16) { TSDE_LEVY_LAUNCH(16); }
-  else if (m == 8) { TSDE_LEVY_LAUNCH(8); }
-  else { TSDE_LEVY_LAUNCH(0); }
-#undef TSDE_LEVY_LAUNCH
-  return (int)cudaGetLastError();
+  int per_sm = resident_ctas(reinterpret_cast<const void*>(kernel), kLevyWarps * 32, smem);
+  if (per_sm < 1) per_sm = 1;
+  const int64_t per_cta = (int64_t)warps * levy_group_rows((int)m, GEN);
+  return launch_kernel(kernel, capped_grid(L->rows, per_cta, per_sm), kLevyWarps * 32, smem, st, false, key,
+                       row_offset, a_id, L->rows, (int)m, warps, (const T*)w, (const T*)hh, (T)(0.1 * h),
+                       (T)sqrt((1.0 / 12.0) * h * h), foster, (T*)out_a, vec, cell_id, (T)sqrt(h), (T)sqrt(h / 12.0),
+                       (T)h, (T*)out_w, (T*)out_u);
 }
 
 // One launch for a whole-cell query with Levy area: W, U and A of primary cell nz->cell_id.
@@ -661,8 +646,7 @@ static int cell_levy_impl(const tsde_launch* L, const tsde_noise* nz, uint64_t a
     return TSDE_EINVAL;
   const int64_t m = L->m;
   if (m < 4 || m > 64 || (m % 4) != 0 || !aligned16(out_w) || !aligned16(out_u)) return TSDE_EINVAL;
-  if (L->rows == 0) return 0;
-  if (L->rows + nz->row_offset > 0xFFFFFFFFll) return TSDE_EINVAL;
+  if (L->rows + nz->row_offset > kMaxGlobalRows) return TSDE_EINVAL;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
   const int rc = launch_levy_tiles<T, true>(L, nz->key, nz->row_offset, a_id, nullptr, nullptr, nz->h, foster, out_a,
                                             nz->cell_id, out_w, out_u, st);
@@ -673,9 +657,7 @@ template <typename T>
 static int levy_impl(const tsde_launch* L, const void* key, int64_t row_offset, uint64_t a_id,
                      const void* w, const void* hh, double h, int32_t foster, void* out_a) {
   if (!key || !w || !hh || !out_a) return TSDE_EINVAL;
-  const int64_t total = L->rows * L->m * L->m;
-  if (total == 0) return 0;
-  if (L->rows + row_offset > 0xFFFFFFFFll) return TSDE_EINVAL;
+  if (L->rows + row_offset > kMaxGlobalRows) return TSDE_EINVAL;
   if (L->m * L->m > (1ll << 26)) return TSDE_EINVAL;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
   const double r12 = 1.0 / 12.0;
@@ -684,107 +666,76 @@ static int levy_impl(const tsde_launch* L, const void* key, int64_t row_offset, 
     const int rc = launch_levy_tiles<T, false>(L, key, row_offset, a_id, w, hh, h, foster, out_a, 0, nullptr, nullptr, st);
     if (rc != kLevyNoTile) return rc;
   }
-  levy_area_kernel<T><<<grid_for(total), kThreads, 0, st>>>(
-      key, row_offset, a_id, L->rows, L->m, (const T*)w, (const T*)hh, (T)(0.1 * h),
-      (T)sqrt(r12 * h * h), foster, (T*)out_a);
-  return (int)cudaGetLastError();
+  return launch_kernel(levy_area_kernel<T>, capped_grid(L->rows * m * m, kThreads, kBlocksPerSM), kThreads, 0, st,
+                       false, key, row_offset, a_id, L->rows, m, (const T*)w, (const T*)hh, (T)(0.1 * h),
+                       (T)sqrt(r12 * h * h), foster, (T*)out_a);
 }
 
 template <typename T>
 static int merge_area_impl(const tsde_launch* L, void* a0, const void* a1, const void* w0,
                            const void* w1) {
   if (!a0 || !a1 || !w0 || !w1) return TSDE_EINVAL;
-  const int64_t total = L->rows * L->m * L->m;
-  if (total == 0) return 0;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
-  merge_area_kernel<T><<<grid_for(total), kThreads, 0, st>>>(L->rows, L->m, (T*)a0, (const T*)a1,
-                                                           (const T*)w0, (const T*)w1);
-  return (int)cudaGetLastError();
+  return launch_kernel(merge_area_kernel<T>, capped_grid(L->rows * L->m * L->m, kThreads, kBlocksPerSM), kThreads,
+                       0, reinterpret_cast<cudaStream_t>(L->stream), false, L->rows, L->m, (T*)a0, (const T*)a1,
+                       (const T*)w0, (const T*)w1);
 }
 
 
-extern "C" {
-
-int tsde_brownian_cells(const tsde_launch* L, const tsde_noise* nz, void* out_w, void* out_u,
-                        void* out_h) {
-  return TSDE_DISPATCH_DTYPE(L, cells_impl<float>(L, nz, out_w, out_u, out_h),
-                             cells_impl<double>(L, nz, out_w, out_u, out_h));
+TSDE_EXPORT int tsde_brownian_cells(const tsde_launch* L, const tsde_noise* nz, void* out_w, void* out_u,
+                                    void* out_h) {
+  return dispatch(L, [&](auto t) { return cells_impl<decltype(t)>(L, nz, out_w, out_u, out_h); });
 }
 
-int tsde_brownian_cell_levy(const tsde_launch* L, const tsde_noise* nz, uint64_t a_id, int32_t foster, void* out_w,
-                            void* out_u, void* out_a) {
-  return TSDE_DISPATCH_DTYPE(L, cell_levy_impl<float>(L, nz, a_id, foster, out_w, out_u, out_a),
-                             cell_levy_impl<double>(L, nz, a_id, foster, out_w, out_u, out_a));
+TSDE_EXPORT int tsde_brownian_cell_levy(const tsde_launch* L, const tsde_noise* nz, uint64_t a_id, int32_t foster,
+                                        void* out_w, void* out_u, void* out_a) {
+  return dispatch(L, [&](auto t) { return cell_levy_impl<decltype(t)>(L, nz, a_id, foster, out_w, out_u, out_a); });
 }
 
-int tsde_brownian_bridge(const tsde_launch* L, const void* key, int64_t row_offset, int32_t depth,
-                         const uint64_t* ids, const int32_t* is_left, const double* times,
-                         const void* in_w, const void* in_h, void* out_w, void* out_h) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      bridge_impl<float>(L, key, row_offset, depth, ids, is_left, times, in_w, in_h, out_w, out_h),
-      bridge_impl<double>(L, key, row_offset, depth, ids, is_left, times, in_w, in_h, out_w,
-                          out_h));
+TSDE_EXPORT int tsde_brownian_bridge(const tsde_launch* L, const void* key, int64_t row_offset, int32_t depth,
+                                     const uint64_t* ids, const int32_t* is_left, const double* times,
+                                     const void* in_w, const void* in_h, void* out_w, void* out_h) {
+  return dispatch(L, [&](auto t) {
+    return bridge_impl<decltype(t)>(L, key, row_offset, depth, ids, is_left, times, in_w, in_h, out_w, out_h);
+  });
 }
 
-// The Brownian tensors are (rows, m); reuse the row-wise framework with d := m.
-static tsde_launch as_rows_m(const tsde_launch* L) {
-  tsde_launch r = *L;
-  r.d = L->m;
-  r.noise_type = TSDE_NOISE_DIAGONAL;
-  return r;
+TSDE_EXPORT int tsde_brownian_merge(const tsde_launch* L, void* w0, void* h0, const void* w1, const void* h1,
+                                    double len0, double len1, double tot) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    const tsde_launch r = as_rows_m(L);
+    if (h0 && h1) {
+      const void* ins[4] = {w0, h0, w1, h1};
+      void* outs[2] = {w0, h0};
+      return launch_ew<T>(&r, nullptr, false, ins, outs, MergeWHOp<T>{(T)len1, (T)len0, (T)tot});
+    }
+    const void* ins[2] = {w0, w1};
+    void* outs[1] = {w0};
+    return launch_ew<T>(&r, nullptr, false, ins, outs, AddOp<T>{});
+  });
 }
 
-int tsde_brownian_merge(const tsde_launch* L, void* w0, void* h0, const void* w1, const void* h1,
-                        double len0, double len1, double tot) {
-  if (tsde::launch_invalid(L)) return TSDE_EINVAL;
-  const tsde_launch r = as_rows_m(L);
-  if (h0 && h1) {
-    const void* ins[4] = {w0, h0, w1, h1};
-    void* outs[2] = {w0, h0};
-    return TSDE_DISPATCH_DTYPE(
-        L,
-        (launch_ew<float, MergeWHOp<float>>(
-            &r, nullptr, false, ins, outs,
-            MergeWHOp<float>{(float)len1, (float)len0, (float)tot})),
-        (launch_ew<double, MergeWHOp<double>>(&r, nullptr, false, ins, outs,
-                                              MergeWHOp<double>{len1, len0, tot})));
-  }
-  const void* ins[2] = {w0, w1};
-  void* outs[1] = {w0};
-  return TSDE_DISPATCH_DTYPE(
-      L, (launch_ew<float, AddOp<float>>(&r, nullptr, false, ins, outs, AddOp<float>{})),
-      (launch_ew<double, AddOp<double>>(&r, nullptr, false, ins, outs, AddOp<double>{})));
+TSDE_EXPORT int tsde_brownian_h_to_u(const tsde_launch* L, const void* w, const void* hh, double h, void* out_u) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    const tsde_launch r = as_rows_m(L);
+    const void* ins[2] = {w, hh};
+    void* outs[1] = {out_u};
+    return launch_ew<T>(&r, nullptr, false, ins, outs, HToUOp<T>{(T)h});
+  });
 }
 
-int tsde_brownian_h_to_u(const tsde_launch* L, const void* w, const void* hh, double h,
-                         void* out_u) {
-  if (tsde::launch_invalid(L)) return TSDE_EINVAL;
-  const tsde_launch r = as_rows_m(L);
-  const void* ins[2] = {w, hh};
-  void* outs[1] = {out_u};
-  return TSDE_DISPATCH_DTYPE(
-      L, (launch_ew<float, HToUOp<float>>(&r, nullptr, false, ins, outs, HToUOp<float>{(float)h})),
-      (launch_ew<double, HToUOp<double>>(&r, nullptr, false, ins, outs, HToUOp<double>{h})));
+TSDE_EXPORT int tsde_brownian_levy_area(const tsde_launch* L, const void* key, int64_t row_offset, uint64_t a_id,
+                                        const void* w, const void* hh, double h, int32_t foster, void* out_a) {
+  return dispatch(L, [&](auto t) {
+    return levy_impl<decltype(t)>(L, key, row_offset, a_id, w, hh, h, foster, out_a);
+  });
 }
 
-int tsde_brownian_levy_area(const tsde_launch* L, const void* key, int64_t row_offset,
-                            uint64_t a_id, const void* w, const void* hh, double h, int32_t foster,
-                            void* out_a) {
-  if (tsde::launch_invalid(L)) return TSDE_EINVAL;
-  return TSDE_DISPATCH_DTYPE(
-      L, levy_impl<float>(L, key, row_offset, a_id, w, hh, h, foster, out_a),
-      levy_impl<double>(L, key, row_offset, a_id, w, hh, h, foster, out_a));
+TSDE_EXPORT int tsde_brownian_merge_area(const tsde_launch* L, void* a0, const void* a1, const void* w0,
+                                         const void* w1) {
+  return dispatch(L, [&](auto t) { return merge_area_impl<decltype(t)>(L, a0, a1, w0, w1); });
 }
-
-int tsde_brownian_merge_area(const tsde_launch* L, void* a0, const void* a1, const void* w0,
-                             const void* w1) {
-  if (tsde::launch_invalid(L)) return TSDE_EINVAL;
-  return TSDE_DISPATCH_DTYPE(L, merge_area_impl<float>(L, a0, a1, w0, w1),
-                             merge_area_impl<double>(L, a0, a1, w0, w1));
-}
-
-}  // extern "C"
 
 // ---- adaptive step-size control: error estimate --------------------------------------------------
 // Sum over all elements of ((y11 - y12) / tol)^2 with tol = clamp_min(rtol*max(|y11|,|y12|) + atol, eps):
@@ -836,17 +787,17 @@ static int err_impl(const tsde_launch* L, const void* y11, const void* y12, doub
   cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
   int nb = (int)((n + kThreads - 1) / kThreads);
   if (nb > kErrBlocks) nb = kErrBlocks;
-  if (nb < 1) nb = 1;
-  err_partial_kernel<T><<<nb, kThreads, 0, st>>>((const T*)y11, (const T*)y12, n, (T)rtol, (T)atol, (T)eps,
-                                               (double*)scratch);
-  err_final_kernel<<<1, 32, 0, st>>>((const double*)scratch, nb, (double*)out);
-  return (int)cudaGetLastError();
+  if (int e = launch_kernel(err_partial_kernel<T>, nb, kThreads, 0, st, false, (const T*)y11, (const T*)y12, n,
+                            (T)rtol, (T)atol, (T)eps, (double*)scratch))
+    return e;
+  return launch_kernel(err_final_kernel, 1, 32, 0, st, false, (const double*)scratch, nb, (double*)out);
 }
 
 }  // namespace tsde
 
-extern "C" int tsde_adaptive_error_sumsq(const tsde_launch* L, const void* y11, const void* y12, double rtol,
-                                         double atol, double eps, void* scratch, void* out) {
-  return TSDE_DISPATCH_DTYPE(L, tsde::err_impl<float>(L, y11, y12, rtol, atol, eps, scratch, out),
-                             tsde::err_impl<double>(L, y11, y12, rtol, atol, eps, scratch, out));
+TSDE_EXPORT int tsde_adaptive_error_sumsq(const tsde_launch* L, const void* y11, const void* y12, double rtol,
+                                          double atol, double eps, void* scratch, void* out) {
+  return tsde::dispatch(L, [&](auto t) {
+    return tsde::err_impl<decltype(t)>(L, y11, y12, rtol, atol, eps, scratch, out);
+  });
 }

@@ -9,22 +9,16 @@
 // thread); the grid is one resident wave (SM count x occupancy), each CTA owning an equal
 // contiguous slice of the quads.
 #pragma once
-#include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
 
-#include <mutex>
-#include <type_traits>
-#include <unordered_map>
-
-#include "../../include/torchsde_b200.h"
+#include "host.cuh"
 #include "philox.cuh"
 #include "rowdiv.cuh"
 
 namespace tsde {
 
 constexpr int kThreads = 256;
-constexpr int kSMs = 132;        // H100 SXM; only a fallback, sm_count() asks the device
 constexpr int kBlocksPerSM = 8;  // 2048 threads / SM
 
 inline bool stream_loads_enabled() {
@@ -54,33 +48,6 @@ inline int ctas_per_sm_limit() {
     v = e ? atoi(e) : 0;
   }
   return v;
-}
-
-inline int sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = kSMs;
-  }
-  return n;
-}
-
-// Resident CTAs per SM of one kernel instantiation at kThreads threads, queried once per kernel.
-// (Keyed by the kernel's address: instantiations that differ only in a non-type template argument
-// share a function-pointer type, so a function-local static would be shared between them.)
-template <typename K>
-inline int resident_ctas(K kernel) {
-  static std::mutex mu;
-  static std::unordered_map<const void*, int> cache;
-  const void* id = reinterpret_cast<const void*>(kernel);
-  std::lock_guard<std::mutex> lock(mu);
-  auto it = cache.find(id);
-  if (it != cache.end()) return it->second;
-  int n = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, kThreads, 0) != cudaSuccess || n < 1) n = 1;
-  cache.emplace(id, n);
-  return n;
 }
 
 template <typename T>
@@ -478,6 +445,7 @@ inline int fill_noise(const tsde_launch* L, const tsde_noise* nz, bool bcast, No
   out = NoiseP<T>{};
   out.m = bcast ? 1 : L->m;
   out.bcast = bcast ? 1 : 0;
+  if (L->rows + (nz ? nz->row_offset : 0) > kMaxGlobalRows) return TSDE_EINVAL;
   if (!nz) return 0;
   out.w = reinterpret_cast<const T*>(nz->w);
   out.u = reinterpret_cast<const T*>(nz->u);
@@ -501,7 +469,6 @@ template <typename T, typename Op>
 inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
                      const void* const* ins, void* const* outs, const Op& op) {
   EwP<Op::NIN, Op::NOUT> p{};
-  if (L->rows == 0) return 0;
   bool vec = (L->d % 4) == 0;
   for (int i = 0; i < Op::NIN; ++i) {
     if (!ins[i]) return TSDE_EINVAL;
@@ -526,8 +493,6 @@ inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
   p.qpr = (L->d + 3) / 4;
   p.nquads = p.rows * p.qpr;
   p.vec = vec ? (stream_loads_enabled() ? 2 : 1) : 0;
-  if (p.nquads == 0) return 0;
-  if (L->rows + (nz ? nz->row_offset : 0) > 0xFFFFFFFFll) return TSDE_EINVAL;
   p.qshift = -1;
   if ((p.qpr & (p.qpr - 1)) == 0 && p.qpr < (1ll << 30)) {
     int sh = 0;
@@ -536,35 +501,19 @@ inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
   }
   p.small = p.nquads < (1ll << 31) ? 1 : 0;
   p.qmagic = p.qshift < 0 ? rowdiv_magic((uint64_t)p.qpr) : 0;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
-  bool pdl = false;
-  auto go = [&](auto kernel) -> int {
-    // Persistent, balanced grid: one wave of resident CTAs, each owning an equal contiguous slice.
-    int per_sm = resident_ctas(kernel);
-    if (const int lim = ctas_per_sm_limit(); lim > 0 && lim < per_sm) per_sm = lim;
-    const int64_t cap = (int64_t)sm_count() * per_sm;
-    int64_t blocks = (p.nquads + kThreads - 1) / kThreads;  // small problems: one quad per thread
-    if (blocks > cap) blocks = cap;                          // large: one resident wave, sliced evenly
-    if (pdl) {
-      cudaLaunchConfig_t cfg{};
-      cfg.gridDim = dim3((unsigned)blocks);
-      cfg.blockDim = dim3(kThreads);
-      cfg.dynamicSmemBytes = 0;
-      cfg.stream = st;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[0].val.programmaticStreamSerializationAllowed = 1;
-      cfg.attrs = attr;
-      cfg.numAttrs = 1;
-      return (int)cudaLaunchKernelEx(&cfg, kernel, p, np, op);
-    }
-    kernel<<<(unsigned)blocks, kThreads, 0, st>>>(p, np, op);
-    return (int)cudaGetLastError();
-  };
   // (every quads-per-row divides exactly on the fast path: its quad indices are 32-bit, see rowdiv.cuh)
   const bool fast = p.vec && !bcast && p.small && np.n_cells == 1 &&
-                    (L->rows + (nz ? nz->row_offset : 0)) < 0xFFFFFFFFll;
-  pdl = fast && pdl_enabled();
+                    (L->rows + (nz ? nz->row_offset : 0)) < kMaxGlobalRows;
+  const bool pdl = fast && pdl_enabled();
+  auto go = [&](auto kernel) -> int {
+    // Persistent, balanced grid: small problems get one quad per thread, large ones one wave of resident CTAs, each
+    // owning an equal contiguous slice.
+    int per_sm = resident_ctas(reinterpret_cast<const void*>(kernel), kThreads, 0);
+    if (per_sm < 1) per_sm = 1;
+    if (const int lim = ctas_per_sm_limit(); lim > 0 && lim < per_sm) per_sm = lim;
+    return launch_kernel(kernel, capped_grid(p.nquads, kThreads, per_sm), kThreads, 0,
+                         reinterpret_cast<cudaStream_t>(L->stream), pdl, p, np, op);
+  };
   if constexpr (!Op::USES_NOISE) {
     if (fast) return go(ew_fast_kernel<T, Op, TSDE_SRC_UNIT>);
     return go(ew_kernel<T, Op, TSDE_SRC_UNIT>);
@@ -590,17 +539,5 @@ inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
     }
   }
 }
-
-// A launch descriptor every entry point can rely on: non-null, non-negative row count, positive widths.
-inline bool launch_invalid(const tsde_launch* L) { return !L || L->rows < 0 || L->d <= 0 || L->m <= 0; }
-
-// (an empty batch is a valid launch that does nothing: its tensors have no storage, so their pointers are null)
-#define TSDE_DISPATCH_DTYPE(L, EXPR_F32, EXPR_F64)                                                   \
-  (::tsde::launch_invalid(L) ? TSDE_EINVAL                                                           \
-   : ((L)->dtype != TSDE_F32 && (L)->dtype != TSDE_F64) ? TSDE_EINVAL                                \
-   : (L)->rows == 0          ? 0                                                                     \
-   : (L)->dtype == TSDE_F32  ? (EXPR_F32)                                                            \
-   : (L)->dtype == TSDE_F64  ? (EXPR_F64)                                                            \
-                             : TSDE_EINVAL)
 
 }  // namespace tsde

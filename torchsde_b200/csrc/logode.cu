@@ -110,20 +110,11 @@ bmm_ga_generic_kernel(int64_t rows, int64_t d, int64_t m, const T* __restrict__ 
   }
 }
 
-inline unsigned grid_for_bmm(int64_t n) {
-  int64_t b = (n + kThreads - 1) / kThreads;
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (unsigned)b;
-}
-
 template <typename T>
 static int bmm_ga_impl(const tsde_launch* L, const void* g, const void* a, void* out) {
   if (!g || !a || !out) return TSDE_EINVAL;
   if (L->noise_type != TSDE_NOISE_GENERAL) return TSDE_EINVAL;
   const int64_t rows = L->rows, d = L->d, m = L->m;
-  if (rows * d * m == 0) return 0;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
   const bool al = aligned16(g) && aligned16(a);
   auto tiled = [&](auto kernel, int M) -> int {
@@ -135,9 +126,8 @@ static int bmm_ga_impl(const tsde_launch* L, const void* g, const void* a, void*
     if (rpc < 1) return TSDE_EINVAL;
     const int64_t blocks = (rows + rpc - 1) / rpc;
     if (blocks > 0x7fffffffll) return TSDE_EINVAL;
-    kernel<<<(unsigned)blocks, kBmmThreads, (size_t)rpc * M * M * sizeof(T), st>>>(
-        rows, (int)d, (const T*)g, (const T*)a, (T*)out, (int)rpc);
-    return (int)cudaGetLastError();
+    return launch_kernel(kernel, blocks, kBmmThreads, (size_t)rpc * M * M * sizeof(T), st, false, rows, (int)d,
+                         (const T*)g, (const T*)a, (T*)out, (int)rpc);
   };
   if (d <= (1 << 20) && (al || m % 4 != 0)) {
     switch (m) {
@@ -150,17 +140,16 @@ static int bmm_ga_impl(const tsde_launch* L, const void* g, const void* a, void*
       default: break;
     }
   }
-  bmm_ga_generic_kernel<T><<<grid_for_bmm(rows * d * m), kThreads, 0, st>>>(rows, d, m, (const T*)g, (const T*)a,
-                                                                        (T*)out);
-  return (int)cudaGetLastError();
+  return launch_kernel(bmm_ga_generic_kernel<T>, capped_grid(rows * d * m, kThreads, 16), kThreads, 0, st, false,
+                       rows, d, m, (const T*)g, (const T*)a, (T*)out);
 }
 
 }  // namespace tsde
 
 using namespace tsde;
 
-extern "C" int tsde_bmm_ga(const tsde_launch* L, const void* g, const void* a, void* out_t) {
-  return TSDE_DISPATCH_DTYPE(L, bmm_ga_impl<float>(L, g, a, out_t), bmm_ga_impl<double>(L, g, a, out_t));
+TSDE_EXPORT int tsde_bmm_ga(const tsde_launch* L, const void* g, const void* a, void* out_t) {
+  return dispatch(L, [&](auto t) { return bmm_ga_impl<decltype(t)>(L, g, a, out_t); });
 }
 
 // ---- logqp: KL-integrand augmentation, diagonal noise ---------------------------------------------------------
@@ -206,20 +195,17 @@ static int logqp_augment_impl(const tsde_launch* L, const void* f, const void* g
                               void* f_aug, void* g_aug) {
   if (!f || !g || !h || !f_aug || !g_aug) return TSDE_EINVAL;
   if (L->noise_type != TSDE_NOISE_DIAGONAL || L->d > (1 << 24)) return TSDE_EINVAL;
-  if (L->rows == 0) return 0;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
-  int64_t blocks = (L->rows * 32 + kThreads - 1) / kThreads;
-  const int64_t cap = (int64_t)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
-  logqp_augment_kernel<T><<<(unsigned)blocks, kThreads, 0, st>>>(L->rows, (int)L->d, (const T*)f, (const T*)g,
-                                                              (const T*)h, (T)eps, (T*)f_aug, (T*)g_aug);
-  return (int)cudaGetLastError();
+  // one warp per row
+  return launch_kernel(logqp_augment_kernel<T>, capped_grid(L->rows * 32, kThreads, kBlocksPerSM), kThreads, 0,
+                       reinterpret_cast<cudaStream_t>(L->stream), false, L->rows, (int)L->d, (const T*)f,
+                       (const T*)g, (const T*)h, (T)eps, (T*)f_aug, (T*)g_aug);
 }
 
 }  // namespace tsde
 
-extern "C" int tsde_logqp_augment(const tsde_launch* L, const void* f, const void* g, const void* h, double eps,
-                                  void* f_aug, void* g_aug) {
-  return TSDE_DISPATCH_DTYPE(L, tsde::logqp_augment_impl<float>(L, f, g, h, eps, f_aug, g_aug),
-                             tsde::logqp_augment_impl<double>(L, f, g, h, eps, f_aug, g_aug));
+TSDE_EXPORT int tsde_logqp_augment(const tsde_launch* L, const void* f, const void* g, const void* h, double eps,
+                                   void* f_aug, void* g_aug) {
+  return tsde::dispatch(L, [&](auto t) {
+    return tsde::logqp_augment_impl<decltype(t)>(L, f, g, h, eps, f_aug, g_aug);
+  });
 }

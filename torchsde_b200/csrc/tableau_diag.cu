@@ -275,10 +275,6 @@ static int run(const tsde_launch* L, const tsde_noise* nz, std::initializer_list
   return launch_ew<T, Op>(L, nz, bcast, ins.begin(), outs.begin(), op);
 }
 
-}  // namespace tsde
-
-using namespace tsde;
-
 template <typename T>
 static SrkDiagFinalOp<T> make_srk_final(double dt, double rdt, double sqrt_dt, double three_dt) {
   SrkDiagFinalOp<T> op;
@@ -302,169 +298,162 @@ static SrkDiagFinalOp<T> make_srk_final(double dt, double rdt, double sqrt_dt, d
   return op;
 }
 
-
-// Entry points that are element-wise for every noise type they are called with.  The
-// general-noise (rows,d,m) contractions live in tableau_general.cu; the exported C symbols
-// dispatch on L->noise_type there.
-extern "C" {
-
-int tsde_diag_step_euler(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f,
-                         const void* g, double dt, void* y1) {
-  return TSDE_DISPATCH_DTYPE(
-      L, (run<float>(L, nz, {y0, f, g}, {y1}, EulerOp<float>{(float)dt})),
-      (run<double>(L, nz, {y0, f, g}, {y1}, EulerOp<double>{dt})));
+// ---- entry points ---------------------------------------------------------------------------------------------------
+// The routes of cabi.cu for row-wise noise (the (rows,d,m) contractions of general noise live in tableau_general.cu).
+int diag_step_euler(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f, const void* g,
+                    double dt, void* y1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, f, g}, {y1}, EulerOp<T>{(T)dt});
+  });
 }
 
-int tsde_diag_milstein_vjp_seed(const tsde_launch* L, const tsde_noise* nz, const void* g,
-                                double dt, int32_t ito, void* go) {
-  return TSDE_DISPATCH_DTYPE(
-      L, (run<float>(L, nz, {g}, {go}, MilsteinSeedOp<float>{(float)dt, ito})),
-      (run<double>(L, nz, {g}, {go}, MilsteinSeedOp<double>{dt, ito})));
+int diag_milstein_vjp_seed(const tsde_launch* L, const tsde_noise* nz, const void* g, double dt, int32_t ito,
+                           void* go) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {g}, {go}, MilsteinSeedOp<T>{(T)dt, ito});
+  });
 }
 
-int tsde_diag_step_milstein(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                            const void* f, const void* g, const void* gdg, double dt, void* y1) {
-  return TSDE_DISPATCH_DTYPE(
-      L, (run<float>(L, nz, {y0, f, g, gdg}, {y1}, MilsteinOp<float>{(float)dt})),
-      (run<double>(L, nz, {y0, f, g, gdg}, {y1}, MilsteinOp<double>{dt})));
+int diag_step_milstein(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f, const void* g,
+                       const void* gdg, double dt, void* y1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, f, g, gdg}, {y1}, MilsteinOp<T>{(T)dt});
+  });
 }
 
-int tsde_milstein_gf_predict(const tsde_launch* L, const void* y0, const void* f, const void* g,
-                             double dt, double sqrt_dt, int32_t ito, void* yp) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (run<float>(L, nullptr, {y0, f, g}, {yp},
-                  MilsteinGfPredictOp<float>{(float)dt, (float)sqrt_dt, ito})),
-      (run<double>(L, nullptr, {y0, f, g}, {yp}, MilsteinGfPredictOp<double>{dt, sqrt_dt, ito})));
+int diag_step_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f, const void* fp,
+                   const void* g, const void* gp, double dt, void* y1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, f, fp, g, gp}, {y1}, HeunOp<T>{(T)dt});
+  });
 }
 
-int tsde_step_milstein_gf(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                          const void* f, const void* g, const void* gp, double dt,
-                          double two_sqrt_dt, int32_t ito, void* y1) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (run<float>(L, nz, {y0, f, g, gp}, {y1},
-                  MilsteinGfOp<float>{(float)dt, (float)two_sqrt_dt, ito})),
-      (run<double>(L, nz, {y0, f, g, gp}, {y1}, MilsteinGfOp<double>{dt, two_sqrt_dt, ito})));
+int diag_midpoint_predict(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f, const void* g,
+                          double half_dt, void* yp) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, f, g}, {yp}, MidpointPredictOp<T>{(T)half_dt});
+  });
 }
 
-int tsde_diag_step_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f,
-                        const void* fp, const void* g, const void* gp, double dt, void* y1) {
-  return TSDE_DISPATCH_DTYPE(
-      L, (run<float>(L, nz, {y0, f, fp, g, gp}, {y1}, HeunOp<float>{(float)dt})),
-      (run<double>(L, nz, {y0, f, fp, g, gp}, {y1}, HeunOp<double>{dt})));
+int diag_euler_heun_predict(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* g, void* yp) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, g}, {yp}, EulerHeunPredictOp<T>{});
+  });
 }
 
-int tsde_diag_midpoint_predict(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                               const void* f, const void* g, double half_dt, void* yp) {
-  return TSDE_DISPATCH_DTYPE(
-      L, (run<float>(L, nz, {y0, f, g}, {yp}, MidpointPredictOp<float>{(float)half_dt})),
-      (run<double>(L, nz, {y0, f, g}, {yp}, MidpointPredictOp<double>{half_dt})));
+int diag_step_euler_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f, const void* g,
+                         const void* gp, double dt, void* y1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, f, g, gp}, {y1}, EulerHeunOp<T>{(T)dt});
+  });
 }
 
-int tsde_diag_euler_heun_predict(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                                 const void* g, void* yp) {
-  return TSDE_DISPATCH_DTYPE(L, (run<float>(L, nz, {y0, g}, {yp}, EulerHeunPredictOp<float>{})),
-                             (run<double>(L, nz, {y0, g}, {yp}, EulerHeunPredictOp<double>{})));
+int diag_reversible_heun_z(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* z0,
+                           const void* f0, const void* g0, double dt, void* z1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, z0, f0, g0}, {z1}, RevHeunZOp<T>{(T)dt});
+  });
 }
 
-int tsde_diag_step_euler_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                              const void* f, const void* g, const void* gp, double dt, void* y1) {
-  return TSDE_DISPATCH_DTYPE(
-      L, (run<float>(L, nz, {y0, f, g, gp}, {y1}, EulerHeunOp<float>{(float)dt})),
-      (run<double>(L, nz, {y0, f, g, gp}, {y1}, EulerHeunOp<double>{dt})));
+int diag_step_reversible_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f0,
+                              const void* f1, const void* g0, const void* g1, double half_dt, void* y1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, f0, f1, g0, g1}, {y1}, RevHeunOp<T>{(T)half_dt});
+  });
 }
 
-int tsde_diag_reversible_heun_z(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                                const void* z0, const void* f0, const void* g0, double dt,
-                                void* z1) {
-  return TSDE_DISPATCH_DTYPE(
-      L, (run<float>(L, nz, {y0, z0, f0, g0}, {z1}, RevHeunZOp<float>{(float)dt})),
-      (run<double>(L, nz, {y0, z0, f0, g0}, {z1}, RevHeunZOp<double>{dt})));
+int diag_adjoint_reversible_heun_a(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* z0,
+                                   const void* f0, const void* g0, const void* adj_y0, const void* adj_f0,
+                                   const void* adj_g0, double dt, double half_dt, void* z1, void* adj_f0_out,
+                                   void* adj_g0_out) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, z0, f0, g0, adj_y0, adj_f0, adj_g0}, {z1, adj_f0_out, adj_g0_out},
+                  AdjRevHeunAOp<T>{(T)dt, (T)half_dt});
+  });
 }
 
-int tsde_diag_step_reversible_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                                   const void* f0, const void* f1, const void* g0, const void* g1,
-                                   double half_dt, void* y1) {
-  return TSDE_DISPATCH_DTYPE(
-      L, (run<float>(L, nz, {y0, f0, f1, g0, g1}, {y1}, RevHeunOp<float>{(float)half_dt})),
-      (run<double>(L, nz, {y0, f0, f1, g0, g1}, {y1}, RevHeunOp<double>{half_dt})));
+int diag_adjoint_reversible_heun_b(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f0,
+                                   const void* f1, const void* g0, const void* g1, const void* adj_y0,
+                                   const void* adj_z0, const void* vjp_z, double dt, double half_dt, void* y1,
+                                   void* adj_y1, void* adj_z1, void* adj_f1, void* adj_g1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, f0, f1, g0, g1, adj_y0, adj_z0, vjp_z}, {y1, adj_y1, adj_z1, adj_f1, adj_g1},
+                  AdjRevHeunBOp<T>{(T)dt, (T)half_dt});
+  });
 }
 
-int tsde_srk_diag_stage1(const tsde_launch* L, const void* y0, const void* f0, const void* g0,
-                         double dt, double sqrt_dt, void* h0_1, void* h1_1) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (run<float>(L, nullptr, {y0, f0, g0}, {h0_1, h1_1},
-                  SrkDiagStage1Op<float>{(float)dt, (float)sqrt_dt})),
-      (run<double>(L, nullptr, {y0, f0, g0}, {h0_1, h1_1}, SrkDiagStage1Op<double>{dt, sqrt_dt})));
+}  // namespace tsde
+
+using namespace tsde;
+
+// Exported entry points that are row-wise for every noise type they are called with.
+TSDE_EXPORT int tsde_milstein_gf_predict(const tsde_launch* L, const void* y0, const void* f, const void* g,
+                                         double dt, double sqrt_dt, int32_t ito, void* yp) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nullptr, {y0, f, g}, {yp}, MilsteinGfPredictOp<T>{(T)dt, (T)sqrt_dt, ito});
+  });
 }
 
-int tsde_srk_diag_stage2(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                         const void* f0, const void* g0, const void* f1, const void* g1, double dt,
-                         double rdt, double sqrt_dt, void* h0_2, void* h1_2) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (run<float>(L, nz, {y0, f0, g0, f1, g1}, {h0_2, h1_2},
-                  SrkDiagStage2Op<float>{(float)dt, (float)rdt, (float)sqrt_dt})),
-      (run<double>(L, nz, {y0, f0, g0, f1, g1}, {h0_2, h1_2},
-                   SrkDiagStage2Op<double>{dt, rdt, sqrt_dt})));
+TSDE_EXPORT int tsde_step_milstein_gf(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f,
+                                      const void* g, const void* gp, double dt, double two_sqrt_dt, int32_t ito,
+                                      void* y1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, f, g, gp}, {y1}, MilsteinGfOp<T>{(T)dt, (T)two_sqrt_dt, ito});
+  });
 }
 
-int tsde_srk_diag_stage3(const tsde_launch* L, const void* y0, const void* g0, const void* g1,
-                         const void* f2, const void* g2, double dt, double sqrt_dt, void* h1_3) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (run<float>(L, nullptr, {y0, g0, g1, f2, g2}, {h1_3},
-                  SrkDiagStage3Op<float>{(float)dt, (float)sqrt_dt})),
-      (run<double>(L, nullptr, {y0, g0, g1, f2, g2}, {h1_3},
-                   SrkDiagStage3Op<double>{dt, sqrt_dt})));
+TSDE_EXPORT int tsde_srk_diag_stage1(const tsde_launch* L, const void* y0, const void* f0, const void* g0, double dt,
+                                     double sqrt_dt, void* h0_1, void* h1_1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nullptr, {y0, f0, g0}, {h0_1, h1_1}, SrkDiagStage1Op<T>{(T)dt, (T)sqrt_dt});
+  });
 }
 
-int tsde_step_srk_diag(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f0,
-                       const void* f1, const void* f2, const void* g0, const void* g1,
-                       const void* g2, const void* g3, double dt, double rdt, double sqrt_dt,
-                       double three_dt, void* y1) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (run<float>(L, nz, {y0, f0, f1, f2, g0, g1, g2, g3}, {y1},
-                  make_srk_final<float>(dt, rdt, sqrt_dt, three_dt))),
-      (run<double>(L, nz, {y0, f0, f1, f2, g0, g1, g2, g3}, {y1},
-                   make_srk_final<double>(dt, rdt, sqrt_dt, three_dt))));
+TSDE_EXPORT int tsde_srk_diag_stage2(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f0,
+                                     const void* g0, const void* f1, const void* g1, double dt, double rdt,
+                                     double sqrt_dt, void* h0_2, void* h1_2) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, f0, g0, f1, g1}, {h0_2, h1_2}, SrkDiagStage2Op<T>{(T)dt, (T)rdt, (T)sqrt_dt});
+  });
 }
 
-int tsde_linear_interp(const tsde_launch* L, const void* y0, const void* y1, double w0, double w1,
-                       void* out) {
-  return TSDE_DISPATCH_DTYPE(
-      L, (run<float>(L, nullptr, {y0, y1}, {out}, LerpOp<float>{(float)w0, (float)w1})),
-      (run<double>(L, nullptr, {y0, y1}, {out}, LerpOp<double>{w0, w1})));
+TSDE_EXPORT int tsde_srk_diag_stage3(const tsde_launch* L, const void* y0, const void* g0, const void* g1,
+                                     const void* f2, const void* g2, double dt, double sqrt_dt, void* h1_3) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nullptr, {y0, g0, g1, f2, g2}, {h1_3}, SrkDiagStage3Op<T>{(T)dt, (T)sqrt_dt});
+  });
 }
 
-int tsde_diag_adjoint_reversible_heun_a(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                                        const void* z0, const void* f0, const void* g0,
-                                        const void* adj_y0, const void* adj_f0,
-                                        const void* adj_g0, double dt, double half_dt, void* z1,
-                                        void* adj_f0_out, void* adj_g0_out) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (run<float>(L, nz, {y0, z0, f0, g0, adj_y0, adj_f0, adj_g0}, {z1, adj_f0_out, adj_g0_out},
-                  AdjRevHeunAOp<float>{(float)dt, (float)half_dt})),
-      (run<double>(L, nz, {y0, z0, f0, g0, adj_y0, adj_f0, adj_g0}, {z1, adj_f0_out, adj_g0_out},
-                   AdjRevHeunAOp<double>{dt, half_dt})));
+TSDE_EXPORT int tsde_step_srk_diag(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f0,
+                                   const void* f1, const void* f2, const void* g0, const void* g1, const void* g2,
+                                   const void* g3, double dt, double rdt, double sqrt_dt, double three_dt,
+                                   void* y1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nz, {y0, f0, f1, f2, g0, g1, g2, g3}, {y1}, make_srk_final<T>(dt, rdt, sqrt_dt, three_dt));
+  });
 }
 
-int tsde_diag_adjoint_reversible_heun_b(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                                        const void* f0, const void* f1, const void* g0,
-                                        const void* g1, const void* adj_y0, const void* adj_z0,
-                                        const void* vjp_z, double dt, double half_dt, void* y1,
-                                        void* adj_y1, void* adj_z1, void* adj_f1, void* adj_g1) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (run<float>(L, nz, {y0, f0, f1, g0, g1, adj_y0, adj_z0, vjp_z},
-                  {y1, adj_y1, adj_z1, adj_f1, adj_g1},
-                  AdjRevHeunBOp<float>{(float)dt, (float)half_dt})),
-      (run<double>(L, nz, {y0, f0, f1, g0, g1, adj_y0, adj_z0, vjp_z},
-                   {y1, adj_y1, adj_z1, adj_f1, adj_g1}, AdjRevHeunBOp<double>{dt, half_dt})));
+TSDE_EXPORT int tsde_linear_interp(const tsde_launch* L, const void* y0, const void* y1, double w0, double w1,
+                                   void* out) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return run<T>(L, nullptr, {y0, y1}, {out}, LerpOp<T>{(T)w0, (T)w1});
+  });
 }
-
-}  // extern "C"

@@ -13,8 +13,6 @@
 // are bitwise reproducible and independent of batch sharding, and agree with torch.bmm to
 // rounding (bmm's own order is unspecified), which is how the parity tests treat them.
 #include <atomic>
-#include <map>
-#include <utility>
 
 #include "ew.cuh"
 
@@ -599,30 +597,6 @@ inline int gen_tma_mode(int64_t mq, int n_g_operands) {
 
 constexpr int kTmaNotEligible = -12345;
 
-// Per kernel instantiation: opt in to the dynamic shared memory once, and cache the occupancy.
-template <typename K>
-static int tma_resident_ctas(K kernel, size_t smem) {
-  static std::mutex mu;
-  static std::map<std::pair<const void*, int>, std::pair<size_t, int>> cache;  // (kernel, device) -> (smem opted in, CTAs/SM)
-  int dev = 0;
-  cudaGetDevice(&dev);  // function attributes are per device
-  const std::pair<const void*, int> id(reinterpret_cast<const void*>(kernel), dev);
-  std::lock_guard<std::mutex> lock(mu);
-  auto it = cache.find(id);
-  if (it != cache.end() && it->second.first == smem) return it->second.second;
-  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-    cudaGetLastError();
-    return 0;
-  }
-  int n = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, kTmaThreads + 32, smem) != cudaSuccess) {
-    cudaGetLastError();
-    n = 0;
-  }
-  cache[id] = std::make_pair(smem, n);
-  return n;
-}
-
 template <typename T, typename Op>
 static int launch_gen_tma(const tsde_launch* L, const tsde_noise* nz, GenP<Op::NE, Op::NG, Op::NO> p,
                           const NoiseP<T>& np, const Op& op, int mode, cudaStream_t st) {
@@ -658,23 +632,13 @@ static int launch_gen_tma(const tsde_launch* L, const tsde_noise* nz, GenP<Op::N
   if (smem > 200 * 1024) return kTmaNotEligible;
   p.rb = (int32_t)rs;
   auto go = [&](auto kernel) -> int {
-    const int resident = tma_resident_ctas(kernel, smem);
+    const int resident = resident_ctas(reinterpret_cast<const void*>(kernel), kTmaThreads + 32, smem);
     if (resident < 1) return kTmaNotEligible;
     const int64_t cap = (int64_t)sm_count() * resident;
     if (mode < 2 && tp.n_tiles < 2 * kTmaStages * cap) return kTmaNotEligible;  // too small to fill the pipeline
-    const int64_t blocks = tp.n_tiles < cap ? tp.n_tiles : cap;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)blocks);
-    cfg.blockDim = dim3(kTmaThreads + 32);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
     g_launches[TSDE_KERNEL_GEN_TMA].fetch_add(1, std::memory_order_relaxed);
-    return (int)cudaLaunchKernelEx(&cfg, kernel, p, np, op, tp);
+    return launch_kernel(kernel, tp.n_tiles < cap ? tp.n_tiles : cap, kTmaThreads + 32, smem, st, pdl_enabled(), p,
+                         np, op, tp);
   };
   const bool mem = nz->source == TSDE_SRC_MEMORY;
   switch (mq) {
@@ -692,7 +656,6 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
   if (!nz) return TSDE_EINVAL;
   if (nz->source != TSDE_SRC_MEMORY && nz->source != TSDE_SRC_COUNTER)
     return TSDE_EINVAL;  // (a user-supplied product, TSDE_SRC_UNIT, goes through the element-wise entry points)
-  if (L->rows == 0) return 0;  // empty batch: nothing to do (its tensors have no storage)
   GenP<Op::NE, Op::NG, Op::NO> p{};
   bool vec = (L->m % 4) == 0;
   int i = 0;
@@ -710,8 +673,7 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
   p.mq = (int32_t)mq;
   p.vec = vec ? 1 : 0;
   p.gbcast = (nz->flags & TSDE_FLAG_G_BROADCAST) ? 1 : 0;
-  if (L->rows == 0) return 0;
-  if (L->rows + nz->row_offset > 0xFFFFFFFFll) return TSDE_EINVAL;
+  const bool mem = nz->source == TSDE_SRC_MEMORY;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
   if (vec) {
     if (int mode = p.gbcast ? 0 : gen_tma_mode(mq, Op::NG)) {  // (a broadcast g has no tile stream to stage)
@@ -724,20 +686,9 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
     const int64_t ngroups = (L->rows + rw - 1) / rw;
     if (ngroups > 0x7fffffffll) return TSDE_EINVAL;
     const size_t smem = (size_t)rw * L->m * sizeof(T) * (Op::WANT_U ? 2 : 1);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)ngroups);
-    cfg.blockDim = dim3(kGenThreads);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
     g_launches[TSDE_KERNEL_GEN_CTA].fetch_add(1, std::memory_order_relaxed);
-    if (nz->source == TSDE_SRC_MEMORY)
-      return (int)cudaLaunchKernelEx(&cfg, gen_cta_kernel<T, Op, TSDE_SRC_MEMORY>, p, np, op);
-    return (int)cudaLaunchKernelEx(&cfg, gen_cta_kernel<T, Op, TSDE_SRC_COUNTER>, p, np, op);
+    return launch_kernel(mem ? gen_cta_kernel<T, Op, TSDE_SRC_MEMORY> : gen_cta_kernel<T, Op, TSDE_SRC_COUNTER>,
+                         ngroups, kGenThreads, smem, st, pdl_enabled(), p, np, op);
   }
   // generic path: rows per block ~16 work items per thread, bounded by shared memory for the increments
   const int64_t per_row = L->d;
@@ -752,13 +703,8 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
   p.rb = (int32_t)rb;
   const int64_t blocks = (L->rows + rb - 1) / rb;
   if (blocks > 0x7fffffffll) return TSDE_EINVAL;
-  const size_t smem = (size_t)(rb * smem_per_row);
-  if (nz->source == TSDE_SRC_MEMORY) {
-    gen_kernel<T, Op, TSDE_SRC_MEMORY><<<(unsigned)blocks, kThreads, smem, st>>>(p, np, op);
-  } else {
-    gen_kernel<T, Op, TSDE_SRC_COUNTER><<<(unsigned)blocks, kThreads, smem, st>>>(p, np, op);
-  }
-  return (int)cudaGetLastError();
+  return launch_kernel(mem ? gen_kernel<T, Op, TSDE_SRC_MEMORY> : gen_kernel<T, Op, TSDE_SRC_COUNTER>, blocks,
+                       kThreads, (size_t)(rb * smem_per_row), st, false, p, np, op);
 }
 
 // ---- ops ---------------------------------------------------------------------------------------
@@ -932,21 +878,11 @@ static int launch_outer(const tsde_launch* L, const tsde_noise* nz, const void* 
   NoiseP<T> np;
   if (int e = fill_noise<T>(L, nz, false, np)) return e;
   const int64_t total = L->rows * L->d * ((L->m + 3) / 4);
-  if (total == 0) return 0;
-  int64_t blocks = (total + kThreads - 1) / kThreads;
-  const int64_t cap = (int64_t)sm_count() * kBlocksPerSM;
-  if (blocks > cap) blocks = cap;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
-  if (nz->source == TSDE_SRC_MEMORY) {
-    outer_kernel<T, TSDE_SRC_MEMORY><<<(unsigned)blocks, kThreads, 0, st>>>(
-        np, L->rows, L->d, L->m, (const T*)base, (const T*)a1, (T)c1, (const T*)a2, (T)c2, (T*)out);
-  } else if (nz->source == TSDE_SRC_COUNTER) {
-    outer_kernel<T, TSDE_SRC_COUNTER><<<(unsigned)blocks, kThreads, 0, st>>>(
-        np, L->rows, L->d, L->m, (const T*)base, (const T*)a1, (T)c1, (const T*)a2, (T)c2, (T*)out);
-  } else {
-    return TSDE_EINVAL;
-  }
-  return (int)cudaGetLastError();
+  const auto kernel =
+      nz->source == TSDE_SRC_MEMORY ? outer_kernel<T, TSDE_SRC_MEMORY> : outer_kernel<T, TSDE_SRC_COUNTER>;
+  return launch_kernel(kernel, capped_grid(total, kThreads, kBlocksPerSM), kThreads, 0,
+                       reinterpret_cast<cudaStream_t>(L->stream), false, np, L->rows, L->d, L->m, (const T*)base,
+                       (const T*)a1, (T)c1, (const T*)a2, (T)c2, (T*)out);
 }
 
 // element-wise (rows,d) parts of the adjoint
@@ -973,182 +909,134 @@ struct AdjBElemOp {  // in: adj_y0, adj_z0, vjp_z -> adj_y1, adj_z1, adj_f1
   }
 };
 
+// ---- entry points ---------------------------------------------------------------------------------------------------
+// The routes of cabi.cu for general noise with m > 1.
+int general_step_euler(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f, const void* g,
+                       double dt, void* y1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return launch_gen<T>(L, nz, {y0, f}, {g}, {y1}, GEulerOp<T>{(T)dt});
+  });
+}
+
+int general_step_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f, const void* fp,
+                      const void* g, const void* gp, double dt, void* y1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return launch_gen<T>(L, nz, {y0, f, fp}, {g, gp}, {y1}, GHeunOp<T>{(T)dt});
+  });
+}
+
+int general_midpoint_predict(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f,
+                             const void* g, double half_dt, void* yp) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return launch_gen<T>(L, nz, {y0, f}, {g}, {yp}, GMidpointPredictOp<T>{(T)half_dt});
+  });
+}
+
+int general_euler_heun_predict(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* g, void* yp) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return launch_gen<T>(L, nz, {y0}, {g}, {yp}, GEulerHeunPredictOp<T>{});
+  });
+}
+
+int general_step_euler_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f,
+                            const void* g, const void* gp, double dt, void* y1) {
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return launch_gen<T>(L, nz, {y0, f}, {g, gp}, {y1}, GEulerHeunOp<T>{(T)dt});
+  });
+}
+
+// The reversible-Heun pair rejects launch flags: its g operands are saved and differentiated, so always dense.
+int general_reversible_heun_z(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* z0,
+                              const void* f0, const void* g0, double dt, void* z1) {
+  if (nz && nz->flags) return TSDE_EINVAL;
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return launch_gen<T>(L, nz, {y0, z0, f0}, {g0}, {z1}, GRevHeunZOp<T>{(T)dt, 0});
+  });
+}
+
+int general_step_reversible_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f0,
+                                 const void* f1, const void* g0, const void* g1, double half_dt, void* y1) {
+  if (nz && nz->flags) return TSDE_EINVAL;
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return launch_gen<T>(L, nz, {y0, f0, f1}, {g0, g1}, {y1}, GRevHeunOp<T>{(T)half_dt, 0});
+  });
+}
+
+int general_adjoint_reversible_heun_a(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* z0,
+                                      const void* f0, const void* g0, const void* adj_y0, const void* adj_f0,
+                                      const void* adj_g0, double dt, double half_dt, void* z1, void* adj_f0_out,
+                                      void* adj_g0_out) {
+  if (nz && nz->flags) return TSDE_EINVAL;
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    // z1 = 2*y0 - z0 - f0*dt - g0.dW                                              :109
+    if (int e = launch_gen<T>(L, nz, {y0, z0, f0}, {g0}, {z1}, GRevHeunZOp<T>{(T)dt, 1})) return e;
+    // adj_f0' = adj_f0 + adj_y0*half_dt                                            :104,113
+    tsde_launch r = *L;
+    r.noise_type = TSDE_NOISE_DIAGONAL;
+    r.m = r.d;
+    const void* ins[2] = {adj_y0, adj_f0};
+    void* outs[1] = {adj_f0_out};
+    if (int e = launch_ew<T>(&r, nullptr, false, ins, outs, AdjAElemOp<T>{(T)half_dt})) return e;
+    // adj_g0' = adj_g0 + adj_y0 (x) half_dW                                        :105,115
+    return launch_outer<T>(L, nz, adj_g0, adj_y0, 0.5, nullptr, 0.0, adj_g0_out);
+  });
+}
+
+int general_adjoint_reversible_heun_b(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f0,
+                                      const void* f1, const void* g0, const void* g1, const void* adj_y0,
+                                      const void* adj_z0, const void* vjp_z, double dt, double half_dt, void* y1,
+                                      void* adj_y1, void* adj_z1, void* adj_f1, void* adj_g1) {
+  if (nz && nz->flags) return TSDE_EINVAL;
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    // y1 = y0 - (f0+f1)*half_dt - (g0+g1).half_dW                                   :134-135
+    if (int e = launch_gen<T>(L, nz, {y0, f0, f1}, {g0, g1}, {y1}, GRevHeunOp<T>{(T)half_dt, 1})) return e;
+    // element-wise part: adj_y1, adj_z1 = -(adj_z0 + vjp_z), adj_f1
+    tsde_launch r = *L;
+    r.noise_type = TSDE_NOISE_DIAGONAL;
+    r.m = r.d;
+    const void* ins[3] = {adj_y0, adj_z0, vjp_z};
+    void* outs[3] = {adj_y1, adj_z1, adj_f1};
+    if (int e = launch_ew<T>(&r, nullptr, false, ins, outs, AdjBElemOp<T>{(T)dt, (T)half_dt})) return e;
+    // adj_g1 = adj_y0 (x) half_dW + adj_z0' (x) dW = adj_y0 (x) (0.5 dW) + adj_z1 (x) (-1 dW)   :114,140
+    return launch_outer<T>(L, nz, nullptr, adj_y0, 0.5, adj_z1, -1.0, adj_g1);
+  });
+}
+
 }  // namespace tsde
 
 using namespace tsde;
 
-extern "C" {
-
-int tsde_general_step_euler(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                            const void* f, const void* g, double dt, void* y1) {
-  return TSDE_DISPATCH_DTYPE(
-      L, (launch_gen<float, GEulerOp<float>>(L, nz, {y0, f}, {g}, {y1}, GEulerOp<float>{(float)dt})),
-      (launch_gen<double, GEulerOp<double>>(L, nz, {y0, f}, {g}, {y1}, GEulerOp<double>{dt})));
-}
-
-int tsde_general_step_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                           const void* f, const void* fp, const void* g, const void* gp, double dt,
-                           void* y1) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (launch_gen<float, GHeunOp<float>>(L, nz, {y0, f, fp}, {g, gp}, {y1}, GHeunOp<float>{(float)dt})),
-      (launch_gen<double, GHeunOp<double>>(L, nz, {y0, f, fp}, {g, gp}, {y1}, GHeunOp<double>{dt})));
-}
-
-int tsde_general_midpoint_predict(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                                  const void* f, const void* g, double half_dt, void* yp) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (launch_gen<float, GMidpointPredictOp<float>>(L, nz, {y0, f}, {g}, {yp},
-                                                    GMidpointPredictOp<float>{(float)half_dt})),
-      (launch_gen<double, GMidpointPredictOp<double>>(L, nz, {y0, f}, {g}, {yp},
-                                                      GMidpointPredictOp<double>{half_dt})));
-}
-
-int tsde_general_euler_heun_predict(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                                    const void* g, void* yp) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (launch_gen<float, GEulerHeunPredictOp<float>>(L, nz, {y0}, {g}, {yp},
-                                                     GEulerHeunPredictOp<float>{})),
-      (launch_gen<double, GEulerHeunPredictOp<double>>(L, nz, {y0}, {g}, {yp},
-                                                       GEulerHeunPredictOp<double>{})));
-}
-
-int tsde_general_step_euler_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                                 const void* f, const void* g, const void* gp, double dt,
-                                 void* y1) {
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (launch_gen<float, GEulerHeunOp<float>>(L, nz, {y0, f}, {g, gp}, {y1},
-                                              GEulerHeunOp<float>{(float)dt})),
-      (launch_gen<double, GEulerHeunOp<double>>(L, nz, {y0, f}, {g, gp}, {y1},
-                                                GEulerHeunOp<double>{dt})));
-}
-
-int tsde_general_reversible_heun_z(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                                   const void* z0, const void* f0, const void* g0, double dt,
-                                   void* z1) {
-  if (nz && nz->flags) return TSDE_EINVAL;  // (saved / differentiated g operands are always dense)
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (launch_gen<float, GRevHeunZOp<float>>(L, nz, {y0, z0, f0}, {g0}, {z1},
-                                             GRevHeunZOp<float>{(float)dt, 0})),
-      (launch_gen<double, GRevHeunZOp<double>>(L, nz, {y0, z0, f0}, {g0}, {z1},
-                                               GRevHeunZOp<double>{dt, 0})));
-}
-
-int tsde_general_step_reversible_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                                      const void* f0, const void* f1, const void* g0,
-                                      const void* g1, double half_dt, void* y1) {
-  if (nz && nz->flags) return TSDE_EINVAL;  // (saved / differentiated g operands are always dense)
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (launch_gen<float, GRevHeunOp<float>>(L, nz, {y0, f0, f1}, {g0, g1}, {y1},
-                                            GRevHeunOp<float>{(float)half_dt, 0})),
-      (launch_gen<double, GRevHeunOp<double>>(L, nz, {y0, f0, f1}, {g0, g1}, {y1},
-                                              GRevHeunOp<double>{half_dt, 0})));
-}
-
-int tsde_srk_additive_stage(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                            const void* f0, const void* ga, double dt, double rdt, void* h0_1) {
+// Exported entry points that exist for additive noise only.
+TSDE_EXPORT int tsde_srk_additive_stage(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f0,
+                                        const void* ga, double dt, double rdt, void* h0_1) {
   if (!L || L->noise_type != TSDE_NOISE_GENERAL) return TSDE_EINVAL;
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (launch_gen<float, GSraStageOp<float>>(L, nz, {y0, f0}, {ga}, {h0_1},
-                                             GSraStageOp<float>{(float)dt, (float)rdt})),
-      (launch_gen<double, GSraStageOp<double>>(L, nz, {y0, f0}, {ga}, {h0_1},
-                                               GSraStageOp<double>{dt, rdt})));
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return launch_gen<T>(L, nz, {y0, f0}, {ga}, {h0_1}, GSraStageOp<T>{(T)dt, (T)rdt});
+  });
 }
 
-int tsde_step_srk_additive(const tsde_launch* L, const tsde_noise* nz, const void* y0,
-                           const void* f0, const void* f1, const void* ga, const void* gb,
-                           double dt, double rdt, void* y1) {
+TSDE_EXPORT int tsde_step_srk_additive(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f0,
+                                       const void* f1, const void* ga, const void* gb, double dt, double rdt,
+                                       void* y1) {
   if (!L || L->noise_type != TSDE_NOISE_GENERAL) return TSDE_EINVAL;
-  return TSDE_DISPATCH_DTYPE(
-      L,
-      (launch_gen<float, GSraFinalOp<float>>(
-          L, nz, {y0, f0, f1}, {ga, gb}, {y1},
-          GSraFinalOp<float>{(float)dt, (float)rdt, (float)(1.0 / 3), (float)(2.0 / 3)})),
-      (launch_gen<double, GSraFinalOp<double>>(
-          L, nz, {y0, f0, f1}, {ga, gb}, {y1},
-          GSraFinalOp<double>{dt, rdt, 1.0 / 3, 2.0 / 3})));
+  return dispatch(L, [&](auto t) {
+    using T = decltype(t);
+    return launch_gen<T>(L, nz, {y0, f0, f1}, {ga, gb}, {y1},
+                         GSraFinalOp<T>{(T)dt, (T)rdt, (T)(1.0 / 3), (T)(2.0 / 3)});
+  });
 }
 
-int tsde_general_adjoint_reversible_heun_a(const tsde_launch* L, const tsde_noise* nz,
-                                           const void* y0, const void* z0, const void* f0,
-                                           const void* g0, const void* adj_y0, const void* adj_f0,
-                                           const void* adj_g0, double dt, double half_dt, void* z1,
-                                           void* adj_f0_out, void* adj_g0_out) {
-  if (nz && nz->flags) return TSDE_EINVAL;  // (saved / differentiated g operands are always dense)
-  // z1 = 2*y0 - z0 - f0*dt - g0.dW                                              :109
-  int e = TSDE_DISPATCH_DTYPE(
-      L,
-      (launch_gen<float, GRevHeunZOp<float>>(L, nz, {y0, z0, f0}, {g0}, {z1},
-                                             GRevHeunZOp<float>{(float)dt, 1})),
-      (launch_gen<double, GRevHeunZOp<double>>(L, nz, {y0, z0, f0}, {g0}, {z1},
-                                               GRevHeunZOp<double>{dt, 1})));
-  if (e) return e;
-  // adj_f0' = adj_f0 + adj_y0*half_dt                                            :104,113
-  {
-    const void* ins[2] = {adj_y0, adj_f0};
-    void* outs[1] = {adj_f0_out};
-    tsde_launch r = *L;
-    r.noise_type = TSDE_NOISE_DIAGONAL;
-    r.m = r.d;
-    e = TSDE_DISPATCH_DTYPE(
-        L,
-        (launch_ew<float, AdjAElemOp<float>>(&r, nullptr, false, ins, outs,
-                                             AdjAElemOp<float>{(float)half_dt})),
-        (launch_ew<double, AdjAElemOp<double>>(&r, nullptr, false, ins, outs,
-                                               AdjAElemOp<double>{half_dt})));
-    if (e) return e;
-  }
-  // adj_g0' = adj_g0 + adj_y0 (x) half_dW                                        :105,115
-  return TSDE_DISPATCH_DTYPE(
-      L, (launch_outer<float>(L, nz, adj_g0, adj_y0, 0.5, nullptr, 0.0, adj_g0_out)),
-      (launch_outer<double>(L, nz, adj_g0, adj_y0, 0.5, nullptr, 0.0, adj_g0_out)));
-}
-
-int tsde_general_adjoint_reversible_heun_b(const tsde_launch* L, const tsde_noise* nz,
-                                           const void* y0, const void* f0, const void* f1,
-                                           const void* g0, const void* g1, const void* adj_y0,
-                                           const void* adj_z0, const void* vjp_z, double dt,
-                                           double half_dt, void* y1, void* adj_y1, void* adj_z1,
-                                           void* adj_f1, void* adj_g1) {
-  if (nz && nz->flags) return TSDE_EINVAL;  // (saved / differentiated g operands are always dense)
-  // y1 = y0 - (f0+f1)*half_dt - (g0+g1).half_dW                                   :134-135
-  int e = TSDE_DISPATCH_DTYPE(
-      L,
-      (launch_gen<float, GRevHeunOp<float>>(L, nz, {y0, f0, f1}, {g0, g1}, {y1},
-                                            GRevHeunOp<float>{(float)half_dt, 1})),
-      (launch_gen<double, GRevHeunOp<double>>(L, nz, {y0, f0, f1}, {g0, g1}, {y1},
-                                              GRevHeunOp<double>{half_dt, 1})));
-  if (e) return e;
-  // element-wise part: adj_y1, adj_z1 = -(adj_z0 + vjp_z), adj_f1
-  {
-    const void* ins[3] = {adj_y0, adj_z0, vjp_z};
-    void* outs[3] = {adj_y1, adj_z1, adj_f1};
-    tsde_launch r = *L;
-    r.noise_type = TSDE_NOISE_DIAGONAL;
-    r.m = r.d;
-    e = TSDE_DISPATCH_DTYPE(
-        L,
-        (launch_ew<float, AdjBElemOp<float>>(&r, nullptr, false, ins, outs,
-                                             AdjBElemOp<float>{(float)dt, (float)half_dt})),
-        (launch_ew<double, AdjBElemOp<double>>(&r, nullptr, false, ins, outs,
-                                               AdjBElemOp<double>{dt, half_dt})));
-    if (e) return e;
-  }
-  // adj_g1 = adj_y0 (x) half_dW + adj_z0' (x) dW = adj_y0 (x) (0.5 dW) + adj_z1 (x) (-1 dW)   :114,140
-  return TSDE_DISPATCH_DTYPE(
-      L, (launch_outer<float>(L, nz, nullptr, adj_y0, 0.5, adj_z1, -1.0, adj_g1)),
-      (launch_outer<double>(L, nz, nullptr, adj_y0, 0.5, adj_z1, -1.0, adj_g1)));
-}
-
-int64_t tsde_general_kernel_launches(int32_t family) {
+TSDE_EXPORT int64_t tsde_kernel_launches(int32_t family) {
   if (family < 0 || family > 1) return -1;
-  return tsde::g_launches[family].load(std::memory_order_relaxed);
+  return g_launches[family].load(std::memory_order_relaxed);
 }
-
-}  // extern "C"
