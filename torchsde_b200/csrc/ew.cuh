@@ -6,7 +6,8 @@
 // HBM plan (H100 SXM: 132 SMs, 3.35 TB/s HBM3 on the data sheet): each input tensor is read
 // once with 128-bit loads, each output written once with 128-bit stores; every thread issues
 // all of its loads before the first dependent use (NIN independent LDG.128 in flight per
-// thread); the grid is one resident wave (SM count x occupancy), each CTA owning an equal
+// thread).  The fast kernel gives each CTA one chunk of U x 256 quads (see ew_fast_kernel); the
+// generic kernel's grid is one resident wave (SM count x occupancy), each CTA owning an equal
 // contiguous slice of the quads.
 #pragma once
 #include <stdint.h>
@@ -37,17 +38,6 @@ inline bool pdl_enabled() {
     v = (e && e[0] == '0') ? 0 : 1;
   }
   return v == 1;
-}
-
-// TSDE_EW_CTAS=n: use at most n resident CTAs per SM for the persistent grids of the row-wise kernels (experiments
-// only; the default is every CTA the occupancy calculator allows).
-inline int ctas_per_sm_limit() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("TSDE_EW_CTAS");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
 }
 
 template <typename T>
@@ -311,8 +301,8 @@ ew_kernel(const EwP<Op::NIN, Op::NOUT> p, const NoiseP<T> nz, const Op op) {
 // predictor stages) are NOT HBM-bound per thread: the Philox + Box-Muller chain (~150 dependent-ish
 // instructions per quad) dominates and one 128-bit load per thread does not cover the HBM latency-bandwidth
 // product (the kernel is issue-bound with every pipe far from saturation).  Those ops
-// process U = 2 quads per thread per iteration: both loads are issued first, the two independent Philox
-// chains interleave (2x ILP, 2x bytes in flight per thread).  Heavy ops (>= 4 tensors) keep U = 1: their
+// process U = 2 quads per thread: the two independent Philox chains interleave, and both loads are issued
+// before the first use (2x ILP, 2x bytes in flight per thread).  Heavy ops (>= 4 tensors) keep U = 1: their
 // loads already cover the latency and the extra registers would cost occupancy.
 template <typename T, typename Op>
 struct quads_per_iter { static constexpr int value = (sizeof(T) == 4 && Op::NIN + Op::NOUT <= 3) ? 2 : 1; };
@@ -338,9 +328,9 @@ struct FastCtx {
   }
 };
 
-// One iteration: U quads Q, Q + kThreads, ... (each warp access stays one contiguous 512-byte run).
-// FIRST: the counter noise was produced ahead of the dependency wait and is passed in (w0, u0).
-template <typename T, typename Op, int SRC, int U, bool FIRST>
+// A thread's U quads Q, Q + kThreads, ... (each warp access stays one contiguous 512-byte run).
+// Counter noise was produced ahead of the dependency wait and is passed in (w0, u0).
+template <typename T, typename Op, int SRC, int U>
 __device__ __forceinline__ void ew_fast_body(const FastCtx<T, Op>& c, uint32_t Q, const T (&w0)[U][4],
                                              const T (&u0)[U][4]) {
   constexpr int NIN = Op::NIN, NOUT = Op::NOUT;
@@ -370,13 +360,8 @@ __device__ __forceinline__ void ew_fast_body(const FastCtx<T, Op>& c, uint32_t Q
     for (int j = 0; j < 4; ++j) { w[k][j] = T(0); u[k][j] = T(0); }
     if (Op::USES_NOISE) {
       if (SRC == TSDE_SRC_COUNTER) {
-        if (FIRST) {
 #pragma unroll
-          for (int j = 0; j < 4; ++j) { w[k][j] = w0[k][j]; u[k][j] = Op::WANT_U ? u0[k][j] : T(0); }
-        } else {
-          c.rng(Qk, w[k], u[k]);  // unconditional (a quad past the slice end costs nothing observable): the U
-                                  // Philox chains must stay in one basic block to interleave
-        }
+        for (int j = 0; j < 4; ++j) { w[k][j] = w0[k][j]; u[k][j] = Op::WANT_U ? u0[k][j] : T(0); }
       } else if (SRC == TSDE_SRC_MEMORY) {
         if (ok[k]) {
           ld4(c.nz.w + base, w[k]);
@@ -407,24 +392,32 @@ __device__ __forceinline__ void ew_fast_body(const FastCtx<T, Op>& c, uint32_t Q
   }
 }
 
+// One chunk of U * kThreads quads per CTA (CTA b owns chunk b), not a persistent grid of contiguous slices: the chunk
+// grid needs no loop, so the Milstein tableau and vjp seed take 38 and 32 registers instead of 56 and 61 and more of
+// their CTAs are resident; both kernels got faster on the H100 (DESIGN §3, which also records the descending and
+// round-robin chunk orders that were measured and rejected).
+template <typename T, typename Op>
+inline uint32_t fast_chunks(uint32_t nquads) {
+  constexpr uint32_t chunk = quads_per_iter<T, Op>::value * kThreads;
+  return (nquads + chunk - 1) / chunk;
+}
+
 template <typename T, typename Op, int SRC>
 __global__ void __launch_bounds__(kThreads, 4)
 ew_fast_kernel(const EwP<Op::NIN, Op::NOUT> p, const NoiseP<T> nz, const Op op) {
   constexpr int U = quads_per_iter<T, Op>::value;
   constexpr bool COUNTER = Op::USES_NOISE && SRC == TSDE_SRC_COUNTER;
   const uint32_t nquads = (uint32_t)p.nquads;
-  const uint32_t q_begin = (uint32_t)(((uint64_t)nquads * blockIdx.x) / gridDim.x);
-  const uint32_t q_end = (uint32_t)(((uint64_t)nquads * (blockIdx.x + 1)) / gridDim.x);
   const bool pow2 = p.qshift >= 0;
   const uint32_t qshift = pow2 ? (uint32_t)p.qshift : 0u;
-  const FastCtx<T, Op> c{p, nz, op, COUNTER ? load_key(nz.key) : Key{0u, 0u}, q_end, qshift, (1u << qshift) - 1u,
+  const FastCtx<T, Op> c{p, nz, op, COUNTER ? load_key(nz.key) : Key{0u, 0u}, nquads, qshift, (1u << qshift) - 1u,
                          (uint32_t)p.qpr, (uint32_t)nz.row_offset, p.qmagic, pow2,
                          p.vec > 1 /* host sets vec = 2 to enable evict-first loads */};
   // Programmatic dependent launch: this grid may start while its predecessor in the stream/graph is
   // still draining.  Everything that does not touch the predecessor's outputs — the Philox/Box-Muller
-  // work of the thread's first U quads — runs before `griddepcontrol.wait`; all loads and stores come after.
+  // work of the thread's U quads — runs before `griddepcontrol.wait`; all loads and stores come after.
   T w0[U][4], u0[U][4];
-  const uint32_t Q0 = q_begin + threadIdx.x;
+  const uint32_t Q0 = blockIdx.x * (uint32_t)(U * kThreads) + threadIdx.x;
   if (COUNTER) {
 #pragma unroll
     for (int k = 0; k < U; ++k) {
@@ -432,9 +425,8 @@ ew_fast_kernel(const EwP<Op::NIN, Op::NOUT> p, const NoiseP<T> nz, const Op op) 
     }
   }
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  if (Q0 >= q_end) return;
-  ew_fast_body<T, Op, SRC, U, true>(c, Q0, w0, u0);
-  for (uint32_t Q = Q0 + U * kThreads; Q < q_end; Q += U * kThreads) ew_fast_body<T, Op, SRC, U, false>(c, Q, w0, u0);
+  if (Q0 >= nquads) return;
+  ew_fast_body<T, Op, SRC, U>(c, Q0, w0, u0);
 }
 
 // ---- host-side launcher -----------------------------------------------------------------------
@@ -505,24 +497,26 @@ inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
   const bool fast = p.vec && !bcast && p.small && np.n_cells == 1 &&
                     (L->rows + (nz ? nz->row_offset : 0)) < kMaxGlobalRows;
   const bool pdl = fast && pdl_enabled();
+  const cudaStream_t stream = reinterpret_cast<cudaStream_t>(L->stream);
   auto go = [&](auto kernel) -> int {
     // Persistent, balanced grid: small problems get one quad per thread, large ones one wave of resident CTAs, each
     // owning an equal contiguous slice.
     int per_sm = resident_ctas(reinterpret_cast<const void*>(kernel), kThreads, 0);
     if (per_sm < 1) per_sm = 1;
-    if (const int lim = ctas_per_sm_limit(); lim > 0 && lim < per_sm) per_sm = lim;
-    return launch_kernel(kernel, capped_grid(p.nquads, kThreads, per_sm), kThreads, 0,
-                         reinterpret_cast<cudaStream_t>(L->stream), pdl, p, np, op);
+    return launch_kernel(kernel, capped_grid(p.nquads, kThreads, per_sm), kThreads, 0, stream, pdl, p, np, op);
+  };
+  auto go_fast = [&](auto kernel) -> int {
+    return launch_kernel(kernel, fast_chunks<T, Op>((uint32_t)p.nquads), kThreads, 0, stream, pdl, p, np, op);
   };
   if constexpr (!Op::USES_NOISE) {
-    if (fast) return go(ew_fast_kernel<T, Op, TSDE_SRC_UNIT>);
+    if (fast) return go_fast(ew_fast_kernel<T, Op, TSDE_SRC_UNIT>);
     return go(ew_kernel<T, Op, TSDE_SRC_UNIT>);
   } else {
     if (fast) {
       switch (src) {
-        case TSDE_SRC_MEMORY: return go(ew_fast_kernel<T, Op, TSDE_SRC_MEMORY>);
-        case TSDE_SRC_COUNTER: return go(ew_fast_kernel<T, Op, TSDE_SRC_COUNTER>);
-        case TSDE_SRC_UNIT: return go(ew_fast_kernel<T, Op, TSDE_SRC_UNIT>);
+        case TSDE_SRC_MEMORY: return go_fast(ew_fast_kernel<T, Op, TSDE_SRC_MEMORY>);
+        case TSDE_SRC_COUNTER: return go_fast(ew_fast_kernel<T, Op, TSDE_SRC_COUNTER>);
+        case TSDE_SRC_UNIT: return go_fast(ew_fast_kernel<T, Op, TSDE_SRC_UNIT>);
         default: return TSDE_EINVAL;
       }
     }
