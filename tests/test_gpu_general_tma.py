@@ -1,123 +1,160 @@
-"""The TMA-staged general-noise path (`gen_tma_kernel`, TSDE_GEN_TMA) against the default tile kernel.
+"""The TMA-staged general-noise tile kernel (`gen_tma_kernel`) against the per-thread-load tile kernel (`gen_cta_kernel`).
 
-Both kernels use the same chunk -> lane mapping, the same fused multiply-add chain inside a 4-chunk and the
-same xor-tree across chunks, so for identical increments their outputs must be BIT-IDENTICAL; the default
-kernel itself is pinned against the oracle / the reference's golden files in test_gpu_solver.py.
+Both kernels use the same chunk -> lane mapping, the same fused multiply-add chain inside a 4-chunk and the same
+xor-tree across chunks, so for identical increments their outputs must be BIT-IDENTICAL; the per-thread-load kernel
+itself is pinned against the oracle / the reference's golden files in test_gpu_solver.py.
+
+Which kernel runs is decided by shape alone (csrc/tableau_general.cu `tma_route` and the eligibility checks of
+`launch_gen_tma`): a batch that fills the pipeline at m = 64, or at m = 16 for tableaus with one g operand, takes the
+TMA-staged kernel; a small batch takes the per-thread-load kernel.  Rows are independent Philox streams, so each test
+launches a batch that takes the TMA-staged kernel, then the same rows again as slices small enough for the
+per-thread-load kernel (counter noise: `row_offset`; memory noise: offset pointers), confirms both routes with the
+launch counters and compares the outputs bit for bit.
 """
+import ctypes
+
 import pytest
 import torch
 
 from . import problems
 
 pytestmark = pytest.mark.gpu
+DEV = 'cuda'
+DT = 2.0 ** -6
+CTA, TMA = 0, 1    # tsde_kernel_launches families
+SLICE = 512        # rows per per-thread-load slice: too few tiles to fill the TMA pipeline at every tested shape
+
+# entry point -> (e operands (rows, d), g operands (rows, d, m), scalar arguments, wants U)
+OPS = {
+    'tsde_step_euler': (2, 1, (DT,), False),
+    'tsde_midpoint_predict': (2, 1, (DT / 2,), False),
+    'tsde_euler_heun_predict': (1, 1, (), False),
+    'tsde_reversible_heun_z': (3, 1, (DT,), False),
+    'tsde_srk_additive_stage': (2, 1, (DT, 1 / DT), True),
+    'tsde_step_heun': (3, 2, (DT,), False),
+    'tsde_step_euler_heun': (2, 2, (DT,), False),
+    'tsde_step_reversible_heun': (3, 2, (DT / 2,), False),
+    'tsde_step_srk_additive': (3, 2, (DT, 1 / DT), True),
+}
+# every (op, m) the TMA-staged kernel is compiled for: one g operand at m = 16 and 64, two g operands at m = 64
+REACHABLE = [(op, m) for op, (_, ng, _, _) in OPS.items() for m in ((16, 64) if ng == 1 else (64,))]
 
 
-def _solve(method, sde_type, kind, B, d, m, dtype, levy, materialise, graph=False):
-    import torchsde_b200 as tsde
-    dev = torch.device('cuda')
-    sde = problems.make(kind, d, m, sde_type, dtype=dtype, seed=11).to(dev)
-    y0 = torch.full((B, d), 0.25, dtype=dtype, device=dev)
-    ts = torch.tensor([0.0, 0.125, 0.25], dtype=dtype, device=dev)
-    bm = tsde.BrownianInterval(0.0, 0.25, size=(B, m), dtype=dtype, device=dev, entropy=99,
-                               levy_area_approximation=levy)
-    if materialise:  # increments handed over as tensors (TSDE_SRC_MEMORY) instead of regenerated from the counter
-        inner = bm
-
-        class Materialised:
-            shape, levy_area_approximation = inner.shape, inner.levy_area_approximation
-
-            def __call__(self, ta, tb=None, return_U=False, return_A=False):
-                return inner(ta, tb, return_U=return_U)
-
-        bm = Materialised()
-    with torch.no_grad():
-        return tsde.sdeint(sde, y0, ts, bm=bm, method=method, dt=2.0 ** -5,
-                           options={'cuda_graph': True} if graph else None).clone()
-
-
-CASES = [
-    # method, sde_type, problem kind, B, d, m, levy       (eligible: d a power of two >= 4, m in {8, 16, 32, 64})
-    ('euler', 'ito', 'general', 1000, 32, 16, 'none'),
-    ('heun', 'stratonovich', 'general', 777, 64, 16, 'none'),          # ragged last tile, two g operands
-    ('midpoint', 'stratonovich', 'general', 513, 8, 8, 'none'),
-    ('euler_heun', 'stratonovich', 'general', 300, 16, 32, 'none'),
-    ('reversible_heun', 'stratonovich', 'general', 260, 16, 8, 'none'),
-    ('srk', 'ito', 'additive', 515, 32, 16, 'space-time'),              # (W, U) weights
-    ('euler', 'ito', 'general', 3, 4, 64, 'none'),                      # fewer tiles than stages
-    ('euler', 'ito', 'general', 2100, 128, 64, 'none'),                 # one 32 KiB row per stage
-]
-
-
-def _launches(family):
+def _launches():
     from torchsde_b200 import _cabi
-    return _cabi.lib().tsde_kernel_launches(family)
+    lib = _cabi.lib()
+    return lib.tsde_kernel_launches(CTA), lib.tsde_kernel_launches(TMA)
+
+
+def _call(op, dtype, rows, d, m, r0, es, gs, w, u, key, out):
+    """One launch of `op` on rows [r0, r0 + rows) of the operands."""
+    from torchsde_b200 import _cabi
+    ne, ng, scalars, want_u = OPS[op]
+    s = torch.finfo(dtype).bits // 8
+    nz = _cabi.Noise()
+    if key is not None:
+        nz.source, nz.key, nz.cell_id, nz.n_cells, nz.h, nz.h_total = _cabi.SRC_COUNTER, key.data_ptr(), 5, 1, DT, DT
+        nz.want_u, nz.row_offset = int(want_u), r0
+    else:
+        nz.source, nz.n_cells, nz.w = _cabi.SRC_MEMORY, 1, w.data_ptr() + r0 * m * s
+        if want_u:
+            nz.want_u, nz.u = 1, u.data_ptr() + r0 * m * s
+    L = _cabi.make_launch(dtype, _cabi.NOISE_GENERAL, rows, d, m)
+    args = [e.data_ptr() + r0 * d * s for e in es] + [g.data_ptr() + r0 * d * m * s for g in gs]
+    _cabi.check(getattr(_cabi.lib(), op)(ctypes.byref(L), ctypes.byref(nz), *args, *scalars,
+                                         out.data_ptr() + r0 * d * s), op)
+
+
+def _whole_and_sliced(op, dtype, B, d, m, memory, first_slice=SLICE):
+    """The launch over all B rows and the same rows launched as slices (the first `first_slice` rows, then SLICE rows
+    at a time); returns both outputs and the (per-thread-load, TMA-staged) launch counts of each."""
+    ne, ng, _, _ = OPS[op]
+    gen = torch.Generator(device=DEV).manual_seed(B * d + m)
+    es = [torch.rand(B, d, generator=gen, device=DEV, dtype=dtype) for _ in range(ne)]
+    gs = [torch.rand(B, d, m, generator=gen, device=DEV, dtype=dtype) - 0.5 for _ in range(ng)]
+    w = u = key = None
+    if memory:
+        w, u = (torch.randn(B, m, generator=gen, device=DEV, dtype=dtype) * DT ** 0.5 for _ in range(2))
+    else:
+        key = torch.tensor([31], dtype=torch.int64, device=DEV)
+    whole, sliced = (torch.full((B, d), float('nan'), device=DEV, dtype=dtype) for _ in range(2))
+    n0 = _launches()
+    _call(op, dtype, B, d, m, 0, es, gs, w, u, key, whole)
+    n1 = _launches()
+    r0 = 0
+    while r0 < B:
+        rows = min(first_slice if r0 == 0 else SLICE, B - r0)
+        _call(op, dtype, rows, d, m, r0, es, gs, w, u, key, sliced)
+        r0 += rows
+    n2 = _launches()
+    return whole, sliced, (n1[0] - n0[0], n1[1] - n0[1]), (n2[0] - n1[0], n2[1] - n1[1])
 
 
 @pytest.mark.parametrize('dtype', [torch.float32, torch.float64], ids=['f32', 'f64'])
-@pytest.mark.parametrize('materialise', [False, True], ids=['counter', 'memory'])
-@pytest.mark.parametrize('case', CASES, ids=lambda c: '-'.join(map(str, c)))
-def test_tma_path_bit_identical(case, materialise, dtype, monkeypatch):
-    method, sde_type, kind, B, d, m, levy = case
-    monkeypatch.setenv('TSDE_GEN_TMA', '0')
-    n_tma = _launches(1)
-    base = _solve(method, sde_type, kind, B, d, m, dtype, levy, materialise)
-    assert _launches(1) == n_tma, "TSDE_GEN_TMA=0 must keep the per-thread-load kernel"
-    monkeypatch.setenv('TSDE_GEN_TMA', '2')
-    n_cta = _launches(0)
-    tma = _solve(method, sde_type, kind, B, d, m, dtype, levy, materialise)
-    if d * m * base.element_size() <= 32 * 1024:  # (fp64 rows of 64 KiB exceed a stage: stays on the default kernel)
-        assert _launches(1) > n_tma and _launches(0) == n_cta, "shape was not routed to the TMA-staged kernel"
-    assert torch.isfinite(base).all()
-    assert torch.equal(base, tma), f"max abs diff {(base - tma).abs().max().item()}"
+@pytest.mark.parametrize('memory', [False, True], ids=['counter', 'memory'])
+@pytest.mark.parametrize('op,m', REACHABLE, ids=[f'{op[5:]}-m{m}' for op, m in REACHABLE])
+def test_tma_path_bit_identical(op, m, memory, dtype):
+    """Every (op, m) the TMA-staged kernel is built for, with a ragged last tile (odd B), against the per-thread-load
+    kernel on the same rows.  The first slice is 3 rows: fewer tiles than stages, which the per-thread-load kernel
+    takes."""
+    B = 65539 if m == 16 else 16387
+    whole, sliced, route, slice_route = _whole_and_sliced(op, dtype, B, 32, m, memory, first_slice=3)
+    assert route == (0, 1), f"B={B} was not routed to the TMA-staged kernel: {route}"
+    n_slices = 1 + -(-(B - 3) // SLICE)
+    assert slice_route == (n_slices, 0), f"slices were not routed to the per-thread-load kernel: {slice_route}"
+    assert torch.isfinite(whole).all()
+    assert torch.equal(whole, sliced), f"max abs diff {(whole - sliced).abs().max().item()}"
 
 
-def test_default_routing(monkeypatch):
-    """Without TSDE_GEN_TMA (r02 routing): once the batch fills the pipeline m = 64 goes to the TMA-staged kernel, and so
-    does m = 16 for tableaus with a single g operand (Euler); two-operand tableaus (Heun) at m = 16 and small batches stay
-    on the per-thread-load kernel."""
-    import ctypes
-    from torchsde_b200 import _cabi
-    monkeypatch.delenv('TSDE_GEN_TMA', raising=False)
-    dev = torch.device('cuda')
-    lib = _cabi.lib()
-    key = torch.tensor([7], dtype=torch.int64, device=dev)
-    for (B, D, M), expect_tma in (((65536, 32, 64), True), ((256, 32, 64), False), ((65536, 32, 16), True),
-                                  ((256, 32, 16), False)):
-        L = _cabi.make_launch(torch.float32, _cabi.NOISE_GENERAL, B, D, M)
-        nz = _cabi.Noise()
-        nz.source, nz.key, nz.cell_id, nz.n_cells, nz.h, nz.h_total = _cabi.SRC_COUNTER, key.data_ptr(), 5, 1, 0.01, 0.01
-        y, f, g = torch.rand(B, D, device=dev), torch.rand(B, D, device=dev), torch.rand(B, D, M, device=dev)
-        outs = []
-        for mode in (None, '0'):
-            if mode is None:
-                monkeypatch.delenv('TSDE_GEN_TMA', raising=False)
-            else:
-                monkeypatch.setenv('TSDE_GEN_TMA', mode)
-            o = torch.empty(B, D, device=dev)
-            before = lib.tsde_kernel_launches(1)
-            _cabi.check(lib.tsde_step_euler(ctypes.byref(L), ctypes.byref(nz), y.data_ptr(), f.data_ptr(),
-                                            g.data_ptr(), 0.01, o.data_ptr()), 'tsde_step_euler')
-            if mode is None:
-                assert (lib.tsde_kernel_launches(1) > before) == expect_tma, (B, D, M)
-            outs.append(o)
-        assert torch.equal(outs[0], outs[1])
-    # two g operands at m = 16: per-thread-load kernel by default
-    B, D, M = 65536, 32, 16
-    L = _cabi.make_launch(torch.float32, _cabi.NOISE_GENERAL, B, D, M)
-    nz = _cabi.Noise()
-    nz.source, nz.key, nz.cell_id, nz.n_cells, nz.h, nz.h_total = _cabi.SRC_COUNTER, key.data_ptr(), 5, 1, 0.01, 0.01
-    e = [torch.rand(B, D, device=dev) for _ in range(4)]
-    g2 = [torch.rand(B, D, M, device=dev) for _ in range(2)]
-    monkeypatch.delenv('TSDE_GEN_TMA', raising=False)
-    before = lib.tsde_kernel_launches(1)
-    _cabi.check(lib.tsde_step_heun(ctypes.byref(L), ctypes.byref(nz), e[0].data_ptr(), e[1].data_ptr(), e[2].data_ptr(),
-                                   g2[0].data_ptr(), g2[1].data_ptr(), 0.01, e[3].data_ptr()), 'tsde_step_heun')
-    assert lib.tsde_kernel_launches(1) == before
+ROUTES = [
+    # entry point, dtype, B, d, m, takes the TMA-staged kernel
+    ('tsde_step_euler', torch.float32, 65536, 32, 64, True),
+    ('tsde_step_euler', torch.float32, 256, 32, 64, False),       # too few tiles to fill the pipeline
+    ('tsde_step_euler', torch.float32, 3, 4, 64, False),          # fewer tiles than stages
+    ('tsde_step_euler', torch.float32, 65536, 32, 16, True),
+    ('tsde_step_euler', torch.float32, 256, 32, 16, False),
+    ('tsde_step_euler', torch.float32, 65536, 32, 8, False),      # m = 8 and 32: per-thread loads at every size
+    ('tsde_midpoint_predict', torch.float32, 65536, 16, 32, False),
+    ('tsde_step_heun', torch.float32, 65536, 32, 16, False),      # two g operands at m = 16
+    ('tsde_step_euler_heun', torch.float64, 32768, 16, 16, False),
+    ('tsde_step_euler', torch.float32, 2100, 128, 64, True),      # one 32 KiB g row per stage
+    ('tsde_step_euler', torch.float64, 2100, 128, 64, False),     # a 64 KiB row exceeds a stage
+]
 
 
-def test_tma_path_in_cuda_graph(monkeypatch):
-    monkeypatch.setenv('TSDE_GEN_TMA', '0')
-    base = _solve('heun', 'stratonovich', 'general', 2048, 32, 16, torch.float32, 'none', False)
-    monkeypatch.setenv('TSDE_GEN_TMA', '2')
-    tma = _solve('heun', 'stratonovich', 'general', 2048, 32, 16, torch.float32, 'none', False, graph=True)
-    assert torch.equal(base, tma)
+def test_default_routing():
+    """The route of each shape, and its output equal to the per-thread-load kernel's on slices of the same rows."""
+    bad = []
+    for op, dtype, B, d, m, tma in ROUTES:
+        whole, sliced, route, slice_route = _whole_and_sliced(op, dtype, B, d, m, memory=False)
+        if route != ((0, 1) if tma else (1, 0)) or slice_route[1] != 0 or slice_route[0] < 1:
+            bad.append(f'{op} {dtype} B={B} d={d} m={m}: routes {route}, slices {slice_route}')
+        elif not torch.equal(whole, sliced):
+            bad.append(f'{op} {dtype} B={B} d={d} m={m}: output differs from the per-thread-load slices')
+    assert not bad, '; '.join(bad)
+
+
+def test_tma_path_in_cuda_graph():
+    """A graph-captured Heun solve at m = 64 (both tableaus on the TMA-staged kernel) equals the same solve split with
+    `shard_rows` into slices that take the per-thread-load kernel, bit for bit."""
+    import torchsde_b200 as tsde
+    B, d, m = 8192, 32, 64
+    sde = problems.make('general', d, m, 'stratonovich', dtype=torch.float32, seed=11).to(DEV)
+    y0 = torch.full((B, d), 0.25, device=DEV)
+    ts = torch.tensor([0.0, 0.125, 0.25], device=DEV)
+
+    def solve(rows, r0, graph):
+        bm = tsde.BrownianInterval(0.0, 0.25, size=(rows, m), dtype=torch.float32, device=DEV, entropy=99)
+        bm.shard_rows(r0)
+        with torch.no_grad():
+            return tsde.sdeint(sde, y0[r0:r0 + rows].contiguous(), ts, bm=bm, method='heun', dt=2.0 ** -5,
+                               options={'cuda_graph': True} if graph else None).clone()
+
+    n0 = _launches()
+    whole = solve(B, 0, graph=True)
+    n1 = _launches()
+    parts = [solve(min(SLICE, B - r0), r0, graph=False) for r0 in range(0, B, SLICE)]
+    n2 = _launches()
+    assert n1[1] > n0[1], "the captured solve did not take the TMA-staged kernel"
+    assert n2[1] == n1[1] and n2[0] > n1[0], "the sliced solves did not take the per-thread-load kernel"
+    assert torch.equal(whole, torch.cat(parts, dim=1))

@@ -19,7 +19,6 @@ What changed underneath:
 """
 import abc
 import ctypes
-import os
 import warnings
 
 import torch
@@ -299,7 +298,7 @@ class BaseSDESolver(metaclass=abc.ABCMeta):
     # their kernels' launch latencies overlap instead of adding up.  That is what limits small-state workloads: at
     # the cfg3 size (1 MiB states) a step is a chain of 4-30 tiny PyTorch kernels of the user's f / g at ~2.5 us of
     # dependent-launch latency each, while the solver's own kernels take a few us.  On by default;
-    # `options={'overlap': False}` (or TSDE_OVERLAP=0) turns it off.
+    # `options={'overlap': False}` turns it off.
     # Memory discipline: a branch's results are allocated on its side stream and consumed on the main stream after
     # the join; they are freed (returned to the side stream's pool) only after that consumer has been enqueued, and
     # the side stream reuses the block only after its next fork, i.e. after waiting for the main stream — so no
@@ -309,10 +308,7 @@ class BaseSDESolver(metaclass=abc.ABCMeta):
     def _overlap_now(self):
         if self._autograd:
             return False  # (AccumulateGrad nodes remember the stream they were created on: keep one stream)
-        opt = self.options.get('overlap', self.options.get('overlap_drift', None))
-        env = os.environ.get('TSDE_OVERLAP')
-        if env is not None and opt is None:
-            opt = env not in ('0', '')
+        opt = self.options.get('overlap')
         return True if opt is None else bool(opt)
 
     def _fork(self, *thunks, main=0):

@@ -306,14 +306,8 @@ __device__ __forceinline__ T levy_pair_value(T wi, T wj, T hi, T hj, T z, T tent
 constexpr int kLevyWarps = 8;
 // Register budget of the fp32 compile-time-m instantiations, as the minimum number of resident CTAs per SM they are
 // compiled for (65536 / (256 n) registers per thread).  n = 2 leaves the compiler the registers it takes when it may:
-// the issue-bound kernel prefers the longer instruction schedule to more resident warps.  Overridable for A/B builds
-// (-DTSDE_LEVY_CTAS=4).
-#ifndef TSDE_LEVY_CTAS
-#define TSDE_LEVY_CTAS 2
-#endif
-#ifndef TSDE_LEVY_CTAS_GEN
-#define TSDE_LEVY_CTAS_GEN 2
-#endif
+// the issue-bound kernel prefers the longer instruction schedule to more resident warps.
+constexpr int kLevyCtasF32 = 2;
 
 // Rows a warp handles per pass in the generating mode: the W and H normals of one row are only m/2 Philox quads, so
 // one warp-wide pass draws them for 32 / (m/2) rows at once (m = 16: 4 rows) instead of leaving most lanes idle.
@@ -327,40 +321,37 @@ __host__ __device__ constexpr int levy_tile_elems(int m, bool gen) {
 
 // The four pairs of one Philox quad: operands through per-lane shared-memory pointers looked up once per kernel
 // (slots past the last pair point at the scratch word, so the pass has no per-pair branch).
-#ifndef TSDE_LEVY_PACKED
-#define TSDE_LEVY_PACKED 1
-#endif
-// fp32: two pairs at a time through the f32x2 helpers of philox.cuh (explicitly rounded, never contracted).
-// The cross term H_i W_j - W_i H_j keeps its three roundings (the subtraction is fma(x, -1, y): the product by -1 is
-// exact).  The sum of squares under the root and the final std * noise + cross term are fused multiply-adds, written
-// out as such, so the source says what runs.  The result differs from the scalar pass (fp64, m > 16) by at most an ulp of the noise
-// term; the area's noise is a fresh draw per query and pinned to the oracle by tolerance, A = -A^T stays exact.
+// fp32: two pairs side by side (both pairs' operands are loaded before either result is stored), one explicitly
+// rounded operation of each per line (never contracted).  The cross term H_i W_j - W_i H_j keeps its three roundings (the subtraction
+// is fma(x, -1, y): the product by -1 is exact).  The sum of squares under the root and the final std * noise + cross
+// term are fused multiply-adds, written out as such, so the source says what runs.  The result differs from the
+// scalar pass (fp64, m > 16) by at most an ulp of the noise term; the area's noise is a fresh draw per query and
+// pinned to the oracle by tolerance, A = -A^T stays exact.
 template <bool FOSTER>
-__device__ __forceinline__ void levy_quad_pairs_f32x2(const float* const (&pw_i)[4], const float* const (&pw_j)[4],
-                                                      int off, int m, float* const (&pa)[4], float* const (&pb)[4],
-                                                      const float (&z)[4], float tenth_h, float davie_std) {
+__device__ __forceinline__ void levy_quad_pairs_f32(const float* const (&pw_i)[4], const float* const (&pw_j)[4],
+                                                    int off, int m, float* const (&pa)[4], float* const (&pb)[4],
+                                                    const float (&z)[4], float tenth_h, float davie_std) {
   const float c2 = 2.0f * 0.70710678118654752440f;
 #pragma unroll
   for (int k = 0; k < 4; k += 2) {
-    const f32x2 wi = pack2(pw_i[k][off], pw_i[k + 1][off]);
-    const f32x2 wj = pack2(pw_j[k][off], pw_j[k + 1][off]);
-    const f32x2 hi = pack2(pw_i[k][off + m], pw_i[k + 1][off + m]);
-    const f32x2 hj = pack2(pw_j[k][off + m], pw_j[k + 1][off + m]);
-    const f32x2 a = fma2(mul2(wi, hj), pack2(-1.0f, -1.0f), mul2(hi, wj));   // hi wj - wi hj
-    const f32x2 noise = mul2(pack2(z[k], z[k + 1]), pack2(c2, c2));
-    f32x2 sd;
+    const float wi0 = pw_i[k][off], wi1 = pw_i[k + 1][off];
+    const float wj0 = pw_j[k][off], wj1 = pw_j[k + 1][off];
+    const float hi0 = pw_i[k][off + m], hi1 = pw_i[k + 1][off + m];
+    const float hj0 = pw_j[k][off + m], hj1 = pw_j[k + 1][off + m];
+    // a = hi wj - wi hj
+    const float x0 = __fmul_rn(wi0, hj0), x1 = __fmul_rn(wi1, hj1);
+    const float y0 = __fmul_rn(hi0, wj0), y1 = __fmul_rn(hi1, wj1);
+    const float a0 = __fmaf_rn(x0, -1.0f, y0), a1 = __fmaf_rn(x1, -1.0f, y1);
+    const float n0 = __fmul_rn(z[k], c2), n1 = __fmul_rn(z[k + 1], c2);
+    float sd0 = davie_std, sd1 = davie_std;
     if (FOSTER) {
-      const f32x2 t = pack2(tenth_h, tenth_h);
-      const f32x2 s = mul2(t, fma2(hj, hj, fma2(hi, hi, t)));
-      float s0, s1;
-      unpack2(s, s0, s1);
-      sd = pack2(levy_sqrt(s0), levy_sqrt(s1));
-    } else {
-      sd = pack2(davie_std, davie_std);
+      const float e0 = __fmaf_rn(hi0, hi0, tenth_h), e1 = __fmaf_rn(hi1, hi1, tenth_h);
+      const float f0 = __fmaf_rn(hj0, hj0, e0), f1 = __fmaf_rn(hj1, hj1, e1);
+      const float s0 = __fmul_rn(tenth_h, f0), s1 = __fmul_rn(tenth_h, f1);
+      sd0 = levy_sqrt(s0);
+      sd1 = levy_sqrt(s1);
     }
-    const f32x2 v = fma2(sd, noise, a);
-    float v0, v1;
-    unpack2(v, v0, v1);
+    const float v0 = __fmaf_rn(sd0, n0, a0), v1 = __fmaf_rn(sd1, n1, a1);
     *pa[k] = v0;
     *pb[k] = -v0;
     *pa[k + 1] = v1;
@@ -372,8 +363,8 @@ template <typename T, bool FOSTER>
 __device__ __forceinline__ void levy_quad_pairs(const T* const (&pw_i)[4], const T* const (&pw_j)[4], int off, int m,
                                                 T* const (&pa)[4], T* const (&pb)[4], const T (&z)[4], T tenth_h,
                                                 T davie_std) {
-  if constexpr (TSDE_LEVY_PACKED && sizeof(T) == 4) {
-    levy_quad_pairs_f32x2<FOSTER>(pw_i, pw_j, off, m, pa, pb, z, tenth_h, davie_std);
+  if constexpr (sizeof(T) == 4) {
+    levy_quad_pairs_f32<FOSTER>(pw_i, pw_j, off, m, pa, pb, z, tenth_h, davie_std);
   } else {
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -391,7 +382,7 @@ __device__ __forceinline__ void levy_quad_pairs(const T* const (&pw_i)[4], const
 // MT: the channel count as a compile-time constant (0 = run-time `m_rt`); with it the tile stride, the pair count
 // and the copy-out pattern fold into immediates.
 template <typename T, bool GEN, int MT>
-__global__ void __launch_bounds__(kLevyWarps * 32, (MT && sizeof(T) == 4) ? (GEN ? TSDE_LEVY_CTAS_GEN : TSDE_LEVY_CTAS) : 3)
+__global__ void __launch_bounds__(kLevyWarps * 32, (MT && sizeof(T) == 4) ? kLevyCtasF32 : 3)
 levy_tile_kernel(const void* keyp, int64_t row_offset, uint64_t a_id, int64_t rows, int m_rt, int warps,
                  const T* __restrict__ w, const T* __restrict__ hh, T tenth_h, T davie_std, int foster,
                  T* __restrict__ out, int vec, uint64_t cell_id, T sqrt_h, T sqrt_h12, T ht, T* __restrict__ out_w,

@@ -11,7 +11,6 @@
 // contiguous slice of the quads.
 #pragma once
 #include <stdint.h>
-#include <stdlib.h>
 
 #include "host.cuh"
 #include "philox.cuh"
@@ -21,24 +20,6 @@ namespace tsde {
 
 constexpr int kThreads = 256;
 constexpr int kBlocksPerSM = 8;  // 2048 threads / SM
-
-inline bool stream_loads_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("TSDE_STREAM");
-    v = (e && e[0] == '0') ? 0 : 1;  // on by default; TSDE_STREAM=0 for A/B measurements
-  }
-  return v == 1;
-}
-
-inline bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("TSDE_PDL");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
 
 template <typename T>
 struct NoiseP {
@@ -315,7 +296,7 @@ struct FastCtx {
   Key key;
   uint32_t q_end, qshift, qmask, qpr32, row_off;
   uint64_t qmagic;
-  bool pow2, stream_hint;
+  bool pow2;
   __device__ __forceinline__ uint32_t row_of(uint32_t Q) const {
     return pow2 ? (Q >> qshift) : rowdiv_row(Q, qmagic);
   }
@@ -344,7 +325,7 @@ __device__ __forceinline__ void ew_fast_body(const FastCtx<T, Op>& c, uint32_t Q
     if (ok[k]) {
 #pragma unroll
       for (int i = 0; i < NIN; ++i) {
-        if (streams_inputs<Op>::value && c.stream_hint)
+        if (streams_inputs<Op>::value)
           ld4cs(reinterpret_cast<const T*>(c.p.in[i]) + base, in[k][i]);
         else
           ld4(reinterpret_cast<const T*>(c.p.in[i]) + base, in[k][i]);
@@ -411,8 +392,7 @@ ew_fast_kernel(const EwP<Op::NIN, Op::NOUT> p, const NoiseP<T> nz, const Op op) 
   const bool pow2 = p.qshift >= 0;
   const uint32_t qshift = pow2 ? (uint32_t)p.qshift : 0u;
   const FastCtx<T, Op> c{p, nz, op, COUNTER ? load_key(nz.key) : Key{0u, 0u}, nquads, qshift, (1u << qshift) - 1u,
-                         (uint32_t)p.qpr, (uint32_t)nz.row_offset, p.qmagic, pow2,
-                         p.vec > 1 /* host sets vec = 2 to enable evict-first loads */};
+                         (uint32_t)p.qpr, (uint32_t)nz.row_offset, p.qmagic, pow2};
   // Programmatic dependent launch: this grid may start while its predecessor in the stream/graph is
   // still draining.  Everything that does not touch the predecessor's outputs — the Philox/Box-Muller
   // work of the thread's U quads — runs before `griddepcontrol.wait`; all loads and stores come after.
@@ -484,7 +464,7 @@ inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
   p.d = L->d;
   p.qpr = (L->d + 3) / 4;
   p.nquads = p.rows * p.qpr;
-  p.vec = vec ? (stream_loads_enabled() ? 2 : 1) : 0;
+  p.vec = vec ? 1 : 0;
   p.qshift = -1;
   if ((p.qpr & (p.qpr - 1)) == 0 && p.qpr < (1ll << 30)) {
     int sh = 0;
@@ -496,17 +476,16 @@ inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
   // (every quads-per-row divides exactly on the fast path: its quad indices are 32-bit, see rowdiv.cuh)
   const bool fast = p.vec && !bcast && p.small && np.n_cells == 1 &&
                     (L->rows + (nz ? nz->row_offset : 0)) < kMaxGlobalRows;
-  const bool pdl = fast && pdl_enabled();
   const cudaStream_t stream = reinterpret_cast<cudaStream_t>(L->stream);
   auto go = [&](auto kernel) -> int {
     // Persistent, balanced grid: small problems get one quad per thread, large ones one wave of resident CTAs, each
     // owning an equal contiguous slice.
     int per_sm = resident_ctas(reinterpret_cast<const void*>(kernel), kThreads, 0);
     if (per_sm < 1) per_sm = 1;
-    return launch_kernel(kernel, capped_grid(p.nquads, kThreads, per_sm), kThreads, 0, stream, pdl, p, np, op);
+    return launch_kernel(kernel, capped_grid(p.nquads, kThreads, per_sm), kThreads, 0, stream, false, p, np, op);
   };
-  auto go_fast = [&](auto kernel) -> int {
-    return launch_kernel(kernel, fast_chunks<T, Op>((uint32_t)p.nquads), kThreads, 0, stream, pdl, p, np, op);
+  auto go_fast = [&](auto kernel) -> int {  // programmatic dependent launch (see ew_fast_kernel)
+    return launch_kernel(kernel, fast_chunks<T, Op>((uint32_t)p.nquads), kThreads, 0, stream, true, p, np, op);
   };
   if constexpr (!Op::USES_NOISE) {
     if (fast) return go_fast(ew_fast_kernel<T, Op, TSDE_SRC_UNIT>);

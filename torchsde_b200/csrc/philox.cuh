@@ -65,7 +65,7 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1
 //     [1, 2) — one funnel shift instead of an int->float conversion and a multiply — and
 //     theta = 2 pi (fb - 1.5) = 2 pi b - pi lies in [-pi, pi) where sin/cos.approx are accurate (~5e-7 abs);
 //     cos(2 pi b) = -cos(theta), sin(2 pi b) = -sin(theta);
-//   * evaluates the two pairs of a quad side by side (f32x2 below), each lane with explicitly rounded operations.
+//   * evaluates the two pairs of a quad side by side, with explicitly rounded operations.
 // Agreement with the float64 oracle: a few 1e-7 relative on r, <= ~1e-6 absolute on a normal.
 __device__ __forceinline__ float mufu_lg2(float x) {
   float y;
@@ -88,52 +88,38 @@ __device__ __forceinline__ float mufu_cos(float x) {
   return y;
 }
 
-// fp32 pair helpers: the two lanes are independent IEEE operations with explicit rounding (never contracted or
-// reassociated, whatever -fmad says), so a pair gives the same bits as two scalar expressions.  sm_90 has no packed
-// fp32x2 arithmetic; each helper is two scalar instructions.
-struct f32x2 {
-  float lo, hi;
-};
-__device__ __forceinline__ f32x2 pack2(float lo, float hi) { return f32x2{lo, hi}; }
-__device__ __forceinline__ void unpack2(f32x2 v, float& lo, float& hi) {
-  lo = v.lo;
-  hi = v.hi;
-}
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-  return f32x2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)};
-}
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { return f32x2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) { return f32x2{__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
-
-// four normals from one Philox output: (x.x, x.y) -> n0, n1 ; (x.z, x.w) -> n2, n3
+// four normals from one Philox output: (x.x, x.y) -> n0, n1 ; (x.z, x.w) -> n2, n3.  The two pairs go side by side,
+// one explicitly rounded operation of each per line (never contracted or reassociated, whatever -fmad says).
 __device__ __forceinline__ void box_muller4(const uint4 x, float (&n)[4]) {
-  const f32x2 k2m32 = pack2(2.3283064365386963e-10f, 2.3283064365386963e-10f);
-  const f32x2 k2m33 = pack2(1.1641532182693481e-10f, 1.1641532182693481e-10f);
-  // radius uniforms a = fma(float(x), 2^-32, 2^-33), both pairs at once
-  const f32x2 a = fma2(pack2(__uint2float_rn(x.x), __uint2float_rn(x.z)), k2m32, k2m33);
-  float a0, a1;
-  unpack2(a, a0, a1);
+  const float k2m32 = 2.3283064365386963e-10f, k2m33 = 1.1641532182693481e-10f;
+  // radius uniforms a = fma(float(x), 2^-32, 2^-33)
+  const float x0 = __uint2float_rn(x.x), x1 = __uint2float_rn(x.z);
+  const float a0 = __fmaf_rn(x0, k2m32, k2m33), a1 = __fmaf_rn(x1, k2m32, k2m33);
   // r^2 through the SFU ...
-  const f32x2 via_log = mul2(pack2(mufu_lg2(a0), mufu_lg2(a1)), pack2(-1.3862943611198906f, -1.3862943611198906f));
+  const float lg0 = mufu_lg2(a0), lg1 = mufu_lg2(a1);
+  const float l0 = __fmul_rn(lg0, -1.3862943611198906f), l1 = __fmul_rn(lg1, -1.3862943611198906f);
   // ... and through the series in v = 1 - a (exact), used where a is within 2^-8 of 1
-  const f32x2 v = add2(pack2(1.0f, 1.0f), mul2(a, pack2(-1.0f, -1.0f)));
-  const f32x2 poly = fma2(v, fma2(v, pack2(0.33333334f, 0.33333334f), pack2(0.5f, 0.5f)), pack2(1.0f, 1.0f));
-  const f32x2 series = mul2(add2(v, v), poly);
-  float l0, l1, s0, s1;
-  unpack2(via_log, l0, l1);
-  unpack2(series, s0, s1);
+  const float na0 = __fmul_rn(a0, -1.0f), na1 = __fmul_rn(a1, -1.0f);
+  const float v0 = __fadd_rn(1.0f, na0), v1 = __fadd_rn(1.0f, na1);
+  const float q0 = __fmaf_rn(v0, 0.33333334f, 0.5f), q1 = __fmaf_rn(v1, 0.33333334f, 0.5f);
+  const float p0 = __fmaf_rn(v0, q0, 1.0f), p1 = __fmaf_rn(v1, q1, 1.0f);
+  const float d0 = __fadd_rn(v0, v0), d1 = __fadd_rn(v1, v1);
+  const float s0 = __fmul_rn(d0, p0), s1 = __fmul_rn(d1, p1);
   const float r0 = mufu_sqrt(x.x >= 0xFF000000u ? s0 : l0);
   const float r1 = mufu_sqrt(x.z >= 0xFF000000u ? s1 : l1);
   // angles: mantissa construction, theta = 2 pi (fb - 1.5) in [-pi, pi); fb - 1.5 is exact, so theta carries one
   // rounding and the rounding of the constant (<= 2.7e-7 absolute)
-  const f32x2 fb = pack2(__uint_as_float(__funnelshift_r(x.y, 0x7Fu, 9)), __uint_as_float(__funnelshift_r(x.w, 0x7Fu, 9)));
-  const f32x2 th = mul2(add2(fb, pack2(-1.5f, -1.5f)), pack2(6.2831853071795865f, 6.2831853071795865f));
-  float t0, t1;
-  unpack2(th, t0, t1);
-  const f32x2 p0 = mul2(pack2(mufu_cos(t0), mufu_sin(t0)), pack2(-r0, -r0));
-  const f32x2 p1 = mul2(pack2(mufu_cos(t1), mufu_sin(t1)), pack2(-r1, -r1));
-  unpack2(p0, n[0], n[1]);
-  unpack2(p1, n[2], n[3]);
+  const float fb0 = __uint_as_float(__funnelshift_r(x.y, 0x7Fu, 9)), fb1 = __uint_as_float(__funnelshift_r(x.w, 0x7Fu, 9));
+  const float c0 = __fadd_rn(fb0, -1.5f), c1 = __fadd_rn(fb1, -1.5f);
+  const float t0 = __fmul_rn(c0, 6.2831853071795865f), t1 = __fmul_rn(c1, 6.2831853071795865f);
+  const float cos0 = mufu_cos(t0), sin0 = mufu_sin(t0);
+  const float n0 = __fmul_rn(cos0, -r0), n1 = __fmul_rn(sin0, -r0);
+  const float cos1 = mufu_cos(t1), sin1 = mufu_sin(t1);
+  const float n2 = __fmul_rn(cos1, -r1), n3 = __fmul_rn(sin1, -r1);
+  n[0] = n0;
+  n[1] = n1;
+  n[2] = n2;
+  n[3] = n3;
 }
 
 // four normals for channels 4q..4q+3 of (row, id, stream)

@@ -582,37 +582,26 @@ gen_tma_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const O
   }
 }
 
-// Which launches take the TMA-staged kernel (TSDE_GEN_TMA):
-//   unset  when the batch fills the pipeline:  m = 64 always, and m = 16 for tableaus with ONE g operand (with two g
-//          operands the per-thread-load kernel already keeps enough bytes in flight);  m = 8, 32: per-thread-load kernel;
-//   0      never;   1  every eligible shape when the batch fills the pipeline;   2  every eligible shape.
-// Both kernels are bit-identical (tests/test_gpu_general_tma.py), so the choice never changes results.
-inline int gen_tma_mode(int64_t mq, int n_g_operands) {
-  const char* e = getenv("TSDE_GEN_TMA");
-  if (!e) return (mq == 16 || (mq == 4 && n_g_operands == 1)) ? 1 : 0;
-  if (e[0] == '0') return 0;
-  if (e[0] == '2' || e[0] == 'f') return 2;
-  return 1;
-}
+// Which tiles take the TMA-staged kernel, when the batch fills the pipeline: m = 64 always, and m = 16 for tableaus
+// with ONE g operand (with two g operands the per-thread-load kernel already keeps enough bytes in flight); m = 8 and
+// m = 32 stay on the per-thread-load kernel.  Both kernels are bit-identical (tests/test_gpu_general_tma.py), so the
+// route never changes results.  gen_tma_kernel is instantiated for exactly these (op, m / 4) pairs.
+template <typename Op>
+constexpr bool tma_route(int64_t mq) { return mq == 16 || (Op::NG == 1 && mq == 4); }
 
 constexpr int kTmaNotEligible = -12345;
 
 template <typename T, typename Op>
 static int launch_gen_tma(const tsde_launch* L, const tsde_noise* nz, GenP<Op::NE, Op::NG, Op::NO> p,
-                          const NoiseP<T>& np, const Op& op, int mode, cudaStream_t st) {
+                          const NoiseP<T>& np, const Op& op, cudaStream_t st) {
   // Eligibility: bulk copies need 16-byte aligned, 16-byte-multiple extents for every operand tile.
   if (L->d % 4 != 0 || (L->d & (L->d - 1)) != 0 || L->d > (1 << 20)) return kTmaNotEligible;  // d = 2^k >= 4
   for (int i = 0; i < Op::NE; ++i) if (!aligned16(p.e[i])) return kTmaNotEligible;
   const int64_t mq = L->m / 4;
-  if (mq != 2 && mq != 4 && mq != 8 && mq != 16) return kTmaNotEligible;  // instantiated shuffle trees
   const size_t row_bytes = (size_t)L->d * L->m * sizeof(T);
   // 16 KiB of every g operand per stage (several resident CTAs per SM keep the ring full; the 200 KiB cap below stays
   // within the 227 KiB of shared memory one CTA may use)
-  size_t kStageTarget = (size_t)Op::NG * 16 * 1024;
-  if (const char* e = getenv("TSDE_GEN_TMA_KB")) {  // tuning knob, KiB per operand
-    const long kb = atol(e);
-    if (kb >= 1 && kb <= 48) kStageTarget = (size_t)Op::NG * kb * 1024;
-  }
+  constexpr size_t kStageTarget = (size_t)Op::NG * 16 * 1024;
   if (Op::NG * row_bytes > 32 * 1024 && Op::NG * row_bytes > kStageTarget) return kTmaNotEligible;
   int64_t rs = (int64_t)(kStageTarget / (Op::NG * row_bytes));
   if (rs < 1) rs = 1;
@@ -635,18 +624,16 @@ static int launch_gen_tma(const tsde_launch* L, const tsde_noise* nz, GenP<Op::N
     const int resident = resident_ctas(reinterpret_cast<const void*>(kernel), kTmaThreads + 32, smem);
     if (resident < 1) return kTmaNotEligible;
     const int64_t cap = (int64_t)sm_count() * resident;
-    if (mode < 2 && tp.n_tiles < 2 * kTmaStages * cap) return kTmaNotEligible;  // too small to fill the pipeline
+    if (tp.n_tiles < 2 * kTmaStages * cap) return kTmaNotEligible;  // too small to fill the pipeline
     g_launches[TSDE_KERNEL_GEN_TMA].fetch_add(1, std::memory_order_relaxed);
-    return launch_kernel(kernel, tp.n_tiles < cap ? tp.n_tiles : cap, kTmaThreads + 32, smem, st, pdl_enabled(), p,
-                         np, op, tp);
+    return launch_kernel(kernel, tp.n_tiles < cap ? tp.n_tiles : cap, kTmaThreads + 32, smem, st, true, p, np, op,
+                         tp);
   };
   const bool mem = nz->source == TSDE_SRC_MEMORY;
-  switch (mq) {
-    case 2: return mem ? go(gen_tma_kernel<T, Op, TSDE_SRC_MEMORY, 1>) : go(gen_tma_kernel<T, Op, TSDE_SRC_COUNTER, 1>);
-    case 4: return mem ? go(gen_tma_kernel<T, Op, TSDE_SRC_MEMORY, 2>) : go(gen_tma_kernel<T, Op, TSDE_SRC_COUNTER, 2>);
-    case 8: return mem ? go(gen_tma_kernel<T, Op, TSDE_SRC_MEMORY, 3>) : go(gen_tma_kernel<T, Op, TSDE_SRC_COUNTER, 3>);
-    default: return mem ? go(gen_tma_kernel<T, Op, TSDE_SRC_MEMORY, 4>) : go(gen_tma_kernel<T, Op, TSDE_SRC_COUNTER, 4>);
+  if constexpr (Op::NG == 1) {
+    if (mq == 4) return mem ? go(gen_tma_kernel<T, Op, TSDE_SRC_MEMORY, 2>) : go(gen_tma_kernel<T, Op, TSDE_SRC_COUNTER, 2>);
   }
+  return mem ? go(gen_tma_kernel<T, Op, TSDE_SRC_MEMORY, 4>) : go(gen_tma_kernel<T, Op, TSDE_SRC_COUNTER, 4>);  // m = 64
 }
 
 template <typename T, typename Op>
@@ -676,8 +663,8 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
   const bool mem = nz->source == TSDE_SRC_MEMORY;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
   if (vec) {
-    if (int mode = p.gbcast ? 0 : gen_tma_mode(mq, Op::NG)) {  // (a broadcast g has no tile stream to stage)
-      int rc = launch_gen_tma<T, Op>(L, nz, p, np, op, mode, st);
+    if (!p.gbcast && tma_route<Op>(mq)) {  // (a broadcast g has no tile stream to stage)
+      int rc = launch_gen_tma<T, Op>(L, nz, p, np, op, st);
       if (rc != kTmaNotEligible) return rc;
     }
     // one 128-thread CTA per group of rw rows
@@ -688,7 +675,7 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
     const size_t smem = (size_t)rw * L->m * sizeof(T) * (Op::WANT_U ? 2 : 1);
     g_launches[TSDE_KERNEL_GEN_CTA].fetch_add(1, std::memory_order_relaxed);
     return launch_kernel(mem ? gen_cta_kernel<T, Op, TSDE_SRC_MEMORY> : gen_cta_kernel<T, Op, TSDE_SRC_COUNTER>,
-                         ngroups, kGenThreads, smem, st, pdl_enabled(), p, np, op);
+                         ngroups, kGenThreads, smem, st, true, p, np, op);
   }
   // generic path: rows per block ~16 work items per thread, bounded by shared memory for the increments
   const int64_t per_row = L->d;
