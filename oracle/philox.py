@@ -36,6 +36,19 @@ def _box_muller(a, b):
     return r * np.cos(th), r * np.sin(th)
 
 
+def _box_muller_f64(a, b):
+    """BoxMuller(a, b) with cos / sin of 2 pi b evaluated as the device's sincospi(2 b) does: b is reduced exactly to
+    the nearest quarter turn, so both keep their relative accuracy near their zeros.  (`cos(2.0 * pi * b)` rounds the
+    angle by up to ~4e-16 absolute, ~20 ulp of a normal close to zero.)"""
+    r = np.sqrt(-2.0 * np.log(a))
+    t = 4.0 * b                          # exact
+    k = np.rint(t)
+    th = (t - k) * (0.5 * np.pi)         # t - k exact, |th| <= pi / 4
+    c, s = np.cos(th), np.sin(th)
+    k = k.astype(np.int64) & 3           # 2 pi b = k pi / 2 + th
+    return r * np.choose(k, [c, -s, -c, s]), r * np.choose(k, [s, c, -s, -c])
+
+
 def normals(key, node_id, stream, rows, m, dtype, row_offset=0, row_ids=None):
     """(rows, m) normals of (key, node_id, stream).  Mirrors normal4() for every quad.
 
@@ -81,6 +94,6 @@ def normals(key, node_id, stream, rows, m, dtype, row_offset=0, row_ids=None):
                   .astype(np.float64) + 0.5) * 1.1102230246251565e-16
             ub = ((((x[2].astype(np.uint64) << np.uint64(32)) | x[3].astype(np.uint64)) >> np.uint64(11))
                   .astype(np.float64) + 0.5) * 1.1102230246251565e-16
-            n0, n1 = _box_muller(ua, ub)
+            n0, n1 = _box_muller_f64(ua, ub)
             out[:, 2 * call::4], out[:, 2 * call + 1::4] = n0, n1
     return out[:, :m].astype(dtype)

@@ -1,4 +1,6 @@
 """Shared helpers of the parity tests."""
+import collections
+import ctypes
 import glob
 import os
 
@@ -8,6 +10,67 @@ import torch
 from . import problems
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
+
+
+# ---- the general-noise entry points, called through the C ABI ------------------------------------------------------
+GEN_DT = 2.0 ** -6
+# args / outs: the operands / outputs in argument order, 'e' for a (rows, d) tensor and 'g' for a (rows, d, m) one;
+# tile_g: g operands of the (rows, d, m) tile kernel the entry point launches (the adjoint halves also launch
+# element-wise and outer-product kernels)
+GeneralOp = collections.namedtuple('GeneralOp', 'args scalars want_u outs tile_g')
+GENERAL_OPS = {
+    'tsde_step_euler': GeneralOp('eeg', (GEN_DT,), False, 'e', 1),
+    'tsde_midpoint_predict': GeneralOp('eeg', (GEN_DT / 2,), False, 'e', 1),
+    'tsde_euler_heun_predict': GeneralOp('eg', (), False, 'e', 1),
+    'tsde_reversible_heun_z': GeneralOp('eeeg', (GEN_DT,), False, 'e', 1),
+    'tsde_srk_additive_stage': GeneralOp('eeg', (GEN_DT, 1 / GEN_DT), True, 'e', 1),
+    'tsde_adjoint_reversible_heun_a': GeneralOp('eeegeeg', (GEN_DT, GEN_DT / 2), False, 'eeg', 1),
+    'tsde_step_heun': GeneralOp('eeegg', (GEN_DT,), False, 'e', 2),
+    'tsde_step_euler_heun': GeneralOp('eegg', (GEN_DT,), False, 'e', 2),
+    'tsde_step_reversible_heun': GeneralOp('eeegg', (GEN_DT / 2,), False, 'e', 2),
+    'tsde_step_srk_additive': GeneralOp('eeegg', (GEN_DT, 1 / GEN_DT), True, 'e', 2),
+    'tsde_adjoint_reversible_heun_b': GeneralOp('eeeggeee', (GEN_DT, GEN_DT / 2), False, 'eeeeg', 2),
+}
+# every (op, m) the TMA-staged tile kernel is compiled for: one tile g operand at m = 16 and 64, two at m = 64
+GENERAL_TMA_REACHABLE = [(op, m) for op, spec in GENERAL_OPS.items() for m in ((16, 64) if spec.tile_g == 1 else (64,))]
+# the entry points that accept TSDE_FLAG_G_BROADCAST (the reversible-Heun family keeps its g operands dense)
+GENERAL_BROADCAST_OPS = [op for op in GENERAL_OPS if 'reversible_heun' not in op]
+# the entry points cabi.cu routes to the row-wise kernels at m = 1 (the SRK-additive pair keeps the tile kernels)
+GENERAL_ROWWISE_OPS = [op for op in GENERAL_OPS if 'srk_additive' not in op]
+GEN_CTA, GEN_TMA = 0, 1  # tsde_kernel_launches families
+
+
+def tile_launches():
+    """(per-thread-load, TMA-staged) general-noise tile kernel launches this process has issued so far."""
+    from torchsde_b200 import _cabi
+    lib = _cabi.lib()
+    return lib.tsde_kernel_launches(GEN_CTA), lib.tsde_kernel_launches(GEN_TMA)
+
+
+def general_noise(key=None, cell_id=0, h=GEN_DT, cell_h=None, h_total=None, row_offset=0, w=None, u=None,
+                  want_u=False, flags=0):
+    """tsde_noise of a general-noise launch: counter noise of `key` (device int64 tensor) over one cell of length h,
+    or over the cells whose lengths the device float64 tensor `cell_h` holds; without a key, memory noise read
+    from the device addresses w (and u)."""
+    from torchsde_b200 import _cabi
+    nz = _cabi.Noise()
+    nz.want_u, nz.flags = int(want_u), flags
+    if key is not None:
+        nz.source, nz.key, nz.cell_id, nz.row_offset = _cabi.SRC_COUNTER, key.data_ptr(), cell_id, row_offset
+        nz.n_cells, nz.h, nz.h_total = 1, h, h if h_total is None else h_total
+        if cell_h is not None:
+            nz.n_cells, nz.cell_h = cell_h.numel(), cell_h.data_ptr()
+    else:
+        nz.source, nz.n_cells, nz.w, nz.u = _cabi.SRC_MEMORY, 1, w, u if want_u else None
+    return nz
+
+
+def general_call(op, dtype, rows, d, m, args, nz, outs):
+    """One launch of general-noise entry point `op`; args / outs are device addresses in argument order."""
+    from torchsde_b200 import _cabi
+    L = _cabi.make_launch(dtype, _cabi.NOISE_GENERAL, rows, d, m)
+    _cabi.check(getattr(_cabi.lib(), op)(ctypes.byref(L), ctypes.byref(nz), *args, *GENERAL_OPS[op].scalars, *outs),
+                op)
 
 
 def golden_files(prefix):

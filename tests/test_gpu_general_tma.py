@@ -1,8 +1,9 @@
 """The TMA-staged general-noise tile kernel (`gen_tma_kernel`) against the per-thread-load tile kernel (`gen_cta_kernel`).
 
 Both kernels use the same chunk -> lane mapping, the same fused multiply-add chain inside a 4-chunk and the same
-xor-tree across chunks, so for identical increments their outputs must be BIT-IDENTICAL; the per-thread-load kernel
-itself is pinned against the oracle / the reference's golden files in test_gpu_solver.py.
+xor-tree across chunks, so for identical increments their outputs must be BIT-IDENTICAL; both kernels are pinned
+against the oracle / the reference's golden files in test_gpu_solver.py and, launch by launch, against a float64
+formula on the oracle's increments in test_gpu_general_paths.py.
 
 Which kernel runs is decided by shape alone (csrc/tableau_general.cu `tma_route` and the eligibility checks of
 `launch_gen_tma`): a batch that fills the pipeline at m = 64, or at m = 16 for tableaus with one g operand, takes the
@@ -11,80 +12,52 @@ launches a batch that takes the TMA-staged kernel, then the same rows again as s
 per-thread-load kernel (counter noise: `row_offset`; memory noise: offset pointers), confirms both routes with the
 launch counters and compares the outputs bit for bit.
 """
-import ctypes
-
 import pytest
 import torch
 
-from . import problems
+from . import helpers, problems
+from .helpers import GENERAL_OPS, GENERAL_TMA_REACHABLE as REACHABLE, tile_launches as _launches
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-DT = 2.0 ** -6
-CTA, TMA = 0, 1    # tsde_kernel_launches families
 SLICE = 512        # rows per per-thread-load slice: too few tiles to fill the TMA pipeline at every tested shape
 
-# entry point -> (e operands (rows, d), g operands (rows, d, m), scalar arguments, wants U)
-OPS = {
-    'tsde_step_euler': (2, 1, (DT,), False),
-    'tsde_midpoint_predict': (2, 1, (DT / 2,), False),
-    'tsde_euler_heun_predict': (1, 1, (), False),
-    'tsde_reversible_heun_z': (3, 1, (DT,), False),
-    'tsde_srk_additive_stage': (2, 1, (DT, 1 / DT), True),
-    'tsde_step_heun': (3, 2, (DT,), False),
-    'tsde_step_euler_heun': (2, 2, (DT,), False),
-    'tsde_step_reversible_heun': (3, 2, (DT / 2,), False),
-    'tsde_step_srk_additive': (3, 2, (DT, 1 / DT), True),
-}
-# every (op, m) the TMA-staged kernel is compiled for: one g operand at m = 16 and 64, two g operands at m = 64
-REACHABLE = [(op, m) for op, (_, ng, _, _) in OPS.items() for m in ((16, 64) if ng == 1 else (64,))]
 
-
-def _launches():
-    from torchsde_b200 import _cabi
-    lib = _cabi.lib()
-    return lib.tsde_kernel_launches(CTA), lib.tsde_kernel_launches(TMA)
-
-
-def _call(op, dtype, rows, d, m, r0, es, gs, w, u, key, out):
-    """One launch of `op` on rows [r0, r0 + rows) of the operands."""
-    from torchsde_b200 import _cabi
-    ne, ng, scalars, want_u = OPS[op]
+def _call(op, dtype, rows, d, m, r0, args, w, u, key, outs):
+    """One launch of `op` on rows [r0, r0 + rows) of the operands and outputs."""
+    spec = GENERAL_OPS[op]
     s = torch.finfo(dtype).bits // 8
-    nz = _cabi.Noise()
     if key is not None:
-        nz.source, nz.key, nz.cell_id, nz.n_cells, nz.h, nz.h_total = _cabi.SRC_COUNTER, key.data_ptr(), 5, 1, DT, DT
-        nz.want_u, nz.row_offset = int(want_u), r0
+        nz = helpers.general_noise(key=key, cell_id=5, row_offset=r0, want_u=spec.want_u)
     else:
-        nz.source, nz.n_cells, nz.w = _cabi.SRC_MEMORY, 1, w.data_ptr() + r0 * m * s
-        if want_u:
-            nz.want_u, nz.u = 1, u.data_ptr() + r0 * m * s
-    L = _cabi.make_launch(dtype, _cabi.NOISE_GENERAL, rows, d, m)
-    args = [e.data_ptr() + r0 * d * s for e in es] + [g.data_ptr() + r0 * d * m * s for g in gs]
-    _cabi.check(getattr(_cabi.lib(), op)(ctypes.byref(L), ctypes.byref(nz), *args, *scalars,
-                                         out.data_ptr() + r0 * d * s), op)
+        nz = helpers.general_noise(w=w.data_ptr() + r0 * m * s, u=u.data_ptr() + r0 * m * s, want_u=spec.want_u)
+    per_row = {'e': d * s, 'g': d * m * s}
+    helpers.general_call(op, dtype, rows, d, m, [x.data_ptr() + r0 * per_row[k] for k, x in zip(spec.args, args)],
+                         nz, [o.data_ptr() + r0 * per_row[k] for k, o in zip(spec.outs, outs)])
 
 
 def _whole_and_sliced(op, dtype, B, d, m, memory, first_slice=SLICE):
     """The launch over all B rows and the same rows launched as slices (the first `first_slice` rows, then SLICE rows
-    at a time); returns both outputs and the (per-thread-load, TMA-staged) launch counts of each."""
-    ne, ng, _, _ = OPS[op]
+    at a time); returns both lists of outputs and the (per-thread-load, TMA-staged) launch counts of each."""
+    spec = GENERAL_OPS[op]
     gen = torch.Generator(device=DEV).manual_seed(B * d + m)
-    es = [torch.rand(B, d, generator=gen, device=DEV, dtype=dtype) for _ in range(ne)]
-    gs = [torch.rand(B, d, m, generator=gen, device=DEV, dtype=dtype) - 0.5 for _ in range(ng)]
+    shape = {'e': (B, d), 'g': (B, d, m)}
+    args = [torch.rand(*shape[k], generator=gen, device=DEV, dtype=dtype) - (0.5 if k == 'g' else 0.0)
+            for k in spec.args]
     w = u = key = None
     if memory:
-        w, u = (torch.randn(B, m, generator=gen, device=DEV, dtype=dtype) * DT ** 0.5 for _ in range(2))
+        w, u = (torch.randn(B, m, generator=gen, device=DEV, dtype=dtype) * helpers.GEN_DT ** 0.5 for _ in range(2))
     else:
         key = torch.tensor([31], dtype=torch.int64, device=DEV)
-    whole, sliced = (torch.full((B, d), float('nan'), device=DEV, dtype=dtype) for _ in range(2))
+    whole, sliced = ([torch.full(shape[k], float('nan'), device=DEV, dtype=dtype) for k in spec.outs]
+                     for _ in range(2))
     n0 = _launches()
-    _call(op, dtype, B, d, m, 0, es, gs, w, u, key, whole)
+    _call(op, dtype, B, d, m, 0, args, w, u, key, whole)
     n1 = _launches()
     r0 = 0
     while r0 < B:
         rows = min(first_slice if r0 == 0 else SLICE, B - r0)
-        _call(op, dtype, rows, d, m, r0, es, gs, w, u, key, sliced)
+        _call(op, dtype, rows, d, m, r0, args, w, u, key, sliced)
         r0 += rows
     n2 = _launches()
     return whole, sliced, (n1[0] - n0[0], n1[1] - n0[1]), (n2[0] - n1[0], n2[1] - n1[1])
@@ -102,8 +75,9 @@ def test_tma_path_bit_identical(op, m, memory, dtype):
     assert route == (0, 1), f"B={B} was not routed to the TMA-staged kernel: {route}"
     n_slices = 1 + -(-(B - 3) // SLICE)
     assert slice_route == (n_slices, 0), f"slices were not routed to the per-thread-load kernel: {slice_route}"
-    assert torch.isfinite(whole).all()
-    assert torch.equal(whole, sliced), f"max abs diff {(whole - sliced).abs().max().item()}"
+    for i, (a, b) in enumerate(zip(whole, sliced)):
+        assert torch.isfinite(a).all(), f"output {i} not written everywhere"
+        assert torch.equal(a, b), f"output {i}: max abs diff {(a - b).abs().max().item()}"
 
 
 ROUTES = [
@@ -129,7 +103,7 @@ def test_default_routing():
         whole, sliced, route, slice_route = _whole_and_sliced(op, dtype, B, d, m, memory=False)
         if route != ((0, 1) if tma else (1, 0)) or slice_route[1] != 0 or slice_route[0] < 1:
             bad.append(f'{op} {dtype} B={B} d={d} m={m}: routes {route}, slices {slice_route}')
-        elif not torch.equal(whole, sliced):
+        elif not all(torch.equal(a, b) for a, b in zip(whole, sliced)):
             bad.append(f'{op} {dtype} B={B} d={d} m={m}: output differs from the per-thread-load slices')
     assert not bad, '; '.join(bad)
 
