@@ -18,7 +18,8 @@
  *       diagonal g    : (rows, d)          (d == m)
  *       general g     : (rows, d, m)       (scalar noise: m == 1; additive: same layout)
  *       noise W, U    : (rows, m)
- *   - `dtype` is TSDE_F32 or TSDE_F64 and applies to every tensor of a call.
+ *   - `dtype` is TSDE_F32 or TSDE_F64 and applies to every tensor of a call,
+ *     except the 16-bit SDE outputs a float32 launch may declare (TSDE_FMT_*).
  *   - Scalars (dt, coefficients) are passed as double and rounded ONCE to the
  *     tensor dtype on the host side of the kernel launch, which is what the
  *     reference's `tensor * python_scalar` / `tensor * 0-d tensor` does.
@@ -45,6 +46,19 @@ extern "C" {
 
 enum { TSDE_F32 = 0, TSDE_F64 = 1 };
 
+/*
+ * 16-bit SDE outputs (a drift / diffusion evaluated under torch.autocast).  Bits 0-7 of tsde_launch.dtype are the
+ * state dtype; above them, two bits per tensor input of the call, in declaration order, give that input's storage
+ * format.  Only inputs that hold what the user's SDE returned may be 16-bit: the f*, fp, g*, gp, ga and gb
+ * arguments of the step tableaus, predictors and stages, tsde_milstein_vjp_seed and the two reversible-Heun adjoint
+ * halves (g also when it holds a user g_prod, TSDE_SRC_UNIT).  The kernels widen such an operand exactly to float32
+ * and run the float32 arithmetic unchanged, so a launch equals the float32 launch on widened copies bit for bit.
+ * TSDE_EINVAL: format bits on any other input or entry point, with a TSDE_F64 state, or the value 3.
+ * tsde_milstein_vjp_seed writes go in g's format (round to nearest even).
+ */
+enum { TSDE_FMT_STATE = 0, TSDE_FMT_BF16 = 1, TSDE_FMT_F16 = 2 };
+#define TSDE_OPERAND_FMT(i, fmt) ((int32_t)(fmt) << (8 + 2 * (i)))
+
 /* noise layouts (torchsde/settings.py:41-45 NOISE_TYPES) */
 enum {
   TSDE_NOISE_DIAGONAL = 0, /* g:(rows,d)      W:(rows,d)                   base_sde.py:98-99   */
@@ -69,7 +83,7 @@ enum {
 
 /* Shape / stream descriptor shared by all launches. */
 typedef struct tsde_launch {
-  int32_t dtype;      /* TSDE_F32 | TSDE_F64                       */
+  int32_t dtype;      /* TSDE_F32 | TSDE_F64, | TSDE_OPERAND_FMT(i, TSDE_FMT_*) for 16-bit SDE outputs */
   int32_t noise_type; /* TSDE_NOISE_*                              */
   int64_t rows;       /* trajectories held by this rank; 0 is a valid launch that does nothing (operand pointers
                          of an empty batch may be NULL)            */

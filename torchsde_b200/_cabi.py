@@ -128,6 +128,59 @@ def dtype_code(dtype):
     raise ValueError(f"torchsde_b200 supports float32 and float64 tensors, got {dtype}.")
 
 
+FMT_STATE, FMT_BF16, FMT_F16 = 0, 1, 2
+_FMT = {torch.bfloat16: FMT_BF16, torch.float16: FMT_F16}
+
+# entry point -> its tensor inputs, in declaration order.  Those named in SDE_OUTPUT_NAMES hold what the user's drift /
+# diffusion returned and may be 16-bit (torch.autocast); every other input has the state dtype.
+INPUTS = {
+    'tsde_step_euler': ('y0', 'f', 'g'),
+    'tsde_milstein_vjp_seed': ('g',),
+    'tsde_step_milstein': ('y0', 'f', 'g', 'gdg'),
+    'tsde_milstein_gf_predict': ('y0', 'f', 'g'),
+    'tsde_step_milstein_gf': ('y0', 'f', 'g', 'gp'),
+    'tsde_step_heun': ('y0', 'f', 'fp', 'g', 'gp'),
+    'tsde_midpoint_predict': ('y0', 'f', 'g'),
+    'tsde_euler_heun_predict': ('y0', 'g'),
+    'tsde_step_euler_heun': ('y0', 'f', 'g', 'gp'),
+    'tsde_reversible_heun_z': ('y0', 'z0', 'f0', 'g0'),
+    'tsde_step_reversible_heun': ('y0', 'f0', 'f1', 'g0', 'g1'),
+    'tsde_srk_diag_stage1': ('y0', 'f0', 'g0'),
+    'tsde_srk_diag_stage2': ('y0', 'f0', 'g0', 'f1', 'g1'),
+    'tsde_srk_diag_stage3': ('y0', 'g0', 'g1', 'f2', 'g2'),
+    'tsde_step_srk_diag': ('y0', 'f0', 'f1', 'f2', 'g0', 'g1', 'g2', 'g3'),
+    'tsde_srk_additive_stage': ('y0', 'f0', 'ga'),
+    'tsde_step_srk_additive': ('y0', 'f0', 'f1', 'ga', 'gb'),
+    'tsde_adjoint_reversible_heun_a': ('y0', 'z0', 'f0', 'g0', 'adj_y0', 'adj_f0', 'adj_g0'),
+    'tsde_adjoint_reversible_heun_b': ('y0', 'f0', 'f1', 'g0', 'g1', 'adj_y0', 'adj_z0', 'vjp_z'),
+    'tsde_linear_interp': ('y0', 'y1'),
+}
+SDE_OUTPUT_NAMES = frozenset(('f', 'f0', 'f1', 'f2', 'fp', 'g', 'g0', 'g1', 'g2', 'g3', 'gp', 'ga', 'gb'))
+
+
+def operands(name, state_dtype, ins):
+    """(tsde_launch.dtype, inputs) of a launch of `name` whose state has `state_dtype`.  A bf16 / fp16 SDE output is
+    passed as it is with its format bits (float32 state) or widened exactly to float64 (float64 state); any other
+    dtype mismatch is a ValueError."""
+    word = dtype_code(state_dtype)
+    if all(t.dtype == state_dtype for t in ins):
+        return word, ins
+    out = list(ins)
+    for i, (arg, t) in enumerate(zip(INPUTS[name], ins)):
+        if t.dtype == state_dtype:
+            continue
+        fmt = _FMT.get(t.dtype) if arg in SDE_OUTPUT_NAMES else None
+        if fmt is None:
+            what = 'the SDE returned' if arg in SDE_OUTPUT_NAMES else 'got'
+            raise ValueError(f"torchsde_b200: `{arg}` of {name} has dtype {t.dtype}, but the state is {state_dtype}; "
+                             f"{what} a tensor that is neither the state dtype nor bfloat16 / float16.")
+        if state_dtype == torch.float64:
+            out[i] = t.to(torch.float64)
+        else:
+            word |= fmt << (8 + 2 * i)
+    return word, out
+
+
 def require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:

@@ -33,6 +33,7 @@ from . import base_solver
 from . import methods
 from . import schedule as schedule_lib
 from . import sdeint as sdeint_mod
+from .base_sde import widen
 from .base_solver import _contig
 from .. import _cabi
 from .._brownian import BrownianInterval, ReverseBrownian
@@ -88,6 +89,12 @@ class _BackwardEngine(base_solver.BaseSDESolver):
     def _step(self, c, y0, extra0, out):
         raise RuntimeError("internal")
 
+    def _half(self, name, L, nz, ins, scalars, outs):
+        """Kernel A or B of a backward step, with the formats of 16-bit SDE outputs (f0, g0, f1, g1) declared like
+        those of every tableau launch (_cabi.operands)."""
+        word, ins = _cabi.operands(name, self.dtype, ins)
+        self._launch(name, L, nz, ins, scalars, outs, word)
+
     def plan(self, ys, ts):
         """Host-side plan of the backward sweep: one schedule per interval [-ts[i], -ts[i-1]], exactly
         as the reference re-enters integrate() (adjoint.py:97-113), merged into one step list."""
@@ -131,7 +138,6 @@ class _BackwardEngine(base_solver.BaseSDESolver):
         return self._sweep(ys, grad_ys, extras, grad_extras, self.params)
 
     def _sweep(self, ys, grad_ys, extras, grad_extras, params):
-        lib = _cabi.lib()
         self._refresh_stream()
         L = self._L
         T = self.T
@@ -159,9 +165,8 @@ class _BackwardEngine(base_solver.BaseSDESolver):
                 z1 = torch.empty_like(y)
                 adj_f_mid = torch.empty_like(adj_f)
                 adj_g_mid = torch.empty_like(adj_g)
-                _check(lib.tsde_adjoint_reversible_heun_a(
-                    L, self._feed.get(c), _p(y), _p(z0), _p(f0), _p(g0), _p(adj_y), _p(adj_f), _p(adj_g),
-                    c.dt, half_dt, _p(z1), _p(adj_f_mid), _p(adj_g_mid)), "tsde_adjoint_reversible_heun_a")
+                self._half('tsde_adjoint_reversible_heun_a', L, self._feed.get(c),
+                           (y, z0, f0, g0, adj_y, adj_f, adj_g), (c.dt, half_dt), (z1, adj_f_mid, adj_g_mid))
                 with torch.enable_grad():
                     if pending is None:
                         z0r = z0.detach().requires_grad_()
@@ -171,7 +176,7 @@ class _BackwardEngine(base_solver.BaseSDESolver):
                     outs, gouts = [], []
                     for o, go in ((re_f0, adj_f_mid), (re_g0, adj_g_mid)):
                         if o.requires_grad:
-                            outs.append(o)
+                            outs.append(widen(o, go.dtype))
                             gouts.append(go.view_as(o))
                     if outs:
                         vjps = torch.autograd.grad(outs, [z0r] + list(params), gouts, allow_unused=True)
@@ -191,10 +196,9 @@ class _BackwardEngine(base_solver.BaseSDESolver):
                 adj_z1 = torch.empty_like(adj_z)
                 adj_f1 = torch.empty_like(adj_f)
                 adj_g1 = torch.empty_like(adj_g)
-                _check(lib.tsde_adjoint_reversible_heun_b(
-                    L, self._feed.get(c), _p(y), _p(f0), _p(f1), _p(g0), _p(g1), _p(adj_y), _p(adj_z),
-                    _p(_contig(vjp_z)), c.dt, half_dt, _p(y1), _p(adj_y1), _p(adj_z1), _p(adj_f1), _p(adj_g1)),
-                    "tsde_adjoint_reversible_heun_b")
+                self._half('tsde_adjoint_reversible_heun_b', L, self._feed.get(c),
+                           (y, f0, f1, g0, g1, adj_y, adj_z, _contig(vjp_z)), (c.dt, half_dt),
+                           (y1, adj_y1, adj_z1, adj_f1, adj_g1))
                 y, adj_y, adj_z, adj_f, adj_g = y1, adj_y1, adj_z1, adj_f1, adj_g1
                 f0, g0, z0 = f1, g1, z1
             # adjoint.py:114-116
@@ -216,7 +220,6 @@ class _BackwardEngine(base_solver.BaseSDESolver):
     def _bstep(self, ta, tb, st, params):
         """One AdjointReversibleHeun.step from reversed time ta to tb (0-d CPU tensors).  `st` = (y, z0, f0, g0, adj_y,
         adj_f, adj_g, adj_z, adj_params); returns the new state without modifying `st`."""
-        lib = _cabi.lib()
         y, z0, f0, g0, adj_y, adj_f, adj_g, adj_z, adj_params = st
         h = tb - ta
         dt, half_dt = float(h), float(0.5 * h)
@@ -225,13 +228,13 @@ class _BackwardEngine(base_solver.BaseSDESolver):
         t_fwd0 = (-ta).to(self.device)
         t_fwd1 = (-tb).to(self.device)
         z1, adj_f_mid, adj_g_mid = torch.empty_like(y), torch.empty_like(adj_f), torch.empty_like(adj_g)
-        _check(lib.tsde_adjoint_reversible_heun_a(
-            self._L, nz, _p(y), _p(z0), _p(f0), _p(g0), _p(adj_y), _p(adj_f), _p(adj_g), dt, half_dt, _p(z1),
-            _p(adj_f_mid), _p(adj_g_mid)), "tsde_adjoint_reversible_heun_a")
+        self._half('tsde_adjoint_reversible_heun_a', self._L, nz, (y, z0, f0, g0, adj_y, adj_f, adj_g),
+                   (dt, half_dt), (z1, adj_f_mid, adj_g_mid))
         with torch.enable_grad():
             z0r = z0.detach().requires_grad_()
             re_f0, re_g0 = self.sde.f_and_g(t_fwd0, z0r)
-            pairs = [(o, go.view_as(o)) for o, go in ((re_f0, adj_f_mid), (re_g0, adj_g_mid)) if o.requires_grad]
+            pairs = [(widen(o, go.dtype), go.view_as(o)) for o, go in ((re_f0, adj_f_mid), (re_g0, adj_g_mid))
+                     if o.requires_grad]
             if pairs:
                 vjps = torch.autograd.grad([o for o, _ in pairs], [z0r] + list(params), [g for _, g in pairs],
                                            allow_unused=True)
@@ -243,9 +246,8 @@ class _BackwardEngine(base_solver.BaseSDESolver):
         f1, g1 = _contig(f1), _contig(g1)
         y1, adj_y1, adj_z1 = torch.empty_like(y), torch.empty_like(adj_y), torch.empty_like(adj_z)
         adj_f1, adj_g1 = torch.empty_like(adj_f), torch.empty_like(adj_g)
-        _check(lib.tsde_adjoint_reversible_heun_b(
-            self._L, nz, _p(y), _p(f0), _p(f1), _p(g0), _p(g1), _p(adj_y), _p(adj_z), _p(vjp_z), dt, half_dt,
-            _p(y1), _p(adj_y1), _p(adj_z1), _p(adj_f1), _p(adj_g1)), "tsde_adjoint_reversible_heun_b")
+        self._half('tsde_adjoint_reversible_heun_b', self._L, nz, (y, f0, f1, g0, g1, adj_y, adj_z, vjp_z),
+                   (dt, half_dt), (y1, adj_y1, adj_z1, adj_f1, adj_g1))
         return (y1, z1, f1, g1, adj_y1, adj_f1, adj_g1, adj_z1, new_params)
 
     def _aug_error(self, a, b, rtol, atol):
@@ -347,13 +349,14 @@ def _backward_plan(engine, ys, ts, extras):
     plan.ys = ys.detach().clone()
     plan.grad_ys = torch.zeros_like(plan.ys)
     plan.extras = tuple(_contig(e.detach()).clone() for e in extras)
-    plan.grad_extras = tuple(torch.zeros_like(e) for e in plan.extras)
+    plan.grad_extras = tuple(torch.zeros_like(e, dtype=ys.dtype) for e in plan.extras)  # (see _backward)
     plan.key = binding.interval.key_tensor().clone()
     engine._feed._key_ptr = plan.key.data_ptr()
     dev = ys.device
     side = torch.cuda.Stream(device=dev)
     side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side):  # warm-up (cuBLAS handles, autograd, allocator): first interval only
+    # warm-up (cuBLAS handles, autograd, allocator): first interval only
+    with torch.cuda.stream(side), graph_mod.uncached_autocast():
         saved = engine.scheds, engine.T
         engine.scheds, engine.T = [engine.scheds[0]], 2
         engine.sweep(plan.ys[-2:], plan.grad_ys[-2:], plan.extras, plan.grad_extras, alias_names=names)
@@ -361,7 +364,7 @@ def _backward_plan(engine, ys, ts, extras):
     torch.cuda.current_stream(dev).wait_stream(side)
     torch.cuda.synchronize(dev)
     g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
+    with graph_mod.no_gc(), torch.cuda.graph(g), graph_mod.uncached_autocast():
         plan.out = engine.sweep(plan.ys, plan.grad_ys, plan.extras, plan.grad_extras, alias_names=names)
     plan.time_table = getattr(engine, '_time_table', None)
     plan.graph = g
@@ -410,6 +413,8 @@ def _generic_backward(sde, bm, dt, ys, ts, grad_ys, params, cfg, differentiable=
     inherited: an Ito SDE whose adjoint needs the Ito correction cannot be double-backwarded (its AdjointSDE has no
     `f_and_g`, adjoint_sde.py:267-271)."""
     from .adjoint_sde import AdjointSDE
+    if hasattr(sde, 'widen_outputs'):
+        sde.widen_outputs(ys.dtype)  # the backward SDE is torch code on the forward SDE's outputs
     aug = [ys[-1], grad_ys[-1]] + [torch.zeros_like(p) for p in params]
     shapes = [t.size() for t in aug]
     numels = [t.numel() for t in aug]
@@ -438,7 +443,8 @@ def _recomputed_solve(sde, bm, dt, ts, y0, extras0):
     """Reversible-Heun forward solve with every tableau launch recorded as an autograd node."""
     solver = methods.ReversibleHeun(sde=sde, bm=bm, dt=dt, adaptive=False, rtol=None, atol=None, dt_min=None, options={})
     solver._autograd = True
-    ys, extras = solver.integrate(y0, ts, tuple(extras0))
+    sde.widen_outputs(y0.dtype)
+    ys, extras = solver.integrate(y0, ts, tuple(widen(e, y0.dtype) for e in extras0))
     return [ys, *extras]
 
 
@@ -540,7 +546,8 @@ class _SdeintAdjointMethod(torch.autograd.Function):
                 adj_y, adj_params = _generic_backward(ctx.sde, ctx.bm, ctx.dt, ys, ts, grad_ys, list(params),
                                                       ctx.adjoint_options['_cfg'], differentiable)
             return (None, None, None, None, None, None, None, None, adj_y, *([None] * ctx.n_extras), *adj_params)
-        grad_extras = [torch.zeros_like(e) if g is None else g for g, e in zip(grad_extras, extras)]
+        # (the adjoint state is kept in the state dtype also for 16-bit solver state (f0, g0))
+        grad_extras = [widen(torch.zeros_like(e) if g is None else g, ys.dtype) for g, e in zip(grad_extras, extras)]
         if differentiable:
             adj_y, adj_extras, adj_params = _reversible_backward_differentiable(
                 ctx.sde, ctx.bm, ctx.dt, ts, y0_in, extras_in, list(params), grad_ys, grad_extras)

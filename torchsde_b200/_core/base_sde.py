@@ -20,6 +20,23 @@ from torch import nn
 from ..settings import NOISE_TYPES, SDE_TYPES
 
 
+_HALF = (torch.bfloat16, torch.float16)
+
+
+def widen(x, dtype):
+    """A bfloat16 / float16 tensor (an SDE output computed under torch.autocast) converted to `dtype`, exactly; anything
+    else as it is.  The package's own torch code computes only on widened outputs: ATen's promotion rules would round
+    intermediates such as `f * dt` to 16 bits otherwise."""
+    return x.to(dtype) if torch.is_tensor(x) and x.dtype in _HALF else x
+
+
+def _widened(fn, dtype):
+    def call(*args):
+        out = fn(*args)
+        return tuple(widen(o, dtype) for o in out) if isinstance(out, tuple) else widen(out, dtype)
+    return call
+
+
 class BaseSDE(abc.ABC, nn.Module):
     """Base class for all SDEs; validates `noise_type` and `sde_type` (base_sde.py:25-39)."""
 
@@ -49,6 +66,19 @@ class ForwardSDE(BaseSDE):
             self.g_prod = sde.g_prod
         if self.user_f_and_g_prod:
             self.f_and_g_prod = sde.f_and_g_prod
+        self.widened_to = None
+
+    def widen_outputs(self, dtype):
+        """From now on hand out every bfloat16 / float16 output of the user's callables widened to `dtype` (exact).
+        Used where the solve is not a chain of this library's launches: gradients through `sdeint` (each output is
+        widened once, so autograd accumulates its gradient in `dtype` before rounding it to 16 bits), the backward
+        SDE of the generic adjoints, and float64 states.  Idempotent."""
+        if self.widened_to is not None:
+            return
+        self.widened_to = dtype
+        for name in ('f', 'g', 'f_and_g', 'g_prod', 'f_and_g_prod'):
+            if name in vars(self):
+                setattr(self, name, _widened(getattr(self, name), dtype))
 
     def f_default(self, t, y):
         raise RuntimeError("Method `f` has not been provided, but is required for this method.")
@@ -145,7 +175,7 @@ class SDELogqp(BaseSDE):
     def f_and_g(self, t, y):
         state = y[:, :-1]
         base = self._base_sde
-        f, g, h = base.f(t, state), base.g(t, state), base.h(t, state)
+        f, g, h = (widen(x, y.dtype) for x in (base.f(t, state), base.g(t, state), base.h(t, state)))
         differentiated = torch.is_grad_enabled() and (f.requires_grad or g.requires_grad or h.requires_grad)
         if self._diagonal and not differentiated and self._on_device(f):
             return self._fused_augment(f, g, h)
@@ -180,4 +210,4 @@ class SDELogqp(BaseSDE):
         return self.f_and_g(t, y)[0]
 
     def g(self, t, y):
-        return self._pad_diffusion(self._base_sde.g(t, y[:, :-1]))
+        return self._pad_diffusion(widen(self._base_sde.g(t, y[:, :-1]), y.dtype))

@@ -214,7 +214,9 @@ class BaseSDESolver(metaclass=abc.ABCMeta):
             return torch.empty_like(ins[0])  # grad_outputs has g's shape
         return torch.empty((self.rows, self.d), dtype=self.dtype, device=self.device)
 
-    def _launch(self, name, L, nz, ins, scalars, outs):
+    def _launch(self, name, L, nz, ins, scalars, outs, dtype_word):
+        """`dtype_word`: the state dtype and the formats of 16-bit SDE outputs (_cabi.operands); the shared launch
+        descriptor carries it for this call only."""
         flags = 0
         g3 = [t for t in ins if t.dim() == 3 and not t.is_contiguous()]
         if g3:
@@ -232,7 +234,13 @@ class BaseSDESolver(metaclass=abc.ABCMeta):
         args += [t.data_ptr() for t in ins]
         args += list(scalars)
         args += [o.data_ptr() for o in outs]
-        _cabi.check(getattr(self._lib, name)(*args), name)
+        launch = L._obj
+        launch.dtype = dtype_word
+        try:
+            code = getattr(self._lib, name)(*args)
+        finally:
+            launch.dtype = dtype_word & 0xff
+        _cabi.check(code, name)
 
     def _k(self, name, L, nz, ins, scalars, out, n_out=1, raw=False):
         """One C-ABI tableau launch `name(L, [nz], *ins, *scalars, *outs)`.  Fast path: direct launch into
@@ -245,12 +253,13 @@ class BaseSDESolver(metaclass=abc.ABCMeta):
             if nz is not None and not unit:
                 noise = self._feed.tensors(self._cur_c, self.want_u)
             return TableauFn.apply(self, name, L is self._L, unit, noise, tuple(scalars), n_out, *ins)
+        word, ins = _cabi.operands(name, self.dtype, ins)
         if n_out == 1:
             o = out if out is not None else self._out_like(name, ins)
-            self._launch(name, L, nz, ins, scalars, (o,))
+            self._launch(name, L, nz, ins, scalars, (o,), word)
             return o
         outs = tuple(self._out_like(name, ins) for _ in range(n_out))
-        self._launch(name, L, nz, ins, scalars, outs)
+        self._launch(name, L, nz, ins, scalars, outs, word)
         return outs
 
     def _launch_raw(self, name, use_general, unit, noise, ins, scalars, n_out):
@@ -262,9 +271,9 @@ class BaseSDESolver(metaclass=abc.ABCMeta):
             nz = self._feed.from_tensors(noise[0], noise[1])
         else:
             nz = None
-        ins = [_contig(t) for t in ins]
+        word, ins = _cabi.operands(name, self.dtype, [_contig(t) for t in ins])
         outs = tuple(self._out_like(name, ins) for _ in range(n_out))
-        self._launch(name, L, nz, ins, scalars, outs)
+        self._launch(name, L, nz, ins, scalars, outs, word)
         return outs
 
     # ------------------------------------------------------------------------------------------

@@ -31,6 +31,8 @@ addresses, shapes, dtype, grid, dt, Brownian structure).  The cache is a WeakKey
 reference to the SDE (only tensors and the graph), so dropping the SDE frees its plans — each of which pins a
 full output series, hence also the small bound MAX_PLANS_PER_SDE.
 """
+import contextlib
+import gc
 import weakref
 
 import torch
@@ -105,7 +107,31 @@ def _plan_key(solver, y0, ts, extra0, binding):
             solver.bm.levy_area_approximation, tuple(solver.bm.shape),
             node.cell_base, tuple(binding.first), tuple(binding.count), binding.reverse,
             binding.interval._row_offset,
-            tuple((tuple(e.shape), e.dtype) for e in extra0))
+            tuple((tuple(e.shape), e.dtype) for e in extra0),
+            # f / g may return 16-bit tensors under autocast, and the captured launches have their formats baked in
+            torch.is_autocast_enabled('cuda'), torch.get_autocast_dtype('cuda'))
+
+
+def uncached_autocast():
+    """The caller's CUDA autocast state, without its cast cache, for warm-up and capture: a cached 16-bit copy of a
+    parameter lives only as long as the caller's autocast region, while the graph reads it on every later replay."""
+    if not torch.is_autocast_enabled('cuda'):
+        return contextlib.nullcontext()
+    return torch.autocast('cuda', dtype=torch.get_autocast_dtype('cuda'), cache_enabled=False)
+
+
+@contextlib.contextmanager
+def no_gc():
+    """No cyclic garbage collection while a graph is captured.  A collection can free an unreachable SDE object, and
+    with it the CUDA graphs of its cached plans; destroying a graph while a stream captures invalidates the capture
+    (and leaves torch's CUDA generator in capture mode).  Which allocation triggers a collection is arbitrary."""
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        yield
+    finally:
+        if enabled:
+            gc.enable()
 
 
 def _hand_out(plan, solver, static_ok):
@@ -195,7 +221,7 @@ def _capture(solver, sched, binding, y0, ts, extra0):
     # Warm-up on a side stream (lazy initialisations: cuBLAS handles, autograd, allocator)
     side = torch.cuda.Stream(device=dev)
     side.wait_stream(torch.cuda.current_stream(dev))
-    with torch.cuda.stream(side), torch.no_grad():
+    with torch.cuda.stream(side), torch.no_grad(), uncached_autocast():
         plan.ys[0].copy_(plan.y0)
         n_warm = min(3, sched.n_steps)
         if n_warm:
@@ -211,7 +237,7 @@ def _capture(solver, sched, binding, y0, ts, extra0):
 
     graph = torch.cuda.CUDAGraph()
     launches0 = _cabi.LAUNCHES
-    with torch.no_grad(), torch.cuda.graph(graph):
+    with no_gc(), torch.no_grad(), torch.cuda.graph(graph), uncached_autocast():
         extra_out = body()
     plan.abi_launches = _cabi.LAUNCHES - launches0  # kernels of THIS library captured in the graph (per replay)
     plan.graph = graph
@@ -294,13 +320,13 @@ def _integrate_captured_split(solver, y0, ts, static_ok=False):
 
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side), torch.no_grad():
+        with torch.cuda.stream(side), torch.no_grad(), uncached_autocast():
             body(min(3, sched.n_steps))
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         graph = torch.cuda.CUDAGraph()
         launches0 = _cabi.LAUNCHES
-        with torch.no_grad(), torch.cuda.graph(graph):
+        with no_gc(), torch.no_grad(), torch.cuda.graph(graph), uncached_autocast():
             body()
         plan.abi_launches = _cabi.LAUNCHES - launches0
         plan.graph = graph

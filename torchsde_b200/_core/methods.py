@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from . import base_solver
+from .base_sde import widen
 from .base_solver import _contig, _gop
 from .. import _cabi
 from ..settings import SDE_TYPES, NOISE_TYPES, LEVY_AREA_APPROXIMATIONS, METHODS, METHOD_OPTIONS
@@ -25,6 +26,22 @@ def _ieee_sqrt(dt):
     expression on the host would make SRK / derivative-free Milstein depend on the host's vector ISA; numpy's sqrt is the
     hardware instruction."""
     return torch.tensor(np.sqrt(dt.detach().numpy()), dtype=dt.dtype)
+
+class _WidenedSDE:
+    """The callables an SRK step with a user g_prod computes on in torch, returning 16-bit outputs widened."""
+
+    def __init__(self, sde, dtype):
+        self._sde, self._dtype = sde, dtype
+
+    def f(self, t, y):
+        return widen(self._sde.f(t, y), self._dtype)
+
+    def g(self, t, y):
+        return widen(self._sde.g(t, y), self._dtype)
+
+    def g_prod(self, t, y, v):
+        return widen(self._sde.g_prod(t, y, v), self._dtype)
+
 
 class _ProdMixin:
     """Shared handling of the reference's `f_and_g_prod` / `g_prod` call sites (base_sde.py:51-56)."""
@@ -319,7 +336,7 @@ class SRK(base_solver.BaseSDESolver):
         return w.reshape(shape), u.reshape(shape)
 
     def _diagonal_step_user_prod(self, c, y0):
-        sde, s = self.sde, c.scalars
+        sde, s = _WidenedSDE(self.sde, y0.dtype), c.scalars
         t_00, t_1, t_q, t_h = c.aux_t
         dt, rdt, sqrt_dt, three_dt = c.dt, s['rdt'], s['sqrt_dt'], s['three_dt']
         w, u = self._weights(c)
@@ -345,7 +362,7 @@ class SRK(base_solver.BaseSDESolver):
         return y1
 
     def _additive_step_user_prod(self, c, y0):
-        sde, s = self.sde, c.scalars
+        sde, s = _WidenedSDE(self.sde, y0.dtype), c.scalars
         t_1, t_34, t_00 = c.aux_t
         dt, rdt = c.dt, s['rdt']
         w, u = self._weights(c)
@@ -417,7 +434,7 @@ class LogODEMidpoint(_ProdMixin, base_solver.BaseSDESolver):
         track = self._autograd
         with torch.enable_grad():
             y = y if (track and y.requires_grad) else y.detach().requires_grad_(True)
-            g = self.sde.g(t, y)
+            g = widen(self.sde.g(t, y), y.dtype)  # (bmm_ga and the jvp's below take the state dtype)
             if track:
                 # gradients flow through the tangents as well (create_graph): keep the product in autograd
                 ga_cols = torch.bmm(g, a).unbind(-1)

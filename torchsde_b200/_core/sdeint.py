@@ -68,6 +68,7 @@ def _solve(sde, solver, y0, ts, adaptive, options, logqp, extra, extra_solver_st
         # (autograd_ops.py); eager loop, increments materialised (memory O(T), like the reference).  Adaptive
         # solves take the same route: their accepted steps are ordinary (differentiable) steps.
         solver._autograd = True
+        sde.widen_outputs(y0.dtype)  # each 16-bit output widened once: see ForwardSDE.widen_outputs
         if extra_solver_state is None:
             extra_solver_state = solver.init_extra_solver_state(ts[0], y0)
         ys, extra_solver_state = solver.integrate(y0, ts, extra_solver_state)
@@ -273,6 +274,8 @@ def check_contract(sde, y0, ts, bm, method, adaptive, options, names, logqp):
 
     sde = base_sde.ForwardSDE(sde)
     sde.probe_requires_grad = sizes.requires_grad
+    if y0.dtype == torch.float64:
+        sde.widen_outputs(torch.float64)  # (the kernels take 16-bit SDE outputs with a float32 state only)
     if bm is None:
         span = schedule_lib.ts_values(ts)
         bm = BrownianInterval(t0=span[0], t1=span[-1], size=(sizes.batch[0], sizes.noise[0]), dtype=y0.dtype,

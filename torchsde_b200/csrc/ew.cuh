@@ -10,6 +10,8 @@
 // generic kernel's grid is one resident wave (SM count x occupancy), each CTA owning an equal
 // contiguous slice of the quads.
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 
 #include "host.cuh"
@@ -47,7 +49,7 @@ struct EwP {
   int64_t d;
   int64_t qpr;     // quads per row
   int64_t nquads;  // rows * qpr
-  int32_t vec;     // all pointers 16B-aligned and d % 4 == 0
+  int32_t vec;     // all pointers 16B-aligned (8B for a 16-bit Mixed operand) and d % 4 == 0
   int32_t qshift;  // log2(qpr) if qpr is a power of two, else -1
   int32_t small;   // nquads < 2^31: 32-bit index arithmetic
   uint64_t qmagic; // rowdiv_magic(qpr) = ceil(2^64 / qpr): row = umulhi(Q, qmagic), exact for every 32-bit Q
@@ -86,6 +88,106 @@ template <typename Op, typename = void>
 struct streams_inputs { static constexpr bool value = false; };
 template <typename Op>
 struct streams_inputs<Op, decltype((void)Op::STREAM_INPUTS)> { static constexpr bool value = Op::STREAM_INPUTS; };
+
+// ---- 16-bit SDE outputs (TSDE_FMT_*, float32 state only) ----------------------------------------------------------
+// Mixed<Op> is Op with the storage format of each input (and output) as a launch argument, two bits per tensor in
+// the op's order.  The kernels instantiated for it load a 16-bit quad with one 64-bit load instead of a 128-bit one,
+// widen it exactly and run Op's float32 arithmetic unchanged, so the result equals the float32 launch on widened
+// copies bit for bit.  The formats ride in the op rather than in EwP / GenP so that the parameter layout, and hence
+// the SASS, of every all-float32 / float64 instantiation stays exactly what it was.
+template <typename Op>
+struct Mixed : Op {
+  static constexpr bool MIXED = true;
+  uint32_t fmt;   // inputs
+  uint32_t ofmt;  // outputs (only tsde_milstein_vjp_seed writes a 16-bit one: go in g's format)
+};
+template <typename Op, typename = void>
+struct is_mixed { static constexpr bool value = false; };
+template <typename Op>
+struct is_mixed<Op, decltype((void)Op::MIXED)> { static constexpr bool value = Op::MIXED; };
+
+__host__ __device__ inline uint32_t operand_fmt(uint32_t fmt, int i) { return (fmt >> (2 * i)) & 3u; }
+
+__device__ __forceinline__ float widen16(uint32_t bits, uint32_t f) {  // exact
+  return f == TSDE_FMT_BF16 ? __uint_as_float(bits << 16) : __half2float(__ushort_as_half((unsigned short)bits));
+}
+__device__ __forceinline__ uint32_t narrow16(float x, uint32_t f) {  // round to nearest even, as torch's .to()
+  return f == TSDE_FMT_BF16 ? (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(x))
+                            : (uint32_t)__half_as_ushort(__float2half_rn(x));
+}
+// Loads return raw bits and widening is a separate step: a thread issues all of its loads first and converts after,
+// as the float32 kernels do (a load whose widening sat next to it would be consumed before the next load issued).
+// element i of a tensor in format f
+__device__ __forceinline__ uint32_t ld1raw(const void* p, int64_t i, uint32_t f) {
+  return f == TSDE_FMT_STATE ? static_cast<const uint32_t*>(p)[i] : (uint32_t)static_cast<const uint16_t*>(p)[i];
+}
+__device__ __forceinline__ float widen1(uint32_t r, uint32_t f) {
+  return f == TSDE_FMT_STATE ? __uint_as_float(r) : widen16(r, f);
+}
+__device__ __forceinline__ float ld1f(const void* p, int64_t i, uint32_t f) { return widen1(ld1raw(p, i, f), f); }
+__device__ __forceinline__ void st1f(void* p, int64_t i, uint32_t f, float x) {
+  if (f == TSDE_FMT_STATE) static_cast<float*>(p)[i] = x;
+  else static_cast<uint16_t*>(p)[i] = (uint16_t)narrow16(x, f);
+}
+// elements i..i+3: one 128-bit load (16-byte aligned float32) or one 64-bit load (8-byte aligned 16-bit, in .x, .y);
+// CS: evict-first
+template <bool CS>
+__device__ __forceinline__ uint4 ld4raw(const void* p, int64_t i, uint32_t f) {
+  if (f == TSDE_FMT_STATE) {
+    const uint4* q = reinterpret_cast<const uint4*>(static_cast<const float*>(p) + i);
+    return CS ? __ldcs(q) : *q;
+  }
+  const uint2* q = reinterpret_cast<const uint2*>(static_cast<const uint16_t*>(p) + i);
+  const uint2 h = CS ? __ldcs(q) : *q;
+  return make_uint4(h.x, h.y, 0u, 0u);
+}
+__device__ __forceinline__ void widen4(const uint4 r, uint32_t f, float (&v)[4]) {
+  if (f == TSDE_FMT_STATE) {
+    v[0] = __uint_as_float(r.x); v[1] = __uint_as_float(r.y); v[2] = __uint_as_float(r.z); v[3] = __uint_as_float(r.w);
+    return;
+  }
+  v[0] = widen16(r.x & 0xffffu, f);
+  v[1] = widen16(r.x >> 16, f);
+  v[2] = widen16(r.y & 0xffffu, f);
+  v[3] = widen16(r.y >> 16, f);
+}
+__device__ __forceinline__ void st4f(void* p, int64_t i, uint32_t f, const float (&v)[4]) {
+  if (f == TSDE_FMT_STATE) {
+    st4(static_cast<float*>(p) + i, v);
+    return;
+  }
+  *reinterpret_cast<uint2*>(static_cast<uint16_t*>(p) + i) =
+      make_uint2(narrow16(v[0], f) | (narrow16(v[1], f) << 16), narrow16(v[2], f) | (narrow16(v[3], f) << 16));
+}
+// raw bits of one quad in format f (vector path: ld4raw; otherwise element by element, in .x .. .w)
+__device__ __forceinline__ uint4 load_quad_raw(const void* p, int64_t base, bool vec, int nvalid, uint32_t f) {
+  if (vec) return ld4raw<false>(p, base, f);
+  uint32_t r[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) r[j] = j < nvalid ? ld1raw(p, base + j, f) : 0u;
+  return make_uint4(r[0], r[1], r[2], r[3]);
+}
+__device__ __forceinline__ void widen_quad(const uint4 r, bool vec, uint32_t f, float (&v)[4]) {
+  if (vec) {
+    widen4(r, f, v);
+  } else {
+    v[0] = widen1(r.x, f); v[1] = widen1(r.y, f); v[2] = widen1(r.z, f); v[3] = widen1(r.w, f);
+  }
+}
+__device__ __forceinline__ void store_quad_fmt(void* p, int64_t base, bool vec, int nvalid, uint32_t f,
+                                               const float (&v)[4]) {
+  if (vec) {
+    st4f(p, base, f, v);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (j < nvalid) st1f(p, base + j, f, v[j]);
+  }
+}
+// the host's fast-path alignment: 16 bytes for a float32 / float64 operand, 8 for a 16-bit one
+inline bool aligned_for(const void* p, uint32_t f) {
+  return (reinterpret_cast<uintptr_t>(p) & (f == TSDE_FMT_STATE ? 15u : 7u)) == 0;
+}
 
 template <typename T>
 __device__ __forceinline__ void load_quad(const T* p, int64_t base, bool vec, int nvalid,
@@ -216,8 +318,10 @@ __device__ __forceinline__ void quad_noise(const NoiseP<T>& nz, Key key, int64_t
 // ---- the kernel -----------------------------------------------------------------------------
 // Op: struct with  static constexpr int NIN, NOUT; static constexpr bool USES_NOISE, WANT_U;
 //     template<T> __device__ void operator()(const T (&in)[NIN], T w, T u, T (&out)[NOUT]) const
+// (Mixed<Op>: the raw bits of all NIN operands stay live across the increment's draw, and then their widened values;
+// at 4 resident CTAs (64 registers) the 8-input ops would spill, so the bound is 2 CTAs for them)
 template <typename T, typename Op, int SRC>
-__global__ void __launch_bounds__(kThreads, 4)
+__global__ void __launch_bounds__(kThreads, is_mixed<Op>::value ? 2 : 4)
 ew_kernel(const EwP<Op::NIN, Op::NOUT> p, const NoiseP<T> nz, const Op op) {
   constexpr int NIN = Op::NIN, NOUT = Op::NOUT;
   Key key{0u, 0u};
@@ -245,14 +349,22 @@ ew_kernel(const EwP<Op::NIN, Op::NOUT> p, const NoiseP<T> nz, const Op op) {
     const int64_t rem = p.d - 4 * q;
     const int nvalid = rem < 4 ? (int)rem : 4;
     T in[NIN > 0 ? NIN : 1][4];
+    uint4 raw[NIN > 0 ? NIN : 1];  // (Mixed: every load issued before the first widening)
 #pragma unroll
-    for (int i = 0; i < NIN; ++i) load_quad(reinterpret_cast<const T*>(p.in[i]), base, vec, nvalid, in[i]);
+    for (int i = 0; i < NIN; ++i) {
+      if constexpr (is_mixed<Op>::value) raw[i] = load_quad_raw(p.in[i], base, vec, nvalid, operand_fmt(op.fmt, i));
+      else load_quad(reinterpret_cast<const T*>(p.in[i]), base, vec, nvalid, in[i]);
+    }
     T w[4], u[4];
     if (Op::USES_NOISE) {
       quad_noise<T, SRC, Op::WANT_U>(nz, key, row, q, vec, nvalid, w, u);
     } else {
 #pragma unroll
       for (int j = 0; j < 4; ++j) { w[j] = T(0); u[j] = T(0); }
+    }
+    if constexpr (is_mixed<Op>::value) {
+#pragma unroll
+      for (int i = 0; i < NIN; ++i) widen_quad(raw[i], vec, operand_fmt(op.fmt, i), in[i]);
     }
     T out[NOUT][4];
 #pragma unroll
@@ -265,7 +377,10 @@ ew_kernel(const EwP<Op::NIN, Op::NOUT> p, const NoiseP<T> nz, const Op op) {
       for (int i = 0; i < NOUT; ++i) out[i][j] = b[i];
     }
 #pragma unroll
-    for (int i = 0; i < NOUT; ++i) store_quad(reinterpret_cast<T*>(p.out[i]), base, vec, nvalid, out[i]);
+    for (int i = 0; i < NOUT; ++i) {
+      if constexpr (is_mixed<Op>::value) store_quad_fmt(p.out[i], base, vec, nvalid, operand_fmt(op.ofmt, i), out[i]);
+      else store_quad(reinterpret_cast<T*>(p.out[i]), base, vec, nvalid, out[i]);
+    }
   }
 }
 
@@ -317,15 +432,22 @@ __device__ __forceinline__ void ew_fast_body(const FastCtx<T, Op>& c, uint32_t Q
   constexpr int NIN = Op::NIN, NOUT = Op::NOUT;
   bool ok[U];
   T in[U][NIN > 0 ? NIN : 1][4];
+  uint4 raw[U][NIN > 0 ? NIN : 1];  // (Mixed: raw bits, widened once every load has been issued)
 #pragma unroll
   for (int k = 0; k < U; ++k) {
     const uint32_t Qk = Q + (uint32_t)k * kThreads;
     ok[k] = k == 0 || Qk < c.q_end;
     const size_t base = (size_t)Qk * 4;  // d == 4 * qpr: quads are laid out contiguously
+    if constexpr (is_mixed<Op>::value) {
+#pragma unroll
+      for (int i = 0; i < NIN; ++i) raw[k][i] = make_uint4(0u, 0u, 0u, 0u);
+    }
     if (ok[k]) {
 #pragma unroll
       for (int i = 0; i < NIN; ++i) {
-        if (streams_inputs<Op>::value)
+        if constexpr (is_mixed<Op>::value)
+          raw[k][i] = ld4raw<streams_inputs<Op>::value>(c.p.in[i], (int64_t)base, operand_fmt(c.op.fmt, i));
+        else if (streams_inputs<Op>::value)
           ld4cs(reinterpret_cast<const T*>(c.p.in[i]) + base, in[k][i]);
         else
           ld4(reinterpret_cast<const T*>(c.p.in[i]) + base, in[k][i]);
@@ -354,6 +476,13 @@ __device__ __forceinline__ void ew_fast_body(const FastCtx<T, Op>& c, uint32_t Q
       }
     }
   }
+  if constexpr (is_mixed<Op>::value) {
+#pragma unroll
+    for (int k = 0; k < U; ++k) {
+#pragma unroll
+      for (int i = 0; i < NIN; ++i) widen4(raw[k][i], operand_fmt(c.op.fmt, i), in[k][i]);
+    }
+  }
 #pragma unroll
   for (int k = 0; k < U; ++k) {
     if (!ok[k]) continue;
@@ -369,7 +498,10 @@ __device__ __forceinline__ void ew_fast_body(const FastCtx<T, Op>& c, uint32_t Q
       for (int i = 0; i < NOUT; ++i) out[i][j] = b[i];
     }
 #pragma unroll
-    for (int i = 0; i < NOUT; ++i) st4(reinterpret_cast<T*>(c.p.out[i]) + base, out[i]);
+    for (int i = 0; i < NOUT; ++i) {
+      if constexpr (is_mixed<Op>::value) st4f(c.p.out[i], (int64_t)base, operand_fmt(c.op.ofmt, i), out[i]);
+      else st4(reinterpret_cast<T*>(c.p.out[i]) + base, out[i]);
+    }
   }
 }
 
@@ -442,15 +574,20 @@ inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
                      const void* const* ins, void* const* outs, const Op& op) {
   EwP<Op::NIN, Op::NOUT> p{};
   bool vec = (L->d % 4) == 0;
+  uint32_t fmt = 0, ofmt = 0;
+  if constexpr (is_mixed<Op>::value) {
+    fmt = op.fmt;
+    ofmt = op.ofmt;
+  }
   for (int i = 0; i < Op::NIN; ++i) {
     if (!ins[i]) return TSDE_EINVAL;
     p.in[i] = ins[i];
-    vec = vec && aligned16(ins[i]);
+    vec = vec && aligned_for(ins[i], operand_fmt(fmt, i));
   }
   for (int i = 0; i < Op::NOUT; ++i) {
     if (!outs[i]) return TSDE_EINVAL;
     p.out[i] = outs[i];
-    vec = vec && aligned16(outs[i]);
+    vec = vec && aligned_for(outs[i], operand_fmt(ofmt, i));
   }
   NoiseP<T> np;
   if (int e = fill_noise<T>(L, Op::USES_NOISE ? nz : nullptr, bcast, np)) return e;

@@ -35,6 +35,25 @@ inline int dispatch(const tsde_launch* L, F&& body) {
   return L->dtype == TSDE_F32 ? body(float{}) : body(double{});
 }
 
+// dispatch() for the entry points whose SDE outputs may be 16-bit (TSDE_FMT_*).  Bit i of `sde_outputs` marks input
+// i as an SDE output.  Format bits anywhere else, with an F64 state, or of value 3 are TSDE_EINVAL (checked before
+// the empty-batch no-op).  `body` gets the element type of the state and the launch's format word (dtype >> 8; 0 for
+// an all-state-dtype launch, always 0 with an F64 state).
+template <typename F>
+inline int dispatch_fmt(const tsde_launch* L, uint32_t sde_outputs, F&& body) {
+  if (!valid_launch(L)) return TSDE_EINVAL;
+  const int32_t state = L->dtype & 0xff;
+  const uint32_t fmt = (uint32_t)L->dtype >> 8;
+  if (state != TSDE_F32 && state != TSDE_F64) return TSDE_EINVAL;
+  if (fmt && state != TSDE_F32) return TSDE_EINVAL;
+  for (int i = 0; i < 12; ++i) {
+    const uint32_t f = (fmt >> (2 * i)) & 3u;
+    if (f == 3u || (f && !((sde_outputs >> i) & 1u))) return TSDE_EINVAL;
+  }
+  if (L->rows == 0) return 0;
+  return state == TSDE_F32 ? body(float{}, fmt) : body(double{}, 0u);
+}
+
 inline int current_device() {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) cudaGetLastError();
@@ -117,6 +136,29 @@ inline int launch_kernel(void (*kernel)(P...), int64_t grid, int block, size_t s
   if (e != cudaSuccess) cudaGetLastError();
   return (int)e;
 }
+
+// ---- which inputs of an entry point are SDE outputs (dispatch_fmt): bit i = input i of its declaration -------------
+namespace sde_out {
+constexpr uint32_t step_euler = 0b110;              // y0, f, g
+constexpr uint32_t milstein_vjp_seed = 0b1;         // g
+constexpr uint32_t step_milstein = 0b0110;          // y0, f, g, gdg
+constexpr uint32_t milstein_gf_predict = 0b110;     // y0, f, g
+constexpr uint32_t step_milstein_gf = 0b1110;       // y0, f, g, gp
+constexpr uint32_t step_heun = 0b11110;             // y0, f, fp, g, gp
+constexpr uint32_t midpoint_predict = 0b110;        // y0, f, g
+constexpr uint32_t euler_heun_predict = 0b10;       // y0, g
+constexpr uint32_t step_euler_heun = 0b1110;        // y0, f, g, gp
+constexpr uint32_t reversible_heun_z = 0b1100;      // y0, z0, f0, g0
+constexpr uint32_t step_reversible_heun = 0b11110;  // y0, f0, f1, g0, g1
+constexpr uint32_t adjoint_a = 0b1100;              // y0, z0, f0, g0, adj_y0, adj_f0, adj_g0
+constexpr uint32_t adjoint_b = 0b11110;             // y0, f0, f1, g0, g1, adj_y0, adj_z0, vjp_z
+constexpr uint32_t srk_diag_stage1 = 0b110;         // y0, f0, g0
+constexpr uint32_t srk_diag_stage2 = 0b11110;       // y0, f0, g0, f1, g1
+constexpr uint32_t srk_diag_stage3 = 0b11110;       // y0, g0, g1, f2, g2
+constexpr uint32_t step_srk_diag = 0b11111110;      // y0, f0, f1, f2, g0, g1, g2, g3
+constexpr uint32_t srk_additive_stage = 0b110;      // y0, f0, ga
+constexpr uint32_t step_srk_additive = 0b11110;     // y0, f0, f1, ga, gb
+}  // namespace sde_out
 
 // ---- noise-layout routing of the tableau entry points (cabi.cu) ----------------------------------------------------
 // Row-wise kernels (tableau_diag.cu): DIAGONAL noise, and GENERAL noise with a single Brownian channel.

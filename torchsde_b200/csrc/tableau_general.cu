@@ -13,6 +13,7 @@
 // are bitwise reproducible and independent of batch sharding, and agree with torch.bmm to
 // rounding (bmm's own order is unspecified), which is how the parity tests treat them.
 #include <atomic>
+#include <type_traits>
 
 #include "ew.cuh"
 
@@ -98,14 +99,21 @@ gen_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const Op op
       const int mc = (int)(rem - dd * mq);
       const int64_t goff = ((p.gbcast ? 0 : (row0 + r) * d) + dd) * m + 4 * mc;
       T gv[NG][4];
+      uint4 graw[NG];  // (Mixed: every g load issued before the first widening)
 #pragma unroll
       for (int i = 0; i < NG; ++i) {
         if (valid) {
-          ld4(reinterpret_cast<const T*>(p.g[i]) + goff, gv[i]);
+          if constexpr (is_mixed<Op>::value) graw[i] = ld4raw<false>(p.g[i], goff, operand_fmt(op.fmt, NE + i));
+          else ld4(reinterpret_cast<const T*>(p.g[i]) + goff, gv[i]);
         } else {
+          graw[i] = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll
           for (int j = 0; j < 4; ++j) gv[i][j] = T(0);
         }
+      }
+      if constexpr (is_mixed<Op>::value) {
+#pragma unroll
+        for (int i = 0; i < NG; ++i) widen4(graw[i], operand_fmt(op.fmt, NE + i), gv[i]);
       }
       T part[NP];
 #pragma unroll
@@ -128,7 +136,14 @@ gen_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const Op op
         const int64_t eoff = (row0 + r) * d + dd;
         T e[NE > 0 ? NE : 1], o[NO];
 #pragma unroll
-        for (int i = 0; i < NE; ++i) e[i] = reinterpret_cast<const T*>(p.e[i])[eoff];
+        for (int i = 0; i < NE; ++i) {
+          if constexpr (is_mixed<Op>::value) e[i] = __uint_as_float(ld1raw(p.e[i], eoff, operand_fmt(op.fmt, i)));
+          else e[i] = reinterpret_cast<const T*>(p.e[i])[eoff];
+        }
+        if constexpr (is_mixed<Op>::value) {
+#pragma unroll
+          for (int i = 0; i < NE; ++i) e[i] = widen1(__float_as_uint(e[i]), operand_fmt(op.fmt, i));
+        }
         op.combine(e, part, o);
 #pragma unroll
         for (int i = 0; i < NO; ++i) reinterpret_cast<T*>(p.o[i])[eoff] = o[i];
@@ -148,14 +163,29 @@ gen_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const Op op
         const T u = Op::WANT_U ? su[r * m + mm] : T(0);
         T gj[NG];
 #pragma unroll
-        for (int i = 0; i < NG; ++i) gj[i] = reinterpret_cast<const T*>(p.g[i])[goff + mm];
+        for (int i = 0; i < NG; ++i) {
+          if constexpr (is_mixed<Op>::value)
+            gj[i] = __uint_as_float(ld1raw(p.g[i], goff + mm, operand_fmt(op.fmt, NE + i)));
+          else gj[i] = reinterpret_cast<const T*>(p.g[i])[goff + mm];
+        }
+        if constexpr (is_mixed<Op>::value) {
+#pragma unroll
+          for (int i = 0; i < NG; ++i) gj[i] = widen1(__float_as_uint(gj[i]), operand_fmt(op.fmt, NE + i));
+        }
 #pragma unroll
         for (int k = 0; k < NP; ++k) part[k] = part[k] + op.gval(k, gj) * op.weight(k, w, u);
       }
       const int64_t eoff = (row0 + r) * d + dd;
       T e[NE > 0 ? NE : 1], o[NO];
 #pragma unroll
-      for (int i = 0; i < NE; ++i) e[i] = reinterpret_cast<const T*>(p.e[i])[eoff];
+      for (int i = 0; i < NE; ++i) {
+        if constexpr (is_mixed<Op>::value) e[i] = __uint_as_float(ld1raw(p.e[i], eoff, operand_fmt(op.fmt, i)));
+        else e[i] = reinterpret_cast<const T*>(p.e[i])[eoff];
+      }
+      if constexpr (is_mixed<Op>::value) {
+#pragma unroll
+        for (int i = 0; i < NE; ++i) e[i] = widen1(__float_as_uint(e[i]), operand_fmt(op.fmt, i));
+      }
       op.combine(e, part, o);
 #pragma unroll
       for (int i = 0; i < NO; ++i) reinterpret_cast<T*>(p.o[i])[eoff] = o[i];
@@ -223,6 +253,7 @@ gen_cta_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const O
     const int c0 = base + tid;
     T gv[kGenUnroll][NG][4];
     T ev[kGenUnroll][NE > 0 ? NE : 1];  // element-wise operands, fetched together with g (not after the reduce)
+    uint4 graw[kGenUnroll][NG];  // (Mixed: raw bits, widened once every load of the pass has been issued)
     int rr[kGenUnroll], slots[kGenUnroll];
     bool valid[kGenUnroll];
 #pragma unroll
@@ -236,16 +267,28 @@ gen_cta_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const O
       const int64_t goff = p.gbcast ? (int64_t)4 * (dd * mq + mc) : tile0 + 4 * (int64_t)c;
       if (valid[un] && mc == 0) {
 #pragma unroll
-        for (int i = 0; i < NE; ++i) ev[un][i] = reinterpret_cast<const T*>(p.e[i])[slot0 + slot];
+        for (int i = 0; i < NE; ++i) {
+          if constexpr (is_mixed<Op>::value)
+            ev[un][i] = __uint_as_float(ld1raw(p.e[i], slot0 + slot, operand_fmt(op.fmt, i)));
+          else ev[un][i] = reinterpret_cast<const T*>(p.e[i])[slot0 + slot];
+        }
       }
 #pragma unroll
       for (int i = 0; i < NG; ++i) {
         if (valid[un]) {
-          if (streams_inputs<Op>::value && !p.gbcast) ld4cs(reinterpret_cast<const T*>(p.g[i]) + goff, gv[un][i]);
-          else ld4(reinterpret_cast<const T*>(p.g[i]) + goff, gv[un][i]);
+          if constexpr (is_mixed<Op>::value) {
+            const uint32_t f = operand_fmt(op.fmt, NE + i);
+            if (streams_inputs<Op>::value && !p.gbcast) graw[un][i] = ld4raw<true>(p.g[i], goff, f);
+            else graw[un][i] = ld4raw<false>(p.g[i], goff, f);
+          } else if (streams_inputs<Op>::value && !p.gbcast) {
+            ld4cs(reinterpret_cast<const T*>(p.g[i]) + goff, gv[un][i]);
+          } else {
+            ld4(reinterpret_cast<const T*>(p.g[i]) + goff, gv[un][i]);
+          }
         } else {
 #pragma unroll
           for (int j = 0; j < 4; ++j) gv[un][i][j] = T(0);
+          if constexpr (is_mixed<Op>::value) graw[un][i] = make_uint4(0u, 0u, 0u, 0u);
         }
       }
       slot += slots_per_load;
@@ -253,6 +296,15 @@ gen_cta_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const O
       while (dd >= d) { dd -= d; ++r; }
     }
     if (!synced) { __syncthreads(); synced = true; }  // increments visible (first pass is uniform)
+    if constexpr (is_mixed<Op>::value) {
+#pragma unroll
+      for (int un = 0; un < kGenUnroll; ++un) {
+#pragma unroll
+        for (int i = 0; i < NG; ++i) widen4(graw[un][i], operand_fmt(op.fmt, NE + i), gv[un][i]);
+#pragma unroll
+        for (int i = 0; i < NE; ++i) ev[un][i] = widen1(__float_as_uint(ev[un][i]), operand_fmt(op.fmt, i));
+      }
+    }
 #pragma unroll
     for (int un = 0; un < kGenUnroll; ++un) {
       T part[NP];
@@ -645,10 +697,16 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
     return TSDE_EINVAL;  // (a user-supplied product, TSDE_SRC_UNIT, goes through the element-wise entry points)
   GenP<Op::NE, Op::NG, Op::NO> p{};
   bool vec = (L->m % 4) == 0;
+  uint32_t fmt = 0;
+  if constexpr (is_mixed<Op>::value) fmt = op.fmt;
   int i = 0;
   for (const void* q : es) { if (!q) return TSDE_EINVAL; p.e[i++] = q; }
   i = 0;
-  for (const void* q : gs) { if (!q) return TSDE_EINVAL; p.g[i++] = q; vec = vec && aligned16(q); }
+  for (const void* q : gs) {
+    if (!q) return TSDE_EINVAL;
+    vec = vec && aligned_for(q, operand_fmt(fmt, Op::NE + i));
+    p.g[i++] = q;
+  }
   i = 0;
   for (void* q : os) { if (!q) return TSDE_EINVAL; p.o[i++] = q; }
   NoiseP<T> np;
@@ -663,9 +721,12 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
   const bool mem = nz->source == TSDE_SRC_MEMORY;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
   if (vec) {
-    if (!p.gbcast && tma_route<Op>(mq)) {  // (a broadcast g has no tile stream to stage)
-      int rc = launch_gen_tma<T, Op>(L, nz, p, np, op, st);
-      if (rc != kTmaNotEligible) return rc;
+    // (a broadcast g has no tile stream to stage; 16-bit operands are not staged by the TMA kernel)
+    if constexpr (!is_mixed<Op>::value) {
+      if (!p.gbcast && tma_route<Op>(mq)) {
+        int rc = launch_gen_tma<T, Op>(L, nz, p, np, op, st);
+        if (rc != kTmaNotEligible) return rc;
+      }
     }
     // one 128-thread CTA per group of rw rows
     const int64_t rw = 32 / mq;
@@ -692,6 +753,18 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
   if (blocks > 0x7fffffffll) return TSDE_EINVAL;
   return launch_kernel(mem ? gen_kernel<T, Op, TSDE_SRC_MEMORY> : gen_kernel<T, Op, TSDE_SRC_COUNTER>, blocks,
                        kThreads, (size_t)(rb * smem_per_row), st, false, p, np, op);
+}
+
+// A launch that declares 16-bit SDE outputs (float32 state only, see dispatch_fmt) takes the Mixed<Op> tile kernels;
+// `fmt` covers the element-wise operands, then the g operands, in the entry point's order.
+template <typename T, typename Op>
+static int launch_gen_fmt(const tsde_launch* L, const tsde_noise* nz, std::initializer_list<const void*> es,
+                          std::initializer_list<const void*> gs, std::initializer_list<void*> os, const Op& op,
+                          uint32_t fmt) {
+  if constexpr (std::is_same<T, float>::value) {
+    if (fmt) return launch_gen<T>(L, nz, es, gs, os, Mixed<Op>{op, fmt, 0u});
+  }
+  return launch_gen<T>(L, nz, es, gs, os, op);
 }
 
 // ---- ops ---------------------------------------------------------------------------------------
@@ -900,40 +973,40 @@ struct AdjBElemOp {  // in: adj_y0, adj_z0, vjp_z -> adj_y1, adj_z1, adj_f1
 // The routes of cabi.cu for general noise with m > 1.
 int general_step_euler(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f, const void* g,
                        double dt, void* y1) {
-  return dispatch(L, [&](auto t) {
+  return dispatch_fmt(L, sde_out::step_euler, [&](auto t, uint32_t fmt) {
     using T = decltype(t);
-    return launch_gen<T>(L, nz, {y0, f}, {g}, {y1}, GEulerOp<T>{(T)dt});
+    return launch_gen_fmt<T>(L, nz, {y0, f}, {g}, {y1}, GEulerOp<T>{(T)dt}, fmt);
   });
 }
 
 int general_step_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f, const void* fp,
                       const void* g, const void* gp, double dt, void* y1) {
-  return dispatch(L, [&](auto t) {
+  return dispatch_fmt(L, sde_out::step_heun, [&](auto t, uint32_t fmt) {
     using T = decltype(t);
-    return launch_gen<T>(L, nz, {y0, f, fp}, {g, gp}, {y1}, GHeunOp<T>{(T)dt});
+    return launch_gen_fmt<T>(L, nz, {y0, f, fp}, {g, gp}, {y1}, GHeunOp<T>{(T)dt}, fmt);
   });
 }
 
 int general_midpoint_predict(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f,
                              const void* g, double half_dt, void* yp) {
-  return dispatch(L, [&](auto t) {
+  return dispatch_fmt(L, sde_out::midpoint_predict, [&](auto t, uint32_t fmt) {
     using T = decltype(t);
-    return launch_gen<T>(L, nz, {y0, f}, {g}, {yp}, GMidpointPredictOp<T>{(T)half_dt});
+    return launch_gen_fmt<T>(L, nz, {y0, f}, {g}, {yp}, GMidpointPredictOp<T>{(T)half_dt}, fmt);
   });
 }
 
 int general_euler_heun_predict(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* g, void* yp) {
-  return dispatch(L, [&](auto t) {
+  return dispatch_fmt(L, sde_out::euler_heun_predict, [&](auto t, uint32_t fmt) {
     using T = decltype(t);
-    return launch_gen<T>(L, nz, {y0}, {g}, {yp}, GEulerHeunPredictOp<T>{});
+    return launch_gen_fmt<T>(L, nz, {y0}, {g}, {yp}, GEulerHeunPredictOp<T>{}, fmt);
   });
 }
 
 int general_step_euler_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f,
                             const void* g, const void* gp, double dt, void* y1) {
-  return dispatch(L, [&](auto t) {
+  return dispatch_fmt(L, sde_out::step_euler_heun, [&](auto t, uint32_t fmt) {
     using T = decltype(t);
-    return launch_gen<T>(L, nz, {y0, f}, {g, gp}, {y1}, GEulerHeunOp<T>{(T)dt});
+    return launch_gen_fmt<T>(L, nz, {y0, f}, {g, gp}, {y1}, GEulerHeunOp<T>{(T)dt}, fmt);
   });
 }
 
@@ -941,18 +1014,18 @@ int general_step_euler_heun(const tsde_launch* L, const tsde_noise* nz, const vo
 int general_reversible_heun_z(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* z0,
                               const void* f0, const void* g0, double dt, void* z1) {
   if (nz && nz->flags) return TSDE_EINVAL;
-  return dispatch(L, [&](auto t) {
+  return dispatch_fmt(L, sde_out::reversible_heun_z, [&](auto t, uint32_t fmt) {
     using T = decltype(t);
-    return launch_gen<T>(L, nz, {y0, z0, f0}, {g0}, {z1}, GRevHeunZOp<T>{(T)dt, 0});
+    return launch_gen_fmt<T>(L, nz, {y0, z0, f0}, {g0}, {z1}, GRevHeunZOp<T>{(T)dt, 0}, fmt);
   });
 }
 
 int general_step_reversible_heun(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f0,
                                  const void* f1, const void* g0, const void* g1, double half_dt, void* y1) {
   if (nz && nz->flags) return TSDE_EINVAL;
-  return dispatch(L, [&](auto t) {
+  return dispatch_fmt(L, sde_out::step_reversible_heun, [&](auto t, uint32_t fmt) {
     using T = decltype(t);
-    return launch_gen<T>(L, nz, {y0, f0, f1}, {g0, g1}, {y1}, GRevHeunOp<T>{(T)half_dt, 0});
+    return launch_gen_fmt<T>(L, nz, {y0, f0, f1}, {g0, g1}, {y1}, GRevHeunOp<T>{(T)half_dt, 0}, fmt);
   });
 }
 
@@ -961,10 +1034,10 @@ int general_adjoint_reversible_heun_a(const tsde_launch* L, const tsde_noise* nz
                                       const void* adj_g0, double dt, double half_dt, void* z1, void* adj_f0_out,
                                       void* adj_g0_out) {
   if (nz && nz->flags) return TSDE_EINVAL;
-  return dispatch(L, [&](auto t) {
+  return dispatch_fmt(L, sde_out::adjoint_a, [&](auto t, uint32_t fmt) {
     using T = decltype(t);
     // z1 = 2*y0 - z0 - f0*dt - g0.dW                                              :109
-    if (int e = launch_gen<T>(L, nz, {y0, z0, f0}, {g0}, {z1}, GRevHeunZOp<T>{(T)dt, 1})) return e;
+    if (int e = launch_gen_fmt<T>(L, nz, {y0, z0, f0}, {g0}, {z1}, GRevHeunZOp<T>{(T)dt, 1}, fmt)) return e;
     // adj_f0' = adj_f0 + adj_y0*half_dt                                            :104,113
     tsde_launch r = *L;
     r.noise_type = TSDE_NOISE_DIAGONAL;
@@ -982,10 +1055,10 @@ int general_adjoint_reversible_heun_b(const tsde_launch* L, const tsde_noise* nz
                                       const void* adj_z0, const void* vjp_z, double dt, double half_dt, void* y1,
                                       void* adj_y1, void* adj_z1, void* adj_f1, void* adj_g1) {
   if (nz && nz->flags) return TSDE_EINVAL;
-  return dispatch(L, [&](auto t) {
+  return dispatch_fmt(L, sde_out::adjoint_b, [&](auto t, uint32_t fmt) {
     using T = decltype(t);
     // y1 = y0 - (f0+f1)*half_dt - (g0+g1).half_dW                                   :134-135
-    if (int e = launch_gen<T>(L, nz, {y0, f0, f1}, {g0, g1}, {y1}, GRevHeunOp<T>{(T)half_dt, 1})) return e;
+    if (int e = launch_gen_fmt<T>(L, nz, {y0, f0, f1}, {g0, g1}, {y1}, GRevHeunOp<T>{(T)half_dt, 1}, fmt)) return e;
     // element-wise part: adj_y1, adj_z1 = -(adj_z0 + vjp_z), adj_f1
     tsde_launch r = *L;
     r.noise_type = TSDE_NOISE_DIAGONAL;
@@ -1006,9 +1079,9 @@ using namespace tsde;
 TSDE_EXPORT int tsde_srk_additive_stage(const tsde_launch* L, const tsde_noise* nz, const void* y0, const void* f0,
                                         const void* ga, double dt, double rdt, void* h0_1) {
   if (!L || L->noise_type != TSDE_NOISE_GENERAL) return TSDE_EINVAL;
-  return dispatch(L, [&](auto t) {
+  return dispatch_fmt(L, sde_out::srk_additive_stage, [&](auto t, uint32_t fmt) {
     using T = decltype(t);
-    return launch_gen<T>(L, nz, {y0, f0}, {ga}, {h0_1}, GSraStageOp<T>{(T)dt, (T)rdt});
+    return launch_gen_fmt<T>(L, nz, {y0, f0}, {ga}, {h0_1}, GSraStageOp<T>{(T)dt, (T)rdt}, fmt);
   });
 }
 
@@ -1016,10 +1089,10 @@ TSDE_EXPORT int tsde_step_srk_additive(const tsde_launch* L, const tsde_noise* n
                                        const void* f1, const void* ga, const void* gb, double dt, double rdt,
                                        void* y1) {
   if (!L || L->noise_type != TSDE_NOISE_GENERAL) return TSDE_EINVAL;
-  return dispatch(L, [&](auto t) {
+  return dispatch_fmt(L, sde_out::step_srk_additive, [&](auto t, uint32_t fmt) {
     using T = decltype(t);
-    return launch_gen<T>(L, nz, {y0, f0, f1}, {ga, gb}, {y1},
-                         GSraFinalOp<T>{(T)dt, (T)rdt, (T)(1.0 / 3), (T)(2.0 / 3)});
+    return launch_gen_fmt<T>(L, nz, {y0, f0, f1}, {ga, gb}, {y1},
+                             GSraFinalOp<T>{(T)dt, (T)rdt, (T)(1.0 / 3), (T)(2.0 / 3)}, fmt);
   });
 }
 
