@@ -49,8 +49,11 @@ def _box_muller_f64(a, b):
     return r * np.choose(k, [c, -s, -c, s]), r * np.choose(k, [s, c, -s, -c])
 
 
-def normals(key, node_id, stream, rows, m, dtype, row_offset=0, row_ids=None):
+def normals(key, node_id, stream, rows, m, dtype, row_offset=0, row_ids=None, exact=False):
     """(rows, m) normals of (key, node_id, stream).  Mirrors normal4() for every quad.
+
+    `exact`: return the float64 values the specification of `dtype` is computed in, before the final rounding to
+    `dtype` (for a float64 restatement of a kernel that bounds its own rounding errors).
 
     `row_ids` (optional 1-D integer array) selects arbitrary global rows instead of the contiguous block
     row_offset .. row_offset + rows - 1: rows are independent streams, which is what lets the full-size
@@ -96,4 +99,4 @@ def normals(key, node_id, stream, rows, m, dtype, row_offset=0, row_ids=None):
                   .astype(np.float64) + 0.5) * 1.1102230246251565e-16
             n0, n1 = _box_muller_f64(ua, ub)
             out[:, 2 * call::4], out[:, 2 * call + 1::4] = n0, n1
-    return out[:, :m].astype(dtype)
+    return out[:, :m] if exact else out[:, :m].astype(dtype)

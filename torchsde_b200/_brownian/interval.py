@@ -44,6 +44,8 @@ from ..settings import LEVY_AREA_APPROXIMATIONS
 
 _MASK64 = (1 << 64) - 1
 _LEAF, _BINARY, _GRID = 0, 1, 2
+# channels of one row: channel / 4 is a 24-bit field of the Philox counter (csrc/philox.cuh); the library refuses more
+MAX_CHANNELS = 1 << 26
 
 
 def mix64(x):
@@ -278,6 +280,10 @@ class BrownianInterval(brownian_base.BaseBrownian):
             self._rows, self._m = 1, int(size[0])
         else:
             self._rows, self._m = 1, 1
+        if self._m > MAX_CHANNELS:
+            raise ValueError(f"BrownianInterval supports at most 2**26 channels (the last dimension of `size`), got "
+                             f"{self._m}: the samples are drawn from a counter whose channel field has 26 bits, so "
+                             f"further channels would repeat the normals of other channels.")
 
         self._key = key_from_entropy(entropy)
         self._key_dev = None

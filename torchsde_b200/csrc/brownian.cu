@@ -184,7 +184,7 @@ static int bridge_impl(const tsde_launch* L, const void* key, int64_t row_offset
   const bool have_h = in_h != nullptr;
   if (have_h && !out_h) return TSDE_EINVAL;
   const int64_t m = L->m, rows = L->rows, qpr = (m + 3) / 4, nquads = rows * qpr;
-  if (rows + row_offset > kMaxGlobalRows) return TSDE_EINVAL;
+  if (rows + row_offset > kMaxGlobalRows || m > kMaxCounterChannels) return TSDE_EINVAL;
   const bool vec = (m % 4 == 0) && aligned16(in_w) && aligned16(out_w) &&
                    (!have_h || (aligned16(in_h) && aligned16(out_h)));
   cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
@@ -284,8 +284,14 @@ struct HToUOp {
 // triangle, mirror it (A is antisymmetric, exactly: this translation unit is compiled without FMA contraction)
 // into a warp-private shared tile, and the warp stores the tile with fully coalesced 128-bit writes.
 // Foster's std needs one square root per pair: fp32 takes the SFU's (MUFU.SQRT, ~1 ulp; the IEEE-rounded `sqrtf`
-// is a ~10-instruction Newton sequence and the kernel is issue-bound), fp64 the correctly rounded one.
-__device__ __forceinline__ float levy_sqrt(float x) { return mufu_sqrt(x); }
+// is a ~10-instruction Newton sequence and the kernel is issue-bound), fp64 the correctly rounded one.  The SFU flushes
+// a subnormal operand to zero, and Foster's variance ~0.027 h^2 is subnormal for h below ~2^-60, where the noise term
+// is as large as the cross term: such an operand is scaled by 2^64 first and the root by 2^-32 after (both exact).
+__device__ __forceinline__ float levy_sqrt(float x) {
+  const bool tiny = x < 1.17549435e-38f;   // FLT_MIN
+  const float r = mufu_sqrt(tiny ? x * 18446744073709551616.0f : x);
+  return tiny ? r * 2.3283064365386963e-10f : r;
+}
 __device__ __forceinline__ double levy_sqrt(double x) { return sqrt(x); }
 
 template <typename T, bool FOSTER>

@@ -566,6 +566,10 @@ inline int fill_noise(const tsde_launch* L, const tsde_noise* nz, bool bcast, No
   if (nz->source == TSDE_SRC_MEMORY && !nz->w) return TSDE_EINVAL;
   if (nz->source == TSDE_SRC_MEMORY && nz->want_u && !nz->u) return TSDE_EINVAL;
   if (nz->source == TSDE_SRC_COUNTER && !nz->key) return TSDE_EINVAL;
+  // the channels drawn: m (the row-wise kernels draw one per column of d, d = m for diagonal noise)
+  if (nz->source == TSDE_SRC_COUNTER && !bcast &&
+      (L->m > kMaxCounterChannels || (L->noise_type == TSDE_NOISE_DIAGONAL && L->d > kMaxCounterChannels)))
+    return TSDE_EINVAL;
   return 0;
 }
 

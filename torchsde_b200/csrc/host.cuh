@@ -21,6 +21,9 @@ constexpr int kSMs = 132;  // H100 SXM; only a fallback, sm_count() asks the dev
 
 // Global rows (local row + row_offset) are one 32-bit word of the Philox counter.
 constexpr int64_t kMaxGlobalRows = 0xFFFFFFFFll;
+// A channel quad (channel / 4) is the low 24 bits of another word, with the stream tag above it (philox.cuh): past
+// 2^26 channels one stream's normals would be another stream's.
+constexpr int64_t kMaxCounterChannels = 1ll << 26;
 
 // A launch descriptor every entry point can rely on: non-null, non-negative row count, positive widths.
 inline bool valid_launch(const tsde_launch* L) { return L && L->rows >= 0 && L->d > 0 && L->m > 0; }
