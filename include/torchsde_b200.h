@@ -177,12 +177,17 @@ int tsde_brownian_cell_levy(const tsde_launch* L, const tsde_noise* nz, uint64_t
                             void* out_u, void* out_a);
 
 /*
- * `logqp=True` (diagonal noise): the KL-integrand augmentation of SDELogqp.f_and_g_diagonal
- * (base_sde.py:266-283, misc.py:66-68):  u = (f - h) / stable(g),  f_aug = [f, 0.5 sum_d u^2],  g_aug = [g, 0].
- * f, g, h are (rows,d); f_aug, g_aug are (rows,d+1).  L: noise_type DIAGONAL, d = m = state channels WITHOUT the
- * log-ratio channel.  (General noise solves a least-squares problem per row, `pinverse`: it stays in the host's
- * linear algebra.)
+ * `logqp=True`: the KL-integrand augmentation of SDELogqp.f_and_g_* (base_sde.py:240-306).  d (and m) count the
+ * state channels WITHOUT the log-ratio channel; f, h are (rows,d) and f_aug is (rows,d+1).
+ *   DIAGONAL (f_and_g_diagonal :266-283, misc.py:66-68):  u = (f - h) / stable(g),  f_aug = [f, 0.5 sum_d u^2],
+ *     g_aug = [g, 0];  g is (rows,d), g_aug (rows,d+1), d == m, and `eps` is stable_division's epsilon.
+ *   GENERAL, also additive and scalar noise (f_and_g_general :285-306):  u = pinverse(g, rcond) (f - h),
+ *     f_aug = [f, 0.5 |u|^2],  g_aug = [g ; 0] (a zero row appended);  g is a dense (rows,d,m), g_aug (rows,d+1,m),
+ *     and `eps` is pinverse's rcond (singular values s <= rcond * s_max are dropped).  Per row, a one-sided Jacobi
+ *     SVD in shared memory: min(d,m) * max(d,m) + d must not exceed TSDE_LOGQP_GENERAL_MAX, else TSDE_EINVAL.
+ *     A row whose g or f - h holds a NaN / Inf gets a NaN rate.
  */
+#define TSDE_LOGQP_GENERAL_MAX 16384
 int tsde_logqp_augment(const tsde_launch* L, const void* f, const void* g, const void* h, double eps,
                        void* f_aug, void* g_aug);
 

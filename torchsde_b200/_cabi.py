@@ -21,6 +21,13 @@ NOISE_DIAGONAL, NOISE_GENERAL = 0, 1
 SRC_MEMORY, SRC_COUNTER, SRC_UNIT = 0, 1, 2
 EINVAL = -22
 FLAG_G_BROADCAST = 1
+LOGQP_GENERAL_MAX = 16384  # TSDE_LOGQP_GENERAL_MAX
+
+
+def logqp_general_fits(d, m):
+    """Whether tsde_logqp_augment takes a general-noise (d, m) row: its min(d,m) x max(d,m) matrix plus f - h within
+    LOGQP_GENERAL_MAX elements of shared memory."""
+    return min(d, m) * max(d, m) + d <= LOGQP_GENERAL_MAX
 
 
 class LibraryNotBuilt(RuntimeError):

@@ -177,8 +177,12 @@ class SDELogqp(BaseSDE):
         base = self._base_sde
         f, g, h = (widen(x, y.dtype) for x in (base.f(t, state), base.g(t, state), base.h(t, state)))
         differentiated = torch.is_grad_enabled() and (f.requires_grad or g.requires_grad or h.requires_grad)
-        if self._diagonal and not differentiated and self._on_device(f):
-            return self._fused_augment(f, g, h)
+        if not differentiated and self._on_device(f):
+            if self._diagonal:
+                return self._fused_augment(f, g, h)
+            from .. import _cabi
+            if _cabi.logqp_general_fits(g.size(1), g.size(2)):
+                return self._fused_augment_general(f, g, h)
         rate = _kl_rate(f, g, h, self._diagonal)
         return torch.cat([f, rate], dim=1), self._pad_diffusion(g)
 
@@ -203,6 +207,22 @@ class SDELogqp(BaseSDE):
         g_aug = torch.empty_like(f_aug)
         L = _cabi.make_launch(f.dtype, _cabi.NOISE_DIAGONAL, rows, d, d, device=f.device)
         _cabi.check(_cabi.lib().tsde_logqp_augment(ctypes.byref(L), f.data_ptr(), g.data_ptr(), h.data_ptr(), epsilon,
+                                                   f_aug.data_ptr(), g_aug.data_ptr()), "tsde_logqp_augment")
+        return f_aug, g_aug
+
+    @staticmethod
+    def _fused_augment_general(f, g, h, rcond=1e-15):
+        """General, additive and scalar noise: |pinverse(g) (f - h)|^2 by a per-row Jacobi SVD in one kernel instead of
+        a batched SVD that synchronises the host, so such solves can be captured into a CUDA graph.  An `expand`ed g
+        (additive noise) is materialised first, as the torch path's `cat` does."""
+        import ctypes
+        from .. import _cabi
+        f, g, h = (x if x.is_contiguous() else x.contiguous() for x in (f, g, h))
+        rows, d, m = g.shape
+        f_aug = torch.empty((rows, d + 1), dtype=f.dtype, device=f.device)
+        g_aug = torch.empty((rows, d + 1, m), dtype=g.dtype, device=g.device)
+        L = _cabi.make_launch(f.dtype, _cabi.NOISE_GENERAL, rows, d, m, device=f.device)
+        _cabi.check(_cabi.lib().tsde_logqp_augment(ctypes.byref(L), f.data_ptr(), g.data_ptr(), h.data_ptr(), rcond,
                                                    f_aug.data_ptr(), g_aug.data_ptr()), "tsde_logqp_augment")
         return f_aug, g_aug
 

@@ -168,8 +168,9 @@ def integrate_captured(solver, y0, ts, extra0, static_ok=False):
                 plan = _capture(solver, sched, binding, y0, ts, extra0)
         except RuntimeError as e:
             # f / g did something a stream capture cannot record (a host sync or a host<->device copy — e.g.
-            # `pinverse` in the general-noise KL rate of logqp=True, or `.item()` in user code).  Such SDEs run
-            # with the ordinary eager loop; remember it so that the capture is not attempted on every call.
+            # `.item()` in user code, or `pinverse` in the KL rate of a general-noise logqp=True solve whose (d, m)
+            # is over tsde_logqp_augment's bound).  Such SDEs run with the ordinary eager loop; remember it so that
+            # the capture is not attempted on every call.
             if 'captur' not in str(e).lower():
                 raise
             import warnings

@@ -203,9 +203,219 @@ static int logqp_augment_impl(const tsde_launch* L, const void* f, const void* g
 
 }  // namespace tsde
 
+// ---- logqp: KL-integrand augmentation, general / additive / scalar noise ---------------------------------------
+// torchsde/_core/base_sde.py:285-306 (SDELogqp.f_and_g_general):
+//     u = pinverse(g) (f - h);   f_aug = [f, 0.5 |u|^2];   g_aug = [g ; 0]      g:(d, m) per row, rcond = 1e-15
+// The reference runs a batched SVD (cuSOLVER, with a host synchronisation) on every drift evaluation.  Here one
+// group of warps per row runs a one-sided (Hestenes) Jacobi SVD on the row's matrix in shared memory; neither U nor V
+// is stored, only what |u|^2 needs:
+//   * tall, d >= m: the m columns of g (length d) are orthogonalised, G V = U S.  With c_i = (G V)_i . r and
+//     s_i^2 = |(G V)_i|^2:  |u|^2 = sum_i c_i^2 / s_i^4  (V is orthogonal, so it drops out of the norm);
+//   * wide, d < m: the d columns of g^T (the rows of g, length m) are orthogonalised, g^T V = U S, and every rotation
+//     of the pair (i, j) is applied to (r_i, r_j) too, so r ends as V^T r:  |u|^2 = sum_i r'_i^2 / s_i^2.
+// Singular values are kept as pinverse keeps them: s_i > rcond * s_max.  A structurally zero column (or row) of g
+// stays exactly zero under the rotations and contributes nothing.
+// Pairs are visited in round-robin (tournament) order: n/2 disjoint pairs per round, one warp per pair, dot products
+// reduced with shuffles and the rotation applied in place.  A sweep in which no pair of any row of the CTA rotated
+// ends the loop (a CTA-wide vote), at most kLqMaxSweeps sweeps: extra sweeps of a converged row rotate nothing, so
+// its result does not depend on which rows share its CTA.  A pair is rotated only if |a_i.a_j| > tol |a_i| |a_j|,
+// so NaN / Inf never rotate; a row with a non-finite g or f - h gets a NaN rate, as the torch path's SVD gives.
+namespace tsde {
+
+constexpr int kLqMaxSweeps = 30;
+constexpr int kLqWarps = 8;  // warps per CTA
+
+// Per-row shared-memory layout (elements of T): A[n*k] | r[d] | s2[n] | c[n], padded to an even count.
+__host__ __device__ inline int lq_stride(int d, int m) {
+  const int n = d < m ? d : m, k = d < m ? m : d;
+  return (n * k + d + 2 * n + 1) & ~1;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kLqWarps * 32)
+logqp_augment_general_kernel(int64_t rows, int d, int m, const T* __restrict__ f, const T* __restrict__ g,
+                             const T* __restrict__ h, T rcond, T* __restrict__ f_aug, T* __restrict__ g_aug,
+                             int rows_per_cta, int warps_per_row) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const bool tall = d >= m;
+  const int n = tall ? m : d, k = tall ? d : m;
+  const int n2 = n + (n & 1);                         // even number of players (one idle for odd n)
+  const int stride = lq_stride(d, m);
+  const int group_threads = warps_per_row * 32;
+  const int grp = threadIdx.x / group_threads, t = threadIdx.x - grp * group_threads;
+  const int w = t >> 5, lane = t & 31;
+  T* A = reinterpret_cast<T*>(smem_raw) + (size_t)grp * stride;
+  T* r = A + n * k;
+  T* s2 = r + d;
+  T* cc = s2 + n;
+  int* bad = reinterpret_cast<int*>(reinterpret_cast<T*>(smem_raw) + (size_t)rows_per_cta * stride);
+  const int64_t row = (int64_t)blockIdx.x * rows_per_cta + grp;
+  const bool active = row < rows;
+  constexpr T u = sizeof(T) == 4 ? T(5.9604644775390625e-8) : T(1.1102230246251565e-16);
+  // below the rounding error of the dot products themselves: a (k/32)-term chain per lane, then 5 shuffle levels
+  const T tol = T((k + 31) / 32 + 5) * u;
+
+  if (t == 0) bad[grp] = 0;
+  __syncthreads();
+  if (active) {
+    const int64_t dm = (int64_t)d * m;
+    const T* gr = g + row * dm;
+    T* go = g_aug + row * (dm + m);
+    bool nf = false;
+    for (int e = t; e < d * m; e += group_threads) {
+      const T v = gr[e];
+      go[e] = v;
+      nf |= !isfinite(v);
+      if (tall) {
+        const int i = e / m, j = e - i * m;
+        A[j * k + i] = v;                                // column j of g
+      } else {
+        A[e] = v;                                        // row i of g = column i of g^T
+      }
+    }
+    for (int e = t; e < m; e += group_threads) go[dm + e] = T(0);
+    const T* fr = f + row * d;
+    const T* hr = h + row * d;
+    T* fo = f_aug + row * (d + 1);
+    for (int e = t; e < d; e += group_threads) {
+      const T fv = fr[e];
+      fo[e] = fv;
+      const T rv = fv - hr[e];
+      r[e] = rv;
+      nf |= !isfinite(rv);
+    }
+    if (__any_sync(0xffffffffu, nf) && lane == 0) atomicOr(&bad[grp], 1);
+  }
+  __syncthreads();
+  const bool live = active && !bad[grp];
+
+  for (int sweep = 0; sweep < kLqMaxSweeps; ++sweep) {
+    int rotated = 0;
+    for (int round = 0; round < n2 - 1; ++round) {
+      for (int p = w; p < n2 / 2; p += warps_per_row) {
+        // circle method: slot 0 holds player 0, slots 1..n2-1 hold the others shifted by `round`; pair p is the
+        // players of slots p and n2-1-p
+        const int a = p == 0 ? 0 : (p - 1 + round) % (n2 - 1) + 1;
+        const int b = (n2 - 2 - p + round) % (n2 - 1) + 1;
+        if (!live || a >= n || b >= n) continue;
+        T* x = A + a * k;
+        T* y = A + b * k;
+        T app = T(0), aqq = T(0), apq = T(0);
+        for (int i = lane; i < k; i += 32) {
+          const T xv = x[i], yv = y[i];
+          app = fma(xv, xv, app);
+          aqq = fma(yv, yv, aqq);
+          apq = fma(xv, yv, apq);
+        }
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) {
+          app += __shfl_xor_sync(0xffffffffu, app, off);
+          aqq += __shfl_xor_sync(0xffffffffu, aqq, off);
+          apq += __shfl_xor_sync(0xffffffffu, apq, off);
+        }
+        // (false for NaN / Inf: such a pair is never rotated)
+        if (!(fabs(apq) > tol * sqrt(app) * sqrt(aqq))) continue;
+        const T zeta = (aqq - app) / (T(2) * apq);
+        const T az = fabs(zeta);
+        const T root = az < T(1e8) ? sqrt(T(1) + zeta * zeta) : az;
+        const T tn = (zeta < T(0) ? T(-1) : T(1)) / (az + root);
+        const T cs = T(1) / sqrt(T(1) + tn * tn), sn = cs * tn;
+        for (int i = lane; i < k; i += 32) {
+          const T xv = x[i], yv = y[i];
+          x[i] = cs * xv - sn * yv;
+          y[i] = sn * xv + cs * yv;
+        }
+        if (!tall && lane == 0) {
+          const T ra = r[a], rb = r[b];
+          r[a] = cs * ra - sn * rb;
+          r[b] = sn * ra + cs * rb;
+        }
+        rotated = 1;
+      }
+      __syncthreads();
+    }
+    if (!__syncthreads_or(rotated)) break;
+  }
+
+  if (active) {
+    for (int j = w; j < n; j += warps_per_row) {
+      const T* x = A + j * k;
+      T ss = T(0), c = T(0);
+      for (int i = lane; i < k; i += 32) {
+        ss = fma(x[i], x[i], ss);
+        if (tall) c = fma(x[i], r[i], c);
+      }
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) {
+        ss += __shfl_xor_sync(0xffffffffu, ss, off);
+        c += __shfl_xor_sync(0xffffffffu, c, off);
+      }
+      if (lane == 0) {
+        s2[j] = ss;
+        cc[j] = tall ? c : r[j];
+      }
+    }
+  }
+  __syncthreads();
+  if (active && w == 0) {
+    const T qnan = sizeof(T) == 4 ? T(__int_as_float(0x7fc00000)) : T(__longlong_as_double(0x7ff8000000000000ll));
+    T smax = T(0);
+    for (int j = lane; j < n; j += 32) smax = fmax(smax, sqrt(s2[j]));
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) smax = fmax(smax, __shfl_xor_sync(0xffffffffu, smax, off));
+    const T cut = rcond * smax;
+    T acc = T(0);
+    for (int j = lane; j < n; j += 32) {
+      const T s = sqrt(s2[j]);
+      if (s > cut) {
+        const T q = tall ? (cc[j] / s) / s : cc[j] / s;
+        acc = fma(q, q, acc);
+      }
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
+    if (lane == 0) f_aug[row * (d + 1) + d] = bad[grp] ? qnan : T(0.5) * acc;
+  }
+}
+
+// One row's tall-orientation matrix (min(d,m) x max(d,m)) plus r = f - h within TSDE_LOGQP_GENERAL_MAX elements.
+// (d, m <= the bound first: then neither the product nor d + 1 can overflow.)
+inline bool logqp_general_fits(int64_t d, int64_t m) {
+  if (d > TSDE_LOGQP_GENERAL_MAX || m > TSDE_LOGQP_GENERAL_MAX) return false;
+  return (d < m ? d : m) * (d < m ? m : d) + d <= TSDE_LOGQP_GENERAL_MAX;
+}
+
+template <typename T>
+static int logqp_augment_general_impl(const tsde_launch* L, const void* f, const void* g, const void* h,
+                                      double rcond, void* f_aug, void* g_aug) {
+  if (!f || !g || !h || !f_aug || !g_aug) return TSDE_EINVAL;
+  const int64_t rows = L->rows, d = L->d, m = L->m;
+  if (!logqp_general_fits(d, m)) return TSDE_EINVAL;
+  if (rows > INT64_MAX / ((d + 1) * m)) return TSDE_EINVAL;   // element offsets of g_aug
+  const int n = (int)(d < m ? d : m);
+  const int pairs = (n + 1) / 2;
+  const int wpr = pairs < kLqWarps ? pairs : kLqWarps;
+  const size_t row_bytes = (size_t)lq_stride((int)d, (int)m) * sizeof(T);
+  // small rows share a CTA (up to kLqWarps warps, at most 48 KiB of shared memory); a large row has one to itself
+  int rpc = kLqWarps / wpr;
+  while (rpc > 1 && rpc * row_bytes > 48 * 1024) --rpc;
+  const int64_t blocks = (rows + rpc - 1) / rpc;
+  if (blocks > 0x7fffffffll) return TSDE_EINVAL;
+  const size_t smem = rpc * row_bytes + rpc * sizeof(int);
+  const int threads = rpc * wpr * 32;
+  auto kernel = logqp_augment_general_kernel<T>;
+  if (resident_ctas(reinterpret_cast<const void*>(kernel), threads, smem) == 0) return (int)cudaErrorInvalidConfiguration;
+  return launch_kernel(kernel, blocks, threads, smem, reinterpret_cast<cudaStream_t>(L->stream), false, rows, (int)d,
+                       (int)m, (const T*)f, (const T*)g, (const T*)h, (T)rcond, (T*)f_aug, (T*)g_aug, rpc, wpr);
+}
+
+}  // namespace tsde
+
 TSDE_EXPORT int tsde_logqp_augment(const tsde_launch* L, const void* f, const void* g, const void* h, double eps,
                                    void* f_aug, void* g_aug) {
   return tsde::dispatch(L, [&](auto t) {
+    if (L->noise_type == TSDE_NOISE_GENERAL)
+      return tsde::logqp_augment_general_impl<decltype(t)>(L, f, g, h, eps, f_aug, g_aug);
     return tsde::logqp_augment_impl<decltype(t)>(L, f, g, h, eps, f_aug, g_aug);
   });
 }
