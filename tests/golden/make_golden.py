@@ -292,22 +292,31 @@ def generic_adjoint_cases():
 
 
 def log_ode_cases():
-    """methods/log_ode.py with davie / foster Levy area (the recorder also logs A)."""
-    for i, (name, kind, d, m, levy) in enumerate((('general_foster', 'general', 4, 3, 'foster'),
-                                                  ('general_davie', 'general', 3, 4, 'davie'),
-                                                  ('gbm_foster', 'gbm', 5, 5, 'foster'),
-                                                  ('additive_davie', 'additive', 3, 2, 'davie'))):
+    """methods/log_ode.py with davie / foster Levy area (the recorder also logs A).  The general-noise cases at
+    m = 2, 5, 8, 16, 32 reach every route of the g.A product: B = 9 rows of d = 40 channels leave the last CTA of the
+    tile kernel partial (7 rows per CTA, 4 at m = 32 in fp64, where B = 5), m = 5 takes the generic kernel.  Their
+    problem (TanhMixedGeneral) has a Levy-area term that changes sign with A, so the solution depends on which way
+    round the product takes A.  Their time grid is exact in fp32, so the same increments replay an fp32 solve too."""
+    cases = [('general_foster', 'general', 4, 3, 'foster', 4, [0.0, 0.1, 0.2, 0.3], 0.05),
+             ('general_davie', 'general', 3, 4, 'davie', 4, [0.0, 0.1, 0.2, 0.3], 0.05),
+             ('gbm_foster', 'gbm', 5, 5, 'foster', 4, [0.0, 0.1, 0.2, 0.3], 0.05),
+             ('additive_davie', 'additive', 3, 2, 'davie', 4, [0.0, 0.1, 0.2, 0.3], 0.05)]
+    for m in (2, 5, 8, 16, 32):
+        for levy in ('davie', 'foster'):
+            cases.append((f'general_m{m}_{levy}', 'general_mixed', 40, m, levy, 5 if m == 32 else 9,
+                          [0.0, 0.125, 0.25], 0.125))
+    for i, (name, kind, d, m, levy, B, ts, dt) in enumerate(cases):
         torch.manual_seed(55 + i)
         tdt = torch.float64
         sde = problems.make(kind, d, m, 'stratonovich', dtype=tdt, seed=i)
-        B = 4
         y0 = (0.1 + 0.5 * torch.rand(B, d, dtype=tdt))
-        ts = torch.tensor([0.0, 0.1, 0.2, 0.3], dtype=tdt)
+        ts = torch.tensor(ts, dtype=tdt)
         bm_m = d if kind == 'gbm' else m
-        bm = torchsde.BrownianInterval(0.0, 0.3, size=(B, bm_m), dtype=tdt, entropy=300 + i, levy_area_approximation=levy)
+        bm = torchsde.BrownianInterval(float(ts[0]), float(ts[-1]), size=(B, bm_m), dtype=tdt, entropy=300 + i,
+                                       levy_area_approximation=levy)
         rec = Recorder(bm)
-        ys = torchsde.sdeint(sde, y0, ts, bm=rec, method='log_ode', dt=0.05)
-        save = dict(y0=y0.numpy(), ts=ts.numpy(), dt=np.float64(0.05), ys=ys.detach().numpy(), kind=kind, d=d, m=m,
+        ys = torchsde.sdeint(sde, y0, ts, bm=rec, method='log_ode', dt=dt)
+        save = dict(y0=y0.numpy(), ts=ts.numpy(), dt=np.float64(dt), ys=ys.detach().numpy(), kind=kind, d=d, m=m,
                     sde_type='stratonovich', method='log_ode', dtype='f64', seed=i, grad_free=False, levy=levy,
                     ta=np.array([r[0] for r in rec.log]), tb=np.array([r[1] for r in rec.log]),
                     W=np.stack([r[2] for r in rec.log]), U=np.stack([r[3] for r in rec.log]),

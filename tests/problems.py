@@ -125,6 +125,28 @@ class TanhGeneral(nn.Module):
         return torch.tanh(y).unsqueeze(-1) * self.S
 
 
+class TanhMixedGeneral(nn.Module):
+    """General noise whose columns see the state at different rates: g_il = tanh(c_l y_i) S_il, f = mu * y.  Unlike
+    TanhGeneral, sum_{k,l} dg_il/dy_i g_ik A_kl = sum_{k,l} c_l sech^2(c_l y_i) tanh(c_k y_i) S_il S_ik A_kl is not
+    symmetric in (k, l), so the log-ODE's Levy-area term does not vanish for an antisymmetric A and changes sign with
+    it: a step that takes A the wrong way round (g A^T = -g A) gives a different solution."""
+    noise_type = 'general'
+
+    def __init__(self, d, m, sde_type='ito', seed=0, dtype=torch.float64):
+        super().__init__()
+        self.sde_type = sde_type
+        g = _gen(seed)
+        self.S = nn.Parameter((0.5 * torch.rand(d, m, generator=g, dtype=torch.float64)).to(dtype))
+        self.mu = nn.Parameter((-torch.rand(d, generator=g, dtype=torch.float64)).to(dtype))
+        self.c = nn.Parameter((0.25 + 2.0 * torch.rand(m, generator=g, dtype=torch.float64)).to(dtype))
+
+    def f(self, t, y):
+        return self.mu * y
+
+    def g(self, t, y):
+        return torch.tanh(y.unsqueeze(-1) * self.c) * self.S
+
+
 class MLPDiagonal(nn.Module):
     """Architecture of the reference's NeuralDiagonal (tests/problems.py:135-162): the fixture SDE
     of diagnostics/ito_diagonal.py.  Weights are loaded from the golden file."""
@@ -226,7 +248,7 @@ class LatentPrior(nn.Module):
 
 
 PROBLEMS = {'gbm': GBMDiagonal, 'scalar': CosScalar, 'additive': TimeAdditive, 'general': TanhGeneral,
-            'additive_expand': TimeAdditiveExpand}
+            'additive_expand': TimeAdditiveExpand, 'general_mixed': TanhMixedGeneral}
 
 
 def make(kind, d, m, sde_type, dtype=torch.float64, seed=0):

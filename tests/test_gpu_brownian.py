@@ -326,24 +326,6 @@ def test_levy_area_noise_law(levy, m):
         assert float(off.abs().max()) < 0.03
 
 
-@pytest.mark.parametrize('dtype', [torch.float32, torch.float64])
-@pytest.mark.parametrize('B,d,m', [(8192, 32, 16), (257, 5, 3), (64, 7, 8), (33, 4, 2), (100, 40, 32), (50, 6, 5), (3, 2, 20)])
-def test_bmm_ga_kernel_vs_torch(dtype, B, d, m):
-    """tsde_bmm_ga (log-ODE: ga = bmm(g, A), base_sde.py:170,191) against torch.bmm; the kernel writes the product
-    transposed, (m, rows, d)."""
-    import ctypes
-    from torchsde_b200 import _cabi
-    g = torch.randn(B, d, m, dtype=dtype, device=DEV)
-    a = torch.randn(B, m, m, dtype=dtype, device=DEV)
-    a = a - a.transpose(1, 2)
-    out = torch.empty(m, B, d, dtype=dtype, device=DEV)
-    L = _cabi.make_launch(dtype, _cabi.NOISE_GENERAL, B, d, m)
-    _cabi.check(_cabi.lib().tsde_bmm_ga(ctypes.byref(L), g.data_ptr(), a.data_ptr(), out.data_ptr()), 'tsde_bmm_ga')
-    ref = torch.bmm(g.double(), a.double()).permute(2, 0, 1)
-    tol = dict(rtol=1e-5, atol=1e-5) if dtype == torch.float32 else dict(rtol=1e-12, atol=1e-12)
-    torch.testing.assert_close(out.double(), ref, **tol)
-
-
 @pytest.mark.parametrize('levy', ['davie', 'foster'])
 @pytest.mark.parametrize('dtype', [torch.float32, torch.float64])
 @pytest.mark.parametrize('size', [(257, 8), (1030, 16), (77, 4), (45, 32), (19, 12), (5, 64)])

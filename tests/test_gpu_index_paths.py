@@ -79,16 +79,52 @@ NOISE_OPS = [
     ('tsde_brownian_cells', 0, 1, False, (), lambda x, w, u: [w]),
     ('tsde_brownian_cells', 0, 2, True, (), lambda x, w, u: [w, u]),
 ]
-# element-wise entry points without noise (the generic / fast comparison only)
+# element-wise entry points without noise: milstein.py:63 (ito, then Stratonovich), the SRK stage values H0_1 / H1_1
+# and H1_3 (srk.py:70-76), and linear_interp as output times and log-ODE (weights 1, 1) use it
 PLAIN_OPS = [
-    ('tsde_milstein_gf_predict', 3, 1, False, (DT, SQ, 1), None),
-    ('tsde_srk_diag_stage1', 3, 2, False, (DT, SQ), None),
-    ('tsde_srk_diag_stage3', 5, 1, False, (DT, SQ), None),
-    ('tsde_linear_interp', 2, 1, False, (0.3, 0.7), None),
+    ('tsde_milstein_gf_predict', 3, 1, False, (DT, SQ, 1), lambda x, w, u: [x[0] + DT * x[1] + x[2] * SQ]),
+    ('tsde_milstein_gf_predict', 3, 1, False, (DT, SQ, 0), lambda x, w, u: [x[0] + x[2] * SQ]),
+    ('tsde_srk_diag_stage1', 3, 2, False, (DT, SQ),
+     lambda x, w, u: [x[0] + x[1] * DT, x[0] + 0.25 * x[1] * DT - 0.5 * x[2] * SQ]),
+    ('tsde_srk_diag_stage3', 5, 1, False, (DT, SQ),
+     lambda x, w, u: [x[0] + (2 * x[1] - x[2] + 0.5 * x[4]) * SQ + 0.25 * x[3] * DT]),
+    ('tsde_linear_interp', 2, 1, False, (0.3, 0.7), lambda x, w, u: [0.3 * x[0] + 0.7 * x[1]]),
+    ('tsde_linear_interp', 2, 1, False, (1.0, 1.0), lambda x, w, u: [x[0] + x[1]]),
 ]
 
 
+def plain_emulated(op, x):
+    """The outputs of noise-free op `op` on numpy inputs x in T, in the op's written order (tableau_diag.cu: one IEEE
+    rounding per operation, no fma under -fmad=false); the double scalars are cast to T."""
+    name, nin, _, _, scalars, _ = op
+    T = x[0].dtype.type
+    s = [T(v) for v in scalars]
+    if name == 'tsde_milstein_gf_predict':
+        y0, f, g = x[:3]
+        fac = s[0] * f if scalars[2] else np.zeros_like(f)
+        return [(y0 + fac) + g * s[1]]
+    if name == 'tsde_srk_diag_stage1':
+        y0, f0, g0 = x[:3]
+        return [y0 + (T(1) * f0) * s[0], (y0 + (T(0.25) * f0) * s[0]) + (T(-0.5) * g0) * s[1]]
+    if name == 'tsde_srk_diag_stage3':
+        y0, g0, g1, f2, g2 = x[:5]
+        h1 = y0 + (T(2) * g0) * s[1]
+        h1 = h1 + (T(-1) * g1) * s[1]
+        return [(h1 + (T(0.25) * f2) * s[0]) + (T(0.5) * g2) * s[1]]
+    assert name == 'tsde_linear_interp'
+    return [s[0] * x[0] + s[1] * x[1]]
+
+
+def tol_of(npdt):
+    """The formula checks' tolerance."""
+    return dict(rtol=5e-5, atol=1e-5) if npdt == np.float32 else dict(rtol=1e-11, atol=1e-12)
+
+
 def _op_id(op):
+    if op[0] == 'tsde_milstein_gf_predict' and not op[4][2]:
+        return 'milstein_gf_predict_strat'
+    if op[0] == 'tsde_linear_interp':
+        return 'linear_interp_%g_%g' % op[4]
     return op[0][5:] + ('_wu' if op[0] == 'tsde_brownian_cells' and op[2] == 2 else '')
 
 
@@ -147,7 +183,7 @@ def test_rows_past_2_24(d, dtype):
     if _free_memory() < 1.1 * need + (1 << 30):
         pytest.skip(f'needs ~{need / 2 ** 30:.0f} GiB of free device memory')
     npdt = np.float32 if dtype == torch.float32 else np.float64
-    tol = dict(rtol=5e-5, atol=1e-5) if dtype == torch.float32 else dict(rtol=1e-11, atol=1e-12)
+    tol = tol_of(npdt)
     gen = torch.Generator(device=DEV).manual_seed(d)
     pool = [torch.rand(B, d, generator=gen, device=DEV, dtype=dtype) + 0.5 for _ in range(3)]
     pool_u = []  # the same values one element past a 16-byte boundary
@@ -163,7 +199,7 @@ def test_rows_past_2_24(d, dtype):
     rows_dev = torch.from_numpy(rows).to(DEV)
     x_rows = [x[rows_dev].double().cpu().numpy() for x in pool]
     bad = []
-    for op in NOISE_OPS:
+    for op in NOISE_OPS + PLAIN_OPS:
         name, nin, nout, want_u, _, formula = op
         _launch(op, dtype, B, d, _ins(pool, nin), [o.data_ptr() for o in out_a], _noise(key, want_u))
         # the same work as two launches split at local row 2^24
@@ -176,9 +212,12 @@ def test_rows_past_2_24(d, dtype):
                 first = int((out_a[i].view(-1) != out_b[i][:n]).nonzero()[0]) // d
                 bad.append(f'{_op_id(op)} out{i}: one launch != split at 2^24 (first differing row {first})')
         # float64 formula on the oracle's increments, sampled rows
-        W, Hh = obm.cell(KEY, CELL, H, len(rows), d, npdt, want_u, row_ids=rows)
-        U = obm.h_to_u(W, Hh, H).astype(np.float64) if want_u else None
-        ref = formula([x_rows[i % 3] for i in range(nin)], W.astype(np.float64), U)
+        W = U = None
+        if op in NOISE_OPS:
+            W, Hh = obm.cell(KEY, CELL, H, len(rows), d, npdt, want_u, row_ids=rows)
+            U = obm.h_to_u(W, Hh, H).astype(np.float64) if want_u else None
+            W = W.astype(np.float64)
+        ref = formula([x_rows[i % 3] for i in range(nin)], W, U)
         for i in range(nout):
             got = out_a[i][rows_dev].double().cpu().numpy()
             if not np.allclose(got, ref[i], **tol):
@@ -250,11 +289,12 @@ def test_generic_kernel_equals_fast_kernel(d, dtype):
     """Operands one element off 16-byte alignment take the generic kernel (ew_kernel); aligned ones take the fast
     kernel (ew_fast_kernel).  Every diagonal entry point, with counter and with memory noise, must give the same bits
     either way.  Batch sizes cover one partial CTA, and full grids whose per-CTA slices end in a partial iteration of
-    the two-quads-per-thread ops."""
+    the two-quads-per-thread ops.  The noise-free ops must also give the bits of a numpy emulation of their written
+    order in T."""
     es = torch.finfo(dtype).bits // 8
     key = torch.tensor([KEY], dtype=torch.int64, device=DEV)
     gen = torch.Generator(device=DEV).manual_seed(d)
-    bad = []
+    bad, host = [], None
     for B in (1, 37, 1000, 300007):
         n = B * d
         pool_u = [torch.rand(n + 1, generator=gen, device=DEV, dtype=dtype) + 0.5 for _ in range(5)]
@@ -273,8 +313,14 @@ def test_generic_kernel_equals_fast_kernel(d, dtype):
                 _launch(op, dtype, B, d, _ins(pool_u, op[1], es), [o.data_ptr() + es for o in out_b], nz_b)
                 for i in range(op[2]):
                     if not torch.equal(out_a[i], out_b[i][1:]):
-                        bad.append(f'B={B} {_op_id(op)} {src} out{i}')
-    assert not bad, 'fast kernel != generic kernel: ' + ', '.join(bad)
+                        bad.append(f'B={B} {_op_id(op)} {src} out{i}: fast kernel != generic kernel')
+                if op in PLAIN_OPS:
+                    host = host or [x.cpu().numpy() for x in pool]
+                    for i, e in enumerate(plain_emulated(op, host[:op[1]])):
+                        if not np.array_equal(out_a[i].cpu().numpy().view(np.uint8), e.view(np.uint8)):
+                            bad.append(f'B={B} {_op_id(op)} out{i}: not the numpy emulation\'s bits')
+        host = None
+    assert not bad, ', '.join(bad)
 
 
 # ---- (e) adaptive-step error reduction -----------------------------------------------------------------------------
