@@ -127,6 +127,7 @@ const char* tsde_error_string(int code);
    check which general-noise tile kernel a shape was routed to). */
 #define TSDE_KERNEL_GEN_CTA 0  /* per-thread-load tile kernel                       */
 #define TSDE_KERNEL_GEN_TMA 1  /* TMA-staged persistent tile kernel (bulk copies)   */
+#define TSDE_KERNEL_GEN_WIDE 2 /* chunked tile kernel for rows whose increments exceed shared memory */
 int64_t tsde_kernel_launches(int32_t family);
 
 /* ------------------------------------------------------------------------ */
@@ -220,6 +221,9 @@ int tsde_brownian_merge_area(const tsde_launch* L, void* a0, const void* a1,
 /* ------------------------------------------------------------------------ */
 /* Step tableaus  (replace torchsde/_core/methods/<name>.py  .step bodies)        */
 /* `g*` arguments are (rows,d) for DIAGONAL and (rows,d,m) for GENERAL.      */
+/* GENERAL accepts any d and any m the Brownian source accepts (counter     */
+/* noise: m <= 2^26), whether or not one row's increments fit in shared     */
+/* memory.                                                                  */
 /* ------------------------------------------------------------------------ */
 
 /* y1 = y0 + f*dt + g.dW                    methods/euler.py:36

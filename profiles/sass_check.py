@@ -21,6 +21,8 @@ PICK = [  # (label, regex on the demangled kernel name)
     ('general Heun tile, per-thread loads, fp32', r'gen_cta_kernel<float, tsde::GHeunOp<float>, 1>'),
     ('general Euler tile, TMA-staged, fp32, m=16', r'gen_tma_kernel<float, tsde::GEulerOp<float>, 1, 2>'),
     ('general Heun tile, TMA-staged, fp32, m=64', r'gen_tma_kernel<float, tsde::GHeunOp<float>, 1, 4>'),
+    ('general Euler tile, wide rows (m in chunks), fp32', r'gen_wide_kernel<float, tsde::GEulerOp<float>, 1>'),
+    ('general SRK-additive final tile, wide rows, fp64', r'gen_wide_kernel<double, tsde::GSraFinalOp<double>, 1>'),
     ('Brownian cells W (materialised queries), fp32', r'ew_fast_kernel<float, tsde::CellsOp<float, false>, 1>|ew_fast_kernel<float, tsde::CellsOp<float>, 1>'),
     ('Brownian bridge', r'bridge_kernel<float'),
     ('Levy area (Davie / Foster), fp32, m = 16: one normal per pair, pair arithmetic two at a time', r'levy_tile_kernel<float, false, 16>|levy_tile_kernel<float, \(bool\)0, 16>'),

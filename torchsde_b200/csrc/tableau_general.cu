@@ -21,7 +21,7 @@ namespace tsde {
 
 constexpr int kMaxRowsPerBlock = 64;
 
-static std::atomic<int64_t> g_launches[2];  // TSDE_KERNEL_GEN_CTA, TSDE_KERNEL_GEN_TMA
+static std::atomic<int64_t> g_launches[3];  // TSDE_KERNEL_GEN_CTA, TSDE_KERNEL_GEN_TMA, TSDE_KERNEL_GEN_WIDE
 
 template <int NE, int NG, int NO>
 struct GenP {
@@ -688,6 +688,159 @@ static int launch_gen_tma(const tsde_launch* L, const tsde_noise* nz, GenP<Op::N
   return mem ? go(gen_tma_kernel<T, Op, TSDE_SRC_MEMORY, 4>) : go(gen_tma_kernel<T, Op, TSDE_SRC_COUNTER, 4>);  // m = 64
 }
 
+// ---- wide rows: one row's increments do not fit in shared memory ---------------------------------------------------
+// Taken exactly where `gen_kernel` cannot stage even one row (m * s * (WANT_U ? 2 : 1) > 40 KiB), for any m the
+// Brownian source accepts.  One CTA per row walks m in chunks of kWideChunkBytes: the threads produce the chunk's
+// increments (one Philox quad per thread and pass, on the channel-quad counters of every other kernel, or a coalesced
+// load of the user's W / U) into shared memory once, then each warp takes whole (row, d) outputs and streams their g
+// run over the chunk, lanes along the contiguous m axis: quad q of the chunk is lane q % 32's, one 128-bit load per
+// operand when g is aligned and m % 4 == 0, else four scalar loads of the same quad.  The running sums of up to
+// kWideOutputs outputs stay in shared memory across the chunks; a row with a larger d is walked once per block of
+// kWideOutputs outputs, drawing its increments again each time (one extra draw per kWideOutputs g runs).
+//
+// Summation order, per output and product: a lane sums its quads in increasing order, each quad's four channels left
+// to right with fused multiply-adds; the 32 lane sums of a chunk are combined by the xor-tree (offsets 16, 8, 4, 2, 1)
+// and the chunk sums are added left to right.  It depends on m alone: the same bits for aligned and unaligned
+// operands, for any batch size and for any split of the batch by row_offset.
+constexpr int kWideThreads = 256;
+constexpr int kWideLoads = 4;               // g quads per lane in flight (over all g operands)
+constexpr int kWideChunkBytes = 8 * 1024;   // one chunk of W (and one of U) in shared memory
+constexpr int kWideOutputs = 1024;          // outputs per block: their running sums stay in shared memory
+
+template <typename T, typename Op, int SRC>
+__global__ void __launch_bounds__(kWideThreads, 1)
+gen_wide_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const Op op) {
+  constexpr int NE = Op::NE, NG = Op::NG, NP = Op::NP, NO = Op::NO;
+  constexpr int CW = kWideChunkBytes / (int)sizeof(T);  // channels per chunk, a multiple of 4 * 32
+  constexpr int UN = kWideLoads / NG;                    // quads per lane and pass
+  constexpr int kWarps = kWideThreads / 32;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  T* sw = reinterpret_cast<T*>(smem_raw);
+  T* su = sw + CW;
+  T* tot = sw + (Op::WANT_U ? 2 : 1) * CW;  // [NP][outputs of the block]
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int64_t row = blockIdx.x, m = p.m, d = p.d;
+  const bool vec = p.vec != 0;
+  Key key{0u, 0u};
+  if (SRC != TSDE_SRC_MEMORY) key = load_key(nz.key);
+  const uint32_t grow = (uint32_t)(row + nz.row_offset);
+  const int64_t slot_g = p.gbcast ? 0 : row * d;  // first (d, m) run of this row's g
+  for (int64_t d0 = 0; d0 < d; d0 += kWideOutputs) {
+    const int nout = (int)(d - d0 < kWideOutputs ? d - d0 : kWideOutputs);
+    for (int64_t c0 = 0; c0 < m; c0 += CW) {
+      const int len = (int)(m - c0 < CW ? m - c0 : CW);
+      const int nq = (len + 3) / 4;
+      __syncthreads();  // the previous chunk's increments have been read
+      if (SRC != TSDE_SRC_MEMORY) {
+        for (int q = tid; q < nq; q += kWideThreads) {
+          T w[4], u[4];
+          counter_noise<T, Op::WANT_U, SRC == kSrcCounterMulti>(nz, key, grow, (uint32_t)(c0 / 4 + q), w, u);
+          st4(sw + 4 * q, w);
+          if (Op::WANT_U) st4(su + 4 * q, u);
+        }
+      } else {
+        const int64_t base = row * m + c0;
+        for (int i = tid; i < len; i += kWideThreads) {
+          sw[i] = nz.w[base + i];
+          if (Op::WANT_U) su[i] = nz.u[base + i];
+        }
+      }
+      __syncthreads();
+      for (int j = warp; j < nout; j += kWarps) {
+        const int64_t goff = (slot_g + d0 + j) * m + c0;
+        T part[NP];
+#pragma unroll
+        for (int k = 0; k < NP; ++k) part[k] = T(0);
+        for (int b = 0; b < nq; b += 32 * UN) {
+          T gv[UN][NG][4];
+          uint4 graw[UN][NG];  // (Mixed: every g load of the pass issued before the first widening)
+#pragma unroll
+          for (int un = 0; un < UN; ++un) {
+            const int q = b + 32 * un + lane;
+            const int nv = len - 4 * q;  // valid channels of the quad (<= 0: past the chunk)
+#pragma unroll
+            for (int i = 0; i < NG; ++i) {
+              if constexpr (is_mixed<Op>::value) {
+                const uint32_t f = operand_fmt(op.fmt, NE + i);
+                if (q >= nq) graw[un][i] = make_uint4(0u, 0u, 0u, 0u);
+                else if (vec && streams_inputs<Op>::value && !p.gbcast) graw[un][i] = ld4raw<true>(p.g[i], goff + 4 * q, f);
+                else if (vec) graw[un][i] = ld4raw<false>(p.g[i], goff + 4 * q, f);
+                else graw[un][i] = load_quad_raw(p.g[i], goff + 4 * q, false, nv, f);
+              } else {
+                const T* g = reinterpret_cast<const T*>(p.g[i]);
+                if (q >= nq) {
+#pragma unroll
+                  for (int jj = 0; jj < 4; ++jj) gv[un][i][jj] = T(0);
+                } else if (vec && streams_inputs<Op>::value && !p.gbcast) {
+                  ld4cs(g + goff + 4 * q, gv[un][i]);
+                } else {
+                  load_quad(g, goff + 4 * q, vec, nv, gv[un][i]);
+                }
+              }
+            }
+          }
+          if constexpr (is_mixed<Op>::value) {
+#pragma unroll
+            for (int un = 0; un < UN; ++un) {
+#pragma unroll
+              for (int i = 0; i < NG; ++i) widen_quad(graw[un][i], vec, operand_fmt(op.fmt, NE + i), gv[un][i]);
+            }
+          }
+#pragma unroll
+          for (int un = 0; un < UN; ++un) {
+            const int q = b + 32 * un + lane;
+            if (q < nq) {
+              const int nv = len - 4 * q;
+              T w4[4], u4[4];
+              ld4(sw + 4 * q, w4);
+              if (Op::WANT_U) ld4(su + 4 * q, u4);
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) {
+                if (jj < nv) {
+                  T gj[NG];
+#pragma unroll
+                  for (int i = 0; i < NG; ++i) gj[i] = gv[un][i][jj];
+#pragma unroll
+                  for (int k = 0; k < NP; ++k)
+                    part[k] = fma(op.gval(k, gj), op.weight(k, w4[jj], Op::WANT_U ? u4[jj] : T(0)), part[k]);
+                }
+              }
+            }
+          }
+        }
+#pragma unroll
+        for (int off = 16; off >= 1; off >>= 1) {
+#pragma unroll
+          for (int k = 0; k < NP; ++k) part[k] = part[k] + __shfl_xor_sync(0xffffffffu, part[k], off);
+        }
+        if (lane == 0) {
+#pragma unroll
+          for (int k = 0; k < NP; ++k) tot[k * nout + j] = c0 == 0 ? part[k] : tot[k * nout + j] + part[k];
+        }
+      }
+    }
+    __syncthreads();  // the block's sums are complete
+    for (int j = tid; j < nout; j += kWideThreads) {
+      const int64_t eoff = row * d + d0 + j;
+      T e[NE > 0 ? NE : 1], gp[NP], o[NO];
+#pragma unroll
+      for (int i = 0; i < NE; ++i) {
+        if constexpr (is_mixed<Op>::value) e[i] = __uint_as_float(ld1raw(p.e[i], eoff, operand_fmt(op.fmt, i)));
+        else e[i] = reinterpret_cast<const T*>(p.e[i])[eoff];
+      }
+      if constexpr (is_mixed<Op>::value) {
+#pragma unroll
+        for (int i = 0; i < NE; ++i) e[i] = widen1(__float_as_uint(e[i]), operand_fmt(op.fmt, i));
+      }
+#pragma unroll
+      for (int k = 0; k < NP; ++k) gp[k] = tot[k * nout + j];
+      op.combine(e, gp, o);
+#pragma unroll
+      for (int i = 0; i < NO; ++i) reinterpret_cast<T*>(p.o[i])[eoff] = o[i];
+    }
+  }
+}
+
 template <typename T, typename Op>
 static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
                       std::initializer_list<const void*> es, std::initializer_list<const void*> gs,
@@ -707,6 +860,7 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
     vec = vec && aligned_for(q, operand_fmt(fmt, Op::NE + i));
     p.g[i++] = q;
   }
+  const bool gvec = vec;  // m % 4 == 0 and every g aligned for quad loads (gen_wide_kernel)
   i = 0;
   for (void* q : os) { if (!q) return TSDE_EINVAL; p.o[i++] = q; }
   NoiseP<T> np;
@@ -745,7 +899,18 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
   if (rb > kMaxRowsPerBlock) rb = kMaxRowsPerBlock;
   const int64_t smem_per_row = L->m * (int64_t)sizeof(T) * (Op::WANT_U ? 2 : 1);
   while (rb > 1 && rb * smem_per_row > 40 * 1024) rb >>= 1;
-  if (rb * smem_per_row > 40 * 1024) return TSDE_EINVAL;  // m too large for one row in smem
+  if (rb * smem_per_row > 40 * 1024) {  // not even one row's increments fit: walk m in chunks, one CTA per row
+    if (L->rows > 0x7fffffffll) return TSDE_EINVAL;
+    p.vec = gvec ? 1 : 0;
+    p.rb = 1;
+    const int64_t outs = L->d < kWideOutputs ? L->d : kWideOutputs;
+    const size_t smem = ((Op::WANT_U ? 2 : 1) * (size_t)(kWideChunkBytes / sizeof(T)) + Op::NP * (size_t)outs) * sizeof(T);
+    g_launches[TSDE_KERNEL_GEN_WIDE].fetch_add(1, std::memory_order_relaxed);
+    const auto kernel = mem                ? gen_wide_kernel<T, Op, TSDE_SRC_MEMORY>
+                        : np.n_cells > 1 ? gen_wide_kernel<T, Op, kSrcCounterMulti>
+                                         : gen_wide_kernel<T, Op, TSDE_SRC_COUNTER>;
+    return launch_kernel(kernel, L->rows, kWideThreads, smem, st, false, p, np, op);
+  }
   // keep every SM busy on small batches
   while (rb > 1 && (L->rows + rb - 1) / rb < 2 * sm_count()) rb >>= 1;
   p.rb = (int32_t)rb;
@@ -1097,6 +1262,6 @@ TSDE_EXPORT int tsde_step_srk_additive(const tsde_launch* L, const tsde_noise* n
 }
 
 TSDE_EXPORT int64_t tsde_kernel_launches(int32_t family) {
-  if (family < 0 || family > 1) return -1;
+  if (family < 0 || family > 2) return -1;
   return g_launches[family].load(std::memory_order_relaxed);
 }
