@@ -128,6 +128,7 @@ const char* tsde_error_string(int code);
 #define TSDE_KERNEL_GEN_CTA 0  /* per-thread-load tile kernel                       */
 #define TSDE_KERNEL_GEN_TMA 1  /* TMA-staged persistent tile kernel (bulk copies)   */
 #define TSDE_KERNEL_GEN_WIDE 2 /* chunked tile kernel for rows whose increments exceed shared memory */
+#define TSDE_KERNEL_PW_MILSTEIN 3 /* whole Milstein step with an element-wise SDE (tsde_step_milstein_pointwise) */
 int64_t tsde_kernel_launches(int32_t family);
 
 /* ------------------------------------------------------------------------ */
@@ -241,6 +242,53 @@ int tsde_milstein_vjp_seed(const tsde_launch* L, const tsde_noise* nz, const voi
 /* y1 = y0 + f*dt + g.dW + gdg              methods/milstein.py:72 */
 int tsde_step_milstein(const tsde_launch* L, const tsde_noise* nz, const void* y0,
                        const void* f, const void* g, const void* gdg, double dt, void* y1);
+
+/*
+ * A whole diagonal-noise Milstein step (milstein.py:68-72) for an SDE whose f(t, y), g(t, y) and the vjp of g
+ * are element-wise programs: one launch reads y0, draws dW, evaluates
+ *     f, g (program), go = g * (0.5 * v) (as tsde_milstein_vjp_seed), gdg = vjp(go) (program),
+ *     y1 = ((y0 + f*dt) + g*dW) + gdg (as tsde_step_milstein)
+ * in registers and writes y1.  The program restates ATen ops one IEEE rounding each, in the order they ran, so
+ * the step equals the unfused one bit for bit.
+ *
+ * Program: `n_instr` instructions; [0, n_fg) compute f and g, [n_fg, n_instr) the vjp.  An instruction writes
+ * register `dst` (< n_regs <= TSDE_PW_MAX_REGS) from sources `a`, `b` (b unused by NEG / SQRT).  A source is a
+ * register, TSDE_PW_SRC_Y (y0), TSDE_PW_SRC_GO (the seed go, vjp part only) or TSDE_PW_OPERAND(k).  f_src,
+ * g_src (read after n_fg instructions) and gdg_src (read at the end) name the three results.  Operands:
+ *   IMM      value `imm` (a value of the state dtype, stored as double)
+ *   T0       the 0-d step time `t0` of the call (state dtype)
+ *   SCALAR   ptr[0]                 (a one-element device tensor)
+ *   CHANNEL  ptr[channel]           (a (d,) tensor broadcast over the rows)
+ *   ROW      ptr[row * d + channel] (a (rows, d) tensor)
+ * Device operands are read at every launch, after the kernel's dependency wait.  The struct is passed by value
+ * to the kernel (it fits the 4 KiB parameter space), so a captured launch carries it.
+ * Requires DIAGONAL noise, counter noise (nz->source == TSDE_SRC_COUNTER) and no 16-bit formats.
+ */
+#define TSDE_PW_MAX_INSTR 96
+#define TSDE_PW_MAX_OPERANDS 24
+#define TSDE_PW_MAX_REGS 24
+#define TSDE_PW_SRC_Y 0xFE
+#define TSDE_PW_SRC_GO 0xFF
+#define TSDE_PW_OPERAND(k) (0x80 + (k))
+enum { TSDE_PW_MUL = 0, TSDE_PW_ADD = 1, TSDE_PW_SUB = 2, TSDE_PW_DIV = 3, TSDE_PW_NEG = 4, TSDE_PW_SQRT = 5 };
+enum { TSDE_PW_IMM = 0, TSDE_PW_T0 = 1, TSDE_PW_SCALAR = 2, TSDE_PW_CHANNEL = 3, TSDE_PW_ROW = 4 };
+typedef struct tsde_pw_instr {
+  uint8_t op, dst, a, b;
+} tsde_pw_instr;
+typedef struct tsde_pw_operand {
+  int32_t kind;
+  int32_t reserved;
+  const void* ptr;
+  double imm;
+} tsde_pw_operand;
+typedef struct tsde_pointwise {
+  int32_t n_instr, n_fg, n_regs, n_operands;
+  uint8_t f_src, g_src, gdg_src, reserved;
+  tsde_pw_instr instr[TSDE_PW_MAX_INSTR];
+  tsde_pw_operand operand[TSDE_PW_MAX_OPERANDS];
+} tsde_pointwise;
+int tsde_step_milstein_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                 const void* y0, const void* t0, double dt, int32_t ito, void* y1);
 
 /* derivative-free Milstein, predictor: y' = y0 + (Ito ? dt*f : 0) + g*sqrt_dt
  * methods/milstein.py:58-63,83-84,93-94.  g is (rows,d) also for scalar noise (squeezed). */

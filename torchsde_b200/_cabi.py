@@ -46,6 +46,29 @@ class Noise(ctypes.Structure):
                 ('h', ctypes.c_double), ('cell_h', ctypes.c_void_p), ('h_total', ctypes.c_double)]
 
 
+PW_MAX_INSTR, PW_MAX_OPERANDS, PW_MAX_REGS = 96, 24, 24  # TSDE_PW_MAX_*
+PW_SRC_Y, PW_SRC_GO, PW_OPERAND0 = 0xFE, 0xFF, 0x80
+PW_MUL, PW_ADD, PW_SUB, PW_DIV, PW_NEG, PW_SQRT = range(6)
+PW_IMM, PW_T0, PW_SCALAR, PW_CHANNEL, PW_ROW = range(5)
+KERNEL_PW_MILSTEIN = 3  # TSDE_KERNEL_PW_MILSTEIN
+
+
+class PwInstr(ctypes.Structure):
+    _fields_ = [('op', ctypes.c_uint8), ('dst', ctypes.c_uint8), ('a', ctypes.c_uint8), ('b', ctypes.c_uint8)]
+
+
+class PwOperand(ctypes.Structure):
+    _fields_ = [('kind', ctypes.c_int32), ('reserved', ctypes.c_int32), ('ptr', ctypes.c_void_p),
+                ('imm', ctypes.c_double)]
+
+
+class Pointwise(ctypes.Structure):
+    _fields_ = [('n_instr', ctypes.c_int32), ('n_fg', ctypes.c_int32), ('n_regs', ctypes.c_int32),
+                ('n_operands', ctypes.c_int32), ('f_src', ctypes.c_uint8), ('g_src', ctypes.c_uint8),
+                ('gdg_src', ctypes.c_uint8), ('reserved', ctypes.c_uint8),
+                ('instr', PwInstr * PW_MAX_INSTR), ('operand', PwOperand * PW_MAX_OPERANDS)]
+
+
 _P = ctypes.c_void_p
 _D = ctypes.c_double
 _I = ctypes.c_int32
@@ -67,6 +90,7 @@ SIGNATURES = {
     'tsde_step_euler': [_L, _N, _P, _P, _P, _D, _P],
     'tsde_milstein_vjp_seed': [_L, _N, _P, _D, _I, _P],
     'tsde_step_milstein': [_L, _N, _P, _P, _P, _P, _D, _P],
+    'tsde_step_milstein_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _D, _I, _P],
     'tsde_milstein_gf_predict': [_L, _P, _P, _P, _D, _D, _I, _P],
     'tsde_step_milstein_gf': [_L, _N, _P, _P, _P, _P, _D, _D, _I, _P],
     'tsde_step_heun': [_L, _N, _P, _P, _P, _P, _P, _D, _P],

@@ -8,10 +8,13 @@ reference's ``step`` by one or two launches through the C ABI (include/torchsde_
 ``self._k(name, L, nz, inputs, scalars, outputs)`` (base_solver.py) — a direct launch on the fast path,
 an autograd node when gradients must flow through the solve.
 """
+import ctypes
+
 import numpy as np
 import torch
 
 from . import base_solver
+from . import pointwise
 from .base_sde import widen
 from .base_solver import _contig, _gop
 from .. import _cabi
@@ -110,6 +113,7 @@ class BaseMilstein(_ProdMixin, base_solver.BaseSDESolver):
                                  f"`adjoint_options=dict({METHOD_OPTIONS.grad_free}=False)`")
         super(BaseMilstein, self).__init__(sde=sde, options=options, **kwargs)
         self._ones = None
+        self._pw = None  # the element-wise program of the step (pointwise.py), False once rejected
 
     def scalars(self, dt):
         sqrt_dt = _ieee_sqrt(dt)
@@ -146,23 +150,42 @@ class BaseMilstein(_ProdMixin, base_solver.BaseSDESolver):
             return self._k('tsde_step_euler', L, nz, (y0, f, g), (c.dt,), out), ()
         # g_prod_and_gdg_prod_{diagonal,default}: vjp of g wrt y with grad_outputs g * (0.5 v)
         # base_sde.py:127-155 (always calls self.g, never g_prod)
+        if self._pw and self._feed.binding is not None:
+            # f, g and the vjp were recorded as an element-wise program (pointwise.py): the whole step is one kernel
+            prog, _ = self._pw
+            out = out if out is not None else torch.empty_like(y0)
+            _cabi.check(self._lib.tsde_step_milstein_pointwise(self._L, self._feed.get(c), ctypes.byref(prog),
+                                                               y0.data_ptr(), c.t0.data_ptr(), c.dt, ito,
+                                                               out.data_ptr()), 'tsde_step_milstein_pointwise')
+            return out, ()
         track = self._autograd
+        # the first step of an eligible solve runs as always, with the user's ops recorded
+        rec = None
+        if self._pw is None and sde.noise_type == NOISE_TYPES.diagonal and pointwise.eligible(self):
+            rec = pointwise.Recorder(y0, c.t0)
+        raw = {}
+
+        def user(name, fn, **kw):
+            raw[name] = rec.segment(fn, **kw) if rec is not None else fn()
+            return raw[name]
 
         def diffusion_chain():
             with torch.enable_grad():
                 y = y0 if (track and y0.requires_grad) else y0.detach().requires_grad_(True)
-                g = sde.g(c.t0, y)
+                g = user('g', lambda: sde.g(c.t0, y), y=y)
                 gd = _contig(g if track else g.detach())
                 go = self._k('tsde_milstein_vjp_seed', self._L, self._feed.get(c), (gd,), (c.dt, ito), None)
                 if g.requires_grad:
-                    gdg, = torch.autograd.grad(g, y, grad_outputs=go.view_as(g), allow_unused=True,
-                                               retain_graph=track, create_graph=track)
+                    gdg, = user('gdg', lambda: torch.autograd.grad(g, y, grad_outputs=go.view_as(g), allow_unused=True,
+                                                                   retain_graph=track, create_graph=track), go=go)
                 else:
                     gdg = None
             return gd, (torch.zeros_like(y0) if gdg is None else _contig(gdg))
 
         # f and the chain g -> seed -> vjp are independent given y0 (reference order: f first, milstein.py:68)
-        f, (gd, gdg) = self._fork(lambda: _contig(sde.f(c.t0, y0)), diffusion_chain, main=1)
+        f, (gd, gdg) = self._fork(lambda: _contig(user('f', lambda: sde.f(c.t0, y0))), diffusion_chain, main=1)
+        if rec is not None:
+            self._pw = rec.finish(raw['f'], raw['g'], raw.get('gdg', (None,))[0]) or False
         return self._k('tsde_step_milstein', self._L, self._feed.get(c), (y0, f, gd, gdg), (c.dt,), out), ()
 
 

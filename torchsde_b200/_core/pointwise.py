@@ -1,0 +1,338 @@
+"""Element-wise tapes of the user's SDE: a diagonal-noise Milstein step as one kernel.
+
+The unfused step runs five full-batch passes: the user's f and g, the vjp seed, autograd's vjp of g and the tableau
+(methods.BaseMilstein._step).  When f(t, y), g(t, y) and the vjp of g are made only of element-wise ATen ops whose
+CUDA result is one IEEE rounding per element, the whole step is one launch of tsde_step_milstein_pointwise, which
+reads y0 and writes y1 (include/torchsde_b200.h).
+
+How the program is obtained: one step runs the ordinary way under `Recorder`, a TorchDispatchMode that sees every
+ATen op that actually runs in three segments: f(t0, y), g(t0, y) and torch.autograd.grad(g, y, go).  The vjp is not
+derived symbolically: autograd's own op sequence (`grad * other`, the `add` that accumulates a twice-used `y`, ...)
+is what decides the bits, so it is what gets recorded.  The tape accepts only
+
+    mul; add / sub / rsub with alpha = +-1 (any other alpha lets ATen contract to an FMA); neg; sqrt;
+    div by a tensor; div by a CPU scalar (ATen computes a * (1/b), with 1/b rounded in the state dtype);
+    pow(x, 2) (ATen computes x * x); aliasing views that keep every element where it is (no-ops),
+
+on operands that are y, the step's 0-d time t0, go, Python numbers and CPU 0-d tensors (immediates, rounded to the
+state dtype as ATen rounds them), one-element device tensors, (d,)-shaped device tensors broadcast over the rows and
+(rows, d) device tensors, all of the state dtype, on y's device and contiguous.  Anything else — another op, a
+reduction, `.item()`, an in-place op on anything the tape did not produce, a read of a tensor whose storage was
+written in place through another tensor (a view, `detach()`, `.data`), an operand that shares storage with a value of
+the tape, a 16-bit result, a tensor created by a factory — rejects the tape, and the solve keeps its ordinary step.
+
+Device operands are passed by address and read at every launch: in-place updates of parameters (optimiser steps) are
+followed, exactly as by a captured CUDA graph; f and g must not depend on anything else (the purity contract of
+graph capture, README).  SDEs whose callables have side effects say so with options={'overlap': False}, and keep
+calling them every step.
+"""
+import numbers
+
+import numpy as np
+import torch
+from torch.utils._python_dispatch import TorchDispatchMode
+
+from .. import _cabi
+
+aten = torch.ops.aten
+
+# op -> (opcode, swap operands)
+_BINARY = {
+    aten.mul.Tensor: (_cabi.PW_MUL, False), aten.mul.Scalar: (_cabi.PW_MUL, False),
+    aten.add.Tensor: (_cabi.PW_ADD, False), aten.add.Scalar: (_cabi.PW_ADD, False),
+    aten.sub.Tensor: (_cabi.PW_SUB, False), aten.sub.Scalar: (_cabi.PW_SUB, False),
+    aten.rsub.Tensor: (_cabi.PW_SUB, True), aten.rsub.Scalar: (_cabi.PW_SUB, True),
+    aten.div.Tensor: (_cabi.PW_DIV, False), aten.div.Scalar: (_cabi.PW_DIV, False),
+}
+_UNARY = {aten.neg.default: _cabi.PW_NEG, aten.sqrt.default: _cabi.PW_SQRT}
+_IN_PLACE = {aten.mul_.Tensor: aten.mul.Tensor, aten.add_.Tensor: aten.add.Tensor,
+             aten.sub_.Tensor: aten.sub.Tensor, aten.div_.Tensor: aten.div.Tensor}
+_ALIAS = {aten.view.default, aten._unsafe_view.default, aten.expand.default, aten.unsqueeze.default,
+          aten.detach.default, aten.alias.default}
+
+Y, GO, T0 = ('y',), ('go',), ('t0',)
+STALE = ('stale',)  # a tensor whose storage was written in place through another tensor
+
+
+class Reject(Exception):
+    pass
+
+
+def _strip(shape):
+    """Shape without its leading ones: the element mapping of a tensor broadcast right-aligned to (rows, d)."""
+    shape = tuple(shape)
+    while shape and shape[0] == 1:
+        shape = shape[1:]
+    return shape
+
+
+class Recorder(TorchDispatchMode):
+    """Records the element-wise tape of one Milstein step; `finish` turns it into a tsde_pointwise program."""
+
+    def __init__(self, y, t0):
+        super().__init__()
+        self.rows, self.d = y.shape
+        self.dtype, self.device = y.dtype, y.device
+        self.ok, self.reason = True, None
+        self.instrs = []       # (opcode, value id, source, source)
+        self.n_fg = None
+        self.operands = []     # (kind, ptr, imm)
+        self._operand_ix = {}
+        self._keep = []        # every tensor seen: no address is reused while recording
+        self._by_obj = {}      # id(tensor) -> source
+        self._by_addr = {}     # (data_ptr, shape, stride) -> source
+        self._storage = {}     # id(tensor) / address key -> storage of every bound tensor
+        self._shapes = {(), _strip((self.d,)), _strip((self.rows, self.d))}
+        self._vjp = False
+        self._bind(y, Y)
+        if t0.dtype == self.dtype and t0.device == self.device:  # (else an op on t0 rejects the tape)
+            self._bind(t0, T0)
+
+    # -- the three segments ---------------------------------------------------------------------------------------
+    def segment(self, fn, y=None, go=None):
+        """fn() with its ATen ops recorded.  `y` is the tensor the segment calls the state (a detached alias of the
+        state for g), `go` the vjp seed (vjp segment)."""
+        if y is not None:
+            self._bind(y, Y)
+        if go is not None:
+            self._bind(go, GO)
+            self._vjp = True
+            self.n_fg = len(self.instrs)
+        with self:
+            return fn()
+
+    def reject(self, reason):
+        if self.ok:
+            self.ok, self.reason = False, reason
+
+    def __torch_dispatch__(self, func, types, args=(), kwargs=None):
+        kwargs = kwargs or {}
+        out = func(*args, **kwargs)
+        if self.ok:
+            try:
+                self._record(func, args, kwargs, out)
+            except Exception as e:  # (anything the recorder cannot account for keeps the ordinary step)
+                self.reject(f"{type(e).__name__}: {e}")
+        return out
+
+    # -- values ------------------------------------------------------------------------------------------------
+    @staticmethod
+    def _addr(t):
+        return (t.data_ptr(), tuple(t.shape), tuple(t.stride()), t.dtype)
+
+    def _bind(self, t, src):
+        self._keep.append(t)
+        self._by_obj[id(t)] = src
+        self._by_addr[self._addr(t)] = src
+        self._storage[id(t)] = self._storage[self._addr(t)] = t.untyped_storage().data_ptr()
+
+    def _written(self, t):
+        """`t` is about to be written in place: every other tensor bound to its storage (a view, `detach()`,
+        `.data`) would keep the old value, so reading one of them rejects the tape."""
+        st, own = t.untyped_storage().data_ptr(), (id(t), self._addr(t))
+        for key, s in self._storage.items():
+            if s == st and key not in own:
+                (self._by_addr if isinstance(key, tuple) else self._by_obj)[key] = STALE
+
+    def _operand(self, kind, ptr, imm):
+        key = (kind, ptr, float(imm).hex())
+        if key not in self._operand_ix:
+            self._operand_ix[key] = len(self.operands)
+            self.operands.append(key[:2] + (imm,))
+        return ('k', self._operand_ix[key])
+
+    def _immediate(self, x):
+        if isinstance(x, bool) or not isinstance(x, numbers.Real):
+            raise Reject(f"unsupported scalar {x!r}")
+        return float(np.asarray(x).astype(self._np))
+
+    @property
+    def _np(self):
+        return np.float32 if self.dtype == torch.float32 else np.float64
+
+    def _source(self, x):
+        """What an op input is: a value of the tape, y, go, or an operand."""
+        if not torch.is_tensor(x):
+            return self._operand(_cabi.PW_IMM, None, self._immediate(x))
+        src = self._by_obj.get(id(x))
+        if src is None:
+            src = self._by_addr.get(self._addr(x))
+        if src == T0:
+            return self._operand(_cabi.PW_T0, None, 0.0)
+        if src == STALE:
+            raise Reject("a tensor aliasing one written in place is read")
+        if src is not None:
+            return src
+        if x.device.type == 'cpu' and x.dim() == 0 and x.device != self.device:
+            return self._operand(_cabi.PW_IMM, None, self._immediate(x.item()))
+        if x.device != self.device or x.dtype != self.dtype or x.requires_grad and x.grad_fn is not None:
+            raise Reject(f"operand {tuple(x.shape)} {x.dtype} on {x.device}")
+        if not x.is_contiguous():
+            raise Reject(f"non-contiguous operand {tuple(x.shape)}")
+        if x.untyped_storage().data_ptr() in self._storage.values():
+            raise Reject("an operand shares storage with a value of the tape")
+        if x.numel() == 1:
+            kind = _cabi.PW_SCALAR
+        elif _strip(x.shape) == (self.d,):
+            kind = _cabi.PW_CHANNEL
+        elif tuple(x.shape) == (self.rows, self.d):
+            kind = _cabi.PW_ROW
+        else:
+            raise Reject(f"operand of shape {tuple(x.shape)}")
+        self._keep.append(x)
+        return self._operand(kind, x.data_ptr(), 0.0)
+
+    def _result(self, out):
+        if not torch.is_tensor(out) or out.dtype != self.dtype or out.device != self.device:
+            raise Reject("result is not a tensor of the state dtype")
+        if _strip(out.shape) not in self._shapes:
+            raise Reject(f"result of shape {tuple(out.shape)}")
+
+    def _emit(self, op, a, b, out):
+        self._result(out)
+        v = ('v', len(self.instrs))
+        self.instrs.append((op, v, a, b))
+        self._bind(out, v)
+
+    def _record(self, func, args, kwargs, out):
+        if func in _ALIAS:
+            self._result(out)
+            if _strip(args[0].shape) != _strip(out.shape) and not (
+                    func is aten.expand.default and _strip(out.shape) == (self.rows, self.d)):
+                raise Reject(f"{func} moves elements")
+            self._bind(out, self._source(args[0]))
+            return
+        if func in _IN_PLACE:
+            if self._source(args[0])[0] != 'v':
+                raise Reject(f"{func} writes a tensor the tape did not produce")
+            self._written(args[0])
+            func = _IN_PLACE[func]
+        elif func._schema.is_mutable or 'out' in kwargs:
+            raise Reject(f"{func} mutates its arguments")
+        if func in _UNARY:
+            self._emit(_UNARY[func], self._source(args[0]), None, out)
+            return
+        if func is aten.pow.Tensor_Scalar:
+            if not (isinstance(args[1], numbers.Real) and not isinstance(args[1], bool) and args[1] == 2):
+                raise Reject(f"pow with exponent {args[1]!r}")
+            a = self._source(args[0])
+            self._emit(_cabi.PW_MUL, a, a, out)
+            return
+        if func not in _BINARY:
+            raise Reject(f"{func} is not an element-wise op the kernel restates")
+        op, swap = _BINARY[func]
+        alpha = kwargs.get('alpha', args[2] if len(args) > 2 else 1)
+        if op in (_cabi.PW_MUL, _cabi.PW_DIV) and (len(args) > 2 or kwargs):
+            raise Reject(f"{func} with {kwargs}")
+        if op in (_cabi.PW_ADD, _cabi.PW_SUB):
+            if isinstance(alpha, bool) or alpha not in (1, -1):
+                raise Reject(f"{func} with alpha={alpha!r}")
+            if alpha == -1:
+                op = _cabi.PW_SUB if op == _cabi.PW_ADD else _cabi.PW_ADD
+        a, b = (args[1], args[0]) if swap else (args[0], args[1])
+        if op == _cabi.PW_DIV and (not torch.is_tensor(b) or b.device.type == 'cpu' and b.dim() == 0
+                                   and b.device != self.device):
+            # ATen: a CPU-scalar divisor becomes a multiplication by its reciprocal, rounded in the state dtype
+            inv = self._np(1) / self._np(self._immediate(b.item() if torch.is_tensor(b) else b))
+            self._emit(_cabi.PW_MUL, self._source(a), self._operand(_cabi.PW_IMM, None, float(inv)), out)
+            return
+        self._emit(op, self._source(a), self._source(b), out)
+
+    # -- the program -----------------------------------------------------------------------------------------------
+    def finish(self, f, g, gdg):
+        """The tsde_pointwise program of the recorded step (and the tensors it reads), or None if it was rejected."""
+        if self.ok and self.n_fg is None:
+            self.reject("no vjp segment")
+        if not self.ok:
+            return None
+        try:
+            outs = []
+            for t, vjp in ((f, False), (g, False), (gdg, True)):
+                if not torch.is_tensor(t) or tuple(t.shape) != (self.rows, self.d) or t.dtype != self.dtype:
+                    raise Reject("a result is not a (rows, d) tensor of the state dtype")
+                src = self._source(t)
+                if src[0] == 'k' or src == GO and not vjp:
+                    raise Reject("a result is not computed from the state")
+                outs.append(src)
+            return self._compile(*outs)
+        except Exception as e:
+            self.reject(f"{type(e).__name__}: {e}")
+            return None
+
+    def _compile(self, f, g, gdg):
+        n_fg = self.n_fg
+        # dead-code elimination and last uses (the boundary reads f, g at n_fg, gdg at the end)
+        last = {}
+        for pos, v in ((n_fg, f), (n_fg, g), (len(self.instrs), gdg)):
+            if v[0] == 'v':
+                last[v] = max(last.get(v, -1), pos)
+        live = []
+        for i in range(len(self.instrs) - 1, -1, -1):
+            op, v, a, b = self.instrs[i]
+            if v not in last:
+                continue
+            live.append(i)
+            for s in (a, b):
+                if s is not None and s[0] == 'v':
+                    last[s] = max(last.get(s, -1), i)
+        live.reverse()
+        if len(live) > _cabi.PW_MAX_INSTR or len(self.operands) > _cabi.PW_MAX_OPERANDS:
+            raise Reject("program too long")
+        # registers: linear scan; a register whose value was last read by this instruction may be its destination
+        reg, free, n_regs = {}, [], 0
+        prog = _cabi.Pointwise()
+
+        def code(s):
+            if s == Y:
+                return _cabi.PW_SRC_Y
+            if s == GO:
+                return _cabi.PW_SRC_GO
+            if s[0] == 'k':
+                return _cabi.PW_OPERAND0 + s[1]
+            return reg[s]
+
+        new_fg = sum(1 for i in live if i < n_fg)
+        for j, i in enumerate(live):
+            op, v, a, b = self.instrs[i]
+            if j == new_fg:
+                prog.f_src, prog.g_src = code(f), code(g)
+            ins = prog.instr[j]
+            ins.op, ins.a = op, code(a)
+            ins.b = code(b) if b is not None else 0
+            # (the kernel reads both sources before it writes the destination)
+            for s in [s for s in reg if last[s] <= i]:
+                free.append(reg.pop(s))
+            if free:
+                reg[v] = free.pop()
+            else:
+                reg[v] = n_regs
+                n_regs += 1
+            ins.dst = reg[v]
+        if new_fg == len(live):
+            prog.f_src, prog.g_src = code(f), code(g)
+        prog.gdg_src = code(gdg)
+        if n_regs > _cabi.PW_MAX_REGS:
+            raise Reject("too many live values")
+        prog.n_instr, prog.n_fg, prog.n_regs, prog.n_operands = len(live), new_fg, n_regs, len(self.operands)
+        for k, (kind, ptr, imm) in enumerate(self.operands):
+            prog.operand[k].kind, prog.operand[k].ptr, prog.operand[k].imm = kind, ptr, imm
+        return prog, tuple(t for t in self._keep if self._is_operand(t))
+
+    def _is_operand(self, t):
+        src = self._by_obj.get(id(t))
+        return src is None or src[0] == 'k'
+
+
+def eligible(solver):
+    """Whether a fixed-step Milstein solve may run its diagonal-noise steps as element-wise programs."""
+    from .base_sde import SDELogqp
+    sde = solver.sde
+    obj = sde
+    while hasattr(obj, '_base_sde'):
+        obj = obj._base_sde
+        if isinstance(obj, SDELogqp):
+            return False
+    feed = getattr(solver, '_feed', None)
+    overlap = solver.options.get('overlap')
+    return (not solver._autograd and feed is not None and feed.binding is not None
+            and (overlap is None or bool(overlap)) and not torch.is_autocast_enabled('cuda'))

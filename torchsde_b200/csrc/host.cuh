@@ -25,6 +25,10 @@ constexpr int64_t kMaxGlobalRows = 0xFFFFFFFFll;
 // 2^26 channels one stream's normals would be another stream's.
 constexpr int64_t kMaxCounterChannels = 1ll << 26;
 
+// Launches issued per kernel family (TSDE_KERNEL_*), read by tsde_kernel_launches.
+constexpr int kKernelFamilies = 4;
+inline std::atomic<int64_t> g_launches[kKernelFamilies];
+
 // A launch descriptor every entry point can rely on: non-null, non-negative row count, positive widths.
 inline bool valid_launch(const tsde_launch* L) { return L && L->rows >= 0 && L->d > 0 && L->m > 0; }
 

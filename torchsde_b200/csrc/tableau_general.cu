@@ -21,8 +21,6 @@ namespace tsde {
 
 constexpr int kMaxRowsPerBlock = 64;
 
-static std::atomic<int64_t> g_launches[3];  // TSDE_KERNEL_GEN_CTA, TSDE_KERNEL_GEN_TMA, TSDE_KERNEL_GEN_WIDE
-
 template <int NE, int NG, int NO>
 struct GenP {
   const void* e[NE > 0 ? NE : 1];
@@ -1262,6 +1260,6 @@ TSDE_EXPORT int tsde_step_srk_additive(const tsde_launch* L, const tsde_noise* n
 }
 
 TSDE_EXPORT int64_t tsde_kernel_launches(int32_t family) {
-  if (family < 0 || family > 2) return -1;
+  if (family < 0 || family >= kKernelFamilies) return -1;
   return g_launches[family].load(std::memory_order_relaxed);
 }
