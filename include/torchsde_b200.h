@@ -129,6 +129,7 @@ const char* tsde_error_string(int code);
 #define TSDE_KERNEL_GEN_TMA 1  /* TMA-staged persistent tile kernel (bulk copies)   */
 #define TSDE_KERNEL_GEN_WIDE 2 /* chunked tile kernel for rows whose increments exceed shared memory */
 #define TSDE_KERNEL_PW_MILSTEIN 3 /* whole Milstein step with an element-wise SDE (tsde_step_milstein_pointwise) */
+#define TSDE_KERNEL_PW_SRK 4      /* whole SRK step with an element-wise SDE (tsde_step_srk_diag_pointwise)     */
 int64_t tsde_kernel_launches(int32_t family);
 
 /* ------------------------------------------------------------------------ */
@@ -289,6 +290,29 @@ typedef struct tsde_pointwise {
 } tsde_pointwise;
 int tsde_step_milstein_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
                                  const void* y0, const void* t0, double dt, int32_t ito, void* y1);
+
+/*
+ * A whole diagonal-noise SRK (srid2) step (srk.py:57-88) for an SDE whose f(t, y) and g(t, y) are element-wise
+ * programs: one launch reads y0, draws W and U, and evaluates the step's seven SDE calls and four tableau stages
+ *     f0 = f(t_0, y0), g0 = g(t_0, y0); H0_1, H1_1 as tsde_srk_diag_stage1;
+ *     f1 = f(t_1, H0_1), g1 = g(t_q, H1_1); H0_2, H1_2 as tsde_srk_diag_stage2;
+ *     f2 = f(t_h, H0_2), g2 = g(t_1, H1_2); H1_3 as tsde_srk_diag_stage3; g3 = g(t_q, H1_3);
+ *     y1 as tsde_step_srk_diag
+ * in registers and writes y1.  t_0, t_1, t_q, t_h are the 0-d stage times t0 + 0*dt, t0 + dt, t0 + dt/4 and
+ * t0 + dt/2 (state dtype), read at every launch; dt, rdt, sqrt_dt, three_dt are the scalars tsde_step_srk_diag
+ * takes.  The step equals the unfused one bit for bit.
+ *
+ * Program: the tsde_pointwise layout above holds two programs.  Instructions [0, n_fg) are f, whose result is f_src;
+ * [n_fg, n_instr) are g, whose result is g_src; gdg_src is unused.  Each program starts with no register defined
+ * and reads only its own; TSDE_PW_SRC_Y is the state it is evaluated at, TSDE_PW_T0 its time, TSDE_PW_SRC_GO is
+ * not a source.  The operand table is shared.  n_regs <= TSDE_PW_SRK_MAX_REGS: the kernel may keep six stage values
+ * in the rest of the register file.
+ * Requires DIAGONAL noise, counter noise (nz->source == TSDE_SRC_COUNTER) and no 16-bit formats.
+ */
+#define TSDE_PW_SRK_MAX_REGS 18
+int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                 const void* y0, const void* t_0, const void* t_1, const void* t_q,
+                                 const void* t_h, double dt, double rdt, double sqrt_dt, double three_dt, void* y1);
 
 /* derivative-free Milstein, predictor: y' = y0 + (Ito ? dt*f : 0) + g*sqrt_dt
  * methods/milstein.py:58-63,83-84,93-94.  g is (rows,d) also for scalar noise (squeezed). */

@@ -50,7 +50,9 @@ PW_MAX_INSTR, PW_MAX_OPERANDS, PW_MAX_REGS = 96, 24, 24  # TSDE_PW_MAX_*
 PW_SRC_Y, PW_SRC_GO, PW_OPERAND0 = 0xFE, 0xFF, 0x80
 PW_MUL, PW_ADD, PW_SUB, PW_DIV, PW_NEG, PW_SQRT = range(6)
 PW_IMM, PW_T0, PW_SCALAR, PW_CHANNEL, PW_ROW = range(5)
+PW_SRK_MAX_REGS = 18  # TSDE_PW_SRK_MAX_REGS
 KERNEL_PW_MILSTEIN = 3  # TSDE_KERNEL_PW_MILSTEIN
+KERNEL_PW_SRK = 4  # TSDE_KERNEL_PW_SRK
 
 
 class PwInstr(ctypes.Structure):
@@ -91,6 +93,7 @@ SIGNATURES = {
     'tsde_milstein_vjp_seed': [_L, _N, _P, _D, _I, _P],
     'tsde_step_milstein': [_L, _N, _P, _P, _P, _P, _D, _P],
     'tsde_step_milstein_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _D, _I, _P],
+    'tsde_step_srk_diag_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _P, _P, _P, _D, _D, _D, _D, _P],
     'tsde_milstein_gf_predict': [_L, _P, _P, _P, _D, _D, _I, _P],
     'tsde_step_milstein_gf': [_L, _N, _P, _P, _P, _P, _D, _D, _I, _P],
     'tsde_step_heun': [_L, _N, _P, _P, _P, _P, _P, _D, _P],

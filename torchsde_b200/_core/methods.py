@@ -326,6 +326,7 @@ class SRK(base_solver.BaseSDESolver):
                              "diffusion-vector product. Use a different method instead.")
         self._additive = sde.noise_type == NOISE_TYPES.additive
         super(SRK, self).__init__(sde=sde, **kwargs)
+        self._pw = None  # the element-wise programs of the step (pointwise.py), False once rejected
 
     def aux_times(self, t0, t1, dt):
         if self._additive:
@@ -402,14 +403,36 @@ class SRK(base_solver.BaseSDESolver):
         sde, s = self.sde, c.scalars
         t_00, t_1, t_q, t_h = c.aux_t  # t0 + 0*dt, t0 + dt, t0 + dt/4, t0 + dt/2
         LU, L = self._LU, self._L
-        f0, g0 = self._fork(lambda: _contig(sde.f(t_00, y0)), lambda: _contig(sde.g(t_00, y0)))
+        if self._pw and self._feed.binding is not None:
+            # f and g were recorded as element-wise programs (pointwise.py): the whole step is one kernel
+            prog, _ = self._pw
+            out = out if out is not None else torch.empty_like(y0)
+            _cabi.check(self._lib.tsde_step_srk_diag_pointwise(
+                L, self._feed.get(c, True), ctypes.byref(prog), y0.data_ptr(), t_00.data_ptr(), t_1.data_ptr(),
+                t_q.data_ptr(), t_h.data_ptr(), c.dt, s['rdt'], s['sqrt_dt'], s['three_dt'], out.data_ptr()),
+                'tsde_step_srk_diag_pointwise')
+            return out
+        # the first step of an eligible solve runs as always, with the user's seven evaluations recorded
+        rec = None
+        if self._pw is None and sde.noise_type == NOISE_TYPES.diagonal and pointwise.eligible(self):
+            rec = pointwise.SrkRecorder(y0, t_00)
+
+        def f(t, y):
+            return _contig(rec.evaluation('f', lambda: sde.f(t, y), t, y) if rec is not None else sde.f(t, y))
+
+        def g(t, y):
+            return _contig(rec.evaluation('g', lambda: sde.g(t, y), t, y) if rec is not None else sde.g(t, y))
+
+        f0, g0 = self._fork(lambda: f(t_00, y0), lambda: g(t_00, y0))
         h0_1, h1_1 = self._k('tsde_srk_diag_stage1', LU, None, (y0, f0, g0), (c.dt, s['sqrt_dt']), None, n_out=2)
-        f1, g1 = self._fork(lambda: _contig(sde.f(t_1, h0_1)), lambda: _contig(sde.g(t_q, h1_1)))
+        f1, g1 = self._fork(lambda: f(t_1, h0_1), lambda: g(t_q, h1_1))
         h0_2, h1_2 = self._k('tsde_srk_diag_stage2', L, self._feed.get(c, True), (y0, f0, g0, f1, g1),
                              (c.dt, s['rdt'], s['sqrt_dt']), None, n_out=2)
-        f2, g2 = self._fork(lambda: _contig(sde.f(t_h, h0_2)), lambda: _contig(sde.g(t_1, h1_2)))
+        f2, g2 = self._fork(lambda: f(t_h, h0_2), lambda: g(t_1, h1_2))
         h1_3 = self._k('tsde_srk_diag_stage3', LU, None, (y0, g0, g1, f2, g2), (c.dt, s['sqrt_dt']), None)
-        g3 = _contig(sde.g(t_q, h1_3))
+        g3 = g(t_q, h1_3)
+        if rec is not None:
+            self._pw = rec.finish() or False
         return self._k('tsde_step_srk_diag', L, self._feed.get(c, True), (y0, f0, f1, f2, g0, g1, g2, g3),
                        (c.dt, s['rdt'], s['sqrt_dt'], s['three_dt']), out)
 

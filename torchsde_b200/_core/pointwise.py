@@ -1,4 +1,7 @@
-"""Element-wise tapes of the user's SDE: a diagonal-noise Milstein step as one kernel.
+"""Element-wise tapes of the user's SDE: a diagonal-noise Milstein or SRK step as one kernel.
+
+SRK (`SrkRecorder`) records the step's seven f / g evaluations with the same whitelist and rules as below and runs
+them in tsde_step_srk_diag_pointwise; the rest of this docstring describes the Milstein case.
 
 The unfused step runs five full-batch passes: the user's f and g, the vjp seed, autograd's vjp of g and the tableau
 (methods.BaseMilstein._step).  When f(t, y), g(t, y) and the vjp of g are made only of element-wise ATen ops whose
@@ -52,6 +55,7 @@ _ALIAS = {aten.view.default, aten._unsafe_view.default, aten.expand.default, ate
 
 Y, GO, T0 = ('y',), ('go',), ('t0',)
 STALE = ('stale',)  # a tensor whose storage was written in place through another tensor
+FOREIGN = ('foreign',)  # a value bound by an earlier evaluation of an SRK step
 
 
 class Reject(Exception):
@@ -254,21 +258,20 @@ class Recorder(TorchDispatchMode):
                 if src[0] == 'k' or src == GO and not vjp:
                     raise Reject("a result is not computed from the state")
                 outs.append(src)
-            return self._compile(*outs)
+            return self._compile(self.instrs, self.n_fg, *outs)
         except Exception as e:
             self.reject(f"{type(e).__name__}: {e}")
             return None
 
-    def _compile(self, f, g, gdg):
-        n_fg = self.n_fg
+    def _compile(self, instrs, n_fg, f, g, gdg):
         # dead-code elimination and last uses (the boundary reads f, g at n_fg, gdg at the end)
         last = {}
-        for pos, v in ((n_fg, f), (n_fg, g), (len(self.instrs), gdg)):
+        for pos, v in ((n_fg, f), (n_fg, g), (len(instrs), gdg)):
             if v[0] == 'v':
                 last[v] = max(last.get(v, -1), pos)
         live = []
-        for i in range(len(self.instrs) - 1, -1, -1):
-            op, v, a, b = self.instrs[i]
+        for i in range(len(instrs) - 1, -1, -1):
+            op, v, a, b = instrs[i]
             if v not in last:
                 continue
             live.append(i)
@@ -293,7 +296,7 @@ class Recorder(TorchDispatchMode):
 
         new_fg = sum(1 for i in live if i < n_fg)
         for j, i in enumerate(live):
-            op, v, a, b = self.instrs[i]
+            op, v, a, b = instrs[i]
             if j == new_fg:
                 prog.f_src, prog.g_src = code(f), code(g)
             ins = prog.instr[j]
@@ -323,8 +326,96 @@ class Recorder(TorchDispatchMode):
         return src is None or src[0] == 'k'
 
 
+class SrkRecorder(Recorder):
+    """Records the seven SDE evaluations of one diagonal-noise SRK step (methods.SRK._diagonal_or_scalar_step): f at
+    three (t, y), g at four.  Each is a segment of its own, with its own state and 0-d time.  `finish` accepts the
+    tape when the three f segments are one program (same ops, operands and order) and so are the four g segments,
+    and compiles the first of each into the two-program layout of tsde_step_srk_diag_pointwise.  A Python-side
+    branch between evaluations (or any other difference) therefore keeps the ordinary step."""
+
+    def __init__(self, y, t):
+        super().__init__(y, t)
+        self.segments = []  # (kind, first instruction, end, result source)
+
+    def evaluation(self, kind, fn, t, y):
+        """fn(), the SDE's f (`kind` 'f') or g ('g') at (t, y), with its ATen ops recorded.  Every value bound by an
+        earlier evaluation (its state, its time, its intermediates) is foreign to this one; a view of an operand is
+        an operand again."""
+        for table in (self._by_obj, self._by_addr):
+            for key, src in list(table.items()):
+                if src[0] == 'k':
+                    del table[key]
+                    self._storage.pop(key, None)
+                else:
+                    table[key] = FOREIGN
+        self._bind(y, Y)
+        if t.dtype == self.dtype and t.device == self.device:
+            self._bind(t, T0)
+        start = len(self.instrs)
+        with self:
+            out = fn()
+        if self.ok:
+            try:
+                if not torch.is_tensor(out) or tuple(out.shape) != (self.rows, self.d) or out.dtype != self.dtype:
+                    raise Reject("a result is not a (rows, d) tensor of the state dtype")
+                src = self._source(out)
+                if src[0] == 'k':
+                    raise Reject("a result is not computed from the state")
+                self.segments.append((kind, start, len(self.instrs), src))
+            except Exception as e:
+                self.reject(f"{type(e).__name__}: {e}")
+        return out
+
+    def _source(self, x):
+        src = super()._source(x)
+        if src == FOREIGN:
+            raise Reject("a value of another evaluation is read")
+        return src
+
+    def _tape(self, start, end, src):
+        """Instructions [start, end) and the result, with value ids relative to the segment."""
+        def rel(s):
+            return ('v', s[1] - start) if s is not None and s[0] == 'v' else s
+        return [(op, rel(v), rel(a), rel(b)) for op, v, a, b in self.instrs[start:end]], rel(src)
+
+    def finish(self):
+        """The tsde_pointwise program of the recorded step (and the tensors it reads), or None if it was rejected."""
+        if not self.ok:
+            return None
+        try:
+            if [s[0] for s in self.segments] != list('fgfgfgg'):
+                raise Reject("not the seven evaluations of an SRK step")
+            progs = []
+            for kind in 'fg':
+                segs = [s for s in self.segments if s[0] == kind]
+                tapes = [self._tape(*s[1:]) for s in segs]
+                if any(tp != tapes[0] for tp in tapes[1:]):
+                    raise Reject(f"the {kind} evaluations differ")
+                _, start, end, src = segs[0]
+                instrs = self.instrs[start:end]
+                progs.append(self._compile(instrs, len(instrs), src, src, src)[0])
+            pf, pg = progs
+            if pf.n_instr + pg.n_instr > _cabi.PW_MAX_INSTR:
+                raise Reject("program too long")
+            prog = _cabi.Pointwise()
+            for j in range(pf.n_instr):
+                prog.instr[j] = pf.instr[j]
+            for j in range(pg.n_instr):
+                prog.instr[pf.n_instr + j] = pg.instr[j]
+            prog.n_instr, prog.n_fg = pf.n_instr + pg.n_instr, pf.n_instr
+            prog.n_regs = max(pf.n_regs, pg.n_regs)
+            if prog.n_regs > _cabi.PW_SRK_MAX_REGS:
+                raise Reject("too many live values")
+            prog.f_src, prog.g_src, prog.n_operands = pf.f_src, pg.g_src, pf.n_operands
+            prog.operand = pf.operand
+            return prog, tuple(t for t in self._keep if self._is_operand(t))
+        except Exception as e:
+            self.reject(f"{type(e).__name__}: {e}")
+            return None
+
+
 def eligible(solver):
-    """Whether a fixed-step Milstein solve may run its diagonal-noise steps as element-wise programs."""
+    """Whether a fixed-step Milstein or SRK solve may run its diagonal-noise steps as element-wise programs."""
     from .base_sde import SDELogqp
     sde = solver.sde
     obj = sde

@@ -570,12 +570,162 @@ pw_milstein_kernel(const __grid_constant__ tsde_pointwise pg, const PwP<T> p, co
   store_quad(p.y1, c.base, c.vec, c.nvalid, y1);
 }
 
+// ---- a whole SRK step of an element-wise SDE (tsde_step_srk_diag_pointwise) -----------------------------------------
+// One thread per quad again: W and U are drawn before the dependency wait, y0 is read, and the seven SDE evaluations
+// (the f program at three (t, y), the g program at four) alternate with the unfused step's own stage ops.  y0 and y1
+// are the only tensors the step moves, against 22 reads and 6 writes of the unfused step (41 with f and g).
+//
+// At the last update ten quads are live (y0, f0..f2, g0..g3, W, U).  In fp64 that is 80 registers before the
+// interpreter's own, so there f0..f2 and g0..g2 wait in the shared-memory register file, in the kPwSrkStash slots
+// past the program's registers; in fp32 they stay in registers.
+constexpr int kPwSrkStash = TSDE_PW_MAX_REGS - TSDE_PW_SRK_MAX_REGS;  // six: f0..f2, g0..g2
+
+template <typename T>
+struct PwSrkP {
+  PwP<T> base;    // y0, y1, the quad mapping; base.t0 unused
+  const T* t[4];  // t_0, t_1, t_q, t_h
+  SrkDiagStage1Op<T> s1;
+  SrkDiagStage2Op<T> s2;
+  SrkDiagStage3Op<T> s3;
+  SrkDiagFinalOp<T> fin;
+};
+
+template <typename T>
+struct PwSrkStash {
+  static constexpr bool kShared = sizeof(T) == 8;
+  T r[kShared ? 1 : kPwSrkStash][4];
+  int slot0;  // first shared-memory register past the program's
+  __device__ __forceinline__ void put(void* regs, int k, const T (&x)[4]) {
+    if constexpr (kShared) {
+      pw_sstore(regs, slot0 + k, x);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) r[k][j] = x[j];
+    }
+  }
+  __device__ __forceinline__ void get(const void* regs, int k, T (&x)[4]) const {
+    if constexpr (kShared) {
+      pw_sload(regs, slot0 + k, x);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) x[j] = r[k][j];
+    }
+  }
+};
+
+// f (program [0, n_fg), result f_src) or g (program [n_fg, n_instr), result g_src) at (t, y)
+template <typename T>
+__device__ __forceinline__ void pw_srk_eval(const tsde_pointwise& pg, const PwSrkP<T>& p, PwQuad<T>& c, void* regs,
+                                            bool g, const T* t, const T (&y)[4], T (&out)[4]) {
+  PwP<T> at = p.base;
+  at.t0 = t;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) c.y[j] = y[j];
+  pw_run(pg, at, c, regs, g ? pg.n_fg : 0, g ? pg.n_instr : pg.n_fg);
+  pw_fetch(pg, at, c, regs, g ? pg.g_src : pg.f_src, out);
+}
+
+template <typename T, int SRC>
+__global__ void __launch_bounds__(kThreads)
+pw_srk_kernel(const __grid_constant__ tsde_pointwise pg, const PwSrkP<T> p, const NoiseP<T> nz) {
+  extern __shared__ __align__(16) unsigned char pw_regs[];
+  const PwP<T>& b = p.base;
+  const int64_t Q = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+  int64_t row, q;
+  if (b.qshift >= 0) {
+    row = Q >> b.qshift;
+    q = Q & ((1ll << b.qshift) - 1);
+  } else if (b.small) {
+    const uint32_t r32 = rowdiv_row((uint32_t)Q, b.qmagic);
+    row = r32;
+    q = (int64_t)rowdiv_quad((uint32_t)Q, r32, (uint32_t)b.qpr);
+  } else {
+    row = Q / b.qpr;
+    q = Q - row * b.qpr;
+  }
+  PwQuad<T> c;
+  c.chan = 4 * q;
+  c.base = row * b.d + c.chan;
+  const int64_t rem = b.d - c.chan;
+  c.nvalid = rem < 4 ? (int)rem : 4;
+  c.vec = b.vec != 0;
+  T w[4], u[4];
+  quad_noise<T, SRC, true>(nz, load_key(nz.key), row, q, c.vec, c.nvalid, w, u);
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (Q >= b.nquads) return;
+  T y0[4];
+  load_quad(b.y0, c.base, c.vec, c.nvalid, y0);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) c.go[j] = T(0);
+  PwSrkStash<T> st;
+  st.slot0 = pg.n_regs;
+  enum { F0, F1, F2, G0, G1, G2 };
+  T f[4], g[4], h0[4], h1[4], x[4], z[4];
+  // s = 0: f0, g0 at (t0, y0); H0_1, H1_1
+  pw_srk_eval(pg, p, c, pw_regs, false, p.t[0], y0, f);
+  pw_srk_eval(pg, p, c, pw_regs, true, p.t[0], y0, g);
+  st.put(pw_regs, F0, f);
+  st.put(pw_regs, G0, g);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[2];
+    p.s1({y0[j], f[j], g[j]}, w[j], u[j], o);
+    h0[j] = o[0];
+    h1[j] = o[1];
+  }
+  // s = 1: f1 at (t0 + dt, H0_1), g1 at (t0 + dt/4, H1_1); H0_2, H1_2
+  pw_srk_eval(pg, p, c, pw_regs, false, p.t[1], h0, f);
+  pw_srk_eval(pg, p, c, pw_regs, true, p.t[2], h1, g);
+  st.put(pw_regs, F1, f);
+  st.put(pw_regs, G1, g);
+  st.get(pw_regs, F0, x);
+  st.get(pw_regs, G0, z);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[2];
+    p.s2({y0[j], x[j], z[j], f[j], g[j]}, w[j], u[j], o);
+    h0[j] = o[0];
+    h1[j] = o[1];
+  }
+  // s = 2: f2 at (t0 + dt/2, H0_2), g2 at (t0 + dt, H1_2); H1_3
+  pw_srk_eval(pg, p, c, pw_regs, false, p.t[3], h0, f);
+  pw_srk_eval(pg, p, c, pw_regs, true, p.t[1], h1, g);
+  st.put(pw_regs, F2, f);
+  st.put(pw_regs, G2, g);
+  st.get(pw_regs, G0, x);
+  st.get(pw_regs, G1, z);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[1];
+    p.s3({y0[j], x[j], z[j], f[j], g[j]}, w[j], u[j], o);
+    h1[j] = o[0];
+  }
+  // s = 3: g3 at (t0 + dt/4, H1_3); y1
+  pw_srk_eval(pg, p, c, pw_regs, true, p.t[2], h1, g);
+  T f0[4], f1[4], f2[4], g0[4], g1[4], g2[4], y1[4];
+  st.get(pw_regs, F0, f0);
+  st.get(pw_regs, F1, f1);
+  st.get(pw_regs, F2, f2);
+  st.get(pw_regs, G0, g0);
+  st.get(pw_regs, G1, g1);
+  st.get(pw_regs, G2, g2);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[1];
+    p.fin({y0[j], f0[j], f1[j], f2[j], g0[j], g1[j], g2[j], g[j]}, w[j], u[j], o);
+    y1[j] = o[0];
+  }
+  store_quad(b.y1, c.base, c.vec, c.nvalid, y1);
+}
+
 // A program the kernel can run as given: instruction, register and operand indices in range, every register
-// written before it is read, device operands present (and 16-byte aligned for the vector path).
-static bool pw_valid(const tsde_pointwise& pg, bool* vec) {
+// written before it is read, device operands present (and 16-byte aligned for the vector path).  `two`: the SRK
+// layout, an f program [0, n_fg) and a g program [n_fg, n_instr) that each define their own registers.
+static bool pw_valid(const tsde_pointwise& pg, bool* vec, bool two = false) {
   if (pg.n_instr < 0 || pg.n_instr > TSDE_PW_MAX_INSTR || pg.n_fg < 0 || pg.n_fg > pg.n_instr ||
       pg.n_regs < 0 || pg.n_regs > TSDE_PW_MAX_REGS || pg.n_operands < 0 || pg.n_operands > TSDE_PW_MAX_OPERANDS)
     return false;
+  if (two && pg.n_regs > TSDE_PW_SRK_MAX_REGS) return false;
   for (int k = 0; k < pg.n_operands; ++k) {
     const tsde_pw_operand& o = pg.operand[k];
     if (o.kind < TSDE_PW_IMM || o.kind > TSDE_PW_ROW) return false;
@@ -590,15 +740,44 @@ static bool pw_valid(const tsde_pointwise& pg, bool* vec) {
     return (int)s < pg.n_regs && ((written >> s) & 1u);
   };
   for (int i = 0; i <= pg.n_instr; ++i) {
-    if (i == pg.n_fg && !(source_ok(pg.f_src, false) && source_ok(pg.g_src, false))) return false;
+    if (i == pg.n_fg) {
+      if (!source_ok(pg.f_src, false) || !(two || source_ok(pg.g_src, false))) return false;
+      if (two) written = 0;
+    }
     if (i == pg.n_instr) break;
     const tsde_pw_instr& in = pg.instr[i];
-    const bool vjp = i >= pg.n_fg;
+    const bool vjp = !two && i >= pg.n_fg;
     if (in.op > TSDE_PW_SQRT || (int)in.dst >= pg.n_regs || !source_ok(in.a, vjp)) return false;
     if (in.op != TSDE_PW_NEG && in.op != TSDE_PW_SQRT && !source_ok(in.b, vjp)) return false;
     written |= 1ull << in.dst;
   }
-  return source_ok(pg.gdg_src, true);
+  return two ? source_ok(pg.g_src, false) : source_ok(pg.gdg_src, true);
+}
+
+// The quad mapping of a pointwise step over (rows, d) and its noise; TSDE_EINVAL for a launch it cannot serve.
+template <typename T>
+static int pw_prepare(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
+                      void* y1, bool two, PwP<T>& p, NoiseP<T>& np) {
+  if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !prog || !y0 || !y1) return TSDE_EINVAL;
+  bool vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y1);
+  if (!pw_valid(*prog, &vec, two)) return TSDE_EINVAL;
+  if (int e = fill_noise<T>(L, nz, false, np)) return e;
+  p = PwP<T>{};
+  p.y0 = static_cast<const T*>(y0);
+  p.y1 = static_cast<T*>(y1);
+  p.d = L->d;
+  p.qpr = (L->d + 3) / 4;
+  p.nquads = L->rows * p.qpr;
+  p.qshift = -1;
+  if ((p.qpr & (p.qpr - 1)) == 0) {
+    int sh = 0;
+    while ((1ll << sh) < p.qpr) ++sh;
+    p.qshift = sh;
+  }
+  p.small = p.nquads < (1ll << 31) ? 1 : 0;
+  p.qmagic = p.qshift < 0 ? rowdiv_magic((uint64_t)p.qpr) : 0;
+  p.vec = vec ? 1 : 0;
+  return 0;
 }
 
 }  // namespace tsde
@@ -610,27 +789,11 @@ TSDE_EXPORT int tsde_step_milstein_pointwise(const tsde_launch* L, const tsde_no
   if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
   return dispatch(L, [&](auto t) -> int {
     using T = decltype(t);
-    if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !prog || !y0 || !y1 || !t0) return TSDE_EINVAL;
-    bool vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y1);
-    if (!pw_valid(*prog, &vec)) return TSDE_EINVAL;
+    if (!t0) return TSDE_EINVAL;
+    PwP<T> p;
     NoiseP<T> np;
-    if (int e = fill_noise<T>(L, nz, false, np)) return e;
-    PwP<T> p{};
-    p.y0 = static_cast<const T*>(y0);
-    p.y1 = static_cast<T*>(y1);
+    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, false, p, np)) return e;
     p.t0 = static_cast<const T*>(t0);
-    p.d = L->d;
-    p.qpr = (L->d + 3) / 4;
-    p.nquads = L->rows * p.qpr;
-    p.qshift = -1;
-    if ((p.qpr & (p.qpr - 1)) == 0) {
-      int sh = 0;
-      while ((1ll << sh) < p.qpr) ++sh;
-      p.qshift = sh;
-    }
-    p.small = p.nquads < (1ll << 31) ? 1 : 0;
-    p.qmagic = p.qshift < 0 ? rowdiv_magic((uint64_t)p.qpr) : 0;
-    p.vec = vec ? 1 : 0;
     p.dt = (T)dt;
     p.ito = ito;
     const size_t smem = (size_t)prog->n_regs * kThreads * 4 * sizeof(T);
@@ -640,6 +803,36 @@ TSDE_EXPORT int tsde_step_milstein_pointwise(const tsde_launch* L, const tsde_no
     const int e = launch_kernel(kernel, grid, kThreads, smem, reinterpret_cast<cudaStream_t>(L->stream), true, *prog,
                                 p, np);
     if (e == 0) g_launches[TSDE_KERNEL_PW_MILSTEIN].fetch_add(1, std::memory_order_relaxed);
+    return e;
+  });
+}
+
+TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                             const void* y0, const void* t_0, const void* t_1, const void* t_q,
+                                             const void* t_h, double dt, double rdt, double sqrt_dt, double three_dt,
+                                             void* y1) {
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
+  return dispatch(L, [&](auto t) -> int {
+    using T = decltype(t);
+    if (!t_0 || !t_1 || !t_q || !t_h) return TSDE_EINVAL;
+    PwSrkP<T> p;
+    NoiseP<T> np;
+    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, true, p.base, np)) return e;
+    const void* times[4] = {t_0, t_1, t_q, t_h};
+    for (int i = 0; i < 4; ++i) p.t[i] = static_cast<const T*>(times[i]);
+    // the coefficients of tsde_srk_diag_stage1/2/3 and tsde_step_srk_diag
+    p.s1 = SrkDiagStage1Op<T>{(T)dt, (T)sqrt_dt};
+    p.s2 = SrkDiagStage2Op<T>{(T)dt, (T)rdt, (T)sqrt_dt};
+    p.s3 = SrkDiagStage3Op<T>{(T)dt, (T)sqrt_dt};
+    p.fin = make_srk_final<T>(dt, rdt, sqrt_dt, three_dt);
+    const int slots = prog->n_regs + (PwSrkStash<T>::kShared ? kPwSrkStash : 0);
+    const size_t smem = (size_t)slots * kThreads * 4 * sizeof(T);
+    auto kernel = np.n_cells > 1 ? pw_srk_kernel<T, kSrcCounterMulti> : pw_srk_kernel<T, TSDE_SRC_COUNTER>;
+    if (resident_ctas(reinterpret_cast<const void*>(kernel), kThreads, smem) < 1) return TSDE_EINVAL;
+    const int64_t grid = (p.base.nquads + kThreads - 1) / kThreads;
+    const int e = launch_kernel(kernel, grid, kThreads, smem, reinterpret_cast<cudaStream_t>(L->stream), true, *prog,
+                                p, np);
+    if (e == 0) g_launches[TSDE_KERNEL_PW_SRK].fetch_add(1, std::memory_order_relaxed);
     return e;
   });
 }
