@@ -32,8 +32,8 @@ H = 2.0 ** -4      # cell length = dt: every derived scalar (sqrt, 1/dt, dt/2) i
 DT, SQ, RDT = H, math.sqrt(H), 1.0 / H
 
 # ---- the entry points: (name, inputs, outputs, wants U, scalar arguments, float64 formula) ------------------------
-# Inputs x, increment w, U u: float64 arrays.  The formulas restate torchsde_b200/csrc/tableau_diag.cu (which cites the
-# reference's methods/*.py lines); brownian_cells returns the increment itself.
+# Inputs x, increment w, U u: float64 arrays.  The formulas restate torchsde_b200/csrc/tableau_diag_ops.cuh (which
+# cites the reference's methods/*.py lines); brownian_cells returns the increment itself.
 
 
 def _srk_final(x, w, u):
@@ -94,8 +94,8 @@ PLAIN_OPS = [
 
 
 def plain_emulated(op, x):
-    """The outputs of noise-free op `op` on numpy inputs x in T, in the op's written order (tableau_diag.cu: one IEEE
-    rounding per operation, no fma under -fmad=false); the double scalars are cast to T."""
+    """The outputs of noise-free op `op` on numpy inputs x in T, in the op's written order (tableau_diag_ops.cuh: one
+    IEEE rounding per operation, no fma under -fmad=false); the double scalars are cast to T."""
     name, nin, _, _, scalars, _ = op
     T = x[0].dtype.type
     s = [T(v) for v in scalars]

@@ -8,7 +8,6 @@ reference's ``step`` by one or two launches through the C ABI (include/torchsde_
 ``self._k(name, L, nz, inputs, scalars, outputs)`` (base_solver.py) — a direct launch on the fast path,
 an autograd node when gradients must flow through the solve.
 """
-import ctypes
 
 import numpy as np
 import torch
@@ -150,19 +149,13 @@ class BaseMilstein(_ProdMixin, base_solver.BaseSDESolver):
             return self._k('tsde_step_euler', L, nz, (y0, f, g), (c.dt,), out), ()
         # g_prod_and_gdg_prod_{diagonal,default}: vjp of g wrt y with grad_outputs g * (0.5 v)
         # base_sde.py:127-155 (always calls self.g, never g_prod)
-        if self._pw and self._feed.binding is not None:
+        if pointwise.ready(self):
             # f, g and the vjp were recorded as an element-wise program (pointwise.py): the whole step is one kernel
-            prog, _ = self._pw
-            out = out if out is not None else torch.empty_like(y0)
-            _cabi.check(self._lib.tsde_step_milstein_pointwise(self._L, self._feed.get(c), ctypes.byref(prog),
-                                                               y0.data_ptr(), c.t0.data_ptr(), c.dt, ito,
-                                                               out.data_ptr()), 'tsde_step_milstein_pointwise')
-            return out, ()
+            return pointwise.launch(self, 'tsde_step_milstein_pointwise', self._feed.get(c), y0,
+                                    (c.t0.data_ptr(), c.dt, ito), out), ()
         track = self._autograd
         # the first step of an eligible solve runs as always, with the user's ops recorded
-        rec = None
-        if self._pw is None and sde.noise_type == NOISE_TYPES.diagonal and pointwise.eligible(self):
-            rec = pointwise.Recorder(y0, c.t0)
+        rec = pointwise.Recorder(y0, c.t0) if pointwise.recording(self) else None
         raw = {}
 
         def user(name, fn, **kw):
@@ -352,7 +345,7 @@ class SRK(base_solver.BaseSDESolver):
     # -- user-supplied g_prod (srk.py:87,102,109 call sde.g_prod) -----------------------------------------------
     # The products are the user's own code, so the weights they are applied to have to exist as tensors: W and U are
     # materialised and the tableau arithmetic around the user's calls is a handful of element-wise torch ops in the
-    # order of the fused kernels (csrc/tableau_diag.cu SrkDiagFinalOp, tableau_general.cu GSra*Op).  Not a fast
+    # order of the fused kernels (csrc/tableau_diag_ops.cuh SrkDiagFinalOp, tableau_general.cu GSra*Op).  Not a fast
     # path — SDEs that want the fused one provide g — but the reference accepts it, so it has to work.
     def _weights(self, c):
         w, u = self._feed.tensors(c, True)
@@ -403,19 +396,13 @@ class SRK(base_solver.BaseSDESolver):
         sde, s = self.sde, c.scalars
         t_00, t_1, t_q, t_h = c.aux_t  # t0 + 0*dt, t0 + dt, t0 + dt/4, t0 + dt/2
         LU, L = self._LU, self._L
-        if self._pw and self._feed.binding is not None:
+        if pointwise.ready(self):
             # f and g were recorded as element-wise programs (pointwise.py): the whole step is one kernel
-            prog, _ = self._pw
-            out = out if out is not None else torch.empty_like(y0)
-            _cabi.check(self._lib.tsde_step_srk_diag_pointwise(
-                L, self._feed.get(c, True), ctypes.byref(prog), y0.data_ptr(), t_00.data_ptr(), t_1.data_ptr(),
-                t_q.data_ptr(), t_h.data_ptr(), c.dt, s['rdt'], s['sqrt_dt'], s['three_dt'], out.data_ptr()),
-                'tsde_step_srk_diag_pointwise')
-            return out
+            return pointwise.launch(self, 'tsde_step_srk_diag_pointwise', self._feed.get(c, True), y0,
+                                    (t_00.data_ptr(), t_1.data_ptr(), t_q.data_ptr(), t_h.data_ptr(), c.dt, s['rdt'],
+                                     s['sqrt_dt'], s['three_dt']), out)
         # the first step of an eligible solve runs as always, with the user's seven evaluations recorded
-        rec = None
-        if self._pw is None and sde.noise_type == NOISE_TYPES.diagonal and pointwise.eligible(self):
-            rec = pointwise.SrkRecorder(y0, t_00)
+        rec = pointwise.SrkRecorder(y0, t_00) if pointwise.recording(self) else None
 
         def f(t, y):
             return _contig(rec.evaluation('f', lambda: sde.f(t, y), t, y) if rec is not None else sde.f(t, y))

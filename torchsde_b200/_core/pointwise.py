@@ -1,34 +1,44 @@
 """Element-wise tapes of the user's SDE: a diagonal-noise Milstein or SRK step as one kernel.
 
-SRK (`SrkRecorder`) records the step's seven f / g evaluations with the same whitelist and rules as below and runs
-them in tsde_step_srk_diag_pointwise; the rest of this docstring describes the Milstein case.
+When the SDE's callables are made only of element-wise ATen ops whose CUDA result is one IEEE rounding per element,
+a whole step is one launch that reads y0 and writes y1 (include/torchsde_b200.h, csrc/pointwise.cu) instead of the
+user's ATen launches and the tableau kernels between them.  How the program is obtained: the first step of the solve
+runs the ordinary way under a recorder, a TorchDispatchMode that sees every ATen op that actually runs, and the tape
+is compiled (dead-code elimination, linear-scan register allocation) into a tsde_pointwise program that every later
+step runs.
 
-The unfused step runs five full-batch passes: the user's f and g, the vjp seed, autograd's vjp of g and the tableau
-(methods.BaseMilstein._step).  When f(t, y), g(t, y) and the vjp of g are made only of element-wise ATen ops whose
-CUDA result is one IEEE rounding per element, the whole step is one launch of tsde_step_milstein_pointwise, which
-reads y0 and writes y1 (include/torchsde_b200.h).
-
-How the program is obtained: one step runs the ordinary way under `Recorder`, a TorchDispatchMode that sees every
-ATen op that actually runs in three segments: f(t0, y), g(t0, y) and torch.autograd.grad(g, y, go).  The vjp is not
-derived symbolically: autograd's own op sequence (`grad * other`, the `add` that accumulates a twice-used `y`, ...)
-is what decides the bits, so it is what gets recorded.  The tape accepts only
+What a tape may hold, for both methods.  The tape accepts only
 
     mul; add / sub / rsub with alpha = +-1 (any other alpha lets ATen contract to an FMA); neg; sqrt;
     div by a tensor; div by a CPU scalar (ATen computes a * (1/b), with 1/b rounded in the state dtype);
     pow(x, 2) (ATen computes x * x); aliasing views that keep every element where it is (no-ops),
 
-on operands that are y, the step's 0-d time t0, go, Python numbers and CPU 0-d tensors (immediates, rounded to the
-state dtype as ATen rounds them), one-element device tensors, (d,)-shaped device tensors broadcast over the rows and
-(rows, d) device tensors, all of the state dtype, on y's device and contiguous.  Anything else — another op, a
-reduction, `.item()`, an in-place op on anything the tape did not produce, a read of a tensor whose storage was
-written in place through another tensor (a view, `detach()`, `.data`), an operand that shares storage with a value of
-the tape, a 16-bit result, a tensor created by a factory — rejects the tape, and the solve keeps its ordinary step.
+on operands that are the state y, the 0-d time t the callable was given, Python numbers and CPU 0-d tensors
+(immediates, rounded to the state dtype as ATen rounds them), one-element device tensors, (d,)-shaped device tensors
+broadcast over the rows and (rows, d) device tensors, all of the state dtype, on y's device and contiguous.  Anything
+else — another op, a reduction, `.item()`, an in-place op on anything the tape did not produce, a read of a tensor
+whose storage was written in place through another tensor (a view, `detach()`, `.data`), an operand that shares
+storage with a value of the tape, a 16-bit result, a tensor created by a factory — rejects the tape, and the solve
+keeps its ordinary step.
 
 Device operands are passed by address and read at every launch: in-place updates of parameters (optimiser steps) are
 followed, exactly as by a captured CUDA graph; f and g must not depend on anything else (the purity contract of
 graph capture, README).  SDEs whose callables have side effects say so with options={'overlap': False}, and keep
 calling them every step.
+
+Milstein (`Recorder`, tsde_step_milstein_pointwise).  The unfused step runs five full-batch passes: the user's f and
+g, the vjp seed, autograd's vjp of g and the tableau (methods.BaseMilstein._step).  The tape has three segments:
+f(t0, y), g(t0, y) and torch.autograd.grad(g, y, go), in which the seed go is one more operand.  The vjp is not
+derived symbolically: autograd's own op sequence (`grad * other`, the `add` that accumulates a twice-used `y`, ...)
+is what decides the bits, so it is what gets recorded.  The three segments are one program: the vjp part may read
+what the f / g part computed.
+
+SRK (`SrkRecorder`, tsde_step_srk_diag_pointwise).  The step's seven evaluations, f at three (t, y) and g at four
+(methods.SRK._diagonal_or_scalar_step), are recorded one by one; a value of one evaluation is not an operand of
+another.  The tape is accepted when the three f evaluations are the same ops on the same operands and so are the four
+g evaluations; the first of each is compiled, as two programs that share an operand table.
 """
+import ctypes
 import numbers
 
 import numpy as np
@@ -36,6 +46,7 @@ import torch
 from torch.utils._python_dispatch import TorchDispatchMode
 
 from .. import _cabi
+from ..settings import NOISE_TYPES
 
 aten = torch.ops.aten
 
@@ -70,6 +81,55 @@ def _strip(shape):
     return shape
 
 
+def _allocate(instrs, reads):
+    """Dead-code elimination and register allocation of one tape.  `instrs` are (opcode, value id, source, source);
+    `reads` are the (position, source) at which the kernel reads a result: after the instructions before `position`
+    have run, so the value is kept until then.  Returns the instructions that remain as (position in `instrs`, opcode, register, code, code), the
+    code of each read's source, and the number of registers."""
+    last = {}
+    for pos, v in reads:
+        if v[0] == 'v':
+            last[v] = max(last.get(v, -1), pos)
+    live = []
+    for i in range(len(instrs) - 1, -1, -1):
+        op, v, a, b = instrs[i]
+        if v not in last:
+            continue
+        live.append(i)
+        for s in (a, b):
+            if s is not None and s[0] == 'v':
+                last[s] = max(last.get(s, -1), i)
+    live.reverse()
+    # registers: linear scan; a register whose value was last read by this instruction may be its destination
+    reg, held, free, n_regs = {}, [], [], 0  # value -> its register; the values whose register is in use
+
+    def code(s):
+        if s == Y:
+            return _cabi.PW_SRC_Y
+        if s == GO:
+            return _cabi.PW_SRC_GO
+        if s[0] == 'k':
+            return _cabi.PW_OPERAND0 + s[1]
+        return reg[s]
+
+    out = []
+    for i in live:
+        op, v, a, b = instrs[i]
+        ca, cb = code(a), code(b) if b is not None else 0
+        # (the kernel reads both sources before it writes the destination)
+        for s in [s for s in held if last[s] <= i]:
+            held.remove(s)
+            free.append(reg[s])
+        if free:
+            reg[v] = free.pop()
+        else:
+            reg[v] = n_regs
+            n_regs += 1
+        held.append(v)
+        out.append((i, op, reg[v], ca, cb))
+    return out, [code(s) for _, s in reads], n_regs
+
+
 class Recorder(TorchDispatchMode):
     """Records the element-wise tape of one Milstein step; `finish` turns it into a tsde_pointwise program."""
 
@@ -87,23 +147,29 @@ class Recorder(TorchDispatchMode):
         self._by_addr = {}     # (data_ptr, shape, stride) -> source
         self._storage = {}     # id(tensor) / address key -> storage of every bound tensor
         self._shapes = {(), _strip((self.d,)), _strip((self.rows, self.d))}
-        self._vjp = False
-        self._bind(y, Y)
-        if t0.dtype == self.dtype and t0.device == self.device:  # (else an op on t0 rejects the tape)
-            self._bind(t0, T0)
+        self._at(y, t0)
+
+    def _at(self, y=None, t=None):
+        """From here on `y` is what the user's function calls the state and `t` the time."""
+        if y is not None:
+            self._bind(y, Y)
+        if t is not None and t.dtype == self.dtype and t.device == self.device:  # (else an op on t rejects the tape)
+            self._bind(t, T0)
+
+    def _run(self, fn, y=None, t=None):
+        """fn() at (t, y) with its ATen ops recorded."""
+        self._at(y, t)
+        with self:
+            return fn()
 
     # -- the three segments ---------------------------------------------------------------------------------------
     def segment(self, fn, y=None, go=None):
         """fn() with its ATen ops recorded.  `y` is the tensor the segment calls the state (a detached alias of the
         state for g), `go` the vjp seed (vjp segment)."""
-        if y is not None:
-            self._bind(y, Y)
         if go is not None:
             self._bind(go, GO)
-            self._vjp = True
             self.n_fg = len(self.instrs)
-        with self:
-            return fn()
+        return self._run(fn, y)
 
     def reject(self, reason):
         if self.ok:
@@ -243,6 +309,32 @@ class Recorder(TorchDispatchMode):
         self._emit(op, self._source(a), self._source(b), out)
 
     # -- the program -----------------------------------------------------------------------------------------------
+    def _step_result(self, t, allow_go=False):
+        """The source of `t`, a tensor the step takes as f, g or the vjp of g."""
+        if not torch.is_tensor(t) or tuple(t.shape) != (self.rows, self.d) or t.dtype != self.dtype:
+            raise Reject("a result is not a (rows, d) tensor of the state dtype")
+        src = self._source(t)
+        if src[0] == 'k' or src == GO and not allow_go:
+            raise Reject("a result is not computed from the state")
+        return src
+
+    def _program(self, code, n_fg, results, n_regs, max_regs):
+        """The tsde_pointwise of allocated instructions `code` (_allocate), of which the first `n_fg` come before the
+        boundary, with `results` (f_src, g_src, gdg_src) and the recorder's operand table; and the tensors it reads."""
+        if len(code) > _cabi.PW_MAX_INSTR or len(self.operands) > _cabi.PW_MAX_OPERANDS:
+            raise Reject("program too long")
+        if n_regs > max_regs:
+            raise Reject("too many live values")
+        prog = _cabi.Pointwise()
+        prog.n_instr, prog.n_fg, prog.n_regs, prog.n_operands = len(code), n_fg, n_regs, len(self.operands)
+        prog.f_src, prog.g_src, prog.gdg_src = results
+        for j, (_, op, dst, a, b) in enumerate(code):
+            ins = prog.instr[j]
+            ins.op, ins.dst, ins.a, ins.b = op, dst, a, b
+        for k, (kind, ptr, imm) in enumerate(self.operands):
+            prog.operand[k].kind, prog.operand[k].ptr, prog.operand[k].imm = kind, ptr, imm
+        return prog, tuple(t for t in self._keep if self._by_obj.get(id(t), 'k')[0] == 'k')
+
     def finish(self, f, g, gdg):
         """The tsde_pointwise program of the recorded step (and the tensors it reads), or None if it was rejected."""
         if self.ok and self.n_fg is None:
@@ -250,80 +342,15 @@ class Recorder(TorchDispatchMode):
         if not self.ok:
             return None
         try:
-            outs = []
-            for t, vjp in ((f, False), (g, False), (gdg, True)):
-                if not torch.is_tensor(t) or tuple(t.shape) != (self.rows, self.d) or t.dtype != self.dtype:
-                    raise Reject("a result is not a (rows, d) tensor of the state dtype")
-                src = self._source(t)
-                if src[0] == 'k' or src == GO and not vjp:
-                    raise Reject("a result is not computed from the state")
-                outs.append(src)
-            return self._compile(self.instrs, self.n_fg, *outs)
+            # the kernel reads f and g at the boundary, gdg at the end
+            reads = [(self.n_fg, self._step_result(f)), (self.n_fg, self._step_result(g)),
+                     (len(self.instrs), self._step_result(gdg, allow_go=True))]
+            code, results, n_regs = _allocate(self.instrs, reads)
+            n_fg = sum(1 for c in code if c[0] < self.n_fg)
+            return self._program(code, n_fg, results, n_regs, _cabi.PW_MAX_REGS)
         except Exception as e:
             self.reject(f"{type(e).__name__}: {e}")
             return None
-
-    def _compile(self, instrs, n_fg, f, g, gdg):
-        # dead-code elimination and last uses (the boundary reads f, g at n_fg, gdg at the end)
-        last = {}
-        for pos, v in ((n_fg, f), (n_fg, g), (len(instrs), gdg)):
-            if v[0] == 'v':
-                last[v] = max(last.get(v, -1), pos)
-        live = []
-        for i in range(len(instrs) - 1, -1, -1):
-            op, v, a, b = instrs[i]
-            if v not in last:
-                continue
-            live.append(i)
-            for s in (a, b):
-                if s is not None and s[0] == 'v':
-                    last[s] = max(last.get(s, -1), i)
-        live.reverse()
-        if len(live) > _cabi.PW_MAX_INSTR or len(self.operands) > _cabi.PW_MAX_OPERANDS:
-            raise Reject("program too long")
-        # registers: linear scan; a register whose value was last read by this instruction may be its destination
-        reg, free, n_regs = {}, [], 0
-        prog = _cabi.Pointwise()
-
-        def code(s):
-            if s == Y:
-                return _cabi.PW_SRC_Y
-            if s == GO:
-                return _cabi.PW_SRC_GO
-            if s[0] == 'k':
-                return _cabi.PW_OPERAND0 + s[1]
-            return reg[s]
-
-        new_fg = sum(1 for i in live if i < n_fg)
-        for j, i in enumerate(live):
-            op, v, a, b = instrs[i]
-            if j == new_fg:
-                prog.f_src, prog.g_src = code(f), code(g)
-            ins = prog.instr[j]
-            ins.op, ins.a = op, code(a)
-            ins.b = code(b) if b is not None else 0
-            # (the kernel reads both sources before it writes the destination)
-            for s in [s for s in reg if last[s] <= i]:
-                free.append(reg.pop(s))
-            if free:
-                reg[v] = free.pop()
-            else:
-                reg[v] = n_regs
-                n_regs += 1
-            ins.dst = reg[v]
-        if new_fg == len(live):
-            prog.f_src, prog.g_src = code(f), code(g)
-        prog.gdg_src = code(gdg)
-        if n_regs > _cabi.PW_MAX_REGS:
-            raise Reject("too many live values")
-        prog.n_instr, prog.n_fg, prog.n_regs, prog.n_operands = len(live), new_fg, n_regs, len(self.operands)
-        for k, (kind, ptr, imm) in enumerate(self.operands):
-            prog.operand[k].kind, prog.operand[k].ptr, prog.operand[k].imm = kind, ptr, imm
-        return prog, tuple(t for t in self._keep if self._is_operand(t))
-
-    def _is_operand(self, t):
-        src = self._by_obj.get(id(t))
-        return src is None or src[0] == 'k'
 
 
 class SrkRecorder(Recorder):
@@ -348,20 +375,11 @@ class SrkRecorder(Recorder):
                     self._storage.pop(key, None)
                 else:
                     table[key] = FOREIGN
-        self._bind(y, Y)
-        if t.dtype == self.dtype and t.device == self.device:
-            self._bind(t, T0)
         start = len(self.instrs)
-        with self:
-            out = fn()
+        out = self._run(fn, y, t)
         if self.ok:
             try:
-                if not torch.is_tensor(out) or tuple(out.shape) != (self.rows, self.d) or out.dtype != self.dtype:
-                    raise Reject("a result is not a (rows, d) tensor of the state dtype")
-                src = self._source(out)
-                if src[0] == 'k':
-                    raise Reject("a result is not computed from the state")
-                self.segments.append((kind, start, len(self.instrs), src))
+                self.segments.append((kind, start, len(self.instrs), self._step_result(out)))
             except Exception as e:
                 self.reject(f"{type(e).__name__}: {e}")
         return out
@@ -385,33 +403,41 @@ class SrkRecorder(Recorder):
         try:
             if [s[0] for s in self.segments] != list('fgfgfgg'):
                 raise Reject("not the seven evaluations of an SRK step")
-            progs = []
+            parts = []
             for kind in 'fg':
                 segs = [s for s in self.segments if s[0] == kind]
                 tapes = [self._tape(*s[1:]) for s in segs]
                 if any(tp != tapes[0] for tp in tapes[1:]):
                     raise Reject(f"the {kind} evaluations differ")
+                # each program starts with no register defined; its result is read when it ends
                 _, start, end, src = segs[0]
-                instrs = self.instrs[start:end]
-                progs.append(self._compile(instrs, len(instrs), src, src, src)[0])
-            pf, pg = progs
-            if pf.n_instr + pg.n_instr > _cabi.PW_MAX_INSTR:
-                raise Reject("program too long")
-            prog = _cabi.Pointwise()
-            for j in range(pf.n_instr):
-                prog.instr[j] = pf.instr[j]
-            for j in range(pg.n_instr):
-                prog.instr[pf.n_instr + j] = pg.instr[j]
-            prog.n_instr, prog.n_fg = pf.n_instr + pg.n_instr, pf.n_instr
-            prog.n_regs = max(pf.n_regs, pg.n_regs)
-            if prog.n_regs > _cabi.PW_SRK_MAX_REGS:
-                raise Reject("too many live values")
-            prog.f_src, prog.g_src, prog.n_operands = pf.f_src, pg.g_src, pf.n_operands
-            prog.operand = pf.operand
-            return prog, tuple(t for t in self._keep if self._is_operand(t))
+                parts.append(_allocate(self.instrs[start:end], [(end - start, src)]))
+            (code_f, (f_src,), regs_f), (code_g, (g_src,), regs_g) = parts
+            return self._program(code_f + code_g, len(code_f), (f_src, g_src, 0), max(regs_f, regs_g),
+                                 _cabi.PW_SRK_MAX_REGS)
         except Exception as e:
             self.reject(f"{type(e).__name__}: {e}")
             return None
+
+
+def recording(solver):
+    """Whether this step of `solver` (its `_pw` is the program, None before the first step, False once rejected)
+    is the one to record."""
+    return solver._pw is None and solver.sde.noise_type == NOISE_TYPES.diagonal and eligible(solver)
+
+
+def ready(solver):
+    """Whether `solver` has a program and the counter noise its kernel draws from."""
+    return bool(solver._pw) and solver._feed.binding is not None
+
+
+def launch(solver, name, nz, y0, args, out):
+    """One step y0 -> out of the library's whole-step function `name` on the solver's program."""
+    prog, _ = solver._pw
+    out = out if out is not None else torch.empty_like(y0)
+    fn = getattr(solver._lib, name)
+    _cabi.check(fn(solver._L, nz, ctypes.byref(prog), y0.data_ptr(), *args, out.data_ptr()), name)
+    return out
 
 
 def eligible(solver):

@@ -573,6 +573,23 @@ inline int fill_noise(const tsde_launch* L, const tsde_noise* nz, bool bcast, No
   return 0;
 }
 
+// How a flat quad index maps to (row, quad of the row) over (rows, d): the d, qpr, nquads, qshift, small and qmagic
+// members of a kernel parameter struct (EwP, and the whole-step kernels of pointwise.cu).
+template <typename P>
+inline void fill_quad_map(int64_t rows, int64_t d, P& p) {
+  p.d = d;
+  p.qpr = (d + 3) / 4;
+  p.nquads = rows * p.qpr;
+  p.qshift = -1;
+  if ((p.qpr & (p.qpr - 1)) == 0 && p.qpr < (1ll << 30)) {
+    int sh = 0;
+    while ((1ll << sh) < p.qpr) ++sh;
+    p.qshift = sh;
+  }
+  p.small = p.nquads < (1ll << 31) ? 1 : 0;
+  p.qmagic = p.qshift < 0 ? rowdiv_magic((uint64_t)p.qpr) : 0;
+}
+
 template <typename T, typename Op>
 inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
                      const void* const* ins, void* const* outs, const Op& op) {
@@ -602,18 +619,8 @@ inline int launch_ew(const tsde_launch* L, const tsde_noise* nz, bool bcast,
     if (L->noise_type == TSDE_NOISE_DIAGONAL && L->m != L->d) return TSDE_EINVAL;
   }
   p.rows = L->rows;
-  p.d = L->d;
-  p.qpr = (L->d + 3) / 4;
-  p.nquads = p.rows * p.qpr;
   p.vec = vec ? 1 : 0;
-  p.qshift = -1;
-  if ((p.qpr & (p.qpr - 1)) == 0 && p.qpr < (1ll << 30)) {
-    int sh = 0;
-    while ((1ll << sh) < p.qpr) ++sh;
-    p.qshift = sh;
-  }
-  p.small = p.nquads < (1ll << 31) ? 1 : 0;
-  p.qmagic = p.qshift < 0 ? rowdiv_magic((uint64_t)p.qpr) : 0;
+  fill_quad_map(L->rows, L->d, p);
   // (every quads-per-row divides exactly on the fast path: its quad indices are 32-bit, see rowdiv.cuh)
   const bool fast = p.vec && !bcast && p.small && np.n_cells == 1 &&
                     (L->rows + (nz ? nz->row_offset : 0)) < kMaxGlobalRows;

@@ -1,0 +1,445 @@
+// Whole steps of an element-wise SDE as one kernel: tsde_step_milstein_pointwise and tsde_step_srk_diag_pointwise
+// (include/torchsde_b200.h describes the tsde_pointwise program and its two layouts).
+//
+// The SDE's f and g (and for Milstein the vjp of g) arrive as a small program of element-wise instructions.  Each
+// kernel interprets it between the unfused step's own ops (tableau_diag_ops.cuh), one IEEE rounding per element
+// (this translation unit is compiled with -fmad=false, as the tableaus are), so a fused step equals the unfused one
+// bit for bit.  The file holds, in this order: the program's register file and interpreter, the validation every
+// program passes before a launch, the prologue both kernels share, the two kernels with the layout each accepts,
+// and the launch.
+//
+// One thread per quad, as ew_fast_kernel.  The program's registers live in shared memory as 16-byte vectors laid
+// out [reg][plane][thread] (a float quad is one plane, a double quad two): a warp's 128-bit access is 512 contiguous
+// bytes, conflict-free.  A dynamically indexed per-thread array would live in local memory instead.  The state, go,
+// the SDE's results and the increments stay in registers.
+#include "tableau_diag_ops.cuh"
+
+namespace tsde {
+
+template <typename T>
+struct PwP {
+  const T* y0;
+  T* y1;
+  const T* t0;
+  int64_t d, qpr, nquads;
+  uint64_t qmagic;  // rowdiv_magic(qpr) when qpr is not a power of two
+  int32_t qshift;   // log2(qpr), or -1
+  int32_t small;    // nquads < 2^31
+  int32_t vec;      // d % 4 == 0 and every tensor 16-byte aligned
+  T dt;
+  int32_t ito;
+};
+
+// ---- the interpreter ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void pw_sload(const void* s, int r, float (&v)[4]) {
+  const float4 x = static_cast<const float4*>(s)[r * kThreads + threadIdx.x];
+  v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
+}
+__device__ __forceinline__ void pw_sstore(void* s, int r, const float (&v)[4]) {
+  static_cast<float4*>(s)[r * kThreads + threadIdx.x] = make_float4(v[0], v[1], v[2], v[3]);
+}
+__device__ __forceinline__ void pw_sload(const void* s, int r, double (&v)[4]) {
+  const double2* p = static_cast<const double2*>(s) + 2 * r * kThreads + threadIdx.x;
+  const double2 a = p[0], b = p[kThreads];
+  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
+}
+__device__ __forceinline__ void pw_sstore(void* s, int r, const double (&v)[4]) {
+  double2* p = static_cast<double2*>(s) + 2 * r * kThreads + threadIdx.x;
+  p[0] = make_double2(v[0], v[1]);
+  p[kThreads] = make_double2(v[2], v[3]);
+}
+
+template <typename T>
+struct PwQuad {  // where this thread's quad lives, and the values a program source may name besides registers
+  int64_t base, chan;
+  int nvalid;
+  bool vec;
+  const T* t;  // what a TSDE_PW_T0 operand reads: the time of the evaluation being run
+  T y[4], go[4];
+};
+
+template <typename T>
+__device__ __forceinline__ void pw_fetch(const tsde_pointwise& pg, const PwQuad<T>& c, const void* regs, uint32_t s,
+                                         T (&v)[4]) {
+  if (s == TSDE_PW_SRC_Y || s == TSDE_PW_SRC_GO) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[j] = s == TSDE_PW_SRC_Y ? c.y[j] : c.go[j];
+    return;
+  }
+  if (s < (uint32_t)TSDE_PW_OPERAND(0)) {
+    pw_sload(regs, (int)s, v);
+    return;
+  }
+  const tsde_pw_operand& o = pg.operand[s - TSDE_PW_OPERAND(0)];
+  if (o.kind == TSDE_PW_CHANNEL || o.kind == TSDE_PW_ROW) {
+    load_quad(static_cast<const T*>(o.ptr), o.kind == TSDE_PW_ROW ? c.base : c.chan, c.vec, c.nvalid, v);
+    return;
+  }
+  const T x = o.kind == TSDE_PW_IMM ? (T)o.imm : *(o.kind == TSDE_PW_T0 ? c.t : static_cast<const T*>(o.ptr));
+#pragma unroll
+  for (int j = 0; j < 4; ++j) v[j] = x;
+}
+
+// instructions [i0, i1): one warp-uniform dispatch per instruction, one IEEE rounding per element (-fmad=false)
+template <typename T>
+__device__ __forceinline__ void pw_run(const tsde_pointwise& pg, const PwQuad<T>& c, void* regs, int i0, int i1) {
+  for (int i = i0; i < i1; ++i) {
+    const tsde_pw_instr in = pg.instr[i];
+    T a[4], b[4], r[4];
+    pw_fetch(pg, c, regs, in.a, a);
+    if (in.op != TSDE_PW_NEG && in.op != TSDE_PW_SQRT) pw_fetch(pg, c, regs, in.b, b);
+    switch (in.op) {
+      case TSDE_PW_MUL:
+#pragma unroll
+        for (int j = 0; j < 4; ++j) r[j] = a[j] * b[j];
+        break;
+      case TSDE_PW_ADD:
+#pragma unroll
+        for (int j = 0; j < 4; ++j) r[j] = a[j] + b[j];
+        break;
+      case TSDE_PW_SUB:
+#pragma unroll
+        for (int j = 0; j < 4; ++j) r[j] = a[j] - b[j];
+        break;
+      case TSDE_PW_DIV:
+#pragma unroll
+        for (int j = 0; j < 4; ++j) r[j] = a[j] / b[j];
+        break;
+      case TSDE_PW_NEG:
+#pragma unroll
+        for (int j = 0; j < 4; ++j) r[j] = -a[j];
+        break;
+      default:  // TSDE_PW_SQRT
+#pragma unroll
+        for (int j = 0; j < 4; ++j) r[j] = sqrt(a[j]);
+        break;
+    }
+    pw_sstore(regs, in.dst, r);
+  }
+}
+
+// ---- validation -----------------------------------------------------------------------------------------------------
+// A program the kernels can run as given: counts, register and operand indices in range, every register written
+// before it is read, device operands present (and 16-byte aligned for the vector path).  This is all that stands
+// between a caller's program and an out-of-range shared-memory index.  The parts common to both layouts are here;
+// which instructions and results may read what is spelt out per layout, beside the kernel that reads them so.
+
+// the counts and the operand table; clears *vec when a device operand is not 16-byte aligned
+static bool pw_valid_tables(const tsde_pointwise& pg, bool* vec) {
+  if (pg.n_instr < 0 || pg.n_instr > TSDE_PW_MAX_INSTR || pg.n_fg < 0 || pg.n_fg > pg.n_instr ||
+      pg.n_regs < 0 || pg.n_regs > TSDE_PW_MAX_REGS || pg.n_operands < 0 || pg.n_operands > TSDE_PW_MAX_OPERANDS)
+    return false;
+  for (int k = 0; k < pg.n_operands; ++k) {
+    const tsde_pw_operand& o = pg.operand[k];
+    if (o.kind < TSDE_PW_IMM || o.kind > TSDE_PW_ROW) return false;
+    if (o.kind >= TSDE_PW_SCALAR && !o.ptr) return false;
+    if (o.kind >= TSDE_PW_CHANNEL) *vec = *vec && aligned16(o.ptr);
+  }
+  return true;
+}
+
+// a source that can be read when the registers in `written` are defined
+static bool pw_valid_source(const tsde_pointwise& pg, uint32_t s, bool allow_go, uint64_t written) {
+  if (s == TSDE_PW_SRC_Y) return true;
+  if (s == TSDE_PW_SRC_GO) return allow_go;
+  if (s >= (uint32_t)TSDE_PW_OPERAND(0)) return (int)(s - TSDE_PW_OPERAND(0)) < pg.n_operands;
+  return (int)s < pg.n_regs && ((written >> s) & 1u);
+}
+
+// instructions [i0, i1), run in order from the registers in `written`, which gains the ones they define
+static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, bool allow_go, uint64_t& written) {
+  for (int i = i0; i < i1; ++i) {
+    const tsde_pw_instr& in = pg.instr[i];
+    if (in.op > TSDE_PW_SQRT || (int)in.dst >= pg.n_regs || !pw_valid_source(pg, in.a, allow_go, written)) return false;
+    if (in.op != TSDE_PW_NEG && in.op != TSDE_PW_SQRT && !pw_valid_source(pg, in.b, allow_go, written)) return false;
+    written |= 1ull << in.dst;
+  }
+  return true;
+}
+
+// ---- what both kernels start with -----------------------------------------------------------------------------------
+// This thread's quad (`c`, but for the state it is evaluated at), its increments and its y0.  The increments depend on
+// no predecessor: they are drawn while the previous kernel drains (programmatic dependent launch), and y0 is read
+// after the dependency wait.  False for a thread past the last quad.
+template <typename T, int SRC, bool WANT_U>
+__device__ __forceinline__ bool pw_begin(const PwP<T>& p, const NoiseP<T>& nz, PwQuad<T>& c, T (&w)[4], T (&u)[4],
+                                         T (&y0)[4]) {
+  const int64_t Q = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+  int64_t row, q;
+  if (p.qshift >= 0) {
+    row = Q >> p.qshift;
+    q = Q & ((1ll << p.qshift) - 1);
+  } else if (p.small) {
+    const uint32_t r32 = rowdiv_row((uint32_t)Q, p.qmagic);
+    row = r32;
+    q = (int64_t)rowdiv_quad((uint32_t)Q, r32, (uint32_t)p.qpr);
+  } else {
+    row = Q / p.qpr;
+    q = Q - row * p.qpr;
+  }
+  c.chan = 4 * q;
+  c.base = row * p.d + c.chan;
+  const int64_t rem = p.d - c.chan;
+  c.nvalid = rem < 4 ? (int)rem : 4;
+  c.vec = p.vec != 0;
+  quad_noise<T, SRC, WANT_U>(nz, load_key(nz.key), row, q, c.vec, c.nvalid, w, u);
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (Q >= p.nquads) return false;
+  load_quad(p.y0, c.base, c.vec, c.nvalid, y0);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) c.go[j] = T(0);
+  return true;
+}
+
+// ---- a whole Milstein step (tsde_step_milstein_pointwise) -----------------------------------------------------------
+// The program's f / g part runs on y0, MilsteinSeedOp forms go, the vjp part runs and MilsteinOp writes y1.  Only y0
+// and y1 (and the program's device operands) touch memory: 2 tensors per step instead of the 13 of the unfused step.
+template <typename T, int SRC>
+__global__ void __launch_bounds__(kThreads)
+pw_milstein_kernel(const __grid_constant__ tsde_pointwise pg, const PwP<T> p, const NoiseP<T> nz) {
+  extern __shared__ __align__(16) unsigned char pw_regs[];
+  PwQuad<T> c;
+  T w[4], u[4];
+  if (!pw_begin<T, SRC, false>(p, nz, c, w, u, c.y)) return;
+  c.t = p.t0;
+  pw_run(pg, c, pw_regs, 0, pg.n_fg);
+  T f[4], g[4];
+  pw_fetch(pg, c, pw_regs, pg.f_src, f);
+  pw_fetch(pg, c, pw_regs, pg.g_src, g);
+  const MilsteinSeedOp<T> seed{p.dt, p.ito};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[1];
+    seed({g[j]}, w[j], u[j], o);
+    c.go[j] = o[0];
+  }
+  pw_run(pg, c, pw_regs, pg.n_fg, pg.n_instr);
+  T gdg[4], y1[4];
+  pw_fetch(pg, c, pw_regs, pg.gdg_src, gdg);
+  const MilsteinOp<T> step{p.dt};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[1];
+    step({c.y[j], f[j], g[j], gdg[j]}, w[j], u[j], o);
+    y1[j] = o[0];
+  }
+  store_quad(p.y1, c.base, c.vec, c.nvalid, y1);
+}
+
+// The Milstein layout, in the order the kernel reads it: go exists from the vjp part on, registers carry over.
+static bool pw_valid_milstein(const tsde_pointwise& pg) {
+  uint64_t written = 0;
+  return pw_valid_range(pg, 0, pg.n_fg, false, written) &&
+         pw_valid_source(pg, pg.f_src, false, written) && pw_valid_source(pg, pg.g_src, false, written) &&
+         pw_valid_range(pg, pg.n_fg, pg.n_instr, true, written) && pw_valid_source(pg, pg.gdg_src, true, written);
+}
+
+// ---- a whole SRK step (tsde_step_srk_diag_pointwise) ----------------------------------------------------------------
+// W and U are drawn, y0 is read, and the seven SDE evaluations (the f program at three (t, y), the g program at four)
+// alternate with the unfused step's own stage ops.  y0 and y1 are the only tensors the step moves, against 22 reads
+// and 6 writes of the unfused step (41 with f and g).
+//
+// At the last update ten quads are live (y0, f0..f2, g0..g3, W, U).  In fp64 that is 80 registers before the
+// interpreter's own, so there f0..f2 and g0..g2 wait in the shared-memory register file, in the kPwSrkStash slots
+// past the program's registers; in fp32 they stay in registers.
+constexpr int kPwSrkStash = TSDE_PW_MAX_REGS - TSDE_PW_SRK_MAX_REGS;  // six: f0..f2, g0..g2
+
+template <typename T>
+struct PwSrkP {
+  PwP<T> base;    // y0, y1, the quad mapping; base.t0 unused
+  const T* t[4];  // t_0, t_1, t_q, t_h
+  SrkDiagStage1Op<T> s1;
+  SrkDiagStage2Op<T> s2;
+  SrkDiagStage3Op<T> s3;
+  SrkDiagFinalOp<T> fin;
+};
+
+template <typename T>
+struct PwSrkStash {
+  static constexpr bool kShared = sizeof(T) == 8;
+  T r[kShared ? 1 : kPwSrkStash][4];
+  int slot0;  // first shared-memory register past the program's
+  __device__ __forceinline__ void put(void* regs, int k, const T (&x)[4]) {
+    if constexpr (kShared) {
+      pw_sstore(regs, slot0 + k, x);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) r[k][j] = x[j];
+    }
+  }
+  __device__ __forceinline__ void get(const void* regs, int k, T (&x)[4]) const {
+    if constexpr (kShared) {
+      pw_sload(regs, slot0 + k, x);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) x[j] = r[k][j];
+    }
+  }
+};
+
+// f (program [0, n_fg), result f_src) or g (program [n_fg, n_instr), result g_src) at (t, y)
+template <typename T>
+__device__ __forceinline__ void pw_srk_eval(const tsde_pointwise& pg, PwQuad<T>& c, void* regs, bool g, const T* t,
+                                            const T (&y)[4], T (&out)[4]) {
+  c.t = t;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) c.y[j] = y[j];
+  pw_run(pg, c, regs, g ? pg.n_fg : 0, g ? pg.n_instr : pg.n_fg);
+  pw_fetch(pg, c, regs, g ? pg.g_src : pg.f_src, out);
+}
+
+template <typename T, int SRC>
+__global__ void __launch_bounds__(kThreads)
+pw_srk_kernel(const __grid_constant__ tsde_pointwise pg, const PwSrkP<T> p, const NoiseP<T> nz) {
+  extern __shared__ __align__(16) unsigned char pw_regs[];
+  PwQuad<T> c;
+  T w[4], u[4], y0[4];
+  if (!pw_begin<T, SRC, true>(p.base, nz, c, w, u, y0)) return;
+  PwSrkStash<T> st;
+  st.slot0 = pg.n_regs;
+  enum { F0, F1, F2, G0, G1, G2 };
+  T f[4], g[4], h0[4], h1[4], x[4], z[4];
+  // s = 0: f0, g0 at (t0, y0); H0_1, H1_1
+  pw_srk_eval(pg, c, pw_regs, false, p.t[0], y0, f);
+  pw_srk_eval(pg, c, pw_regs, true, p.t[0], y0, g);
+  st.put(pw_regs, F0, f);
+  st.put(pw_regs, G0, g);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[2];
+    p.s1({y0[j], f[j], g[j]}, w[j], u[j], o);
+    h0[j] = o[0];
+    h1[j] = o[1];
+  }
+  // s = 1: f1 at (t0 + dt, H0_1), g1 at (t0 + dt/4, H1_1); H0_2, H1_2
+  pw_srk_eval(pg, c, pw_regs, false, p.t[1], h0, f);
+  pw_srk_eval(pg, c, pw_regs, true, p.t[2], h1, g);
+  st.put(pw_regs, F1, f);
+  st.put(pw_regs, G1, g);
+  st.get(pw_regs, F0, x);
+  st.get(pw_regs, G0, z);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[2];
+    p.s2({y0[j], x[j], z[j], f[j], g[j]}, w[j], u[j], o);
+    h0[j] = o[0];
+    h1[j] = o[1];
+  }
+  // s = 2: f2 at (t0 + dt/2, H0_2), g2 at (t0 + dt, H1_2); H1_3
+  pw_srk_eval(pg, c, pw_regs, false, p.t[3], h0, f);
+  pw_srk_eval(pg, c, pw_regs, true, p.t[1], h1, g);
+  st.put(pw_regs, F2, f);
+  st.put(pw_regs, G2, g);
+  st.get(pw_regs, G0, x);
+  st.get(pw_regs, G1, z);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[1];
+    p.s3({y0[j], x[j], z[j], f[j], g[j]}, w[j], u[j], o);
+    h1[j] = o[0];
+  }
+  // s = 3: g3 at (t0 + dt/4, H1_3); y1
+  pw_srk_eval(pg, c, pw_regs, true, p.t[2], h1, g);
+  T f0[4], f1[4], f2[4], g0[4], g1[4], g2[4], y1[4];
+  st.get(pw_regs, F0, f0);
+  st.get(pw_regs, F1, f1);
+  st.get(pw_regs, F2, f2);
+  st.get(pw_regs, G0, g0);
+  st.get(pw_regs, G1, g1);
+  st.get(pw_regs, G2, g2);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[1];
+    p.fin({y0[j], f0[j], f1[j], f2[j], g0[j], g1[j], g2[j], g[j]}, w[j], u[j], o);
+    y1[j] = o[0];
+  }
+  store_quad(p.base.y1, c.base, c.vec, c.nvalid, y1);
+}
+
+// The SRK layout: an f program and a g program that each start with no register defined; go is never a source, and
+// the registers past TSDE_PW_SRK_MAX_REGS are the kernel's stash.
+static bool pw_valid_srk(const tsde_pointwise& pg) {
+  if (pg.n_regs > TSDE_PW_SRK_MAX_REGS) return false;
+  uint64_t written = 0;
+  if (!pw_valid_range(pg, 0, pg.n_fg, false, written) || !pw_valid_source(pg, pg.f_src, false, written)) return false;
+  written = 0;
+  return pw_valid_range(pg, pg.n_fg, pg.n_instr, false, written) && pw_valid_source(pg, pg.g_src, false, written);
+}
+
+// ---- launch ---------------------------------------------------------------------------------------------------------
+// The noise and the part of the kernel parameters every pointwise step has (y0, y1, the quad mapping, vec) for a
+// program that passes `layout`; TSDE_EINVAL for a launch the kernels cannot serve.
+template <typename T>
+static int pw_prepare(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
+                      void* y1, bool (*layout)(const tsde_pointwise&), PwP<T>& p, NoiseP<T>& np) {
+  if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !prog || !y0 || !y1) return TSDE_EINVAL;
+  bool vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y1);
+  if (!pw_valid_tables(*prog, &vec) || !layout(*prog)) return TSDE_EINVAL;
+  if (int e = fill_noise<T>(L, nz, false, np)) return e;
+  p = PwP<T>{};
+  p.y0 = static_cast<const T*>(y0);
+  p.y1 = static_cast<T*>(y1);
+  fill_quad_map(L->rows, L->d, p);
+  p.vec = vec ? 1 : 0;
+  return 0;
+}
+
+// One thread per quad, `slots` shared-memory registers per thread; `single` draws from one Brownian cell, `multi` sums
+// the cells of a step that spans several.
+template <typename T, typename P>
+static int pw_launch(const tsde_launch* L, const tsde_pointwise& prog, void (*single)(tsde_pointwise, P, NoiseP<T>),
+                     void (*multi)(tsde_pointwise, P, NoiseP<T>), const P& p, const NoiseP<T>& np, int64_t nquads,
+                     int slots, int family) {
+  const size_t smem = (size_t)slots * kThreads * 4 * sizeof(T);
+  auto kernel = np.n_cells > 1 ? multi : single;
+  if (resident_ctas(reinterpret_cast<const void*>(kernel), kThreads, smem) < 1) return TSDE_EINVAL;
+  const int64_t grid = (nquads + kThreads - 1) / kThreads;
+  const int e = launch_kernel(kernel, grid, kThreads, smem, reinterpret_cast<cudaStream_t>(L->stream), true, prog, p,
+                              np);
+  if (e == 0) g_launches[family].fetch_add(1, std::memory_order_relaxed);
+  return e;
+}
+
+}  // namespace tsde
+
+using namespace tsde;
+
+TSDE_EXPORT int tsde_step_milstein_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                             const void* y0, const void* t0, double dt, int32_t ito, void* y1) {
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
+  return dispatch(L, [&](auto t) -> int {
+    using T = decltype(t);
+    if (!t0) return TSDE_EINVAL;
+    PwP<T> p;
+    NoiseP<T> np;
+    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_milstein, p, np)) return e;
+    p.t0 = static_cast<const T*>(t0);
+    p.dt = (T)dt;
+    p.ito = ito;
+    return pw_launch<T>(L, *prog, pw_milstein_kernel<T, TSDE_SRC_COUNTER>, pw_milstein_kernel<T, kSrcCounterMulti>, p,
+                        np, p.nquads, prog->n_regs, TSDE_KERNEL_PW_MILSTEIN);
+  });
+}
+
+TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                             const void* y0, const void* t_0, const void* t_1, const void* t_q,
+                                             const void* t_h, double dt, double rdt, double sqrt_dt, double three_dt,
+                                             void* y1) {
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
+  return dispatch(L, [&](auto t) -> int {
+    using T = decltype(t);
+    if (!t_0 || !t_1 || !t_q || !t_h) return TSDE_EINVAL;
+    PwSrkP<T> p;
+    NoiseP<T> np;
+    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_srk, p.base, np)) return e;
+    const void* times[4] = {t_0, t_1, t_q, t_h};
+    for (int i = 0; i < 4; ++i) p.t[i] = static_cast<const T*>(times[i]);
+    // the coefficients of tsde_srk_diag_stage1/2/3 and tsde_step_srk_diag
+    p.s1 = SrkDiagStage1Op<T>{(T)dt, (T)sqrt_dt};
+    p.s2 = SrkDiagStage2Op<T>{(T)dt, (T)rdt, (T)sqrt_dt};
+    p.s3 = SrkDiagStage3Op<T>{(T)dt, (T)sqrt_dt};
+    p.fin = make_srk_final<T>(dt, rdt, sqrt_dt, three_dt);
+    return pw_launch<T>(L, *prog, pw_srk_kernel<T, TSDE_SRC_COUNTER>, pw_srk_kernel<T, kSrcCounterMulti>, p, np,
+                        p.base.nquads, prog->n_regs + (PwSrkStash<T>::kShared ? kPwSrkStash : 0), TSDE_KERNEL_PW_SRK);
+  });
+}
