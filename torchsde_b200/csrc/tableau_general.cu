@@ -3,15 +3,20 @@
 // The batched matrix-vector product of the reference (`misc.batch_mvp` = torch.bmm(g, v[...,None]),
 // torchsde/_core/misc.py:62-63, reached through base_sde.py:101-102) is fused with the tableau's
 // element-wise combination: g — the only large operand, used exactly once (0.5 flop/byte, HBM
-// bound; tensor cores cannot help, SURVEY.md fact 5) — is streamed with fully coalesced 128-bit
-// loads, lanes run along the contiguous (d,m) axis, the m/4 lanes that hold one (row,d) output
-// reduce their partial dot products with warp shuffles, and one of them applies the tableau.
-// The Brownian increments of the block's rows are produced once per block (Philox, or a load
-// of the user's tensor) into shared memory, so they are not regenerated d times.
+// bound; tensor cores cannot help, SURVEY.md fact 5) — is streamed once, and the Brownian
+// increments of the rows a CTA owns are produced once (Philox, or a load of the user's tensor)
+// into shared memory, so they are not regenerated d times.  `launch_gen` picks the kernel by shape:
+//   * m / 4 a power of two <= 32, every g quad-aligned (memory noise: W / U 16-byte aligned):
+//     gen_tma_kernel (TMA-staged, persistent) for 32/64-bit operands at m = 64, or m = 16 with one
+//     g operand, when d is a power of two, g is not batch-broadcast and the batch fills its
+//     pipeline; gen_cta_kernel (one 128-thread CTA per 32 / (m/4) rows, 128-bit loads) otherwise.
+//   * every other shape whose row of increments fits in 40 KiB of shared memory: gen_kernel, one
+//     thread per (row, d) output walking its m-run of g;
+//   * rows wider than that: gen_wide_kernel, one CTA per row walking m in chunks.
 //
-// Summation order: within a 4-chunk left to right, chunks combined by a fixed xor-tree; results
-// are bitwise reproducible and independent of batch sharding, and agree with torch.bmm to
-// rounding (bmm's own order is unspecified), which is how the parity tests treat them.
+// Summation order: fixed per kernel (see each kernel) and independent of batch sharding, so results
+// are bitwise reproducible; they agree with torch.bmm to rounding (bmm's own order is
+// unspecified), which is how the parity tests treat them.
 #include <atomic>
 #include <type_traits>
 
@@ -27,9 +32,9 @@ struct GenP {
   const void* g[NG];
   void* o[NO];
   int64_t rows, d, m;
-  int32_t mq;    // m / 4 (vector path)
+  int32_t mq;    // m / 4 (gen_cta_kernel)
   int32_t rb;    // rows per block
-  int32_t vec;   // vector path usable
+  int32_t vec;   // m % 4 == 0 and every g aligned for quad loads (gen_wide_kernel)
   int32_t gbcast;  // every g operand is ONE (d, m) block shared by all rows (row stride 0): additive noise whose
                    // diffusion does not depend on y, returned as `sigma.expand(B, d, m)`.  Nothing of size
                    // (rows, d, m) exists then; the block (d*m*s bytes, KiBs) is served from L1/L2.
@@ -40,10 +45,62 @@ struct GenP {
 //   T gval(int p, const T (&g)[NG]) const;      value contracted in product p
 //   T weight(int p, T w, T u) const;            weight of product p for this Brownian channel
 //   void combine(const T (&e)[NE], const T (&gp)[NP], T (&o)[NO]) const;
+
+// ---- pieces the kernels share --------------------------------------------------------------------------------------
+// Quad q of row `row` of the increments (W, and U when WANT_U) -> shared memory at sw / su + r * m + 4 * q, one 128-bit
+// store per tensor: drawn on the channel-quad counters (MULTI: merging nz.n_cells primary cells when there are several)
+// or, for memory noise, one 128-bit load of the user's (rows, m) tensors.
+template <bool WANT_U, int SRC, bool MULTI, typename T>
+__device__ __forceinline__ void stage_quad(const NoiseP<T>& nz, Key key, int64_t row, int m, int r, int q, T* sw,
+                                           T* su) {
+  T w[4], u[4];
+  if (SRC == TSDE_SRC_MEMORY) {
+    const int64_t base = row * m + 4 * q;
+    ld4(nz.w + base, w);
+    if (WANT_U) ld4(nz.u + base, u);
+  } else {
+    counter_noise<T, WANT_U, MULTI>(nz, key, (uint32_t)(row + nz.row_offset), (uint32_t)q, w, u);
+  }
+  st4(sw + r * m + 4 * q, w);
+  if (WANT_U) st4(su + r * m + 4 * q, u);
+}
+
+// The element-wise operands at eoff (Mixed<Op>: raw bits, converted by widen_e).
+template <typename T, typename Op, int N>
+__device__ __forceinline__ void load_e(const GenP<Op::NE, Op::NG, Op::NO>& p, const Op& op, int64_t eoff,
+                                       T (&e)[N]) {
+#pragma unroll
+  for (int i = 0; i < Op::NE; ++i) {
+    if constexpr (is_mixed<Op>::value) e[i] = __uint_as_float(ld1raw(p.e[i], eoff, operand_fmt(op.fmt, i)));
+    else e[i] = reinterpret_cast<const T*>(p.e[i])[eoff];
+  }
+}
+template <typename Op, int N>
+__device__ __forceinline__ void widen_e(const Op& op, float (&e)[N]) {
+#pragma unroll
+  for (int i = 0; i < Op::NE; ++i) e[i] = widen1(__float_as_uint(e[i]), operand_fmt(op.fmt, i));
+}
+
+// Epilogue of one (row, d) output: its element-wise operands at eoff, the tableau on the contracted products gp, the
+// outputs stored at eoff.
+template <typename T, typename Op, int NP>
+__device__ __forceinline__ void epilogue(const GenP<Op::NE, Op::NG, Op::NO>& p, const Op& op, int64_t eoff,
+                                         const T (&gp)[NP]) {
+  T e[Op::NE > 0 ? Op::NE : 1], o[Op::NO];
+  load_e(p, op, eoff, e);
+  if constexpr (is_mixed<Op>::value) widen_e(op, e);
+  op.combine(e, gp, o);
+#pragma unroll
+  for (int i = 0; i < Op::NO; ++i) reinterpret_cast<T*>(p.o[i])[eoff] = o[i];
+}
+
+// ---- generic path: any m, any alignment ----------------------------------------------------------------------------
+// rb rows per CTA.  Their increments are staged in shared memory element by element (row r at r * m, for any m); then
+// one thread per (row, d) output walks its m-run of g left to right, one separately rounded multiply-add per channel.
 template <typename T, typename Op, int SRC>
 __global__ void __launch_bounds__(kThreads)
 gen_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const Op op) {
-  constexpr int NE = Op::NE, NG = Op::NG, NP = Op::NP, NO = Op::NO;
+  constexpr int NE = Op::NE, NG = Op::NG, NP = Op::NP;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   T* sw = reinterpret_cast<T*>(smem_raw);
   T* su = sw + (size_t)p.rb * p.m;
@@ -83,111 +140,32 @@ gen_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const Op op
   __syncthreads();
 
   // ---- phase 2: stream g, contract, combine ----------------------------------------------------
-  if (p.vec) {
-    const int mq = p.mq;
-    const int64_t per_row = d * mq;
-    const int64_t total = (int64_t)nrows * per_row;
-    const int64_t total_pad = (total + 31) & ~(int64_t)31;
-    for (int64_t c = threadIdx.x; c < total_pad; c += kThreads) {
-      const bool valid = c < total;
-      const int64_t cc = valid ? c : 0;
-      const int r = (int)(cc / per_row);
-      const int64_t rem = cc - (int64_t)r * per_row;
-      const int64_t dd = rem / mq;
-      const int mc = (int)(rem - dd * mq);
-      const int64_t goff = ((p.gbcast ? 0 : (row0 + r) * d) + dd) * m + 4 * mc;
-      T gv[NG][4];
-      uint4 graw[NG];  // (Mixed: every g load issued before the first widening)
+  const int64_t total = (int64_t)nrows * d;
+  for (int64_t c = threadIdx.x; c < total; c += kThreads) {
+    const int r = (int)(c / d);
+    const int64_t dd = c - (int64_t)r * d;
+    const int64_t goff = ((p.gbcast ? 0 : (row0 + r) * d) + dd) * m;
+    T part[NP];
+#pragma unroll
+    for (int k = 0; k < NP; ++k) part[k] = T(0);
+    for (int64_t mm = 0; mm < m; ++mm) {
+      const T w = sw[r * m + mm];
+      const T u = Op::WANT_U ? su[r * m + mm] : T(0);
+      T gj[NG];
 #pragma unroll
       for (int i = 0; i < NG; ++i) {
-        if (valid) {
-          if constexpr (is_mixed<Op>::value) graw[i] = ld4raw<false>(p.g[i], goff, operand_fmt(op.fmt, NE + i));
-          else ld4(reinterpret_cast<const T*>(p.g[i]) + goff, gv[i]);
-        } else {
-          graw[i] = make_uint4(0u, 0u, 0u, 0u);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) gv[i][j] = T(0);
-        }
+        if constexpr (is_mixed<Op>::value)
+          gj[i] = __uint_as_float(ld1raw(p.g[i], goff + mm, operand_fmt(op.fmt, NE + i)));
+        else gj[i] = reinterpret_cast<const T*>(p.g[i])[goff + mm];
       }
       if constexpr (is_mixed<Op>::value) {
 #pragma unroll
-        for (int i = 0; i < NG; ++i) widen4(graw[i], operand_fmt(op.fmt, NE + i), gv[i]);
+        for (int i = 0; i < NG; ++i) gj[i] = widen1(__float_as_uint(gj[i]), operand_fmt(op.fmt, NE + i));
       }
-      T part[NP];
 #pragma unroll
-      for (int k = 0; k < NP; ++k) part[k] = T(0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const T w = sw[r * m + 4 * mc + j];
-        const T u = Op::WANT_U ? su[r * m + 4 * mc + j] : T(0);
-        T gj[NG];
-#pragma unroll
-        for (int i = 0; i < NG; ++i) gj[i] = gv[i][j];
-#pragma unroll
-        for (int k = 0; k < NP; ++k) part[k] = part[k] + op.gval(k, gj) * op.weight(k, w, u);
-      }
-      for (int off = 1; off < mq; off <<= 1) {
-#pragma unroll
-        for (int k = 0; k < NP; ++k) part[k] = part[k] + __shfl_xor_sync(0xffffffffu, part[k], off);
-      }
-      if (valid && mc == 0) {
-        const int64_t eoff = (row0 + r) * d + dd;
-        T e[NE > 0 ? NE : 1], o[NO];
-#pragma unroll
-        for (int i = 0; i < NE; ++i) {
-          if constexpr (is_mixed<Op>::value) e[i] = __uint_as_float(ld1raw(p.e[i], eoff, operand_fmt(op.fmt, i)));
-          else e[i] = reinterpret_cast<const T*>(p.e[i])[eoff];
-        }
-        if constexpr (is_mixed<Op>::value) {
-#pragma unroll
-          for (int i = 0; i < NE; ++i) e[i] = widen1(__float_as_uint(e[i]), operand_fmt(op.fmt, i));
-        }
-        op.combine(e, part, o);
-#pragma unroll
-        for (int i = 0; i < NO; ++i) reinterpret_cast<T*>(p.o[i])[eoff] = o[i];
-      }
+      for (int k = 0; k < NP; ++k) part[k] = part[k] + op.gval(k, gj) * op.weight(k, w, u);
     }
-  } else {
-    const int64_t total = (int64_t)nrows * d;
-    for (int64_t c = threadIdx.x; c < total; c += kThreads) {
-      const int r = (int)(c / d);
-      const int64_t dd = c - (int64_t)r * d;
-      const int64_t goff = ((p.gbcast ? 0 : (row0 + r) * d) + dd) * m;
-      T part[NP];
-#pragma unroll
-      for (int k = 0; k < NP; ++k) part[k] = T(0);
-      for (int64_t mm = 0; mm < m; ++mm) {
-        const T w = sw[r * m + mm];
-        const T u = Op::WANT_U ? su[r * m + mm] : T(0);
-        T gj[NG];
-#pragma unroll
-        for (int i = 0; i < NG; ++i) {
-          if constexpr (is_mixed<Op>::value)
-            gj[i] = __uint_as_float(ld1raw(p.g[i], goff + mm, operand_fmt(op.fmt, NE + i)));
-          else gj[i] = reinterpret_cast<const T*>(p.g[i])[goff + mm];
-        }
-        if constexpr (is_mixed<Op>::value) {
-#pragma unroll
-          for (int i = 0; i < NG; ++i) gj[i] = widen1(__float_as_uint(gj[i]), operand_fmt(op.fmt, NE + i));
-        }
-#pragma unroll
-        for (int k = 0; k < NP; ++k) part[k] = part[k] + op.gval(k, gj) * op.weight(k, w, u);
-      }
-      const int64_t eoff = (row0 + r) * d + dd;
-      T e[NE > 0 ? NE : 1], o[NO];
-#pragma unroll
-      for (int i = 0; i < NE; ++i) {
-        if constexpr (is_mixed<Op>::value) e[i] = __uint_as_float(ld1raw(p.e[i], eoff, operand_fmt(op.fmt, i)));
-        else e[i] = reinterpret_cast<const T*>(p.e[i])[eoff];
-      }
-      if constexpr (is_mixed<Op>::value) {
-#pragma unroll
-        for (int i = 0; i < NE; ++i) e[i] = widen1(__float_as_uint(e[i]), operand_fmt(op.fmt, i));
-      }
-      op.combine(e, part, o);
-#pragma unroll
-      for (int i = 0; i < NO; ++i) reinterpret_cast<T*>(p.o[i])[eoff] = o[i];
-    }
+    epilogue(p, op, (row0 + r) * d + dd, part);
   }
 }
 
@@ -222,16 +200,7 @@ gen_cta_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const O
     Key key{0u, 0u};
     if (SRC == TSDE_SRC_COUNTER) key = load_key(nz.key);
     const int r = tid >> mq_shift, q = tid & (mq - 1);
-    T w[4], u[4];
-    if (SRC == TSDE_SRC_COUNTER) {
-      counter_noise<T, Op::WANT_U>(nz, key, (uint32_t)(row0 + r + nz.row_offset), (uint32_t)q, w, u);
-    } else {
-      const int64_t base = (row0 + r) * m + 4 * q;
-      ld4(nz.w + base, w);
-      if (Op::WANT_U) ld4(nz.u + base, u);
-    }
-    st4(sw + r * m + 4 * q, w);
-    if (Op::WANT_U) st4(su + r * m + 4 * q, u);
+    stage_quad<Op::WANT_U, SRC, true>(nz, key, row0 + r, m, r, q, sw, su);
   }
   if (SRC != TSDE_SRC_MEMORY) asm volatile("griddepcontrol.wait;" ::: "memory");
   // Streaming sweep over the group's g tile (contiguous: element offset = tile0 + 4 * chunk).
@@ -263,14 +232,7 @@ gen_cta_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const O
       // element offset of this chunk inside a g operand: contiguous tile, or — batch-broadcast g — the chunk's
       // position inside the one shared (d, m) block
       const int64_t goff = p.gbcast ? (int64_t)4 * (dd * mq + mc) : tile0 + 4 * (int64_t)c;
-      if (valid[un] && mc == 0) {
-#pragma unroll
-        for (int i = 0; i < NE; ++i) {
-          if constexpr (is_mixed<Op>::value)
-            ev[un][i] = __uint_as_float(ld1raw(p.e[i], slot0 + slot, operand_fmt(op.fmt, i)));
-          else ev[un][i] = reinterpret_cast<const T*>(p.e[i])[slot0 + slot];
-        }
-      }
+      if (valid[un] && mc == 0) load_e(p, op, slot0 + slot, ev[un]);
 #pragma unroll
       for (int i = 0; i < NG; ++i) {
         if (valid[un]) {
@@ -299,8 +261,7 @@ gen_cta_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const O
       for (int un = 0; un < kGenUnroll; ++un) {
 #pragma unroll
         for (int i = 0; i < NG; ++i) widen4(graw[un][i], operand_fmt(op.fmt, NE + i), gv[un][i]);
-#pragma unroll
-        for (int i = 0; i < NE; ++i) ev[un][i] = widen1(__float_as_uint(ev[un][i]), operand_fmt(op.fmt, i));
+        widen_e(op, ev[un]);
       }
     }
 #pragma unroll
@@ -512,16 +473,7 @@ gen_tma_kernel(const GenP<Op::NE, Op::NG, Op::NO> p, const NoiseP<T> nz, const O
       T* sub = reinterpret_cast<T*>(sp + u_off);
       for (int i = lane; i < nr * mq; i += 32) {  // one Philox quad per lane and pass
         const int r = i >> mq_shift, q = i & (mq - 1);
-        const int64_t row = t * rs + r;
-        T w[4], u[4];
-        if (SRC == TSDE_SRC_COUNTER) {
-          counter_noise<T, Op::WANT_U>(nz, key, (uint32_t)(row + nz.row_offset), (uint32_t)q, w, u);
-        } else {
-          ld4(nz.w + row * m + 4 * q, w);
-          if (Op::WANT_U) ld4(nz.u + row * m + 4 * q, u);
-        }
-        st4(swb + r * m + 4 * q, w);
-        if (Op::WANT_U) st4(sub + r * m + 4 * q, u);
+        stage_quad<Op::WANT_U, SRC, true>(nz, key, t * rs + r, m, r, q, swb, sub);
       }
       __syncwarp();
       if (lane == 0) mbar_arrive(&full[s]);  // increments written (ordered by __syncwarp; arrive releases)
@@ -847,7 +799,7 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
   if (nz->source != TSDE_SRC_MEMORY && nz->source != TSDE_SRC_COUNTER)
     return TSDE_EINVAL;  // (a user-supplied product, TSDE_SRC_UNIT, goes through the element-wise entry points)
   GenP<Op::NE, Op::NG, Op::NO> p{};
-  bool vec = (L->m % 4) == 0;
+  bool vec = (L->m % 4) == 0;  // and every g aligned for quad loads: p.vec
   uint32_t fmt = 0;
   if constexpr (is_mixed<Op>::value) fmt = op.fmt;
   int i = 0;
@@ -858,21 +810,21 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
     vec = vec && aligned_for(q, operand_fmt(fmt, Op::NE + i));
     p.g[i++] = q;
   }
-  const bool gvec = vec;  // m % 4 == 0 and every g aligned for quad loads (gen_wide_kernel)
   i = 0;
   for (void* q : os) { if (!q) return TSDE_EINVAL; p.o[i++] = q; }
   NoiseP<T> np;
   if (int e = fill_noise<T>(L, nz, false, np)) return e;
   const int64_t mq = L->m / 4;
-  vec = vec && mq >= 1 && mq <= 32 && (mq & (mq - 1)) == 0;
-  if (nz->source == TSDE_SRC_MEMORY) vec = vec && aligned16(np.w) && (!Op::WANT_U || aligned16(np.u));
+  const bool mem = nz->source == TSDE_SRC_MEMORY;
+  // the tile kernels: m / 4 a power of two <= 32, g and (memory noise) W / U loadable as quads
+  const bool tile = vec && mq >= 1 && mq <= 32 && (mq & (mq - 1)) == 0 &&
+                    (!mem || (aligned16(np.w) && (!Op::WANT_U || aligned16(np.u))));
   p.rows = L->rows; p.d = L->d; p.m = L->m;
   p.mq = (int32_t)mq;
   p.vec = vec ? 1 : 0;
   p.gbcast = (nz->flags & TSDE_FLAG_G_BROADCAST) ? 1 : 0;
-  const bool mem = nz->source == TSDE_SRC_MEMORY;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(L->stream);
-  if (vec) {
+  if (tile) {
     // (a broadcast g has no tile stream to stage; 16-bit operands are not staged by the TMA kernel)
     if constexpr (!is_mixed<Op>::value) {
       if (!p.gbcast && tma_route<Op>(mq)) {
@@ -899,7 +851,6 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
   while (rb > 1 && rb * smem_per_row > 40 * 1024) rb >>= 1;
   if (rb * smem_per_row > 40 * 1024) {  // not even one row's increments fit: walk m in chunks, one CTA per row
     if (L->rows > 0x7fffffffll) return TSDE_EINVAL;
-    p.vec = gvec ? 1 : 0;
     p.rb = 1;
     const int64_t outs = L->d < kWideOutputs ? L->d : kWideOutputs;
     const size_t smem = ((Op::WANT_U ? 2 : 1) * (size_t)(kWideChunkBytes / sizeof(T)) + Op::NP * (size_t)outs) * sizeof(T);
