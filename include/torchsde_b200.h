@@ -130,6 +130,8 @@ const char* tsde_error_string(int code);
 #define TSDE_KERNEL_GEN_WIDE 2 /* chunked tile kernel for rows whose increments exceed shared memory */
 #define TSDE_KERNEL_PW_MILSTEIN 3 /* whole Milstein step with an element-wise SDE (tsde_step_milstein_pointwise) */
 #define TSDE_KERNEL_PW_SRK 4      /* whole SRK step with an element-wise SDE (tsde_step_srk_diag_pointwise)     */
+#define TSDE_KERNEL_PW_PC 5       /* whole Heun / midpoint / Euler-Heun step with an element-wise SDE
+                                     (tsde_step_predictor_corrector_pointwise)                                  */
 int64_t tsde_kernel_launches(int32_t family);
 
 /* ------------------------------------------------------------------------ */
@@ -313,6 +315,29 @@ int tsde_step_milstein_pointwise(const tsde_launch* L, const tsde_noise* nz, con
 int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
                                  const void* y0, const void* t_0, const void* t_1, const void* t_q,
                                  const void* t_h, double dt, double rdt, double sqrt_dt, double three_dt, void* y1);
+
+/*
+ * A whole diagonal-noise Stratonovich predictor-corrector step for an SDE whose f(t, y) and g(t, y) are element-wise
+ * programs: one launch reads y0, draws dW, evaluates f0 = f(t0, y0) and g0 = g(t0, y0), and then, by `method`,
+ *     TSDE_PC_HEUN        y' as tsde_step_euler (dt);         f', g' at (t_p, y'); y1 as tsde_step_heun (dt)
+ *                         (heun.py:40-46, t_p = t1)
+ *     TSDE_PC_MIDPOINT    y' as tsde_midpoint_predict (half_dt); f', g' at (t_p, y'); y1 as tsde_step_euler on
+ *                         (y0, f', g') (dt)  (midpoint.py:34-43, t_p = t0 + half_dt)
+ *     TSDE_PC_EULER_HEUN  y' as tsde_euler_heun_predict;       g' at (t_p, y');      y1 as tsde_step_euler_heun (dt)
+ *                         (euler_heun.py:34-40, t_p = t1)
+ * in registers and writes y1.  t0 and t_p are 0-d device times (state dtype), read at every launch; dt and half_dt
+ * are the scalars the unfused kernels take (half_dt is read by TSDE_PC_MIDPOINT only).  The step equals the unfused
+ * one bit for bit.
+ *
+ * Program: the two-program layout of tsde_step_srk_diag_pointwise (f in [0, n_fg), g in [n_fg, n_instr), gdg_src
+ * unused, the operand table shared, TSDE_PW_SRC_GO not a source), with n_regs <= TSDE_PW_MAX_REGS.
+ * Requires DIAGONAL noise, counter noise (nz->source == TSDE_SRC_COUNTER) and no 16-bit formats.  An unknown
+ * `method` or a null time is TSDE_EINVAL.
+ */
+enum { TSDE_PC_HEUN = 0, TSDE_PC_MIDPOINT = 1, TSDE_PC_EULER_HEUN = 2 };
+int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                            const void* y0, const void* t0, const void* t_p, int32_t method,
+                                            double dt, double half_dt, void* y1);
 
 /* derivative-free Milstein, predictor: y' = y0 + (Ito ? dt*f : 0) + g*sqrt_dt
  * methods/milstein.py:58-63,83-84,93-94.  g is (rows,d) also for scalar noise (squeezed). */

@@ -53,6 +53,8 @@ PW_IMM, PW_T0, PW_SCALAR, PW_CHANNEL, PW_ROW = range(5)
 PW_SRK_MAX_REGS = 18  # TSDE_PW_SRK_MAX_REGS
 KERNEL_PW_MILSTEIN = 3  # TSDE_KERNEL_PW_MILSTEIN
 KERNEL_PW_SRK = 4  # TSDE_KERNEL_PW_SRK
+KERNEL_PW_PC = 5  # TSDE_KERNEL_PW_PC
+PC_HEUN, PC_MIDPOINT, PC_EULER_HEUN = range(3)  # TSDE_PC_*
 
 
 class PwInstr(ctypes.Structure):
@@ -94,6 +96,7 @@ SIGNATURES = {
     'tsde_step_milstein': [_L, _N, _P, _P, _P, _P, _D, _P],
     'tsde_step_milstein_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _D, _I, _P],
     'tsde_step_srk_diag_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _P, _P, _P, _D, _D, _D, _D, _P],
+    'tsde_step_predictor_corrector_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _P, _I, _D, _D, _P],
     'tsde_milstein_gf_predict': [_L, _P, _P, _P, _D, _D, _I, _P],
     'tsde_step_milstein_gf': [_L, _N, _P, _P, _P, _P, _D, _D, _I, _P],
     'tsde_step_heun': [_L, _N, _P, _P, _P, _P, _P, _D, _P],

@@ -48,14 +48,18 @@ class _WidenedSDE:
 class _ProdMixin:
     """Shared handling of the reference's `f_and_g_prod` / `g_prod` call sites (base_sde.py:51-56)."""
 
-    def _f_and_g_prod(self, c, t, y):
+    def _f_and_g_prod(self, c, t, y, rec=None):
         """Evaluate drift and diffusion at (t, y) the way ForwardSDE.f_and_g_prod would.  Returns
         (L, nz, f, g) where (L, nz, g) is either (noise-type launch, step noise, g) or
-        (element-wise launch, unit noise, user-computed g_prod)."""
+        (element-wise launch, unit noise, user-computed g_prod).  `rec` (pointwise.pc_recorder) records f and g."""
         sde = self.sde
         mode = sde.f_and_g_prod_mode
         if mode == 'fused':
-            f, g = self._f_and_g(t, y)
+            if rec is not None:
+                f, g = self._fork(lambda: rec.evaluation('f', lambda: sde.f(t, y), t, y),
+                                  lambda: rec.evaluation('g', lambda: sde.g(t, y), t, y))
+            else:
+                f, g = self._f_and_g(t, y)
             return self._L, self._feed.get(c, self.want_u), _contig(f), _gop(g)
         w, _ = self._feed.tensors(c)
         w = w.reshape(self.bm.shape)
@@ -65,10 +69,11 @@ class _ProdMixin:
             f, gp = sde.f(t, y), sde.g_prod(t, y, w)
         return self._LU, self._feed.unit(), _contig(f), _contig(gp)
 
-    def _g_prod(self, c, t, y):
+    def _g_prod(self, c, t, y, rec=None):
         sde = self.sde
         if sde.g_prod_mode == 'fused':
-            return self._L, self._feed.get(c, self.want_u), _gop(sde.g(t, y))
+            g = rec.evaluation('g', lambda: sde.g(t, y), t, y) if rec is not None else sde.g(t, y)
+            return self._L, self._feed.get(c, self.want_u), _gop(g)
         w, _ = self._feed.tensors(c)
         return self._LU, self._feed.unit(), _contig(sde.g_prod(t, y, w.reshape(self.bm.shape)))
 
@@ -202,11 +207,20 @@ class Heun(_ProdMixin, base_solver.BaseSDESolver):
     def __init__(self, sde, **kwargs):
         self.strong_order = 0.5 if sde.noise_type == NOISE_TYPES.general else 1.0
         super(Heun, self).__init__(sde=sde, **kwargs)
+        self._pw = None  # the element-wise programs of the step (pointwise.py), False once rejected
 
     def _step(self, c, y0, extra0, out):
-        L, nz, f, g = self._f_and_g_prod(c, c.t0, y0)
+        if pointwise.ready(self):
+            # f and g were recorded as element-wise programs (pointwise.py): the whole step is one kernel
+            return pointwise.launch(self, 'tsde_step_predictor_corrector_pointwise', self._feed.get(c), y0,
+                                    (c.t0.data_ptr(), c.t1.data_ptr(), _cabi.PC_HEUN, c.dt, 0.0), out), ()
+        # the first step of an eligible solve runs as always, with the user's four evaluations recorded
+        rec = pointwise.pc_recorder(self, y0, c.t0, 'fgfg')
+        L, nz, f, g = self._f_and_g_prod(c, c.t0, y0, rec)
         yp = self._k('tsde_step_euler', L, nz, (y0, f, g), (c.dt,), None)
-        L, nz, fp, gp = self._f_and_g_prod(c, c.t1, yp)
+        L, nz, fp, gp = self._f_and_g_prod(c, c.t1, yp, rec)
+        if rec is not None:
+            self._pw = rec.finish() or False
         return self._k('tsde_step_heun', L, nz, (y0, f, fp, g, gp), (c.dt,), out), ()
 
 
@@ -220,6 +234,7 @@ class Midpoint(_ProdMixin, base_solver.BaseSDESolver):
     def __init__(self, sde, **kwargs):
         self.strong_order = 0.5 if sde.noise_type == NOISE_TYPES.general else 1.0
         super(Midpoint, self).__init__(sde=sde, **kwargs)
+        self._pw = None  # the element-wise programs of the step (pointwise.py), False once rejected
 
     def aux_times(self, t0, t1, dt):
         return [t0 + 0.5 * dt]  # t_prime = t0 + half_dt, midpoint.py:35-37
@@ -228,9 +243,18 @@ class Midpoint(_ProdMixin, base_solver.BaseSDESolver):
         return {'half_dt': float(0.5 * dt)}
 
     def _step(self, c, y0, extra0, out):
-        L, nz, f, g = self._f_and_g_prod(c, c.t0, y0)
+        if pointwise.ready(self):
+            # f and g were recorded as element-wise programs (pointwise.py): the whole step is one kernel
+            return pointwise.launch(self, 'tsde_step_predictor_corrector_pointwise', self._feed.get(c), y0,
+                                    (c.t0.data_ptr(), c.aux_t[0].data_ptr(), _cabi.PC_MIDPOINT, c.dt,
+                                     c.scalars['half_dt']), out), ()
+        # the first step of an eligible solve runs as always, with the user's four evaluations recorded
+        rec = pointwise.pc_recorder(self, y0, c.t0, 'fgfg')
+        L, nz, f, g = self._f_and_g_prod(c, c.t0, y0, rec)
         yp = self._k('tsde_midpoint_predict', L, nz, (y0, f, g), (c.scalars['half_dt'],), None)
-        L, nz, fp, gp = self._f_and_g_prod(c, c.aux_t[0], yp)
+        L, nz, fp, gp = self._f_and_g_prod(c, c.aux_t[0], yp, rec)
+        if rec is not None:
+            self._pw = rec.finish() or False
         return self._k('tsde_step_euler', L, nz, (y0, fp, gp), (c.dt,), out), ()
 
 
@@ -244,10 +268,17 @@ class EulerHeun(_ProdMixin, base_solver.BaseSDESolver):
     def __init__(self, sde, **kwargs):
         self.strong_order = 0.5 if sde.noise_type == NOISE_TYPES.general else 1.0
         super(EulerHeun, self).__init__(sde=sde, **kwargs)
+        self._pw = None  # the element-wise programs of the step (pointwise.py), False once rejected
 
     def _step(self, c, y0, extra0, out):
         sde = self.sde
-        L, nz, f, g = self._f_and_g_prod(c, c.t0, y0)
+        if pointwise.ready(self):
+            # f and g were recorded as element-wise programs (pointwise.py): the whole step is one kernel
+            return pointwise.launch(self, 'tsde_step_predictor_corrector_pointwise', self._feed.get(c), y0,
+                                    (c.t0.data_ptr(), c.t1.data_ptr(), _cabi.PC_EULER_HEUN, c.dt, 0.0), out), ()
+        # the first step of an eligible solve runs as always, with the user's three evaluations recorded
+        rec = pointwise.pc_recorder(self, y0, c.t0, 'fgg')
+        L, nz, f, g = self._f_and_g_prod(c, c.t0, y0, rec)
         unit = L is self._LU
         yp = self._k('tsde_euler_heun_predict', L, nz, (y0, g), (), None)
         if unit:
@@ -270,7 +301,9 @@ class EulerHeun(_ProdMixin, base_solver.BaseSDESolver):
                              None)
             L2, nz2, gp = self._LU, self._feed.unit(), _contig(gp)
         else:
-            L2, nz2, gp = self._g_prod(c, c.t1, yp)
+            L2, nz2, gp = self._g_prod(c, c.t1, yp, rec)
+        if rec is not None:
+            self._pw = rec.finish() or False
         return self._k('tsde_step_euler_heun', L2, nz2, (y0, f, g, gp), (c.dt,), out), ()
 
 

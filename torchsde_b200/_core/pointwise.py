@@ -1,4 +1,5 @@
-"""Element-wise tapes of the user's SDE: a diagonal-noise Milstein or SRK step as one kernel.
+"""Element-wise tapes of the user's SDE: a diagonal-noise Milstein, SRK, Heun, midpoint or Euler-Heun step as one
+kernel.
 
 When the SDE's callables are made only of element-wise ATen ops whose CUDA result is one IEEE rounding per element,
 a whole step is one launch that reads y0 and writes y1 (include/torchsde_b200.h, csrc/pointwise.cu) instead of the
@@ -37,6 +38,12 @@ SRK (`SrkRecorder`, tsde_step_srk_diag_pointwise).  The step's seven evaluations
 (methods.SRK._diagonal_or_scalar_step), are recorded one by one; a value of one evaluation is not an operand of
 another.  The tape is accepted when the three f evaluations are the same ops on the same operands and so are the four
 g evaluations; the first of each is compiled, as two programs that share an operand table.
+
+Heun, midpoint and Euler-Heun (`SrkRecorder` with pattern 'fgfg' or 'fgg', tsde_step_predictor_corrector_pointwise).
+The Stratonovich predictor-corrector steps (methods.Heun, Midpoint, EulerHeun) evaluate f and g at (t0, y0) and again
+at the predicted state (g only for Euler-Heun).  They are recorded and compiled as SRK's are, with the full register
+bound.  Only SDEs whose f and g the step calls as two separate callables are recorded (`pc_recorder`): a user
+`f_and_g`, `g_prod` or `f_and_g_prod`, and the adjoint SDE of `sdeint_adjoint`'s backward, keep the ordinary step.
 """
 import ctypes
 import numbers
@@ -353,15 +360,22 @@ class Recorder(TorchDispatchMode):
             return None
 
 
-class SrkRecorder(Recorder):
-    """Records the seven SDE evaluations of one diagonal-noise SRK step (methods.SRK._diagonal_or_scalar_step): f at
-    three (t, y), g at four.  Each is a segment of its own, with its own state and 0-d time.  `finish` accepts the
-    tape when the three f segments are one program (same ops, operands and order) and so are the four g segments,
-    and compiles the first of each into the two-program layout of tsde_step_srk_diag_pointwise.  A Python-side
-    branch between evaluations (or any other difference) therefore keeps the ordinary step."""
+_COUNT = 'zero one two three four five six seven'.split()
 
-    def __init__(self, y, t):
+
+class SrkRecorder(Recorder):
+    """Records the SDE evaluations of one step whose kernel takes an f program and a g program: by default the seven
+    of a diagonal-noise SRK step (methods.SRK._diagonal_or_scalar_step), f at three (t, y), g at four; `pattern`
+    names another step's evaluations in order ('fgfg' for Heun and midpoint, 'fgg' for Euler-Heun) and `max_regs`
+    its kernel's register bound.  Each evaluation is a segment of its own, with its own state and 0-d time.  `finish`
+    accepts the tape when the f segments are one program (same ops, operands and order) and so are the g segments,
+    and compiles the first of each into the two-program layout of tsde_step_srk_diag_pointwise and
+    tsde_step_predictor_corrector_pointwise.  A Python-side branch between evaluations (or any other difference)
+    therefore keeps the ordinary step."""
+
+    def __init__(self, y, t, pattern='fgfgfgg', max_regs=_cabi.PW_SRK_MAX_REGS):
         super().__init__(y, t)
+        self.pattern, self.max_regs = pattern, max_regs
         self.segments = []  # (kind, first instruction, end, result source)
 
     def evaluation(self, kind, fn, t, y):
@@ -401,8 +415,8 @@ class SrkRecorder(Recorder):
         if not self.ok:
             return None
         try:
-            if [s[0] for s in self.segments] != list('fgfgfgg'):
-                raise Reject("not the seven evaluations of an SRK step")
+            if ''.join(s[0] for s in self.segments) != self.pattern:
+                raise Reject(f"not the {_COUNT[len(self.pattern)]} evaluations {self.pattern!r} of the step")
             parts = []
             for kind in 'fg':
                 segs = [s for s in self.segments if s[0] == kind]
@@ -413,8 +427,7 @@ class SrkRecorder(Recorder):
                 _, start, end, src = segs[0]
                 parts.append(_allocate(self.instrs[start:end], [(end - start, src)]))
             (code_f, (f_src,), regs_f), (code_g, (g_src,), regs_g) = parts
-            return self._program(code_f + code_g, len(code_f), (f_src, g_src, 0), max(regs_f, regs_g),
-                                 _cabi.PW_SRK_MAX_REGS)
+            return self._program(code_f + code_g, len(code_f), (f_src, g_src, 0), max(regs_f, regs_g), self.max_regs)
         except Exception as e:
             self.reject(f"{type(e).__name__}: {e}")
             return None
@@ -424,6 +437,17 @@ def recording(solver):
     """Whether this step of `solver` (its `_pw` is the program, None before the first step, False once rejected)
     is the one to record."""
     return solver._pw is None and solver.sde.noise_type == NOISE_TYPES.diagonal and eligible(solver)
+
+
+def pc_recorder(solver, y, t, pattern):
+    """The recorder of this step of a Heun, midpoint or Euler-Heun `solver` (evaluations `pattern`), or None when it
+    is not the one to record.  Only an SDE whose f and g the step calls as the user's two callables is recorded: not
+    one with a user f_and_g (one call yields both), g_prod or f_and_g_prod, and not an adjoint SDE."""
+    sde = solver.sde
+    if (not recording(solver) or sde.f_and_g_prod_mode != 'fused' or sde.g_prod_mode != 'fused'
+            or getattr(sde, 'user_f_and_g', True) or getattr(sde, 'is_adjoint_sde', False)):
+        return None
+    return SrkRecorder(y, t, pattern, _cabi.PW_MAX_REGS)
 
 
 def ready(solver):
@@ -441,7 +465,9 @@ def launch(solver, name, nz, y0, args, out):
 
 
 def eligible(solver):
-    """Whether a fixed-step Milstein or SRK solve may run its diagonal-noise steps as element-wise programs."""
+    """Whether a fixed-step Milstein, SRK, Heun, midpoint or Euler-Heun solve may run its diagonal-noise steps as
+    element-wise programs: no gradients, a Brownian motion bound to the solver grid (counter noise), `overlap` not
+    False, no logqp and no autocast."""
     from .base_sde import SDELogqp
     sde = solver.sde
     obj = sde

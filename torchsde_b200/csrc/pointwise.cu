@@ -1,12 +1,13 @@
-// Whole steps of an element-wise SDE as one kernel: tsde_step_milstein_pointwise and tsde_step_srk_diag_pointwise
-// (include/torchsde_b200.h describes the tsde_pointwise program and its two layouts).
+// Whole steps of an element-wise SDE as one kernel: tsde_step_milstein_pointwise, tsde_step_srk_diag_pointwise and
+// tsde_step_predictor_corrector_pointwise (include/torchsde_b200.h describes the tsde_pointwise program and its two
+// layouts).
 //
 // The SDE's f and g (and for Milstein the vjp of g) arrive as a small program of element-wise instructions.  Each
 // kernel interprets it between the unfused step's own ops (tableau_diag_ops.cuh), one IEEE rounding per element
 // (this translation unit is compiled with -fmad=false, as the tableaus are), so a fused step equals the unfused one
 // bit for bit.  The file holds, in this order: the program's register file and interpreter, the validation every
-// program passes before a launch, the prologue both kernels share, the two kernels with the layout each accepts,
-// and the launch.
+// program passes before a launch, the prologue the kernels share, the kernels with the layout each accepts, and the
+// launch.
 //
 // One thread per quad, as ew_fast_kernel.  The program's registers live in shared memory as 16-byte vectors laid
 // out [reg][plane][thread] (a float quad is one plane, a double quad two): a warp's 128-bit access is 512 contiguous
@@ -157,7 +158,7 @@ static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, bool allow_
   return true;
 }
 
-// ---- what both kernels start with -----------------------------------------------------------------------------------
+// ---- what every kernel starts with ----------------------------------------------------------------------------------
 // This thread's quad (`c`, but for the state it is evaluated at), its increments and its y0.  The increments depend on
 // no predecessor: they are drawn while the previous kernel drains (programmatic dependent launch), and y0 is read
 // after the dependency wait.  False for a thread past the last quad.
@@ -277,10 +278,11 @@ struct PwSrkStash {
   }
 };
 
-// f (program [0, n_fg), result f_src) or g (program [n_fg, n_instr), result g_src) at (t, y)
+// One SDE evaluation of the two-program layout (SRK, predictor-corrector): f (program [0, n_fg), result f_src) or g
+// (program [n_fg, n_instr), result g_src) at (t, y)
 template <typename T>
-__device__ __forceinline__ void pw_srk_eval(const tsde_pointwise& pg, PwQuad<T>& c, void* regs, bool g, const T* t,
-                                            const T (&y)[4], T (&out)[4]) {
+__device__ __forceinline__ void pw_eval(const tsde_pointwise& pg, PwQuad<T>& c, void* regs, bool g, const T* t,
+                                        const T (&y)[4], T (&out)[4]) {
   c.t = t;
 #pragma unroll
   for (int j = 0; j < 4; ++j) c.y[j] = y[j];
@@ -300,8 +302,8 @@ pw_srk_kernel(const __grid_constant__ tsde_pointwise pg, const PwSrkP<T> p, cons
   enum { F0, F1, F2, G0, G1, G2 };
   T f[4], g[4], h0[4], h1[4], x[4], z[4];
   // s = 0: f0, g0 at (t0, y0); H0_1, H1_1
-  pw_srk_eval(pg, c, pw_regs, false, p.t[0], y0, f);
-  pw_srk_eval(pg, c, pw_regs, true, p.t[0], y0, g);
+  pw_eval(pg, c, pw_regs, false, p.t[0], y0, f);
+  pw_eval(pg, c, pw_regs, true, p.t[0], y0, g);
   st.put(pw_regs, F0, f);
   st.put(pw_regs, G0, g);
 #pragma unroll
@@ -312,8 +314,8 @@ pw_srk_kernel(const __grid_constant__ tsde_pointwise pg, const PwSrkP<T> p, cons
     h1[j] = o[1];
   }
   // s = 1: f1 at (t0 + dt, H0_1), g1 at (t0 + dt/4, H1_1); H0_2, H1_2
-  pw_srk_eval(pg, c, pw_regs, false, p.t[1], h0, f);
-  pw_srk_eval(pg, c, pw_regs, true, p.t[2], h1, g);
+  pw_eval(pg, c, pw_regs, false, p.t[1], h0, f);
+  pw_eval(pg, c, pw_regs, true, p.t[2], h1, g);
   st.put(pw_regs, F1, f);
   st.put(pw_regs, G1, g);
   st.get(pw_regs, F0, x);
@@ -326,8 +328,8 @@ pw_srk_kernel(const __grid_constant__ tsde_pointwise pg, const PwSrkP<T> p, cons
     h1[j] = o[1];
   }
   // s = 2: f2 at (t0 + dt/2, H0_2), g2 at (t0 + dt, H1_2); H1_3
-  pw_srk_eval(pg, c, pw_regs, false, p.t[3], h0, f);
-  pw_srk_eval(pg, c, pw_regs, true, p.t[1], h1, g);
+  pw_eval(pg, c, pw_regs, false, p.t[3], h0, f);
+  pw_eval(pg, c, pw_regs, true, p.t[1], h1, g);
   st.put(pw_regs, F2, f);
   st.put(pw_regs, G2, g);
   st.get(pw_regs, G0, x);
@@ -339,7 +341,7 @@ pw_srk_kernel(const __grid_constant__ tsde_pointwise pg, const PwSrkP<T> p, cons
     h1[j] = o[0];
   }
   // s = 3: g3 at (t0 + dt/4, H1_3); y1
-  pw_srk_eval(pg, c, pw_regs, true, p.t[2], h1, g);
+  pw_eval(pg, c, pw_regs, true, p.t[2], h1, g);
   T f0[4], f1[4], f2[4], g0[4], g1[4], g2[4], y1[4];
   st.get(pw_regs, F0, f0);
   st.get(pw_regs, F1, f1);
@@ -356,14 +358,70 @@ pw_srk_kernel(const __grid_constant__ tsde_pointwise pg, const PwSrkP<T> p, cons
   store_quad(p.base.y1, c.base, c.vec, c.nvalid, y1);
 }
 
-// The SRK layout: an f program and a g program that each start with no register defined; go is never a source, and
-// the registers past TSDE_PW_SRK_MAX_REGS are the kernel's stash.
-static bool pw_valid_srk(const tsde_pointwise& pg) {
-  if (pg.n_regs > TSDE_PW_SRK_MAX_REGS) return false;
+// The two-program layout (SRK, predictor-corrector): an f program and a g program that each start with no register
+// defined; go is never a source.  At most MAX_REGS registers: SRK keeps the ones past TSDE_PW_SRK_MAX_REGS for its
+// stash.
+template <int MAX_REGS>
+static bool pw_valid_two(const tsde_pointwise& pg) {
+  if (pg.n_regs > MAX_REGS) return false;
   uint64_t written = 0;
   if (!pw_valid_range(pg, 0, pg.n_fg, false, written) || !pw_valid_source(pg, pg.f_src, false, written)) return false;
   written = 0;
   return pw_valid_range(pg, pg.n_fg, pg.n_instr, false, written) && pw_valid_source(pg, pg.g_src, false, written);
+}
+
+// ---- a whole Heun, midpoint or Euler-Heun step (tsde_step_predictor_corrector_pointwise) ----------------------------
+// W is drawn, y0 is read, f0 and g0 are evaluated at (t0, y0), the method's predictor forms y', the second evaluation
+// runs at (t_p, y') (g only for Euler-Heun) and the method's final op writes y1: the unfused step's own ops with the
+// scalars its kernels take, so the step equals the unfused one bit for bit.  Five quads are live at most (y0, W, f0,
+// g0, y'), which fits registers in fp64 too: no stash.  The minimum of one resident CTA in the launch bounds lets
+// ptxas keep them there; without it, it caps some instantiations at 64 or 80 registers and spills.
+template <typename T>
+struct PwPcP {
+  PwP<T> base;   // y0, y1, the quad mapping, t0 and dt
+  const T* t_p;  // the time of the second evaluation
+  T half_dt;
+};
+
+template <typename T, int SRC, int METHOD>
+__global__ void __launch_bounds__(kThreads, 1)
+pw_pc_kernel(const __grid_constant__ tsde_pointwise pg, const PwPcP<T> p, const NoiseP<T> nz) {
+  extern __shared__ __align__(16) unsigned char pw_regs[];
+  PwQuad<T> c;
+  T w[4], u[4], y0[4];
+  if (!pw_begin<T, SRC, false>(p.base, nz, c, w, u, y0)) return;
+  const T dt = p.base.dt;
+  T f0[4], g0[4], yp[4];
+  pw_eval(pg, c, pw_regs, false, p.base.t0, y0, f0);
+  pw_eval(pg, c, pw_regs, true, p.base.t0, y0, g0);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[1];
+    if constexpr (METHOD == TSDE_PC_HEUN) {
+      EulerOp<T>{dt}({y0[j], f0[j], g0[j]}, w[j], u[j], o);                  // heun.py:42
+    } else if constexpr (METHOD == TSDE_PC_MIDPOINT) {
+      MidpointPredictOp<T>{p.half_dt}({y0[j], f0[j], g0[j]}, w[j], u[j], o);  // midpoint.py:38
+    } else {
+      EulerHeunPredictOp<T>{}({y0[j], g0[j]}, w[j], u[j], o);                // euler_heun.py:36
+    }
+    yp[j] = o[0];
+  }
+  T f[4], g[4], y1[4];
+  if constexpr (METHOD != TSDE_PC_EULER_HEUN) pw_eval(pg, c, pw_regs, false, p.t_p, yp, f);
+  pw_eval(pg, c, pw_regs, true, p.t_p, yp, g);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    T o[1];
+    if constexpr (METHOD == TSDE_PC_HEUN) {
+      HeunOp<T>{dt}({y0[j], f0[j], f[j], g0[j], g[j]}, w[j], u[j], o);       // heun.py:46
+    } else if constexpr (METHOD == TSDE_PC_MIDPOINT) {
+      EulerOp<T>{dt}({y0[j], f[j], g[j]}, w[j], u[j], o);                    // midpoint.py:43
+    } else {
+      EulerHeunOp<T>{dt}({y0[j], f0[j], g0[j], g[j]}, w[j], u[j], o);        // euler_heun.py:40
+    }
+    y1[j] = o[0];
+  }
+  store_quad(p.base.y1, c.base, c.vec, c.nvalid, y1);
 }
 
 // ---- launch ---------------------------------------------------------------------------------------------------------
@@ -431,7 +489,7 @@ TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_no
     if (!t_0 || !t_1 || !t_q || !t_h) return TSDE_EINVAL;
     PwSrkP<T> p;
     NoiseP<T> np;
-    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_srk, p.base, np)) return e;
+    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_two<TSDE_PW_SRK_MAX_REGS>, p.base, np)) return e;
     const void* times[4] = {t_0, t_1, t_q, t_h};
     for (int i = 0; i < 4; ++i) p.t[i] = static_cast<const T*>(times[i]);
     // the coefficients of tsde_srk_diag_stage1/2/3 and tsde_step_srk_diag
@@ -441,5 +499,36 @@ TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_no
     p.fin = make_srk_final<T>(dt, rdt, sqrt_dt, three_dt);
     return pw_launch<T>(L, *prog, pw_srk_kernel<T, TSDE_SRC_COUNTER>, pw_srk_kernel<T, kSrcCounterMulti>, p, np,
                         p.base.nquads, prog->n_regs + (PwSrkStash<T>::kShared ? kPwSrkStash : 0), TSDE_KERNEL_PW_SRK);
+  });
+}
+
+TSDE_EXPORT int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, const tsde_noise* nz,
+                                                        const tsde_pointwise* prog, const void* y0, const void* t0,
+                                                        const void* t_p, int32_t method, double dt, double half_dt,
+                                                        void* y1) {
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
+  return dispatch(L, [&](auto t) -> int {
+    using T = decltype(t);
+    if (!t0 || !t_p || method < TSDE_PC_HEUN || method > TSDE_PC_EULER_HEUN) return TSDE_EINVAL;
+    PwPcP<T> p;
+    NoiseP<T> np;
+    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_two<TSDE_PW_MAX_REGS>, p.base, np)) return e;
+    p.base.t0 = static_cast<const T*>(t0);
+    p.base.dt = (T)dt;
+    p.t_p = static_cast<const T*>(t_p);
+    p.half_dt = (T)half_dt;
+    auto go = [&](auto single, auto multi) {
+      return pw_launch<T>(L, *prog, single, multi, p, np, p.base.nquads, prog->n_regs, TSDE_KERNEL_PW_PC);
+    };
+    switch (method) {
+      case TSDE_PC_HEUN:
+        return go(pw_pc_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_HEUN>, pw_pc_kernel<T, kSrcCounterMulti, TSDE_PC_HEUN>);
+      case TSDE_PC_MIDPOINT:
+        return go(pw_pc_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_MIDPOINT>,
+                  pw_pc_kernel<T, kSrcCounterMulti, TSDE_PC_MIDPOINT>);
+      default:
+        return go(pw_pc_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_EULER_HEUN>,
+                  pw_pc_kernel<T, kSrcCounterMulti, TSDE_PC_EULER_HEUN>);
+    }
   });
 }
