@@ -294,6 +294,29 @@ int tsde_step_milstein_pointwise(const tsde_launch* L, const tsde_noise* nz, con
                                  const void* y0, const void* t0, double dt, int32_t ito, void* y1);
 
 /*
+ * `n_steps` consecutive steps of tsde_step_milstein_pointwise as one launch: each thread reads its quad of y0 once,
+ * runs step j = 0 .. n_steps-1 on the state the step before left in its registers, and stores step j's y1 only to
+ * steps[j].y1 (an output row, the last state); a step whose y1 is NULL is not stored.  Step j draws its increment
+ * from the one Brownian cell steps[j].cell_id of length steps[j].h (W = sqrt(h) N, the square root rounded once to
+ * the state dtype, as for tsde_noise), runs the program at the 0-d time steps[j].t0 and uses steps[j].dt; every
+ * stored y1 equals what tsde_step_milstein_pointwise gives step by step, bit for bit.  `nz` gives the key, the row
+ * offset and the source (COUNTER); its cell_id and h are the first step's.  A step that spans several cells
+ * (nz->n_cells > 1, merged as tsde_noise describes from steps[0].cell_id) must run alone (n_steps == 1).
+ * TSDE_EINVAL: n_steps outside [1, TSDE_PW_MAX_STEPS], a null steps[j].t0, a null last y1, and whatever
+ * tsde_step_milstein_pointwise refuses.  The step table is passed by value, so a captured launch carries it.
+ */
+#define TSDE_PW_MAX_STEPS 64
+typedef struct tsde_pw_step {
+  uint64_t    cell_id;  /* the step's Brownian cell                                     */
+  double      h;        /* that cell's length                                           */
+  double      dt;       /* the step's dt                                                */
+  const void* t0;       /* DEVICE 0-d time of the step (state dtype), read by TSDE_PW_T0 */
+  void*       y1;       /* where the step's y1 is stored, or NULL (not stored)          */
+} tsde_pw_step;
+int tsde_solve_milstein_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                  const void* y0, const tsde_pw_step* steps, int32_t n_steps, int32_t ito);
+
+/*
  * A whole diagonal-noise SRK (srid2) step (srk.py:57-88) for an SDE whose f(t, y) and g(t, y) are element-wise
  * programs: one launch reads y0, draws W and U, and evaluates the step's seven SDE calls and four tableau stages
  *     f0 = f(t_0, y0), g0 = g(t_0, y0); H0_1, H1_1 as tsde_srk_diag_stage1;

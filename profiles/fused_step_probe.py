@@ -1,4 +1,5 @@
-"""CUDA-event probe of the fused Milstein step (tsde_step_milstein_pointwise) at the cfg2 size (65536 x 64 fp32).
+"""CUDA-event probe of the fused Milstein step (tsde_step_milstein_pointwise) and of chunks of K steps per launch
+(tsde_solve_milstein_pointwise) at the cfg2 size (65536 x 64 fp32).
 
     python profiles/fused_step_probe.py
 
@@ -8,6 +9,10 @@ The program is the one the solver records for cfg2's SDE (f = mu*y, g = sigma*y,
   in situ  the launches chained as the solver chains them: y1 of launch k is y0 of launch k + 1
   seed     tsde_milstein_vjp_seed on the same sets, cold: the same Philox + Box-Muller work per quad with one tensor
            read and one written, i.e. the RNG-bound time of a kernel of this shape
+  chunk_K  K consecutive steps in one launch, every step's y1 stored to its row of an output series (as cfg2 stores
+           every step), in situ (the next launch starts from the last row) and cold (y0 from the rotating sets);
+           microseconds per step and the achieved write bandwidth.  K = 128 does not fit the step table
+           (TSDE_PW_MAX_STEPS = 64, bounded by the 4 KiB parameter space) and is reported as such.
 Algorithmic bytes of the fused step: 2 * D * 4 per trajectory (y0 read, y1 written).  Prints one JSON line with the
 card's name and power limit.
 """
@@ -64,6 +69,26 @@ def fused(s_in, s_out):
                                                  dt, 1, P(s_out)), 'fused')
 
 
+series = [torch.empty(_cabi.PW_MAX_STEPS, B, D, device=dev) for _ in range(2)]
+
+
+def chunk(k, y0, rows):
+    steps = (_cabi.PwStep * k)()
+    for j, st in enumerate(steps):
+        st.cell_id, st.h, st.dt, st.t0, st.y1 = 7 + j, dt, dt, P(t0), P(rows[j])
+    _cabi.check(lib.tsde_solve_milstein_pointwise(ctypes.byref(L), ctypes.byref(nz), ctypes.byref(prog), P(y0), steps,
+                                                  k, 1), 'chunk')
+
+
+def timed_chunk(k, chained):
+    """Microseconds per launch of a k-step chunk, graph-captured."""
+    def issue():
+        for i in range(REPS):
+            src, dst = series[i % 2], series[(i + 1) % 2]
+            chunk(k, src[k - 1] if chained else sets[i % NSET]['y0'], dst)
+    return timed_issue(issue)
+
+
 def seed(s_in, s_out):
     _cabi.check(lib.tsde_milstein_vjp_seed(ctypes.byref(L), ctypes.byref(nz), P(s_in), dt, 1, P(s_out)), 'seed')
 
@@ -78,6 +103,11 @@ def timed(launch, chained):
             else:
                 s = sets[i % NSET]
                 launch(s['y0'], s['y1'])
+    return timed_issue(issue)
+
+
+def timed_issue(issue):
+    """Microseconds per launch of REPS launches `issue()`, graph-captured."""
     issue()
     torch.cuda.synchronize()
     graph = torch.cuda.CUDAGraph()
@@ -114,4 +144,11 @@ out = {'gpu': gpu(), 'B': B, 'D': D, 'program': {'instructions': prog.n_instr, '
 for name, launch, chained in (('fused_cold', fused, False), ('fused_in_situ', fused, True), ('seed_cold', seed, False)):
     us = timed(launch, chained)
     out[name] = {'us': round(us, 2), 'GBps': round(nbytes / (us * 1e-6) / 1e9, 1)}
+for k in (1, 8, 32, 64, 128):
+    if k > _cabi.PW_MAX_STEPS:
+        out[f'chunk_{k}'] = 'exceeds TSDE_PW_MAX_STEPS'
+        continue
+    for mode, chained in (('in_situ', True), ('cold', False)):
+        us = timed_chunk(k, chained)
+        out[f'chunk_{k}_{mode}'] = {'us_per_step': round(us / k, 2), 'write_GBps': round(k * B * D * 4 / (us * 1e-6) / 1e9, 1)}
 print(json.dumps(out), flush=True)

@@ -14,10 +14,12 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, 'torchsde_b200', 'lib', 'libtorchsde_b200.so')
 PICK = [  # (label, regex on the demangled kernel name)
     ('Milstein tableau, fp32, counter noise (headline)', r'ew_fast_kernel<float, tsde::MilsteinOp<float>, 1>'),
-    ('fused Milstein step of an element-wise SDE (interpreter), fp32, counter noise',
+    ('fused Milstein steps of an element-wise SDE, up to 64 per launch (interpreter), fp32, counter noise',
      r'pw_milstein_kernel<float, 1>'),
-    ('fused Milstein step of an element-wise SDE (interpreter), fp64, counter noise',
+    ('fused Milstein steps of an element-wise SDE, up to 64 per launch (interpreter), fp64, counter noise',
      r'pw_milstein_kernel<double, 1>'),
+    ('fused Milstein step of an element-wise SDE spanning several cells, fp32', r'pw_milstein_kernel<float, 3>'),
+    ('fused Milstein step of an element-wise SDE spanning several cells, fp64', r'pw_milstein_kernel<double, 3>'),
     ('fused SRK step of an element-wise SDE (interpreter), fp32, counter noise', r'pw_srk_kernel<float, 1>'),
     ('fused SRK step of an element-wise SDE (interpreter), fp64, counter noise', r'pw_srk_kernel<double, 1>'),
     ('fused Heun step of an element-wise SDE (interpreter), fp32, counter noise', r'pw_pc_kernel<float, 1, 0>'),

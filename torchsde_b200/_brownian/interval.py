@@ -184,6 +184,14 @@ class GridBinding:
     def n_steps(self):
         return len(self.first)
 
+    def cell(self, k):
+        """(counter id, length) of the first primary cell of solver step k, and the number of cells the step merges:
+        what `fill` puts in cell_id, h and n_cells."""
+        if self.reverse:
+            k = len(self.first) - 1 - k
+        i = self.first[k]
+        return (self.node.cell_base + i) & _MASK64, self.node.bounds[i + 1] - self.node.bounds[i], self.count[k]
+
     def fill(self, nz, k, want_u, key_ptr, row_offset=0):
         """Fill a `_cabi.Noise` for solver step k (k counts in solver order; for a reversed
         binding the solver's step k is the forward grid's step n-1-k)."""

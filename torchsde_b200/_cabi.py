@@ -55,6 +55,7 @@ KERNEL_PW_MILSTEIN = 3  # TSDE_KERNEL_PW_MILSTEIN
 KERNEL_PW_SRK = 4  # TSDE_KERNEL_PW_SRK
 KERNEL_PW_PC = 5  # TSDE_KERNEL_PW_PC
 PC_HEUN, PC_MIDPOINT, PC_EULER_HEUN = range(3)  # TSDE_PC_*
+PW_MAX_STEPS = 64  # TSDE_PW_MAX_STEPS
 
 
 class PwInstr(ctypes.Structure):
@@ -71,6 +72,11 @@ class Pointwise(ctypes.Structure):
                 ('n_operands', ctypes.c_int32), ('f_src', ctypes.c_uint8), ('g_src', ctypes.c_uint8),
                 ('gdg_src', ctypes.c_uint8), ('reserved', ctypes.c_uint8),
                 ('instr', PwInstr * PW_MAX_INSTR), ('operand', PwOperand * PW_MAX_OPERANDS)]
+
+
+class PwStep(ctypes.Structure):
+    _fields_ = [('cell_id', ctypes.c_uint64), ('h', ctypes.c_double), ('dt', ctypes.c_double), ('t0', ctypes.c_void_p),
+                ('y1', ctypes.c_void_p)]
 
 
 _P = ctypes.c_void_p
@@ -95,6 +101,7 @@ SIGNATURES = {
     'tsde_milstein_vjp_seed': [_L, _N, _P, _D, _I, _P],
     'tsde_step_milstein': [_L, _N, _P, _P, _P, _P, _D, _P],
     'tsde_step_milstein_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _D, _I, _P],
+    'tsde_solve_milstein_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, ctypes.POINTER(PwStep), _I, _I],
     'tsde_step_srk_diag_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _P, _P, _P, _D, _D, _D, _D, _P],
     'tsde_step_predictor_corrector_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _P, _I, _D, _D, _P],
     'tsde_milstein_gf_predict': [_L, _P, _P, _P, _D, _D, _I, _P],

@@ -23,6 +23,7 @@ import warnings
 
 import torch
 
+from . import pointwise
 from . import schedule as schedule_lib
 from .. import _cabi
 from .._brownian import BrownianInterval, ReverseBrownian
@@ -539,26 +540,52 @@ class BaseSDESolver(metaclass=abc.ABCMeta):
             return torch.stack(rows, dim=0), curr_extra
         return ys, curr_extra
 
+    def _chunks_ready(self):
+        """Whether the steps from here on may run several per launch (`_step_chunk`)."""
+        return False
+
+    def _step_chunk(self, ctxs, y0, extra0, outs):
+        """Advance the consecutive steps `ctxs` in one launch, storing step j's y1 to outs[j] (None: not stored; the
+        last is given).  Returns (y1 of the last step, extra1)."""
+        raise NotImplementedError
+
     def _run(self, sched, ctxs, ys, extra):
-        """The time loop proper: capturable (no syncs, no host-dependent control flow)."""
+        """The time loop proper: capturable (no syncs, no host-dependent control flow).  Once `_chunks_ready`, steps
+        run in the chunks of pointwise.plan_chunks."""
         self._refresh_stream()
         curr = ys[0]
         prev = curr
         scratch = [None, None]
         flip = 0
-        for k, c in enumerate(ctxs):
+
+        def dest(k):  # where the state after step k must be: its output row, else a scratch buffer
+            nonlocal flip
             row = sched.aligned_row(k)
             if row is not None:
-                out = ys[row]
+                return ys[row]
+            if scratch[flip] is None:
+                scratch[flip] = torch.empty_like(ys[0])
+            flip ^= 1
+            return scratch[flip ^ 1]
+
+        chunks = None
+        k = 0
+        while k < len(ctxs):
+            if chunks is None and self._chunks_ready():
+                interpolated = [j for j, os in sched.outputs_after.items() if any(not o.aligned for o in os)]
+                multi = [j for j in range(k, len(ctxs)) if self._feed.binding.cell(ctxs[j].k)[2] > 1]
+                chunks = iter(pointwise.plan_chunks(k, len(ctxs), interpolated, multi, pointwise.chunk_length(self)))
+            k1 = next(chunks)[1] if chunks is not None else k + 1
+            self._cur_c = ctxs[k1 - 1]
+            if k1 == k + 1:
+                y1, extra = self._step(ctxs[k], curr, extra, dest(k))
             else:
-                if scratch[flip] is None:
-                    scratch[flip] = torch.empty_like(ys[0])
-                out = scratch[flip]
-                flip ^= 1
-            self._cur_c = c
-            y1, extra = self._step(c, curr, extra, out)
+                rows = [sched.aligned_row(j) for j in range(k, k1 - 1)]
+                outs = [None if r is None else ys[r] for r in rows] + [dest(k1 - 1)]
+                y1, extra = self._step_chunk(ctxs[k:k1], curr, extra, outs)
+            k = k1
             prev, curr = curr, y1
-            for o in sched.outputs_after.get(k, ()):
+            for o in sched.outputs_after.get(k - 1, ()):
                 if not o.aligned:
                     # interp.py:15-18
                     _cabi.check(self._lib.tsde_linear_interp(self._LU, prev.data_ptr(), curr.data_ptr(),

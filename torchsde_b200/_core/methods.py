@@ -123,6 +123,13 @@ class BaseMilstein(_ProdMixin, base_solver.BaseSDESolver):
         sqrt_dt = _ieee_sqrt(dt)
         return {'sqrt_dt': float(sqrt_dt), 'two_sqrt_dt': float(2 * sqrt_dt)}
 
+    def _chunks_ready(self):
+        return pointwise.ready(self)
+
+    def _step_chunk(self, ctxs, y0, extra0, outs):
+        # the recorded element-wise program (pointwise.py), several steps per kernel with the state in registers
+        return pointwise.solve_chunk(self, ctxs, y0, outs, 1 if self.ito else 0), ()
+
     def _step(self, c, y0, extra0, out):
         sde = self.sde
         ito = 1 if self.ito else 0

@@ -32,7 +32,8 @@ g, the vjp seed, autograd's vjp of g and the tableau (methods.BaseMilstein._step
 f(t0, y), g(t0, y) and torch.autograd.grad(g, y, go), in which the seed go is one more operand.  The vjp is not
 derived symbolically: autograd's own op sequence (`grad * other`, the `add` that accumulates a twice-used `y`, ...)
 is what decides the bits, so it is what gets recorded.  The three segments are one program: the vjp part may read
-what the f / g part computed.
+what the f / g part computed.  When the batch fills the GPU, up to TSDE_PW_MAX_STEPS consecutive steps run as one
+launch of tsde_solve_milstein_pointwise with the state in registers (`plan_chunks`, `chunk_length`, `solve_chunk`).
 
 SRK (`SrkRecorder`, tsde_step_srk_diag_pointwise).  The step's seven evaluations, f at three (t, y) and g at four
 (methods.SRK._diagonal_or_scalar_step), are recorded one by one; a value of one evaluation is not an operand of
@@ -462,6 +463,54 @@ def launch(solver, name, nz, y0, args, out):
     fn = getattr(solver._lib, name)
     _cabi.check(fn(solver._L, nz, ctypes.byref(prog), y0.data_ptr(), *args, out.data_ptr()), name)
     return out
+
+
+def plan_chunks(first, n_steps, interpolated=(), multi_cell=(), max_steps=_cabi.PW_MAX_STEPS):
+    """Steps [first, n_steps) of a fixed-step solve grouped into the launches of its element-wise Milstein program, as
+    (k0, k1) ranges of at most `max_steps` consecutive steps.  Inside a chunk a state lives in registers only, so a
+    chunk ends where a step's state has to be in memory for someone else:
+      * a step in `multi_cell` (it spans several Brownian cells; tsde_solve_milstein_pointwise draws one cell per
+        step) runs alone;
+      * a step in `interpolated` (a non-aligned output falls inside it) runs alone, and the step before it ends a
+        chunk: the interpolation reads the states before and after the step.
+    Aligned outputs do not end a chunk: the kernel stores those rows as it passes them."""
+    solo = set(interpolated) | set(multi_cell)
+    out, k0 = [], first
+    for k in range(first, n_steps):
+        if k + 1 == n_steps or k in solo or k + 1 in solo or k + 1 - k0 == max_steps:
+            out.append((k0, k + 1))
+            k0 = k + 1
+    return out
+
+
+def chunk_length(solver):
+    """Steps per launch of the element-wise Milstein program: TSDE_PW_MAX_STEPS when the batch fills the GPU with at
+    least one wave of the kernel's CTAs (256 quads each, 4 resident per SM in float32 and 2 in float64), else 1.  A
+    smaller grid leaves SMs idle; consecutive one-step kernels fill them by overlapping one step's tail with the next
+    one's start (programmatic dependent launch), which a chunk, whose steps are sequential per thread, cannot.  (On an
+    H100 at B = 4096, D = 64, fp32, one session alternating the two: 3.3 us per step one step per launch, 4.3 in
+    chunks of 64.)"""
+    if solver.device.type != 'cuda':  # (the host-side dry run of the tests; a solve always runs on a CUDA device)
+        return _cabi.PW_MAX_STEPS
+    ctas = solver.rows * ((solver.d + 3) // 4) / 256
+    wave = torch.cuda.get_device_properties(solver.device).multi_processor_count * (
+        4 if solver.dtype == torch.float32 else 2)
+    return _cabi.PW_MAX_STEPS if ctas >= wave else 1
+
+
+def solve_chunk(solver, ctxs, y0, outs, ito):
+    """Consecutive single-cell Milstein steps `ctxs` from y0 as one launch of tsde_solve_milstein_pointwise on the
+    solver's program.  Step j's y1 is stored to outs[j] (None: kept in registers only; the last must be given)."""
+    prog, _ = solver._pw
+    feed = solver._feed
+    nz = feed.get(ctxs[0])
+    steps = (_cabi.PwStep * len(ctxs))()
+    for s, c, out in zip(steps, ctxs, outs):
+        s.cell_id, s.h, _ = feed.binding.cell(c.k)
+        s.dt, s.t0, s.y1 = c.dt, c.t0.data_ptr(), None if out is None else out.data_ptr()
+    _cabi.check(solver._lib.tsde_solve_milstein_pointwise(solver._L, nz, ctypes.byref(prog), y0.data_ptr(), steps,
+                                                         len(ctxs), ito), 'tsde_solve_milstein_pointwise')
+    return outs[-1]
 
 
 def eligible(solver):

@@ -1,4 +1,5 @@
-// Whole steps of an element-wise SDE as one kernel: tsde_step_milstein_pointwise, tsde_step_srk_diag_pointwise and
+// Whole steps of an element-wise SDE as one kernel: tsde_step_milstein_pointwise (and tsde_solve_milstein_pointwise,
+// up to TSDE_PW_MAX_STEPS consecutive Milstein steps in one kernel), tsde_step_srk_diag_pointwise and
 // tsde_step_predictor_corrector_pointwise (include/torchsde_b200.h describes the tsde_pointwise program and its two
 // layouts).
 //
@@ -159,6 +160,30 @@ static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, bool allow_
 }
 
 // ---- what every kernel starts with ----------------------------------------------------------------------------------
+// pw_begin's quad mapping on its own, for a kernel that draws again later: the flat index Q (past the last quad when
+// Q >= p.nquads), the row and quad of the row, and `c` but for the state.  (pw_begin keeps its own copy: calling this
+// from it reschedules the SRK and predictor-corrector kernels.)
+template <typename T>
+__device__ __forceinline__ void pw_locate(const PwP<T>& p, PwQuad<T>& c, int64_t& Q, int64_t& row, int64_t& q) {
+  Q = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+  if (p.qshift >= 0) {
+    row = Q >> p.qshift;
+    q = Q & ((1ll << p.qshift) - 1);
+  } else if (p.small) {
+    const uint32_t r32 = rowdiv_row((uint32_t)Q, p.qmagic);
+    row = r32;
+    q = (int64_t)rowdiv_quad((uint32_t)Q, r32, (uint32_t)p.qpr);
+  } else {
+    row = Q / p.qpr;
+    q = Q - row * p.qpr;
+  }
+  c.chan = 4 * q;
+  c.base = row * p.d + c.chan;
+  const int64_t rem = p.d - c.chan;
+  c.nvalid = rem < 4 ? (int)rem : 4;
+  c.vec = p.vec != 0;
+}
+
 // This thread's quad (`c`, but for the state it is evaluated at), its increments and its y0.  The increments depend on
 // no predecessor: they are drawn while the previous kernel drains (programmatic dependent launch), and y0 is read
 // after the dependency wait.  False for a thread past the last quad.
@@ -192,39 +217,74 @@ __device__ __forceinline__ bool pw_begin(const PwP<T>& p, const NoiseP<T>& nz, P
   return true;
 }
 
-// ---- a whole Milstein step (tsde_step_milstein_pointwise) -----------------------------------------------------------
-// The program's f / g part runs on y0, MilsteinSeedOp forms go, the vjp part runs and MilsteinOp writes y1.  Only y0
-// and y1 (and the program's device operands) touch memory: 2 tensors per step instead of the 13 of the unfused step.
+// ---- consecutive Milstein steps (tsde_solve_milstein_pointwise, tsde_step_milstein_pointwise) -----------------------
+// Per step: the program's f / g part runs on y, MilsteinSeedOp forms go, the vjp part runs and MilsteinOp forms y1.
+// A quad's trajectory depends on nothing but its own state (element-wise SDE, diagonal noise), so one thread runs the
+// whole chunk of up to kPwMaxSteps steps: y0 is read once, y1 stays in registers from one step to the next and is
+// stored only where the step table gives it a destination (an output row, the chunk's last state).  The unfused
+// step moves 13 tensors; a chunk moves one read and the stores it is asked for.
+constexpr int kPwMaxSteps = TSDE_PW_MAX_STEPS;
+
+template <typename T>
+struct PwStep {  // one step of a chunk, as tsde_pw_step with its scalars rounded to T on the host
+  uint64_t cell;   // Brownian cell (the kSrcCounterMulti kernel merges nz.n_cells cells from here)
+  const T* t0;     // what TSDE_PW_T0 reads during this step
+  T* y1;           // destination of this step's y1, or null
+  T sqrt_h, dt;    // (T)sqrt(h) of the cell, (T)dt
+};
+template <typename T>
+struct PwSteps {  // by value: a captured launch carries the whole table
+  int32_t n;
+  PwStep<T> s[kPwMaxSteps];
+};
+static_assert(sizeof(tsde_pointwise) + sizeof(PwP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <= 4096,
+              "the Milstein kernel's parameters fit the 4 KiB parameter space");
+
 template <typename T, int SRC>
 __global__ void __launch_bounds__(kThreads)
-pw_milstein_kernel(const __grid_constant__ tsde_pointwise pg, const PwP<T> p, const NoiseP<T> nz) {
+pw_milstein_kernel(const __grid_constant__ tsde_pointwise pg, const PwP<T> p, const NoiseP<T> nz,
+                   const __grid_constant__ PwSteps<T> st) {
   extern __shared__ __align__(16) unsigned char pw_regs[];
   PwQuad<T> c;
-  T w[4], u[4];
-  if (!pw_begin<T, SRC, false>(p, nz, c, w, u, c.y)) return;
-  c.t = p.t0;
-  pw_run(pg, c, pw_regs, 0, pg.n_fg);
-  T f[4], g[4];
-  pw_fetch(pg, c, pw_regs, pg.f_src, f);
-  pw_fetch(pg, c, pw_regs, pg.g_src, g);
-  const MilsteinSeedOp<T> seed{p.dt, p.ito};
+  int64_t Q, row, q;
+  pw_locate(p, c, Q, row, q);
+  const Key key = load_key(nz.key);
+  for (int j = 0; j < st.n; ++j) {
+    const PwStep<T>& s = st.s[j];
+    T w[4], u[4];
+    NoiseP<T> z = nz;  // this step's cell
+    z.cell_id = s.cell;
+    z.sqrt_h = s.sqrt_h;
+    quad_noise<T, SRC, false>(z, key, row, q, c.vec, c.nvalid, w, u);
+    if (j == 0) {  // the first increment is drawn while the previous kernel drains; y0 is read after the wait
+      asm volatile("griddepcontrol.wait;" ::: "memory");
+      if (Q >= p.nquads) return;
+      load_quad(p.y0, c.base, c.vec, c.nvalid, c.y);
+    }
+    c.t = s.t0;
+    pw_run(pg, c, pw_regs, 0, pg.n_fg);
+    T f[4], g[4];
+    pw_fetch(pg, c, pw_regs, pg.f_src, f);
+    pw_fetch(pg, c, pw_regs, pg.g_src, g);
+    const MilsteinSeedOp<T> seed{s.dt, p.ito};
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    T o[1];
-    seed({g[j]}, w[j], u[j], o);
-    c.go[j] = o[0];
-  }
-  pw_run(pg, c, pw_regs, pg.n_fg, pg.n_instr);
-  T gdg[4], y1[4];
-  pw_fetch(pg, c, pw_regs, pg.gdg_src, gdg);
-  const MilsteinOp<T> step{p.dt};
+    for (int i = 0; i < 4; ++i) {
+      T o[1];
+      seed({g[i]}, w[i], u[i], o);
+      c.go[i] = o[0];
+    }
+    pw_run(pg, c, pw_regs, pg.n_fg, pg.n_instr);
+    T gdg[4];
+    pw_fetch(pg, c, pw_regs, pg.gdg_src, gdg);
+    const MilsteinOp<T> step{s.dt};
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    T o[1];
-    step({c.y[j], f[j], g[j], gdg[j]}, w[j], u[j], o);
-    y1[j] = o[0];
+    for (int i = 0; i < 4; ++i) {
+      T o[1];
+      step({c.y[i], f[i], g[i], gdg[i]}, w[i], u[i], o);
+      c.y[i] = o[0];
+    }
+    if (s.y1) store_quad(s.y1, c.base, c.vec, c.nvalid, c.y);
   }
-  store_quad(p.y1, c.base, c.vec, c.nvalid, y1);
 }
 
 // The Milstein layout, in the order the kernel reads it: go exists from the vjp part on, registers carry over.
@@ -443,17 +503,18 @@ static int pw_prepare(const tsde_launch* L, const tsde_noise* nz, const tsde_poi
 }
 
 // One thread per quad, `slots` shared-memory registers per thread; `single` draws from one Brownian cell, `multi` sums
-// the cells of a step that spans several.
-template <typename T, typename P>
-static int pw_launch(const tsde_launch* L, const tsde_pointwise& prog, void (*single)(tsde_pointwise, P, NoiseP<T>),
-                     void (*multi)(tsde_pointwise, P, NoiseP<T>), const P& p, const NoiseP<T>& np, int64_t nquads,
-                     int slots, int family) {
+// the cells of a step that spans several.  `x` are the kernel's parameters past the noise (the Milstein step table).
+template <typename T, typename P, typename... X>
+static int pw_launch(const tsde_launch* L, const tsde_pointwise& prog,
+                     void (*single)(tsde_pointwise, P, NoiseP<T>, X...),
+                     void (*multi)(tsde_pointwise, P, NoiseP<T>, X...), const P& p, const NoiseP<T>& np,
+                     int64_t nquads, int slots, int family, const X&... x) {
   const size_t smem = (size_t)slots * kThreads * 4 * sizeof(T);
   auto kernel = np.n_cells > 1 ? multi : single;
   if (resident_ctas(reinterpret_cast<const void*>(kernel), kThreads, smem) < 1) return TSDE_EINVAL;
   const int64_t grid = (nquads + kThreads - 1) / kThreads;
   const int e = launch_kernel(kernel, grid, kThreads, smem, reinterpret_cast<cudaStream_t>(L->stream), true, prog, p,
-                              np);
+                              np, x...);
   if (e == 0) g_launches[family].fetch_add(1, std::memory_order_relaxed);
   return e;
 }
@@ -462,21 +523,48 @@ static int pw_launch(const tsde_launch* L, const tsde_pointwise& prog, void (*si
 
 using namespace tsde;
 
+// The chunk `steps[0, n_steps)` from y0 (both entry points): one launch of pw_milstein_kernel.  A step that merges
+// several Brownian cells (nz->n_cells > 1) runs alone, in the kSrcCounterMulti instantiation.
+template <typename T>
+static int pw_milstein_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
+                             const tsde_pw_step* steps, int32_t n_steps, int32_t ito) {
+  if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
+  PwP<T> p;
+  NoiseP<T> np;
+  if (int e = pw_prepare<T>(L, nz, prog, y0, steps[n_steps - 1].y1, pw_valid_milstein, p, np)) return e;
+  if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
+  PwSteps<T> st{};
+  st.n = n_steps;
+  for (int j = 0; j < n_steps; ++j) {
+    const tsde_pw_step& s = steps[j];
+    if (!s.t0) return TSDE_EINVAL;
+    if (s.y1 && !aligned16(s.y1)) p.vec = 0;
+    st.s[j] = PwStep<T>{s.cell_id, static_cast<const T*>(s.t0), static_cast<T*>(s.y1), (T)sqrt(s.h), (T)s.dt};
+  }
+  // (the multi-cell merge reads the first cell and the uniform length from the noise descriptor)
+  np.cell_id = steps[0].cell_id;
+  np.h = steps[0].h;
+  p.ito = ito;
+  return pw_launch<T>(L, *prog, pw_milstein_kernel<T, TSDE_SRC_COUNTER>, pw_milstein_kernel<T, kSrcCounterMulti>, p,
+                      np, p.nquads, prog->n_regs, TSDE_KERNEL_PW_MILSTEIN, st);
+}
+
 TSDE_EXPORT int tsde_step_milstein_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
                                              const void* y0, const void* t0, double dt, int32_t ito, void* y1) {
   if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
   return dispatch(L, [&](auto t) -> int {
     using T = decltype(t);
-    if (!t0) return TSDE_EINVAL;
-    PwP<T> p;
-    NoiseP<T> np;
-    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_milstein, p, np)) return e;
-    p.t0 = static_cast<const T*>(t0);
-    p.dt = (T)dt;
-    p.ito = ito;
-    return pw_launch<T>(L, *prog, pw_milstein_kernel<T, TSDE_SRC_COUNTER>, pw_milstein_kernel<T, kSrcCounterMulti>, p,
-                        np, p.nquads, prog->n_regs, TSDE_KERNEL_PW_MILSTEIN);
+    if (!t0 || !nz) return TSDE_EINVAL;
+    const tsde_pw_step step{nz->cell_id, nz->h, dt, t0, y1};  // a chunk of one
+    return pw_milstein_chunk<T>(L, nz, prog, y0, &step, 1, ito);
   });
+}
+
+TSDE_EXPORT int tsde_solve_milstein_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                              const void* y0, const tsde_pw_step* steps, int32_t n_steps,
+                                              int32_t ito) {
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
+  return dispatch(L, [&](auto t) -> int { return pw_milstein_chunk<decltype(t)>(L, nz, prog, y0, steps, n_steps, ito); });
 }
 
 TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
