@@ -132,6 +132,9 @@ const char* tsde_error_string(int code);
 #define TSDE_KERNEL_PW_SRK 4      /* whole SRK step with an element-wise SDE (tsde_step_srk_diag_pointwise)     */
 #define TSDE_KERNEL_PW_PC 5       /* whole Heun / midpoint / Euler-Heun step with an element-wise SDE
                                      (tsde_step_predictor_corrector_pointwise)                                  */
+#define TSDE_KERNEL_PW_CHUNK 6    /* Euler / reversible-Heun steps with an element-wise SDE, up to
+                                     TSDE_PW_MAX_STEPS per launch (tsde_solve_euler_pointwise,
+                                     tsde_solve_reversible_heun_pointwise)                                      */
 int64_t tsde_kernel_launches(int32_t family);
 
 /* ------------------------------------------------------------------------ */
@@ -361,6 +364,35 @@ enum { TSDE_PC_HEUN = 0, TSDE_PC_MIDPOINT = 1, TSDE_PC_EULER_HEUN = 2 };
 int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
                                             const void* y0, const void* t0, const void* t_p, int32_t method,
                                             double dt, double half_dt, void* y1);
+
+/*
+ * `n_steps` consecutive diagonal-noise Euler-Maruyama steps (euler.py:34-37) of an SDE whose f(t, y) and g(t, y) are
+ * element-wise programs, as one launch: each thread reads its quad of y0 once and per step evaluates f and g at
+ * (steps[j].t0, y) and forms y1 as tsde_step_euler (steps[j].dt), in registers.  The step table, the noise, what is
+ * stored and the rule for steps that span several cells are those of tsde_solve_milstein_pointwise; a single step is
+ * a chunk of one.  Every stored y1 equals the unfused step's bit for bit.
+ * Program: the two-program layout of tsde_step_predictor_corrector_pointwise (n_regs <= TSDE_PW_MAX_REGS).
+ * TSDE_EINVAL: whatever tsde_step_predictor_corrector_pointwise refuses, n_steps outside [1, TSDE_PW_MAX_STEPS], a
+ * null steps[j].t0, a null last y1, and a step that spans several cells in a chunk of more than one.  An empty batch
+ * is a no-op.
+ */
+int tsde_solve_euler_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                               const void* y0, const tsde_pw_step* steps, int32_t n_steps);
+
+/*
+ * `n_steps` consecutive diagonal-noise reversible Heun steps (reversible_heun.py:64-73) as one launch, under the rules
+ * of tsde_solve_euler_pointwise.  The chunk starts from y0 and the solver state (z0, f0, g0), each read once, and per
+ * step forms
+ *     z1 as tsde_reversible_heun_z (dt);  f1, g1 at (steps[j].t0, z1);  y1 as tsde_step_reversible_heun on
+ *     (y, f, f1, g, g1) with half_dt = 0.5 * dt rounded once to the state dtype;  (y, z, f, g) <- (y1, z1, f1, g1)
+ * in registers.  steps[j].t0 is the time the program runs at, the step's t1.  The state after the last step is stored
+ * once, to z1, f1 and g1, which must not overlap z0, f0 or g0.  Every stored value equals the unfused steps' bit for
+ * bit when (state dtype) 0.5 * (state dtype) dt equals the unfused step's half_dt, which holds unless it is subnormal.
+ * TSDE_EINVAL: as tsde_solve_euler_pointwise, and any null z0, f0, g0, z1, f1 or g1.
+ */
+int tsde_solve_reversible_heun_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                         const void* y0, const void* z0, const void* f0, const void* g0,
+                                         const tsde_pw_step* steps, int32_t n_steps, void* z1, void* f1, void* g1);
 
 /* derivative-free Milstein, predictor: y' = y0 + (Ito ? dt*f : 0) + g*sqrt_dt
  * methods/milstein.py:58-63,83-84,93-94.  g is (rows,d) also for scalar noise (squeezed). */

@@ -24,6 +24,12 @@ PICK = [  # (label, regex on the demangled kernel name)
     ('fused SRK step of an element-wise SDE (interpreter), fp64, counter noise', r'pw_srk_kernel<double, 1>'),
     ('fused Heun step of an element-wise SDE (interpreter), fp32, counter noise', r'pw_pc_kernel<float, 1, 0>'),
     ('fused midpoint step of an element-wise SDE (interpreter), fp64, counter noise', r'pw_pc_kernel<double, 1, 1>'),
+    ('fused Euler steps of an element-wise SDE, up to 64 per launch (interpreter), fp32, counter noise',
+     r'pw_chunk_kernel<float, 1, 0>'),
+    ('fused reversible-Heun steps of an element-wise SDE, up to 64 per launch (interpreter), fp32, counter noise',
+     r'pw_chunk_kernel<float, 1, 1>'),
+    ('fused reversible-Heun steps of an element-wise SDE, up to 64 per launch (interpreter), fp64, counter noise',
+     r'pw_chunk_kernel<double, 1, 1>'),
     ('Milstein vjp seed, fp32, counter noise', r'ew_fast_kernel<float, tsde::MilsteinVjpSeedOp<float>, 1>|ew_fast_kernel<float, tsde::MilsteinSeedOp<float>, 1>'),
     ('SRK srid2 final stage, fp32', r'ew_fast_kernel<float, tsde::SrkDiagFinalOp<float>, 1>'),
     ('Euler tableau, fp64, counter noise', r'ew_fast_kernel<double, tsde::EulerOp<double>, 1>'),

@@ -54,6 +54,7 @@ PW_SRK_MAX_REGS = 18  # TSDE_PW_SRK_MAX_REGS
 KERNEL_PW_MILSTEIN = 3  # TSDE_KERNEL_PW_MILSTEIN
 KERNEL_PW_SRK = 4  # TSDE_KERNEL_PW_SRK
 KERNEL_PW_PC = 5  # TSDE_KERNEL_PW_PC
+KERNEL_PW_CHUNK = 6  # TSDE_KERNEL_PW_CHUNK
 PC_HEUN, PC_MIDPOINT, PC_EULER_HEUN = range(3)  # TSDE_PC_*
 PW_MAX_STEPS = 64  # TSDE_PW_MAX_STEPS
 
@@ -104,6 +105,9 @@ SIGNATURES = {
     'tsde_solve_milstein_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, ctypes.POINTER(PwStep), _I, _I],
     'tsde_step_srk_diag_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _P, _P, _P, _D, _D, _D, _D, _P],
     'tsde_step_predictor_corrector_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _P, _I, _D, _D, _P],
+    'tsde_solve_euler_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, ctypes.POINTER(PwStep), _I],
+    'tsde_solve_reversible_heun_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _P, _P,
+                                             ctypes.POINTER(PwStep), _I, _P, _P, _P],
     'tsde_milstein_gf_predict': [_L, _P, _P, _P, _D, _D, _I, _P],
     'tsde_step_milstein_gf': [_L, _N, _P, _P, _P, _P, _D, _D, _I, _P],
     'tsde_step_heun': [_L, _N, _P, _P, _P, _P, _P, _D, _P],

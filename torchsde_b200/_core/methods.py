@@ -85,12 +85,29 @@ class Euler(_ProdMixin, base_solver.BaseSDESolver):
     noise_types = NOISE_TYPES.all()
     levy_area_approximations = LEVY_AREA_APPROXIMATIONS.all()
 
+    _pw_method = 'euler'
+
     def __init__(self, sde, **kwargs):
         self.strong_order = 1.0 if sde.noise_type == NOISE_TYPES.additive else 0.5
         super(Euler, self).__init__(sde=sde, **kwargs)
+        self._pw = None  # the element-wise programs of the step (pointwise.py), False once rejected
+
+    def _chunks_ready(self):
+        return pointwise.ready(self)
+
+    def _step_chunk(self, ctxs, y0, extra0, outs):
+        # the recorded element-wise programs (pointwise.py), several steps per kernel with the state in registers
+        return pointwise.solve_chunk(self, ctxs, y0, outs, 'euler'), ()
 
     def _step(self, c, y0, extra0, out):
-        L, nz, f, g = self._f_and_g_prod(c, c.t0, y0)
+        if pointwise.ready(self):
+            # a single step is a chunk of one
+            return self._step_chunk([c], y0, extra0, [out if out is not None else torch.empty_like(y0)])
+        # the first step of an eligible solve runs as always, with the user's two evaluations recorded
+        rec = pointwise.pc_recorder(self, y0, c.t0, 'fg')
+        L, nz, f, g = self._f_and_g_prod(c, c.t0, y0, rec)
+        if rec is not None:
+            self._pw = rec.finish() or False
         return self._k('tsde_step_euler', L, nz, (y0, f, g), (c.dt,), out), ()
 
 
@@ -101,6 +118,7 @@ class BaseMilstein(_ProdMixin, base_solver.BaseSDESolver):
     noise_types = (NOISE_TYPES.additive, NOISE_TYPES.diagonal, NOISE_TYPES.scalar)
     levy_area_approximations = LEVY_AREA_APPROXIMATIONS.all()
     ito = None
+    _pw_method = 'milstein'
 
     def __init__(self, sde, options, **kwargs):
         # milstein.py:29-41
@@ -128,7 +146,7 @@ class BaseMilstein(_ProdMixin, base_solver.BaseSDESolver):
 
     def _step_chunk(self, ctxs, y0, extra0, outs):
         # the recorded element-wise program (pointwise.py), several steps per kernel with the state in registers
-        return pointwise.solve_chunk(self, ctxs, y0, outs, 1 if self.ito else 0), ()
+        return pointwise.solve_chunk(self, ctxs, y0, outs, 'milstein', ito=1 if self.ito else 0), ()
 
     def _step(self, c, y0, extra0, out):
         sde = self.sde
@@ -321,9 +339,14 @@ class ReversibleHeun(base_solver.BaseSDESolver):
     noise_types = NOISE_TYPES.all()
     levy_area_approximations = LEVY_AREA_APPROXIMATIONS.all()
 
+    _pw_method = 'reversible_heun'
+
     def __init__(self, sde, **kwargs):
         self.strong_order = 1.0 if sde.noise_type == NOISE_TYPES.additive else 0.5
         super(ReversibleHeun, self).__init__(sde=sde, **kwargs)
+        self._pw = None  # the element-wise programs of the step (pointwise.py), False once rejected
+        self._halves = False  # per solve: pointwise.halves_exactly of its steps
+        self._pw_state = None  # per solve: the two alternating (f, g, z) sets the chunks store their state to
 
     def scalars(self, dt):
         return {'half_dt': float(0.5 * dt)}
@@ -331,10 +354,52 @@ class ReversibleHeun(base_solver.BaseSDESolver):
     def init_extra_solver_state(self, t0, y0):
         return self.sde.f_and_g(t0, y0) + (y0,)
 
+    def _run(self, sched, ctxs, ys, extra):
+        self._halves = pointwise.halves_exactly(self.dtype, ctxs)
+        self._pw_state = None  # allocated at the solve's first chunk (under capture, from the graph's pool)
+        return super()._run(sched, ctxs, ys, extra)
+
+    def _chunks_ready(self):
+        return self._halves and pointwise.ready(self)
+
+    def _step_chunk(self, ctxs, y0, extra0, outs):
+        state = tuple(_contig(x) for x in extra0)
+        if not pointwise.state_fits(self, state):
+            # a state the kernel cannot read (a captured solve starts from the caller's): the ordinary steps
+            y1 = y0
+            for c, out in zip(ctxs, outs):
+                y1, extra0 = self._unfused_step(c, y1, extra0, out)
+            return y1, extra0
+        if self._pw_state is None:
+            self._pw_state = [tuple(torch.empty_like(y0) for _ in range(3)) for _ in range(2)]
+        # the recorded element-wise programs (pointwise.py), several steps per kernel with y, z, f and g in registers;
+        # the chunk stores its state to the set it does not read
+        a, b = self._pw_state
+        f1, g1, z1 = b if state[0] is a[0] else a
+        f0, g0, z0 = state
+        y1 = pointwise.solve_chunk(self, ctxs, y0, outs, 'reversible_heun', state=((z0, f0, g0), (z1, f1, g1)))
+        return y1, (f1, g1, z1)
+
     def _step(self, c, y0, extra0, out):
+        if self._chunks_ready():
+            # a single step is a chunk of one
+            return self._step_chunk([c], y0, extra0, [out if out is not None else torch.empty_like(y0)])
+        return self._unfused_step(c, y0, extra0, out)
+
+    def _unfused_step(self, c, y0, extra0, out):
+        sde = self.sde
         f0, g0, z0 = (_contig(x) for x in extra0)
         z1 = self._k('tsde_reversible_heun_z', self._L, self._feed.get(c), (y0, z0, f0, g0), (c.dt,), None)
-        f1, g1 = self._f_and_g(c.t1, z1)
+        # the first step of an eligible solve runs as always, with the user's f and g at (t1, z1) recorded
+        rec = None
+        if self._halves and pointwise.state_fits(self, (f0, g0, z0)):
+            rec = pointwise.pc_recorder(self, z1, c.t1, 'fg')
+        if rec is not None:
+            f1, g1 = self._fork(lambda: rec.evaluation('f', lambda: sde.f(c.t1, z1), c.t1, z1),
+                                lambda: rec.evaluation('g', lambda: sde.g(c.t1, z1), c.t1, z1))
+            self._pw = rec.finish() or False
+        else:
+            f1, g1 = self._f_and_g(c.t1, z1)
         f1, g1 = _contig(f1), _contig(g1)
         y1 = self._k('tsde_step_reversible_heun', self._L, self._feed.get(c), (y0, f0, f1, g0, g1),
                      (c.scalars['half_dt'],), out)

@@ -1,5 +1,5 @@
-"""Element-wise tapes of the user's SDE: a diagonal-noise Milstein, SRK, Heun, midpoint or Euler-Heun step as one
-kernel.
+"""Element-wise tapes of the user's SDE: a diagonal-noise Milstein, SRK, Heun, midpoint, Euler-Heun, Euler or
+reversible-Heun step as one kernel.
 
 When the SDE's callables are made only of element-wise ATen ops whose CUDA result is one IEEE rounding per element,
 a whole step is one launch that reads y0 and writes y1 (include/torchsde_b200.h, csrc/pointwise.cu) instead of the
@@ -45,6 +45,16 @@ The Stratonovich predictor-corrector steps (methods.Heun, Midpoint, EulerHeun) e
 at the predicted state (g only for Euler-Heun).  They are recorded and compiled as SRK's are, with the full register
 bound.  Only SDEs whose f and g the step calls as two separate callables are recorded (`pc_recorder`): a user
 `f_and_g`, `g_prod` or `f_and_g_prod`, and the adjoint SDE of `sdeint_adjoint`'s backward, keep the ordinary step.
+
+Euler and reversible Heun (`pc_recorder` with pattern 'fg', tsde_solve_euler_pointwise,
+tsde_solve_reversible_heun_pointwise).  Both evaluate f and g once per step: Euler at (t0, y0), reversible Heun at
+(t1, z1), after its z kernel (methods.Euler, ReversibleHeun).  They are recorded as Heun is and run as Milstein does:
+up to TSDE_PW_MAX_STEPS steps per launch once the batch fills the GPU, a single step being a chunk of one.
+Reversible Heun's solver state (f, g, z) stays in registers inside a chunk and is stored at its end, alternately to
+two sets of solver-owned buffers; its half step T(0.5) * T(dt) must equal the unfused step's half_dt at every step
+(`halves_exactly`), and the state it starts from must be (rows, d) tensors of the state dtype (`state_fits`), else
+the solve keeps the ordinary step.  `sdeint_adjoint`'s forward solve is a no-grad solve, so the reversible pair's
+forward steps fuse too.
 """
 import ctypes
 import numbers
@@ -436,7 +446,8 @@ class SrkRecorder(Recorder):
 
 def recording(solver):
     """Whether this step of `solver` (its `_pw` is the program, None before the first step, False once rejected)
-    is the one to record."""
+    is the one to record: the first diagonal-noise step of an `eligible` solve (for reversible Heun, the first whose
+    solver state the chunk kernel can read, methods.ReversibleHeun)."""
     return solver._pw is None and solver.sde.noise_type == NOISE_TYPES.diagonal and eligible(solver)
 
 
@@ -466,11 +477,10 @@ def launch(solver, name, nz, y0, args, out):
 
 
 def plan_chunks(first, n_steps, interpolated=(), multi_cell=(), max_steps=_cabi.PW_MAX_STEPS):
-    """Steps [first, n_steps) of a fixed-step solve grouped into the launches of its element-wise Milstein program, as
-    (k0, k1) ranges of at most `max_steps` consecutive steps.  Inside a chunk a state lives in registers only, so a
-    chunk ends where a step's state has to be in memory for someone else:
-      * a step in `multi_cell` (it spans several Brownian cells; tsde_solve_milstein_pointwise draws one cell per
-        step) runs alone;
+    """Steps [first, n_steps) of a fixed-step solve grouped into the launches of its element-wise program (Milstein,
+    Euler, reversible Heun), as (k0, k1) ranges of at most `max_steps` consecutive steps.  Inside a chunk a state lives
+    in registers only, so a chunk ends where a step's state has to be in memory for someone else:
+      * a step in `multi_cell` (it spans several Brownian cells; the chunk kernels draw one cell per step) runs alone;
       * a step in `interpolated` (a non-aligned output falls inside it) runs alone, and the step before it ends a
         chunk: the interpolation reads the states before and after the step.
     Aligned outputs do not end a chunk: the kernel stores those rows as it passes them."""
@@ -483,39 +493,72 @@ def plan_chunks(first, n_steps, interpolated=(), multi_cell=(), max_steps=_cabi.
     return out
 
 
+# Resident CTAs (256 threads) per SM of each chunked kernel, (float32, float64), from its registers (-Xptxas -v,
+# sm_90a: 64 K registers per SM): Milstein; Euler at 56 and 102-110 registers; reversible Heun at 78-79 and 118-128.
+_RESIDENT_CTAS = {'milstein': (4, 2), 'euler': (4, 2), 'reversible_heun': (3, 2)}
+
+
 def chunk_length(solver):
-    """Steps per launch of the element-wise Milstein program: TSDE_PW_MAX_STEPS when the batch fills the GPU with at
-    least one wave of the kernel's CTAs (256 quads each, 4 resident per SM in float32 and 2 in float64), else 1.  A
-    smaller grid leaves SMs idle; consecutive one-step kernels fill them by overlapping one step's tail with the next
-    one's start (programmatic dependent launch), which a chunk, whose steps are sequential per thread, cannot.  (On an
-    H100 at B = 4096, D = 64, fp32, one session alternating the two: 3.3 us per step one step per launch, 4.3 in
-    chunks of 64.)"""
+    """Steps per launch of the solver's element-wise program (`solver._pw_method`: 'milstein', 'euler' or
+    'reversible_heun'): TSDE_PW_MAX_STEPS when the batch fills the GPU with at least one wave of its chunk kernel's
+    CTAs (256 quads each, _RESIDENT_CTAS per SM), else 1.  A smaller grid leaves SMs idle; consecutive one-step kernels
+    fill them by overlapping one step's tail with the next one's start (programmatic dependent launch), which a chunk,
+    whose steps are sequential per thread, cannot.  (On an H100 at B = 4096, D = 64, fp32, Milstein, one session
+    alternating the two: 3.3 us per step one step per launch, 4.3 in chunks of 64.)"""
     if solver.device.type != 'cuda':  # (the host-side dry run of the tests; a solve always runs on a CUDA device)
         return _cabi.PW_MAX_STEPS
     ctas = solver.rows * ((solver.d + 3) // 4) / 256
     wave = torch.cuda.get_device_properties(solver.device).multi_processor_count * (
-        4 if solver.dtype == torch.float32 else 2)
+        _RESIDENT_CTAS[solver._pw_method][0 if solver.dtype == torch.float32 else 1])
     return _cabi.PW_MAX_STEPS if ctas >= wave else 1
 
 
-def solve_chunk(solver, ctxs, y0, outs, ito):
-    """Consecutive single-cell Milstein steps `ctxs` from y0 as one launch of tsde_solve_milstein_pointwise on the
-    solver's program.  Step j's y1 is stored to outs[j] (None: kept in registers only; the last must be given)."""
+def solve_chunk(solver, ctxs, y0, outs, method, ito=0, state=None):
+    """Consecutive single-cell steps `ctxs` of `method` ('milstein', 'euler' or 'reversible_heun') from y0 as one
+    launch of its tsde_solve_*_pointwise on the solver's program.  Step j's y1 is stored to outs[j] (None: kept in
+    registers only; the last must be given).  `ito` is Milstein's; `state` is reversible Heun's ((z0, f0, g0) the chunk
+    starts from, (z1, f1, g1) where it leaves its state)."""
     prog, _ = solver._pw
     feed = solver._feed
     nz = feed.get(ctxs[0])
     steps = (_cabi.PwStep * len(ctxs))()
     for s, c, out in zip(steps, ctxs, outs):
         s.cell_id, s.h, _ = feed.binding.cell(c.k)
-        s.dt, s.t0, s.y1 = c.dt, c.t0.data_ptr(), None if out is None else out.data_ptr()
-    _cabi.check(solver._lib.tsde_solve_milstein_pointwise(solver._L, nz, ctypes.byref(prog), y0.data_ptr(), steps,
-                                                         len(ctxs), ito), 'tsde_solve_milstein_pointwise')
+        # the time the program runs at: reversible Heun evaluates f and g at t1 (reversible_heun.py:70)
+        t = c.t1 if method == 'reversible_heun' else c.t0
+        s.dt, s.t0, s.y1 = c.dt, t.data_ptr(), None if out is None else out.data_ptr()
+    lib, args = solver._lib, (solver._L, nz, ctypes.byref(prog), y0.data_ptr())
+    name = f'tsde_solve_{method}_pointwise'
+    if method == 'milstein':
+        code = lib.tsde_solve_milstein_pointwise(*args, steps, len(ctxs), ito)
+    elif method == 'euler':
+        code = lib.tsde_solve_euler_pointwise(*args, steps, len(ctxs))
+    else:
+        state_in, state_out = state
+        code = lib.tsde_solve_reversible_heun_pointwise(*args, *(x.data_ptr() for x in state_in), steps, len(ctxs),
+                                                         *(x.data_ptr() for x in state_out))
+    _cabi.check(code, name)
     return outs[-1]
 
 
+def halves_exactly(dtype, ctxs):
+    """Whether every step of `ctxs` has the half step reversible Heun's chunk kernel forms, T(0.5) * T(dt) in the state
+    dtype T, equal to the unfused step's half_dt (0.5 * dt rounded once to T).  Halving is exact, so the two differ
+    only where the result is subnormal in T; a solve with such a step keeps the ordinary step."""
+    t = np.float32 if dtype == torch.float32 else np.float64
+    return all(t(0.5) * t(c.dt) == t(c.scalars['half_dt']) for c in ctxs)
+
+
+def state_fits(solver, tensors):
+    """Whether solver-state tensors (reversible Heun's f, g, z) are what a chunk kernel reads: contiguous (rows, d)
+    tensors of the state dtype on the state's device."""
+    return all(torch.is_tensor(x) and tuple(x.shape) == (solver.rows, solver.d) and x.dtype == solver.dtype
+               and x.device == solver.device and x.is_contiguous() for x in tensors)
+
+
 def eligible(solver):
-    """Whether a fixed-step Milstein, SRK, Heun, midpoint or Euler-Heun solve may run its diagonal-noise steps as
-    element-wise programs: no gradients, a Brownian motion bound to the solver grid (counter noise), `overlap` not
+    """Whether a fixed-step Milstein, SRK, Heun, midpoint, Euler-Heun, Euler or reversible-Heun solve may run its
+    diagonal-noise steps as element-wise programs: no gradients (the forward solve of `sdeint_adjoint` has none), a Brownian motion bound to the solver grid (counter noise), `overlap` not
     False, no logqp and no autocast."""
     from .base_sde import SDELogqp
     sde = solver.sde

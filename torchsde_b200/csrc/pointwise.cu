@@ -1,7 +1,8 @@
 // Whole steps of an element-wise SDE as one kernel: tsde_step_milstein_pointwise (and tsde_solve_milstein_pointwise,
-// up to TSDE_PW_MAX_STEPS consecutive Milstein steps in one kernel), tsde_step_srk_diag_pointwise and
-// tsde_step_predictor_corrector_pointwise (include/torchsde_b200.h describes the tsde_pointwise program and its two
-// layouts).
+// up to TSDE_PW_MAX_STEPS consecutive Milstein steps in one kernel), tsde_step_srk_diag_pointwise,
+// tsde_step_predictor_corrector_pointwise, and tsde_solve_euler_pointwise and tsde_solve_reversible_heun_pointwise
+// (up to TSDE_PW_MAX_STEPS Euler or reversible-Heun steps in one kernel) (include/torchsde_b200.h describes the
+// tsde_pointwise program and its two layouts).
 //
 // The SDE's f and g (and for Milstein the vjp of g) arrive as a small program of element-wise instructions.  Each
 // kernel interprets it between the unfused step's own ops (tableau_diag_ops.cuh), one IEEE rounding per element
@@ -484,6 +485,95 @@ pw_pc_kernel(const __grid_constant__ tsde_pointwise pg, const PwPcP<T> p, const 
   store_quad(p.base.y1, c.base, c.vec, c.nvalid, y1);
 }
 
+// ---- consecutive Euler or reversible-Heun steps (tsde_solve_euler_pointwise, tsde_solve_reversible_heun_pointwise) --
+// The chunked loop of pw_milstein_kernel around the two-program layout: one thread runs up to kPwMaxSteps steps of
+// its quad, draws step j's increment from st.s[j].cell, and stores y1 only where st.s[j].y1 is given.  Per step:
+//   Euler            f, g at (t, y);  y <- EulerOp{dt}                                       (euler.py:36)
+//   reversible Heun  z1 = RevHeunZOp{dt}(y, z, f, g);  f1, g1 at (t, z1);
+//                    y1 = RevHeunOp{dt/2}(y, f, f1, g, g1);  (y, z, f, g) <- (y1, z1, f1, g1) (reversible_heun.py:69-71)
+// where t is st.s[j].t0, the time the program runs at: the step's t0 for Euler, its t1 for reversible Heun.  dt/2 is
+// T(0.5) * dt, which equals the host-rounded (T)(0.5 * dt) of the unfused step whenever that is a normal number (the
+// caller checks).  Reversible Heun's solver state (z, f, g) is read once at the chunk's start and stored once at its
+// end, to pointers the chunk does not read: its whole state stays in registers in between.
+enum { kPwEuler = 0, kPwReversibleHeun = 1 };
+
+template <typename T>
+struct PwChunkP {
+  PwP<T> base;           // y0, the quad mapping (base.y1, t0, dt and ito unused: the step table has them)
+  const T *z0, *f0, *g0;  // reversible Heun: the solver state the chunk starts from
+  T *z1, *f1, *g1;        // and where the chunk leaves it
+};
+static_assert(sizeof(tsde_pointwise) + sizeof(PwChunkP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <=
+                  4096,
+              "the chunk kernel's parameters fit the 4 KiB parameter space");
+
+template <typename T, int SRC, int METHOD>
+__global__ void __launch_bounds__(kThreads, 1)
+pw_chunk_kernel(const __grid_constant__ tsde_pointwise pg, const PwChunkP<T> p, const NoiseP<T> nz,
+                const __grid_constant__ PwSteps<T> st) {
+  extern __shared__ __align__(16) unsigned char pw_regs[];
+  PwQuad<T> c;
+  int64_t Q, row, q;
+  pw_locate(p.base, c, Q, row, q);
+  const Key key = load_key(nz.key);
+  T y[4], z[4], f[4], g[4];
+  for (int j = 0; j < st.n; ++j) {
+    const PwStep<T>& s = st.s[j];
+    T w[4], u[4];
+    NoiseP<T> n = nz;  // this step's cell
+    n.cell_id = s.cell;
+    n.sqrt_h = s.sqrt_h;
+    quad_noise<T, SRC, false>(n, key, row, q, c.vec, c.nvalid, w, u);
+    if (j == 0) {  // the first increment is drawn while the previous kernel drains; the state is read after the wait
+      asm volatile("griddepcontrol.wait;" ::: "memory");
+      if (Q >= p.base.nquads) return;
+      load_quad(p.base.y0, c.base, c.vec, c.nvalid, y);
+      if constexpr (METHOD == kPwReversibleHeun) {
+        load_quad(p.z0, c.base, c.vec, c.nvalid, z);
+        load_quad(p.f0, c.base, c.vec, c.nvalid, f);
+        load_quad(p.g0, c.base, c.vec, c.nvalid, g);
+      }
+    }
+    if constexpr (METHOD == kPwEuler) {
+      pw_eval(pg, c, pw_regs, false, s.t0, y, f);
+      pw_eval(pg, c, pw_regs, true, s.t0, y, g);
+      const EulerOp<T> step{s.dt};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        T o[1];
+        step({y[i], f[i], g[i]}, w[i], u[i], o);
+        y[i] = o[0];
+      }
+    } else {
+      const RevHeunZOp<T> zop{s.dt};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        T o[1];
+        zop({y[i], z[i], f[i], g[i]}, w[i], u[i], o);
+        z[i] = o[0];
+      }
+      T f1[4], g1[4];
+      pw_eval(pg, c, pw_regs, false, s.t0, z, f1);
+      pw_eval(pg, c, pw_regs, true, s.t0, z, g1);
+      const RevHeunOp<T> step{T(0.5) * s.dt};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        T o[1];
+        step({y[i], f[i], f1[i], g[i], g1[i]}, w[i], u[i], o);
+        y[i] = o[0];
+        f[i] = f1[i];
+        g[i] = g1[i];
+      }
+    }
+    if (s.y1) store_quad(s.y1, c.base, c.vec, c.nvalid, y);
+  }
+  if constexpr (METHOD == kPwReversibleHeun) {
+    store_quad(p.z1, c.base, c.vec, c.nvalid, z);
+    store_quad(p.f1, c.base, c.vec, c.nvalid, f);
+    store_quad(p.g1, c.base, c.vec, c.nvalid, g);
+  }
+}
+
 // ---- launch ---------------------------------------------------------------------------------------------------------
 // The noise and the part of the kernel parameters every pointwise step has (y0, y1, the quad mapping, vec) for a
 // program that passes `layout`; TSDE_EINVAL for a launch the kernels cannot serve.
@@ -547,6 +637,66 @@ static int pw_milstein_chunk(const tsde_launch* L, const tsde_noise* nz, const t
   p.ito = ito;
   return pw_launch<T>(L, *prog, pw_milstein_kernel<T, TSDE_SRC_COUNTER>, pw_milstein_kernel<T, kSrcCounterMulti>, p,
                       np, p.nquads, prog->n_regs, TSDE_KERNEL_PW_MILSTEIN, st);
+}
+
+// The chunk `steps[0, n_steps)` of Euler or reversible Heun from y0 (and, for reversible Heun, from the solver state
+// in[] = z0, f0, g0, left in out[] = z1, f1, g1): one launch of pw_chunk_kernel, under the rules of
+// pw_milstein_chunk.
+template <typename T, int METHOD>
+static int pw_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
+                    const tsde_pw_step* steps, int32_t n_steps, const void* const (&in)[3], void* const (&out)[3]) {
+  if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
+  PwChunkP<T> p{};
+  NoiseP<T> np;
+  if (int e = pw_prepare<T>(L, nz, prog, y0, steps[n_steps - 1].y1, pw_valid_two<TSDE_PW_MAX_REGS>, p.base, np))
+    return e;
+  if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
+  if constexpr (METHOD == kPwReversibleHeun) {
+    for (int i = 0; i < 3; ++i) {
+      if (!in[i] || !out[i]) return TSDE_EINVAL;
+      if (!aligned16(in[i]) || !aligned16(out[i])) p.base.vec = 0;
+    }
+    p.z0 = static_cast<const T*>(in[0]);
+    p.f0 = static_cast<const T*>(in[1]);
+    p.g0 = static_cast<const T*>(in[2]);
+    p.z1 = static_cast<T*>(out[0]);
+    p.f1 = static_cast<T*>(out[1]);
+    p.g1 = static_cast<T*>(out[2]);
+  }
+  PwSteps<T> st{};
+  st.n = n_steps;
+  for (int j = 0; j < n_steps; ++j) {
+    const tsde_pw_step& s = steps[j];
+    if (!s.t0) return TSDE_EINVAL;
+    if (s.y1 && !aligned16(s.y1)) p.base.vec = 0;
+    st.s[j] = PwStep<T>{s.cell_id, static_cast<const T*>(s.t0), static_cast<T*>(s.y1), (T)sqrt(s.h), (T)s.dt};
+  }
+  np.cell_id = steps[0].cell_id;
+  np.h = steps[0].h;
+  return pw_launch<T>(L, *prog, pw_chunk_kernel<T, TSDE_SRC_COUNTER, METHOD>, pw_chunk_kernel<T, kSrcCounterMulti, METHOD>,
+                      p, np, p.base.nquads, prog->n_regs, TSDE_KERNEL_PW_CHUNK, st);
+}
+
+TSDE_EXPORT int tsde_solve_euler_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                           const void* y0, const tsde_pw_step* steps, int32_t n_steps) {
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
+  const void* const in[3] = {};
+  void* const out[3] = {};
+  return dispatch(L, [&](auto t) -> int {
+    return pw_chunk<decltype(t), kPwEuler>(L, nz, prog, y0, steps, n_steps, in, out);
+  });
+}
+
+TSDE_EXPORT int tsde_solve_reversible_heun_pointwise(const tsde_launch* L, const tsde_noise* nz,
+                                                     const tsde_pointwise* prog, const void* y0, const void* z0,
+                                                     const void* f0, const void* g0, const tsde_pw_step* steps,
+                                                     int32_t n_steps, void* z1, void* f1, void* g1) {
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
+  const void* const in[3] = {z0, f0, g0};
+  void* const out[3] = {z1, f1, g1};
+  return dispatch(L, [&](auto t) -> int {
+    return pw_chunk<decltype(t), kPwReversibleHeun>(L, nz, prog, y0, steps, n_steps, in, out);
+  });
 }
 
 TSDE_EXPORT int tsde_step_milstein_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
