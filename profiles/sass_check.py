@@ -1,7 +1,10 @@
 """Static SASS evidence for the shipped library (no GPU needed): per kernel family, registers / spills and the
 counts of the instructions that carry the design — 128-bit global loads/stores, evict-first loads, bulk copies
 (UBLKCP) and mbarrier ops (SYNCS) of the TMA-staged tile kernel, SFU ops of the in-register Box-Muller, and the
-absence of FFMA in the tableau kernels that follow the reference's separately rounded op order (-fmad=false).
+absence of FFMA in the tableau kernels that follow the reference's separately rounded op order (-fmad=false).  In the
+chunked pointwise kernels it checks the element-wise program's interpreter loops (the innermost loops that load and
+store the shared-memory register file): the loop that runs programs whose operands all sit in shared memory reads no
+global memory (LDG) and decodes no byte fields from the parameter space (LDC.U8); exit status 1 otherwise.
 
     python profiles/sass_check.py > out/sass_evidence.txt
 """
@@ -47,8 +50,28 @@ PICK = [  # (label, regex on the demangled kernel name)
     ('bmm(g, A) of the log-ODE correction, fp32, m = 16', r'bmm_ga_kernel<float, 16>'),
     ('logqp KL-integrand augmentation, fp32', r'logqp_augment_kernel<float>'),
 ]
+INTERPRETED = [r'pw_milstein_kernel<float, 1>', r'pw_milstein_kernel<double, 1>', r'pw_chunk_kernel<float, 1, 0>',
+               r'pw_chunk_kernel<double, 1, 0>', r'pw_chunk_kernel<float, 1, 1>', r'pw_chunk_kernel<double, 1, 1>']
 COUNT = ['LDG.E.128', 'LDG.E.EF.128', 'STG.E.128', 'LDS.128', 'UBLKCP', 'SYNCS', 'MUFU', 'FFMA', 'FMUL', 'FADD', 'DFMA',
          'SHFL', 'BAR.SYNC', 'LDL', 'STL', 'IMAD.WIDE']
+
+
+def interpreter_loops(sass):
+    """The innermost loops (a backward branch and its target, holding no other backward branch) that load and store
+    the shared-memory register file, as lists of instructions."""
+    ins = []
+    for ln in sass.splitlines():
+        m = re.match(r'\s+/\*([0-9a-f]{4,})\*/\s+(.*?);', ln)
+        if m:
+            ins.append((int(m.group(1), 16), m.group(2)))
+    back = []
+    for i, (addr, op) in enumerate(ins):
+        m = re.search(r'\bBRA\s+(?:`\()?0x([0-9a-f]+)', op)
+        if m and int(m.group(1), 16) < addr:
+            back.append((int(m.group(1), 16), addr))
+    inner = [(a, b) for a, b in back if not any(a <= c < d <= b and (c, d) != (a, b) for c, d in back)]
+    loops = [[op for addr, op in ins if a <= addr <= b] for a, b in inner]
+    return [body for body in loops if any('LDS.128' in o for o in body) and any('STS.128' in o for o in body)]
 
 
 def main():
@@ -85,6 +108,17 @@ def main():
         print(f"## {label}\n   {d.split('(')[0]}\n   instructions {len(ops)}  REG {reg}  STACK {stack}  SHARED(static) {shared}  LOCAL {local}")
         cnt = {k: sum(1 for o in ops if re.search(r'\b' + re.escape(k) + r'\b', o)) for k in COUNT}
         print('   ' + '  '.join(f"{k}={v}" for k, v in cnt.items() if v) + '\n')
+    bad = 0
+    for pat in INTERPRETED:
+        hit = [n for n, d in zip(names, dem) if re.search(pat, d)]
+        sass = subprocess.run(['cuobjdump', '-sass', '-fun', hit[0], LIB], capture_output=True, text=True).stdout
+        loops = interpreter_loops(sass)
+        clean = [b for b in loops if not any(re.search(r'\bLDG\b|\bLDC\.U8\b', o) for o in b)]
+        sizes = ', '.join(str(len(b)) for b in clean)
+        print(f"## interpreter loops of {pat}: {len(loops)}, of which {len(clean)} read only shared memory and the"
+              f" instruction word ({sizes} instructions)")
+        bad += not clean
+    sys.exit(1 if bad else 0)
 
 
 if __name__ == '__main__':

@@ -494,7 +494,8 @@ def plan_chunks(first, n_steps, interpolated=(), multi_cell=(), max_steps=_cabi.
 
 
 # Resident CTAs (256 threads) per SM of each chunked kernel, (float32, float64), from its registers (-Xptxas -v,
-# sm_90a: 64 K registers per SM): Milstein; Euler at 56 and 102-110 registers; reversible Heun at 78-79 and 118-128.
+# sm_90a: 64 K registers per SM): Milstein at 58-59 and 88-92 registers; Euler at 54 and 88-96; reversible Heun at 72
+# and 110-120.
 _RESIDENT_CTAS = {'milstein': (4, 2), 'euler': (4, 2), 'reversible_heun': (3, 2)}
 
 

@@ -7,14 +7,14 @@
 // The SDE's f and g (and for Milstein the vjp of g) arrive as a small program of element-wise instructions.  Each
 // kernel interprets it between the unfused step's own ops (tableau_diag_ops.cuh), one IEEE rounding per element
 // (this translation unit is compiled with -fmad=false, as the tableaus are), so a fused step equals the unfused one
-// bit for bit.  The file holds, in this order: the program's register file and interpreter, the validation every
-// program passes before a launch, the prologue the kernels share, the kernels with the layout each accepts, and the
-// launch.
+// bit for bit.  The file holds, in this order: the decoded program, its register file and interpreter, the validation
+// every program passes before a launch and the decoding that follows it, the prologue the kernels share, the kernels
+// with the layout each accepts, and the launch.
 //
 // One thread per quad, as ew_fast_kernel.  The program's registers live in shared memory as 16-byte vectors laid
 // out [reg][plane][thread] (a float quad is one plane, a double quad two): a warp's 128-bit access is 512 contiguous
 // bytes, conflict-free.  A dynamically indexed per-thread array would live in local memory instead.  The state, go,
-// the SDE's results and the increments stay in registers.
+// the SDE's results and the increments stay in registers; the program reads y and go from their own slots.
 #include "tableau_diag_ops.cuh"
 
 namespace tsde {
@@ -33,65 +33,103 @@ struct PwP {
   int32_t ito;
 };
 
-// ---- the interpreter ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void pw_sload(const void* s, int r, float (&v)[4]) {
-  const float4 x = static_cast<const float4*>(s)[r * kThreads + threadIdx.x];
-  v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
-}
-__device__ __forceinline__ void pw_sstore(void* s, int r, const float (&v)[4]) {
-  static_cast<float4*>(s)[r * kThreads + threadIdx.x] = make_float4(v[0], v[1], v[2], v[3]);
-}
-__device__ __forceinline__ void pw_sload(const void* s, int r, double (&v)[4]) {
-  const double2* p = static_cast<const double2*>(s) + 2 * r * kThreads + threadIdx.x;
-  const double2 a = p[0], b = p[kThreads];
-  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
-}
-__device__ __forceinline__ void pw_sstore(void* s, int r, const double (&v)[4]) {
-  double2* p = static_cast<double2*>(s) + 2 * r * kThreads + threadIdx.x;
-  p[0] = make_double2(v[0], v[1]);
-  p[kThreads] = make_double2(v[2], v[3]);
-}
+// ---- the decoded program --------------------------------------------------------------------------------------------
+// pw_prepare decodes the caller's tsde_pointwise once per launch into a PwProg, in which every source is a slot of the
+// shared-memory register file:
+//   [0, n_regs)  the program's registers
+//   y            the state the program runs at, stored there before each evaluation
+//   go           the Milstein seed (Milstein layout only)
+//   t0           the evaluation's time, stored once per evaluation (when a TSDE_PW_T0 operand is read)
+//   u            the launch-uniform values: IMM and SCALAR operands, one per "thread" lane of the slot, written once
+//                per launch after the dependency wait
+//   hoisted      one slot per CHANNEL / ROW operand, this thread's quad of it, loaded once per launch after the wait
+//   end          the first slot past the layout (SRK's fp64 stash starts there)
+// A source is then one 16-byte-vector load at (slot, lane): lane = threadIdx.x, or the entry's lane of the u slot (a
+// broadcast).  CHANNEL / ROW operands past kPwHoistSlots are read from global memory at every use instead.
+//
+// An instruction is one word: op in bits [0, 3), dst in [3, 8), source a in [8, 20), source b in [20, 32) (b = a for
+// NEG and SQRT).  A source is a slot in bits [0, 5), with kPwSrcUniform its lane in bits [6, 11); or kPwSrcGlobal and
+// the index of its operand in bits [0, 5).
+constexpr uint32_t kPwSrcUniform = 1u << 5, kPwSrcGlobal = 1u << 11;
+
+// CHANNEL / ROW operands are hoisted into slots only while the layout stays within kPwHoistSlots slots, the footprint
+// of a program of TSDE_PW_MAX_REGS registers: hoisting never raises a program's shared memory past what the library's
+// largest program takes.  Registers, y, go, t0 and u always have their slots, at most TSDE_PW_MAX_REGS + 4.
+constexpr int kPwHoistSlots = TSDE_PW_MAX_REGS;
+constexpr int kPwMaxSlots = TSDE_PW_MAX_REGS + 4;
+static_assert(kPwMaxSlots * kThreads * 4 * sizeof(double) <= 227 * 1024,
+              "every accepted program's fp64 register file fits one CTA's shared memory");
+static_assert(kPwMaxSlots <= 32 && TSDE_PW_MAX_OPERANDS <= 32, "slots and operand indices fit five bits");
 
 template <typename T>
-struct PwQuad {  // where this thread's quad lives, and the values a program source may name besides registers
-  int64_t base, chan;
-  int nvalid;
-  bool vec;
-  const T* t;  // what a TSDE_PW_T0 operand reads: the time of the evaluation being run
-  T y[4], go[4];
+struct PwOperand {
+  const T* ptr;  // SCALAR, CHANNEL, ROW; null for IMM
+  T imm;
 };
 
 template <typename T>
-__device__ __forceinline__ void pw_fetch(const tsde_pointwise& pg, const PwQuad<T>& c, const void* regs, uint32_t s,
+struct PwProg {
+  int32_t n_fg, n_instr;
+  uint16_t f_src, g_src, gdg_src;
+  int8_t y, go, t0, u, hoist, end;  // slots (t0: -1 when no operand reads the time)
+  int8_t n_uniform, n_hoisted;      // operand[0, n_uniform) fill the u slot, the next n_hoisted the hoisted slots
+  int8_t n_global;                  // the operands past those, read from global memory at every use
+  uint32_t row;                     // bit k: operand[k] is a ROW operand (else CHANNEL)
+  uint32_t instr[TSDE_PW_MAX_INSTR];
+  PwOperand<T> operand[TSDE_PW_MAX_OPERANDS];
+};
+
+// ---- the interpreter ------------------------------------------------------------------------------------------------
+// slot r, lane l: float4 r * kThreads + l; a double quad is the double2 pair 2 r kThreads + l and that + kThreads
+__device__ __forceinline__ void pw_sload(const void* s, int r, int l, float (&v)[4]) {
+  const float4 x = static_cast<const float4*>(s)[r * kThreads + l];
+  v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
+}
+__device__ __forceinline__ void pw_sstore(void* s, int r, int l, const float (&v)[4]) {
+  static_cast<float4*>(s)[r * kThreads + l] = make_float4(v[0], v[1], v[2], v[3]);
+}
+__device__ __forceinline__ void pw_sload(const void* s, int r, int l, double (&v)[4]) {
+  const double2* p = static_cast<const double2*>(s) + 2 * r * kThreads + l;
+  const double2 a = p[0], b = p[kThreads];
+  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
+}
+__device__ __forceinline__ void pw_sstore(void* s, int r, int l, const double (&v)[4]) {
+  double2* p = static_cast<double2*>(s) + 2 * r * kThreads + l;
+  p[0] = make_double2(v[0], v[1]);
+  p[kThreads] = make_double2(v[2], v[3]);
+}
+template <typename T>
+__device__ __forceinline__ void pw_sstore(void* s, int r, const T (&v)[4]) {
+  pw_sstore(s, r, threadIdx.x, v);
+}
+
+struct PwQuad {  // where this thread's quad lives
+  int64_t base, chan;
+  int nvalid;
+  bool vec;
+};
+
+// GLOBAL: the source may be a CHANNEL / ROW operand that did not fit the slots, read from global memory
+template <bool GLOBAL = true, typename T>
+__device__ __forceinline__ void pw_fetch(const PwProg<T>& pg, const PwQuad& c, const void* regs, uint32_t s,
                                          T (&v)[4]) {
-  if (s == TSDE_PW_SRC_Y || s == TSDE_PW_SRC_GO) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) v[j] = s == TSDE_PW_SRC_Y ? c.y[j] : c.go[j];
+  if (GLOBAL && (s & kPwSrcGlobal)) {
+    const int k = s & 31;
+    load_quad(pg.operand[k].ptr, (pg.row >> k) & 1 ? c.base : c.chan, c.vec, c.nvalid, v);
     return;
   }
-  if (s < (uint32_t)TSDE_PW_OPERAND(0)) {
-    pw_sload(regs, (int)s, v);
-    return;
-  }
-  const tsde_pw_operand& o = pg.operand[s - TSDE_PW_OPERAND(0)];
-  if (o.kind == TSDE_PW_CHANNEL || o.kind == TSDE_PW_ROW) {
-    load_quad(static_cast<const T*>(o.ptr), o.kind == TSDE_PW_ROW ? c.base : c.chan, c.vec, c.nvalid, v);
-    return;
-  }
-  const T x = o.kind == TSDE_PW_IMM ? (T)o.imm : *(o.kind == TSDE_PW_T0 ? c.t : static_cast<const T*>(o.ptr));
-#pragma unroll
-  for (int j = 0; j < 4; ++j) v[j] = x;
+  pw_sload(regs, s & 31, s & kPwSrcUniform ? s >> 6 : threadIdx.x, v);
 }
 
 // instructions [i0, i1): one warp-uniform dispatch per instruction, one IEEE rounding per element (-fmad=false)
-template <typename T>
-__device__ __forceinline__ void pw_run(const tsde_pointwise& pg, const PwQuad<T>& c, void* regs, int i0, int i1) {
+template <bool GLOBAL, typename T>
+__device__ __forceinline__ void pw_loop(const PwProg<T>& pg, const PwQuad& c, void* regs, int i0, int i1) {
   for (int i = i0; i < i1; ++i) {
-    const tsde_pw_instr in = pg.instr[i];
+    const uint32_t in = pg.instr[i];
     T a[4], b[4], r[4];
-    pw_fetch(pg, c, regs, in.a, a);
-    if (in.op != TSDE_PW_NEG && in.op != TSDE_PW_SQRT) pw_fetch(pg, c, regs, in.b, b);
-    switch (in.op) {
+    pw_fetch<GLOBAL>(pg, c, regs, (in >> 8) & 0xFFF, a);
+    pw_fetch<GLOBAL>(pg, c, regs, in >> 20, b);
+    switch (in & 7) {
       case TSDE_PW_MUL:
 #pragma unroll
         for (int j = 0; j < 4; ++j) r[j] = a[j] * b[j];
@@ -117,7 +155,52 @@ __device__ __forceinline__ void pw_run(const tsde_pointwise& pg, const PwQuad<T>
         for (int j = 0; j < 4; ++j) r[j] = sqrt(a[j]);
         break;
     }
-    pw_sstore(regs, in.dst, r);
+    pw_sstore(regs, (in >> 3) & 31, r);
+  }
+}
+
+// The loop that reads only shared memory unless the program has operands in global memory, which is rare (see
+// kPwHoistSlots)
+template <typename T>
+__device__ __forceinline__ void pw_run(const PwProg<T>& pg, const PwQuad& c, void* regs, int i0, int i1) {
+  if (pg.n_global)
+    pw_loop<true>(pg, c, regs, i0, i1);
+  else
+    pw_loop<false>(pg, c, regs, i0, i1);
+}
+
+// The launch-uniform values into the u slot; every thread of the CTA calls it (it ends in a barrier), after the
+// dependency wait.
+template <typename T>
+__device__ __forceinline__ void pw_load_uniform(const PwProg<T>& pg, void* regs) {
+  if ((int)threadIdx.x < pg.n_uniform) {
+    const PwOperand<T>& o = pg.operand[threadIdx.x];
+    const T x = o.ptr ? *o.ptr : o.imm;
+    const T v[4] = {x, x, x, x};
+    pw_sstore(regs, pg.u, threadIdx.x, v);
+  }
+  __syncthreads();
+}
+
+// This thread's quads of the hoisted operands into their slots, after the dependency wait
+template <typename T>
+__device__ __forceinline__ void pw_load_hoisted(const PwProg<T>& pg, const PwQuad& c, void* regs) {
+  for (int h = 0; h < pg.n_hoisted; ++h) {
+    const int k = pg.n_uniform + h;
+    T v[4];
+    load_quad(pg.operand[k].ptr, (pg.row >> k) & 1 ? c.base : c.chan, c.vec, c.nvalid, v);
+    pw_sstore(regs, pg.hoist + h, v);
+  }
+}
+
+// The state an evaluation runs at and, when the program reads it, its time
+template <typename T>
+__device__ __forceinline__ void pw_set_state(const PwProg<T>& pg, void* regs, const T* t, const T (&y)[4]) {
+  pw_sstore(regs, pg.y, y);
+  if (pg.t0 >= 0) {
+    const T x = *t;
+    const T v[4] = {x, x, x, x};
+    pw_sstore(regs, pg.t0, v);
   }
 }
 
@@ -160,12 +243,73 @@ static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, bool allow_
   return true;
 }
 
+// ---- decoding -------------------------------------------------------------------------------------------------------
+// The PwProg of a program that passed validation: with a go slot for the Milstein layout (`go`), and `extra` slots past
+// the layout (SRK's fp64 stash) counted against kPwHoistSlots.  Returns the slots a launch takes, extra included.
+template <typename T>
+static int pw_decode(const tsde_pointwise& in, bool go, int extra, PwProg<T>& pg) {
+  pg = PwProg<T>{};
+  pg.n_fg = in.n_fg;
+  pg.n_instr = in.n_instr;
+  int n_uniform = 0, n_local = 0;
+  bool t0 = false;
+  for (int k = 0; k < in.n_operands; ++k) {
+    const int kind = in.operand[k].kind;
+    t0 = t0 || kind == TSDE_PW_T0;
+    n_uniform += kind == TSDE_PW_IMM || kind == TSDE_PW_SCALAR;
+    n_local += kind >= TSDE_PW_CHANNEL;
+  }
+  int slot = in.n_regs;
+  pg.y = slot++;
+  pg.go = go ? slot++ : -1;
+  pg.t0 = t0 ? slot++ : -1;
+  pg.u = n_uniform ? slot++ : -1;
+  pg.hoist = slot;
+  pg.n_uniform = n_uniform;
+  pg.n_hoisted = std::min(n_local, std::max(kPwHoistSlots - slot - extra, 0));
+  pg.n_global = n_local - pg.n_hoisted;
+  slot += pg.n_hoisted;
+  pg.end = slot;
+  // the operand table in decoded order (uniform, hoisted, global), and the source that names each caller operand
+  uint32_t src[TSDE_PW_MAX_OPERANDS];
+  int n_u = 0, n_l = 0;
+  for (int k = 0; k < in.n_operands; ++k) {
+    const tsde_pw_operand& o = in.operand[k];
+    if (o.kind == TSDE_PW_T0) {
+      src[k] = pg.t0;
+      continue;
+    }
+    const bool local = o.kind >= TSDE_PW_CHANNEL;
+    const int j = local ? n_uniform + n_l++ : n_u++;
+    pg.operand[j] = PwOperand<T>{o.kind == TSDE_PW_IMM ? nullptr : static_cast<const T*>(o.ptr), (T)o.imm};
+    if (o.kind == TSDE_PW_ROW) pg.row |= 1u << j;
+    if (!local)
+      src[k] = pg.u | kPwSrcUniform | (uint32_t)j << 6;
+    else
+      src[k] = j - n_uniform < pg.n_hoisted ? pg.hoist + (j - n_uniform) : kPwSrcGlobal | j;
+  }
+  auto source = [&](uint32_t s) -> uint32_t {
+    if (s == TSDE_PW_SRC_Y) return pg.y;
+    if (s == TSDE_PW_SRC_GO) return pg.go;
+    return s >= (uint32_t)TSDE_PW_OPERAND(0) ? src[s - TSDE_PW_OPERAND(0)] : s;
+  };
+  for (int i = 0; i < in.n_instr; ++i) {
+    const tsde_pw_instr& x = in.instr[i];
+    const uint32_t a = source(x.a), b = x.op == TSDE_PW_NEG || x.op == TSDE_PW_SQRT ? a : source(x.b);
+    pg.instr[i] = x.op | (uint32_t)x.dst << 3 | a << 8 | b << 20;
+  }
+  pg.f_src = source(in.f_src);
+  pg.g_src = source(in.g_src);
+  pg.gdg_src = go ? source(in.gdg_src) : pg.y;  // (the two-program layouts have no gdg)
+  return slot + extra;
+}
+
 // ---- what every kernel starts with ----------------------------------------------------------------------------------
 // pw_begin's quad mapping on its own, for a kernel that draws again later: the flat index Q (past the last quad when
-// Q >= p.nquads), the row and quad of the row, and `c` but for the state.  (pw_begin keeps its own copy: calling this
-// from it reschedules the SRK and predictor-corrector kernels.)
+// Q >= p.nquads), the row and quad of the row, and `c`.  (pw_begin keeps its own copy: calling this from it
+// reschedules the SRK and predictor-corrector kernels.)
 template <typename T>
-__device__ __forceinline__ void pw_locate(const PwP<T>& p, PwQuad<T>& c, int64_t& Q, int64_t& row, int64_t& q) {
+__device__ __forceinline__ void pw_locate(const PwP<T>& p, PwQuad& c, int64_t& Q, int64_t& row, int64_t& q) {
   Q = (int64_t)blockIdx.x * kThreads + threadIdx.x;
   if (p.qshift >= 0) {
     row = Q >> p.qshift;
@@ -185,12 +329,12 @@ __device__ __forceinline__ void pw_locate(const PwP<T>& p, PwQuad<T>& c, int64_t
   c.vec = p.vec != 0;
 }
 
-// This thread's quad (`c`, but for the state it is evaluated at), its increments and its y0.  The increments depend on
-// no predecessor: they are drawn while the previous kernel drains (programmatic dependent launch), and y0 is read
-// after the dependency wait.  False for a thread past the last quad.
+// This thread's quad `c`, its increments and its y0, and the program's operands in their slots.  The increments
+// depend on no predecessor: they are drawn while the previous kernel drains (programmatic dependent launch); y0 and
+// the operands are read after the dependency wait.  False for a thread past the last quad.
 template <typename T, int SRC, bool WANT_U>
-__device__ __forceinline__ bool pw_begin(const PwP<T>& p, const NoiseP<T>& nz, PwQuad<T>& c, T (&w)[4], T (&u)[4],
-                                         T (&y0)[4]) {
+__device__ __forceinline__ bool pw_begin(const PwProg<T>& pg, const PwP<T>& p, const NoiseP<T>& nz, void* regs,
+                                         PwQuad& c, T (&w)[4], T (&u)[4], T (&y0)[4]) {
   const int64_t Q = (int64_t)blockIdx.x * kThreads + threadIdx.x;
   int64_t row, q;
   if (p.qshift >= 0) {
@@ -211,10 +355,10 @@ __device__ __forceinline__ bool pw_begin(const PwP<T>& p, const NoiseP<T>& nz, P
   c.vec = p.vec != 0;
   quad_noise<T, SRC, WANT_U>(nz, load_key(nz.key), row, q, c.vec, c.nvalid, w, u);
   asm volatile("griddepcontrol.wait;" ::: "memory");
+  pw_load_uniform(pg, regs);
   if (Q >= p.nquads) return false;
   load_quad(p.y0, c.base, c.vec, c.nvalid, y0);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) c.go[j] = T(0);
+  pw_load_hoisted(pg, c, regs);
   return true;
 }
 
@@ -238,18 +382,19 @@ struct PwSteps {  // by value: a captured launch carries the whole table
   int32_t n;
   PwStep<T> s[kPwMaxSteps];
 };
-static_assert(sizeof(tsde_pointwise) + sizeof(PwP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <= 4096,
+static_assert(sizeof(PwProg<double>) + sizeof(PwP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <= 4096,
               "the Milstein kernel's parameters fit the 4 KiB parameter space");
 
 template <typename T, int SRC>
 __global__ void __launch_bounds__(kThreads)
-pw_milstein_kernel(const __grid_constant__ tsde_pointwise pg, const PwP<T> p, const NoiseP<T> nz,
+pw_milstein_kernel(const __grid_constant__ PwProg<T> pg, const PwP<T> p, const NoiseP<T> nz,
                    const __grid_constant__ PwSteps<T> st) {
   extern __shared__ __align__(16) unsigned char pw_regs[];
-  PwQuad<T> c;
+  PwQuad c;
   int64_t Q, row, q;
   pw_locate(p, c, Q, row, q);
   const Key key = load_key(nz.key);
+  T y[4];
   for (int j = 0; j < st.n; ++j) {
     const PwStep<T>& s = st.s[j];
     T w[4], u[4];
@@ -257,14 +402,16 @@ pw_milstein_kernel(const __grid_constant__ tsde_pointwise pg, const PwP<T> p, co
     z.cell_id = s.cell;
     z.sqrt_h = s.sqrt_h;
     quad_noise<T, SRC, false>(z, key, row, q, c.vec, c.nvalid, w, u);
-    if (j == 0) {  // the first increment is drawn while the previous kernel drains; y0 is read after the wait
+    if (j == 0) {  // the first increment is drawn while the previous kernel drains; the rest is read after the wait
       asm volatile("griddepcontrol.wait;" ::: "memory");
+      pw_load_uniform(pg, pw_regs);
       if (Q >= p.nquads) return;
-      load_quad(p.y0, c.base, c.vec, c.nvalid, c.y);
+      load_quad(p.y0, c.base, c.vec, c.nvalid, y);
+      pw_load_hoisted(pg, c, pw_regs);
     }
-    c.t = s.t0;
+    pw_set_state(pg, pw_regs, s.t0, y);
     pw_run(pg, c, pw_regs, 0, pg.n_fg);
-    T f[4], g[4];
+    T f[4], g[4], go[4];
     pw_fetch(pg, c, pw_regs, pg.f_src, f);
     pw_fetch(pg, c, pw_regs, pg.g_src, g);
     const MilsteinSeedOp<T> seed{s.dt, p.ito};
@@ -272,8 +419,9 @@ pw_milstein_kernel(const __grid_constant__ tsde_pointwise pg, const PwP<T> p, co
     for (int i = 0; i < 4; ++i) {
       T o[1];
       seed({g[i]}, w[i], u[i], o);
-      c.go[i] = o[0];
+      go[i] = o[0];
     }
+    pw_sstore(pw_regs, pg.go, go);
     pw_run(pg, c, pw_regs, pg.n_fg, pg.n_instr);
     T gdg[4];
     pw_fetch(pg, c, pw_regs, pg.gdg_src, gdg);
@@ -281,10 +429,10 @@ pw_milstein_kernel(const __grid_constant__ tsde_pointwise pg, const PwP<T> p, co
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       T o[1];
-      step({c.y[i], f[i], g[i], gdg[i]}, w[i], u[i], o);
-      c.y[i] = o[0];
+      step({y[i], f[i], g[i], gdg[i]}, w[i], u[i], o);
+      y[i] = o[0];
     }
-    if (s.y1) store_quad(s.y1, c.base, c.vec, c.nvalid, c.y);
+    if (s.y1) store_quad(s.y1, c.base, c.vec, c.nvalid, y);
   }
 }
 
@@ -320,7 +468,7 @@ template <typename T>
 struct PwSrkStash {
   static constexpr bool kShared = sizeof(T) == 8;
   T r[kShared ? 1 : kPwSrkStash][4];
-  int slot0;  // first shared-memory register past the program's
+  int slot0;  // first slot past the program's layout (PwProg::end)
   __device__ __forceinline__ void put(void* regs, int k, const T (&x)[4]) {
     if constexpr (kShared) {
       pw_sstore(regs, slot0 + k, x);
@@ -331,7 +479,7 @@ struct PwSrkStash {
   }
   __device__ __forceinline__ void get(const void* regs, int k, T (&x)[4]) const {
     if constexpr (kShared) {
-      pw_sload(regs, slot0 + k, x);
+      pw_sload(regs, slot0 + k, threadIdx.x, x);
     } else {
 #pragma unroll
       for (int j = 0; j < 4; ++j) x[j] = r[k][j];
@@ -342,24 +490,22 @@ struct PwSrkStash {
 // One SDE evaluation of the two-program layout (SRK, predictor-corrector): f (program [0, n_fg), result f_src) or g
 // (program [n_fg, n_instr), result g_src) at (t, y)
 template <typename T>
-__device__ __forceinline__ void pw_eval(const tsde_pointwise& pg, PwQuad<T>& c, void* regs, bool g, const T* t,
+__device__ __forceinline__ void pw_eval(const PwProg<T>& pg, const PwQuad& c, void* regs, bool g, const T* t,
                                         const T (&y)[4], T (&out)[4]) {
-  c.t = t;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) c.y[j] = y[j];
+  pw_set_state(pg, regs, t, y);
   pw_run(pg, c, regs, g ? pg.n_fg : 0, g ? pg.n_instr : pg.n_fg);
   pw_fetch(pg, c, regs, g ? pg.g_src : pg.f_src, out);
 }
 
 template <typename T, int SRC>
 __global__ void __launch_bounds__(kThreads)
-pw_srk_kernel(const __grid_constant__ tsde_pointwise pg, const PwSrkP<T> p, const NoiseP<T> nz) {
+pw_srk_kernel(const __grid_constant__ PwProg<T> pg, const PwSrkP<T> p, const NoiseP<T> nz) {
   extern __shared__ __align__(16) unsigned char pw_regs[];
-  PwQuad<T> c;
+  PwQuad c;
   T w[4], u[4], y0[4];
-  if (!pw_begin<T, SRC, true>(p.base, nz, c, w, u, y0)) return;
+  if (!pw_begin<T, SRC, true>(pg, p.base, nz, pw_regs, c, w, u, y0)) return;
   PwSrkStash<T> st;
-  st.slot0 = pg.n_regs;
+  st.slot0 = pg.end;
   enum { F0, F1, F2, G0, G1, G2 };
   T f[4], g[4], h0[4], h1[4], x[4], z[4];
   // s = 0: f0, g0 at (t0, y0); H0_1, H1_1
@@ -446,11 +592,11 @@ struct PwPcP {
 
 template <typename T, int SRC, int METHOD>
 __global__ void __launch_bounds__(kThreads, 1)
-pw_pc_kernel(const __grid_constant__ tsde_pointwise pg, const PwPcP<T> p, const NoiseP<T> nz) {
+pw_pc_kernel(const __grid_constant__ PwProg<T> pg, const PwPcP<T> p, const NoiseP<T> nz) {
   extern __shared__ __align__(16) unsigned char pw_regs[];
-  PwQuad<T> c;
+  PwQuad c;
   T w[4], u[4], y0[4];
-  if (!pw_begin<T, SRC, false>(p.base, nz, c, w, u, y0)) return;
+  if (!pw_begin<T, SRC, false>(pg, p.base, nz, pw_regs, c, w, u, y0)) return;
   const T dt = p.base.dt;
   T f0[4], g0[4], yp[4];
   pw_eval(pg, c, pw_regs, false, p.base.t0, y0, f0);
@@ -503,16 +649,16 @@ struct PwChunkP {
   const T *z0, *f0, *g0;  // reversible Heun: the solver state the chunk starts from
   T *z1, *f1, *g1;        // and where the chunk leaves it
 };
-static_assert(sizeof(tsde_pointwise) + sizeof(PwChunkP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <=
+static_assert(sizeof(PwProg<double>) + sizeof(PwChunkP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <=
                   4096,
               "the chunk kernel's parameters fit the 4 KiB parameter space");
 
 template <typename T, int SRC, int METHOD>
 __global__ void __launch_bounds__(kThreads, 1)
-pw_chunk_kernel(const __grid_constant__ tsde_pointwise pg, const PwChunkP<T> p, const NoiseP<T> nz,
+pw_chunk_kernel(const __grid_constant__ PwProg<T> pg, const PwChunkP<T> p, const NoiseP<T> nz,
                 const __grid_constant__ PwSteps<T> st) {
   extern __shared__ __align__(16) unsigned char pw_regs[];
-  PwQuad<T> c;
+  PwQuad c;
   int64_t Q, row, q;
   pw_locate(p.base, c, Q, row, q);
   const Key key = load_key(nz.key);
@@ -524,8 +670,9 @@ pw_chunk_kernel(const __grid_constant__ tsde_pointwise pg, const PwChunkP<T> p, 
     n.cell_id = s.cell;
     n.sqrt_h = s.sqrt_h;
     quad_noise<T, SRC, false>(n, key, row, q, c.vec, c.nvalid, w, u);
-    if (j == 0) {  // the first increment is drawn while the previous kernel drains; the state is read after the wait
+    if (j == 0) {  // the first increment is drawn while the previous kernel drains; the rest is read after the wait
       asm volatile("griddepcontrol.wait;" ::: "memory");
+      pw_load_uniform(pg, pw_regs);
       if (Q >= p.base.nquads) return;
       load_quad(p.base.y0, c.base, c.vec, c.nvalid, y);
       if constexpr (METHOD == kPwReversibleHeun) {
@@ -533,6 +680,7 @@ pw_chunk_kernel(const __grid_constant__ tsde_pointwise pg, const PwChunkP<T> p, 
         load_quad(p.f0, c.base, c.vec, c.nvalid, f);
         load_quad(p.g0, c.base, c.vec, c.nvalid, g);
       }
+      pw_load_hoisted(pg, c, pw_regs);
     }
     if constexpr (METHOD == kPwEuler) {
       pw_eval(pg, c, pw_regs, false, s.t0, y, f);
@@ -575,15 +723,18 @@ pw_chunk_kernel(const __grid_constant__ tsde_pointwise pg, const PwChunkP<T> p, 
 }
 
 // ---- launch ---------------------------------------------------------------------------------------------------------
-// The noise and the part of the kernel parameters every pointwise step has (y0, y1, the quad mapping, vec) for a
-// program that passes `layout`; TSDE_EINVAL for a launch the kernels cannot serve.
+// The noise, the decoded program `pg` with the shared-memory slots its launch takes (`extra` past its layout; a go
+// slot for the Milstein layout, `go`), and the part of the kernel parameters every pointwise step has (y0, y1, the
+// quad mapping, vec) for a program that passes `layout`; TSDE_EINVAL for a launch the kernels cannot serve.
 template <typename T>
 static int pw_prepare(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
-                      void* y1, bool (*layout)(const tsde_pointwise&), PwP<T>& p, NoiseP<T>& np) {
+                      void* y1, bool (*layout)(const tsde_pointwise&), bool go, int extra, PwProg<T>& pg, int& slots,
+                      PwP<T>& p, NoiseP<T>& np) {
   if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !prog || !y0 || !y1) return TSDE_EINVAL;
   bool vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y1);
   if (!pw_valid_tables(*prog, &vec) || !layout(*prog)) return TSDE_EINVAL;
   if (int e = fill_noise<T>(L, nz, false, np)) return e;
+  slots = pw_decode<T>(*prog, go, extra, pg);
   p = PwP<T>{};
   p.y0 = static_cast<const T*>(y0);
   p.y1 = static_cast<T*>(y1);
@@ -595,9 +746,9 @@ static int pw_prepare(const tsde_launch* L, const tsde_noise* nz, const tsde_poi
 // One thread per quad, `slots` shared-memory registers per thread; `single` draws from one Brownian cell, `multi` sums
 // the cells of a step that spans several.  `x` are the kernel's parameters past the noise (the Milstein step table).
 template <typename T, typename P, typename... X>
-static int pw_launch(const tsde_launch* L, const tsde_pointwise& prog,
-                     void (*single)(tsde_pointwise, P, NoiseP<T>, X...),
-                     void (*multi)(tsde_pointwise, P, NoiseP<T>, X...), const P& p, const NoiseP<T>& np,
+static int pw_launch(const tsde_launch* L, const PwProg<T>& prog,
+                     void (*single)(PwProg<T>, P, NoiseP<T>, X...),
+                     void (*multi)(PwProg<T>, P, NoiseP<T>, X...), const P& p, const NoiseP<T>& np,
                      int64_t nquads, int slots, int family, const X&... x) {
   const size_t smem = (size_t)slots * kThreads * 4 * sizeof(T);
   auto kernel = np.n_cells > 1 ? multi : single;
@@ -619,9 +770,12 @@ template <typename T>
 static int pw_milstein_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
                              const tsde_pw_step* steps, int32_t n_steps, int32_t ito) {
   if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
+  PwProg<T> pg;
+  int slots;
   PwP<T> p;
   NoiseP<T> np;
-  if (int e = pw_prepare<T>(L, nz, prog, y0, steps[n_steps - 1].y1, pw_valid_milstein, p, np)) return e;
+  if (int e = pw_prepare<T>(L, nz, prog, y0, steps[n_steps - 1].y1, pw_valid_milstein, true, 0, pg, slots, p, np))
+    return e;
   if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
   PwSteps<T> st{};
   st.n = n_steps;
@@ -635,8 +789,8 @@ static int pw_milstein_chunk(const tsde_launch* L, const tsde_noise* nz, const t
   np.cell_id = steps[0].cell_id;
   np.h = steps[0].h;
   p.ito = ito;
-  return pw_launch<T>(L, *prog, pw_milstein_kernel<T, TSDE_SRC_COUNTER>, pw_milstein_kernel<T, kSrcCounterMulti>, p,
-                      np, p.nquads, prog->n_regs, TSDE_KERNEL_PW_MILSTEIN, st);
+  return pw_launch<T>(L, pg, pw_milstein_kernel<T, TSDE_SRC_COUNTER>, pw_milstein_kernel<T, kSrcCounterMulti>, p, np,
+                      p.nquads, slots, TSDE_KERNEL_PW_MILSTEIN, st);
 }
 
 // The chunk `steps[0, n_steps)` of Euler or reversible Heun from y0 (and, for reversible Heun, from the solver state
@@ -646,9 +800,12 @@ template <typename T, int METHOD>
 static int pw_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
                     const tsde_pw_step* steps, int32_t n_steps, const void* const (&in)[3], void* const (&out)[3]) {
   if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
+  PwProg<T> pg;
+  int slots;
   PwChunkP<T> p{};
   NoiseP<T> np;
-  if (int e = pw_prepare<T>(L, nz, prog, y0, steps[n_steps - 1].y1, pw_valid_two<TSDE_PW_MAX_REGS>, p.base, np))
+  if (int e = pw_prepare<T>(L, nz, prog, y0, steps[n_steps - 1].y1, pw_valid_two<TSDE_PW_MAX_REGS>, false, 0, pg,
+                            slots, p.base, np))
     return e;
   if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
   if constexpr (METHOD == kPwReversibleHeun) {
@@ -673,8 +830,8 @@ static int pw_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_point
   }
   np.cell_id = steps[0].cell_id;
   np.h = steps[0].h;
-  return pw_launch<T>(L, *prog, pw_chunk_kernel<T, TSDE_SRC_COUNTER, METHOD>, pw_chunk_kernel<T, kSrcCounterMulti, METHOD>,
-                      p, np, p.base.nquads, prog->n_regs, TSDE_KERNEL_PW_CHUNK, st);
+  return pw_launch<T>(L, pg, pw_chunk_kernel<T, TSDE_SRC_COUNTER, METHOD>, pw_chunk_kernel<T, kSrcCounterMulti, METHOD>,
+                      p, np, p.base.nquads, slots, TSDE_KERNEL_PW_CHUNK, st);
 }
 
 TSDE_EXPORT int tsde_solve_euler_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
@@ -725,9 +882,13 @@ TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_no
   return dispatch(L, [&](auto t) -> int {
     using T = decltype(t);
     if (!t_0 || !t_1 || !t_q || !t_h) return TSDE_EINVAL;
+    PwProg<T> pg;
+    int slots;
     PwSrkP<T> p;
     NoiseP<T> np;
-    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_two<TSDE_PW_SRK_MAX_REGS>, p.base, np)) return e;
+    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_two<TSDE_PW_SRK_MAX_REGS>, false,
+                              PwSrkStash<T>::kShared ? kPwSrkStash : 0, pg, slots, p.base, np))
+      return e;
     const void* times[4] = {t_0, t_1, t_q, t_h};
     for (int i = 0; i < 4; ++i) p.t[i] = static_cast<const T*>(times[i]);
     // the coefficients of tsde_srk_diag_stage1/2/3 and tsde_step_srk_diag
@@ -735,8 +896,8 @@ TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_no
     p.s2 = SrkDiagStage2Op<T>{(T)dt, (T)rdt, (T)sqrt_dt};
     p.s3 = SrkDiagStage3Op<T>{(T)dt, (T)sqrt_dt};
     p.fin = make_srk_final<T>(dt, rdt, sqrt_dt, three_dt);
-    return pw_launch<T>(L, *prog, pw_srk_kernel<T, TSDE_SRC_COUNTER>, pw_srk_kernel<T, kSrcCounterMulti>, p, np,
-                        p.base.nquads, prog->n_regs + (PwSrkStash<T>::kShared ? kPwSrkStash : 0), TSDE_KERNEL_PW_SRK);
+    return pw_launch<T>(L, pg, pw_srk_kernel<T, TSDE_SRC_COUNTER>, pw_srk_kernel<T, kSrcCounterMulti>, p, np,
+                        p.base.nquads, slots, TSDE_KERNEL_PW_SRK);
   });
 }
 
@@ -748,15 +909,18 @@ TSDE_EXPORT int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, co
   return dispatch(L, [&](auto t) -> int {
     using T = decltype(t);
     if (!t0 || !t_p || method < TSDE_PC_HEUN || method > TSDE_PC_EULER_HEUN) return TSDE_EINVAL;
+    PwProg<T> pg;
+    int slots;
     PwPcP<T> p;
     NoiseP<T> np;
-    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_two<TSDE_PW_MAX_REGS>, p.base, np)) return e;
+    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_two<TSDE_PW_MAX_REGS>, false, 0, pg, slots, p.base, np))
+      return e;
     p.base.t0 = static_cast<const T*>(t0);
     p.base.dt = (T)dt;
     p.t_p = static_cast<const T*>(t_p);
     p.half_dt = (T)half_dt;
     auto go = [&](auto single, auto multi) {
-      return pw_launch<T>(L, *prog, single, multi, p, np, p.base.nquads, prog->n_regs, TSDE_KERNEL_PW_PC);
+      return pw_launch<T>(L, pg, single, multi, p, np, p.base.nquads, slots, TSDE_KERNEL_PW_PC);
     };
     switch (method) {
       case TSDE_PC_HEUN:
