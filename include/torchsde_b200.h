@@ -258,9 +258,17 @@ int tsde_step_milstein(const tsde_launch* L, const tsde_noise* nz, const void* y
  * the step equals the unfused one bit for bit.
  *
  * Program: `n_instr` instructions; [0, n_fg) compute f and g, [n_fg, n_instr) the vjp.  An instruction writes
- * register `dst` (< n_regs <= TSDE_PW_MAX_REGS) from sources `a`, `b` (b unused by NEG / SQRT).  A source is a
- * register, TSDE_PW_SRC_Y (y0), TSDE_PW_SRC_GO (the seed go, vjp part only) or TSDE_PW_OPERAND(k).  f_src,
- * g_src (read after n_fg instructions) and gdg_src (read at the end) name the three results.  Operands:
+ * register `dst` (< n_regs <= TSDE_PW_MAX_REGS) from sources `a`, `b` (b unused by NEG / SQRT / ABS).  A source
+ * is a register, TSDE_PW_SRC_Y (y0), TSDE_PW_SRC_GO (the seed go, vjp part only) or TSDE_PW_OPERAND(k).  f_src,
+ * g_src (read after n_fg instructions) and gdg_src (read at the end) name the three results.  Opcodes, each the
+ * expression of the ATen CUDA kernel it restates, in the state dtype T:
+ *   MUL a * b   ADD a + b   SUB a - b   DIV a / b   NEG -a   SQRT sqrt(a)    (6, 7: reserved, invalid)
+ *   LT  a < b ? 1 : 0    LE a <= b ? 1 : 0    EQ a == b ? 1 : 0    (a boolean is T(0) or T(1))
+ *   MAXIMUM  isnan(a) ? a : isnan(b) ? b : max(a, b)    (torch.maximum; clamp with a non-NaN lower bound)
+ *   MINIMUM  isnan(a) ? a : isnan(b) ? b : min(a, b)    (torch.minimum; clamp with a non-NaN upper bound)
+ *   ABS  fabs(a)
+ *   SEL  dst = dst != 0 ? a : b: the condition is the destination register itself, which must have been written
+ *        (torch.where, masked_fill).
  *   IMM      value `imm` (a value of the state dtype, stored as double)
  *   T0       the 0-d step time `t0` of the call (state dtype)
  *   SCALAR   ptr[0]                 (a one-element device tensor)
@@ -277,6 +285,8 @@ int tsde_step_milstein(const tsde_launch* L, const tsde_noise* nz, const void* y
 #define TSDE_PW_SRC_GO 0xFF
 #define TSDE_PW_OPERAND(k) (0x80 + (k))
 enum { TSDE_PW_MUL = 0, TSDE_PW_ADD = 1, TSDE_PW_SUB = 2, TSDE_PW_DIV = 3, TSDE_PW_NEG = 4, TSDE_PW_SQRT = 5 };
+enum { TSDE_PW_LT = 8, TSDE_PW_LE = 9, TSDE_PW_EQ = 10, TSDE_PW_MAXIMUM = 11, TSDE_PW_MINIMUM = 12, TSDE_PW_ABS = 13,
+       TSDE_PW_SEL = 14 };
 enum { TSDE_PW_IMM = 0, TSDE_PW_T0 = 1, TSDE_PW_SCALAR = 2, TSDE_PW_CHANNEL = 3, TSDE_PW_ROW = 4 };
 typedef struct tsde_pw_instr {
   uint8_t op, dst, a, b;

@@ -49,6 +49,7 @@ class Noise(ctypes.Structure):
 PW_MAX_INSTR, PW_MAX_OPERANDS, PW_MAX_REGS = 96, 24, 24  # TSDE_PW_MAX_*
 PW_SRC_Y, PW_SRC_GO, PW_OPERAND0 = 0xFE, 0xFF, 0x80
 PW_MUL, PW_ADD, PW_SUB, PW_DIV, PW_NEG, PW_SQRT = range(6)
+PW_LT, PW_LE, PW_EQ, PW_MAXIMUM, PW_MINIMUM, PW_ABS, PW_SEL = range(8, 15)  # (6, 7 reserved)
 PW_IMM, PW_T0, PW_SCALAR, PW_CHANNEL, PW_ROW = range(5)
 PW_SRK_MAX_REGS = 18  # TSDE_PW_SRK_MAX_REGS
 KERNEL_PW_MILSTEIN = 3  # TSDE_KERNEL_PW_MILSTEIN

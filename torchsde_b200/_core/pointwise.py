@@ -12,7 +12,16 @@ What a tape may hold, for both methods.  The tape accepts only
 
     mul; add / sub / rsub with alpha = +-1 (any other alpha lets ATen contract to an FMA); neg; sqrt;
     div by a tensor; div by a CPU scalar (ATen computes a * (1/b), with 1/b rounded in the state dtype);
-    pow(x, 2) (ATen computes x * x); aliasing views that keep every element where it is (no-ops),
+    pow(x, 2) (ATen computes x * x); aliasing views that keep every element where it is (no-ops);
+
+and the ops that do not round, or round once, each restated as its ATen CUDA kernel computes it, NaN and signed zeros
+included:
+
+    abs; sign / sgn ((0 < x) - (x < 0)); reciprocal (1 / x); maximum / minimum (NaN-propagating); clamp, clamp_min,
+    clamp_max with scalar bounds that are not NaN or with tensor bounds (maximum with the lower bound, then minimum
+    with the upper one), relu (clamp_min(x, 0)); lt / le / gt / ge / eq / ne (.Scalar and .Tensor); where.self;
+    masked_fill(_).Scalar; logical_and / or / not and their bitwise forms on bools (and in place); threshold_backward
+    (x <= threshold ? 0 : grad); scalar_tensor (an immediate: autograd's clamp and where backward emit it),
 
 on operands that are the state y, the 0-d time t the callable was given, Python numbers and CPU 0-d tensors
 (immediates, rounded to the state dtype as ATen rounds them), one-element device tensors, (d,)-shaped device tensors
@@ -21,6 +30,13 @@ else — another op, a reduction, `.item()`, an in-place op on anything the tape
 whose storage was written in place through another tensor (a view, `detach()`, `.data`), an operand that shares
 storage with a value of the tape, a 16-bit result, a tensor created by a factory — rejects the tape, and the solve
 keeps its ordinary step.
+
+Bools.  A comparison or logical result is a bool tensor; in the program it is a register holding 0 or 1 of the state
+dtype (logical_and is then a product, logical_or a maximum, logical_not 1 - c, ne 1 - eq, gt / ge lt / le with the
+operands swapped, all exact).  A bool may only be the condition of where / masked_fill or an operand of a logical op:
+one used as a number (in arithmetic, a comparison, `.float()`), returned as f, g or the vjp, or a bool tensor from
+outside the tape (a user mask) rejects the tape.  where(c, a, b) compiles to SEL, whose condition is its destination
+register: c's own register when this is c's last read, else a copy of it (`_allocate`).
 
 Device operands are passed by address and read at every launch: in-place updates of parameters (optimiser steps) are
 followed, exactly as by a captured CUDA graph; f and g must not depend on anything else (the purity contract of
@@ -76,9 +92,24 @@ _BINARY = {
     aten.rsub.Tensor: (_cabi.PW_SUB, True), aten.rsub.Scalar: (_cabi.PW_SUB, True),
     aten.div.Tensor: (_cabi.PW_DIV, False), aten.div.Scalar: (_cabi.PW_DIV, False),
 }
-_UNARY = {aten.neg.default: _cabi.PW_NEG, aten.sqrt.default: _cabi.PW_SQRT}
+_UNARY = {aten.neg.default: _cabi.PW_NEG, aten.sqrt.default: _cabi.PW_SQRT, aten.abs.default: _cabi.PW_ABS}
+# comparisons: op -> (opcode, swap operands); gt / ge are lt / le with the operands swapped, exactly (NaN included)
+_COMPARE = {}
+for _name, _entry in (('lt', (_cabi.PW_LT, False)), ('le', (_cabi.PW_LE, False)), ('gt', (_cabi.PW_LT, True)),
+                      ('ge', (_cabi.PW_LE, True)), ('eq', (_cabi.PW_EQ, False)), ('ne', (_cabi.PW_EQ, False))):
+    for _overload in ('Tensor', 'Scalar'):
+        _COMPARE[getattr(getattr(aten, _name), _overload)] = _entry
+_NEGATED = {aten.ne.Tensor, aten.ne.Scalar}  # 1 - eq
+# logical ops of comparison results (0 or 1): and is a product, or a maximum, not 1 - c (`&`, `|`, `~` of bool
+# tensors are the bitwise ops)
+_LOGICAL = {aten.logical_and.default: _cabi.PW_MUL, aten.bitwise_and.Tensor: _cabi.PW_MUL,
+            aten.logical_or.default: _cabi.PW_MAXIMUM, aten.bitwise_or.Tensor: _cabi.PW_MAXIMUM,
+            aten.logical_not.default: _cabi.PW_SUB, aten.bitwise_not.default: _cabi.PW_SUB}
 _IN_PLACE = {aten.mul_.Tensor: aten.mul.Tensor, aten.add_.Tensor: aten.add.Tensor,
-             aten.sub_.Tensor: aten.sub.Tensor, aten.div_.Tensor: aten.div.Tensor}
+             aten.sub_.Tensor: aten.sub.Tensor, aten.div_.Tensor: aten.div.Tensor,
+             aten.masked_fill_.Scalar: aten.masked_fill.Scalar, aten.logical_and_.default: aten.logical_and.default,
+             aten.logical_or_.default: aten.logical_or.default, aten.bitwise_and_.Tensor: aten.bitwise_and.Tensor,
+             aten.bitwise_or_.Tensor: aten.bitwise_or.Tensor}
 _ALIAS = {aten.view.default, aten._unsafe_view.default, aten.expand.default, aten.unsqueeze.default,
           aten.detach.default, aten.alias.default}
 
@@ -100,21 +131,22 @@ def _strip(shape):
 
 
 def _allocate(instrs, reads):
-    """Dead-code elimination and register allocation of one tape.  `instrs` are (opcode, value id, source, source);
-    `reads` are the (position, source) at which the kernel reads a result: after the instructions before `position`
-    have run, so the value is kept until then.  Returns the instructions that remain as (position in `instrs`, opcode, register, code, code), the
-    code of each read's source, and the number of registers."""
+    """Dead-code elimination and register allocation of one tape.  `instrs` are (opcode, value id, source, source,
+    condition), the condition being SEL's (else None); `reads` are the (position, source) at which the kernel reads a
+    result: after the instructions before `position` have run, so the value is kept until then.  Returns the
+    instructions that remain as (position in `instrs`, opcode, register, code, code), the code of each read's source,
+    and the number of registers."""
     last = {}
     for pos, v in reads:
         if v[0] == 'v':
             last[v] = max(last.get(v, -1), pos)
     live = []
     for i in range(len(instrs) - 1, -1, -1):
-        op, v, a, b = instrs[i]
+        op, v, *srcs = instrs[i]
         if v not in last:
             continue
         live.append(i)
-        for s in (a, b):
+        for s in srcs:
             if s is not None and s[0] == 'v':
                 last[s] = max(last.get(s, -1), i)
     live.reverse()
@@ -130,19 +162,32 @@ def _allocate(instrs, reads):
             return _cabi.PW_OPERAND0 + s[1]
         return reg[s]
 
+    def fresh():
+        nonlocal n_regs
+        if free:
+            return free.pop()
+        n_regs += 1
+        return n_regs - 1
+
     out = []
     for i in live:
-        op, v, a, b = instrs[i]
+        op, v, a, b, c = instrs[i]
         ca, cb = code(a), code(b) if b is not None else 0
+        if c is not None:
+            # SEL reads its condition from its destination: the condition's own register when this is its last read,
+            # else a copy (maximum(c, c) is c exactly), made before the sources below are released
+            if last[c] <= i:
+                held.remove(c)
+                reg[v] = reg[c]
+            else:
+                reg[v] = fresh()
+                out.append((i, _cabi.PW_MAXIMUM, reg[v], reg[c], reg[c]))
         # (the kernel reads both sources before it writes the destination)
         for s in [s for s in held if last[s] <= i]:
             held.remove(s)
             free.append(reg[s])
-        if free:
-            reg[v] = free.pop()
-        else:
-            reg[v] = n_regs
-            n_regs += 1
+        if c is None:
+            reg[v] = fresh()
         held.append(v)
         out.append((i, op, reg[v], ca, cb))
     return out, [code(s) for _, s in reads], n_regs
@@ -156,7 +201,8 @@ class Recorder(TorchDispatchMode):
         self.rows, self.d = y.shape
         self.dtype, self.device = y.dtype, y.device
         self.ok, self.reason = True, None
-        self.instrs = []       # (opcode, value id, source, source)
+        self.instrs = []       # (opcode, value id, source, source, condition of a SEL or None)
+        self._bools = set()    # the values that are comparison results (0 or 1 in the state dtype)
         self.n_fg = None
         self.operands = []     # (kind, ptr, imm)
         self._operand_ix = {}
@@ -270,21 +316,115 @@ class Recorder(TorchDispatchMode):
         self._keep.append(x)
         return self._operand(kind, x.data_ptr(), 0.0)
 
-    def _result(self, out):
-        if not torch.is_tensor(out) or out.dtype != self.dtype or out.device != self.device:
+    def _number(self, x):
+        """The source of an op input that is a number: a comparison result is a condition only."""
+        src = self._source(x)
+        if src in self._bools:
+            raise Reject("a comparison result is used as a number")
+        return src
+
+    def _condition(self, x):
+        """The source of a condition (of where, masked_fill, a logical op): a comparison result of the tape."""
+        src = self._source(x)
+        if src not in self._bools:
+            raise Reject("a condition is not a comparison result of the tape")
+        return src
+
+    def _result(self, out, boolean=False):
+        want = torch.bool if boolean else self.dtype
+        if not torch.is_tensor(out) or out.dtype != want or out.device != self.device:
             raise Reject("result is not a tensor of the state dtype")
         if _strip(out.shape) not in self._shapes:
             raise Reject(f"result of shape {tuple(out.shape)}")
 
-    def _emit(self, op, a, b, out):
-        self._result(out)
+    def _value(self, op, a, b=None, cond=None, boolean=False):
         v = ('v', len(self.instrs))
-        self.instrs.append((op, v, a, b))
-        self._bind(out, v)
+        self.instrs.append((op, v, a, b, cond))
+        if boolean:
+            self._bools.add(v)
+        return v
+
+    def _emit(self, op, a, b, out, cond=None, boolean=False):
+        self._result(out, boolean)
+        self._bind(out, self._value(op, a, b, cond, boolean))
+
+    def _one(self):
+        return self._operand(_cabi.PW_IMM, None, 1.0)
+
+    def _bound(self, x):
+        """A scalar clamp bound as an immediate: clamp restates as maximum / minimum only when it is not NaN."""
+        imm = self._immediate(x)
+        if imm != imm:
+            raise Reject("a NaN clamp bound")
+        return self._operand(_cabi.PW_IMM, None, imm)
+
+    def _record_select(self, func, args, kwargs, out):
+        """The comparison and selection ops; False for any other op."""
+        if func in _COMPARE:
+            op, swap = _COMPARE[func]
+            a, b = self._number(args[0]), self._number(args[1])
+            if func in _NEGATED:
+                self._emit(_cabi.PW_SUB, self._one(), self._value(op, a, b, boolean=True), out, boolean=True)
+            else:
+                self._emit(op, *((b, a) if swap else (a, b)), out, boolean=True)
+        elif func in _LOGICAL:
+            c = self._condition(args[0])
+            if _LOGICAL[func] == _cabi.PW_SUB:
+                self._emit(_cabi.PW_SUB, self._one(), c, out, boolean=True)
+            else:
+                self._emit(_LOGICAL[func], c, self._condition(args[1]), out, boolean=True)
+        elif func is aten.where.self:
+            self._emit(_cabi.PW_SEL, self._number(args[1]), self._number(args[2]), out, self._condition(args[0]))
+        elif func is aten.masked_fill.Scalar:
+            self._emit(_cabi.PW_SEL, self._operand(_cabi.PW_IMM, None, self._immediate(args[2])),
+                       self._number(args[0]), out, self._condition(args[1]))
+        elif func in (aten.maximum.default, aten.minimum.default, aten.clamp_min.Tensor, aten.clamp_max.Tensor):
+            op = _cabi.PW_MAXIMUM if func in (aten.maximum.default, aten.clamp_min.Tensor) else _cabi.PW_MINIMUM
+            self._emit(op, self._number(args[0]), self._number(args[1]), out)
+        elif func in (aten.clamp.default, aten.clamp.Tensor, aten.clamp_min.default, aten.clamp_max.default,
+                      aten.relu.default):
+            # clamp is maximum with the lower bound, then minimum with the upper one: exactly ATen's clamp kernels
+            # when a scalar bound is not NaN (relu is clamp_min(y, 0)); a tensor bound propagates NaN as maximum does
+            x, scalar = self._number(args[0]), func in (aten.clamp.default, aten.clamp_min.default,
+                                                          aten.clamp_max.default)
+            lo = kwargs.get('min', args[1] if len(args) > 1 else None)
+            hi = kwargs.get('max', args[2] if len(args) > 2 else None)
+            if func is aten.clamp_max.default:
+                lo, hi = None, args[1]
+            elif func is aten.relu.default:
+                lo = 0
+            bounds = [(op, b) for op, b in ((_cabi.PW_MAXIMUM, lo), (_cabi.PW_MINIMUM, hi)) if b is not None]
+            if not bounds:
+                raise Reject(f"{func} without bounds")
+            for k, (op, b) in enumerate(bounds):
+                src = self._bound(b) if scalar else self._number(b)
+                if k + 1 < len(bounds):
+                    x = self._value(op, x, src)
+                else:
+                    self._emit(op, x, src, out)
+        elif func is aten.threshold_backward.default:  # x <= threshold ? 0 : grad
+            c = self._value(_cabi.PW_LE, self._number(args[1]), self._bound(args[2]), boolean=True)
+            self._emit(_cabi.PW_SEL, self._operand(_cabi.PW_IMM, None, 0.0), self._number(args[0]), out, c)
+        elif func in (aten.sign.default, aten.sgn.default):  # (0 < x) - (x < 0)
+            x, zero = self._number(args[0]), self._operand(_cabi.PW_IMM, None, 0.0)
+            pos = self._value(_cabi.PW_LT, zero, x, boolean=True)
+            self._emit(_cabi.PW_SUB, pos, self._value(_cabi.PW_LT, x, zero, boolean=True), out)
+        elif func is aten.reciprocal.default:  # 1 / x
+            self._emit(_cabi.PW_DIV, self._one(), self._number(args[0]), out)
+        elif func is aten.scalar_tensor.default:  # an immediate, rounded to its own dtype, then to the state's
+            dtype = kwargs.get('dtype') or torch.get_default_dtype()
+            if dtype not in (torch.float32, torch.float64) or isinstance(args[0], bool) or \
+                    not isinstance(args[0], numbers.Real):
+                raise Reject(f"scalar_tensor({args[0]!r}) of {dtype}")
+            own = (np.float32 if dtype == torch.float32 else np.float64)(args[0])
+            self._bind(out, self._operand(_cabi.PW_IMM, None, self._immediate(float(own))))
+        else:
+            return False
+        return True
 
     def _record(self, func, args, kwargs, out):
         if func in _ALIAS:
-            self._result(out)
+            self._result(out, self._source(args[0]) in self._bools)
             if _strip(args[0].shape) != _strip(out.shape) and not (
                     func is aten.expand.default and _strip(out.shape) == (self.rows, self.d)):
                 raise Reject(f"{func} moves elements")
@@ -297,13 +437,15 @@ class Recorder(TorchDispatchMode):
             func = _IN_PLACE[func]
         elif func._schema.is_mutable or 'out' in kwargs:
             raise Reject(f"{func} mutates its arguments")
+        if self._record_select(func, args, kwargs, out):
+            return
         if func in _UNARY:
-            self._emit(_UNARY[func], self._source(args[0]), None, out)
+            self._emit(_UNARY[func], self._number(args[0]), None, out)
             return
         if func is aten.pow.Tensor_Scalar:
             if not (isinstance(args[1], numbers.Real) and not isinstance(args[1], bool) and args[1] == 2):
                 raise Reject(f"pow with exponent {args[1]!r}")
-            a = self._source(args[0])
+            a = self._number(args[0])
             self._emit(_cabi.PW_MUL, a, a, out)
             return
         if func not in _BINARY:
@@ -322,9 +464,9 @@ class Recorder(TorchDispatchMode):
                                    and b.device != self.device):
             # ATen: a CPU-scalar divisor becomes a multiplication by its reciprocal, rounded in the state dtype
             inv = self._np(1) / self._np(self._immediate(b.item() if torch.is_tensor(b) else b))
-            self._emit(_cabi.PW_MUL, self._source(a), self._operand(_cabi.PW_IMM, None, float(inv)), out)
+            self._emit(_cabi.PW_MUL, self._number(a), self._operand(_cabi.PW_IMM, None, float(inv)), out)
             return
-        self._emit(op, self._source(a), self._source(b), out)
+        self._emit(op, self._number(a), self._number(b), out)
 
     # -- the program -----------------------------------------------------------------------------------------------
     def _step_result(self, t, allow_go=False):
@@ -419,7 +561,7 @@ class SrkRecorder(Recorder):
         """Instructions [start, end) and the result, with value ids relative to the segment."""
         def rel(s):
             return ('v', s[1] - start) if s is not None and s[0] == 'v' else s
-        return [(op, rel(v), rel(a), rel(b)) for op, v, a, b in self.instrs[start:end]], rel(src)
+        return [(op, *map(rel, srcs)) for op, *srcs in self.instrs[start:end]], rel(src)
 
     def finish(self):
         """The tsde_pointwise program of the recorded step (and the tensors it reads), or None if it was rejected."""

@@ -48,9 +48,12 @@ struct PwP {
 // broadcast).  CHANNEL / ROW operands past kPwHoistSlots are read from global memory at every use instead.
 //
 // An instruction is one word: op in bits [0, 3), dst in [3, 8), source a in [8, 20), source b in [20, 32) (b = a for
-// NEG and SQRT).  A source is a slot in bits [0, 5), with kPwSrcUniform its lane in bits [6, 11); or kPwSrcGlobal and
-// the index of its operand in bits [0, 5).
-constexpr uint32_t kPwSrcUniform = 1u << 5, kPwSrcGlobal = 1u << 11;
+// NEG, SQRT and ABS).  A source is a slot in bits [0, 5), with kPwSrcUniform its lane in bits [6, 11); or kPwSrcGlobal
+// and the index of its operand in bits [0, 5).  A program with comparison and selection ops (PwProg::ext) needs a
+// fourth op bit: its words keep it in bit 31, and its sources are 11 bits, a global operand being kPwExtGlobal (the
+// uniform bit with lane 31, which no uniform operand has).  SEL's third source, its condition, is the dst slot.  The
+// six-op programs keep the encoding, and the loop, they always had.
+constexpr uint32_t kPwSrcUniform = 1u << 5, kPwSrcGlobal = 1u << 11, kPwExtGlobal = kPwSrcUniform | 31u << 6;
 
 // CHANNEL / ROW operands are hoisted into slots only while the layout stays within kPwHoistSlots slots, the footprint
 // of a program of TSDE_PW_MAX_REGS registers: hoisting never raises a program's shared memory past what the library's
@@ -59,7 +62,7 @@ constexpr int kPwHoistSlots = TSDE_PW_MAX_REGS;
 constexpr int kPwMaxSlots = TSDE_PW_MAX_REGS + 4;
 static_assert(kPwMaxSlots * kThreads * 4 * sizeof(double) <= 227 * 1024,
               "every accepted program's fp64 register file fits one CTA's shared memory");
-static_assert(kPwMaxSlots <= 32 && TSDE_PW_MAX_OPERANDS <= 32, "slots and operand indices fit five bits");
+static_assert(kPwMaxSlots <= 32 && TSDE_PW_MAX_OPERANDS <= 31, "slots, operand indices and lanes fit five bits");
 
 template <typename T>
 struct PwOperand {
@@ -74,6 +77,7 @@ struct PwProg {
   int8_t y, go, t0, u, hoist, end;  // slots (t0: -1 when no operand reads the time)
   int8_t n_uniform, n_hoisted;      // operand[0, n_uniform) fill the u slot, the next n_hoisted the hoisted slots
   int8_t n_global;                  // the operands past those, read from global memory at every use
+  int8_t ext;                       // some instruction has an opcode past TSDE_PW_SQRT
   uint32_t row;                     // bit k: operand[k] is a ROW operand (else CHANNEL)
   uint32_t instr[TSDE_PW_MAX_INSTR];
   PwOperand<T> operand[TSDE_PW_MAX_OPERANDS];
@@ -109,11 +113,12 @@ struct PwQuad {  // where this thread's quad lives
   bool vec;
 };
 
-// GLOBAL: the source may be a CHANNEL / ROW operand that did not fit the slots, read from global memory
-template <bool GLOBAL = true, typename T>
+// GLOBAL: the source may be a CHANNEL / ROW operand that did not fit the slots, read from global memory; EXT: the
+// source is in the encoding of a program with comparison and selection ops
+template <bool GLOBAL = true, bool EXT = false, typename T>
 __device__ __forceinline__ void pw_fetch(const PwProg<T>& pg, const PwQuad& c, const void* regs, uint32_t s,
                                          T (&v)[4]) {
-  if (GLOBAL && (s & kPwSrcGlobal)) {
+  if (GLOBAL && (EXT ? (s & kPwExtGlobal) == kPwExtGlobal : (s & kPwSrcGlobal) != 0)) {
     const int k = s & 31;
     load_quad(pg.operand[k].ptr, (pg.row >> k) & 1 ? c.base : c.chan, c.vec, c.nvalid, v);
     return;
@@ -121,14 +126,53 @@ __device__ __forceinline__ void pw_fetch(const PwProg<T>& pg, const PwQuad& c, c
   pw_sload(regs, s & 31, s & kPwSrcUniform ? s >> 6 : threadIdx.x, v);
 }
 
-// instructions [i0, i1): one warp-uniform dispatch per instruction, one IEEE rounding per element (-fmad=false)
-template <bool GLOBAL, typename T>
+// instructions [i0, i1): one warp-uniform dispatch per instruction, one IEEE rounding per element (-fmad=false).  EXT:
+// the program has comparison and selection ops (opcodes past TSDE_PW_SQRT), which round nothing; each case is the
+// expression of the ATen CUDA kernel it restates (::max / ::min are fmax / fmin), so NaN payloads and signed zeros come
+// out as ATen's do.  Programs without them run the six-op loop.
+template <bool GLOBAL, bool EXT, typename T>
 __device__ __forceinline__ void pw_loop(const PwProg<T>& pg, const PwQuad& c, void* regs, int i0, int i1) {
   for (int i = i0; i < i1; ++i) {
     const uint32_t in = pg.instr[i];
     T a[4], b[4], r[4];
-    pw_fetch<GLOBAL>(pg, c, regs, (in >> 8) & 0xFFF, a);
-    pw_fetch<GLOBAL>(pg, c, regs, in >> 20, b);
+    pw_fetch<GLOBAL, EXT>(pg, c, regs, (in >> 8) & 0xFFF, a);
+    pw_fetch<GLOBAL, EXT>(pg, c, regs, EXT ? (in >> 20) & 0x7FF : in >> 20, b);
+    if (EXT && (in >> 31)) {  // (opcodes 8 to 14)
+      const int dst = (in >> 3) & 31;
+      switch ((in & 7) | 8) {
+        case TSDE_PW_LT:  // lt, and gt with the operands swapped
+#pragma unroll
+          for (int j = 0; j < 4; ++j) r[j] = a[j] < b[j] ? T(1) : T(0);
+          break;
+        case TSDE_PW_LE:  // le, ge with the operands swapped, threshold_backward's x <= threshold
+#pragma unroll
+          for (int j = 0; j < 4; ++j) r[j] = a[j] <= b[j] ? T(1) : T(0);
+          break;
+        case TSDE_PW_EQ:
+#pragma unroll
+          for (int j = 0; j < 4; ++j) r[j] = a[j] == b[j] ? T(1) : T(0);
+          break;
+        case TSDE_PW_MAXIMUM:  // maximum_kernel_cuda
+#pragma unroll
+          for (int j = 0; j < 4; ++j) r[j] = a[j] != a[j] ? a[j] : b[j] != b[j] ? b[j] : ::max(a[j], b[j]);
+          break;
+        case TSDE_PW_MINIMUM:  // minimum_kernel_cuda
+#pragma unroll
+          for (int j = 0; j < 4; ++j) r[j] = a[j] != a[j] ? a[j] : b[j] != b[j] ? b[j] : ::min(a[j], b[j]);
+          break;
+        case TSDE_PW_ABS:
+#pragma unroll
+          for (int j = 0; j < 4; ++j) r[j] = fabs(a[j]);
+          break;
+        default:  // TSDE_PW_SEL: where_kernel, masked_fill; the condition is the destination (read into r)
+          pw_sload(regs, dst, threadIdx.x, r);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) r[j] = r[j] != T(0) ? a[j] : b[j];
+          break;
+      }
+      pw_sstore(regs, dst, r);
+      continue;
+    }
     switch (in & 7) {
       case TSDE_PW_MUL:
 #pragma unroll
@@ -160,13 +204,16 @@ __device__ __forceinline__ void pw_loop(const PwProg<T>& pg, const PwQuad& c, vo
 }
 
 // The loop that reads only shared memory unless the program has operands in global memory, which is rare (see
-// kPwHoistSlots)
-template <typename T>
+// kPwHoistSlots).  EXT: the program has comparison and selection ops; those programs run in kernels of their own (the
+// *_ext_kernel instantiations), so that the six-op programs run the code, and the registers, they always ran.
+template <bool EXT, typename T>
 __device__ __forceinline__ void pw_run(const PwProg<T>& pg, const PwQuad& c, void* regs, int i0, int i1) {
-  if (pg.n_global)
-    pw_loop<true>(pg, c, regs, i0, i1);
+  if (EXT)
+    pw_loop<true, true>(pg, c, regs, i0, i1);
+  else if (pg.n_global)
+    pw_loop<true, false>(pg, c, regs, i0, i1);
   else
-    pw_loop<false>(pg, c, regs, i0, i1);
+    pw_loop<false, false>(pg, c, regs, i0, i1);
 }
 
 // The launch-uniform values into the u slot; every thread of the CTA calls it (it ends in a barrier), after the
@@ -232,12 +279,17 @@ static bool pw_valid_source(const tsde_pointwise& pg, uint32_t s, bool allow_go,
   return (int)s < pg.n_regs && ((written >> s) & 1u);
 }
 
+// NEG, SQRT and ABS read source a only
+static bool pw_unary(int op) { return op == TSDE_PW_NEG || op == TSDE_PW_SQRT || op == TSDE_PW_ABS; }
+
 // instructions [i0, i1), run in order from the registers in `written`, which gains the ones they define
 static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, bool allow_go, uint64_t& written) {
   for (int i = i0; i < i1; ++i) {
     const tsde_pw_instr& in = pg.instr[i];
-    if (in.op > TSDE_PW_SQRT || (int)in.dst >= pg.n_regs || !pw_valid_source(pg, in.a, allow_go, written)) return false;
-    if (in.op != TSDE_PW_NEG && in.op != TSDE_PW_SQRT && !pw_valid_source(pg, in.b, allow_go, written)) return false;
+    if ((in.op > TSDE_PW_SQRT && in.op < TSDE_PW_LT) || in.op > TSDE_PW_SEL) return false;
+    if ((int)in.dst >= pg.n_regs || !pw_valid_source(pg, in.a, allow_go, written)) return false;
+    if (!pw_unary(in.op) && !pw_valid_source(pg, in.b, allow_go, written)) return false;
+    if (in.op == TSDE_PW_SEL && !((written >> in.dst) & 1u)) return false;  // the condition
     written |= 1ull << in.dst;
   }
   return true;
@@ -249,6 +301,7 @@ static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, bool allow_
 template <typename T>
 static int pw_decode(const tsde_pointwise& in, bool go, int extra, PwProg<T>& pg) {
   pg = PwProg<T>{};
+  for (int i = 0; i < in.n_instr; ++i) pg.ext = pg.ext || in.instr[i].op > TSDE_PW_SQRT;
   pg.n_fg = in.n_fg;
   pg.n_instr = in.n_instr;
   int n_uniform = 0, n_local = 0;
@@ -285,8 +338,10 @@ static int pw_decode(const tsde_pointwise& in, bool go, int extra, PwProg<T>& pg
     if (o.kind == TSDE_PW_ROW) pg.row |= 1u << j;
     if (!local)
       src[k] = pg.u | kPwSrcUniform | (uint32_t)j << 6;
+    else if (j - n_uniform < pg.n_hoisted)
+      src[k] = pg.hoist + (j - n_uniform);
     else
-      src[k] = j - n_uniform < pg.n_hoisted ? pg.hoist + (j - n_uniform) : kPwSrcGlobal | j;
+      src[k] = (pg.ext ? kPwExtGlobal : kPwSrcGlobal) | j;
   }
   auto source = [&](uint32_t s) -> uint32_t {
     if (s == TSDE_PW_SRC_Y) return pg.y;
@@ -295,8 +350,8 @@ static int pw_decode(const tsde_pointwise& in, bool go, int extra, PwProg<T>& pg
   };
   for (int i = 0; i < in.n_instr; ++i) {
     const tsde_pw_instr& x = in.instr[i];
-    const uint32_t a = source(x.a), b = x.op == TSDE_PW_NEG || x.op == TSDE_PW_SQRT ? a : source(x.b);
-    pg.instr[i] = x.op | (uint32_t)x.dst << 3 | a << 8 | b << 20;
+    const uint32_t a = source(x.a), b = pw_unary(x.op) ? a : source(x.b);
+    pg.instr[i] = (x.op & 7u) | (uint32_t)x.dst << 3 | a << 8 | b << 20 | (uint32_t)(x.op >> 3) << 31;
   }
   pg.f_src = source(in.f_src);
   pg.g_src = source(in.g_src);
@@ -385,10 +440,9 @@ struct PwSteps {  // by value: a captured launch carries the whole table
 static_assert(sizeof(PwProg<double>) + sizeof(PwP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <= 4096,
               "the Milstein kernel's parameters fit the 4 KiB parameter space");
 
-template <typename T, int SRC>
-__global__ void __launch_bounds__(kThreads)
-pw_milstein_kernel(const __grid_constant__ PwProg<T> pg, const PwP<T> p, const NoiseP<T> nz,
-                   const __grid_constant__ PwSteps<T> st) {
+template <typename T, int SRC, bool EXT>
+__device__ __forceinline__ void pw_milstein(const PwProg<T>& pg, const PwP<T> p, const NoiseP<T> nz,
+                                           const PwSteps<T>& st) {
   extern __shared__ __align__(16) unsigned char pw_regs[];
   PwQuad c;
   int64_t Q, row, q;
@@ -410,10 +464,10 @@ pw_milstein_kernel(const __grid_constant__ PwProg<T> pg, const PwP<T> p, const N
       pw_load_hoisted(pg, c, pw_regs);
     }
     pw_set_state(pg, pw_regs, s.t0, y);
-    pw_run(pg, c, pw_regs, 0, pg.n_fg);
+    pw_run<EXT>(pg, c, pw_regs, 0, pg.n_fg);
     T f[4], g[4], go[4];
-    pw_fetch(pg, c, pw_regs, pg.f_src, f);
-    pw_fetch(pg, c, pw_regs, pg.g_src, g);
+    pw_fetch<true, EXT>(pg, c, pw_regs, pg.f_src, f);
+    pw_fetch<true, EXT>(pg, c, pw_regs, pg.g_src, g);
     const MilsteinSeedOp<T> seed{s.dt, p.ito};
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -422,9 +476,9 @@ pw_milstein_kernel(const __grid_constant__ PwProg<T> pg, const PwP<T> p, const N
       go[i] = o[0];
     }
     pw_sstore(pw_regs, pg.go, go);
-    pw_run(pg, c, pw_regs, pg.n_fg, pg.n_instr);
+    pw_run<EXT>(pg, c, pw_regs, pg.n_fg, pg.n_instr);
     T gdg[4];
-    pw_fetch(pg, c, pw_regs, pg.gdg_src, gdg);
+    pw_fetch<true, EXT>(pg, c, pw_regs, pg.gdg_src, gdg);
     const MilsteinOp<T> step{s.dt};
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -434,6 +488,19 @@ pw_milstein_kernel(const __grid_constant__ PwProg<T> pg, const PwP<T> p, const N
     }
     if (s.y1) store_quad(s.y1, c.base, c.vec, c.nvalid, y);
   }
+}
+
+template <typename T, int SRC>
+__global__ void __launch_bounds__(kThreads)
+pw_milstein_kernel(const __grid_constant__ PwProg<T> pg, const PwP<T> p, const NoiseP<T> nz,
+                   const __grid_constant__ PwSteps<T> st) {
+  pw_milstein<T, SRC, false>(pg, p, nz, st);
+}
+template <typename T, int SRC>
+__global__ void __launch_bounds__(kThreads)
+pw_milstein_ext_kernel(const __grid_constant__ PwProg<T> pg, const PwP<T> p, const NoiseP<T> nz,
+                       const __grid_constant__ PwSteps<T> st) {
+  pw_milstein<T, SRC, true>(pg, p, nz, st);
 }
 
 // The Milstein layout, in the order the kernel reads it: go exists from the vjp part on, registers carry over.
@@ -489,17 +556,16 @@ struct PwSrkStash {
 
 // One SDE evaluation of the two-program layout (SRK, predictor-corrector): f (program [0, n_fg), result f_src) or g
 // (program [n_fg, n_instr), result g_src) at (t, y)
-template <typename T>
+template <bool EXT, typename T>
 __device__ __forceinline__ void pw_eval(const PwProg<T>& pg, const PwQuad& c, void* regs, bool g, const T* t,
                                         const T (&y)[4], T (&out)[4]) {
   pw_set_state(pg, regs, t, y);
-  pw_run(pg, c, regs, g ? pg.n_fg : 0, g ? pg.n_instr : pg.n_fg);
-  pw_fetch(pg, c, regs, g ? pg.g_src : pg.f_src, out);
+  pw_run<EXT>(pg, c, regs, g ? pg.n_fg : 0, g ? pg.n_instr : pg.n_fg);
+  pw_fetch<true, EXT>(pg, c, regs, g ? pg.g_src : pg.f_src, out);
 }
 
-template <typename T, int SRC>
-__global__ void __launch_bounds__(kThreads)
-pw_srk_kernel(const __grid_constant__ PwProg<T> pg, const PwSrkP<T> p, const NoiseP<T> nz) {
+template <typename T, int SRC, bool EXT>
+__device__ __forceinline__ void pw_srk(const PwProg<T>& pg, const PwSrkP<T> p, const NoiseP<T> nz) {
   extern __shared__ __align__(16) unsigned char pw_regs[];
   PwQuad c;
   T w[4], u[4], y0[4];
@@ -509,8 +575,8 @@ pw_srk_kernel(const __grid_constant__ PwProg<T> pg, const PwSrkP<T> p, const Noi
   enum { F0, F1, F2, G0, G1, G2 };
   T f[4], g[4], h0[4], h1[4], x[4], z[4];
   // s = 0: f0, g0 at (t0, y0); H0_1, H1_1
-  pw_eval(pg, c, pw_regs, false, p.t[0], y0, f);
-  pw_eval(pg, c, pw_regs, true, p.t[0], y0, g);
+  pw_eval<EXT>(pg, c, pw_regs, false, p.t[0], y0, f);
+  pw_eval<EXT>(pg, c, pw_regs, true, p.t[0], y0, g);
   st.put(pw_regs, F0, f);
   st.put(pw_regs, G0, g);
 #pragma unroll
@@ -521,8 +587,8 @@ pw_srk_kernel(const __grid_constant__ PwProg<T> pg, const PwSrkP<T> p, const Noi
     h1[j] = o[1];
   }
   // s = 1: f1 at (t0 + dt, H0_1), g1 at (t0 + dt/4, H1_1); H0_2, H1_2
-  pw_eval(pg, c, pw_regs, false, p.t[1], h0, f);
-  pw_eval(pg, c, pw_regs, true, p.t[2], h1, g);
+  pw_eval<EXT>(pg, c, pw_regs, false, p.t[1], h0, f);
+  pw_eval<EXT>(pg, c, pw_regs, true, p.t[2], h1, g);
   st.put(pw_regs, F1, f);
   st.put(pw_regs, G1, g);
   st.get(pw_regs, F0, x);
@@ -535,8 +601,8 @@ pw_srk_kernel(const __grid_constant__ PwProg<T> pg, const PwSrkP<T> p, const Noi
     h1[j] = o[1];
   }
   // s = 2: f2 at (t0 + dt/2, H0_2), g2 at (t0 + dt, H1_2); H1_3
-  pw_eval(pg, c, pw_regs, false, p.t[3], h0, f);
-  pw_eval(pg, c, pw_regs, true, p.t[1], h1, g);
+  pw_eval<EXT>(pg, c, pw_regs, false, p.t[3], h0, f);
+  pw_eval<EXT>(pg, c, pw_regs, true, p.t[1], h1, g);
   st.put(pw_regs, F2, f);
   st.put(pw_regs, G2, g);
   st.get(pw_regs, G0, x);
@@ -548,7 +614,7 @@ pw_srk_kernel(const __grid_constant__ PwProg<T> pg, const PwSrkP<T> p, const Noi
     h1[j] = o[0];
   }
   // s = 3: g3 at (t0 + dt/4, H1_3); y1
-  pw_eval(pg, c, pw_regs, true, p.t[2], h1, g);
+  pw_eval<EXT>(pg, c, pw_regs, true, p.t[2], h1, g);
   T f0[4], f1[4], f2[4], g0[4], g1[4], g2[4], y1[4];
   st.get(pw_regs, F0, f0);
   st.get(pw_regs, F1, f1);
@@ -563,6 +629,17 @@ pw_srk_kernel(const __grid_constant__ PwProg<T> pg, const PwSrkP<T> p, const Noi
     y1[j] = o[0];
   }
   store_quad(p.base.y1, c.base, c.vec, c.nvalid, y1);
+}
+
+template <typename T, int SRC>
+__global__ void __launch_bounds__(kThreads)
+pw_srk_kernel(const __grid_constant__ PwProg<T> pg, const PwSrkP<T> p, const NoiseP<T> nz) {
+  pw_srk<T, SRC, false>(pg, p, nz);
+}
+template <typename T, int SRC>
+__global__ void __launch_bounds__(kThreads)
+pw_srk_ext_kernel(const __grid_constant__ PwProg<T> pg, const PwSrkP<T> p, const NoiseP<T> nz) {
+  pw_srk<T, SRC, true>(pg, p, nz);
 }
 
 // The two-program layout (SRK, predictor-corrector): an f program and a g program that each start with no register
@@ -590,17 +667,16 @@ struct PwPcP {
   T half_dt;
 };
 
-template <typename T, int SRC, int METHOD>
-__global__ void __launch_bounds__(kThreads, 1)
-pw_pc_kernel(const __grid_constant__ PwProg<T> pg, const PwPcP<T> p, const NoiseP<T> nz) {
+template <typename T, int SRC, int METHOD, bool EXT>
+__device__ __forceinline__ void pw_pc(const PwProg<T>& pg, const PwPcP<T> p, const NoiseP<T> nz) {
   extern __shared__ __align__(16) unsigned char pw_regs[];
   PwQuad c;
   T w[4], u[4], y0[4];
   if (!pw_begin<T, SRC, false>(pg, p.base, nz, pw_regs, c, w, u, y0)) return;
   const T dt = p.base.dt;
   T f0[4], g0[4], yp[4];
-  pw_eval(pg, c, pw_regs, false, p.base.t0, y0, f0);
-  pw_eval(pg, c, pw_regs, true, p.base.t0, y0, g0);
+  pw_eval<EXT>(pg, c, pw_regs, false, p.base.t0, y0, f0);
+  pw_eval<EXT>(pg, c, pw_regs, true, p.base.t0, y0, g0);
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     T o[1];
@@ -614,8 +690,8 @@ pw_pc_kernel(const __grid_constant__ PwProg<T> pg, const PwPcP<T> p, const Noise
     yp[j] = o[0];
   }
   T f[4], g[4], y1[4];
-  if constexpr (METHOD != TSDE_PC_EULER_HEUN) pw_eval(pg, c, pw_regs, false, p.t_p, yp, f);
-  pw_eval(pg, c, pw_regs, true, p.t_p, yp, g);
+  if constexpr (METHOD != TSDE_PC_EULER_HEUN) pw_eval<EXT>(pg, c, pw_regs, false, p.t_p, yp, f);
+  pw_eval<EXT>(pg, c, pw_regs, true, p.t_p, yp, g);
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     T o[1];
@@ -629,6 +705,17 @@ pw_pc_kernel(const __grid_constant__ PwProg<T> pg, const PwPcP<T> p, const Noise
     y1[j] = o[0];
   }
   store_quad(p.base.y1, c.base, c.vec, c.nvalid, y1);
+}
+
+template <typename T, int SRC, int METHOD>
+__global__ void __launch_bounds__(kThreads, 1)
+pw_pc_kernel(const __grid_constant__ PwProg<T> pg, const PwPcP<T> p, const NoiseP<T> nz) {
+  pw_pc<T, SRC, METHOD, false>(pg, p, nz);
+}
+template <typename T, int SRC, int METHOD>
+__global__ void __launch_bounds__(kThreads, 1)
+pw_pc_ext_kernel(const __grid_constant__ PwProg<T> pg, const PwPcP<T> p, const NoiseP<T> nz) {
+  pw_pc<T, SRC, METHOD, true>(pg, p, nz);
 }
 
 // ---- consecutive Euler or reversible-Heun steps (tsde_solve_euler_pointwise, tsde_solve_reversible_heun_pointwise) --
@@ -653,10 +740,9 @@ static_assert(sizeof(PwProg<double>) + sizeof(PwChunkP<double>) + sizeof(NoiseP<
                   4096,
               "the chunk kernel's parameters fit the 4 KiB parameter space");
 
-template <typename T, int SRC, int METHOD>
-__global__ void __launch_bounds__(kThreads, 1)
-pw_chunk_kernel(const __grid_constant__ PwProg<T> pg, const PwChunkP<T> p, const NoiseP<T> nz,
-                const __grid_constant__ PwSteps<T> st) {
+template <typename T, int SRC, int METHOD, bool EXT>
+__device__ __forceinline__ void pw_chunk_steps(const PwProg<T>& pg, const PwChunkP<T> p, const NoiseP<T> nz,
+                                               const PwSteps<T>& st) {
   extern __shared__ __align__(16) unsigned char pw_regs[];
   PwQuad c;
   int64_t Q, row, q;
@@ -683,8 +769,8 @@ pw_chunk_kernel(const __grid_constant__ PwProg<T> pg, const PwChunkP<T> p, const
       pw_load_hoisted(pg, c, pw_regs);
     }
     if constexpr (METHOD == kPwEuler) {
-      pw_eval(pg, c, pw_regs, false, s.t0, y, f);
-      pw_eval(pg, c, pw_regs, true, s.t0, y, g);
+      pw_eval<EXT>(pg, c, pw_regs, false, s.t0, y, f);
+      pw_eval<EXT>(pg, c, pw_regs, true, s.t0, y, g);
       const EulerOp<T> step{s.dt};
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
@@ -701,8 +787,8 @@ pw_chunk_kernel(const __grid_constant__ PwProg<T> pg, const PwChunkP<T> p, const
         z[i] = o[0];
       }
       T f1[4], g1[4];
-      pw_eval(pg, c, pw_regs, false, s.t0, z, f1);
-      pw_eval(pg, c, pw_regs, true, s.t0, z, g1);
+      pw_eval<EXT>(pg, c, pw_regs, false, s.t0, z, f1);
+      pw_eval<EXT>(pg, c, pw_regs, true, s.t0, z, g1);
       const RevHeunOp<T> step{T(0.5) * s.dt};
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
@@ -720,6 +806,19 @@ pw_chunk_kernel(const __grid_constant__ PwProg<T> pg, const PwChunkP<T> p, const
     store_quad(p.f1, c.base, c.vec, c.nvalid, f);
     store_quad(p.g1, c.base, c.vec, c.nvalid, g);
   }
+}
+
+template <typename T, int SRC, int METHOD>
+__global__ void __launch_bounds__(kThreads, 1)
+pw_chunk_kernel(const __grid_constant__ PwProg<T> pg, const PwChunkP<T> p, const NoiseP<T> nz,
+                const __grid_constant__ PwSteps<T> st) {
+  pw_chunk_steps<T, SRC, METHOD, false>(pg, p, nz, st);
+}
+template <typename T, int SRC, int METHOD>
+__global__ void __launch_bounds__(kThreads, 1)
+pw_chunk_ext_kernel(const __grid_constant__ PwProg<T> pg, const PwChunkP<T> p, const NoiseP<T> nz,
+                    const __grid_constant__ PwSteps<T> st) {
+  pw_chunk_steps<T, SRC, METHOD, true>(pg, p, nz, st);
 }
 
 // ---- launch ---------------------------------------------------------------------------------------------------------
@@ -789,6 +888,9 @@ static int pw_milstein_chunk(const tsde_launch* L, const tsde_noise* nz, const t
   np.cell_id = steps[0].cell_id;
   np.h = steps[0].h;
   p.ito = ito;
+  if (pg.ext)
+    return pw_launch<T>(L, pg, pw_milstein_ext_kernel<T, TSDE_SRC_COUNTER>, pw_milstein_ext_kernel<T, kSrcCounterMulti>,
+                        p, np, p.nquads, slots, TSDE_KERNEL_PW_MILSTEIN, st);
   return pw_launch<T>(L, pg, pw_milstein_kernel<T, TSDE_SRC_COUNTER>, pw_milstein_kernel<T, kSrcCounterMulti>, p, np,
                       p.nquads, slots, TSDE_KERNEL_PW_MILSTEIN, st);
 }
@@ -830,6 +932,10 @@ static int pw_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_point
   }
   np.cell_id = steps[0].cell_id;
   np.h = steps[0].h;
+  if (pg.ext)
+    return pw_launch<T>(L, pg, pw_chunk_ext_kernel<T, TSDE_SRC_COUNTER, METHOD>,
+                        pw_chunk_ext_kernel<T, kSrcCounterMulti, METHOD>, p, np, p.base.nquads, slots,
+                        TSDE_KERNEL_PW_CHUNK, st);
   return pw_launch<T>(L, pg, pw_chunk_kernel<T, TSDE_SRC_COUNTER, METHOD>, pw_chunk_kernel<T, kSrcCounterMulti, METHOD>,
                       p, np, p.base.nquads, slots, TSDE_KERNEL_PW_CHUNK, st);
 }
@@ -896,6 +1002,9 @@ TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_no
     p.s2 = SrkDiagStage2Op<T>{(T)dt, (T)rdt, (T)sqrt_dt};
     p.s3 = SrkDiagStage3Op<T>{(T)dt, (T)sqrt_dt};
     p.fin = make_srk_final<T>(dt, rdt, sqrt_dt, three_dt);
+    if (pg.ext)
+      return pw_launch<T>(L, pg, pw_srk_ext_kernel<T, TSDE_SRC_COUNTER>, pw_srk_ext_kernel<T, kSrcCounterMulti>, p, np,
+                          p.base.nquads, slots, TSDE_KERNEL_PW_SRK);
     return pw_launch<T>(L, pg, pw_srk_kernel<T, TSDE_SRC_COUNTER>, pw_srk_kernel<T, kSrcCounterMulti>, p, np,
                         p.base.nquads, slots, TSDE_KERNEL_PW_SRK);
   });
@@ -922,6 +1031,19 @@ TSDE_EXPORT int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, co
     auto go = [&](auto single, auto multi) {
       return pw_launch<T>(L, pg, single, multi, p, np, p.base.nquads, slots, TSDE_KERNEL_PW_PC);
     };
+    if (pg.ext) {
+      switch (method) {
+        case TSDE_PC_HEUN:
+          return go(pw_pc_ext_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_HEUN>,
+                    pw_pc_ext_kernel<T, kSrcCounterMulti, TSDE_PC_HEUN>);
+        case TSDE_PC_MIDPOINT:
+          return go(pw_pc_ext_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_MIDPOINT>,
+                    pw_pc_ext_kernel<T, kSrcCounterMulti, TSDE_PC_MIDPOINT>);
+        default:
+          return go(pw_pc_ext_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_EULER_HEUN>,
+                    pw_pc_ext_kernel<T, kSrcCounterMulti, TSDE_PC_EULER_HEUN>);
+      }
+    }
     switch (method) {
       case TSDE_PC_HEUN:
         return go(pw_pc_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_HEUN>, pw_pc_kernel<T, kSrcCounterMulti, TSDE_PC_HEUN>);
