@@ -43,6 +43,7 @@ extern "C" {
 
 #define TSDE_ABI_VERSION 1
 #define TSDE_EINVAL (-22)
+#define TSDE_ECOMPILE (-38) /* an element-wise program could not be compiled (tsde_pointwise_compile) */
 
 enum { TSDE_F32 = 0, TSDE_F64 = 1 };
 
@@ -328,6 +329,27 @@ typedef struct tsde_pw_step {
 } tsde_pw_step;
 int tsde_solve_milstein_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
                                   const void* y0, const tsde_pw_step* steps, int32_t n_steps, int32_t ito);
+
+/*
+ * The Milstein entry points above do not interpret `prog`: each program structure is compiled at run time into a
+ * kernel of its own, with the program as straight-line register code (NVRTC, sm_90a, the IEEE options of the library
+ * build), and loaded into a process-wide cache.  The structure is everything but the operand values and addresses
+ * (instructions, n_regs, n_fg, the result sources, the operand kinds) and the dtype: programs that differ only in
+ * IMM values or device pointers share one kernel, which reads those as launch parameters.  A program is compiled on
+ * its first launch unless tsde_pointwise_compile compiled it before.
+ *
+ * tsde_pointwise_compile compiles and loads the kernels of Milstein program `prog` for the launches `L` describes
+ * (its dtype; DIAGONAL noise, m == d) without launching anything: call it before a stream capture, since a capture
+ * should not load modules.  Returns 0 (also for an empty launch, which compiles nothing), TSDE_EINVAL for a launch or
+ * program tsde_solve_milstein_pointwise refuses, TSDE_ECOMPILE when NVRTC (libnvrtc.so.12) is not found or the
+ * compilation fails (tsde_error_string(TSDE_ECOMPILE) then holds the compiler's log), or the cudaError_t of loading
+ * the kernels.
+ * tsde_pointwise_source writes the source compiled for such a program (at most `size` bytes, NUL-terminated, when
+ * `buf` is given) and returns its length, or TSDE_EINVAL (0 for an empty launch); it needs no device.  Two programs
+ * share a kernel exactly when their sources are equal.
+ */
+int tsde_pointwise_compile(const tsde_launch* L, const tsde_pointwise* prog);
+int64_t tsde_pointwise_source(const tsde_launch* L, const tsde_pointwise* prog, char* buf, int64_t size);
 
 /*
  * A whole diagonal-noise SRK (srid2) step (srk.py:57-88) for an SDE whose f(t, y) and g(t, y) are element-wise

@@ -12,7 +12,11 @@ The program is the one the solver records for cfg2's SDE (f = mu*y, g = sigma*y,
   chunk_K  K consecutive steps in one launch, every step's y1 stored to its row of an output series (as cfg2 stores
            every step), in situ (the next launch starts from the last row) and cold (y0 from the rotating sets);
            microseconds per step and the achieved write bandwidth.  K = 128 does not fit the step table
-           (TSDE_PW_MAX_STEPS = 64, bounded by the 4 KiB parameter space) and is reported as such.
+           (TSDE_PW_MAX_STEPS = 64, bounded by the 4 KiB parameter space) and is reported as such.  The write bandwidth is also
+           given as a share of the H100 SXM data sheet's 3.35 TB/s, the floor of a step being its y1 store.
+  compile  the one-time cost of the program's kernels: tsde_pointwise_compile (NVRTC to an sm_90a cubin, then the
+           library load) in a process that has not compiled the program yet, in ms.  The solver pays it on the recording
+           step, outside bench.py's timed region; a later program of the same structure pays nothing.
 Algorithmic bytes of the fused step: 2 * D * 4 per trajectory (y0 read, y1 written).  Prints one JSON line with the
 card's name and power limit.
 """
@@ -21,6 +25,7 @@ import json
 import os
 import subprocess
 import sys
+import time
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
@@ -61,6 +66,9 @@ def record_program():
 
 
 prog = record_program()
+_t = time.perf_counter()
+_cabi.check(_cabi.compile_pointwise(prog, torch.float32), 'compile')
+compile_ms = (time.perf_counter() - _t) * 1e3
 sets = [{k: torch.rand(B, D, device=dev) + 0.5 for k in ('y0', 'y1')} for _ in range(NSET)]
 
 
@@ -131,8 +139,9 @@ def timed_issue(issue):
 
 def gpu():
     try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
+        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm',
+                            '--format=csv,noheader'], capture_output=True, text=True, timeout=30)
+        q = q.stdout.strip().splitlines()
         return q[torch.cuda.current_device()] if q else None
     except Exception:
         return None
@@ -140,7 +149,8 @@ def gpu():
 
 nbytes = 2 * D * 4 * B
 out = {'gpu': gpu(), 'B': B, 'D': D, 'program': {'instructions': prog.n_instr, 'registers': prog.n_regs},
-       'algorithmic_bytes_per_launch': nbytes}
+       'algorithmic_bytes_per_launch': nbytes, 'compile_ms': round(compile_ms, 1)}
+DATASHEET_GBPS = 3350.0
 for name, launch, chained in (('fused_cold', fused, False), ('fused_in_situ', fused, True), ('seed_cold', seed, False)):
     us = timed(launch, chained)
     out[name] = {'us': round(us, 2), 'GBps': round(nbytes / (us * 1e-6) / 1e9, 1)}
@@ -150,5 +160,7 @@ for k in (1, 8, 32, 64, 128):
         continue
     for mode, chained in (('in_situ', True), ('cold', False)):
         us = timed_chunk(k, chained)
-        out[f'chunk_{k}_{mode}'] = {'us_per_step': round(us / k, 2), 'write_GBps': round(k * B * D * 4 / (us * 1e-6) / 1e9, 1)}
+        gbps = k * B * D * 4 / (us * 1e-6) / 1e9
+        out[f'chunk_{k}_{mode}'] = {'us_per_step': round(us / k, 2), 'write_GBps': round(gbps, 1),
+                                    'of_datasheet': round(gbps / DATASHEET_GBPS, 3)}
 print(json.dumps(out), flush=True)

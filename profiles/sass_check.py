@@ -2,9 +2,12 @@
 counts of the instructions that carry the design — 128-bit global loads/stores, evict-first loads, bulk copies
 (UBLKCP) and mbarrier ops (SYNCS) of the TMA-staged tile kernel, SFU ops of the in-register Box-Muller, and the
 absence of FFMA in the tableau kernels that follow the reference's separately rounded op order (-fmad=false).  In the
-chunked pointwise kernels it checks the element-wise program's interpreter loops (the innermost loops that load and
-store the shared-memory register file): the loop that runs programs whose operands all sit in shared memory reads no
-global memory (LDG) and decodes no byte fields from the parameter space (LDC.U8); exit status 1 otherwise.
+chunked Euler / reversible-Heun kernels it checks the element-wise program's interpreter loops (the innermost loops that
+load and store the shared-memory register file): the loop that runs programs whose operands all sit in shared memory
+reads no global memory (LDG) and decodes no byte fields from the parameter space (LDC.U8).  Milstein programs are not
+interpreted but compiled at run time (NVRTC): it writes cfg2's program out (tsde_pointwise_source), compiles it as the
+library does and checks that the compiled kernel's step loop touches no shared memory (LDS / STS), no local memory
+(LDL / STL, spills) and reads no instruction word from the parameter space (an indexed LDC); exit status 1 otherwise.
 
     python profiles/sass_check.py > out/sass_evidence.txt
 """
@@ -17,12 +20,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, 'torchsde_b200', 'lib', 'libtorchsde_b200.so')
 PICK = [  # (label, regex on the demangled kernel name)
     ('Milstein tableau, fp32, counter noise (headline)', r'ew_fast_kernel<float, tsde::MilsteinOp<float>, 1>'),
-    ('fused Milstein steps of an element-wise SDE, up to 64 per launch (interpreter), fp32, counter noise',
-     r'pw_milstein_kernel<float, 1>'),
-    ('fused Milstein steps of an element-wise SDE, up to 64 per launch (interpreter), fp64, counter noise',
-     r'pw_milstein_kernel<double, 1>'),
-    ('fused Milstein step of an element-wise SDE spanning several cells, fp32', r'pw_milstein_kernel<float, 3>'),
-    ('fused Milstein step of an element-wise SDE spanning several cells, fp64', r'pw_milstein_kernel<double, 3>'),
     ('fused SRK step of an element-wise SDE (interpreter), fp32, counter noise', r'pw_srk_kernel<float, 1>'),
     ('fused SRK step of an element-wise SDE (interpreter), fp64, counter noise', r'pw_srk_kernel<double, 1>'),
     ('fused Heun step of an element-wise SDE (interpreter), fp32, counter noise', r'pw_pc_kernel<float, 1, 0>'),
@@ -50,8 +47,7 @@ PICK = [  # (label, regex on the demangled kernel name)
     ('bmm(g, A) of the log-ODE correction, fp32, m = 16', r'bmm_ga_kernel<float, 16>'),
     ('logqp KL-integrand augmentation, fp32', r'logqp_augment_kernel<float>'),
 ]
-INTERPRETED = [r'pw_milstein_kernel<float, 1>', r'pw_milstein_kernel<double, 1>', r'pw_chunk_kernel<float, 1, 0>',
-               r'pw_chunk_kernel<double, 1, 0>', r'pw_chunk_kernel<float, 1, 1>', r'pw_chunk_kernel<double, 1, 1>']
+INTERPRETED = [r'pw_chunk_kernel<float, 1, 0>', r'pw_chunk_kernel<double, 1, 0>', r'pw_chunk_kernel<float, 1, 1>', r'pw_chunk_kernel<double, 1, 1>']
 COUNT = ['LDG.E.128', 'LDG.E.EF.128', 'STG.E.128', 'LDS.128', 'UBLKCP', 'SYNCS', 'MUFU', 'FFMA', 'FMUL', 'FADD', 'DFMA',
          'SHFL', 'BAR.SYNC', 'LDL', 'STL', 'IMAD.WIDE']
 
@@ -72,6 +68,54 @@ def interpreter_loops(sass):
     inner = [(a, b) for a, b in back if not any(a <= c < d <= b and (c, d) != (a, b) for c, d in back)]
     loops = [[op for addr, op in ins if a <= addr <= b] for a, b in inner]
     return [body for body in loops if any('LDS.128' in o for o in body) and any('STS.128' in o for o in body)]
+
+
+def compiled_milstein():
+    """cfg2's Milstein program as the library compiles it: its step loop, registers and spills; False if it fails."""
+    import tempfile
+    sys.path.insert(0, ROOT)
+    import torch
+    from tests import test_host_pointwise as milstein
+    from tests.test_host_pointwise_compile import OPTIONS, HEADERS, STDINT, _tape
+    from torchsde_b200 import _cabi
+    import ctypes
+    src = _cabi.pointwise_source(_tape(milstein.ACCEPTED, 'gbm_ito', torch.float32), torch.float32)
+    nv = ctypes.CDLL('libnvrtc.so.12')
+    arr = lambda xs: (ctypes.c_char_p * len(xs))(*[x.encode() for x in xs])  # noqa: E731
+    prog = ctypes.c_void_p()
+    names = list(HEADERS) + ['stdint.h']
+    nv.nvrtcCreateProgram(ctypes.byref(prog), src.encode(), b'cfg2.cu', len(names),
+                          arr([open(p).read() for p in HEADERS.values()] + [STDINT]), arr(names))
+    assert nv.nvrtcCompileProgram(prog, len(OPTIONS), arr(OPTIONS)) == 0
+    n = ctypes.c_size_t()
+    nv.nvrtcGetCUBINSize(prog, ctypes.byref(n))
+    cubin = ctypes.create_string_buffer(n.value)
+    nv.nvrtcGetCUBIN(prog, cubin)
+    with tempfile.NamedTemporaryFile(suffix='.cubin') as f:
+        f.write(cubin.raw)
+        f.flush()
+        res = subprocess.run(['cuobjdump', '-res-usage', f.name], capture_output=True, text=True).stdout
+        sass = subprocess.run(['cuobjdump', '-sass', '-fun', 'tsde_pw_milstein_single', f.name], capture_output=True,
+                              text=True).stdout
+    m = re.search(r'Function tsde_pw_milstein_single:\n\s*REG:(\d+) STACK:(\d+) SHARED:(\d+) LOCAL:(\d+)', res)
+    reg, stack, shared, local = (int(m.group(i)) for i in range(1, 5))
+    ins = []
+    for ln in sass.splitlines():
+        mm = re.match(r'\s+/\*([0-9a-f]{4,})\*/\s+(.*?);', ln)
+        if mm:
+            ins.append((int(mm.group(1), 16), mm.group(2)))
+    back = [(int(re.search(r'0x([0-9a-f]+)', op.split('BRA')[1]).group(1), 16), addr) for addr, op in ins
+            if re.search(r'\bBRA\b', op) and re.search(r'0x([0-9a-f]+)', op.split('BRA')[1])
+            and int(re.search(r'0x([0-9a-f]+)', op.split('BRA')[1]).group(1), 16) < addr]
+    a, b = max(back, key=lambda x: x[1] - x[0])  # the step loop: the outermost backward branch
+    loop = [op for addr, op in ins if a <= addr <= b]
+    bad = [o for o in loop if re.search(r'\bLDS|\bSTS|\bLDL|\bSTL|LDC[.\w]*\s+\S+,\s*c\[0x0\]\[R', o)]
+    cnt = {k: sum(1 for o in loop if re.search(r'\b' + re.escape(k) + r'\b', o)) for k in COUNT}
+    print(f"## cfg2's Milstein program, compiled at run time (NVRTC), fp32, one cell per step\n"
+          f"   REG {reg}  STACK {stack}  SHARED {shared}  LOCAL {local}  step loop: {len(loop)} instructions\n   " +
+          '  '.join(f"{k}={v}" for k, v in cnt.items() if v) +
+          f"\n   shared / local memory or indexed parameter reads in the step loop: {len(bad)}\n")
+    return not bad and not stack and not local
 
 
 def main():
@@ -108,7 +152,7 @@ def main():
         print(f"## {label}\n   {d.split('(')[0]}\n   instructions {len(ops)}  REG {reg}  STACK {stack}  SHARED(static) {shared}  LOCAL {local}")
         cnt = {k: sum(1 for o in ops if re.search(r'\b' + re.escape(k) + r'\b', o)) for k in COUNT}
         print('   ' + '  '.join(f"{k}={v}" for k, v in cnt.items() if v) + '\n')
-    bad = 0
+    bad = 0 if compiled_milstein() else 1
     for pat in INTERPRETED:
         hit = [n for n, d in zip(names, dem) if re.search(pat, d)]
         sass = subprocess.run(['cuobjdump', '-sass', '-fun', hit[0], LIB], capture_output=True, text=True).stdout

@@ -20,6 +20,7 @@ F32, F64 = 0, 1
 NOISE_DIAGONAL, NOISE_GENERAL = 0, 1
 SRC_MEMORY, SRC_COUNTER, SRC_UNIT = 0, 1, 2
 EINVAL = -22
+ECOMPILE = -38  # TSDE_ECOMPILE: an element-wise program could not be compiled (NVRTC missing, or its log)
 FLAG_G_BROADCAST = 1
 LOGQP_GENERAL_MAX = 16384  # TSDE_LOGQP_GENERAL_MAX
 
@@ -28,6 +29,29 @@ def logqp_general_fits(d, m):
     """Whether tsde_logqp_augment takes a general-noise (d, m) row: its min(d,m) x max(d,m) matrix plus f - h within
     LOGQP_GENERAL_MAX elements of shared memory."""
     return min(d, m) * max(d, m) + d <= LOGQP_GENERAL_MAX
+
+
+def _program_launch(dtype):
+    # (a one-row diagonal launch: what tsde_pointwise_source / _compile read of it is the dtype)
+    return Launch(dtype_code(dtype), NOISE_DIAGONAL, 1, 4, 4, None)
+
+
+def pointwise_source(prog, dtype):
+    """The CUDA source the library compiles for Milstein program `prog` (a Pointwise) in `dtype`, or None if the library
+    refuses the program (tsde_pointwise_source; no device needed)."""
+    L = _program_launch(dtype)
+    n = lib().tsde_pointwise_source(ctypes.byref(L), ctypes.byref(prog), None, 0)
+    if n < 0:
+        return None
+    buf = ctypes.create_string_buffer(n + 1)
+    lib().tsde_pointwise_source(ctypes.byref(L), ctypes.byref(prog), buf, n + 1)
+    return buf.value.decode()
+
+
+def compile_pointwise(prog, dtype):
+    """tsde_pointwise_compile: compile and load the kernels of Milstein program `prog` in `dtype`; 0 or an error
+    code."""
+    return lib().tsde_pointwise_compile(ctypes.byref(_program_launch(dtype)), ctypes.byref(prog))
 
 
 class LibraryNotBuilt(RuntimeError):
@@ -104,6 +128,8 @@ SIGNATURES = {
     'tsde_step_milstein': [_L, _N, _P, _P, _P, _P, _D, _P],
     'tsde_step_milstein_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _D, _I, _P],
     'tsde_solve_milstein_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, ctypes.POINTER(PwStep), _I, _I],
+    'tsde_pointwise_compile': [_L, ctypes.POINTER(Pointwise)],
+    'tsde_pointwise_source': [_L, ctypes.POINTER(Pointwise), ctypes.c_char_p, ctypes.c_int64],
     'tsde_step_srk_diag_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _P, _P, _P, _D, _D, _D, _D, _P],
     'tsde_step_predictor_corrector_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _P, _I, _D, _D, _P],
     'tsde_solve_euler_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, ctypes.POINTER(PwStep), _I],
@@ -132,6 +158,24 @@ SIGNATURES = {
 _lib = None
 
 
+def _preload_nvrtc():
+    """Load NVRTC from the nvidia-cuda-nvrtc package PyTorch installs, if there is one, so that the library's
+    dlopen("libnvrtc.so.12") finds it when the Milstein programs are compiled (tsde_pointwise_compile).  Without it the
+    library still loads, and those solves keep the unfused step."""
+    try:
+        import nvidia.cuda_nvrtc as pkg
+    except ImportError:
+        return
+    for d in getattr(pkg, '__path__', ()):
+        path = os.path.join(d, 'lib', 'libnvrtc.so.12')
+        if os.path.exists(path):
+            try:
+                ctypes.CDLL(path, mode=ctypes.RTLD_GLOBAL)
+            except OSError:
+                continue
+            return
+
+
 def lib():
     """Load the shared library (once) and attach prototypes."""
     global _lib
@@ -142,6 +186,7 @@ def lib():
             f"torchsde_b200: CUDA library not found at {LIB_PATH}. Build it with "
             f"`python -c 'import __graft_entry__ as g; g.build()'` from the repository root. "
             f"There is no CPU or PyTorch fallback.")
+    _preload_nvrtc()
     handle = ctypes.CDLL(LIB_PATH)
     handle.tsde_abi_version.restype = ctypes.c_int
     handle.tsde_error_string.restype = ctypes.c_char_p
@@ -152,6 +197,7 @@ def lib():
         fn = getattr(handle, name)  # AttributeError here = header/library mismatch: fail loudly
         fn.restype = ctypes.c_int
         fn.argtypes = argtypes
+    handle.tsde_pointwise_source.restype = ctypes.c_int64
     if handle.tsde_abi_version() != 1:
         raise LibraryNotBuilt("torchsde_b200: ABI version mismatch, rebuild the library.")
     _lib = handle

@@ -208,7 +208,8 @@ class BaseMilstein(_ProdMixin, base_solver.BaseSDESolver):
         # f and the chain g -> seed -> vjp are independent given y0 (reference order: f first, milstein.py:68)
         f, (gd, gdg) = self._fork(lambda: _contig(user('f', lambda: sde.f(c.t0, y0))), diffusion_chain, main=1)
         if rec is not None:
-            self._pw = rec.finish(raw['f'], raw['g'], raw.get('gdg', (None,))[0]) or False
+            res = rec.finish(raw['f'], raw['g'], raw.get('gdg', (None,))[0])
+            self._pw = pointwise.compile_milstein(rec, res) or False
         return self._k('tsde_step_milstein', self._L, self._feed.get(c), (y0, f, gd, gdg), (c.dt,), out), ()
 
 

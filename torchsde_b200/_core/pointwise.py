@@ -50,6 +50,12 @@ derived symbolically: autograd's own op sequence (`grad * other`, the `add` that
 is what decides the bits, so it is what gets recorded.  The three segments are one program: the vjp part may read
 what the f / g part computed.  When the batch fills the GPU, up to TSDE_PW_MAX_STEPS consecutive steps run as one
 launch of tsde_solve_milstein_pointwise with the state in registers (`plan_chunks`, `chunk_length`, `solve_chunk`).
+The library does not interpret a Milstein program: it writes it out as CUDA with the program as straight-line register
+code and compiles it at run time (NVRTC, sm_90a, the IEEE options of its own build), one kernel per program structure
+and dtype, shared by every SDE of that structure whatever its parameter values.  The step compiles it right after
+`Recorder.finish` (`compile_milstein`, tsde_pointwise_compile), on the recording step: the warm-up and capture of a
+graph solve come later and never load a module.  If it cannot be compiled (no NVRTC, or a compiler error) the tape is
+rejected with the compiler's reason and the solve keeps the ordinary step.
 
 SRK (`SrkRecorder`, tsde_step_srk_diag_pointwise).  The step's seven evaluations, f at three (t, y) and g at four
 (methods.SRK._diagonal_or_scalar_step), are recorded one by one; a value of one evaluation is not an operand of
@@ -74,6 +80,7 @@ forward steps fuse too.
 """
 import ctypes
 import numbers
+import weakref
 
 import numpy as np
 import torch
@@ -513,6 +520,36 @@ class Recorder(TorchDispatchMode):
             return None
 
 
+# library -> the sources (tsde_pointwise_source) of the Milstein programs it compiled in this process
+_COMPILED = weakref.WeakKeyDictionary()
+COMPILES = 0  # how many of them were compiled: SDEs of one structure share the first one's kernels
+
+
+def compile_milstein(rec, res):
+    """`res`, what `rec.finish` returned, once its program's kernels are compiled and loaded (tsde_pointwise_compile);
+    None if `res` is, or if the library cannot compile the program (the tape is then rejected with the compiler's
+    reason).  Called on the recording step, so a graph solve's warm-up and capture never compile or load a module.
+    A program whose source (its structure: values and addresses are launch parameters) was compiled before is not
+    compiled again."""
+    global COMPILES
+    if res is None:
+        return None
+    prog = res[0]
+    src = _cabi.pointwise_source(prog, rec.dtype)
+    if src is None:
+        rec.reject("the library refuses the program")
+        return None
+    done = _COMPILED.setdefault(_cabi.lib(), set())
+    if src not in done:
+        err = _cabi.compile_pointwise(prog, rec.dtype)
+        if err != 0:
+            rec.reject(_cabi.lib().tsde_error_string(err).decode())
+            return None
+        done.add(src)
+        COMPILES += 1
+    return res
+
+
 _COUNT = 'zero one two three four five six seven'.split()
 
 
@@ -636,8 +673,8 @@ def plan_chunks(first, n_steps, interpolated=(), multi_cell=(), max_steps=_cabi.
 
 
 # Resident CTAs (256 threads) per SM of each chunked kernel, (float32, float64), from its registers (-Xptxas -v,
-# sm_90a: 64 K registers per SM): Milstein at 58-59 and 88-92 registers; Euler at 54 and 88-96; reversible Heun at 72
-# and 110-120.
+# sm_90a: 64 K registers per SM): Milstein's compiled kernels are pinned there by their launch bounds (256, 4) and
+# (256, 2) (cfg2's program: 41 registers in fp32); Euler at 54 and 88-96; reversible Heun at 72 and 110-120.
 _RESIDENT_CTAS = {'milstein': (4, 2), 'euler': (4, 2), 'reversible_heun': (3, 2)}
 
 

@@ -24,6 +24,11 @@ TSDE_EXPORT int tsde_abi_version(void) { return TSDE_ABI_VERSION; }
 
 TSDE_EXPORT const char* tsde_error_string(int code) {
   if (code == TSDE_EINVAL) return "torchsde_b200: invalid argument (contract violation)";
+  if (code == TSDE_ECOMPILE) {
+    static thread_local std::string msg;
+    msg = pw_compile_error();
+    return msg.c_str();
+  }
   return cudaGetErrorString((cudaError_t)code);
 }
 

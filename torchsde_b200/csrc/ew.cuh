@@ -15,31 +15,11 @@
 #include <stdint.h>
 
 #include "host.cuh"
-#include "philox.cuh"
-#include "rowdiv.cuh"
+#include "pw_device.cuh"
 
 namespace tsde {
 
-constexpr int kThreads = 256;
 constexpr int kBlocksPerSM = 8;  // 2048 threads / SM
-
-template <typename T>
-struct NoiseP {
-  const T* w;         // MEMORY
-  const T* u;         // MEMORY
-  const void* key;    // COUNTER
-  uint64_t cell_id;
-  int64_t row_offset;
-  int32_t n_cells;
-  int32_t bcast;      // noise has a single channel shared by all d (scalar noise, squeezed g)
-  double h;           // uniform cell length
-  const double* cell_h;  // device, or nullptr
-  double h_total;     // tb - ta of the whole query (for U)
-  int64_t m;          // channels of the noise tensor
-  T sqrt_h;           // (T)sqrt(h), (T)sqrt(h/12), (T)h_total: host-rounded once (single-cell path)
-  T sqrt_h12;
-  T ht;
-};
 
 template <int NIN, int NOUT>
 struct EwP {
@@ -54,24 +34,6 @@ struct EwP {
   int32_t small;   // nquads < 2^31: 32-bit index arithmetic
   uint64_t qmagic; // rowdiv_magic(qpr) = ceil(2^64 / qpr): row = umulhi(Q, qmagic), exact for every 32-bit Q
 };
-
-// ---- vector load / store helpers ---------------------------------------------------------
-__device__ __forceinline__ void ld4(const float* p, float (&v)[4]) {
-  const float4 t = *reinterpret_cast<const float4*>(p);
-  v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
-}
-__device__ __forceinline__ void ld4(const double* p, double (&v)[4]) {
-  const double2 a = *reinterpret_cast<const double2*>(p);
-  const double2 b = *reinterpret_cast<const double2*>(p + 2);
-  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
-}
-__device__ __forceinline__ void st4(float* p, const float (&v)[4]) {
-  *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
-}
-__device__ __forceinline__ void st4(double* p, const double (&v)[4]) {
-  *reinterpret_cast<double2*>(p) = make_double2(v[0], v[1]);
-  *reinterpret_cast<double2*>(p + 2) = make_double2(v[2], v[3]);
-}
 
 // streaming variants (ld.global.cs: evict-first) for operands that are dead after this kernel
 __device__ __forceinline__ void ld4cs(const float* p, float (&v)[4]) {
@@ -189,131 +151,6 @@ inline bool aligned_for(const void* p, uint32_t f) {
   return (reinterpret_cast<uintptr_t>(p) & (f == TSDE_FMT_STATE ? 15u : 7u)) == 0;
 }
 
-template <typename T>
-__device__ __forceinline__ void load_quad(const T* p, int64_t base, bool vec, int nvalid,
-                                          T (&v)[4]) {
-  if (vec) {
-    ld4(p + base, v);
-  } else {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) v[j] = j < nvalid ? p[base + j] : T(0);
-  }
-}
-template <typename T>
-__device__ __forceinline__ void store_quad(T* p, int64_t base, bool vec, int nvalid,
-                                           const T (&v)[4]) {
-  if (vec) {
-    st4(p + base, v);
-  } else {
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      if (j < nvalid) p[base + j] = v[j];
-  }
-}
-
-// ---- Brownian increment of one quad --------------------------------------------------------
-// Counter mode: merge of n_cells primary cells, left to right, with the reference's
-// aggregation rule (brownian_interval.py:643-672):
-//     H <- ( len_i (H_i + W/2) + (start_i - ta)(H - W_i/2) ) / (end_i - ta) ;  W <- W + W_i
-// Lengths are host doubles rounded once to T (python-float * tensor semantics).
-constexpr int kSrcCounterMulti = 3;  // internal: COUNTER source merging several primary cells
-
-template <typename T, bool WANT_U, bool MULTI = true>
-__device__ __forceinline__ void counter_noise(const NoiseP<T>& nz, Key key, uint32_t row,
-                                              uint32_t q, T (&w)[4], T (&u)[4]) {
-  T hh[4];
-  if (!MULTI || nz.n_cells == 1) {
-    // the solver's own grid: one primary cell per step, scales rounded once on the host
-    T n[4];
-    normal4(key, nz.cell_id, STREAM_W, row, q, n);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) w[j] = n[j] * nz.sqrt_h;
-    if (WANT_U) {
-      normal4(key, nz.cell_id, STREAM_H, row, q, n);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        hh[j] = n[j] * nz.sqrt_h12;
-        u[j] = nz.ht * (T(0.5) * w[j] + hh[j]);  // _H_to_U :102-103
-      }
-    }
-    return;
-  }
-  if (!MULTI) return;  // (unreachable; lets the compiler drop the merge loop from single-cell kernels)
-  double len0 = nz.cell_h ? nz.cell_h[0] : nz.h;
-  {
-    T n[4];
-    normal4(key, nz.cell_id, STREAM_W, row, q, n);
-    const T s = (T)sqrt(len0);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) w[j] = n[j] * s;
-    if (WANT_U) {
-      normal4(key, nz.cell_id, STREAM_H, row, q, n);
-      const T s12 = (T)sqrt(len0 / 12.0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) hh[j] = n[j] * s12;
-    }
-  }
-  double elapsed = len0;  // start_i - ta
-  for (int c = 1; c < nz.n_cells; ++c) {
-    const double len = nz.cell_h ? nz.cell_h[c] : nz.h;
-    T n[4], wi[4];
-    normal4(key, nz.cell_id + (uint64_t)c, STREAM_W, row, q, n);
-    const T s = (T)sqrt(len);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) wi[j] = n[j] * s;
-    if (WANT_U) {
-      normal4(key, nz.cell_id + (uint64_t)c, STREAM_H, row, q, n);
-      const T s12 = (T)sqrt(len / 12.0);
-      const T tl = (T)len, te = (T)elapsed, tt = (T)(elapsed + len);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const T hi = n[j] * s12;
-        const T term1 = tl * (hi + T(0.5) * w[j]);
-        const T term2 = te * (hh[j] - T(0.5) * wi[j]);
-        hh[j] = (term1 + term2) / tt;
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j) w[j] = w[j] + wi[j];
-    elapsed += len;
-  }
-  if (WANT_U) {
-    const T ht = (T)nz.h_total;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) u[j] = ht * (T(0.5) * w[j] + hh[j]);  // _H_to_U :102-103
-  }
-}
-
-template <typename T, int SRC, bool WANT_U>
-__device__ __forceinline__ void quad_noise(const NoiseP<T>& nz, Key key, int64_t row, int64_t q,
-                                           bool vec, int nvalid, T (&w)[4], T (&u)[4]) {
-  if (SRC == TSDE_SRC_UNIT) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) { w[j] = T(1); u[j] = T(0); }
-  } else if (SRC == TSDE_SRC_MEMORY) {
-    if (nz.bcast) {
-      const T a = nz.w[row];
-      const T b = WANT_U ? nz.u[row] : T(0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) { w[j] = a; u[j] = b; }
-    } else {
-      const int64_t base = row * nz.m + 4 * q;
-      load_quad(nz.w, base, vec, nvalid, w);
-      if (WANT_U) load_quad(nz.u, base, vec, nvalid, u);
-    }
-  } else {
-    constexpr bool MULTI = SRC == kSrcCounterMulti;
-    const uint32_t grow = (uint32_t)(row + nz.row_offset);
-    if (nz.bcast) {
-      T w4[4], u4[4];
-      counter_noise<T, WANT_U, MULTI>(nz, key, grow, 0u, w4, u4);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) { w[j] = w4[0]; u[j] = WANT_U ? u4[0] : T(0); }
-    } else {
-      counter_noise<T, WANT_U, MULTI>(nz, key, grow, (uint32_t)q, w, u);
-    }
-  }
-}
 
 // ---- the kernel -----------------------------------------------------------------------------
 // Op: struct with  static constexpr int NIN, NOUT; static constexpr bool USES_NOISE, WANT_U;

@@ -7,6 +7,7 @@
 #include <atomic>
 #include <map>
 #include <mutex>
+#include <string>
 #include <utility>
 
 #include "../../include/torchsde_b200.h"
@@ -143,6 +144,26 @@ inline int launch_kernel(void (*kernel)(P...), int64_t grid, int block, size_t s
   if (e != cudaSuccess) cudaGetLastError();
   return (int)e;
 }
+
+// launch_kernel for a kernel handle of a library loaded at run time (cudaLibraryGetKernel): `args` points at each of its
+// parameters.  No dynamic shared memory.
+inline int launch_kernel_handle(cudaKernel_t kernel, int64_t grid, int block, cudaStream_t st, void** args) {
+  cudaLaunchAttribute attr{};
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3(block);
+  cfg.stream = st;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  const cudaError_t e = cudaLaunchKernelExC(&cfg, reinterpret_cast<const void*>(kernel), args);
+  if (e != cudaSuccess) cudaGetLastError();
+  return (int)e;
+}
+
+// Why the last run-time compilation of an element-wise program failed (pointwise.cu; tsde_error_string(TSDE_ECOMPILE))
+std::string pw_compile_error();
 
 // ---- which inputs of an entry point are SDE outputs (dispatch_fmt): bit i = input i of its declaration -------------
 namespace sde_out {

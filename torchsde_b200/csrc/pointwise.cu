@@ -4,34 +4,36 @@
 // (up to TSDE_PW_MAX_STEPS Euler or reversible-Heun steps in one kernel) (include/torchsde_b200.h describes the
 // tsde_pointwise program and its two layouts).
 //
-// The SDE's f and g (and for Milstein the vjp of g) arrive as a small program of element-wise instructions.  Each
-// kernel interprets it between the unfused step's own ops (tableau_diag_ops.cuh), one IEEE rounding per element
-// (this translation unit is compiled with -fmad=false, as the tableaus are), so a fused step equals the unfused one
-// bit for bit.  The file holds, in this order: the decoded program, its register file and interpreter, the validation
-// every program passes before a launch and the decoding that follows it, the prologue the kernels share, the kernels
-// with the layout each accepts, and the launch.
+// The SDE's f and g (and for Milstein the vjp of g) arrive as a small program of element-wise instructions.  The SRK,
+// predictor-corrector and Euler / reversible-Heun kernels interpret it between the unfused step's own ops
+// (tableau_diag_ops.cuh), one IEEE rounding per element (this translation unit is compiled with -fmad=false, as the
+// tableaus are), so a fused step equals the unfused one bit for bit.  A Milstein program is compiled instead, at run
+// time, into a kernel of its own with the same roundings (pw_milstein_source, NVRTC).  The file holds, in this order:
+// the decoded program, its register file and interpreter, the validation every program passes before a launch and the
+// decoding that follows it, the prologue the kernels share, the Milstein code generator and its kernel cache, the
+// interpreting kernels with the layout each accepts, and the launches.
 //
 // One thread per quad, as ew_fast_kernel.  The program's registers live in shared memory as 16-byte vectors laid
 // out [reg][plane][thread] (a float quad is one plane, a double quad two): a warp's 128-bit access is 512 contiguous
 // bytes, conflict-free.  A dynamically indexed per-thread array would live in local memory instead.  The state, go,
 // the SDE's results and the increments stay in registers; the program reads y and go from their own slots.
+#include <dlfcn.h>
+#include <nvrtc.h>
+#include <stdio.h>
+#include <string.h>
+
+#include <string>
+#include <type_traits>
+
 #include "tableau_diag_ops.cuh"
 
 namespace tsde {
 
-template <typename T>
-struct PwP {
-  const T* y0;
-  T* y1;
-  const T* t0;
-  int64_t d, qpr, nquads;
-  uint64_t qmagic;  // rowdiv_magic(qpr) when qpr is not a power of two
-  int32_t qshift;   // log2(qpr), or -1
-  int32_t small;    // nquads < 2^31
-  int32_t vec;      // d % 4 == 0 and every tensor 16-byte aligned
-  T dt;
-  int32_t ito;
-};
+// pw_device.cuh and the headers it includes, as NVRTC is given them: their names as pw_device.cuh includes them, and
+// their text (embedded by build() into a generated source of the library)
+constexpr int kPwHeaderCount = 4;  // pw_device.cuh, philox.cuh, rowdiv.cuh, include/torchsde_b200.h
+extern const char* const kPwHeaderNames[kPwHeaderCount];
+extern const char* const kPwHeaderSources[kPwHeaderCount];
 
 // ---- the decoded program --------------------------------------------------------------------------------------------
 // pw_prepare decodes the caller's tsde_pointwise once per launch into a PwProg, in which every source is a slot of the
@@ -65,15 +67,9 @@ static_assert(kPwMaxSlots * kThreads * 4 * sizeof(double) <= 227 * 1024,
 static_assert(kPwMaxSlots <= 32 && TSDE_PW_MAX_OPERANDS <= 31, "slots, operand indices and lanes fit five bits");
 
 template <typename T>
-struct PwOperand {
-  const T* ptr;  // SCALAR, CHANNEL, ROW; null for IMM
-  T imm;
-};
-
-template <typename T>
 struct PwProg {
   int32_t n_fg, n_instr;
-  uint16_t f_src, g_src, gdg_src;
+  uint16_t f_src, g_src, gdg_src;    // (gdg_src, go: the Milstein layout's, which runs compiled instead: y and -1)
   int8_t y, go, t0, u, hoist, end;  // slots (t0: -1 when no operand reads the time)
   int8_t n_uniform, n_hoisted;      // operand[0, n_uniform) fill the u slot, the next n_hoisted the hoisted slots
   int8_t n_global;                  // the operands past those, read from global memory at every use
@@ -106,12 +102,6 @@ template <typename T>
 __device__ __forceinline__ void pw_sstore(void* s, int r, const T (&v)[4]) {
   pw_sstore(s, r, threadIdx.x, v);
 }
-
-struct PwQuad {  // where this thread's quad lives
-  int64_t base, chan;
-  int nvalid;
-  bool vec;
-};
 
 // GLOBAL: the source may be a CHANNEL / ROW operand that did not fit the slots, read from global memory; EXT: the
 // source is in the encoding of a program with comparison and selection ops
@@ -296,10 +286,10 @@ static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, bool allow_
 }
 
 // ---- decoding -------------------------------------------------------------------------------------------------------
-// The PwProg of a program that passed validation: with a go slot for the Milstein layout (`go`), and `extra` slots past
-// the layout (SRK's fp64 stash) counted against kPwHoistSlots.  Returns the slots a launch takes, extra included.
+// The PwProg of a two-program layout that passed validation, with `extra` slots past the layout (SRK's fp64 stash)
+// counted against kPwHoistSlots.  Returns the slots a launch takes, extra included.
 template <typename T>
-static int pw_decode(const tsde_pointwise& in, bool go, int extra, PwProg<T>& pg) {
+static int pw_decode(const tsde_pointwise& in, int extra, PwProg<T>& pg) {
   pg = PwProg<T>{};
   for (int i = 0; i < in.n_instr; ++i) pg.ext = pg.ext || in.instr[i].op > TSDE_PW_SQRT;
   pg.n_fg = in.n_fg;
@@ -314,7 +304,7 @@ static int pw_decode(const tsde_pointwise& in, bool go, int extra, PwProg<T>& pg
   }
   int slot = in.n_regs;
   pg.y = slot++;
-  pg.go = go ? slot++ : -1;
+  pg.go = -1;
   pg.t0 = t0 ? slot++ : -1;
   pg.u = n_uniform ? slot++ : -1;
   pg.hoist = slot;
@@ -345,7 +335,6 @@ static int pw_decode(const tsde_pointwise& in, bool go, int extra, PwProg<T>& pg
   }
   auto source = [&](uint32_t s) -> uint32_t {
     if (s == TSDE_PW_SRC_Y) return pg.y;
-    if (s == TSDE_PW_SRC_GO) return pg.go;
     return s >= (uint32_t)TSDE_PW_OPERAND(0) ? src[s - TSDE_PW_OPERAND(0)] : s;
   };
   for (int i = 0; i < in.n_instr; ++i) {
@@ -355,35 +344,11 @@ static int pw_decode(const tsde_pointwise& in, bool go, int extra, PwProg<T>& pg
   }
   pg.f_src = source(in.f_src);
   pg.g_src = source(in.g_src);
-  pg.gdg_src = go ? source(in.gdg_src) : pg.y;  // (the two-program layouts have no gdg)
+  pg.gdg_src = pg.y;  // (the two-program layouts have no gdg)
   return slot + extra;
 }
 
 // ---- what every kernel starts with ----------------------------------------------------------------------------------
-// pw_begin's quad mapping on its own, for a kernel that draws again later: the flat index Q (past the last quad when
-// Q >= p.nquads), the row and quad of the row, and `c`.  (pw_begin keeps its own copy: calling this from it
-// reschedules the SRK and predictor-corrector kernels.)
-template <typename T>
-__device__ __forceinline__ void pw_locate(const PwP<T>& p, PwQuad& c, int64_t& Q, int64_t& row, int64_t& q) {
-  Q = (int64_t)blockIdx.x * kThreads + threadIdx.x;
-  if (p.qshift >= 0) {
-    row = Q >> p.qshift;
-    q = Q & ((1ll << p.qshift) - 1);
-  } else if (p.small) {
-    const uint32_t r32 = rowdiv_row((uint32_t)Q, p.qmagic);
-    row = r32;
-    q = (int64_t)rowdiv_quad((uint32_t)Q, r32, (uint32_t)p.qpr);
-  } else {
-    row = Q / p.qpr;
-    q = Q - row * p.qpr;
-  }
-  c.chan = 4 * q;
-  c.base = row * p.d + c.chan;
-  const int64_t rem = p.d - c.chan;
-  c.nvalid = rem < 4 ? (int)rem : 4;
-  c.vec = p.vec != 0;
-}
-
 // This thread's quad `c`, its increments and its y0, and the program's operands in their slots.  The increments
 // depend on no predecessor: they are drawn while the previous kernel drains (programmatic dependent launch); y0 and
 // the operands are read after the dependency wait.  False for a thread past the last quad.
@@ -417,90 +382,275 @@ __device__ __forceinline__ bool pw_begin(const PwProg<T>& pg, const PwP<T>& p, c
   return true;
 }
 
-// ---- consecutive Milstein steps (tsde_solve_milstein_pointwise, tsde_step_milstein_pointwise) -----------------------
-// Per step: the program's f / g part runs on y, MilsteinSeedOp forms go, the vjp part runs and MilsteinOp forms y1.
-// A quad's trajectory depends on nothing but its own state (element-wise SDE, diagonal noise), so one thread runs the
-// whole chunk of up to kPwMaxSteps steps: y0 is read once, y1 stays in registers from one step to the next and is
-// stored only where the step table gives it a destination (an output row, the chunk's last state).  The unfused
-// step moves 13 tensors; a chunk moves one read and the stores it is asked for.
-constexpr int kPwMaxSteps = TSDE_PW_MAX_STEPS;
+// ---- consecutive Milstein steps, compiled (tsde_solve_milstein_pointwise, tsde_step_milstein_pointwise) -----------
+// A Milstein program is not interpreted: once validated, it is written out as one CUDA translation unit
+// (pw_milstein_source) whose kernels run pw_milstein_steps (pw_device.cuh) with the program inlined as straight-line
+// register code, compiled at run time by NVRTC to an sm_90a cubin and loaded as a CUDA library.  Each instruction is
+// the expression of the matching `case` of pw_loop, one statement per lane, and the translation unit is compiled with
+// the library's IEEE options (-fmad=false, NVRTC's default -prec-div=true, -prec-sqrt=true, -ftz=false), so a compiled
+// step equals the unfused one bit for bit.  Operand values and addresses are not in the source: IMM values and
+// SCALAR / CHANNEL / ROW pointers are the kernel's PwOperands parameter, so the source is a function of the program's
+// structure alone (instruction words, n_regs, n_fg, result sources, operand kinds, dtype), and it is the key of the
+// process-wide cache of loaded kernels: SDEs that differ only in parameter values share one compiled kernel.
 
-template <typename T>
-struct PwStep {  // one step of a chunk, as tsde_pw_step with its scalars rounded to T on the host
-  uint64_t cell;   // Brownian cell (the kSrcCounterMulti kernel merges nz.n_cells cells from here)
-  const T* t0;     // what TSDE_PW_T0 reads during this step
-  T* y1;           // destination of this step's y1, or null
-  T sqrt_h, dt;    // (T)sqrt(h) of the cell, (T)dt
-};
-template <typename T>
-struct PwSteps {  // by value: a captured launch carries the whole table
-  int32_t n;
-  PwStep<T> s[kPwMaxSteps];
-};
-static_assert(sizeof(PwProg<double>) + sizeof(PwP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <= 4096,
-              "the Milstein kernel's parameters fit the 4 KiB parameter space");
+// CHANNEL / ROW operand quads a compiled program keeps in registers for the whole chunk (loaded once per launch after
+// the dependency wait); any past these are loaded again at every step.  Within the launch bounds below, cfg2's program
+// (two CHANNEL operands) takes 41 registers in fp32.
+constexpr int kPwJitHoistQuads[2] = {4, 2};  // float, double
 
-template <typename T, int SRC, bool EXT>
-__device__ __forceinline__ void pw_milstein(const PwProg<T>& pg, const PwP<T> p, const NoiseP<T> nz,
-                                           const PwSteps<T>& st) {
-  extern __shared__ __align__(16) unsigned char pw_regs[];
-  PwQuad c;
-  int64_t Q, row, q;
-  pw_locate(p, c, Q, row, q);
-  const Key key = load_key(nz.key);
-  T y[4];
-  for (int j = 0; j < st.n; ++j) {
-    const PwStep<T>& s = st.s[j];
-    T w[4], u[4];
-    NoiseP<T> z = nz;  // this step's cell
-    z.cell_id = s.cell;
-    z.sqrt_h = s.sqrt_h;
-    quad_noise<T, SRC, false>(z, key, row, q, c.vec, c.nvalid, w, u);
-    if (j == 0) {  // the first increment is drawn while the previous kernel drains; the rest is read after the wait
-      asm volatile("griddepcontrol.wait;" ::: "memory");
-      pw_load_uniform(pg, pw_regs);
-      if (Q >= p.nquads) return;
-      load_quad(p.y0, c.base, c.vec, c.nvalid, y);
-      pw_load_hoisted(pg, c, pw_regs);
+// The compiled kernels run at the resident CTAs per SM the interpreted Milstein kernel had (58-59 registers in fp32,
+// 88-92 in fp64): pointwise.py's _RESIDENT_CTAS and chunk_length count on it.
+constexpr int kPwJitCtas[2] = {4, 2};
+
+static_assert(sizeof(PwOperands<double>) + sizeof(PwP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <=
+                  4096,
+              "the compiled Milstein kernel's parameters fit the 4 KiB parameter space");
+
+static std::string num(int x) {
+  char b[16];
+  snprintf(b, sizeof(b), "%d", x);
+  return b;
+}
+
+// The translation unit of a program that passed pw_valid_tables and pw_valid_milstein, for dtype `f64`.
+static std::string pw_milstein_source(const tsde_pointwise& in, bool f64) {
+  const char* T = f64 ? "double" : "float";
+  bool hoisted[TSDE_PW_MAX_OPERANDS] = {};
+  for (int k = 0, n = 0; k < in.n_operands; ++k)
+    if (in.operand[k].kind >= TSDE_PW_CHANNEL) hoisted[k] = n++ < kPwJitHoistQuads[f64];
+  auto operand = [&](uint8_t s) { return s >= TSDE_PW_OPERAND(0) && s != TSDE_PW_SRC_Y && s != TSDE_PW_SRC_GO; };
+  // the value of source s in lane j
+  auto src = [&](uint8_t s) -> std::string {
+    if (s == TSDE_PW_SRC_Y) return "y[j]";
+    if (s == TSDE_PW_SRC_GO) return "go[j]";
+    if (!operand(s)) return "r" + num(s) + "[j]";
+    const int k = s - TSDE_PW_OPERAND(0);
+    const std::string n = num(k);
+    switch (in.operand[k].kind) {
+      case TSDE_PW_IMM: return "ops.k[" + n + "].imm";
+      case TSDE_PW_T0: return "t0";
+      case TSDE_PW_SCALAR: return "u" + n;
+      default: return (hoisted[k] ? "k" : "x") + n + "[j]";
     }
-    pw_set_state(pg, pw_regs, s.t0, y);
-    pw_run<EXT>(pg, c, pw_regs, 0, pg.n_fg);
-    T f[4], g[4], go[4];
-    pw_fetch<true, EXT>(pg, c, pw_regs, pg.f_src, f);
-    pw_fetch<true, EXT>(pg, c, pw_regs, pg.g_src, g);
-    const MilsteinSeedOp<T> seed{s.dt, p.ito};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      T o[1];
-      seed({g[i]}, w[i], u[i], o);
-      go[i] = o[0];
+  };
+  // instruction i, as pw_loop's case of its opcode
+  auto statement = [&](const tsde_pw_instr& x) -> std::string {
+    const std::string a = src(x.a), b = pw_unary(x.op) ? a : src(x.b), d = "r" + num(x.dst) + "[j]";
+    const std::string f = f64 ? "" : "f";
+    std::string e;
+    switch (x.op) {
+      case TSDE_PW_MUL: e = a + " * " + b; break;
+      case TSDE_PW_ADD: e = a + " + " + b; break;
+      case TSDE_PW_SUB: e = a + " - " + b; break;
+      case TSDE_PW_DIV: e = a + " / " + b; break;
+      case TSDE_PW_NEG: e = "-" + a; break;
+      case TSDE_PW_SQRT: e = "sqrt" + f + "(" + a + ")"; break;
+      case TSDE_PW_LT: e = a + " < " + b + " ? T(1) : T(0)"; break;
+      case TSDE_PW_LE: e = a + " <= " + b + " ? T(1) : T(0)"; break;
+      case TSDE_PW_EQ: e = a + " == " + b + " ? T(1) : T(0)"; break;
+      case TSDE_PW_MAXIMUM:  // maximum_kernel_cuda (::max is fmax)
+        e = a + " != " + a + " ? " + a + " : " + b + " != " + b + " ? " + b + " : fmax" + f + "(" + a + ", " + b + ")";
+        break;
+      case TSDE_PW_MINIMUM:  // minimum_kernel_cuda (::min is fmin)
+        e = a + " != " + a + " ? " + a + " : " + b + " != " + b + " ? " + b + " : fmin" + f + "(" + a + ", " + b + ")";
+        break;
+      case TSDE_PW_ABS: e = "fabs" + f + "(" + a + ")"; break;
+      default: e = d + " != T(0) ? " + a + " : " + b; break;  // TSDE_PW_SEL: the condition is the destination
     }
-    pw_sstore(pw_regs, pg.go, go);
-    pw_run<EXT>(pg, c, pw_regs, pg.n_fg, pg.n_instr);
-    T gdg[4];
-    pw_fetch<true, EXT>(pg, c, pw_regs, pg.gdg_src, gdg);
-    const MilsteinOp<T> step{s.dt};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      T o[1];
-      step({y[i], f[i], g[i], gdg[i]}, w[i], u[i], o);
-      y[i] = o[0];
+    return "      " + d + " = " + e + ";\n";
+  };
+  // instructions [i0, i1) and then `results` (name = source); the time and the operands not kept in registers that
+  // they read are loaded first
+  auto part = [&](int i0, int i1, std::initializer_list<std::pair<const char*, uint8_t>> results) {
+    uint8_t reads[2 * TSDE_PW_MAX_INSTR + 2];
+    int n = 0;
+    for (int i = i0; i < i1; ++i) {
+      reads[n++] = in.instr[i].a;
+      if (!pw_unary(in.instr[i].op)) reads[n++] = in.instr[i].b;
     }
-    if (s.y1) store_quad(s.y1, c.base, c.vec, c.nvalid, y);
+    for (const auto& r : results) reads[n++] = r.second;
+    std::string o;
+    bool t0 = false, x[TSDE_PW_MAX_OPERANDS] = {};
+    for (int i = 0; i < n; ++i) {
+      const uint8_t s = reads[i];
+      if (!operand(s)) continue;
+      const int k = s - TSDE_PW_OPERAND(0), kind = in.operand[k].kind;
+      if (kind == TSDE_PW_T0 && !t0) {
+        t0 = true;
+        o += "    const T t0 = *s.t0;\n";
+      } else if (kind >= TSDE_PW_CHANNEL && !hoisted[k] && !x[k]) {
+        x[k] = true;
+        const std::string n = num(k);
+        o += "    T x" + n + "[4];\n    load_quad(ops.k[" + n + "].ptr, c." + (kind == TSDE_PW_ROW ? "base" : "chan") +
+             ", c.vec, c.nvalid, x" + n + ");\n";
+      }
+    }
+    o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
+    for (int i = i0; i < i1; ++i) o += statement(in.instr[i]);
+    for (const auto& r : results) o += std::string("      ") + r.first + "[j] = " + src(r.second) + ";\n";
+    return o + "    }\n";
+  };
+  std::string o = "// A Milstein program of torchsde_b200, generated by pw_milstein_source\n"
+                  "#include \"pw_device.cuh\"\n\n";
+  o += "namespace tsde {\nnamespace {\ntypedef " + std::string(T) + " T;\n\nstruct Prog {\n";
+  for (int r = 0; r < in.n_regs; ++r) o += "  T r" + num(r) + "[4];\n";
+  for (int k = 0; k < in.n_operands; ++k) {
+    const std::string n = num(k);
+    if (in.operand[k].kind == TSDE_PW_SCALAR) o += "  T u" + n + ";\n";
+    if (hoisted[k]) o += "  T k" + n + "[4];\n";
   }
+  o += "  __device__ __forceinline__ void load(const PwOperands<T>& ops, const PwQuad& c) {\n";
+  for (int k = 0; k < in.n_operands; ++k) {
+    const std::string n = num(k);
+    if (in.operand[k].kind == TSDE_PW_SCALAR) o += "    u" + n + " = *ops.k[" + n + "].ptr;\n";
+    if (hoisted[k])
+      o += "    load_quad(ops.k[" + n + "].ptr, c." + (in.operand[k].kind == TSDE_PW_ROW ? "base" : "chan") +
+           ", c.vec, c.nvalid, k" + n + ");\n";
+  }
+  o += "  }\n  __device__ __forceinline__ void fg(const PwOperands<T>& ops, const PwQuad& c, const PwStep<T>& s,\n"
+       "                                     const T (&y)[4], T (&f)[4], T (&g)[4]) {\n";
+  o += part(0, in.n_fg, {{"f", in.f_src}, {"g", in.g_src}});
+  o += "  }\n  __device__ __forceinline__ void vjp(const PwOperands<T>& ops, const PwQuad& c, const PwStep<T>& s,\n"
+       "                                      const T (&y)[4], const T (&go)[4], T (&gdg)[4]) {\n";
+  o += part(in.n_fg, in.n_instr, {{"gdg", in.gdg_src}});
+  o += "  }\n};\n}  // namespace\n}  // namespace tsde\n";
+  const std::string bounds = "__launch_bounds__(" + num(kThreads) + ", " + num(kPwJitCtas[f64]) + ")";
+  for (const char* v : {"single", "multi"}) {
+    o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_milstein_" + v +
+         "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwP<tsde::T> p,\n"
+         "    const tsde::NoiseP<tsde::T> nz, const __grid_constant__ tsde::PwSteps<tsde::T> st) {\n"
+         "  tsde::pw_milstein_steps<tsde::T, " + (v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti") +
+         ", tsde::Prog>(ops, p, nz, st);\n}\n";
+  }
+  return o;
 }
 
-template <typename T, int SRC>
-__global__ void __launch_bounds__(kThreads)
-pw_milstein_kernel(const __grid_constant__ PwProg<T> pg, const PwP<T> p, const NoiseP<T> nz,
-                   const __grid_constant__ PwSteps<T> st) {
-  pw_milstein<T, SRC, false>(pg, p, nz, st);
+// ---- NVRTC --------------------------------------------------------------------------------------------------------
+// libnvrtc.so.12 is opened the first time a program is compiled, not linked: the library loads where NVRTC is missing
+// (and every other entry point works there).  torchsde_b200/_cabi.py preloads it from the nvidia-cuda-nvrtc package
+// that PyTorch installs.
+struct Nvrtc {
+  decltype(&nvrtcCreateProgram) create;
+  decltype(&nvrtcCompileProgram) compile;
+  decltype(&nvrtcGetProgramLogSize) log_size;
+  decltype(&nvrtcGetProgramLog) log;
+  decltype(&nvrtcGetCUBINSize) cubin_size;
+  decltype(&nvrtcGetCUBIN) cubin;
+  decltype(&nvrtcDestroyProgram) destroy;
+  decltype(&nvrtcGetErrorString) error;
+};
+
+static const Nvrtc* nvrtc() {
+  static const Nvrtc* api = []() -> const Nvrtc* {
+    void* h = dlopen("libnvrtc.so.12", RTLD_NOW | RTLD_GLOBAL);
+    if (!h) return nullptr;
+    static Nvrtc n;
+    bool ok = true;
+    auto sym = [&](auto& fn, const char* name) {
+      fn = reinterpret_cast<std::remove_reference_t<decltype(fn)>>(dlsym(h, name));
+      ok = ok && fn;
+    };
+    sym(n.create, "nvrtcCreateProgram");
+    sym(n.compile, "nvrtcCompileProgram");
+    sym(n.log_size, "nvrtcGetProgramLogSize");
+    sym(n.log, "nvrtcGetProgramLog");
+    sym(n.cubin_size, "nvrtcGetCUBINSize");
+    sym(n.cubin, "nvrtcGetCUBIN");
+    sym(n.destroy, "nvrtcDestroyProgram");
+    sym(n.error, "nvrtcGetErrorString");
+    return ok ? &n : nullptr;
+  }();
+  return api;
 }
-template <typename T, int SRC>
-__global__ void __launch_bounds__(kThreads)
-pw_milstein_ext_kernel(const __grid_constant__ PwProg<T> pg, const PwP<T> p, const NoiseP<T> nz,
-                       const __grid_constant__ PwSteps<T> st) {
-  pw_milstein<T, SRC, true>(pg, p, nz, st);
+
+// NVRTC has no <stdint.h>
+static const char kPwStdint[] =
+    "#pragma once\n"
+    "typedef signed char int8_t; typedef short int16_t; typedef int int32_t; typedef long long int64_t;\n"
+    "typedef unsigned char uint8_t; typedef unsigned short uint16_t; typedef unsigned int uint32_t;\n"
+    "typedef unsigned long long uint64_t; typedef unsigned long long uintptr_t;\n";
+
+static std::mutex g_pw_error_mu;
+static std::string g_pw_error;  // why the last compilation failed (tsde_error_string(TSDE_ECOMPILE))
+
+static int pw_compile_failed(const std::string& why) {
+  std::lock_guard<std::mutex> lock(g_pw_error_mu);
+  g_pw_error = "torchsde_b200: the element-wise Milstein program could not be compiled: " + why;
+  return TSDE_ECOMPILE;
+}
+
+std::string pw_compile_error() {
+  std::lock_guard<std::mutex> lock(g_pw_error_mu);
+  return g_pw_error;
+}
+
+// The sm_90a cubin of `source`, or TSDE_ECOMPILE with the compiler's log
+static int pw_nvrtc(const std::string& source, std::string& cubin) {
+  const Nvrtc* nv = nvrtc();
+  if (!nv) return pw_compile_failed("libnvrtc.so.12 (NVRTC) was not found");
+  const char* names[kPwHeaderCount + 1];
+  const char* bodies[kPwHeaderCount + 1];
+  for (int i = 0; i < kPwHeaderCount; ++i) {
+    names[i] = kPwHeaderNames[i];
+    bodies[i] = kPwHeaderSources[i];
+  }
+  names[kPwHeaderCount] = "stdint.h";
+  bodies[kPwHeaderCount] = kPwStdint;
+  nvrtcProgram prog;
+  nvrtcResult r = nv->create(&prog, source.c_str(), "tsde_pw_milstein.cu", kPwHeaderCount + 1, bodies, names);
+  if (r != NVRTC_SUCCESS) return pw_compile_failed(nv->error(r));
+  // straight to SASS (no PTX for the driver to JIT); the public header's declarations are host functions, which NVRTC
+  // refuses unless unannotated functions are taken as device ones
+  const char* opts[] = {"-arch=sm_90a", "-std=c++17", "-fmad=false", "-prec-div=true", "-prec-sqrt=true",
+                        "-ftz=false", "-default-device"};
+  r = nv->compile(prog, (int)(sizeof(opts) / sizeof(opts[0])), opts);
+  std::string log;
+  size_t n = 0;
+  if (nv->log_size(prog, &n) == NVRTC_SUCCESS && n > 1) {
+    log.resize(n);
+    nv->log(prog, &log[0]);
+    log.resize(n - 1);
+  }
+  if (r == NVRTC_SUCCESS && nv->cubin_size(prog, &n) == NVRTC_SUCCESS) {
+    cubin.resize(n);
+    r = nv->cubin(prog, &cubin[0]);
+  }
+  nv->destroy(&prog);
+  if (r != NVRTC_SUCCESS) return pw_compile_failed(std::string(nv->error(r)) + "\n" + log);
+  return 0;
+}
+
+struct PwCompiled {
+  cudaKernel_t kernel[2];  // one Brownian cell per step, several cells merged (kSrcCounterMulti)
+};
+
+// The loaded kernels of a program that passed validation, compiled on first use.  Libraries are context-independent:
+// one entry serves every device.
+static int pw_compiled(const tsde_pointwise& prog, bool f64, PwCompiled& out) {
+  static std::mutex mu;
+  static std::map<std::string, PwCompiled> cache;
+  std::string source = pw_milstein_source(prog, f64);
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = cache.find(source);
+  if (it != cache.end()) {
+    out = it->second;
+    return 0;
+  }
+  std::string cubin;
+  if (int e = pw_nvrtc(source, cubin)) return e;
+  cudaLibrary_t lib;
+  cudaError_t e = cudaLibraryLoadData(&lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0);
+  if (e == cudaSuccess) {
+    e = cudaLibraryGetKernel(&out.kernel[0], lib, "tsde_pw_milstein_single");
+    if (e == cudaSuccess) e = cudaLibraryGetKernel(&out.kernel[1], lib, "tsde_pw_milstein_multi");
+    if (e != cudaSuccess) cudaLibraryUnload(lib);
+  }
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return (int)e;
+  }
+  cache.emplace(std::move(source), out);
+  return 0;
 }
 
 // The Milstein layout, in the order the kernel reads it: go exists from the vjp part on, registers carry over.
@@ -822,18 +972,17 @@ pw_chunk_ext_kernel(const __grid_constant__ PwProg<T> pg, const PwChunkP<T> p, c
 }
 
 // ---- launch ---------------------------------------------------------------------------------------------------------
-// The noise, the decoded program `pg` with the shared-memory slots its launch takes (`extra` past its layout; a go
-// slot for the Milstein layout, `go`), and the part of the kernel parameters every pointwise step has (y0, y1, the
+// The noise, the decoded program `pg` with the shared-memory slots its launch takes (`extra` past its layout), and the part of the kernel parameters every pointwise step has (y0, y1, the
 // quad mapping, vec) for a program that passes `layout`; TSDE_EINVAL for a launch the kernels cannot serve.
 template <typename T>
 static int pw_prepare(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
-                      void* y1, bool (*layout)(const tsde_pointwise&), bool go, int extra, PwProg<T>& pg, int& slots,
+                      void* y1, bool (*layout)(const tsde_pointwise&), int extra, PwProg<T>& pg, int& slots,
                       PwP<T>& p, NoiseP<T>& np) {
   if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !prog || !y0 || !y1) return TSDE_EINVAL;
   bool vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y1);
   if (!pw_valid_tables(*prog, &vec) || !layout(*prog)) return TSDE_EINVAL;
   if (int e = fill_noise<T>(L, nz, false, np)) return e;
-  slots = pw_decode<T>(*prog, go, extra, pg);
+  slots = pw_decode<T>(*prog, extra, pg);
   p = PwP<T>{};
   p.y0 = static_cast<const T*>(y0);
   p.y1 = static_cast<T*>(y1);
@@ -843,7 +992,7 @@ static int pw_prepare(const tsde_launch* L, const tsde_noise* nz, const tsde_poi
 }
 
 // One thread per quad, `slots` shared-memory registers per thread; `single` draws from one Brownian cell, `multi` sums
-// the cells of a step that spans several.  `x` are the kernel's parameters past the noise (the Milstein step table).
+// the cells of a step that spans several.  `x` are the kernel's parameters past the noise (a chunk's step table).
 template <typename T, typename P, typename... X>
 static int pw_launch(const tsde_launch* L, const PwProg<T>& prog,
                      void (*single)(PwProg<T>, P, NoiseP<T>, X...),
@@ -863,36 +1012,45 @@ static int pw_launch(const tsde_launch* L, const PwProg<T>& prog,
 
 using namespace tsde;
 
-// The chunk `steps[0, n_steps)` from y0 (both entry points): one launch of pw_milstein_kernel.  A step that merges
-// several Brownian cells (nz->n_cells > 1) runs alone, in the kSrcCounterMulti instantiation.
+// The chunk `steps[0, n_steps)` from y0 (both entry points): one launch of the program's compiled kernel (compiled
+// here if this is the first launch of its structure).  A step that merges several Brownian cells (nz->n_cells > 1)
+// runs alone, in the kSrcCounterMulti kernel.
 template <typename T>
 static int pw_milstein_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
                              const tsde_pw_step* steps, int32_t n_steps, int32_t ito) {
   if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
-  PwProg<T> pg;
-  int slots;
-  PwP<T> p;
+  if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !prog || !y0) return TSDE_EINVAL;
+  bool vec = L->d % 4 == 0 && aligned16(y0);
+  if (!pw_valid_tables(*prog, &vec) || !pw_valid_milstein(*prog)) return TSDE_EINVAL;
   NoiseP<T> np;
-  if (int e = pw_prepare<T>(L, nz, prog, y0, steps[n_steps - 1].y1, pw_valid_milstein, true, 0, pg, slots, p, np))
-    return e;
+  if (int e = fill_noise<T>(L, nz, false, np)) return e;
   if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
   PwSteps<T> st{};
   st.n = n_steps;
   for (int j = 0; j < n_steps; ++j) {
     const tsde_pw_step& s = steps[j];
     if (!s.t0) return TSDE_EINVAL;
-    if (s.y1 && !aligned16(s.y1)) p.vec = 0;
+    if (s.y1 && !aligned16(s.y1)) vec = false;
     st.s[j] = PwStep<T>{s.cell_id, static_cast<const T*>(s.t0), static_cast<T*>(s.y1), (T)sqrt(s.h), (T)s.dt};
   }
+  PwCompiled kc;
+  if (int e = pw_compiled(*prog, sizeof(T) == 8, kc)) return e;
+  PwOperands<T> ops{};
+  for (int k = 0; k < prog->n_operands; ++k)
+    ops.k[k] = PwOperand<T>{static_cast<const T*>(prog->operand[k].ptr), (T)prog->operand[k].imm};
+  PwP<T> p{};
+  p.y0 = static_cast<const T*>(y0);
+  fill_quad_map(L->rows, L->d, p);
+  p.vec = vec ? 1 : 0;
+  p.ito = ito;
   // (the multi-cell merge reads the first cell and the uniform length from the noise descriptor)
   np.cell_id = steps[0].cell_id;
   np.h = steps[0].h;
-  p.ito = ito;
-  if (pg.ext)
-    return pw_launch<T>(L, pg, pw_milstein_ext_kernel<T, TSDE_SRC_COUNTER>, pw_milstein_ext_kernel<T, kSrcCounterMulti>,
-                        p, np, p.nquads, slots, TSDE_KERNEL_PW_MILSTEIN, st);
-  return pw_launch<T>(L, pg, pw_milstein_kernel<T, TSDE_SRC_COUNTER>, pw_milstein_kernel<T, kSrcCounterMulti>, p, np,
-                      p.nquads, slots, TSDE_KERNEL_PW_MILSTEIN, st);
+  void* args[] = {&ops, &p, &np, &st};
+  const int e = launch_kernel_handle(kc.kernel[np.n_cells > 1], (p.nquads + kThreads - 1) / kThreads, kThreads,
+                                     reinterpret_cast<cudaStream_t>(L->stream), args);
+  if (e == 0) g_launches[TSDE_KERNEL_PW_MILSTEIN].fetch_add(1, std::memory_order_relaxed);
+  return e;
 }
 
 // The chunk `steps[0, n_steps)` of Euler or reversible Heun from y0 (and, for reversible Heun, from the solver state
@@ -906,7 +1064,7 @@ static int pw_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_point
   int slots;
   PwChunkP<T> p{};
   NoiseP<T> np;
-  if (int e = pw_prepare<T>(L, nz, prog, y0, steps[n_steps - 1].y1, pw_valid_two<TSDE_PW_MAX_REGS>, false, 0, pg,
+  if (int e = pw_prepare<T>(L, nz, prog, y0, steps[n_steps - 1].y1, pw_valid_two<TSDE_PW_MAX_REGS>, 0, pg,
                             slots, p.base, np))
     return e;
   if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
@@ -992,7 +1150,7 @@ TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_no
     int slots;
     PwSrkP<T> p;
     NoiseP<T> np;
-    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_two<TSDE_PW_SRK_MAX_REGS>, false,
+    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_two<TSDE_PW_SRK_MAX_REGS>,
                               PwSrkStash<T>::kShared ? kPwSrkStash : 0, pg, slots, p.base, np))
       return e;
     const void* times[4] = {t_0, t_1, t_q, t_h};
@@ -1022,7 +1180,7 @@ TSDE_EXPORT int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, co
     int slots;
     PwPcP<T> p;
     NoiseP<T> np;
-    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_two<TSDE_PW_MAX_REGS>, false, 0, pg, slots, p.base, np))
+    if (int e = pw_prepare<T>(L, nz, prog, y0, y1, pw_valid_two<TSDE_PW_MAX_REGS>, 0, pg, slots, p.base, np))
       return e;
     p.base.t0 = static_cast<const T*>(t0);
     p.base.dt = (T)dt;
@@ -1054,5 +1212,33 @@ TSDE_EXPORT int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, co
         return go(pw_pc_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_EULER_HEUN>,
                   pw_pc_kernel<T, kSrcCounterMulti, TSDE_PC_EULER_HEUN>);
     }
+  });
+}
+
+// A Milstein program the launches `L` may run (tsde_solve_milstein_pointwise's checks of L and prog)
+static bool pw_milstein_program(const tsde_launch* L, const tsde_pointwise* prog) {
+  bool vec = true;
+  return L->noise_type == TSDE_NOISE_DIAGONAL && L->m == L->d && prog && pw_valid_tables(*prog, &vec) &&
+         pw_valid_milstein(*prog);
+}
+
+TSDE_EXPORT int tsde_pointwise_compile(const tsde_launch* L, const tsde_pointwise* prog) {
+  return dispatch(L, [&](auto t) -> int {
+    if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
+    PwCompiled kc;
+    return pw_compiled(*prog, sizeof(t) == 8, kc);
+  });
+}
+
+TSDE_EXPORT int64_t tsde_pointwise_source(const tsde_launch* L, const tsde_pointwise* prog, char* buf, int64_t size) {
+  return dispatch(L, [&](auto t) -> int64_t {
+    if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
+    const std::string src = pw_milstein_source(*prog, sizeof(t) == 8);
+    if (buf && size > 0) {
+      const size_t n = std::min(src.size(), (size_t)size - 1);
+      memcpy(buf, src.data(), n);
+      buf[n] = 0;
+    }
+    return (int64_t)src.size();
   });
 }

@@ -1,0 +1,334 @@
+// Device code that both the library's nvcc build and its run-time compiler (NVRTC, pointwise.cu) compile: the
+// quad-per-thread layout, the Brownian increment of one quad, the Milstein step's two ops, and the chunked Milstein
+// step loop of an element-wise program compiled into its own kernel.  Nothing here includes a host header: NVRTC has
+// none, so the library hands it this file, philox.cuh, rowdiv.cuh, the public header and a <stdint.h> of its own
+// (build() embeds them into the library as strings; the library never reads csrc/ at run time).
+#pragma once
+#include <stdint.h>
+
+#include "../../include/torchsde_b200.h"
+#include "philox.cuh"
+#include "rowdiv.cuh"
+
+namespace tsde {
+
+constexpr int kThreads = 256;
+
+template <typename T>
+struct NoiseP {
+  const T* w;         // MEMORY
+  const T* u;         // MEMORY
+  const void* key;    // COUNTER
+  uint64_t cell_id;
+  int64_t row_offset;
+  int32_t n_cells;
+  int32_t bcast;      // noise has a single channel shared by all d (scalar noise, squeezed g)
+  double h;           // uniform cell length
+  const double* cell_h;  // device, or nullptr
+  double h_total;     // tb - ta of the whole query (for U)
+  int64_t m;          // channels of the noise tensor
+  T sqrt_h;           // (T)sqrt(h), (T)sqrt(h/12), (T)h_total: host-rounded once (single-cell path)
+  T sqrt_h12;
+  T ht;
+};
+
+// ---- vector load / store helpers ---------------------------------------------------------
+__device__ __forceinline__ void ld4(const float* p, float (&v)[4]) {
+  const float4 t = *reinterpret_cast<const float4*>(p);
+  v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+}
+__device__ __forceinline__ void ld4(const double* p, double (&v)[4]) {
+  const double2 a = *reinterpret_cast<const double2*>(p);
+  const double2 b = *reinterpret_cast<const double2*>(p + 2);
+  v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
+}
+__device__ __forceinline__ void st4(float* p, const float (&v)[4]) {
+  *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+}
+__device__ __forceinline__ void st4(double* p, const double (&v)[4]) {
+  *reinterpret_cast<double2*>(p) = make_double2(v[0], v[1]);
+  *reinterpret_cast<double2*>(p + 2) = make_double2(v[2], v[3]);
+}
+
+template <typename T>
+__device__ __forceinline__ void load_quad(const T* p, int64_t base, bool vec, int nvalid,
+                                          T (&v)[4]) {
+  if (vec) {
+    ld4(p + base, v);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[j] = j < nvalid ? p[base + j] : T(0);
+  }
+}
+template <typename T>
+__device__ __forceinline__ void store_quad(T* p, int64_t base, bool vec, int nvalid,
+                                           const T (&v)[4]) {
+  if (vec) {
+    st4(p + base, v);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (j < nvalid) p[base + j] = v[j];
+  }
+}
+
+// ---- Brownian increment of one quad --------------------------------------------------------
+// Counter mode: merge of n_cells primary cells, left to right, with the reference's
+// aggregation rule (brownian_interval.py:643-672):
+//     H <- ( len_i (H_i + W/2) + (start_i - ta)(H - W_i/2) ) / (end_i - ta) ;  W <- W + W_i
+// Lengths are host doubles rounded once to T (python-float * tensor semantics).
+constexpr int kSrcCounterMulti = 3;  // internal: COUNTER source merging several primary cells
+
+template <typename T, bool WANT_U, bool MULTI = true>
+__device__ __forceinline__ void counter_noise(const NoiseP<T>& nz, Key key, uint32_t row,
+                                              uint32_t q, T (&w)[4], T (&u)[4]) {
+  T hh[4];
+  if (!MULTI || nz.n_cells == 1) {
+    // the solver's own grid: one primary cell per step, scales rounded once on the host
+    T n[4];
+    normal4(key, nz.cell_id, STREAM_W, row, q, n);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) w[j] = n[j] * nz.sqrt_h;
+    if (WANT_U) {
+      normal4(key, nz.cell_id, STREAM_H, row, q, n);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        hh[j] = n[j] * nz.sqrt_h12;
+        u[j] = nz.ht * (T(0.5) * w[j] + hh[j]);  // _H_to_U :102-103
+      }
+    }
+    return;
+  }
+  if (!MULTI) return;  // (unreachable; lets the compiler drop the merge loop from single-cell kernels)
+  double len0 = nz.cell_h ? nz.cell_h[0] : nz.h;
+  {
+    T n[4];
+    normal4(key, nz.cell_id, STREAM_W, row, q, n);
+    const T s = (T)sqrt(len0);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) w[j] = n[j] * s;
+    if (WANT_U) {
+      normal4(key, nz.cell_id, STREAM_H, row, q, n);
+      const T s12 = (T)sqrt(len0 / 12.0);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) hh[j] = n[j] * s12;
+    }
+  }
+  double elapsed = len0;  // start_i - ta
+  for (int c = 1; c < nz.n_cells; ++c) {
+    const double len = nz.cell_h ? nz.cell_h[c] : nz.h;
+    T n[4], wi[4];
+    normal4(key, nz.cell_id + (uint64_t)c, STREAM_W, row, q, n);
+    const T s = (T)sqrt(len);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) wi[j] = n[j] * s;
+    if (WANT_U) {
+      normal4(key, nz.cell_id + (uint64_t)c, STREAM_H, row, q, n);
+      const T s12 = (T)sqrt(len / 12.0);
+      const T tl = (T)len, te = (T)elapsed, tt = (T)(elapsed + len);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const T hi = n[j] * s12;
+        const T term1 = tl * (hi + T(0.5) * w[j]);
+        const T term2 = te * (hh[j] - T(0.5) * wi[j]);
+        hh[j] = (term1 + term2) / tt;
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) w[j] = w[j] + wi[j];
+    elapsed += len;
+  }
+  if (WANT_U) {
+    const T ht = (T)nz.h_total;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) u[j] = ht * (T(0.5) * w[j] + hh[j]);  // _H_to_U :102-103
+  }
+}
+
+template <typename T, int SRC, bool WANT_U>
+__device__ __forceinline__ void quad_noise(const NoiseP<T>& nz, Key key, int64_t row, int64_t q,
+                                           bool vec, int nvalid, T (&w)[4], T (&u)[4]) {
+  if (SRC == TSDE_SRC_UNIT) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { w[j] = T(1); u[j] = T(0); }
+  } else if (SRC == TSDE_SRC_MEMORY) {
+    if (nz.bcast) {
+      const T a = nz.w[row];
+      const T b = WANT_U ? nz.u[row] : T(0);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) { w[j] = a; u[j] = b; }
+    } else {
+      const int64_t base = row * nz.m + 4 * q;
+      load_quad(nz.w, base, vec, nvalid, w);
+      if (WANT_U) load_quad(nz.u, base, vec, nvalid, u);
+    }
+  } else {
+    constexpr bool MULTI = SRC == kSrcCounterMulti;
+    const uint32_t grow = (uint32_t)(row + nz.row_offset);
+    if (nz.bcast) {
+      T w4[4], u4[4];
+      counter_noise<T, WANT_U, MULTI>(nz, key, grow, 0u, w4, u4);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) { w[j] = w4[0]; u[j] = WANT_U ? u4[0] : T(0); }
+    } else {
+      counter_noise<T, WANT_U, MULTI>(nz, key, grow, (uint32_t)q, w, u);
+    }
+  }
+}
+
+// ---- the Milstein step's ops (tableau_diag_ops.cuh holds the others) --------------------------
+// go = g * (0.5 * v)                       methods/milstein.py:56,69,80-81,90-91 base_sde.py:142-155
+template <typename T>
+struct MilsteinSeedOp {
+  static constexpr int NIN = 1, NOUT = 1;
+  static constexpr bool USES_NOISE = true, WANT_U = false;
+  T dt;
+  int ito;
+  __device__ __forceinline__ void operator()(const T (&in)[1], T w, T, T (&out)[1]) const {
+    const T v = ito ? (w * w - dt) : (w * w);
+    out[0] = in[0] * (T(0.5) * v);
+  }
+};
+
+// y1 = y0 + f*dt + g*dW + gdg                                               methods/milstein.py:72
+template <typename T>
+struct MilsteinOp {
+  static constexpr int NIN = 4, NOUT = 1;
+  static constexpr bool USES_NOISE = true, WANT_U = false;
+  static constexpr bool STREAM_INPUTS = true;  // y0, f, g, gdg are all dead after the step's last kernel
+  T dt;
+  __device__ __forceinline__ void operator()(const T (&in)[4], T w, T, T (&out)[1]) const {
+    const T y0 = in[0], f = in[1], g = in[2], gdg = in[3];
+    out[0] = ((y0 + f * dt) + g * w) + gdg;
+  }
+};
+
+// ---- the whole-step kernels' parameters (pointwise.cu) --------------------------------------
+template <typename T>
+struct PwP {
+  const T* y0;
+  T* y1;
+  const T* t0;
+  int64_t d, qpr, nquads;
+  uint64_t qmagic;  // rowdiv_magic(qpr) when qpr is not a power of two
+  int32_t qshift;   // log2(qpr), or -1
+  int32_t small;    // nquads < 2^31
+  int32_t vec;      // d % 4 == 0 and every tensor 16-byte aligned
+  T dt;
+  int32_t ito;
+};
+
+template <typename T>
+struct PwOperand {
+  const T* ptr;  // SCALAR, CHANNEL, ROW; null for IMM
+  T imm;
+};
+
+struct PwQuad {  // where this thread's quad lives
+  int64_t base, chan;
+  int nvalid;
+  bool vec;
+};
+
+// The flat index Q of this thread's quad (past the last quad when Q >= p.nquads), the row and quad of the row, and `c`.
+template <typename T>
+__device__ __forceinline__ void pw_locate(const PwP<T>& p, PwQuad& c, int64_t& Q, int64_t& row, int64_t& q) {
+  Q = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+  if (p.qshift >= 0) {
+    row = Q >> p.qshift;
+    q = Q & ((1ll << p.qshift) - 1);
+  } else if (p.small) {
+    const uint32_t r32 = rowdiv_row((uint32_t)Q, p.qmagic);
+    row = r32;
+    q = (int64_t)rowdiv_quad((uint32_t)Q, r32, (uint32_t)p.qpr);
+  } else {
+    row = Q / p.qpr;
+    q = Q - row * p.qpr;
+  }
+  c.chan = 4 * q;
+  c.base = row * p.d + c.chan;
+  const int64_t rem = p.d - c.chan;
+  c.nvalid = rem < 4 ? (int)rem : 4;
+  c.vec = p.vec != 0;
+}
+
+// A chunk of consecutive steps (tsde_solve_milstein_pointwise, tsde_solve_euler_pointwise, ...): one thread runs up to
+// kPwMaxSteps steps of its quad.
+constexpr int kPwMaxSteps = TSDE_PW_MAX_STEPS;
+
+template <typename T>
+struct PwStep {  // one step of a chunk, as tsde_pw_step with its scalars rounded to T on the host
+  uint64_t cell;   // Brownian cell (the kSrcCounterMulti kernel merges nz.n_cells cells from here)
+  const T* t0;     // what TSDE_PW_T0 reads during this step
+  T* y1;           // destination of this step's y1, or null
+  T sqrt_h, dt;    // (T)sqrt(h) of the cell, (T)dt
+};
+template <typename T>
+struct PwSteps {  // by value: a captured launch carries the whole table
+  int32_t n;
+  PwStep<T> s[kPwMaxSteps];
+};
+
+// ---- consecutive Milstein steps of a compiled program ----------------------------------------
+// The operands of a compiled program, in the caller's order: IMM values and device pointers are launch parameters,
+// so one compiled kernel serves every value and address of its program's structure.
+template <typename T>
+struct PwOperands {
+  PwOperand<T> k[TSDE_PW_MAX_OPERANDS];
+};
+
+// Per step: the program's f / g part runs on y, MilsteinSeedOp forms go, the vjp part runs and MilsteinOp forms y1.
+// A quad's trajectory depends on nothing but its own state (element-wise SDE, diagonal noise), so one thread runs the
+// whole chunk: y0 is read once, y stays in registers from one step to the next and is stored only where the step table
+// gives it a destination (an output row, the chunk's last state).  The unfused step moves 13 tensors; a chunk moves one
+// read and the stores it is asked for.
+//
+// `Prog` is the program, generated by the library as straight-line code (pw_codegen in pointwise.cu):
+//   load(ops, c)                    its operands, after the dependency wait (CHANNEL / ROW quads it keeps in registers)
+//   fg(ops, c, s, y, f, g)          instructions [0, n_fg) at (s.t0, y), and the f and g results
+//   vjp(ops, c, s, y, go, gdg)      instructions [n_fg, n_instr), and the gdg result
+// Its registers are members: values of the f / g part that the vjp part reads carry over.
+template <typename T, int SRC, typename Prog>
+__device__ __forceinline__ void pw_milstein_steps(const PwOperands<T>& ops, const PwP<T>& p, const NoiseP<T>& nz,
+                                                  const PwSteps<T>& st) {
+  PwQuad c;
+  int64_t Q, row, q;
+  pw_locate(p, c, Q, row, q);
+  const Key key = load_key(nz.key);
+  Prog prog;
+  T y[4];
+  for (int j = 0; j < st.n; ++j) {
+    const PwStep<T>& s = st.s[j];
+    T w[4], u[4];
+    NoiseP<T> z = nz;  // this step's cell
+    z.cell_id = s.cell;
+    z.sqrt_h = s.sqrt_h;
+    quad_noise<T, SRC, false>(z, key, row, q, c.vec, c.nvalid, w, u);
+    if (j == 0) {  // the first increment is drawn while the previous kernel drains; the rest is read after the wait
+      asm volatile("griddepcontrol.wait;" ::: "memory");
+      if (Q >= p.nquads) return;
+      load_quad(p.y0, c.base, c.vec, c.nvalid, y);
+      prog.load(ops, c);
+    }
+    T f[4], g[4], go[4], gdg[4];
+    prog.fg(ops, c, s, y, f, g);
+    const MilsteinSeedOp<T> seed{s.dt, p.ito};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      T o[1];
+      seed({g[i]}, w[i], u[i], o);
+      go[i] = o[0];
+    }
+    prog.vjp(ops, c, s, y, go, gdg);
+    const MilsteinOp<T> step{s.dt};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      T o[1];
+      step({y[i], f[i], g[i], gdg[i]}, w[i], u[i], o);
+      y[i] = o[0];
+    }
+    if (s.y1) store_quad(s.y1, c.base, c.vec, c.nvalid, y);
+  }
+}
+
+}  // namespace tsde

@@ -21,31 +21,7 @@ struct EulerOp {
   }
 };
 
-// go = g * (0.5 * v)                       methods/milstein.py:56,69,80-81,90-91 base_sde.py:142-155
-template <typename T>
-struct MilsteinSeedOp {
-  static constexpr int NIN = 1, NOUT = 1;
-  static constexpr bool USES_NOISE = true, WANT_U = false;
-  T dt;
-  int ito;
-  __device__ __forceinline__ void operator()(const T (&in)[1], T w, T, T (&out)[1]) const {
-    const T v = ito ? (w * w - dt) : (w * w);
-    out[0] = in[0] * (T(0.5) * v);
-  }
-};
-
-// y1 = y0 + f*dt + g*dW + gdg                                               methods/milstein.py:72
-template <typename T>
-struct MilsteinOp {
-  static constexpr int NIN = 4, NOUT = 1;
-  static constexpr bool USES_NOISE = true, WANT_U = false;
-  static constexpr bool STREAM_INPUTS = true;  // y0, f, g, gdg are all dead after the step's last kernel
-  T dt;
-  __device__ __forceinline__ void operator()(const T (&in)[4], T w, T, T (&out)[1]) const {
-    const T y0 = in[0], f = in[1], g = in[2], gdg = in[3];
-    out[0] = ((y0 + f * dt) + g * w) + gdg;
-  }
-};
+// (MilsteinSeedOp, MilsteinOp: pw_device.cuh, which the run-time compiled Milstein kernels include too)
 
 // y' = y0 + (dt*f | 0.) + g*sqrt_dt                                          methods/milstein.py:63
 template <typename T>
