@@ -136,6 +136,8 @@ const char* tsde_error_string(int code);
 #define TSDE_KERNEL_PW_CHUNK 6    /* Euler / reversible-Heun steps with an element-wise SDE, up to
                                      TSDE_PW_MAX_STEPS per launch (tsde_solve_euler_pointwise,
                                      tsde_solve_reversible_heun_pointwise)                                      */
+#define TSDE_KERNEL_PW_ADAPTIVE 7 /* an adaptive solve's proposal with an element-wise SDE, the full step and both
+                                     half steps in one launch (tsde_adaptive_proposal_pointwise)                */
 int64_t tsde_kernel_launches(int32_t family);
 
 /* ------------------------------------------------------------------------ */
@@ -425,6 +427,45 @@ int tsde_solve_euler_pointwise(const tsde_launch* L, const tsde_noise* nz, const
 int tsde_solve_reversible_heun_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
                                          const void* y0, const void* z0, const void* f0, const void* g0,
                                          const tsde_pw_step* steps, int32_t n_steps, void* z1, void* f1, void* g1);
+
+/*
+ * One proposal of an adaptive solve's step doubling, for an SDE whose f(t, y) and g(t, y) are element-wise programs:
+ * one launch reads y0 and runs `method`'s step three times in registers,
+ *     subs[0]  the full step from y0, stored to y_full;
+ *     subs[1]  the first half step from y0, to the midpoint state (not stored);
+ *     subs[2]  the second half step from the midpoint state, stored to y_next.
+ * Each sub-step reads its increment from memory: w, and for SRK the space-time Levy area u, both (rows, d) tensors of
+ * the state dtype (the Brownian motion's answers to the sub-step's query).  It runs the program at the 0-d device
+ * times t[] (state dtype, read at every launch) and takes dt and the scalars s[] the unfused step takes:
+ *     TSDE_PROPOSAL_EULER                    t[0] = t0; as tsde_solve_euler_pointwise
+ *     TSDE_PROPOSAL_MILSTEIN_ITO / _STRATONOVICH
+ *                                            t[0] = t0; as tsde_step_milstein_pointwise (Milstein layout; the
+ *                                            program is compiled into a kernel of its own, as for that entry point)
+ *     TSDE_PROPOSAL_SRK                      t[0..3] = t_0, t_1, t_q, t_h; s = (rdt, sqrt_dt, three_dt); as
+ *                                            tsde_step_srk_diag_pointwise
+ *     TSDE_PROPOSAL_HEUN, _MIDPOINT, _EULER_HEUN
+ *                                            t[0] = t0, t[1] = t_p; midpoint: s[0] = half_dt; as
+ *                                            tsde_step_predictor_corrector_pointwise
+ * Both stored states equal the three unfused steps' bit for bit.  Requires DIAGONAL noise (m == d) and no 16-bit
+ * formats.  TSDE_EINVAL: an unknown method, a null y0, subs, y_full or y_next, a null w (u for SRK) or time the
+ * method reads, and a program of another layout than its method's; all checked before anything is compiled or
+ * launched.  An empty batch is a no-op.
+ *
+ * tsde_adaptive_pointwise_compile compiles and loads the proposal kernel of Milstein program `prog` without
+ * launching anything, under the rules of tsde_pointwise_compile; the proposal compiles it on first use otherwise.
+ */
+enum { TSDE_PROPOSAL_EULER = 0, TSDE_PROPOSAL_MILSTEIN_ITO = 1, TSDE_PROPOSAL_MILSTEIN_STRATONOVICH = 2,
+       TSDE_PROPOSAL_SRK = 3, TSDE_PROPOSAL_HEUN = 4, TSDE_PROPOSAL_MIDPOINT = 5, TSDE_PROPOSAL_EULER_HEUN = 6 };
+typedef struct tsde_pw_substep {
+  const void* w;     /* DEVICE (rows, d) increment                                  */
+  const void* u;     /* DEVICE (rows, d) space-time Levy area (SRK), else unused     */
+  const void* t[4];  /* DEVICE 0-d times (state dtype); unused entries may be NULL   */
+  double      dt;    /* the sub-step's dt                                            */
+  double      s[3];  /* the method's scalars                                         */
+} tsde_pw_substep;
+int tsde_adaptive_proposal_pointwise(const tsde_launch* L, const tsde_pointwise* prog, int32_t method,
+                                     const void* y0, const tsde_pw_substep* subs, void* y_full, void* y_next);
+int tsde_adaptive_pointwise_compile(const tsde_launch* L, const tsde_pointwise* prog);
 
 /* derivative-free Milstein, predictor: y' = y0 + (Ito ? dt*f : 0) + g*sqrt_dt
  * methods/milstein.py:58-63,83-84,93-94.  g is (rows,d) also for scalar noise (squeezed). */

@@ -54,6 +54,12 @@ def compile_pointwise(prog, dtype):
     return lib().tsde_pointwise_compile(ctypes.byref(_program_launch(dtype)), ctypes.byref(prog))
 
 
+def compile_adaptive_pointwise(prog, dtype):
+    """tsde_adaptive_pointwise_compile: compile and load the adaptive proposal kernel of Milstein program `prog` in
+    `dtype`; 0 or an error code."""
+    return lib().tsde_adaptive_pointwise_compile(ctypes.byref(_program_launch(dtype)), ctypes.byref(prog))
+
+
 class LibraryNotBuilt(RuntimeError):
     pass
 
@@ -80,6 +86,10 @@ KERNEL_PW_MILSTEIN = 3  # TSDE_KERNEL_PW_MILSTEIN
 KERNEL_PW_SRK = 4  # TSDE_KERNEL_PW_SRK
 KERNEL_PW_PC = 5  # TSDE_KERNEL_PW_PC
 KERNEL_PW_CHUNK = 6  # TSDE_KERNEL_PW_CHUNK
+KERNEL_PW_ADAPTIVE = 7  # TSDE_KERNEL_PW_ADAPTIVE
+# TSDE_PROPOSAL_*: the method of tsde_adaptive_proposal_pointwise
+(PROPOSAL_EULER, PROPOSAL_MILSTEIN_ITO, PROPOSAL_MILSTEIN_STRATONOVICH, PROPOSAL_SRK, PROPOSAL_HEUN, PROPOSAL_MIDPOINT,
+ PROPOSAL_EULER_HEUN) = range(7)
 PC_HEUN, PC_MIDPOINT, PC_EULER_HEUN = range(3)  # TSDE_PC_*
 PW_MAX_STEPS = 64  # TSDE_PW_MAX_STEPS
 
@@ -103,6 +113,11 @@ class Pointwise(ctypes.Structure):
 class PwStep(ctypes.Structure):
     _fields_ = [('cell_id', ctypes.c_uint64), ('h', ctypes.c_double), ('dt', ctypes.c_double), ('t0', ctypes.c_void_p),
                 ('y1', ctypes.c_void_p)]
+
+
+class PwSubstep(ctypes.Structure):
+    _fields_ = [('w', ctypes.c_void_p), ('u', ctypes.c_void_p), ('t', ctypes.c_void_p * 4), ('dt', ctypes.c_double),
+                ('s', ctypes.c_double * 3)]
 
 
 _P = ctypes.c_void_p
@@ -135,6 +150,8 @@ SIGNATURES = {
     'tsde_solve_euler_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, ctypes.POINTER(PwStep), _I],
     'tsde_solve_reversible_heun_pointwise': [_L, _N, ctypes.POINTER(Pointwise), _P, _P, _P, _P,
                                              ctypes.POINTER(PwStep), _I, _P, _P, _P],
+    'tsde_adaptive_proposal_pointwise': [_L, ctypes.POINTER(Pointwise), _I, _P, ctypes.POINTER(PwSubstep), _P, _P],
+    'tsde_adaptive_pointwise_compile': [_L, ctypes.POINTER(Pointwise)],
     'tsde_milstein_gf_predict': [_L, _P, _P, _P, _D, _D, _I, _P],
     'tsde_step_milstein_gf': [_L, _N, _P, _P, _P, _P, _D, _D, _I, _P],
     'tsde_step_heun': [_L, _N, _P, _P, _P, _P, _P, _D, _P],
@@ -232,6 +249,8 @@ INPUTS = {
     'tsde_step_euler': ('y0', 'f', 'g'),
     'tsde_milstein_vjp_seed': ('g',),
     'tsde_step_milstein': ('y0', 'f', 'g', 'gdg'),
+    'tsde_adaptive_proposal_pointwise': [_L, ctypes.POINTER(Pointwise), _I, _P, ctypes.POINTER(PwSubstep), _P, _P],
+    'tsde_adaptive_pointwise_compile': [_L, ctypes.POINTER(Pointwise)],
     'tsde_milstein_gf_predict': ('y0', 'f', 'g'),
     'tsde_step_milstein_gf': ('y0', 'f', 'g', 'gp'),
     'tsde_step_heun': ('y0', 'f', 'fp', 'g', 'gp'),

@@ -395,18 +395,22 @@ class BaseSDESolver(metaclass=abc.ABCMeta):
         return ctxs
 
     # ------------------------------------------------------------------------------------------
-    def step(self, t0, t1, y0, extra0):
-        """Reference-compatible single step (base_solver.py:75-90): queries ``self.bm(t0, t1)``."""
-        if not self._prepared:
-            self._prepare(y0)
-        self._refresh_stream()
+    def _context(self, t0, t1):
+        """The context of a single step from t0 to t1 (`step`, and the sub-steps of a fused adaptive proposal)."""
         t0 = torch.as_tensor(t0)
         t1 = torch.as_tensor(t1)
         c0, c1 = t0.detach().cpu(), t1.detach().cpu()
         dt = c1 - c0
         aux = [a.to(self.device) for a in self.aux_times(c0, c1, dt)]
-        c = StepContext(self, 0, t0.to(self.device), t1.to(self.device), float(c0), float(c1), float(dt),
-                        self.scalars(dt), aux)
+        return StepContext(self, 0, t0.to(self.device), t1.to(self.device), float(c0), float(c1), float(dt),
+                           self.scalars(dt), aux)
+
+    def step(self, t0, t1, y0, extra0):
+        """Reference-compatible single step (base_solver.py:75-90): queries ``self.bm(t0, t1)``."""
+        if not self._prepared:
+            self._prepare(y0)
+        self._refresh_stream()
+        c = self._context(t0, t1)
         self._feed = NoiseFeed(self, self.bm, None)
         self._cur_c = c
         if self._autograd:
@@ -479,11 +483,20 @@ class BaseSDESolver(metaclass=abc.ABCMeta):
         factor = min(facmax, max(facmin, factor))
         return prev_step_size * factor, prev_error_ratio
 
+    def _propose(self, curr_t, next_t, midpoint_t, curr_y, curr_extra):
+        """One proposal of the adaptive loop: the full step to next_t and the two half steps through midpoint_t, as
+        (y_full, y_next, extra_next).  Methods whose proposal can run as one kernel override it (methods.py)."""
+        next_y_full, _ = self.step(curr_t, next_t, curr_y, curr_extra)
+        midpoint_y, midpoint_extra = self.step(curr_t, midpoint_t, curr_y, curr_extra)
+        next_y, next_extra = self.step(midpoint_t, next_t, midpoint_y, midpoint_extra)
+        return next_y_full, next_y, next_extra
+
     def _integrate_adaptive(self, y0, ts, extra0):
         """One full step vs two half steps per proposal; accept / reject on the host.  Step sizes are
         data dependent, so this branch is an eager loop (one device->host scalar per proposal, exactly
         the reference's sync count) and the Brownian motion is queried at arbitrary times through
-        ``bm(ta, tb)``; every step still runs the fused tableau kernels.  When gradients flow through the solve
+        ``bm(ta, tb)``; every step still runs the fused tableau kernels, and an element-wise SDE's proposal is one
+        kernel (`_propose`, pointwise.propose).  When gradients flow through the solve
         (`self._autograd`) every launch is an autograd node, as in the fixed-step loop; the error estimate
         never carries gradient (the reference turns it into a Python float, base_solver.py:127-134)."""
         track = self._autograd
@@ -507,10 +520,8 @@ class BaseSDESolver(metaclass=abc.ABCMeta):
                 out_t = ts_cpu[i]
                 while curr_t < out_t:
                     next_t = min(curr_t + step_size, ts_cpu[-1])
-                    next_y_full, _ = self.step(curr_t, next_t, curr_y, curr_extra)
                     midpoint_t = 0.5 * (curr_t + next_t)
-                    midpoint_y, midpoint_extra = self.step(curr_t, midpoint_t, curr_y, curr_extra)
-                    next_y, next_extra = self.step(midpoint_t, next_t, midpoint_y, midpoint_extra)
+                    next_y_full, next_y, next_extra = self._propose(curr_t, next_t, midpoint_t, curr_y, curr_extra)
                     error_estimate = self._error_estimate(_contig(next_y_full.detach()), _contig(next_y.detach()))
                     step_size, prev_error_ratio = self._update_step_size(
                         error_estimate=error_estimate, prev_step_size=step_size, prev_error_ratio=prev_error_ratio)

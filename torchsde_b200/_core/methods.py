@@ -45,6 +45,17 @@ class _WidenedSDE:
         return widen(self._sde.g_prod(t, y, v), self._dtype)
 
 
+class _ProposalMixin:
+    """An adaptive solve's proposals as one kernel each (pointwise.propose) once the first one has recorded the SDE's
+    element-wise program; `_proposal` is the method's TSDE_PROPOSAL_*."""
+    _proposal = None
+
+    def _propose(self, curr_t, next_t, midpoint_t, curr_y, curr_extra):
+        if pointwise.proposing(self):
+            return pointwise.propose(self, self._proposal, curr_t, next_t, midpoint_t, curr_y) + (curr_extra,)
+        return super()._propose(curr_t, next_t, midpoint_t, curr_y, curr_extra)
+
+
 class _ProdMixin:
     """Shared handling of the reference's `f_and_g_prod` / `g_prod` call sites (base_sde.py:51-56)."""
 
@@ -78,8 +89,9 @@ class _ProdMixin:
         return self._LU, self._feed.unit(), _contig(sde.g_prod(t, y, w.reshape(self.bm.shape)))
 
 
-class Euler(_ProdMixin, base_solver.BaseSDESolver):
+class Euler(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
     """methods/euler.py:19-37."""
+    _proposal = _cabi.PROPOSAL_EULER
     weak_order = 1.0
     sde_type = SDE_TYPES.ito
     noise_types = NOISE_TYPES.all()
@@ -111,7 +123,7 @@ class Euler(_ProdMixin, base_solver.BaseSDESolver):
         return self._k('tsde_step_euler', L, nz, (y0, f, g), (c.dt,), out), ()
 
 
-class BaseMilstein(_ProdMixin, base_solver.BaseSDESolver):
+class BaseMilstein(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
     """methods/milstein.py:22-74."""
     strong_order = 1.0
     weak_order = 1.0
@@ -209,22 +221,25 @@ class BaseMilstein(_ProdMixin, base_solver.BaseSDESolver):
         f, (gd, gdg) = self._fork(lambda: _contig(user('f', lambda: sde.f(c.t0, y0))), diffusion_chain, main=1)
         if rec is not None:
             res = rec.finish(raw['f'], raw['g'], raw.get('gdg', (None,))[0])
-            self._pw = pointwise.compile_milstein(rec, res) or False
+            self._pw = pointwise.compile_milstein(rec, res, self.adaptive) or False
         return self._k('tsde_step_milstein', self._L, self._feed.get(c), (y0, f, gd, gdg), (c.dt,), out), ()
 
 
 class MilsteinIto(BaseMilstein):
     sde_type = SDE_TYPES.ito
     ito = True
+    _proposal = _cabi.PROPOSAL_MILSTEIN_ITO
 
 
 class MilsteinStratonovich(BaseMilstein):
     sde_type = SDE_TYPES.stratonovich
     ito = False
+    _proposal = _cabi.PROPOSAL_MILSTEIN_STRATONOVICH
 
 
-class Heun(_ProdMixin, base_solver.BaseSDESolver):
+class Heun(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
     """methods/heun.py:25-48."""
+    _proposal = _cabi.PROPOSAL_HEUN
     weak_order = 1.0
     sde_type = SDE_TYPES.stratonovich
     noise_types = NOISE_TYPES.all()
@@ -250,8 +265,9 @@ class Heun(_ProdMixin, base_solver.BaseSDESolver):
         return self._k('tsde_step_heun', L, nz, (y0, f, fp, g, gp), (c.dt,), out), ()
 
 
-class Midpoint(_ProdMixin, base_solver.BaseSDESolver):
+class Midpoint(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
     """methods/midpoint.py:19-45."""
+    _proposal = _cabi.PROPOSAL_MIDPOINT
     weak_order = 1.0
     sde_type = SDE_TYPES.stratonovich
     noise_types = NOISE_TYPES.all()
@@ -284,8 +300,9 @@ class Midpoint(_ProdMixin, base_solver.BaseSDESolver):
         return self._k('tsde_step_euler', L, nz, (y0, fp, gp), (c.dt,), out), ()
 
 
-class EulerHeun(_ProdMixin, base_solver.BaseSDESolver):
+class EulerHeun(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
     """methods/euler_heun.py:19-42."""
+    _proposal = _cabi.PROPOSAL_EULER_HEUN
     weak_order = 1.0
     sde_type = SDE_TYPES.stratonovich
     noise_types = NOISE_TYPES.all()
@@ -407,8 +424,9 @@ class ReversibleHeun(base_solver.BaseSDESolver):
         return y1, (f1, g1, z1)
 
 
-class SRK(base_solver.BaseSDESolver):
+class SRK(_ProposalMixin, base_solver.BaseSDESolver):
     """methods/srk.py:31-111 (srid2 for diagonal/scalar noise, sra1 for additive noise)."""
+    _proposal = _cabi.PROPOSAL_SRK
     strong_order = 1.5
     weak_order = 1.5
     sde_type = SDE_TYPES.ito

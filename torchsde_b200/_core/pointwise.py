@@ -1,5 +1,5 @@
 """Element-wise tapes of the user's SDE: a diagonal-noise Milstein, SRK, Heun, midpoint, Euler-Heun, Euler or
-reversible-Heun step as one kernel.
+reversible-Heun step as one kernel, and an adaptive solve's proposal (a full step and two half steps) as one kernel.
 
 When the SDE's callables are made only of element-wise ATen ops whose CUDA result is one IEEE rounding per element,
 a whole step is one launch that reads y0 and writes y1 (include/torchsde_b200.h, csrc/pointwise.cu) instead of the
@@ -77,6 +77,20 @@ two sets of solver-owned buffers; its half step T(0.5) * T(dt) must equal the un
 (`halves_exactly`), and the state it starts from must be (rows, d) tensors of the state dtype (`state_fits`), else
 the solve keeps the ordinary step.  `sdeint_adjoint`'s forward solve is a no-grad solve, so the reversible pair's
 forward steps fuse too.
+
+Adaptive (`proposing`, `propose`, tsde_adaptive_proposal_pointwise).  An adaptive solve proposes a full step and two
+half steps and compares them (BaseSDESolver._integrate_adaptive, `_propose`).  Its Brownian motion is queried at
+data-dependent times, so it is never bound to a grid and the kernels above, which draw counter noise, do not apply.
+For Euler, Milstein, SRK, Heun, midpoint and Euler-Heun, the first proposal runs unfused and its full step records
+the program with the method's usual recorder (Milstein compiles the proposal kernel of its program instead of the
+fixed-step ones, `compile_milstein`).  Every later proposal makes the three Brownian queries the unfused steps make,
+in the same order and with the same arguments, and then one launch reads y0, runs the method's step three times on
+those increments (the midpoint state stays in registers) and writes y_full and y_next.  The error reduction
+(tsde_adaptive_error_sumsq) and the host's accept / reject logic are unchanged, so the solve's outputs, its accepted
+steps and its queries are the unfused solve's, bit for bit.  The conditions are those of `eligible`, with a Brownian
+motion whose answers have the state's shape in place of the grid binding; gradients through the solve and the
+backward solve of `sdeint_adjoint` keep the unfused steps.  Reversible Heun keeps them too: its solver state carries
+over from one proposal to the next.
 """
 import ctypes
 import numbers
@@ -525,12 +539,13 @@ _COMPILED = weakref.WeakKeyDictionary()
 COMPILES = 0  # how many of them were compiled: SDEs of one structure share the first one's kernels
 
 
-def compile_milstein(rec, res):
-    """`res`, what `rec.finish` returned, once its program's kernels are compiled and loaded (tsde_pointwise_compile);
-    None if `res` is, or if the library cannot compile the program (the tape is then rejected with the compiler's
-    reason).  Called on the recording step, so a graph solve's warm-up and capture never compile or load a module.
-    A program whose source (its structure: values and addresses are launch parameters) was compiled before is not
-    compiled again."""
+def compile_milstein(rec, res, adaptive=False):
+    """`res`, what `rec.finish` returned, once its program's kernels are compiled and loaded (tsde_pointwise_compile;
+    with `adaptive`, the proposal kernel of an adaptive solve, tsde_adaptive_pointwise_compile); None if `res` is, or
+    if the library cannot compile the program (the tape is then rejected with the compiler's reason).  Called on the
+    recording step, so a graph solve's warm-up and capture, and an adaptive solve's fused proposals, never compile or
+    load a module.  A program whose source (its structure: values and addresses are launch parameters) was compiled
+    before is not compiled again."""
     global COMPILES
     if res is None:
         return None
@@ -540,12 +555,12 @@ def compile_milstein(rec, res):
         rec.reject("the library refuses the program")
         return None
     done = _COMPILED.setdefault(_cabi.lib(), set())
-    if src not in done:
-        err = _cabi.compile_pointwise(prog, rec.dtype)
+    if (adaptive, src) not in done:
+        err = (_cabi.compile_adaptive_pointwise if adaptive else _cabi.compile_pointwise)(prog, rec.dtype)
         if err != 0:
             rec.reject(_cabi.lib().tsde_error_string(err).decode())
             return None
-        done.add(src)
+        done.add((adaptive, src))
         COMPILES += 1
     return res
 
@@ -737,9 +752,12 @@ def state_fits(solver, tensors):
 
 
 def eligible(solver):
-    """Whether a fixed-step Milstein, SRK, Heun, midpoint, Euler-Heun, Euler or reversible-Heun solve may run its
-    diagonal-noise steps as element-wise programs: no gradients (the forward solve of `sdeint_adjoint` has none), a Brownian motion bound to the solver grid (counter noise), `overlap` not
-    False, no logqp and no autocast."""
+    """Whether a Milstein, SRK, Heun, midpoint, Euler-Heun, Euler or reversible-Heun solve may run its diagonal-noise
+    steps as element-wise programs: no gradients (the forward solve of `sdeint_adjoint` has none), `overlap` not
+    False, no logqp, no autocast, and
+      * a fixed-step solve: a Brownian motion bound to the solver grid (counter noise);
+      * an adaptive one: a Brownian motion whose answers have the state's (rows, d) shape, and not the adjoint SDE of
+        `sdeint_adjoint`'s backward solve (its proposals are `proposing`)."""
     from .base_sde import SDELogqp
     sde = solver.sde
     obj = sde
@@ -747,7 +765,53 @@ def eligible(solver):
         obj = obj._base_sde
         if isinstance(obj, SDELogqp):
             return False
-    feed = getattr(solver, '_feed', None)
+    if solver.adaptive:
+        noise = (not getattr(sde, 'is_adjoint_sde', False)
+                 and tuple(solver.bm.shape) == (solver.rows, solver.d))
+    else:
+        feed = getattr(solver, '_feed', None)
+        noise = feed is not None and feed.binding is not None
     overlap = solver.options.get('overlap')
-    return (not solver._autograd and feed is not None and feed.binding is not None
-            and (overlap is None or bool(overlap)) and not torch.is_autocast_enabled('cuda'))
+    return (not solver._autograd and noise and (overlap is None or bool(overlap))
+            and not torch.is_autocast_enabled('cuda'))
+
+
+def proposing(solver):
+    """Whether this proposal of an adaptive `solver` runs as one launch of its element-wise program (`propose`): the
+    solve is `eligible` and its first proposal recorded the program."""
+    return solver.adaptive and bool(solver._pw) and eligible(solver)
+
+
+def propose(solver, method, curr_t, next_t, midpoint_t, y0):
+    """One proposal of an adaptive solve, (y_full, y_next): the Brownian motion is queried for the full step, the first
+    half step and the second half step, in that order and exactly as the three unfused steps query it (with U for
+    SRK), and one launch of tsde_adaptive_proposal_pointwise (`method`, a TSDE_PROPOSAL_*) runs the three sub-steps
+    on those increments.  Each sub-step's times and scalars are the ones the unfused step computes
+    (BaseSDESolver._context)."""
+    from .base_solver import NoiseFeed
+    prog, _ = solver._pw
+    solver._refresh_stream()
+    feed = solver._feed = NoiseFeed(solver, solver.bm, None)
+    subs, keep = (_cabi.PwSubstep * 3)(), []
+    for sub, (ta, tb) in zip(subs, ((curr_t, next_t), (curr_t, midpoint_t), (midpoint_t, next_t))):
+        c = solver._context(ta, tb)
+        w, u = feed.tensors(c, method == _cabi.PROPOSAL_SRK)
+        keep.append((c, w, u))
+        sub.w, sub.u, sub.dt = w.data_ptr(), None if u is None else u.data_ptr(), c.dt
+        if method == _cabi.PROPOSAL_SRK:
+            times, scalars = c.aux_t, (c.scalars['rdt'], c.scalars['sqrt_dt'], c.scalars['three_dt'])
+        elif method == _cabi.PROPOSAL_MIDPOINT:
+            times, scalars = (c.t0, c.aux_t[0]), (c.scalars['half_dt'],)
+        elif method in (_cabi.PROPOSAL_HEUN, _cabi.PROPOSAL_EULER_HEUN):
+            times, scalars = (c.t0, c.t1), ()
+        else:
+            times, scalars = (c.t0,), ()
+        for i, t in enumerate(times):
+            sub.t[i] = t.data_ptr()
+        for i, x in enumerate(scalars):
+            sub.s[i] = x
+    y_full, y_next = torch.empty_like(y0), torch.empty_like(y0)
+    _cabi.check(solver._lib.tsde_adaptive_proposal_pointwise(solver._L, ctypes.byref(prog), method, y0.data_ptr(),
+                                                             subs, y_full.data_ptr(), y_next.data_ptr()),
+                "tsde_adaptive_proposal_pointwise")
+    return y_full, y_next

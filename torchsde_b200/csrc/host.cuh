@@ -27,7 +27,7 @@ constexpr int64_t kMaxGlobalRows = 0xFFFFFFFFll;
 constexpr int64_t kMaxCounterChannels = 1ll << 26;
 
 // Launches issued per kernel family (TSDE_KERNEL_*), read by tsde_kernel_launches.
-constexpr int kKernelFamilies = 7;
+constexpr int kKernelFamilies = 8;
 inline std::atomic<int64_t> g_launches[kKernelFamilies];
 
 // A launch descriptor every entry point can rely on: non-null, non-negative row count, positive widths.

@@ -1,8 +1,9 @@
 // Whole steps of an element-wise SDE as one kernel: tsde_step_milstein_pointwise (and tsde_solve_milstein_pointwise,
 // up to TSDE_PW_MAX_STEPS consecutive Milstein steps in one kernel), tsde_step_srk_diag_pointwise,
 // tsde_step_predictor_corrector_pointwise, and tsde_solve_euler_pointwise and tsde_solve_reversible_heun_pointwise
-// (up to TSDE_PW_MAX_STEPS Euler or reversible-Heun steps in one kernel) (include/torchsde_b200.h describes the
-// tsde_pointwise program and its two layouts).
+// (up to TSDE_PW_MAX_STEPS Euler or reversible-Heun steps in one kernel), and tsde_adaptive_proposal_pointwise (an
+// adaptive solve's full step and two half steps in one kernel) (include/torchsde_b200.h describes the tsde_pointwise
+// program and its two layouts).
 //
 // The SDE's f and g (and for Milstein the vjp of g) arrive as a small program of element-wise instructions.  The SRK,
 // predictor-corrector and Euler / reversible-Heun kernels interpret it between the unfused step's own ops
@@ -412,8 +413,10 @@ static std::string num(int x) {
   return b;
 }
 
-// The translation unit of a program that passed pw_valid_tables and pw_valid_milstein, for dtype `f64`.
-static std::string pw_milstein_source(const tsde_pointwise& in, bool f64) {
+// The translation unit of a program that passed pw_valid_tables and pw_valid_milstein, for dtype `f64`: the kernels
+// of consecutive steps (single, multi), or with `adaptive` the kernel of an adaptive solve's proposal
+// (tsde_pw_milstein_adaptive, a translation unit of its own).
+static std::string pw_milstein_source(const tsde_pointwise& in, bool f64, bool adaptive = false) {
   const char* T = f64 ? "double" : "float";
   bool hoisted[TSDE_PW_MAX_OPERANDS] = {};
   for (int k = 0, n = 0; k < in.n_operands; ++k)
@@ -515,6 +518,11 @@ static std::string pw_milstein_source(const tsde_pointwise& in, bool f64) {
   o += part(in.n_fg, in.n_instr, {{"gdg", in.gdg_src}});
   o += "  }\n};\n}  // namespace\n}  // namespace tsde\n";
   const std::string bounds = "__launch_bounds__(" + num(kThreads) + ", " + num(kPwJitCtas[f64]) + ")";
+  if (adaptive)
+    return o + "\nextern \"C\" __global__ void " + bounds +
+           "\ntsde_pw_milstein_adaptive(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwP<tsde::T> p,\n"
+           "    tsde::T* y_next, const __grid_constant__ tsde::PwSubs<tsde::T> st) {\n"
+           "  tsde::pw_milstein_proposal<tsde::T, tsde::Prog>(ops, p, y_next, st);\n}\n";
   for (const char* v : {"single", "multi"}) {
     o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_milstein_" + v +
          "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwP<tsde::T> p,\n"
@@ -621,15 +629,15 @@ static int pw_nvrtc(const std::string& source, std::string& cubin) {
 }
 
 struct PwCompiled {
-  cudaKernel_t kernel[2];  // one Brownian cell per step, several cells merged (kSrcCounterMulti)
+  cudaKernel_t kernel[2];  // one Brownian cell per step, several cells merged (kSrcCounterMulti); adaptive: kernel[0]
 };
 
 // The loaded kernels of a program that passed validation, compiled on first use.  Libraries are context-independent:
 // one entry serves every device.
-static int pw_compiled(const tsde_pointwise& prog, bool f64, PwCompiled& out) {
+static int pw_compiled(const tsde_pointwise& prog, bool f64, PwCompiled& out, bool adaptive = false) {
   static std::mutex mu;
   static std::map<std::string, PwCompiled> cache;
-  std::string source = pw_milstein_source(prog, f64);
+  std::string source = pw_milstein_source(prog, f64, adaptive);
   std::lock_guard<std::mutex> lock(mu);
   auto it = cache.find(source);
   if (it != cache.end()) {
@@ -640,7 +648,11 @@ static int pw_compiled(const tsde_pointwise& prog, bool f64, PwCompiled& out) {
   if (int e = pw_nvrtc(source, cubin)) return e;
   cudaLibrary_t lib;
   cudaError_t e = cudaLibraryLoadData(&lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0);
-  if (e == cudaSuccess) {
+  if (e == cudaSuccess && adaptive) {
+    e = cudaLibraryGetKernel(&out.kernel[0], lib, "tsde_pw_milstein_adaptive");
+    out.kernel[1] = out.kernel[0];
+    if (e != cudaSuccess) cudaLibraryUnload(lib);
+  } else if (e == cudaSuccess) {
     e = cudaLibraryGetKernel(&out.kernel[0], lib, "tsde_pw_milstein_single");
     if (e == cudaSuccess) e = cudaLibraryGetKernel(&out.kernel[1], lib, "tsde_pw_milstein_multi");
     if (e != cudaSuccess) cudaLibraryUnload(lib);
@@ -714,31 +726,32 @@ __device__ __forceinline__ void pw_eval(const PwProg<T>& pg, const PwQuad& c, vo
   pw_fetch<true, EXT>(pg, c, regs, g ? pg.g_src : pg.f_src, out);
 }
 
-template <typename T, int SRC, bool EXT>
-__device__ __forceinline__ void pw_srk(const PwProg<T>& pg, const PwSrkP<T> p, const NoiseP<T> nz) {
-  extern __shared__ __align__(16) unsigned char pw_regs[];
-  PwQuad c;
-  T w[4], u[4], y0[4];
-  if (!pw_begin<T, SRC, true>(pg, p.base, nz, pw_regs, c, w, u, y0)) return;
+// One SRK step from y0 on the increments (w, u) at the stage times t[4] with the stage ops of the step: y1
+template <bool EXT, typename T>
+__device__ __forceinline__ void pw_srk_step(const PwProg<T>& pg, const PwQuad& c, void* pw_regs,
+                                            const T* const (&t)[4], const SrkDiagStage1Op<T>& s1,
+                                            const SrkDiagStage2Op<T>& s2, const SrkDiagStage3Op<T>& s3,
+                                            const SrkDiagFinalOp<T>& fin, const T (&w)[4], const T (&u)[4],
+                                            const T (&y0)[4], T (&y1)[4]) {
   PwSrkStash<T> st;
   st.slot0 = pg.end;
   enum { F0, F1, F2, G0, G1, G2 };
   T f[4], g[4], h0[4], h1[4], x[4], z[4];
   // s = 0: f0, g0 at (t0, y0); H0_1, H1_1
-  pw_eval<EXT>(pg, c, pw_regs, false, p.t[0], y0, f);
-  pw_eval<EXT>(pg, c, pw_regs, true, p.t[0], y0, g);
+  pw_eval<EXT>(pg, c, pw_regs, false, t[0], y0, f);
+  pw_eval<EXT>(pg, c, pw_regs, true, t[0], y0, g);
   st.put(pw_regs, F0, f);
   st.put(pw_regs, G0, g);
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     T o[2];
-    p.s1({y0[j], f[j], g[j]}, w[j], u[j], o);
+    s1({y0[j], f[j], g[j]}, w[j], u[j], o);
     h0[j] = o[0];
     h1[j] = o[1];
   }
   // s = 1: f1 at (t0 + dt, H0_1), g1 at (t0 + dt/4, H1_1); H0_2, H1_2
-  pw_eval<EXT>(pg, c, pw_regs, false, p.t[1], h0, f);
-  pw_eval<EXT>(pg, c, pw_regs, true, p.t[2], h1, g);
+  pw_eval<EXT>(pg, c, pw_regs, false, t[1], h0, f);
+  pw_eval<EXT>(pg, c, pw_regs, true, t[2], h1, g);
   st.put(pw_regs, F1, f);
   st.put(pw_regs, G1, g);
   st.get(pw_regs, F0, x);
@@ -746,13 +759,13 @@ __device__ __forceinline__ void pw_srk(const PwProg<T>& pg, const PwSrkP<T> p, c
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     T o[2];
-    p.s2({y0[j], x[j], z[j], f[j], g[j]}, w[j], u[j], o);
+    s2({y0[j], x[j], z[j], f[j], g[j]}, w[j], u[j], o);
     h0[j] = o[0];
     h1[j] = o[1];
   }
   // s = 2: f2 at (t0 + dt/2, H0_2), g2 at (t0 + dt, H1_2); H1_3
-  pw_eval<EXT>(pg, c, pw_regs, false, p.t[3], h0, f);
-  pw_eval<EXT>(pg, c, pw_regs, true, p.t[1], h1, g);
+  pw_eval<EXT>(pg, c, pw_regs, false, t[3], h0, f);
+  pw_eval<EXT>(pg, c, pw_regs, true, t[1], h1, g);
   st.put(pw_regs, F2, f);
   st.put(pw_regs, G2, g);
   st.get(pw_regs, G0, x);
@@ -760,12 +773,12 @@ __device__ __forceinline__ void pw_srk(const PwProg<T>& pg, const PwSrkP<T> p, c
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     T o[1];
-    p.s3({y0[j], x[j], z[j], f[j], g[j]}, w[j], u[j], o);
+    s3({y0[j], x[j], z[j], f[j], g[j]}, w[j], u[j], o);
     h1[j] = o[0];
   }
   // s = 3: g3 at (t0 + dt/4, H1_3); y1
-  pw_eval<EXT>(pg, c, pw_regs, true, p.t[2], h1, g);
-  T f0[4], f1[4], f2[4], g0[4], g1[4], g2[4], y1[4];
+  pw_eval<EXT>(pg, c, pw_regs, true, t[2], h1, g);
+  T f0[4], f1[4], f2[4], g0[4], g1[4], g2[4];
   st.get(pw_regs, F0, f0);
   st.get(pw_regs, F1, f1);
   st.get(pw_regs, F2, f2);
@@ -775,9 +788,18 @@ __device__ __forceinline__ void pw_srk(const PwProg<T>& pg, const PwSrkP<T> p, c
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     T o[1];
-    p.fin({y0[j], f0[j], f1[j], f2[j], g0[j], g1[j], g2[j], g[j]}, w[j], u[j], o);
+    fin({y0[j], f0[j], f1[j], f2[j], g0[j], g1[j], g2[j], g[j]}, w[j], u[j], o);
     y1[j] = o[0];
   }
+}
+
+template <typename T, int SRC, bool EXT>
+__device__ __forceinline__ void pw_srk(const PwProg<T>& pg, const PwSrkP<T> p, const NoiseP<T> nz) {
+  extern __shared__ __align__(16) unsigned char pw_regs[];
+  PwQuad c;
+  T w[4], u[4], y0[4], y1[4];
+  if (!pw_begin<T, SRC, true>(pg, p.base, nz, pw_regs, c, w, u, y0)) return;
+  pw_srk_step<EXT>(pg, c, pw_regs, p.t, p.s1, p.s2, p.s3, p.fin, w, u, y0, y1);
   store_quad(p.base.y1, c.base, c.vec, c.nvalid, y1);
 }
 
@@ -817,31 +839,30 @@ struct PwPcP {
   T half_dt;
 };
 
-template <typename T, int SRC, int METHOD, bool EXT>
-__device__ __forceinline__ void pw_pc(const PwProg<T>& pg, const PwPcP<T> p, const NoiseP<T> nz) {
-  extern __shared__ __align__(16) unsigned char pw_regs[];
-  PwQuad c;
-  T w[4], u[4], y0[4];
-  if (!pw_begin<T, SRC, false>(pg, p.base, nz, pw_regs, c, w, u, y0)) return;
-  const T dt = p.base.dt;
+// One predictor-corrector step of METHOD from y0 on the increment w, evaluated at t0 and t_p: y1
+template <int METHOD, bool EXT, typename T>
+__device__ __forceinline__ void pw_pc_step(const PwProg<T>& pg, const PwQuad& c, void* pw_regs, const T* t0,
+                                           const T* t_p, T dt, T half_dt, const T (&w)[4], const T (&y0)[4],
+                                           T (&y1)[4]) {
+  const T u[4] = {};  // (the ops take no U)
   T f0[4], g0[4], yp[4];
-  pw_eval<EXT>(pg, c, pw_regs, false, p.base.t0, y0, f0);
-  pw_eval<EXT>(pg, c, pw_regs, true, p.base.t0, y0, g0);
+  pw_eval<EXT>(pg, c, pw_regs, false, t0, y0, f0);
+  pw_eval<EXT>(pg, c, pw_regs, true, t0, y0, g0);
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     T o[1];
     if constexpr (METHOD == TSDE_PC_HEUN) {
       EulerOp<T>{dt}({y0[j], f0[j], g0[j]}, w[j], u[j], o);                  // heun.py:42
     } else if constexpr (METHOD == TSDE_PC_MIDPOINT) {
-      MidpointPredictOp<T>{p.half_dt}({y0[j], f0[j], g0[j]}, w[j], u[j], o);  // midpoint.py:38
+      MidpointPredictOp<T>{half_dt}({y0[j], f0[j], g0[j]}, w[j], u[j], o);    // midpoint.py:38
     } else {
       EulerHeunPredictOp<T>{}({y0[j], g0[j]}, w[j], u[j], o);                // euler_heun.py:36
     }
     yp[j] = o[0];
   }
-  T f[4], g[4], y1[4];
-  if constexpr (METHOD != TSDE_PC_EULER_HEUN) pw_eval<EXT>(pg, c, pw_regs, false, p.t_p, yp, f);
-  pw_eval<EXT>(pg, c, pw_regs, true, p.t_p, yp, g);
+  T f[4], g[4];
+  if constexpr (METHOD != TSDE_PC_EULER_HEUN) pw_eval<EXT>(pg, c, pw_regs, false, t_p, yp, f);
+  pw_eval<EXT>(pg, c, pw_regs, true, t_p, yp, g);
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     T o[1];
@@ -854,6 +875,15 @@ __device__ __forceinline__ void pw_pc(const PwProg<T>& pg, const PwPcP<T> p, con
     }
     y1[j] = o[0];
   }
+}
+
+template <typename T, int SRC, int METHOD, bool EXT>
+__device__ __forceinline__ void pw_pc(const PwProg<T>& pg, const PwPcP<T> p, const NoiseP<T> nz) {
+  extern __shared__ __align__(16) unsigned char pw_regs[];
+  PwQuad c;
+  T w[4], u[4], y0[4], y1[4];
+  if (!pw_begin<T, SRC, false>(pg, p.base, nz, pw_regs, c, w, u, y0)) return;
+  pw_pc_step<METHOD, EXT>(pg, c, pw_regs, p.base.t0, p.t_p, p.base.dt, p.half_dt, w, y0, y1);
   store_quad(p.base.y1, c.base, c.vec, c.nvalid, y1);
 }
 
@@ -970,6 +1000,84 @@ pw_chunk_ext_kernel(const __grid_constant__ PwProg<T> pg, const PwChunkP<T> p, c
                     const __grid_constant__ PwSteps<T> st) {
   pw_chunk_steps<T, SRC, METHOD, true>(pg, p, nz, st);
 }
+
+// ---- an adaptive solve's proposal (tsde_adaptive_proposal_pointwise) ------------------------------------------------
+// The full step and the two half steps of Euler, SRK or a predictor-corrector method, each the step body of the
+// method's own kernel above, on increments read from memory (pw_milstein_proposal in pw_device.cuh is Milstein's).
+template <typename T>
+struct PwSrkOps {  // the stage ops of one SRK sub-step
+  SrkDiagStage1Op<T> s1;
+  SrkDiagStage2Op<T> s2;
+  SrkDiagStage3Op<T> s3;
+  SrkDiagFinalOp<T> fin;
+};
+
+template <typename T>
+struct PwProposalP {
+  PwP<T> base;  // y0, y1 (y_full), the quad mapping
+  T* y_next;
+  PwSubs<T> st;
+  PwSrkOps<T> srk[3];  // (SRK only)
+};
+
+// Sub-step k from y0: y1
+template <int METHOD, bool EXT, typename T>
+__device__ __forceinline__ void pw_sub_step(const PwProg<T>& pg, const PwQuad& c, void* pw_regs,
+                                            const PwProposalP<T>& p, int k, const T (&y0)[4], T (&y1)[4]) {
+  const PwSub<T>& s = p.st.sub[k];
+  T w[4];
+  load_quad(s.w, c.base, c.vec, c.nvalid, w);
+  if constexpr (METHOD == TSDE_PROPOSAL_SRK) {
+    T u[4];
+    load_quad(s.u, c.base, c.vec, c.nvalid, u);
+    const PwSrkOps<T>& o = p.srk[k];
+    pw_srk_step<EXT>(pg, c, pw_regs, s.t, o.s1, o.s2, o.s3, o.fin, w, u, y0, y1);
+  } else if constexpr (METHOD == TSDE_PROPOSAL_EULER) {
+    // (pw_chunk_steps' Euler step)
+    T f[4], g[4];
+    pw_eval<EXT>(pg, c, pw_regs, false, s.s.t0, y0, f);
+    pw_eval<EXT>(pg, c, pw_regs, true, s.s.t0, y0, g);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      T o[1];
+      EulerOp<T>{s.s.dt}({y0[j], f[j], g[j]}, w[j], T(0), o);
+      y1[j] = o[0];
+    }
+  } else {
+    constexpr int PC = METHOD == TSDE_PROPOSAL_HEUN       ? TSDE_PC_HEUN
+                       : METHOD == TSDE_PROPOSAL_MIDPOINT ? TSDE_PC_MIDPOINT
+                                                          : TSDE_PC_EULER_HEUN;
+    pw_pc_step<PC, EXT>(pg, c, pw_regs, s.s.t0, s.t[1], s.s.dt, s.half_dt, w, y0, y1);
+  }
+}
+
+template <typename T, int METHOD, bool EXT>
+__device__ __forceinline__ void pw_proposal(const PwProg<T>& pg, const PwProposalP<T>& p) {
+  extern __shared__ __align__(16) unsigned char pw_regs[];
+  PwQuad c;
+  int64_t Q, row, q;
+  pw_locate(p.base, c, Q, row, q);
+  // the increments are the Brownian queries that precede the launch: everything is read after the wait
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  pw_load_uniform(pg, pw_regs);
+  if (Q >= p.base.nquads) return;
+  T y0[4], y[4], ym[4];
+  load_quad(p.base.y0, c.base, c.vec, c.nvalid, y0);
+  pw_load_hoisted(pg, c, pw_regs);
+  pw_sub_step<METHOD, EXT>(pg, c, pw_regs, p, 0, y0, y);
+  store_quad(p.base.y1, c.base, c.vec, c.nvalid, y);
+  pw_sub_step<METHOD, EXT>(pg, c, pw_regs, p, 1, y0, ym);
+  pw_sub_step<METHOD, EXT>(pg, c, pw_regs, p, 2, ym, y);
+  store_quad(p.y_next, c.base, c.vec, c.nvalid, y);
+}
+
+template <typename T, int METHOD, bool EXT>
+__global__ void __launch_bounds__(kThreads, 1)
+pw_proposal_kernel(const __grid_constant__ PwProg<T> pg, const __grid_constant__ PwProposalP<T> p) {
+  pw_proposal<T, METHOD, EXT>(pg, p);
+}
+static_assert(sizeof(PwProg<double>) + sizeof(PwProposalP<double>) <= 4096,
+              "the proposal kernel's parameters fit the 4 KiB parameter space");
 
 // ---- launch ---------------------------------------------------------------------------------------------------------
 // The noise, the decoded program `pg` with the shared-memory slots its launch takes (`extra` past its layout), and the part of the kernel parameters every pointwise step has (y0, y1, the
@@ -1240,5 +1348,117 @@ TSDE_EXPORT int64_t tsde_pointwise_source(const tsde_launch* L, const tsde_point
       buf[n] = 0;
     }
     return (int64_t)src.size();
+  });
+}
+
+// ---- an adaptive solve's proposal -----------------------------------------------------------------------------------
+// The proposal's checks, made before anything is compiled or launched: a known method, sub-steps with the increments,
+// and the times, its method reads, a program of its method's layout.  Fills the sub-step table `st`.
+template <typename T>
+static int pw_proposal_table(const tsde_launch* L, const tsde_pointwise* prog, int32_t method, const void* y0,
+                             const tsde_pw_substep* subs, void* y_full, void* y_next, bool& vec, PwSubs<T>& st) {
+  if (method < TSDE_PROPOSAL_EULER || method > TSDE_PROPOSAL_EULER_HEUN || !prog || !y0 || !subs || !y_full ||
+      !y_next)
+    return TSDE_EINVAL;
+  const bool milstein = method == TSDE_PROPOSAL_MILSTEIN_ITO || method == TSDE_PROPOSAL_MILSTEIN_STRATONOVICH;
+  const int n_times = method == TSDE_PROPOSAL_SRK ? 4 : method >= TSDE_PROPOSAL_HEUN ? 2 : 1;
+  vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y_full) && aligned16(y_next);
+  st = PwSubs<T>{};
+  for (int k = 0; k < 3; ++k) {
+    const tsde_pw_substep& s = subs[k];
+    if (!s.w || (method == TSDE_PROPOSAL_SRK && !s.u)) return TSDE_EINVAL;
+    for (int i = 0; i < n_times; ++i)
+      if (!s.t[i]) return TSDE_EINVAL;
+    vec = vec && aligned16(s.w) && (method != TSDE_PROPOSAL_SRK || aligned16(s.u));
+    PwSub<T>& d = st.sub[k];
+    d.s = PwStep<T>{0, static_cast<const T*>(s.t[0]), nullptr, T(0), (T)s.dt};
+    d.w = static_cast<const T*>(s.w);
+    d.u = method == TSDE_PROPOSAL_SRK ? static_cast<const T*>(s.u) : nullptr;
+    for (int i = 0; i < 4; ++i) d.t[i] = i < n_times ? static_cast<const T*>(s.t[i]) : nullptr;
+    d.half_dt = (T)s.s[0];
+  }
+  if (!pw_valid_tables(*prog, &vec)) return TSDE_EINVAL;
+  const bool layout = milstein                       ? pw_valid_milstein(*prog)
+                      : method == TSDE_PROPOSAL_SRK ? pw_valid_two<TSDE_PW_SRK_MAX_REGS>(*prog)
+                                                     : pw_valid_two<TSDE_PW_MAX_REGS>(*prog);
+  return layout ? 0 : TSDE_EINVAL;
+}
+
+template <typename T>
+static int pw_proposal_launch(const tsde_launch* L, const tsde_pointwise* prog, int32_t method, const void* y0,
+                              const tsde_pw_substep* subs, void* y_full, void* y_next) {
+  bool vec;
+  PwProposalP<T> p{};
+  if (int e = pw_proposal_table<T>(L, prog, method, y0, subs, y_full, y_next, vec, p.st)) return e;
+  p.base.y0 = static_cast<const T*>(y0);
+  p.base.y1 = static_cast<T*>(y_full);
+  fill_quad_map(L->rows, L->d, p.base);
+  p.base.vec = vec ? 1 : 0;
+  p.y_next = static_cast<T*>(y_next);
+  const int64_t grid = (p.base.nquads + kThreads - 1) / kThreads;
+  if (method == TSDE_PROPOSAL_MILSTEIN_ITO || method == TSDE_PROPOSAL_MILSTEIN_STRATONOVICH) {
+    PwCompiled kc;
+    if (int e = pw_compiled(*prog, sizeof(T) == 8, kc, true)) return e;
+    PwOperands<T> ops{};
+    for (int k = 0; k < prog->n_operands; ++k)
+      ops.k[k] = PwOperand<T>{static_cast<const T*>(prog->operand[k].ptr), (T)prog->operand[k].imm};
+    p.base.ito = method == TSDE_PROPOSAL_MILSTEIN_ITO ? 1 : 0;
+    void* args[] = {&ops, &p.base, &p.y_next, &p.st};
+    const int e = launch_kernel_handle(kc.kernel[0], grid, kThreads, reinterpret_cast<cudaStream_t>(L->stream), args);
+    if (e == 0) g_launches[TSDE_KERNEL_PW_ADAPTIVE].fetch_add(1, std::memory_order_relaxed);
+    return e;
+  }
+  if (method == TSDE_PROPOSAL_SRK) {
+    for (int k = 0; k < 3; ++k) {
+      const tsde_pw_substep& s = subs[k];
+      const double dt = s.dt, rdt = s.s[0], sqrt_dt = s.s[1], three_dt = s.s[2];
+      // the coefficients of tsde_srk_diag_stage1/2/3 and tsde_step_srk_diag
+      p.srk[k] = PwSrkOps<T>{SrkDiagStage1Op<T>{(T)dt, (T)sqrt_dt}, SrkDiagStage2Op<T>{(T)dt, (T)rdt, (T)sqrt_dt},
+                             SrkDiagStage3Op<T>{(T)dt, (T)sqrt_dt}, make_srk_final<T>(dt, rdt, sqrt_dt, three_dt)};
+    }
+  }
+  PwProg<T> pg;
+  const int slots = pw_decode<T>(*prog, method == TSDE_PROPOSAL_SRK && PwSrkStash<T>::kShared ? kPwSrkStash : 0, pg);
+  void (*kernel)(PwProg<T>, PwProposalP<T>) = nullptr;
+  auto pick = [&](auto plain, auto ext) { kernel = pg.ext ? ext : plain; };
+  switch (method) {
+    case TSDE_PROPOSAL_EULER:
+      pick(pw_proposal_kernel<T, TSDE_PROPOSAL_EULER, false>, pw_proposal_kernel<T, TSDE_PROPOSAL_EULER, true>);
+      break;
+    case TSDE_PROPOSAL_SRK:
+      pick(pw_proposal_kernel<T, TSDE_PROPOSAL_SRK, false>, pw_proposal_kernel<T, TSDE_PROPOSAL_SRK, true>);
+      break;
+    case TSDE_PROPOSAL_HEUN:
+      pick(pw_proposal_kernel<T, TSDE_PROPOSAL_HEUN, false>, pw_proposal_kernel<T, TSDE_PROPOSAL_HEUN, true>);
+      break;
+    case TSDE_PROPOSAL_MIDPOINT:
+      pick(pw_proposal_kernel<T, TSDE_PROPOSAL_MIDPOINT, false>, pw_proposal_kernel<T, TSDE_PROPOSAL_MIDPOINT, true>);
+      break;
+    default:
+      pick(pw_proposal_kernel<T, TSDE_PROPOSAL_EULER_HEUN, false>,
+           pw_proposal_kernel<T, TSDE_PROPOSAL_EULER_HEUN, true>);
+      break;
+  }
+  const size_t smem = (size_t)slots * kThreads * 4 * sizeof(T);
+  if (resident_ctas(reinterpret_cast<const void*>(kernel), kThreads, smem) < 1) return TSDE_EINVAL;
+  const int e = launch_kernel(kernel, grid, kThreads, smem, reinterpret_cast<cudaStream_t>(L->stream), true, pg, p);
+  if (e == 0) g_launches[TSDE_KERNEL_PW_ADAPTIVE].fetch_add(1, std::memory_order_relaxed);
+  return e;
+}
+
+TSDE_EXPORT int tsde_adaptive_proposal_pointwise(const tsde_launch* L, const tsde_pointwise* prog, int32_t method,
+                                                 const void* y0, const tsde_pw_substep* subs, void* y_full,
+                                                 void* y_next) {
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
+  return dispatch(L, [&](auto t) -> int {
+    return pw_proposal_launch<decltype(t)>(L, prog, method, y0, subs, y_full, y_next);
+  });
+}
+
+TSDE_EXPORT int tsde_adaptive_pointwise_compile(const tsde_launch* L, const tsde_pointwise* prog) {
+  return dispatch(L, [&](auto t) -> int {
+    if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
+    PwCompiled kc;
+    return pw_compiled(*prog, sizeof(t) == 8, kc, true);
   });
 }

@@ -277,8 +277,31 @@ struct PwOperands {
   PwOperand<T> k[TSDE_PW_MAX_OPERANDS];
 };
 
-// Per step: the program's f / g part runs on y, MilsteinSeedOp forms go, the vjp part runs and MilsteinOp forms y1.
-// A quad's trajectory depends on nothing but its own state (element-wise SDE, diagonal noise), so one thread runs the
+// One Milstein step of a compiled program on this thread's quad: the program's f / g part runs on y at s.t0,
+// MilsteinSeedOp forms go from the increment w, the vjp part runs and MilsteinOp forms y1, which replaces y.
+template <typename T, typename Prog>
+__device__ __forceinline__ void pw_milstein_step(Prog& prog, const PwOperands<T>& ops, const PwQuad& c,
+                                                 const PwStep<T>& s, int32_t ito, const T (&w)[4], T (&y)[4]) {
+  T f[4], g[4], go[4], gdg[4];
+  prog.fg(ops, c, s, y, f, g);
+  const MilsteinSeedOp<T> seed{s.dt, ito};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    T o[1];
+    seed({g[i]}, w[i], T(0), o);
+    go[i] = o[0];
+  }
+  prog.vjp(ops, c, s, y, go, gdg);
+  const MilsteinOp<T> step{s.dt};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    T o[1];
+    step({y[i], f[i], g[i], gdg[i]}, w[i], T(0), o);
+    y[i] = o[0];
+  }
+}
+
+// Per step: pw_milstein_step on the state the step before left in registers.  A quad's trajectory depends on nothing but its own state (element-wise SDE, diagonal noise), so one thread runs the
 // whole chunk: y0 is read once, y stays in registers from one step to the next and is stored only where the step table
 // gives it a destination (an output row, the chunk's last state).  The unfused step moves 13 tensors; a chunk moves one
 // read and the stores it is asked for.
@@ -310,25 +333,52 @@ __device__ __forceinline__ void pw_milstein_steps(const PwOperands<T>& ops, cons
       load_quad(p.y0, c.base, c.vec, c.nvalid, y);
       prog.load(ops, c);
     }
-    T f[4], g[4], go[4], gdg[4];
-    prog.fg(ops, c, s, y, f, g);
-    const MilsteinSeedOp<T> seed{s.dt, p.ito};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      T o[1];
-      seed({g[i]}, w[i], u[i], o);
-      go[i] = o[0];
-    }
-    prog.vjp(ops, c, s, y, go, gdg);
-    const MilsteinOp<T> step{s.dt};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      T o[1];
-      step({y[i], f[i], g[i], gdg[i]}, w[i], u[i], o);
-      y[i] = o[0];
-    }
+    pw_milstein_step<T>(prog, ops, c, s, p.ito, w, y);
     if (s.y1) store_quad(s.y1, c.base, c.vec, c.nvalid, y);
   }
+}
+
+// ---- an adaptive solve's step-doubling proposal (tsde_adaptive_proposal_pointwise) -----------------------------------
+// Three sub-steps of one method on increments read from memory: the full step from y0, the first half step from y0
+// and the second half step from the midpoint state, which stays in registers.  Only the full step's and the second
+// half step's results are stored.
+template <typename T>
+struct PwSub {
+  PwStep<T> s;     // s.t0 (the time the program runs at) and s.dt; cell, sqrt_h and y1 unused
+  const T* w;      // (rows, d) increment
+  const T* u;      // (rows, d) space-time Levy area (SRK), or null
+  const T* t[4];   // the sub-step's other times (SRK's stage times; the predictor-corrector's t_p in t[1])
+  T half_dt;       // midpoint's predictor scalar
+};
+template <typename T>
+struct PwSubs {  // by value: the three sub-steps, in order full, first half, second half
+  PwSub<T> sub[3];
+};
+
+// The compiled Milstein variant: y_full and y_next as pw_milstein_step gives them from the increments sub[k].w.
+template <typename T, typename Prog>
+__device__ __forceinline__ void pw_milstein_proposal(const PwOperands<T>& ops, const PwP<T>& p, T* y_next,
+                                                     const PwSubs<T>& st) {
+  PwQuad c;
+  int64_t Q, row, q;
+  pw_locate(p, c, Q, row, q);
+  // the increments are the Brownian queries that precede the launch: everything is read after the wait
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (Q >= p.nquads) return;
+  Prog prog;
+  T y0[4], y[4], w[4];
+  load_quad(p.y0, c.base, c.vec, c.nvalid, y0);
+  prog.load(ops, c);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) y[i] = y0[i];
+  load_quad(st.sub[0].w, c.base, c.vec, c.nvalid, w);
+  pw_milstein_step<T>(prog, ops, c, st.sub[0].s, p.ito, w, y);
+  store_quad(p.y1, c.base, c.vec, c.nvalid, y);
+  load_quad(st.sub[1].w, c.base, c.vec, c.nvalid, w);
+  pw_milstein_step<T>(prog, ops, c, st.sub[1].s, p.ito, w, y0);
+  load_quad(st.sub[2].w, c.base, c.vec, c.nvalid, w);
+  pw_milstein_step<T>(prog, ops, c, st.sub[2].s, p.ito, w, y0);
+  store_quad(y_next, c.base, c.vec, c.nvalid, y0);
 }
 
 }  // namespace tsde
