@@ -138,7 +138,11 @@ const char* tsde_error_string(int code);
                                      tsde_solve_reversible_heun_pointwise)                                      */
 #define TSDE_KERNEL_PW_ADAPTIVE 7 /* an adaptive solve's proposal with an element-wise SDE, the full step and both
                                      half steps in one launch (tsde_adaptive_proposal_pointwise)                */
+#define TSDE_KERNEL_PW_GENERAL 8  /* general / additive-noise Euler steps or a midpoint step with an element-wise
+                                     SDE (tsde_solve_euler_general_pointwise,
+                                     tsde_step_midpoint_general_pointwise)                                       */
 int64_t tsde_kernel_launches(int32_t family);
+
 
 /* ------------------------------------------------------------------------ */
 /* Brownian source  (replaces torchsde/_brownian/brownian_interval.py)       */
@@ -466,6 +470,42 @@ typedef struct tsde_pw_substep {
 int tsde_adaptive_proposal_pointwise(const tsde_launch* L, const tsde_pointwise* prog, int32_t method,
                                      const void* y0, const tsde_pw_substep* subs, void* y_full, void* y_next);
 int tsde_adaptive_pointwise_compile(const tsde_launch* L, const tsde_pointwise* prog);
+
+/*
+ * General and additive noise.  tsde_solve_euler_pointwise, tsde_step_predictor_corrector_pointwise with
+ * TSDE_PC_MIDPOINT, tsde_pointwise_compile and tsde_pointwise_source also take a GENERAL launch with
+ * 1 <= L->m <= TSDE_PW_GENERAL_MAX_M, for an SDE whose f(t, y) is a (rows, d) element-wise program and whose g(t, y)
+ * is a (rows, d, m) one, built from the same ops:
+ *   tsde_solve_euler_pointwise               consecutive Euler steps, y1 = (y0 + f*dt) + g.dW as tsde_step_euler;
+ *   tsde_step_predictor_corrector_pointwise  one midpoint step: y' as tsde_midpoint_predict (half_dt) at (t0, y0), y1
+ *                                            as tsde_step_euler (dt) on f, g at (t_p, y'); other methods: TSDE_EINVAL.
+ * Each thread owns a quad of d of one row; it draws the row's m increments on the channel-quad counters of the
+ * general-noise kernels, evaluates g_ij in registers, channel by channel, and contracts it with them in the order the
+ * unfused tsde_step_euler / tsde_midpoint_predict launch takes for a contiguous g (aligned unless g is a TSDE_PW_DM
+ * operand at an unaligned address):
+ *   m == 1                              one product g * dW (the row-wise kernels);
+ *   m / 4 a power of two <= 32          per channel quad a fused multiply-add chain from 0, the quad sums added as a
+ *                                       pairwise tree in natural order (the tile kernels);
+ *   otherwise                           left to right from 0, one rounded multiply and add per channel;
+ * so g never exists in memory and every stored state equals the unfused step's bit for bit.  The launches count
+ * under TSDE_KERNEL_PW_GENERAL.
+ *
+ * Program: the two-program layout of tsde_step_predictor_corrector_pointwise, tagged reserved =
+ * TSDE_PW_LAYOUT_GENERAL (an untagged program on a GENERAL launch is TSDE_EINVAL), with two more operand kinds that
+ * only the g program may read:
+ *   DM  ptr[channel * m + k]   (a dense (d, m) tensor broadcast over the rows)
+ *   M   ptr[k]                 (an (m,) tensor broadcast over the rows and d)
+ * where k is the Brownian channel.  A value computed from a DM or M operand is per channel; every other value, f's
+ * result among them, is per (row, d) element and broadcast along m.  g_src may be any source, an operand included
+ * (additive noise, `sigma.expand(rows, d, m)`).  As a Milstein program, it is compiled at run time into kernels of its
+ * own (one translation unit per structure, dtype, m and contraction order, holding both methods' kernels), which
+ * tsde_pointwise_compile compiles and loads and tsde_pointwise_source writes out for a GENERAL launch.  Counter noise
+ * only, no 16-bit formats and no launch flags.  TSDE_EINVAL additionally: m outside [1, TSDE_PW_GENERAL_MAX_M] and a
+ * DM or M operand read by f.
+ */
+#define TSDE_PW_GENERAL_MAX_M 32
+enum { TSDE_PW_DM = 5, TSDE_PW_M = 6 };
+#define TSDE_PW_LAYOUT_GENERAL 1 /* tsde_pointwise.reserved of a general-layout program (0 for every other layout) */
 
 /* derivative-free Milstein, predictor: y' = y0 + (Ito ? dt*f : 0) + g*sqrt_dt
  * methods/milstein.py:58-63,83-84,93-94.  g is (rows,d) also for scalar noise (squeezed). */

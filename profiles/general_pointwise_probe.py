@@ -1,0 +1,94 @@
+"""Fused against unfused general-noise solves (tsde_solve_euler_general_pointwise, tsde_step_midpoint_general_pointwise):
+correlated multi-asset GBM, f = mu * y, g = y.unsqueeze(-1) * S, as captured graphs.  The unfused run is the same
+solve with the tape rejected.  Both are alternated three times in one process; prints ms per solve and us per step,
+with the SM clock and power limit read in the same call.
+
+    python profiles/general_pointwise_probe.py
+"""
+import contextlib
+import json
+import os
+import subprocess
+import sys
+
+import torch
+from torch import nn
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import torchsde_b200 as tsde  # noqa: E402
+from torchsde_b200._core import pointwise  # noqa: E402
+
+DEV = 'cuda'
+
+
+class CorrelatedGBM(nn.Module):
+    noise_type = 'general'
+
+    def __init__(self, d, m, sde_type):
+        super().__init__()
+        gen = torch.Generator().manual_seed(0)
+        self.sde_type = sde_type
+        self.mu = nn.Parameter(torch.rand(d, generator=gen) * 0.1)
+        self.S = nn.Parameter(torch.rand(d, m, generator=gen) * (0.3 / m ** 0.5))
+
+    def f(self, t, y):
+        return self.mu * y
+
+    def g(self, t, y):
+        return y.unsqueeze(-1) * self.S
+
+
+@contextlib.contextmanager
+def unfused():
+    finish = pointwise.SrkRecorder.finish
+    pointwise.SrkRecorder.finish = lambda self: None
+    try:
+        yield
+    finally:
+        pointwise.SrkRecorder.finish = finish
+
+
+def clocks():
+    try:
+        out = subprocess.run(['nvidia-smi', '--query-gpu=clocks.sm,power.limit', '--format=csv,noheader'],
+                             capture_output=True, text=True, timeout=10).stdout.strip()
+        return out.splitlines()[0] if out else 'n/a'
+    except Exception:
+        return 'n/a'
+
+
+def timed(B, d, m, T, method, fused, reps=5):
+    sde = CorrelatedGBM(d, m, 'ito' if method == 'euler' else 'stratonovich').to(DEV)
+    y0 = torch.full((B, d), 1.0, device=DEV)
+    dt = 2.0 ** -8
+    ts = torch.tensor([0.0, T * dt], device=DEV)
+    ctx = contextlib.nullcontext() if fused else unfused()
+    with ctx, torch.no_grad():
+        bm = tsde.BrownianInterval(0.0, T * dt, size=(B, m), device=DEV, entropy=1)
+        tsde.sdeint(sde, y0, ts, bm=bm, method=method, dt=dt, options={'cuda_graph': True})  # record, capture
+        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        start.record()
+        for _ in range(reps):
+            tsde.sdeint(sde, y0, ts, bm=bm, method=method, dt=dt, options={'cuda_graph': True})
+        end.record()
+        torch.cuda.synchronize()
+    return start.elapsed_time(end) / reps
+
+
+def main():
+    cases = [('euler', 8192, 32, 16, 500), ('euler', 65536, 64, 16, 100), ('midpoint', 8192, 32, 16, 500)]
+    print(json.dumps({'gpu': torch.cuda.get_device_name(), 'clocks_sm_power_limit': clocks()}))
+    for method, B, d, m, T in cases:
+        res = {'fused': [], 'unfused': []}
+        for _ in range(3):
+            for fused in (True, False):
+                res['fused' if fused else 'unfused'].append(timed(B, d, m, T, method, fused))
+        for k, v in res.items():
+            print(json.dumps({'method': method, 'B': B, 'd': d, 'm': m, 'T': T, 'path': k,
+                              'ms_per_solve': [round(x, 3) for x in v],
+                              'us_per_step': [round(1000 * x / T, 2) for x in v]}))
+    print(json.dumps({'clocks_sm_power_limit_after': clocks()}))
+
+
+if __name__ == '__main__':
+    main()

@@ -54,6 +54,29 @@ def compile_pointwise(prog, dtype):
     return lib().tsde_pointwise_compile(ctypes.byref(_program_launch(dtype)), ctypes.byref(prog))
 
 
+def _general_launch(dtype, d, m):
+    # (a one-row general launch: what tsde_pointwise_source / _compile read of it is the dtype, d and m)
+    return Launch(dtype_code(dtype), NOISE_GENERAL, 1, d, m, None)
+
+
+def general_pointwise_source(prog, dtype, d, m):
+    """The CUDA source the library compiles for general-noise program `prog` in `dtype` with m Brownian channels, or None
+    if the library refuses the program (tsde_pointwise_source on a GENERAL launch; no device needed)."""
+    L = _general_launch(dtype, d, m)
+    n = lib().tsde_pointwise_source(ctypes.byref(L), ctypes.byref(prog), None, 0)
+    if n < 0:
+        return None
+    buf = ctypes.create_string_buffer(n + 1)
+    lib().tsde_pointwise_source(ctypes.byref(L), ctypes.byref(prog), buf, n + 1)
+    return buf.value.decode()
+
+
+def compile_general_pointwise(prog, dtype, d, m):
+    """tsde_pointwise_compile on a GENERAL launch: compile and load the Euler and midpoint kernels of general-noise
+    program `prog`; 0 or an error code."""
+    return lib().tsde_pointwise_compile(ctypes.byref(_general_launch(dtype, d, m)), ctypes.byref(prog))
+
+
 def compile_adaptive_pointwise(prog, dtype):
     """tsde_adaptive_pointwise_compile: compile and load the adaptive proposal kernel of Milstein program `prog` in
     `dtype`; 0 or an error code."""
@@ -80,13 +103,16 @@ PW_MAX_INSTR, PW_MAX_OPERANDS, PW_MAX_REGS = 96, 24, 24  # TSDE_PW_MAX_*
 PW_SRC_Y, PW_SRC_GO, PW_OPERAND0 = 0xFE, 0xFF, 0x80
 PW_MUL, PW_ADD, PW_SUB, PW_DIV, PW_NEG, PW_SQRT = range(6)
 PW_LT, PW_LE, PW_EQ, PW_MAXIMUM, PW_MINIMUM, PW_ABS, PW_SEL = range(8, 15)  # (6, 7 reserved)
-PW_IMM, PW_T0, PW_SCALAR, PW_CHANNEL, PW_ROW = range(5)
+PW_IMM, PW_T0, PW_SCALAR, PW_CHANNEL, PW_ROW, PW_DM, PW_M = range(7)  # (DM, M: the general layout's g only)
 PW_SRK_MAX_REGS = 18  # TSDE_PW_SRK_MAX_REGS
 KERNEL_PW_MILSTEIN = 3  # TSDE_KERNEL_PW_MILSTEIN
 KERNEL_PW_SRK = 4  # TSDE_KERNEL_PW_SRK
 KERNEL_PW_PC = 5  # TSDE_KERNEL_PW_PC
 KERNEL_PW_CHUNK = 6  # TSDE_KERNEL_PW_CHUNK
 KERNEL_PW_ADAPTIVE = 7  # TSDE_KERNEL_PW_ADAPTIVE
+KERNEL_PW_GENERAL = 8  # TSDE_KERNEL_PW_GENERAL
+PW_GENERAL_MAX_M = 32  # TSDE_PW_GENERAL_MAX_M
+PW_LAYOUT_GENERAL = 1  # TSDE_PW_LAYOUT_GENERAL: Pointwise.reserved of a general-noise program
 # TSDE_PROPOSAL_*: the method of tsde_adaptive_proposal_pointwise
 (PROPOSAL_EULER, PROPOSAL_MILSTEIN_ITO, PROPOSAL_MILSTEIN_STRATONOVICH, PROPOSAL_SRK, PROPOSAL_HEUN, PROPOSAL_MIDPOINT,
  PROPOSAL_EULER_HEUN) = range(7)

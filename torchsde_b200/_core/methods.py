@@ -98,6 +98,7 @@ class Euler(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
     levy_area_approximations = LEVY_AREA_APPROXIMATIONS.all()
 
     _pw_method = 'euler'
+    _pw_general = True  # general / additive noise fuses too (pointwise.general)
 
     def __init__(self, sde, **kwargs):
         self.strong_order = 1.0 if sde.noise_type == NOISE_TYPES.additive else 0.5
@@ -118,7 +119,9 @@ class Euler(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
         # the first step of an eligible solve runs as always, with the user's two evaluations recorded
         rec = pointwise.pc_recorder(self, y0, c.t0, 'fg')
         L, nz, f, g = self._f_and_g_prod(c, c.t0, y0, rec)
-        if rec is not None:
+        if isinstance(rec, pointwise.GeneralRecorder):
+            self._pw = pointwise.compile_general(self, rec, rec.finish()) or False
+        elif rec is not None:
             self._pw = rec.finish() or False
         return self._k('tsde_step_euler', L, nz, (y0, f, g), (c.dt,), out), ()
 
@@ -273,6 +276,8 @@ class Midpoint(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
     noise_types = NOISE_TYPES.all()
     levy_area_approximations = LEVY_AREA_APPROXIMATIONS.all()
 
+    _pw_general = True  # general / additive noise fuses too (pointwise.general)
+
     def __init__(self, sde, **kwargs):
         self.strong_order = 0.5 if sde.noise_type == NOISE_TYPES.general else 1.0
         super(Midpoint, self).__init__(sde=sde, **kwargs)
@@ -286,7 +291,8 @@ class Midpoint(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
 
     def _step(self, c, y0, extra0, out):
         if pointwise.ready(self):
-            # f and g were recorded as element-wise programs (pointwise.py): the whole step is one kernel
+            # f and g were recorded as element-wise programs (pointwise.py): the whole step is one kernel (for
+            # general / additive noise, on the solver's GENERAL launch)
             return pointwise.launch(self, 'tsde_step_predictor_corrector_pointwise', self._feed.get(c), y0,
                                     (c.t0.data_ptr(), c.aux_t[0].data_ptr(), _cabi.PC_MIDPOINT, c.dt,
                                      c.scalars['half_dt']), out), ()
@@ -295,7 +301,9 @@ class Midpoint(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
         L, nz, f, g = self._f_and_g_prod(c, c.t0, y0, rec)
         yp = self._k('tsde_midpoint_predict', L, nz, (y0, f, g), (c.scalars['half_dt'],), None)
         L, nz, fp, gp = self._f_and_g_prod(c, c.aux_t[0], yp, rec)
-        if rec is not None:
+        if isinstance(rec, pointwise.GeneralRecorder):
+            self._pw = pointwise.compile_general(self, rec, rec.finish()) or False
+        elif rec is not None:
             self._pw = rec.finish() or False
         return self._k('tsde_step_euler', L, nz, (y0, fp, gp), (c.dt,), out), ()
 

@@ -91,6 +91,13 @@ steps and its queries are the unfused solve's, bit for bit.  The conditions are 
 motion whose answers have the state's shape in place of the grid binding; gradients through the solve and the
 backward solve of `sdeint_adjoint` keep the unfused steps.  Reversible Heun keeps them too: its solver state carries
 over from one proposal to the next.
+
+General and additive noise (`GeneralRecorder`, `general`, `compile_general`).  Fixed-step Euler and midpoint solves
+with 1 <= m <= TSDE_PW_GENERAL_MAX_M Brownian channels record f as above and g as a (rows, d, m) value of the same ops,
+with per-channel operands ((d, m) and (m,) tensors) and `y.unsqueeze(-1)`; the program is compiled into kernels of its
+own that evaluate g_ij in registers and contract it with the increments in the unfused launch's summation order, and
+they run on the solver's GENERAL launch of tsde_solve_euler_pointwise (chunks, as Euler's) and
+tsde_step_predictor_corrector_pointwise (midpoint).  Every other method keeps diagonal-only tapes.
 """
 import ctypes
 import numbers
@@ -638,11 +645,166 @@ class SrkRecorder(Recorder):
             return None
 
 
+def _pad3(shape):
+    return (1,) * (3 - len(shape)) + tuple(shape)
+
+
+class GeneralRecorder(SrkRecorder):
+    """Records the f and g evaluations of a general- or additive-noise Euler ('fg') or midpoint ('fgfg') step, whose
+    g is (rows, d, m).  A value is either of the (rows, d) class of the diagonal tapes or per channel: computed by an
+    op whose result is three-dimensional, or not of a (rows, d) shape, or that reads a per-channel value (`_wide`).
+    Per-channel ops broadcast as torch does, right-aligned on (rows, d, m), and may read
+      * per-channel values;
+      * (rows, d)-class values only through `unsqueeze(-1)` (`y[..., None]`), as (rows, d, 1), or when they have one
+        element: a lifted tensor (`_lifted`) keeps the element mapping of its value, broadcast along m;
+      * device tensors by their layout broadcast to (rows, d, m): one element (SCALAR), a (d, 1) column (CHANNEL),
+        an (m,) row (M), a dense (d, m) block (DM); a (rows, d, m) tensor from outside the tape rejects it.
+    f must be of the (rows, d) class; g must have the shape (rows, d, m) and may be any of those (an operand's
+    `expand` is additive noise).  The kernel derives which instructions are per channel from their sources alone."""
+
+    def __init__(self, y, t, pattern, m):
+        self.m = m
+        self._wide = set()     # the per-channel values
+        self._lifted = set()   # id() of (rows, d)-class tensors viewed as (..., 1)
+        self._w3 = False       # the op being recorded is per channel
+        self._kind = None      # the evaluation being recorded, 'f' or 'g'
+        super().__init__(y, t, pattern, _cabi.PW_MAX_REGS)
+
+    # -- the op's class ------------------------------------------------------------------------------------------
+    def _is_bound(self, x):
+        return torch.is_tensor(x) and (id(x) in self._by_obj or self._addr(x) in self._by_addr)
+
+    def _per_channel_input(self, x):
+        if not torch.is_tensor(x):
+            return False
+        src = self._by_obj.get(id(x)) or self._by_addr.get(self._addr(x))
+        return src in self._wide or (src is None and x.dim() == 3)
+
+    def _record(self, func, args, kwargs, out):
+        tensors = [a for a in list(args) + list(kwargs.values()) if torch.is_tensor(a)]
+        self._w3 = torch.is_tensor(out) and (out.dim() == 3 or _strip(out.shape) not in self._shapes or
+                                             any(self._per_channel_input(a) for a in tensors))
+        if func in _ALIAS and self._w3:
+            self._alias3(args[0], out)
+            return
+        super()._record(func, args, kwargs, out)
+
+    def _alias3(self, x, out):
+        """A view in a per-channel context: a view of an unbound tensor is classified where it is read; a view of a
+        value keeps the value's element mapping when it only adds broadcast axes."""
+        if not self._is_bound(x):
+            return
+        src = SrkRecorder._source(self, x)  # (the view decides below how the tensor may be read)
+        if src[0] == 'k':
+            return
+        lifted = src not in self._wide
+        if lifted:
+            if id(x) in self._lifted:
+                old = _pad3(x.shape)
+            elif tuple(out.shape) == tuple(x.shape) + (1,) and _strip(x.shape) in self._shapes:
+                old = _pad3(tuple(x.shape) + (1,))  # unsqueeze(-1): the (rows, d) class as (rows, d, 1)
+            elif x.numel() == 1:
+                old = (1, 1, 1)
+            else:
+                raise Reject(f"a (rows, d) value viewed as {tuple(out.shape)}")
+        else:
+            old = _pad3(x.shape)
+        if out.dim() > 3 or any(a not in (1, b) for a, b in zip(old, _pad3(out.shape))):
+            raise Reject(f"a view {tuple(x.shape)} -> {tuple(out.shape)} that moves elements")
+        self._result(out, src in self._bools)
+        self._bind(out, src)
+        if lifted:
+            self._lifted.add(id(out))
+
+    def _result(self, out, boolean=False):
+        if not self._w3:
+            return super()._result(out, boolean)
+        want = torch.bool if boolean else self.dtype
+        if not torch.is_tensor(out) or out.dtype != want or out.device != self.device:
+            raise Reject("result is not a tensor of the state dtype")
+        if out.dim() > 3 or any(a not in (1, b) for a, b in zip(_pad3(out.shape), (self.rows, self.d, self.m))):
+            raise Reject(f"result of shape {tuple(out.shape)}")
+
+    def _value(self, op, a, b=None, cond=None, boolean=False):
+        v = super()._value(op, a, b, cond, boolean)
+        if self._w3:
+            self._wide.add(v)
+        return v
+
+    def _source(self, x):
+        if not self._w3 or not torch.is_tensor(x):
+            return super()._source(x)
+        src = self._by_obj.get(id(x)) or self._by_addr.get(self._addr(x))
+        if src is None and not (x.device.type == 'cpu' and x.dim() == 0):
+            return self._operand3(x)
+        src = super()._source(x)
+        if src in self._wide or src[0] == 'k' or x.numel() == 1 or id(x) in self._lifted:
+            return src
+        raise Reject(f"a (rows, d) value of shape {tuple(x.shape)} is read per channel")
+
+    def _operand3(self, x):
+        """A device tensor read per channel, by its layout broadcast right-aligned to (rows, d, m)."""
+        if x.device != self.device or x.dtype != self.dtype or x.requires_grad and x.grad_fn is not None:
+            raise Reject(f"operand {tuple(x.shape)} {x.dtype} on {x.device}")
+        if x.dim() > 3:
+            raise Reject(f"operand of shape {tuple(x.shape)}")
+        if x.untyped_storage().data_ptr() in self._storage.values():
+            raise Reject("an operand shares storage with a value of the tape")
+        shape, stride = _pad3(x.shape), (0,) * (3 - x.dim()) + tuple(x.stride())
+        (a, b, c), (_, sb, sc) = shape, [s if n > 1 else 0 for n, s in zip(shape, stride)]
+        if a > 1 and stride[0] != 0 or b not in (1, self.d) or c not in (1, self.m):
+            raise Reject(f"operand of shape {tuple(x.shape)} read per channel")
+        if b > 1 and c > 1:
+            kind, ok = _cabi.PW_DM, sb == c and sc == 1
+        elif b > 1:
+            kind, ok = _cabi.PW_CHANNEL, sb == 1
+        elif c > 1:
+            kind, ok = _cabi.PW_M, sc == 1
+        else:
+            kind, ok = _cabi.PW_SCALAR, True
+        if not ok:
+            raise Reject(f"operand of shape {tuple(x.shape)} and strides {tuple(x.stride())} is not dense")
+        self._keep.append(x)
+        return self._operand(kind, x.data_ptr(), 0.0)
+
+    # -- the results -------------------------------------------------------------------------------------------
+    def evaluation(self, kind, fn, t, y):
+        self._w3, self._kind = False, kind
+        return super().evaluation(kind, fn, t, y)
+
+    def _program(self, code, n_fg, results, n_regs, max_regs):
+        prog, keep = super()._program(code, n_fg, results, n_regs, max_regs)
+        prog.reserved = _cabi.PW_LAYOUT_GENERAL
+        return prog, keep
+
+    def _step_result(self, t, allow_go=False):
+        if self._kind == 'f':
+            self._w3 = False
+            src = super()._step_result(t)
+            if src in self._wide:
+                raise Reject("f is computed per channel")
+            return src
+        if tuple(t.shape) != (self.rows, self.d, self.m) or t.dtype != self.dtype:
+            raise Reject("g is not a (rows, d, m) tensor of the state dtype")
+        self._w3 = True
+        return self._source(t)
+
+
 def recording(solver):
     """Whether this step of `solver` (its `_pw` is the program, None before the first step, False once rejected)
     is the one to record: the first diagonal-noise step of an `eligible` solve (for reversible Heun, the first whose
-    solver state the chunk kernel can read, methods.ReversibleHeun)."""
-    return solver._pw is None and solver.sde.noise_type == NOISE_TYPES.diagonal and eligible(solver)
+    solver state the chunk kernel can read, methods.ReversibleHeun), or the first general- or additive-noise step of
+    one that `general` serves."""
+    return solver._pw is None and (solver.sde.noise_type == NOISE_TYPES.diagonal or general(solver)) and \
+        eligible(solver)
+
+
+def general(solver):
+    """Whether `solver` runs general- or additive-noise steps that the element-wise general kernels serve: a fixed-step
+    Euler or midpoint solve (`_pw_general`) with 1 <= m <= TSDE_PW_GENERAL_MAX_M Brownian channels."""
+    return (getattr(solver, '_pw_general', False) and not solver.adaptive
+            and solver.sde.noise_type in (NOISE_TYPES.general, NOISE_TYPES.additive)
+            and 1 <= solver.m <= _cabi.PW_GENERAL_MAX_M)
 
 
 def pc_recorder(solver, y, t, pattern):
@@ -653,7 +815,25 @@ def pc_recorder(solver, y, t, pattern):
     if (not recording(solver) or sde.f_and_g_prod_mode != 'fused' or sde.g_prod_mode != 'fused'
             or getattr(sde, 'user_f_and_g', True) or getattr(sde, 'is_adjoint_sde', False)):
         return None
+    if sde.noise_type != NOISE_TYPES.diagonal:
+        return GeneralRecorder(y, t, pattern, solver.m)
     return SrkRecorder(y, t, pattern, _cabi.PW_MAX_REGS)
+
+
+def compile_general(solver, rec, res):
+    """`res`, what a GeneralRecorder's `finish` returned, once the Euler and midpoint kernels of its program are compiled
+    and loaded (tsde_pointwise_compile on the solver's GENERAL launch), on the recording step as for
+    `compile_milstein`; None if `res` is, or if the library refuses or cannot compile the program (the tape is then
+    rejected with the reason)."""
+    global COMPILES
+    if res is None:
+        return None
+    err = _cabi.compile_general_pointwise(res[0], rec.dtype, solver.d, solver.m)
+    if err != 0:
+        rec.reject(_cabi.lib().tsde_error_string(err).decode())
+        return None
+    COMPILES += 1
+    return res
 
 
 def ready(solver):
@@ -665,6 +845,7 @@ def launch(solver, name, nz, y0, args, out):
     """One step y0 -> out of the library's whole-step function `name` on the solver's program."""
     prog, _ = solver._pw
     out = out if out is not None else torch.empty_like(y0)
+    solver._feed._nz.flags = 0  # (an unfused general step may have left TSDE_FLAG_G_BROADCAST; g is not an operand)
     fn = getattr(solver._lib, name)
     _cabi.check(fn(solver._L, nz, ctypes.byref(prog), y0.data_ptr(), *args, out.data_ptr()), name)
     return out
@@ -690,7 +871,8 @@ def plan_chunks(first, n_steps, interpolated=(), multi_cell=(), max_steps=_cabi.
 # Resident CTAs (256 threads) per SM of each chunked kernel, (float32, float64), from its registers (-Xptxas -v,
 # sm_90a: 64 K registers per SM): Milstein's compiled kernels are pinned there by their launch bounds (256, 4) and
 # (256, 2) (cfg2's program: 41 registers in fp32); Euler at 54 and 88-96; reversible Heun at 72 and 110-120.
-_RESIDENT_CTAS = {'milstein': (4, 2), 'euler': (4, 2), 'reversible_heun': (3, 2)}
+# The compiled general-noise Euler kernels are bounded at (256, 1): at least one resident CTA, whatever m.
+_RESIDENT_CTAS = {'milstein': (4, 2), 'euler': (4, 2), 'reversible_heun': (3, 2), 'euler_general': (1, 1)}
 
 
 def chunk_length(solver):
@@ -703,8 +885,9 @@ def chunk_length(solver):
     if solver.device.type != 'cuda':  # (the host-side dry run of the tests; a solve always runs on a CUDA device)
         return _cabi.PW_MAX_STEPS
     ctas = solver.rows * ((solver.d + 3) // 4) / 256
+    method = solver._pw_method + ('_general' if solver.sde.noise_type != NOISE_TYPES.diagonal else '')
     wave = torch.cuda.get_device_properties(solver.device).multi_processor_count * (
-        _RESIDENT_CTAS[solver._pw_method][0 if solver.dtype == torch.float32 else 1])
+        _RESIDENT_CTAS[method][0 if solver.dtype == torch.float32 else 1])
     return _cabi.PW_MAX_STEPS if ctas >= wave else 1
 
 
@@ -716,6 +899,7 @@ def solve_chunk(solver, ctxs, y0, outs, method, ito=0, state=None):
     prog, _ = solver._pw
     feed = solver._feed
     nz = feed.get(ctxs[0])
+    feed._nz.flags = 0  # (an unfused general step may have left TSDE_FLAG_G_BROADCAST; g is not an operand)
     steps = (_cabi.PwStep * len(ctxs))()
     for s, c, out in zip(steps, ctxs, outs):
         s.cell_id, s.h, _ = feed.binding.cell(c.k)
@@ -726,7 +910,7 @@ def solve_chunk(solver, ctxs, y0, outs, method, ito=0, state=None):
     name = f'tsde_solve_{method}_pointwise'
     if method == 'milstein':
         code = lib.tsde_solve_milstein_pointwise(*args, steps, len(ctxs), ito)
-    elif method == 'euler':
+    elif method == 'euler':  # (diagonal, or general / additive noise on the solver's GENERAL launch)
         code = lib.tsde_solve_euler_pointwise(*args, steps, len(ctxs))
     else:
         state_in, state_out = state

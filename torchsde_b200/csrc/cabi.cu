@@ -6,7 +6,7 @@
 using namespace tsde;
 
 static inline bool rowwise(const tsde_launch* L) {
-  return L->noise_type == TSDE_NOISE_DIAGONAL || L->m == 1;
+  return L->noise_type == TSDE_NOISE_DIAGONAL || gen_route(L->m, false, 0) == TSDE_GEN_ROWWISE;
 }
 
 // A valid launch of a known noise layout (diagonal noise has m == d), with launch flags the routed kernels understand:

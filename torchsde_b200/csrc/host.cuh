@@ -27,8 +27,20 @@ constexpr int64_t kMaxGlobalRows = 0xFFFFFFFFll;
 constexpr int64_t kMaxCounterChannels = 1ll << 26;
 
 // Launches issued per kernel family (TSDE_KERNEL_*), read by tsde_kernel_launches.
-constexpr int kKernelFamilies = 8;
+constexpr int kKernelFamilies = 9;
 inline std::atomic<int64_t> g_launches[kKernelFamilies];
+
+// The contraction of a GENERAL-noise launch with m channels: cabi.cu sends m == 1 to the row-wise kernels (one product
+// g * dW), launch_gen picks among the others (tableau_general.cu describes each kernel's summation order), and the
+// element-wise general kernels (pointwise.cu) sum in the order of the route this gives them.  `quads`: g (and memory
+// noise) loadable as 16-byte quads; `row_bytes`: one row of increments (W, and U when the op wants it) in shared memory.
+enum { TSDE_GEN_ROWWISE = 0, TSDE_GEN_TILE = 1, TSDE_GEN_GENERIC = 2, TSDE_GEN_WIDE = 3 };
+inline int gen_route(int64_t m, bool quads, int64_t row_bytes) {
+  if (m == 1) return TSDE_GEN_ROWWISE;
+  const int64_t mq = m / 4;
+  if (quads && m % 4 == 0 && mq >= 1 && mq <= 32 && (mq & (mq - 1)) == 0) return TSDE_GEN_TILE;
+  return row_bytes > 40 * 1024 ? TSDE_GEN_WIDE : TSDE_GEN_GENERIC;
+}
 
 // A launch descriptor every entry point can rely on: non-null, non-negative row count, positive widths.
 inline bool valid_launch(const tsde_launch* L) { return L && L->rows >= 0 && L->d > 0 && L->m > 0; }

@@ -248,16 +248,17 @@ __device__ __forceinline__ void pw_set_state(const PwProg<T>& pg, void* regs, co
 // between a caller's program and an out-of-range shared-memory index.  The parts common to both layouts are here;
 // which instructions and results may read what is spelt out per layout, beside the kernel that reads them so.
 
-// the counts and the operand table; clears *vec when a device operand is not 16-byte aligned
-static bool pw_valid_tables(const tsde_pointwise& pg, bool* vec) {
+// the counts and the operand table (kinds up to `max_kind`: TSDE_PW_M in the general layout); clears *vec when a
+// CHANNEL or ROW operand, which the kernels read as quads, is not 16-byte aligned
+static bool pw_valid_tables(const tsde_pointwise& pg, bool* vec, int max_kind = TSDE_PW_ROW) {
   if (pg.n_instr < 0 || pg.n_instr > TSDE_PW_MAX_INSTR || pg.n_fg < 0 || pg.n_fg > pg.n_instr ||
       pg.n_regs < 0 || pg.n_regs > TSDE_PW_MAX_REGS || pg.n_operands < 0 || pg.n_operands > TSDE_PW_MAX_OPERANDS)
     return false;
   for (int k = 0; k < pg.n_operands; ++k) {
     const tsde_pw_operand& o = pg.operand[k];
-    if (o.kind < TSDE_PW_IMM || o.kind > TSDE_PW_ROW) return false;
+    if (o.kind < TSDE_PW_IMM || o.kind > max_kind) return false;
     if (o.kind >= TSDE_PW_SCALAR && !o.ptr) return false;
-    if (o.kind >= TSDE_PW_CHANNEL) *vec = *vec && aligned16(o.ptr);
+    if (o.kind == TSDE_PW_CHANNEL || o.kind == TSDE_PW_ROW) *vec = *vec && aligned16(o.ptr);
   }
   return true;
 }
@@ -407,7 +408,9 @@ static_assert(sizeof(PwOperands<double>) + sizeof(PwP<double>) + sizeof(NoiseP<d
                   4096,
               "the compiled Milstein kernel's parameters fit the 4 KiB parameter space");
 
-static std::string num(int x) {
+// (const: concatenating two temporaries would instantiate std::operator+(string&&, string&&) out of line, an exported
+// symbol of the library)
+static const std::string num(int x) {
   char b[16];
   snprintf(b, sizeof(b), "%d", x);
   return b;
@@ -629,15 +632,16 @@ static int pw_nvrtc(const std::string& source, std::string& cubin) {
 }
 
 struct PwCompiled {
-  cudaKernel_t kernel[2];  // one Brownian cell per step, several cells merged (kSrcCounterMulti); adaptive: kernel[0]
+  // one Brownian cell per step, several cells merged (kSrcCounterMulti); adaptive: kernel[0]; a general-noise program:
+  // Euler's two, then midpoint's two
+  cudaKernel_t kernel[4];
 };
 
-// The loaded kernels of a program that passed validation, compiled on first use.  Libraries are context-independent:
-// one entry serves every device.
-static int pw_compiled(const tsde_pointwise& prog, bool f64, PwCompiled& out, bool adaptive = false) {
+// The kernels `names` of `source` (kernel[i] for names[i]; a null name takes the kernel before it), compiled and loaded
+// on first use.  Libraries are context-independent: one entry serves every device.
+static int pw_loaded(std::string source, std::initializer_list<const char*> names, PwCompiled& out) {
   static std::mutex mu;
   static std::map<std::string, PwCompiled> cache;
-  std::string source = pw_milstein_source(prog, f64, adaptive);
   std::lock_guard<std::mutex> lock(mu);
   auto it = cache.find(source);
   if (it != cache.end()) {
@@ -648,21 +652,29 @@ static int pw_compiled(const tsde_pointwise& prog, bool f64, PwCompiled& out, bo
   if (int e = pw_nvrtc(source, cubin)) return e;
   cudaLibrary_t lib;
   cudaError_t e = cudaLibraryLoadData(&lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0);
-  if (e == cudaSuccess && adaptive) {
-    e = cudaLibraryGetKernel(&out.kernel[0], lib, "tsde_pw_milstein_adaptive");
-    out.kernel[1] = out.kernel[0];
-    if (e != cudaSuccess) cudaLibraryUnload(lib);
-  } else if (e == cudaSuccess) {
-    e = cudaLibraryGetKernel(&out.kernel[0], lib, "tsde_pw_milstein_single");
-    if (e == cudaSuccess) e = cudaLibraryGetKernel(&out.kernel[1], lib, "tsde_pw_milstein_multi");
-    if (e != cudaSuccess) cudaLibraryUnload(lib);
+  int i = 0;
+  for (const char* name : names) {
+    if (e != cudaSuccess) break;
+    if (name)
+      e = cudaLibraryGetKernel(&out.kernel[i], lib, name);
+    else
+      out.kernel[i] = out.kernel[i - 1];
+    ++i;
   }
+  if (e != cudaSuccess && i > 0) cudaLibraryUnload(lib);
   if (e != cudaSuccess) {
     cudaGetLastError();
     return (int)e;
   }
   cache.emplace(std::move(source), out);
   return 0;
+}
+
+// The loaded kernels of a Milstein program that passed validation, compiled on first use.
+static int pw_compiled(const tsde_pointwise& prog, bool f64, PwCompiled& out, bool adaptive = false) {
+  std::string source = pw_milstein_source(prog, f64, adaptive);
+  return adaptive ? pw_loaded(std::move(source), {"tsde_pw_milstein_adaptive", nullptr}, out)
+                  : pw_loaded(std::move(source), {"tsde_pw_milstein_single", "tsde_pw_milstein_multi"}, out);
 }
 
 // The Milstein layout, in the order the kernel reads it: go exists from the vjp part on, registers carry over.
@@ -1206,8 +1218,24 @@ static int pw_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_point
                       p, np, p.base.nquads, slots, TSDE_KERNEL_PW_CHUNK, st);
 }
 
+// GENERAL launches of tsde_solve_euler_pointwise, tsde_step_predictor_corrector_pointwise, tsde_pointwise_compile and
+// tsde_pointwise_source (general / additive noise; defined with the general-noise code generator below)
+template <typename T>
+static int pw_general_euler(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
+                            const tsde_pw_step* steps, int32_t n_steps);
+template <typename T>
+static int pw_general_midpoint_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                    const void* y0, const void* t0, const void* t_p, int32_t method, double dt,
+                                    double half_dt, void* y1);
+template <typename T>
+static int pw_general_compiled(const tsde_launch* L, const tsde_pointwise* prog, PwCompiled& kc);
+template <typename T>
+static int64_t pw_general_source_of(const tsde_launch* L, const tsde_pointwise* prog, char* buf, int64_t size);
+
 TSDE_EXPORT int tsde_solve_euler_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
                                            const void* y0, const tsde_pw_step* steps, int32_t n_steps) {
+  if (valid_launch(L) && L->noise_type == TSDE_NOISE_GENERAL)
+    return dispatch(L, [&](auto t) -> int { return pw_general_euler<decltype(t)>(L, nz, prog, y0, steps, n_steps); });
   if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
   const void* const in[3] = {};
   void* const out[3] = {};
@@ -1280,6 +1308,10 @@ TSDE_EXPORT int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, co
                                                         const tsde_pointwise* prog, const void* y0, const void* t0,
                                                         const void* t_p, int32_t method, double dt, double half_dt,
                                                         void* y1) {
+  if (valid_launch(L) && L->noise_type == TSDE_NOISE_GENERAL)
+    return dispatch(L, [&](auto t) -> int {
+      return pw_general_midpoint_step<decltype(t)>(L, nz, prog, y0, t0, t_p, method, dt, half_dt, y1);
+    });
   if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
   return dispatch(L, [&](auto t) -> int {
     using T = decltype(t);
@@ -1332,14 +1364,16 @@ static bool pw_milstein_program(const tsde_launch* L, const tsde_pointwise* prog
 
 TSDE_EXPORT int tsde_pointwise_compile(const tsde_launch* L, const tsde_pointwise* prog) {
   return dispatch(L, [&](auto t) -> int {
-    if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
     PwCompiled kc;
+    if (L->noise_type == TSDE_NOISE_GENERAL) return pw_general_compiled<decltype(t)>(L, prog, kc);
+    if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
     return pw_compiled(*prog, sizeof(t) == 8, kc);
   });
 }
 
 TSDE_EXPORT int64_t tsde_pointwise_source(const tsde_launch* L, const tsde_pointwise* prog, char* buf, int64_t size) {
   return dispatch(L, [&](auto t) -> int64_t {
+    if (L->noise_type == TSDE_NOISE_GENERAL) return pw_general_source_of<decltype(t)>(L, prog, buf, size);
     if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
     const std::string src = pw_milstein_source(*prog, sizeof(t) == 8);
     if (buf && size > 0) {
@@ -1461,4 +1495,319 @@ TSDE_EXPORT int tsde_adaptive_pointwise_compile(const tsde_launch* L, const tsde
     PwCompiled kc;
     return pw_compiled(*prog, sizeof(t) == 8, kc, true);
   });
+}
+
+// ---- general / additive noise (tsde_solve_euler_general_pointwise, tsde_step_midpoint_general_pointwise) ------------
+// The two-program layout with per-channel values.  A g program runs m times per output, so it is compiled, never
+// interpreted (an interpreted instruction costs about 30 SASS instructions, DESIGN §4): pw_general_source writes it
+// out as a `Prog` for pw_general_euler_steps / pw_general_midpoint (pw_device.cuh), with the IEEE options and the
+// cache of the Milstein kernels.  A g instruction is per channel when one of its sources is (a DM or M operand, or a
+// per-channel value); the others are per (row, d) element, evaluated once per lane before the channel loop.  The
+// contraction of each lane's m values with the increments is written out for the route the unfused step takes
+// (gen_route), as that kernel sums:
+//   TSDE_GEN_ROWWISE   g * w                                       (the row-wise kernels' single product)
+//   TSDE_GEN_TILE      per channel quad an fma chain from 0; the quad sums as the xor-butterfly adds them, a pairwise
+//                      tree in natural order                       (gen_cta_kernel, gen_tma_kernel)
+//   TSDE_GEN_GENERIC   left to right from 0, a rounded multiply and a rounded add per channel    (gen_kernel)
+// Register use stays bounded: m <= TSDE_PW_GENERAL_MAX_M increments per thread, and the tree keeps at most
+// log2(m / 4) + 1 partial sums.
+
+// The launch bounds of the compiled general kernels: one resident CTA per SM at least, so that ptxas never spills the
+// increments (pointwise.py's _RESIDENT_CTAS counts on one).
+static_assert(sizeof(PwOperands<double>) + sizeof(PwP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <=
+                  4096,
+              "the compiled general Euler kernel's parameters fit the 4 KiB parameter space");
+static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralMidP<double>) + sizeof(NoiseP<double>) <= 4096,
+              "the compiled general midpoint kernel's parameters fit the 4 KiB parameter space");
+
+static bool pw_per_channel_kind(int kind) { return kind == TSDE_PW_DM || kind == TSDE_PW_M; }
+
+// The general layout (tagged TSDE_PW_LAYOUT_GENERAL): the two-program layout with DM / M operands read by g only.
+static bool pw_valid_general(const tsde_pointwise& pg) {
+  if (!pw_valid_two<TSDE_PW_MAX_REGS>(pg)) return false;
+  auto per_channel = [&](uint8_t s) {
+    return s >= TSDE_PW_OPERAND(0) && s != TSDE_PW_SRC_Y && s != TSDE_PW_SRC_GO &&
+           pw_per_channel_kind(pg.operand[s - TSDE_PW_OPERAND(0)].kind);
+  };
+  for (int i = 0; i < pg.n_fg; ++i)
+    if (per_channel(pg.instr[i].a) || (!pw_unary(pg.instr[i].op) && per_channel(pg.instr[i].b))) return false;
+  return !per_channel(pg.f_src);
+}
+
+// A launch and program the general kernels serve; `route` is the contraction order (gen_route) for dtype size `s`.
+static bool pw_general_program(const tsde_launch* L, const tsde_pointwise* prog, int64_t s, int& route) {
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_GENERAL || L->m > TSDE_PW_GENERAL_MAX_M || !prog ||
+      prog->reserved != TSDE_PW_LAYOUT_GENERAL)
+    return false;
+  bool vec = true;
+  if (!pw_valid_tables(*prog, &vec, TSDE_PW_M) || !pw_valid_general(*prog)) return false;
+  // the unfused step's g is a new contiguous tensor (aligned), or the user's (d, m) block itself when g is a DM operand
+  bool quads = true;
+  const uint8_t g = prog->g_src;
+  if (g >= TSDE_PW_OPERAND(0) && g != TSDE_PW_SRC_Y && g != TSDE_PW_SRC_GO &&
+      prog->operand[g - TSDE_PW_OPERAND(0)].kind == TSDE_PW_DM)
+    quads = aligned16(prog->operand[g - TSDE_PW_OPERAND(0)].ptr);
+  route = gen_route(L->m, quads, L->m * s);
+  return route != TSDE_GEN_WIDE;
+}
+
+// The translation unit of a program that passed pw_general_program, for m channels and contraction `route`: the
+// kernels of Euler chunks and of a midpoint step.
+static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t m, int route) {
+  const char* T = f64 ? "double" : "float";
+  const std::string fs = f64 ? "" : "f", M = num((int)m);
+  const int mq = (int)((m + 3) / 4);
+  auto operand = [&](uint8_t s) { return s >= TSDE_PW_OPERAND(0) && s != TSDE_PW_SRC_Y && s != TSDE_PW_SRC_GO; };
+  auto kind = [&](uint8_t s) { return in.operand[s - TSDE_PW_OPERAND(0)].kind; };
+  // an operand's value in lane j (channel k for DM / M; i is the lane's d index)
+  auto operand_value = [&](uint8_t s) -> std::string {
+    const std::string n = num(s - TSDE_PW_OPERAND(0));
+    switch (kind(s)) {
+      case TSDE_PW_IMM: return "ops.k[" + n + "].imm";
+      case TSDE_PW_T0: return "t0";
+      case TSDE_PW_SCALAR: return "u" + n;
+      case TSDE_PW_DM: return "ops.k[" + n + "].ptr[i * " + M + " + k]";
+      case TSDE_PW_M: return "ops.k[" + n + "].ptr[k]";
+      default: return "k" + n + "[j]";
+    }
+  };
+  // the expression of instruction x with sources a, b and destination (SEL's condition) d, as pw_loop's case
+  auto expression = [&](const tsde_pw_instr& x, const std::string& a, const std::string& b,
+                        const std::string& d) -> const std::string {
+    switch (x.op) {
+      case TSDE_PW_MUL: return a + " * " + b;
+      case TSDE_PW_ADD: return a + " + " + b;
+      case TSDE_PW_SUB: return a + " - " + b;
+      case TSDE_PW_DIV: return a + " / " + b;
+      case TSDE_PW_NEG: return "-" + a;
+      case TSDE_PW_SQRT: return "sqrt" + fs + "(" + a + ")";
+      case TSDE_PW_LT: return a + " < " + b + " ? T(1) : T(0)";
+      case TSDE_PW_LE: return a + " <= " + b + " ? T(1) : T(0)";
+      case TSDE_PW_EQ: return a + " == " + b + " ? T(1) : T(0)";
+      case TSDE_PW_MAXIMUM:  // maximum_kernel_cuda (::max is fmax)
+        return a + " != " + a + " ? " + a + " : " + b + " != " + b + " ? " + b + " : fmax" + fs + "(" + a + ", " + b +
+               ")";
+      case TSDE_PW_MINIMUM:  // minimum_kernel_cuda (::min is fmin)
+        return a + " != " + a + " ? " + a + " : " + b + " != " + b + " ? " + b + " : fmin" + fs + "(" + a + ", " + b +
+               ")";
+      case TSDE_PW_ABS: return "fabs" + fs + "(" + a + ")";
+      default: return d + " != T(0) ? " + a + " : " + b;  // TSDE_PW_SEL: the condition is the destination
+    }
+  };
+  std::string o = "// An element-wise general-noise program of torchsde_b200, generated by pw_general_source\n"
+                  "#include \"pw_device.cuh\"\n\n";
+  o += "namespace tsde {\nnamespace {\ntypedef " + std::string(T) + " T;\n\nstruct Prog {\n";
+  o += "  static constexpr int MQ = " + num(mq) + ";\n";
+  for (int k = 0; k < in.n_operands; ++k) {
+    const std::string n = num(k);
+    if (in.operand[k].kind == TSDE_PW_SCALAR) o += "  T u" + n + ";\n";
+    if (in.operand[k].kind == TSDE_PW_CHANNEL || in.operand[k].kind == TSDE_PW_ROW) o += "  T k" + n + "[4];\n";
+  }
+  o += "  __device__ __forceinline__ void load(const PwOperands<T>& ops, const PwQuad& c) {\n";
+  for (int k = 0; k < in.n_operands; ++k) {
+    const std::string n = num(k);
+    const int kd = in.operand[k].kind;
+    if (kd == TSDE_PW_SCALAR) o += "    u" + n + " = *ops.k[" + n + "].ptr;\n";
+    if (kd == TSDE_PW_CHANNEL || kd == TSDE_PW_ROW)
+      o += "    load_quad(ops.k[" + n + "].ptr, c." + (kd == TSDE_PW_ROW ? "base" : "chan") + ", c.vec, c.nvalid, k" +
+           n + ");\n";
+  }
+  o += "  }\n";
+  // f: instructions [0, n_fg) on registers r<n>[4], as the Milstein kernels run them
+  o += "  __device__ __forceinline__ void f(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
+       "                                    T (&out)[4]) {\n    const T t0 = *tp;\n    (void)t0;\n";
+  for (int r = 0; r < in.n_regs; ++r) o += "    T r" + num(r) + "[4];\n";
+  auto fsrc = [&](uint8_t s) -> std::string {
+    if (s == TSDE_PW_SRC_Y) return "y[j]";
+    return operand(s) ? operand_value(s) : "r" + num(s) + "[j]";
+  };
+  o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
+  for (int i = 0; i < in.n_fg; ++i) {
+    const tsde_pw_instr& x = in.instr[i];
+    const std::string a = fsrc(x.a), b = pw_unary(x.op) ? a : fsrc(x.b), d = "r" + num(x.dst) + "[j]";
+    o += "      " + d + " = " + expression(x, a, b, d) + ";\n";
+  }
+  o += "      out[j] = " + fsrc(in.f_src) + ";\n    }\n  }\n";
+  // g: instruction i is n<i>[4] (per element, before the channel loop) or v<i> (per channel, inside G(k)); a register
+  // names the instruction that last wrote it
+  int def[TSDE_PW_MAX_REGS];
+  bool wide[TSDE_PW_MAX_INSTR] = {};
+  for (int r = 0; r < TSDE_PW_MAX_REGS; ++r) def[r] = -1;
+  auto is_wide = [&](uint8_t s) {
+    if (s == TSDE_PW_SRC_Y) return false;
+    if (operand(s)) return pw_per_channel_kind(kind(s));
+    return wide[def[s]];
+  };
+  auto gsrc = [&](uint8_t s) -> std::string {
+    if (s == TSDE_PW_SRC_Y) return "y[j]";
+    if (operand(s)) return operand_value(s);
+    return wide[def[s]] ? "v" + num(def[s]) : "n" + num(def[s]) + "[j]";
+  };
+  std::string narrow, per_channel;
+  for (int i = in.n_fg; i < in.n_instr; ++i) {
+    const tsde_pw_instr& x = in.instr[i];
+    const bool sel = x.op == TSDE_PW_SEL;
+    wide[i] = is_wide(x.a) || (!pw_unary(x.op) && is_wide(x.b)) || (sel && is_wide(x.dst));
+    const std::string a = gsrc(x.a), b = pw_unary(x.op) ? a : gsrc(x.b), d = sel ? gsrc(x.dst) : "";
+    if (wide[i])
+      per_channel += "        const T v" + num(i) + " = " + expression(x, a, b, d) + ";\n";
+    else
+      narrow += "      n" + num(i) + "[j] = " + expression(x, a, b, d) + ";\n";
+    def[x.dst] = i;
+  }
+  o += "  __device__ __forceinline__ void gp(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
+       "                                     const T (&w)[4 * MQ], T (&out)[4]) {\n    const T t0 = *tp;\n"
+       "    (void)t0;\n";
+  for (int i = in.n_fg; i < in.n_instr; ++i)
+    if (!wide[i]) o += "    T n" + num(i) + "[4];\n";
+  o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n" + narrow + "    }\n";
+  o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n"
+       "      const int64_t i = c.chan + (j < c.nvalid ? j : 0);  // (the d index of the lane; padding lanes read lane 0's)\n"
+       "      (void)i;\n      auto G = [&](int k) -> T {\n        (void)k;\n" +
+       per_channel + "        return " + gsrc(in.g_src) + ";\n      };\n";
+  const std::string fma = "fma" + fs;
+  if (route == TSDE_GEN_ROWWISE) {
+    o += "      const T acc = G(0) * w[0];\n";
+  } else if (route == TSDE_GEN_GENERIC) {
+    o += "      T acc = T(0);\n";
+    for (int k = 0; k < m; ++k) o += "      acc = acc + G(" + num(k) + ") * w[" + num(k) + "];\n";
+  } else {
+    std::string level[TSDE_PW_GENERAL_MAX_M / 4];  // the partial sums of the tree's current level
+    for (int q = 0; q < mq; ++q) {
+      const std::string s = "s" + num(q);
+      o += "      T " + s + " = " + fma + "(G(" + num(4 * q) + "), w[" + num(4 * q) + "], T(0));\n";
+      for (int j = 1; j < 4; ++j)
+        o += "      " + s + " = " + fma + "(G(" + num(4 * q + j) + "), w[" + num(4 * q + j) + "], " + s + ");\n";
+      level[q] = s;
+    }
+    for (int l = 0, n = mq; n > 1; ++l, n /= 2) {
+      for (int p = 0; p < n; p += 2) {
+        const std::string s = "a" + num(l) + "_" + num(p / 2);
+        o += "      const T " + s + " = " + level[p] + " + " + level[p + 1] + ";\n";
+        level[p / 2] = s;
+      }
+    }
+    o += "      const T acc = " + level[0] + ";\n";
+  }
+  o += "      out[j] = acc;\n    }\n  }\n};\n}  // namespace\n}  // namespace tsde\n";
+  const std::string bounds = "__launch_bounds__(" + num(kThreads) + ", 1)";
+  for (const char* v : {"single", "multi"}) {
+    const std::string src = v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti";
+    o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_general_euler_" + v +
+           "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwP<tsde::T> p,\n"
+           "    const tsde::NoiseP<tsde::T> nz, const __grid_constant__ tsde::PwSteps<tsde::T> st) {\n"
+           "  tsde::pw_general_euler_steps<tsde::T, " + src + ", tsde::Prog>(ops, p, nz, st);\n}\n";
+  }
+  for (const char* v : {"single", "multi"}) {
+    const std::string src = v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti";
+    o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_general_midpoint_" + v +
+           "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwGeneralMidP<tsde::T> p,\n"
+           "    const tsde::NoiseP<tsde::T> nz) {\n"
+           "  tsde::pw_general_midpoint<tsde::T, " + src + ", tsde::Prog>(ops, p, nz);\n}\n";
+  }
+  return o;
+}
+
+template <typename T>
+static int pw_general_compiled(const tsde_launch* L, const tsde_pointwise* prog, PwCompiled& kc) {
+  int route;
+  if (!pw_general_program(L, prog, sizeof(T), route)) return TSDE_EINVAL;
+  return pw_loaded(pw_general_source(*prog, sizeof(T) == 8, L->m, route),
+                   {"tsde_pw_general_euler_single", "tsde_pw_general_euler_multi", "tsde_pw_general_midpoint_single",
+                    "tsde_pw_general_midpoint_multi"},
+                   kc);
+}
+
+template <typename T>
+static PwOperands<T> pw_operands(const tsde_pointwise* prog) {
+  PwOperands<T> ops{};
+  for (int k = 0; k < prog->n_operands; ++k)
+    ops.k[k] = PwOperand<T>{static_cast<const T*>(prog->operand[k].ptr), (T)prog->operand[k].imm};
+  return ops;
+}
+
+// tsde_solve_euler_pointwise for a GENERAL launch: the chunk `steps[0, n_steps)` from y0 as one launch of the
+// program's compiled Euler kernel, under the rules of pw_milstein_chunk.
+template <typename T>
+static int pw_general_euler(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
+                            const tsde_pw_step* steps, int32_t n_steps) {
+  int route;
+  if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
+  if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !y0 || !pw_general_program(L, prog, sizeof(T), route))
+    return TSDE_EINVAL;
+  bool vec = L->d % 4 == 0 && aligned16(y0);
+  pw_valid_tables(*prog, &vec, TSDE_PW_M);
+  NoiseP<T> np;
+  if (int e = fill_noise<T>(L, nz, false, np)) return e;
+  if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
+  PwSteps<T> st{};
+  st.n = n_steps;
+  for (int j = 0; j < n_steps; ++j) {
+    const tsde_pw_step& s = steps[j];
+    if (!s.t0) return TSDE_EINVAL;
+    if (s.y1 && !aligned16(s.y1)) vec = false;
+    st.s[j] = PwStep<T>{s.cell_id, static_cast<const T*>(s.t0), static_cast<T*>(s.y1), (T)sqrt(s.h), (T)s.dt};
+  }
+  PwCompiled kc;
+  if (int e = pw_general_compiled<T>(L, prog, kc)) return e;
+  PwOperands<T> ops = pw_operands<T>(prog);
+  PwP<T> p{};
+  p.y0 = static_cast<const T*>(y0);
+  fill_quad_map(L->rows, L->d, p);
+  p.vec = vec ? 1 : 0;
+  // (the multi-cell merge reads the first cell and the uniform length from the noise descriptor)
+  np.cell_id = steps[0].cell_id;
+  np.h = steps[0].h;
+  void* args[] = {&ops, &p, &np, &st};
+  const int e = launch_kernel_handle(kc.kernel[np.n_cells > 1 ? 1 : 0], (p.nquads + kThreads - 1) / kThreads,
+                                     kThreads, reinterpret_cast<cudaStream_t>(L->stream), args);
+  if (e == 0) g_launches[TSDE_KERNEL_PW_GENERAL].fetch_add(1, std::memory_order_relaxed);
+  return e;
+}
+
+// tsde_step_predictor_corrector_pointwise for a GENERAL launch: one midpoint step as one launch of the program's
+// compiled midpoint kernel.
+template <typename T>
+static int pw_general_midpoint_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                    const void* y0, const void* t0, const void* t_p, int32_t method, double dt,
+                                    double half_dt, void* y1) {
+  int route;
+  if (method != TSDE_PC_MIDPOINT || !t0 || !t_p || !y0 || !y1 || !nz || nz->source != TSDE_SRC_COUNTER ||
+      nz->flags || !pw_general_program(L, prog, sizeof(T), route))
+    return TSDE_EINVAL;
+  bool vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y1);
+  pw_valid_tables(*prog, &vec, TSDE_PW_M);
+  NoiseP<T> np;
+  if (int e = fill_noise<T>(L, nz, false, np)) return e;
+  PwCompiled kc;
+  if (int e = pw_general_compiled<T>(L, prog, kc)) return e;
+  PwOperands<T> ops = pw_operands<T>(prog);
+  PwGeneralMidP<T> p{};
+  p.base.y0 = static_cast<const T*>(y0);
+  p.base.y1 = static_cast<T*>(y1);
+  p.base.t0 = static_cast<const T*>(t0);
+  p.base.dt = (T)dt;
+  fill_quad_map(L->rows, L->d, p.base);
+  p.base.vec = vec ? 1 : 0;
+  p.t_p = static_cast<const T*>(t_p);
+  p.half_dt = (T)half_dt;
+  void* args[] = {&ops, &p, &np};
+  const int e = launch_kernel_handle(kc.kernel[np.n_cells > 1 ? 3 : 2], (p.base.nquads + kThreads - 1) / kThreads,
+                                     kThreads, reinterpret_cast<cudaStream_t>(L->stream), args);
+  if (e == 0) g_launches[TSDE_KERNEL_PW_GENERAL].fetch_add(1, std::memory_order_relaxed);
+  return e;
+}
+
+// tsde_pointwise_source for a GENERAL launch
+template <typename T>
+static int64_t pw_general_source_of(const tsde_launch* L, const tsde_pointwise* prog, char* buf, int64_t size) {
+  int route;
+  if (!pw_general_program(L, prog, sizeof(T), route)) return TSDE_EINVAL;
+  const std::string src = pw_general_source(*prog, sizeof(T) == 8, L->m, route);
+  if (buf && size > 0) {
+    const size_t n = std::min(src.size(), (size_t)size - 1);
+    memcpy(buf, src.data(), n);
+    buf[n] = 0;
+  }
+  return (int64_t)src.size();
 }

@@ -381,4 +381,137 @@ __device__ __forceinline__ void pw_milstein_proposal(const PwOperands<T>& ops, c
   store_quad(y_next, c.base, c.vec, c.nvalid, y0);
 }
 
+// ---- general-noise tableau ops that the element-wise general kernels share with tableau_general.cu -----------------
+// (the Op interface of tableau_general.cu: gval, weight, combine)
+// y1 = y0 + f*dt + g.dW                                                         methods/euler.py:36
+template <typename T>
+struct GEulerOp {
+  static constexpr int NE = 2, NG = 1, NP = 1, NO = 1;
+  static constexpr bool WANT_U = false;
+  T dt;
+  __device__ __forceinline__ T gval(int, const T (&g)[1]) const { return g[0]; }
+  __device__ __forceinline__ T weight(int, T w, T) const { return w; }
+  __device__ __forceinline__ void combine(const T (&e)[2], const T (&gp)[1], T (&o)[1]) const {
+    o[0] = (e[0] + e[1] * dt) + gp[0];
+  }
+};
+// y' = y0 + half_dt*f + 0.5*(g.dW)                                               methods/midpoint.py:38
+template <typename T>
+struct GMidpointPredictOp {
+  static constexpr int NE = 2, NG = 1, NP = 1, NO = 1;
+  static constexpr bool WANT_U = false;
+  T half_dt;
+  __device__ __forceinline__ T gval(int, const T (&g)[1]) const { return g[0]; }
+  __device__ __forceinline__ T weight(int, T w, T) const { return w; }
+  __device__ __forceinline__ void combine(const T (&e)[2], const T (&gp)[1], T (&o)[1]) const {
+    o[0] = (e[0] + half_dt * e[1]) + T(0.5) * gp[0];
+  }
+};
+
+// ---- general / additive noise with an element-wise f and g (tsde_solve_euler_general_pointwise, ...) ---------------
+// One thread per (row, quad of d), as above.  The thread draws all m increments of its row (MQ channel quads on the
+// counters of the general-noise kernels; the d/4 threads of a row draw the same ones) and never forms g in memory:
+// `Prog` (generated by pw_general_source in pointwise.cu) evaluates g_ij channel by channel in registers and contracts
+// it with the increments in the order of the unfused launch's route (gen_route), so that its g.dW is the unfused one:
+//   load(ops, c)                  the operands kept in registers, after the dependency wait
+//   f(ops, c, t, y, f)            the f program at (*t, y)
+//   gp(ops, c, t, y, w, gp)       the g program at (*t, y), contracted with w[0, 4 MQ)
+
+// The increments of this thread's row: channel k in w[k]
+template <typename T, int SRC, int MQ>
+__device__ __forceinline__ void pw_general_noise(const NoiseP<T>& nz, Key key, int64_t row, T (&w)[4 * MQ]) {
+  const uint32_t grow = (uint32_t)(row + nz.row_offset);
+#pragma unroll
+  for (int q = 0; q < MQ; ++q) {
+    T w4[4], u4[4];
+    counter_noise<T, false, SRC == kSrcCounterMulti>(nz, key, grow, (uint32_t)q, w4, u4);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) w[4 * q + j] = w4[j];
+  }
+}
+
+// Consecutive Euler steps, as pw_milstein_steps: y1 = GEulerOp{dt} on (y, f, g.dW)
+template <typename T, int SRC, typename Prog>
+__device__ __forceinline__ void pw_general_euler_steps(const PwOperands<T>& ops, const PwP<T>& p, const NoiseP<T>& nz,
+                                                       const PwSteps<T>& st) {
+  PwQuad c;
+  int64_t Q, row, q;
+  pw_locate(p, c, Q, row, q);
+  const Key key = load_key(nz.key);
+  Prog prog;
+  T y[4];
+  for (int j = 0; j < st.n; ++j) {
+    const PwStep<T>& s = st.s[j];
+    NoiseP<T> z = nz;  // this step's cell
+    z.cell_id = s.cell;
+    z.sqrt_h = s.sqrt_h;
+    T w[4 * Prog::MQ];
+    pw_general_noise<T, SRC, Prog::MQ>(z, key, row, w);
+    if (j == 0) {  // the first increments are drawn while the previous kernel drains; the rest is read after the wait
+      asm volatile("griddepcontrol.wait;" ::: "memory");
+      if (Q >= p.nquads) return;
+      load_quad(p.y0, c.base, c.vec, c.nvalid, y);
+      prog.load(ops, c);
+    }
+    T f[4], gp[4];
+    prog.f(ops, c, s.t0, y, f);
+    prog.gp(ops, c, s.t0, y, w, gp);
+    const GEulerOp<T> op{s.dt};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const T e[2] = {y[i], f[i]}, g1[1] = {gp[i]};
+      T o[1];
+      op.combine(e, g1, o);
+      y[i] = o[0];
+    }
+    if (s.y1) store_quad(s.y1, c.base, c.vec, c.nvalid, y);
+  }
+}
+
+template <typename T>
+struct PwGeneralMidP {
+  PwP<T> base;   // y0, y1, the quad mapping, t0 and dt
+  const T* t_p;  // the time of the second evaluation, t0 + half_dt
+  T half_dt;
+};
+
+// One midpoint step: y' = GMidpointPredictOp{half_dt} on (y0, f, g.dW) at (t0, y0); y1 = GEulerOp{dt} on
+// (y0, f', g'.dW) at (t_p, y')
+template <typename T, int SRC, typename Prog>
+__device__ __forceinline__ void pw_general_midpoint(const PwOperands<T>& ops, const PwGeneralMidP<T>& p,
+                                                    const NoiseP<T>& nz) {
+  PwQuad c;
+  int64_t Q, row, q;
+  pw_locate(p.base, c, Q, row, q);
+  T w[4 * Prog::MQ];
+  pw_general_noise<T, SRC, Prog::MQ>(nz, load_key(nz.key), row, w);
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (Q >= p.base.nquads) return;
+  Prog prog;
+  T y0[4], yp[4], f[4], gp[4];
+  load_quad(p.base.y0, c.base, c.vec, c.nvalid, y0);
+  prog.load(ops, c);
+  prog.f(ops, c, p.base.t0, y0, f);
+  prog.gp(ops, c, p.base.t0, y0, w, gp);
+  const GMidpointPredictOp<T> predict{p.half_dt};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const T e[2] = {y0[i], f[i]}, g1[1] = {gp[i]};
+    T o[1];
+    predict.combine(e, g1, o);
+    yp[i] = o[0];
+  }
+  prog.f(ops, c, p.t_p, yp, f);
+  prog.gp(ops, c, p.t_p, yp, w, gp);
+  const GEulerOp<T> step{p.base.dt};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const T e[2] = {y0[i], f[i]}, g1[1] = {gp[i]};
+    T o[1];
+    step.combine(e, g1, o);
+    yp[i] = o[0];
+  }
+  store_quad(p.base.y1, c.base, c.vec, c.nvalid, yp);
+}
+
 }  // namespace tsde

@@ -816,9 +816,11 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
   if (int e = fill_noise<T>(L, nz, false, np)) return e;
   const int64_t mq = L->m / 4;
   const bool mem = nz->source == TSDE_SRC_MEMORY;
-  // the tile kernels: m / 4 a power of two <= 32, g and (memory noise) W / U loadable as quads
-  const bool tile = vec && mq >= 1 && mq <= 32 && (mq & (mq - 1)) == 0 &&
-                    (!mem || (aligned16(np.w) && (!Op::WANT_U || aligned16(np.u))));
+  const int64_t smem_per_row = L->m * (int64_t)sizeof(T) * (Op::WANT_U ? 2 : 1);
+  // the tile kernels: m / 4 a power of two <= 32, g and (memory noise) W / U loadable as quads (gen_route)
+  const int route =
+      gen_route(L->m, vec && (!mem || (aligned16(np.w) && (!Op::WANT_U || aligned16(np.u)))), smem_per_row);
+  const bool tile = route == TSDE_GEN_TILE;
   p.rows = L->rows; p.d = L->d; p.m = L->m;
   p.mq = (int32_t)mq;
   p.vec = vec ? 1 : 0;
@@ -847,9 +849,8 @@ static int launch_gen(const tsde_launch* L, const tsde_noise* nz,
   int64_t rb = (16 * kThreads + per_row - 1) / per_row;
   if (rb < 1) rb = 1;
   if (rb > kMaxRowsPerBlock) rb = kMaxRowsPerBlock;
-  const int64_t smem_per_row = L->m * (int64_t)sizeof(T) * (Op::WANT_U ? 2 : 1);
   while (rb > 1 && rb * smem_per_row > 40 * 1024) rb >>= 1;
-  if (rb * smem_per_row > 40 * 1024) {  // not even one row's increments fit: walk m in chunks, one CTA per row
+  if (route == TSDE_GEN_WIDE) {  // not even one row's increments fit: walk m in chunks, one CTA per row
     if (L->rows > 0x7fffffffll) return TSDE_EINVAL;
     p.rb = 1;
     const int64_t outs = L->d < kWideOutputs ? L->d : kWideOutputs;
@@ -882,18 +883,7 @@ static int launch_gen_fmt(const tsde_launch* L, const tsde_noise* nz, std::initi
 }
 
 // ---- ops ---------------------------------------------------------------------------------------
-// y1 = y0 + f*dt + g.dW                                                         methods/euler.py:36
-template <typename T>
-struct GEulerOp {
-  static constexpr int NE = 2, NG = 1, NP = 1, NO = 1;
-  static constexpr bool WANT_U = false;
-  T dt;
-  __device__ __forceinline__ T gval(int, const T (&g)[1]) const { return g[0]; }
-  __device__ __forceinline__ T weight(int, T w, T) const { return w; }
-  __device__ __forceinline__ void combine(const T (&e)[2], const T (&gp)[1], T (&o)[1]) const {
-    o[0] = (e[0] + e[1] * dt) + gp[0];
-  }
-};
+// (GEulerOp and GMidpointPredictOp: pw_device.cuh, which the run-time compiled general-noise kernels include too)
 // y1 = y0 + (dt*(f+f') + g.dW + g'.dW) * 0.5                                     methods/heun.py:46
 template <typename T>
 struct GHeunOp {
@@ -905,18 +895,6 @@ struct GHeunOp {
   __device__ __forceinline__ T weight(int, T w, T) const { return w; }
   __device__ __forceinline__ void combine(const T (&e)[3], const T (&gp)[2], T (&o)[1]) const {
     o[0] = e[0] + ((dt * (e[1] + e[2]) + gp[0]) + gp[1]) * T(0.5);
-  }
-};
-// y' = y0 + half_dt*f + 0.5*(g.dW)                                               methods/midpoint.py:38
-template <typename T>
-struct GMidpointPredictOp {
-  static constexpr int NE = 2, NG = 1, NP = 1, NO = 1;
-  static constexpr bool WANT_U = false;
-  T half_dt;
-  __device__ __forceinline__ T gval(int, const T (&g)[1]) const { return g[0]; }
-  __device__ __forceinline__ T weight(int, T w, T) const { return w; }
-  __device__ __forceinline__ void combine(const T (&e)[2], const T (&gp)[1], T (&o)[1]) const {
-    o[0] = (e[0] + half_dt * e[1]) + T(0.5) * gp[0];
   }
 };
 // y' = y0 + g.dW                                                                 methods/euler_heun.py:36
