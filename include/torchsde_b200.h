@@ -138,9 +138,10 @@ const char* tsde_error_string(int code);
                                      tsde_solve_reversible_heun_pointwise)                                      */
 #define TSDE_KERNEL_PW_ADAPTIVE 7 /* an adaptive solve's proposal with an element-wise SDE, the full step and both
                                      half steps in one launch (tsde_adaptive_proposal_pointwise)                */
-#define TSDE_KERNEL_PW_GENERAL 8  /* general / additive-noise Euler steps or a midpoint step with an element-wise
-                                     SDE (tsde_solve_euler_general_pointwise,
-                                     tsde_step_midpoint_general_pointwise)                                       */
+#define TSDE_KERNEL_PW_GENERAL 8  /* general / additive-noise Euler steps, a midpoint step or an additive-noise
+                                     SRK step with an element-wise SDE (GENERAL launches of
+                                     tsde_solve_euler_pointwise, tsde_step_predictor_corrector_pointwise and
+                                     tsde_step_srk_diag_pointwise)                                               */
 int64_t tsde_kernel_launches(int32_t family);
 
 
@@ -373,7 +374,8 @@ int64_t tsde_pointwise_source(const tsde_launch* L, const tsde_pointwise* prog, 
  * and reads only its own; TSDE_PW_SRC_Y is the state it is evaluated at, TSDE_PW_T0 its time, TSDE_PW_SRC_GO is
  * not a source.  The operand table is shared.  n_regs <= TSDE_PW_SRK_MAX_REGS: the kernel may keep six stage values
  * in the rest of the register file.
- * Requires DIAGONAL noise, counter noise (nz->source == TSDE_SRC_COUNTER) and no 16-bit formats.
+ * Requires DIAGONAL noise (a GENERAL launch runs an additive-noise sra1 step instead: TSDE_PW_LAYOUT_GENERAL_SRA
+ * below), counter noise (nz->source == TSDE_SRC_COUNTER) and no 16-bit formats.
  */
 #define TSDE_PW_SRK_MAX_REGS 18
 int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
@@ -505,7 +507,24 @@ int tsde_adaptive_pointwise_compile(const tsde_launch* L, const tsde_pointwise* 
  */
 #define TSDE_PW_GENERAL_MAX_M 32
 enum { TSDE_PW_DM = 5, TSDE_PW_M = 6 };
-#define TSDE_PW_LAYOUT_GENERAL 1 /* tsde_pointwise.reserved of a general-layout program (0 for every other layout) */
+#define TSDE_PW_LAYOUT_GENERAL 1 /* tsde_pointwise.reserved of a general-layout program (0 for the diagonal layouts) */
+
+/*
+ * Additive noise, SRA1 (methods/srk.py:90-111).  tsde_step_srk_diag_pointwise on a GENERAL launch with
+ * 1 <= L->m <= TSDE_PW_GENERAL_MAX_M runs one SRK step of an element-wise SDE as one launch, for a program of the
+ * general layout tagged reserved = TSDE_PW_LAYOUT_GENERAL_SRA.  t_0, t_1 and t_q are the 0-d times t0, t0 + dt and
+ * t0 + 3/4 dt (state dtype); dt and rdt as tsde_step_srk_additive takes them; t_h, sqrt_dt and three_dt are unused.
+ * The kernel evaluates f0 = f(t_0, y0), gA = g(t_1, y0) and gB = g(t_0, y0); H0_1 as tsde_srk_additive_stage on
+ * (y0, f0, gA); f1 = f(t_q, H0_1); y1 as tsde_step_srk_additive on (y0, f0, f1, gA, gB).  It draws W and U on the
+ * counters of those launches, forms each product's weights per channel as they do and contracts g with them in their
+ * order: the orders above, except that m == 1 sums left to right from 0 (those launches take the generic kernel there,
+ * whose 0 + g*w turns a -0 product into +0).  g never exists in memory and y1 equals the unfused step's bit for bit.
+ * The launches count under TSDE_KERNEL_PW_GENERAL.  tsde_pointwise_compile and tsde_pointwise_source compile and
+ * write out the program's sra1 kernels (a translation unit of their own) for a GENERAL launch and an SRA-tagged
+ * program.  Counter noise only, no 16-bit formats and no launch flags.  TSDE_EINVAL additionally: a program without
+ * the SRA tag and null times.  The Euler and midpoint GENERAL launches refuse an SRA-tagged program.
+ */
+#define TSDE_PW_LAYOUT_GENERAL_SRA 2 /* tsde_pointwise.reserved of a general-layout program for the sra1 step */
 
 /* derivative-free Milstein, predictor: y' = y0 + (Ito ? dt*f : 0) + g*sqrt_dt
  * methods/milstein.py:58-63,83-84,93-94.  g is (rows,d) also for scalar noise (squeezed). */

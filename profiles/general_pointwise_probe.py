@@ -1,9 +1,11 @@
-"""Fused against unfused general-noise solves (tsde_solve_euler_general_pointwise, tsde_step_midpoint_general_pointwise):
-correlated multi-asset GBM, f = mu * y, g = y.unsqueeze(-1) * S, as captured graphs.  The unfused run is the same
-solve with the tape rejected.  Both are alternated three times in one process; prints ms per solve and us per step,
-with the SM clock and power limit read in the same call.
+"""Fused against unfused general- and additive-noise solves (GENERAL launches of tsde_solve_euler_pointwise,
+tsde_step_predictor_corrector_pointwise and tsde_step_srk_diag_pointwise): correlated multi-asset GBM, f = mu * y,
+g = y.unsqueeze(-1) * S, with Euler and midpoint, and cfg3's additive SDE (tests/problems.py TimeAdditiveExpand) with
+SRK, as captured graphs.  The unfused run is the same solve with the tape rejected.  Both are alternated three times
+in one process; prints ms per solve and us per step, with the SM clock and power limit read in the same call.  Method
+names on the command line select cases.
 
-    python profiles/general_pointwise_probe.py
+    python profiles/general_pointwise_probe.py [euler] [midpoint] [srk]
 """
 import contextlib
 import json
@@ -17,6 +19,7 @@ from torch import nn
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torchsde_b200 as tsde  # noqa: E402
 from torchsde_b200._core import pointwise  # noqa: E402
+from tests import problems  # noqa: E402
 
 DEV = 'cuda'
 
@@ -58,13 +61,17 @@ def clocks():
 
 
 def timed(B, d, m, T, method, fused, reps=5):
-    sde = CorrelatedGBM(d, m, 'ito' if method == 'euler' else 'stratonovich').to(DEV)
+    if method == 'srk':  # sra1 on cfg3's additive SDE, g = (a b / sqrt(1 + t)).expand(B, d, m)
+        sde = problems.TimeAdditiveExpand(d, m, 'ito', dtype=torch.float32).to(DEV)
+    else:
+        sde = CorrelatedGBM(d, m, 'ito' if method == 'euler' else 'stratonovich').to(DEV)
     y0 = torch.full((B, d), 1.0, device=DEV)
     dt = 2.0 ** -8
     ts = torch.tensor([0.0, T * dt], device=DEV)
     ctx = contextlib.nullcontext() if fused else unfused()
     with ctx, torch.no_grad():
-        bm = tsde.BrownianInterval(0.0, T * dt, size=(B, m), device=DEV, entropy=1)
+        bm = tsde.BrownianInterval(0.0, T * dt, size=(B, m), device=DEV, entropy=1,
+                                   levy_area_approximation='space-time' if method == 'srk' else 'none')
         tsde.sdeint(sde, y0, ts, bm=bm, method=method, dt=dt, options={'cuda_graph': True})  # record, capture
         start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         start.record()
@@ -76,7 +83,10 @@ def timed(B, d, m, T, method, fused, reps=5):
 
 
 def main():
-    cases = [('euler', 8192, 32, 16, 500), ('euler', 65536, 64, 16, 100), ('midpoint', 8192, 32, 16, 500)]
+    cases = [('euler', 8192, 32, 16, 500), ('euler', 65536, 64, 16, 100), ('midpoint', 8192, 32, 16, 500),
+             ('srk', 8192, 32, 16, 500)]
+    if sys.argv[1:]:
+        cases = [c for c in cases if c[0] in sys.argv[1:]]
     print(json.dumps({'gpu': torch.cuda.get_device_name(), 'clocks_sm_power_limit': clocks()}))
     for method, B, d, m, T in cases:
         res = {'fused': [], 'unfused': []}

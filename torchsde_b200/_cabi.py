@@ -73,7 +73,7 @@ def general_pointwise_source(prog, dtype, d, m):
 
 def compile_general_pointwise(prog, dtype, d, m):
     """tsde_pointwise_compile on a GENERAL launch: compile and load the Euler and midpoint kernels of general-noise
-    program `prog`; 0 or an error code."""
+    program `prog` (the sra1 kernels if it is tagged PW_LAYOUT_GENERAL_SRA); 0 or an error code."""
     return lib().tsde_pointwise_compile(ctypes.byref(_general_launch(dtype, d, m)), ctypes.byref(prog))
 
 
@@ -113,6 +113,7 @@ KERNEL_PW_ADAPTIVE = 7  # TSDE_KERNEL_PW_ADAPTIVE
 KERNEL_PW_GENERAL = 8  # TSDE_KERNEL_PW_GENERAL
 PW_GENERAL_MAX_M = 32  # TSDE_PW_GENERAL_MAX_M
 PW_LAYOUT_GENERAL = 1  # TSDE_PW_LAYOUT_GENERAL: Pointwise.reserved of a general-noise program
+PW_LAYOUT_GENERAL_SRA = 2  # TSDE_PW_LAYOUT_GENERAL_SRA: Pointwise.reserved of a general-noise program of an sra1 step
 # TSDE_PROPOSAL_*: the method of tsde_adaptive_proposal_pointwise
 (PROPOSAL_EULER, PROPOSAL_MILSTEIN_ITO, PROPOSAL_MILSTEIN_STRATONOVICH, PROPOSAL_SRK, PROPOSAL_HEUN, PROPOSAL_MIDPOINT,
  PROPOSAL_EULER_HEUN) = range(7)

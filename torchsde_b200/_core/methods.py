@@ -443,6 +443,7 @@ class SRK(_ProposalMixin, base_solver.BaseSDESolver):
                                 LEVY_AREA_APPROXIMATIONS.davie,
                                 LEVY_AREA_APPROXIMATIONS.foster)
     want_u = True
+    _pw_general = True  # additive noise fuses too (pointwise.general)
 
     def __init__(self, sde, **kwargs):
         if getattr(sde, 'is_adjoint_sde', False):
@@ -559,12 +560,28 @@ class SRK(_ProposalMixin, base_solver.BaseSDESolver):
         """srk.py:90-111: f0 = f(t0, y0); gA = g(t0+dt, y0); f1 = f(t0+3/4dt, H0_1); gB = g(t0, y0)."""
         sde, s = self.sde, c.scalars
         t_1, t_34, t_00 = c.aux_t
+        if pointwise.ready(self):
+            # f and g were recorded as element-wise programs (pointwise.py): the whole step is one kernel
+            # (on the solver's GENERAL launch: the sra1 step, t_q = t_34, t_h and the last two scalars unused)
+            return pointwise.launch(self, 'tsde_step_srk_diag_pointwise', self._feed.get(c, True), y0,
+                                    (t_00.data_ptr(), t_1.data_ptr(), t_34.data_ptr(), None, c.dt, s['rdt'], 0.0,
+                                     0.0), out)
+        # the first step of an eligible solve runs as always, with the user's four evaluations recorded
+        rec = pointwise.pc_recorder(self, y0, t_00, pointwise.SRA_PATTERN)
+
+        def f(t, y):
+            return _contig(rec.evaluation('f', lambda: sde.f(t, y), t, y) if rec is not None else sde.f(t, y))
+
+        def g(t, y):
+            return _gop(rec.evaluation('g', lambda: sde.g(t, y), t, y) if rec is not None else sde.g(t, y))
+
         # f0, g(t1, y0) and g(t0, y0) share their inputs: three parallel branches
-        f0, ga, gb = self._fork(lambda: _contig(sde.f(t_00, y0)), lambda: _gop(sde.g(t_1, y0)),
-                                lambda: _gop(sde.g(t_00, y0)))
+        f0, ga, gb = self._fork(lambda: f(t_00, y0), lambda: g(t_1, y0), lambda: g(t_00, y0))
         h0_1 = self._k('tsde_srk_additive_stage', self._L, self._feed.get(c, True), (y0, f0, ga), (c.dt, s['rdt']),
                        None)
-        f1 = _contig(sde.f(t_34, h0_1))
+        f1 = f(t_34, h0_1)
+        if rec is not None:
+            self._pw = pointwise.compile_general(self, rec, rec.finish()) or False
         return self._k('tsde_step_srk_additive', self._L, self._feed.get(c, True), (y0, f0, f1, ga, gb),
                        (c.dt, s['rdt']), out)
 

@@ -97,7 +97,10 @@ with 1 <= m <= TSDE_PW_GENERAL_MAX_M Brownian channels record f as above and g a
 with per-channel operands ((d, m) and (m,) tensors) and `y.unsqueeze(-1)`; the program is compiled into kernels of its
 own that evaluate g_ij in registers and contract it with the increments in the unfused launch's summation order, and
 they run on the solver's GENERAL launch of tsde_solve_euler_pointwise (chunks, as Euler's) and
-tsde_step_predictor_corrector_pointwise (midpoint).  Every other method keeps diagonal-only tapes.
+tsde_step_predictor_corrector_pointwise (midpoint).  A fixed-step additive-noise SRK solve (sra1) records its step's
+four evaluations f0, gA, gB, f1 the same way (pattern 'fggf'); its program is tagged PW_LAYOUT_GENERAL_SRA and every
+later step is one launch of tsde_step_srk_diag_pointwise on the solver's GENERAL launch, which draws W and U and
+contracts g three times, with the weights of the unfused stage and final launches.  Every other method keeps diagonal-only tapes.
 """
 import ctypes
 import numbers
@@ -645,14 +648,18 @@ class SrkRecorder(Recorder):
             return None
 
 
+SRA_PATTERN = 'fggf'  # an additive-noise SRK step's evaluations, in the order methods.SRK._additive_step makes them
+
+
 def _pad3(shape):
     return (1,) * (3 - len(shape)) + tuple(shape)
 
 
 class GeneralRecorder(SrkRecorder):
-    """Records the f and g evaluations of a general- or additive-noise Euler ('fg') or midpoint ('fgfg') step, whose
-    g is (rows, d, m).  A value is either of the (rows, d) class of the diagonal tapes or per channel: computed by an
-    op whose result is three-dimensional, or not of a (rows, d) shape, or that reads a per-channel value (`_wide`).
+    """Records the f and g evaluations of a general- or additive-noise Euler ('fg') or midpoint ('fgfg') step, or of an
+    additive-noise SRK step ('fggf': f0, gA, gB, f1, methods.SRK._additive_step), whose g is (rows, d, m).  A value is
+    either of the (rows, d) class of the diagonal tapes or per channel: computed by an op whose result is
+    three-dimensional, or not of a (rows, d) shape, or that reads a per-channel value (`_wide`).
     Per-channel ops broadcast as torch does, right-aligned on (rows, d, m), and may read
       * per-channel values;
       * (rows, d)-class values only through `unsqueeze(-1)` (`y[..., None]`), as (rows, d, 1), or when they have one
@@ -660,7 +667,8 @@ class GeneralRecorder(SrkRecorder):
       * device tensors by their layout broadcast to (rows, d, m): one element (SCALAR), a (d, 1) column (CHANNEL),
         an (m,) row (M), a dense (d, m) block (DM); a (rows, d, m) tensor from outside the tape rejects it.
     f must be of the (rows, d) class; g must have the shape (rows, d, m) and may be any of those (an operand's
-    `expand` is additive noise).  The kernel derives which instructions are per channel from their sources alone."""
+    `expand` is additive noise).  The kernel derives which instructions are per channel from their sources alone.  The
+    program is tagged with its step's layout: PW_LAYOUT_GENERAL_SRA for SRK's pattern, else PW_LAYOUT_GENERAL."""
 
     def __init__(self, y, t, pattern, m):
         self.m = m
@@ -774,7 +782,7 @@ class GeneralRecorder(SrkRecorder):
 
     def _program(self, code, n_fg, results, n_regs, max_regs):
         prog, keep = super()._program(code, n_fg, results, n_regs, max_regs)
-        prog.reserved = _cabi.PW_LAYOUT_GENERAL
+        prog.reserved = _cabi.PW_LAYOUT_GENERAL_SRA if self.pattern == SRA_PATTERN else _cabi.PW_LAYOUT_GENERAL
         return prog, keep
 
     def _step_result(self, t, allow_go=False):
@@ -801,16 +809,18 @@ def recording(solver):
 
 def general(solver):
     """Whether `solver` runs general- or additive-noise steps that the element-wise general kernels serve: a fixed-step
-    Euler or midpoint solve (`_pw_general`) with 1 <= m <= TSDE_PW_GENERAL_MAX_M Brownian channels."""
+    Euler, midpoint or (additive-noise) SRK solve (`_pw_general`) with 1 <= m <= TSDE_PW_GENERAL_MAX_M Brownian
+    channels."""
     return (getattr(solver, '_pw_general', False) and not solver.adaptive
             and solver.sde.noise_type in (NOISE_TYPES.general, NOISE_TYPES.additive)
             and 1 <= solver.m <= _cabi.PW_GENERAL_MAX_M)
 
 
 def pc_recorder(solver, y, t, pattern):
-    """The recorder of this step of a Heun, midpoint or Euler-Heun `solver` (evaluations `pattern`), or None when it
-    is not the one to record.  Only an SDE whose f and g the step calls as the user's two callables is recorded: not
-    one with a user f_and_g (one call yields both), g_prod or f_and_g_prod, and not an adjoint SDE."""
+    """The recorder of this step of a Heun, midpoint, Euler-Heun, Euler or additive-noise SRK `solver` (evaluations
+    `pattern`), or None when it is not the one to record.  Only an SDE whose f and g the step calls as the user's two
+    callables is recorded: not one with a user f_and_g (one call yields both), g_prod or f_and_g_prod, and not an
+    adjoint SDE."""
     sde = solver.sde
     if (not recording(solver) or sde.f_and_g_prod_mode != 'fused' or sde.g_prod_mode != 'fused'
             or getattr(sde, 'user_f_and_g', True) or getattr(sde, 'is_adjoint_sde', False)):
@@ -821,8 +831,9 @@ def pc_recorder(solver, y, t, pattern):
 
 
 def compile_general(solver, rec, res):
-    """`res`, what a GeneralRecorder's `finish` returned, once the Euler and midpoint kernels of its program are compiled
-    and loaded (tsde_pointwise_compile on the solver's GENERAL launch), on the recording step as for
+    """`res`, what a GeneralRecorder's `finish` returned, once the Euler and midpoint kernels of its program (the sra1
+    kernels of an SRK program) are compiled and loaded (tsde_pointwise_compile on the solver's GENERAL launch), on the
+    recording step as for
     `compile_milstein`; None if `res` is, or if the library refuses or cannot compile the program (the tape is then
     rejected with the reason)."""
     global COMPILES

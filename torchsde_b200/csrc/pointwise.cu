@@ -1218,8 +1218,9 @@ static int pw_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_point
                       p, np, p.base.nquads, slots, TSDE_KERNEL_PW_CHUNK, st);
 }
 
-// GENERAL launches of tsde_solve_euler_pointwise, tsde_step_predictor_corrector_pointwise, tsde_pointwise_compile and
-// tsde_pointwise_source (general / additive noise; defined with the general-noise code generator below)
+// GENERAL launches of tsde_solve_euler_pointwise, tsde_step_predictor_corrector_pointwise,
+// tsde_step_srk_diag_pointwise, tsde_pointwise_compile and tsde_pointwise_source (general / additive noise; defined
+// with the general-noise code generator below)
 template <typename T>
 static int pw_general_euler(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
                             const tsde_pw_step* steps, int32_t n_steps);
@@ -1229,6 +1230,10 @@ static int pw_general_midpoint_step(const tsde_launch* L, const tsde_noise* nz, 
                                     double half_dt, void* y1);
 template <typename T>
 static int pw_general_compiled(const tsde_launch* L, const tsde_pointwise* prog, PwCompiled& kc);
+template <typename T>
+static int pw_general_sra1_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                const void* y0, const void* t_1, const void* t_34, const void* t_00, double dt,
+                                double rdt, void* y1);
 template <typename T>
 static int64_t pw_general_source_of(const tsde_launch* L, const tsde_pointwise* prog, char* buf, int64_t size);
 
@@ -1278,6 +1283,10 @@ TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_no
                                              const void* y0, const void* t_0, const void* t_1, const void* t_q,
                                              const void* t_h, double dt, double rdt, double sqrt_dt, double three_dt,
                                              void* y1) {
+  if (valid_launch(L) && L->noise_type == TSDE_NOISE_GENERAL)  // additive noise: sra1, t_q = t0 + 3/4 dt
+    return dispatch(L, [&](auto t) -> int {
+      return pw_general_sra1_step<decltype(t)>(L, nz, prog, y0, t_1, t_q, t_0, dt, rdt, y1);
+    });
   if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
   return dispatch(L, [&](auto t) -> int {
     using T = decltype(t);
@@ -1497,18 +1506,19 @@ TSDE_EXPORT int tsde_adaptive_pointwise_compile(const tsde_launch* L, const tsde
   });
 }
 
-// ---- general / additive noise (tsde_solve_euler_general_pointwise, tsde_step_midpoint_general_pointwise) ------------
+// ---- general / additive noise (GENERAL launches) -------------------------------------------------------------------
 // The two-program layout with per-channel values.  A g program runs m times per output, so it is compiled, never
 // interpreted (an interpreted instruction costs about 30 SASS instructions, DESIGN §4): pw_general_source writes it
-// out as a `Prog` for pw_general_euler_steps / pw_general_midpoint (pw_device.cuh), with the IEEE options and the
-// cache of the Milstein kernels.  A g instruction is per channel when one of its sources is (a DM or M operand, or a
-// per-channel value); the others are per (row, d) element, evaluated once per lane before the channel loop.  The
-// contraction of each lane's m values with the increments is written out for the route the unfused step takes
-// (gen_route), as that kernel sums:
+// out as a `Prog` for pw_general_euler_steps / pw_general_midpoint, or for pw_general_sra1 when the program is tagged
+// TSDE_PW_LAYOUT_GENERAL_SRA (pw_device.cuh), with the IEEE options and the cache of the Milstein kernels.  A g
+// instruction is per channel when one of its sources is (a DM or M operand, or a per-channel value); the others are
+// per (row, d) element, evaluated once per lane before the channel loop.  The contraction of each lane's m values with
+// the increments is written out for the route the unfused step takes (gen_route), as that kernel sums:
 //   TSDE_GEN_ROWWISE   g * w                                       (the row-wise kernels' single product)
 //   TSDE_GEN_TILE      per channel quad an fma chain from 0; the quad sums as the xor-butterfly adds them, a pairwise
 //                      tree in natural order                       (gen_cta_kernel, gen_tma_kernel)
 //   TSDE_GEN_GENERIC   left to right from 0, a rounded multiply and a rounded add per channel    (gen_kernel)
+// (the sra1 launches never take the row-wise kernels: their m == 1 route is TSDE_GEN_GENERIC, pw_general_program).
 // Register use stays bounded: m <= TSDE_PW_GENERAL_MAX_M increments per thread, and the tree keeps at most
 // log2(m / 4) + 1 partial sums.
 
@@ -1519,6 +1529,8 @@ static_assert(sizeof(PwOperands<double>) + sizeof(PwP<double>) + sizeof(NoiseP<d
               "the compiled general Euler kernel's parameters fit the 4 KiB parameter space");
 static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralMidP<double>) + sizeof(NoiseP<double>) <= 4096,
               "the compiled general midpoint kernel's parameters fit the 4 KiB parameter space");
+static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralSraP<double>) + sizeof(NoiseP<double>) <= 4096,
+              "the compiled sra1 kernel's parameters fit the 4 KiB parameter space");
 
 static bool pw_per_channel_kind(int kind) { return kind == TSDE_PW_DM || kind == TSDE_PW_M; }
 
@@ -1534,10 +1546,12 @@ static bool pw_valid_general(const tsde_pointwise& pg) {
   return !per_channel(pg.f_src);
 }
 
-// A launch and program the general kernels serve; `route` is the contraction order (gen_route) for dtype size `s`.
-static bool pw_general_program(const tsde_launch* L, const tsde_pointwise* prog, int64_t s, int& route) {
+// A launch and program of layout tag `layout` the general kernels serve; `route` is the contraction order (gen_route)
+// for dtype size `s`.
+static bool pw_general_program(const tsde_launch* L, const tsde_pointwise* prog, int64_t s, int& route,
+                               int layout = TSDE_PW_LAYOUT_GENERAL) {
   if (!valid_launch(L) || L->noise_type != TSDE_NOISE_GENERAL || L->m > TSDE_PW_GENERAL_MAX_M || !prog ||
-      prog->reserved != TSDE_PW_LAYOUT_GENERAL)
+      prog->reserved != layout)
     return false;
   bool vec = true;
   if (!pw_valid_tables(*prog, &vec, TSDE_PW_M) || !pw_valid_general(*prog)) return false;
@@ -1547,13 +1561,21 @@ static bool pw_general_program(const tsde_launch* L, const tsde_pointwise* prog,
   if (g >= TSDE_PW_OPERAND(0) && g != TSDE_PW_SRC_Y && g != TSDE_PW_SRC_GO &&
       prog->operand[g - TSDE_PW_OPERAND(0)].kind == TSDE_PW_DM)
     quads = aligned16(prog->operand[g - TSDE_PW_OPERAND(0)].ptr);
-  route = gen_route(L->m, quads, L->m * s);
+  if (layout == TSDE_PW_LAYOUT_GENERAL_SRA) {
+    // the sra1 launches call launch_gen directly, which stages U too, and take gen_kernel where cabi.cu would take the
+    // row-wise kernels (m == 1: the sum 0 + g * w, which turns a -0 product into +0)
+    route = gen_route(L->m, quads, 2 * L->m * s);
+    if (route == TSDE_GEN_ROWWISE) route = TSDE_GEN_GENERIC;
+  } else {
+    route = gen_route(L->m, quads, L->m * s);
+  }
   return route != TSDE_GEN_WIDE;
 }
 
 // The translation unit of a program that passed pw_general_program, for m channels and contraction `route`: the
-// kernels of Euler chunks and of a midpoint step.
-static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t m, int route) {
+// kernels of Euler chunks and of a midpoint step, or for an SRA-tagged program (`layout`) those of an sra1 step.
+static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t m, int route,
+                                     int layout = TSDE_PW_LAYOUT_GENERAL) {
   const char* T = f64 ? "double" : "float";
   const std::string fs = f64 ? "" : "f", M = num((int)m);
   const int mq = (int)((m + 3) / 4);
@@ -1691,6 +1713,16 @@ static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t
   }
   o += "      out[j] = acc;\n    }\n  }\n};\n}  // namespace\n}  // namespace tsde\n";
   const std::string bounds = "__launch_bounds__(" + num(kThreads) + ", 1)";
+  if (layout == TSDE_PW_LAYOUT_GENERAL_SRA) {
+    for (const char* v : {"single", "multi"}) {
+      const std::string src = v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti";
+      o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_general_sra1_" + v +
+           "(const __grid_constant__ tsde::PwOperands<tsde::T> ops,\n"
+           "    const __grid_constant__ tsde::PwGeneralSraP<tsde::T> p, const tsde::NoiseP<tsde::T> nz) {\n"
+           "  tsde::pw_general_sra1<tsde::T, " + src + ", tsde::Prog>(ops, p, nz);\n}\n";
+    }
+    return o;
+  }
   for (const char* v : {"single", "multi"}) {
     const std::string src = v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti";
     o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_general_euler_" + v +
@@ -1708,11 +1740,22 @@ static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t
   return o;
 }
 
+// The layout a GENERAL launch of tsde_pointwise_compile / tsde_pointwise_source serves `prog` in: the sra1 unit for an
+// SRA-tagged program, else the Euler / midpoint unit (which refuses every other tag).
+static int pw_general_layout(const tsde_pointwise* prog) {
+  return prog && prog->reserved == TSDE_PW_LAYOUT_GENERAL_SRA ? TSDE_PW_LAYOUT_GENERAL_SRA : TSDE_PW_LAYOUT_GENERAL;
+}
+
+// The loaded kernels of a general-layout program: Euler's two, then midpoint's two; of an SRA-tagged one, sra1's two.
 template <typename T>
 static int pw_general_compiled(const tsde_launch* L, const tsde_pointwise* prog, PwCompiled& kc) {
   int route;
-  if (!pw_general_program(L, prog, sizeof(T), route)) return TSDE_EINVAL;
-  return pw_loaded(pw_general_source(*prog, sizeof(T) == 8, L->m, route),
+  const int layout = pw_general_layout(prog);
+  if (!pw_general_program(L, prog, sizeof(T), route, layout)) return TSDE_EINVAL;
+  std::string src = pw_general_source(*prog, sizeof(T) == 8, L->m, route, layout);
+  if (layout == TSDE_PW_LAYOUT_GENERAL_SRA)
+    return pw_loaded(std::move(src), {"tsde_pw_general_sra1_single", "tsde_pw_general_sra1_multi"}, kc);
+  return pw_loaded(std::move(src),
                    {"tsde_pw_general_euler_single", "tsde_pw_general_euler_multi", "tsde_pw_general_midpoint_single",
                     "tsde_pw_general_midpoint_multi"},
                    kc);
@@ -1798,12 +1841,48 @@ static int pw_general_midpoint_step(const tsde_launch* L, const tsde_noise* nz, 
   return e;
 }
 
+// tsde_step_srk_diag_pointwise for a GENERAL launch: one sra1 step as one launch of the SRA-tagged program's
+// compiled kernel.
+template <typename T>
+static int pw_general_sra1_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                const void* y0, const void* t_1, const void* t_34, const void* t_00, double dt,
+                                double rdt, void* y1) {
+  int route;
+  if (!t_1 || !t_34 || !t_00 || !y0 || !y1 || !nz || nz->source != TSDE_SRC_COUNTER || nz->flags ||
+      !pw_general_program(L, prog, sizeof(T), route, TSDE_PW_LAYOUT_GENERAL_SRA))
+    return TSDE_EINVAL;
+  bool vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y1);
+  pw_valid_tables(*prog, &vec, TSDE_PW_M);
+  NoiseP<T> np;
+  if (int e = fill_noise<T>(L, nz, false, np)) return e;
+  PwCompiled kc;
+  if (int e = pw_general_compiled<T>(L, prog, kc)) return e;
+  PwOperands<T> ops = pw_operands<T>(prog);
+  PwGeneralSraP<T> p{};
+  p.base.y0 = static_cast<const T*>(y0);
+  p.base.y1 = static_cast<T*>(y1);
+  p.base.t0 = static_cast<const T*>(t_00);
+  p.base.dt = (T)dt;
+  fill_quad_map(L->rows, L->d, p.base);
+  p.base.vec = vec ? 1 : 0;
+  p.t_1 = static_cast<const T*>(t_1);
+  p.t_34 = static_cast<const T*>(t_34);
+  p.stage = GSraStageOp<T>{(T)dt, (T)rdt};
+  p.final_op = GSraFinalOp<T>{(T)dt, (T)rdt, (T)(1.0 / 3), (T)(2.0 / 3)};
+  void* args[] = {&ops, &p, &np};
+  const int e = launch_kernel_handle(kc.kernel[np.n_cells > 1 ? 1 : 0], (p.base.nquads + kThreads - 1) / kThreads,
+                                     kThreads, reinterpret_cast<cudaStream_t>(L->stream), args);
+  if (e == 0) g_launches[TSDE_KERNEL_PW_GENERAL].fetch_add(1, std::memory_order_relaxed);
+  return e;
+}
+
 // tsde_pointwise_source for a GENERAL launch
 template <typename T>
 static int64_t pw_general_source_of(const tsde_launch* L, const tsde_pointwise* prog, char* buf, int64_t size) {
   int route;
-  if (!pw_general_program(L, prog, sizeof(T), route)) return TSDE_EINVAL;
-  const std::string src = pw_general_source(*prog, sizeof(T) == 8, L->m, route);
+  const int layout = pw_general_layout(prog);
+  if (!pw_general_program(L, prog, sizeof(T), route, layout)) return TSDE_EINVAL;
+  const std::string src = pw_general_source(*prog, sizeof(T) == 8, L->m, route, layout);
   if (buf && size > 0) {
     const size_t n = std::min(src.size(), (size_t)size - 1);
     memcpy(buf, src.data(), n);

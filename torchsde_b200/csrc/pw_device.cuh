@@ -407,6 +407,35 @@ struct GMidpointPredictOp {
     o[0] = (e[0] + half_dt * e[1]) + T(0.5) * gp[0];
   }
 };
+// SRA1 stage: H0_1 = y0 + (3/4 f0) dt + gA.((3/2 U) rdt)             methods/srk.py:100-105, sra1.py:24-36
+template <typename T>
+struct GSraStageOp {
+  static constexpr int NE = 2, NG = 1, NP = 1, NO = 1;
+  static constexpr bool WANT_U = true;
+  T dt, rdt;
+  __device__ __forceinline__ T gval(int, const T (&g)[1]) const { return g[0]; }
+  __device__ __forceinline__ T weight(int, T, T u) const { return (T(1.5) * u) * rdt; }
+  __device__ __forceinline__ void combine(const T (&e)[2], const T (&gp)[1], T (&o)[1]) const {
+    o[0] = (e[0] + (T(0.75) * e[1]) * dt) + gp[0];
+  }
+};
+// SRA1 final: y1 = y0 + (1/3 f0) dt + gA.(W + (-U) rdt) + (2/3 f1) dt + gB.(0*W + U rdt)   srk.py:107-110
+template <typename T>
+struct GSraFinalOp {
+  static constexpr int NE = 3, NG = 2, NP = 2, NO = 1;
+  static constexpr bool WANT_U = true;
+  static constexpr bool STREAM_INPUTS = true;  // last kernel of the step: the g tiles are dead afterwards
+  T dt, rdt, third, two_thirds;
+  __device__ __forceinline__ T gval(int p, const T (&g)[2]) const { return g[p]; }
+  __device__ __forceinline__ T weight(int p, T w, T u) const {
+    return p == 0 ? (T(1) * w + (T(-1) * u) * rdt) : (T(0) * w + (T(1) * u) * rdt);
+  }
+  __device__ __forceinline__ void combine(const T (&e)[3], const T (&gp)[2], T (&o)[1]) const {
+    T y1 = (e[0] + (third * e[1]) * dt) + gp[0];
+    y1 = (y1 + (two_thirds * e[2]) * dt) + gp[1];
+    o[0] = y1;
+  }
+};
 
 // ---- general / additive noise with an element-wise f and g (tsde_solve_euler_general_pointwise, ...) ---------------
 // One thread per (row, quad of d), as above.  The thread draws all m increments of its row (MQ channel quads on the
@@ -417,17 +446,26 @@ struct GMidpointPredictOp {
 //   f(ops, c, t, y, f)            the f program at (*t, y)
 //   gp(ops, c, t, y, w, gp)       the g program at (*t, y), contracted with w[0, 4 MQ)
 
-// The increments of this thread's row: channel k in w[k]
-template <typename T, int SRC, int MQ>
-__device__ __forceinline__ void pw_general_noise(const NoiseP<T>& nz, Key key, int64_t row, T (&w)[4 * MQ]) {
+// The increments of this thread's row: channel k in w[k], and with WANT_U its U in u[k]
+template <typename T, int SRC, int MQ, bool WANT_U>
+__device__ __forceinline__ void pw_general_noise(const NoiseP<T>& nz, Key key, int64_t row, T (&w)[4 * MQ],
+                                                 T (&u)[4 * MQ]) {
   const uint32_t grow = (uint32_t)(row + nz.row_offset);
 #pragma unroll
   for (int q = 0; q < MQ; ++q) {
     T w4[4], u4[4];
-    counter_noise<T, false, SRC == kSrcCounterMulti>(nz, key, grow, (uint32_t)q, w4, u4);
+    counter_noise<T, WANT_U, SRC == kSrcCounterMulti>(nz, key, grow, (uint32_t)q, w4, u4);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) w[4 * q + j] = w4[j];
+    for (int j = 0; j < 4; ++j) {
+      w[4 * q + j] = w4[j];
+      if (WANT_U) u[4 * q + j] = u4[j];
+    }
   }
+}
+template <typename T, int SRC, int MQ>
+__device__ __forceinline__ void pw_general_noise(const NoiseP<T>& nz, Key key, int64_t row, T (&w)[4 * MQ]) {
+  T u[4 * MQ];
+  pw_general_noise<T, SRC, MQ, false>(nz, key, row, w, u);
 }
 
 // Consecutive Euler steps, as pw_milstein_steps: y1 = GEulerOp{dt} on (y, f, g.dW)
@@ -512,6 +550,61 @@ __device__ __forceinline__ void pw_general_midpoint(const PwOperands<T>& ops, co
     yp[i] = o[0];
   }
   store_quad(p.base.y1, c.base, c.vec, c.nvalid, yp);
+}
+
+template <typename T>
+struct PwGeneralSraP {
+  PwP<T> base;                // y0, y1, the quad mapping and t0 = t_00, the time of f0 and gB
+  const T* t_1;               // the time of gA, t0 + dt
+  const T* t_34;              // the time of f1, t0 + 3/4 dt
+  GSraStageOp<T> stage;       // as tsde_srk_additive_stage and tsde_step_srk_additive build them
+  GSraFinalOp<T> final_op;
+};
+
+// One sra1 step (methods/srk.py:90-111): f0 = f(t_00, y0); H0_1 = GSraStageOp on (y0, f0, gA.wS) with gA = g(t_1, y0);
+// f1 = f(t_34, H0_1); y1 = GSraFinalOp on (y0, f0, f1, gA.w0, gB.w1) with gB = g(t_00, y0).  Each weight vector is the
+// op's weight(p, W_k, U_k) per channel, exactly as the unfused launches form it next to the contraction.
+template <typename T, int SRC, typename Prog>
+__device__ __forceinline__ void pw_general_sra1(const PwOperands<T>& ops, const PwGeneralSraP<T>& p,
+                                                const NoiseP<T>& nz) {
+  PwQuad c;
+  int64_t Q, row, q;
+  pw_locate(p.base, c, Q, row, q);
+  T w[4 * Prog::MQ], u[4 * Prog::MQ];
+  pw_general_noise<T, SRC, Prog::MQ, true>(nz, load_key(nz.key), row, w, u);
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (Q >= p.base.nquads) return;
+  Prog prog;
+  T y0[4], f0[4], h[4], ga[4], gb[4], wt[4 * Prog::MQ];
+  load_quad(p.base.y0, c.base, c.vec, c.nvalid, y0);
+  prog.load(ops, c);
+  prog.f(ops, c, p.base.t0, y0, f0);
+#pragma unroll
+  for (int k = 0; k < 4 * Prog::MQ; ++k) wt[k] = p.stage.weight(0, w[k], u[k]);
+  prog.gp(ops, c, p.t_1, y0, wt, ga);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const T e[2] = {y0[i], f0[i]}, g1[1] = {ga[i]};
+    T o[1];
+    p.stage.combine(e, g1, o);
+    h[i] = o[0];
+  }
+#pragma unroll
+  for (int k = 0; k < 4 * Prog::MQ; ++k) wt[k] = p.final_op.weight(0, w[k], u[k]);
+  prog.gp(ops, c, p.t_1, y0, wt, ga);
+#pragma unroll
+  for (int k = 0; k < 4 * Prog::MQ; ++k) wt[k] = p.final_op.weight(1, w[k], u[k]);
+  prog.gp(ops, c, p.base.t0, y0, wt, gb);
+  T f1[4];
+  prog.f(ops, c, p.t_34, h, f1);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const T e[3] = {y0[i], f0[i], f1[i]}, g2[2] = {ga[i], gb[i]};
+    T o[1];
+    p.final_op.combine(e, g2, o);
+    h[i] = o[0];
+  }
+  store_quad(p.base.y1, c.base, c.vec, c.nvalid, h);
 }
 
 }  // namespace tsde

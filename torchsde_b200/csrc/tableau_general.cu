@@ -883,7 +883,8 @@ static int launch_gen_fmt(const tsde_launch* L, const tsde_noise* nz, std::initi
 }
 
 // ---- ops ---------------------------------------------------------------------------------------
-// (GEulerOp and GMidpointPredictOp: pw_device.cuh, which the run-time compiled general-noise kernels include too)
+// (GEulerOp, GMidpointPredictOp, GSraStageOp and GSraFinalOp: pw_device.cuh, which the run-time compiled general-noise
+// kernels include too)
 // y1 = y0 + (dt*(f+f') + g.dW + g'.dW) * 0.5                                     methods/heun.py:46
 template <typename T>
 struct GHeunOp {
@@ -951,36 +952,6 @@ struct GRevHeunOp {
     o[0] = backward ? ((e[0] - fd) - gp[0]) : ((e[0] + fd) + gp[0]);
   }
 };
-// SRA1 stage: H0_1 = y0 + (3/4 f0) dt + gA.((3/2 U) rdt)             methods/srk.py:100-105, sra1.py:24-36
-template <typename T>
-struct GSraStageOp {
-  static constexpr int NE = 2, NG = 1, NP = 1, NO = 1;
-  static constexpr bool WANT_U = true;
-  T dt, rdt;
-  __device__ __forceinline__ T gval(int, const T (&g)[1]) const { return g[0]; }
-  __device__ __forceinline__ T weight(int, T, T u) const { return (T(1.5) * u) * rdt; }
-  __device__ __forceinline__ void combine(const T (&e)[2], const T (&gp)[1], T (&o)[1]) const {
-    o[0] = (e[0] + (T(0.75) * e[1]) * dt) + gp[0];
-  }
-};
-// SRA1 final: y1 = y0 + (1/3 f0) dt + gA.(W + (-U) rdt) + (2/3 f1) dt + gB.(0*W + U rdt)   srk.py:107-110
-template <typename T>
-struct GSraFinalOp {
-  static constexpr int NE = 3, NG = 2, NP = 2, NO = 1;
-  static constexpr bool WANT_U = true;
-  static constexpr bool STREAM_INPUTS = true;  // last kernel of the step: the g tiles are dead afterwards
-  T dt, rdt, third, two_thirds;
-  __device__ __forceinline__ T gval(int p, const T (&g)[2]) const { return g[p]; }
-  __device__ __forceinline__ T weight(int p, T w, T u) const {
-    return p == 0 ? (T(1) * w + (T(-1) * u) * rdt) : (T(0) * w + (T(1) * u) * rdt);
-  }
-  __device__ __forceinline__ void combine(const T (&e)[3], const T (&gp)[2], T (&o)[1]) const {
-    T y1 = (e[0] + (third * e[1]) * dt) + gp[0];
-    y1 = (y1 + (two_thirds * e[2]) * dt) + gp[1];
-    o[0] = y1;
-  }
-};
-
 // ---- outer-product bookkeeping of the reversible-Heun adjoint (g-shaped element-wise) ----------
 // out[b,dd,mm] = (base ? base[b,dd,mm] : 0) + a1[b,dd]*(c1*w[b,mm]) (+ a2[b,dd]*(c2*w[b,mm]))
 // reversible_heun.py:95-96,105,115 (a) and :114,140 (b)
