@@ -277,6 +277,14 @@ int tsde_step_milstein(const tsde_launch* L, const tsde_noise* nz, const void* y
  *   ABS  fabs(a)
  *   SEL  dst = dst != 0 ? a : b: the condition is the destination register itself, which must have been written
  *        (torch.where, masked_fill).
+ * Transcendental opcodes (16 and up), valid only in the programs the library compiles (this Milstein layout, its
+ * adaptive proposal, and the general layouts TSDE_PW_LAYOUT_GENERAL and TSDE_PW_LAYOUT_GENERAL_SRA); the interpreted
+ * entry points refuse them.  Each is the lambda of the ATen CUDA kernel it restates, in T, compiled apart from the
+ * program with FMA contraction on, as ATen's kernels are (libdevice's exp, log, ... of T):
+ *   EXP exp(a)   LOG log(a)   SIN sin(a)   COS cos(a)   TANH tanh(a)   LOG1P log1p(a)   EXPM1 expm1(a)
+ *   RSQRT rsqrt(a)   SIGMOID 1 / (1 + exp(-a))   (unary: b unused)
+ *   POW  pow(a, b), b an IMM operand (torch.pow with a scalar exponent off ATen's special cases)
+ *   TANH_BACKWARD  a * (1 - b * b)   SIGMOID_BACKWARD  a * (1 - b) * b   (a the gradient, b the forward result)
  *   IMM      value `imm` (a value of the state dtype, stored as double)
  *   T0       the 0-d step time `t0` of the call (state dtype)
  *   SCALAR   ptr[0]                 (a one-element device tensor)
@@ -295,6 +303,9 @@ int tsde_step_milstein(const tsde_launch* L, const tsde_noise* nz, const void* y
 enum { TSDE_PW_MUL = 0, TSDE_PW_ADD = 1, TSDE_PW_SUB = 2, TSDE_PW_DIV = 3, TSDE_PW_NEG = 4, TSDE_PW_SQRT = 5 };
 enum { TSDE_PW_LT = 8, TSDE_PW_LE = 9, TSDE_PW_EQ = 10, TSDE_PW_MAXIMUM = 11, TSDE_PW_MINIMUM = 12, TSDE_PW_ABS = 13,
        TSDE_PW_SEL = 14 };
+enum { TSDE_PW_EXP = 16, TSDE_PW_LOG = 17, TSDE_PW_SIN = 18, TSDE_PW_COS = 19, TSDE_PW_TANH = 20,
+       TSDE_PW_LOG1P = 21, TSDE_PW_EXPM1 = 22, TSDE_PW_RSQRT = 23, TSDE_PW_SIGMOID = 24, TSDE_PW_POW = 25,
+       TSDE_PW_TANH_BACKWARD = 26, TSDE_PW_SIGMOID_BACKWARD = 27 };
 enum { TSDE_PW_IMM = 0, TSDE_PW_T0 = 1, TSDE_PW_SCALAR = 2, TSDE_PW_CHANNEL = 3, TSDE_PW_ROW = 4 };
 typedef struct tsde_pw_instr {
   uint8_t op, dst, a, b;

@@ -8,6 +8,7 @@ There is deliberately no fallback: if the shared library is missing, importing t
 raises (`LibraryNotBuilt`) telling the user to run ``python __graft_entry__.py`` (build()).
 """
 import ctypes
+import importlib
 import os
 
 import torch
@@ -103,6 +104,9 @@ PW_MAX_INSTR, PW_MAX_OPERANDS, PW_MAX_REGS = 96, 24, 24  # TSDE_PW_MAX_*
 PW_SRC_Y, PW_SRC_GO, PW_OPERAND0 = 0xFE, 0xFF, 0x80
 PW_MUL, PW_ADD, PW_SUB, PW_DIV, PW_NEG, PW_SQRT = range(6)
 PW_LT, PW_LE, PW_EQ, PW_MAXIMUM, PW_MINIMUM, PW_ABS, PW_SEL = range(8, 15)  # (6, 7 reserved)
+# the transcendental ops, which only the compiled layouts run (15 reserved)
+(PW_EXP, PW_LOG, PW_SIN, PW_COS, PW_TANH, PW_LOG1P, PW_EXPM1, PW_RSQRT, PW_SIGMOID, PW_POW, PW_TANH_BACKWARD,
+ PW_SIGMOID_BACKWARD) = range(16, 28)
 PW_IMM, PW_T0, PW_SCALAR, PW_CHANNEL, PW_ROW, PW_DM, PW_M = range(7)  # (DM, M: the general layout's g only)
 PW_SRK_MAX_REGS = 18  # TSDE_PW_SRK_MAX_REGS
 KERNEL_PW_MILSTEIN = 3  # TSDE_KERNEL_PW_MILSTEIN
@@ -202,22 +206,60 @@ SIGNATURES = {
 _lib = None
 
 
+def _preload(package, name):
+    """Load `name` from the nvidia package `package` PyTorch installs, if there is one, so that the library's dlopen
+    finds it; the handle, or None."""
+    try:
+        pkg = importlib.import_module(f'nvidia.{package}')
+    except ImportError:
+        return None
+    for d in getattr(pkg, '__path__', ()):
+        path = os.path.join(d, 'lib', name)
+        if os.path.exists(path):
+            try:
+                return ctypes.CDLL(path, mode=ctypes.RTLD_GLOBAL)
+            except OSError:
+                continue
+    return None
+
+
 def _preload_nvrtc():
     """Load NVRTC from the nvidia-cuda-nvrtc package PyTorch installs, if there is one, so that the library's
     dlopen("libnvrtc.so.12") finds it when the Milstein programs are compiled (tsde_pointwise_compile).  Without it the
     library still loads, and those solves keep the unfused step."""
-    try:
-        import nvidia.cuda_nvrtc as pkg
-    except ImportError:
-        return
-    for d in getattr(pkg, '__path__', ()):
-        path = os.path.join(d, 'lib', 'libnvrtc.so.12')
-        if os.path.exists(path):
+    _preload('cuda_nvrtc', 'libnvrtc.so.12')
+
+
+_nvjitlink = None
+
+
+def nvjitlink():
+    """nvJitLink, which links the programs with transcendental ops, loaded (once) from the nvidia-nvjitlink package
+    PyTorch installs, else from the library path, so that the library's dlopen("libnvJitLink.so.12") finds it; None
+    if there is none.  Only a solve that records a transcendental op loads it."""
+    global _nvjitlink
+    if _nvjitlink is None:
+        _nvjitlink = _preload('nvjitlink', 'libnvJitLink.so.12')
+        if _nvjitlink is None:
             try:
-                ctypes.CDLL(path, mode=ctypes.RTLD_GLOBAL)
+                _nvjitlink = ctypes.CDLL('libnvJitLink.so.12', mode=ctypes.RTLD_GLOBAL)
             except OSError:
-                continue
-            return
+                return None
+    return _nvjitlink
+
+
+def nvrtc_version():
+    """(major, minor) of the NVRTC the library compiles programs with (the libnvrtc.so.12 its dlopen finds: the
+    package's, preloaded), or None if there is none."""
+    lib()
+    try:
+        nv = ctypes.CDLL('libnvrtc.so.12')
+    except OSError:
+        return None
+    major, minor = ctypes.c_int(), ctypes.c_int()
+    if nv.nvrtcVersion(ctypes.byref(major), ctypes.byref(minor)) != 0:
+        return None
+    return major.value, minor.value
 
 
 def lib():

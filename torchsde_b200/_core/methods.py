@@ -200,7 +200,7 @@ class BaseMilstein(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
                                     (c.t0.data_ptr(), c.dt, ito), out), ()
         track = self._autograd
         # the first step of an eligible solve runs as always, with the user's ops recorded
-        rec = pointwise.Recorder(y0, c.t0) if pointwise.recording(self) else None
+        rec = pointwise.Recorder(y0, c.t0, pointwise.transcendental(self)) if pointwise.recording(self) else None
         raw = {}
 
         def user(name, fn, **kw):
@@ -535,7 +535,8 @@ class SRK(_ProposalMixin, base_solver.BaseSDESolver):
                                     (t_00.data_ptr(), t_1.data_ptr(), t_q.data_ptr(), t_h.data_ptr(), c.dt, s['rdt'],
                                      s['sqrt_dt'], s['three_dt']), out)
         # the first step of an eligible solve runs as always, with the user's seven evaluations recorded
-        rec = pointwise.SrkRecorder(y0, t_00) if pointwise.recording(self) else None
+        rec = pointwise.SrkRecorder(y0, t_00, transcendental=pointwise.transcendental(self)) \
+            if pointwise.recording(self) else None
 
         def f(t, y):
             return _contig(rec.evaluation('f', lambda: sde.f(t, y), t, y) if rec is not None else sde.f(t, y))

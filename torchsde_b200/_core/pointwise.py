@@ -31,6 +31,22 @@ whose storage was written in place through another tensor (a view, `detach()`, `
 storage with a value of the tape, a 16-bit result, a tensor created by a factory — rejects the tape, and the solve
 keeps its ordinary step.
 
+Transcendental ops, with options={'transcendental': True} only (`Recorder.transcendental`, `_allow`):
+
+    exp, log, sin, cos, tanh, log1p, expm1, rsqrt, sigmoid; tanh_backward and sigmoid_backward (what autograd emits
+    for tanh and sigmoid in Milstein's vjp); pow with a scalar exponent as ATen's CUDA kernel dispatches it (`_pow`:
+    0.5 sqrt, -0.5 rsqrt, -1 reciprocal, then the exponent rounded to the state dtype: 2 and 3 products, -2 one over
+    the square, any other a pow, 0 and 1 rejected).
+
+They are libdevice code, not correctly rounded, and ATen's kernels contract their arithmetic into FMAs: the library
+compiles each as a function of its own with ATen's lambda as its body and FMA contraction on, and links it to the
+program (csrc/pointwise.cu, kPwHelpers), so only the compiled layouts take them: Milstein (fixed-step and adaptive)
+and the general / additive-noise Euler, midpoint and sra1 kernels.  The interpreted ones (`SrkRecorder` on diagonal
+noise: SRK, Heun, midpoint, Euler-Heun, Euler, reversible Heun) reject such a tape with the reason.  So does every
+recorder when the NVRTC the library compiles with is not the CUDA release PyTorch was built with (`nvrtc_mismatch`),
+or when there is no nvJitLink to link with (loaded only then, `_cabi.nvjitlink`).
+Without the option the tapes hold what they always held: the default keeps the unfused step for these SDEs.
+
 Bools.  A comparison or logical result is a bool tensor; in the program it is a register holding 0 or 1 of the state
 dtype (logical_and is then a product, logical_or a maximum, logical_not 1 - c, ne 1 - eq, gt / ge lt / le with the
 operands swapped, all exact).  A bool may only be the condition of where / masked_fill or an operand of a logical op:
@@ -141,6 +157,14 @@ _IN_PLACE = {aten.mul_.Tensor: aten.mul.Tensor, aten.add_.Tensor: aten.add.Tenso
              aten.masked_fill_.Scalar: aten.masked_fill.Scalar, aten.logical_and_.default: aten.logical_and.default,
              aten.logical_or_.default: aten.logical_or.default, aten.bitwise_and_.Tensor: aten.bitwise_and.Tensor,
              aten.bitwise_or_.Tensor: aten.bitwise_or.Tensor}
+# the transcendental ops (options={'transcendental': True}; the compiled layouts only): op -> opcode, with the unary
+# ones' operand in source a and the backward ops' gradient in a, their forward result in b
+_TRANSCENDENTAL = {aten.exp.default: _cabi.PW_EXP, aten.log.default: _cabi.PW_LOG, aten.sin.default: _cabi.PW_SIN,
+                   aten.cos.default: _cabi.PW_COS, aten.tanh.default: _cabi.PW_TANH,
+                   aten.log1p.default: _cabi.PW_LOG1P, aten.expm1.default: _cabi.PW_EXPM1,
+                   aten.rsqrt.default: _cabi.PW_RSQRT, aten.sigmoid.default: _cabi.PW_SIGMOID}
+_BACKWARD = {aten.tanh_backward.default: _cabi.PW_TANH_BACKWARD,
+             aten.sigmoid_backward.default: _cabi.PW_SIGMOID_BACKWARD}
 _ALIAS = {aten.view.default, aten._unsafe_view.default, aten.expand.default, aten.unsqueeze.default,
           aten.detach.default, aten.alias.default}
 
@@ -151,6 +175,23 @@ FOREIGN = ('foreign',)  # a value bound by an earlier evaluation of an SRK step
 
 class Reject(Exception):
     pass
+
+
+def nvrtc_mismatch():
+    """Why the transcendental ops cannot be compiled to ATen's bits here, or None.  They are libdevice code, which is
+    not correctly rounded: the program's NVRTC must be the CUDA release (major.minor) PyTorch was built with."""
+    have, want = _cabi.nvrtc_version(), torch.version.cuda
+    if have is None:
+        return "no NVRTC to compile the transcendental ops with"
+    if want is None or tuple(int(x) for x in want.split('.')[:2]) != have:
+        return (f"NVRTC {have[0]}.{have[1]} is not the CUDA {want} that PyTorch was built with: its libdevice may "
+                f"compute the transcendental ops otherwise")
+    return None
+
+
+def transcendental(solver):
+    """Whether `solver` fuses the transcendental ops (options={'transcendental': True})."""
+    return bool(solver.options.get('transcendental', False))
 
 
 def _strip(shape):
@@ -225,10 +266,15 @@ def _allocate(instrs, reads):
 
 
 class Recorder(TorchDispatchMode):
-    """Records the element-wise tape of one Milstein step; `finish` turns it into a tsde_pointwise program."""
+    """Records the element-wise tape of one Milstein step; `finish` turns it into a tsde_pointwise program.  With
+    `transcendental`, the tape may hold the transcendental ops too (`_TRANSCENDENTAL`, `_BACKWARD`, `_pow`): the
+    library compiles this recorder's programs (`compiled`)."""
 
-    def __init__(self, y, t0):
+    compiled = True
+
+    def __init__(self, y, t0, transcendental=False):
         super().__init__()
+        self.transcendental = transcendental
         self.rows, self.d = y.shape
         self.dtype, self.device = y.dtype, y.device
         self.ok, self.reason = True, None
@@ -473,11 +519,16 @@ class Recorder(TorchDispatchMode):
         if func in _UNARY:
             self._emit(_UNARY[func], self._number(args[0]), None, out)
             return
+        if func in _TRANSCENDENTAL:
+            self._allow(func)
+            self._emit(_TRANSCENDENTAL[func], self._number(args[0]), None, out)
+            return
+        if func in _BACKWARD:
+            self._allow(func)
+            self._emit(_BACKWARD[func], self._number(args[0]), self._number(args[1]), out)
+            return
         if func is aten.pow.Tensor_Scalar:
-            if not (isinstance(args[1], numbers.Real) and not isinstance(args[1], bool) and args[1] == 2):
-                raise Reject(f"pow with exponent {args[1]!r}")
-            a = self._number(args[0])
-            self._emit(_cabi.PW_MUL, a, a, out)
+            self._pow(args[0], args[1], out)
             return
         if func not in _BINARY:
             raise Reject(f"{func} is not an element-wise op the kernel restates")
@@ -498,6 +549,45 @@ class Recorder(TorchDispatchMode):
             self._emit(_cabi.PW_MUL, self._number(a), self._operand(_cabi.PW_IMM, None, float(inv)), out)
             return
         self._emit(op, self._number(a), self._number(b), out)
+
+    def _allow(self, what):
+        """A transcendental op is about to be recorded: reject the tape unless this solve fuses them and can."""
+        if not self.transcendental:
+            raise Reject(f"{what} is not an element-wise op the kernel restates")
+        if not self.compiled:
+            raise Reject(f"{what} is fused by the compiled kernels only (Milstein, and Euler, midpoint and SRK on "
+                         f"general or additive noise), not by this method's")
+        reason = nvrtc_mismatch() or (None if _cabi.nvjitlink() else "no nvJitLink to link the transcendental ops")
+        if reason:
+            raise Reject(reason)
+
+    def _pow(self, x, p, out):
+        """pow(x, p) with a scalar exponent, as ATen's CUDA kernel dispatches it: p == 2 is x * x (always); with
+        `transcendental`, 0.5 is sqrt, -0.5 rsqrt, -1 reciprocal, and p rounded to the state dtype e then gives
+        x * x * x for 3, 1 / (x * x) for -2 (computed in double by ATen for float: one division rounded twice, first
+        to double, which gives the float quotient exactly) and pow(x, e) otherwise.  Exponents 0 and 1 are a fill and a
+        copy in ATen and reject the tape."""
+        if isinstance(p, bool) or not isinstance(p, numbers.Real) or p != 2 and (not self.transcendental or p in (0, 1)):
+            raise Reject(f"pow with exponent {p!r}")
+        a = self._number(x)
+        if p == 0.5:
+            self._emit(_cabi.PW_SQRT, a, None, out)
+        elif p == -1:
+            self._emit(_cabi.PW_DIV, self._one(), a, out)
+        elif p == -0.5:
+            self._allow(f"pow with exponent {p!r}")
+            self._emit(_cabi.PW_RSQRT, a, None, out)
+        else:
+            e = self._immediate(p)
+            if e == 2:
+                self._emit(_cabi.PW_MUL, a, a, out)
+            elif e == 3:
+                self._emit(_cabi.PW_MUL, self._value(_cabi.PW_MUL, a, a), a, out)
+            elif e == -2:
+                self._emit(_cabi.PW_DIV, self._one(), self._value(_cabi.PW_MUL, a, a), out)
+            else:
+                self._allow(f"pow with exponent {p!r}")
+                self._emit(_cabi.PW_POW, a, self._operand(_cabi.PW_IMM, None, e), out)
 
     # -- the program -----------------------------------------------------------------------------------------------
     def _step_result(self, t, allow_go=False):
@@ -586,10 +676,13 @@ class SrkRecorder(Recorder):
     accepts the tape when the f segments are one program (same ops, operands and order) and so are the g segments,
     and compiles the first of each into the two-program layout of tsde_step_srk_diag_pointwise and
     tsde_step_predictor_corrector_pointwise.  A Python-side branch between evaluations (or any other difference)
-    therefore keeps the ordinary step."""
+    therefore keeps the ordinary step.  Its kernels interpret the programs, so a transcendental op rejects the tape
+    (`compiled`)."""
 
-    def __init__(self, y, t, pattern='fgfgfgg', max_regs=_cabi.PW_SRK_MAX_REGS):
-        super().__init__(y, t)
+    compiled = False
+
+    def __init__(self, y, t, pattern='fgfgfgg', max_regs=_cabi.PW_SRK_MAX_REGS, transcendental=False):
+        super().__init__(y, t, transcendental)
         self.pattern, self.max_regs = pattern, max_regs
         self.segments = []  # (kind, first instruction, end, result source)
 
@@ -668,15 +761,18 @@ class GeneralRecorder(SrkRecorder):
         an (m,) row (M), a dense (d, m) block (DM); a (rows, d, m) tensor from outside the tape rejects it.
     f must be of the (rows, d) class; g must have the shape (rows, d, m) and may be any of those (an operand's
     `expand` is additive noise).  The kernel derives which instructions are per channel from their sources alone.  The
-    program is tagged with its step's layout: PW_LAYOUT_GENERAL_SRA for SRK's pattern, else PW_LAYOUT_GENERAL."""
+    program is tagged with its step's layout: PW_LAYOUT_GENERAL_SRA for SRK's pattern, else PW_LAYOUT_GENERAL.  Its
+    kernels are compiled, so with `transcendental` it takes the transcendental ops."""
 
-    def __init__(self, y, t, pattern, m):
+    compiled = True
+
+    def __init__(self, y, t, pattern, m, transcendental=False):
         self.m = m
         self._wide = set()     # the per-channel values
         self._lifted = set()   # id() of (rows, d)-class tensors viewed as (..., 1)
         self._w3 = False       # the op being recorded is per channel
         self._kind = None      # the evaluation being recorded, 'f' or 'g'
-        super().__init__(y, t, pattern, _cabi.PW_MAX_REGS)
+        super().__init__(y, t, pattern, _cabi.PW_MAX_REGS, transcendental)
 
     # -- the op's class ------------------------------------------------------------------------------------------
     def _is_bound(self, x):
@@ -826,8 +922,8 @@ def pc_recorder(solver, y, t, pattern):
             or getattr(sde, 'user_f_and_g', True) or getattr(sde, 'is_adjoint_sde', False)):
         return None
     if sde.noise_type != NOISE_TYPES.diagonal:
-        return GeneralRecorder(y, t, pattern, solver.m)
-    return SrkRecorder(y, t, pattern, _cabi.PW_MAX_REGS)
+        return GeneralRecorder(y, t, pattern, solver.m, transcendental(solver))
+    return SrkRecorder(y, t, pattern, _cabi.PW_MAX_REGS, transcendental(solver))
 
 
 def compile_general(solver, rec, res):

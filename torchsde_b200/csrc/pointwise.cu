@@ -271,16 +271,28 @@ static bool pw_valid_source(const tsde_pointwise& pg, uint32_t s, bool allow_go,
   return (int)s < pg.n_regs && ((written >> s) & 1u);
 }
 
-// NEG, SQRT and ABS read source a only
-static bool pw_unary(int op) { return op == TSDE_PW_NEG || op == TSDE_PW_SQRT || op == TSDE_PW_ABS; }
+// the transcendental opcodes, which only the compiled layouts run (pw_milstein_source, pw_general_source)
+static bool pw_transcendental(int op) { return op >= TSDE_PW_EXP && op <= TSDE_PW_SIGMOID_BACKWARD; }
 
-// instructions [i0, i1), run in order from the registers in `written`, which gains the ones they define
-static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, bool allow_go, uint64_t& written) {
+// NEG, SQRT, ABS and the transcendental ops of one argument read source a only
+static bool pw_unary(int op) {
+  return op == TSDE_PW_NEG || op == TSDE_PW_SQRT || op == TSDE_PW_ABS || (op >= TSDE_PW_EXP && op <= TSDE_PW_SIGMOID);
+}
+
+// instructions [i0, i1), run in order from the registers in `written`, which gains the ones they define; `compiled`:
+// the layout is compiled, so the transcendental opcodes are valid too (POW's exponent an IMM operand)
+static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, bool allow_go, uint64_t& written,
+                           bool compiled = false) {
   for (int i = i0; i < i1; ++i) {
     const tsde_pw_instr& in = pg.instr[i];
-    if ((in.op > TSDE_PW_SQRT && in.op < TSDE_PW_LT) || in.op > TSDE_PW_SEL) return false;
+    if (!(compiled && pw_transcendental(in.op)) &&
+        ((in.op > TSDE_PW_SQRT && in.op < TSDE_PW_LT) || in.op > TSDE_PW_SEL))
+      return false;
     if ((int)in.dst >= pg.n_regs || !pw_valid_source(pg, in.a, allow_go, written)) return false;
     if (!pw_unary(in.op) && !pw_valid_source(pg, in.b, allow_go, written)) return false;
+    if (in.op == TSDE_PW_POW && (in.b < TSDE_PW_OPERAND(0) || in.b == TSDE_PW_SRC_Y || in.b == TSDE_PW_SRC_GO ||
+                                 pg.operand[in.b - TSDE_PW_OPERAND(0)].kind != TSDE_PW_IMM))
+      return false;
     if (in.op == TSDE_PW_SEL && !((written >> in.dst) & 1u)) return false;  // the condition
     written |= 1ull << in.dst;
   }
@@ -416,6 +428,60 @@ static const std::string num(int x) {
   return b;
 }
 
+// ---- the transcendental ops (TSDE_PW_EXP .. TSDE_PW_SIGMOID_BACKWARD) -----------------------------------------------
+// libdevice's exp, log, sin, ... are not correctly rounded, and their code, like a * (1 - b * b), compiles to other
+// instructions when FMA contraction is on: ATen's kernels, built by nvcc with its default -fmad=true, contract; the
+// program translation units, compiled with -fmad=false, must not.  So each op is a __noinline__ function of a fixed
+// translation unit of its own, kPwHelpers, whose body is the lambda of the ATen CUDA kernel it restates (opmath is the
+// dtype itself for float and double), compiled by the same NVRTC with -fmad=true -rdc=true.  A program that uses one is
+// compiled with -rdc=true and calls it, and the two relocatable cubins are linked by nvJitLink without LTO, which would
+// recompile both under one fmad setting (pw_loaded).  Programs without these ops keep their source and the plain path.
+static const char kPwHelpers[] =
+    "// The transcendental ops of torchsde_b200's compiled element-wise programs, each as its ATen CUDA kernel's\n"
+    "// lambda; compiled with -fmad=true, as ATen is\n"
+    "namespace tsde {\n"
+    "#define TSDE_PW_OP1(name, ff, fd) \\\n"
+    "  __device__ __noinline__ float pw_##name(float a) { return ff; } \\\n"
+    "  __device__ __noinline__ double pw_##name(double a) { return fd; }\n"
+    "#define TSDE_PW_OP2(name, e) \\\n"
+    "  __device__ __noinline__ float pw_##name(float a, float b) { typedef float T; return e; } \\\n"
+    "  __device__ __noinline__ double pw_##name(double a, double b) { typedef double T; return e; }\n"
+    "TSDE_PW_OP1(exp, expf(a), exp(a))\n"        // exp_kernel_cuda
+    "TSDE_PW_OP1(log, logf(a), log(a))\n"        // log_kernel_cuda
+    "TSDE_PW_OP1(sin, sinf(a), sin(a))\n"        // sin_kernel_cuda
+    "TSDE_PW_OP1(cos, cosf(a), cos(a))\n"        // cos_kernel_cuda
+    "TSDE_PW_OP1(tanh, tanhf(a), tanh(a))\n"     // tanh_kernel_cuda
+    "TSDE_PW_OP1(log1p, log1pf(a), log1p(a))\n"  // log1p_kernel_cuda
+    "TSDE_PW_OP1(expm1, expm1f(a), expm1(a))\n"  // expm1_kernel_cuda
+    "TSDE_PW_OP1(rsqrt, rsqrtf(a), rsqrt(a))\n"  // rsqrt_kernel_cuda
+    "TSDE_PW_OP1(sigmoid, 1.0f / (1.0f + expf(-a)), 1.0 / (1.0 + exp(-a)))\n"  // sigmoid_kernel_cuda
+    "TSDE_PW_OP2(pow, pow(a, b))\n"                          // pow_tensor_scalar_kernel: pow_(base, exp)
+    "TSDE_PW_OP2(tanh_backward, a * (T(1) - b * b))\n"       // tanh_backward_kernel_cuda
+    "TSDE_PW_OP2(sigmoid_backward, a * (T(1) - b) * b)\n"    // sigmoid_backward_kernel_cuda
+    "}  // namespace tsde\n";
+
+static const char* const kPwHelperNames[] = {"exp",   "log",   "sin",     "cos", "tanh",          "log1p",
+                                             "expm1", "rsqrt", "sigmoid", "pow", "tanh_backward", "sigmoid_backward"};
+
+// The call of transcendental instruction op on sources a and b (b for POW and the backward ops only)
+static std::string pw_helper_call(int op, const std::string& a, const std::string& b) {
+  const std::string call = std::string("pw_") + kPwHelperNames[op - TSDE_PW_EXP] + "(" + a;
+  return pw_unary(op) ? call + ")" : call + ", " + b + ")";
+}
+
+// The declarations of kPwHelpers' functions of dtype `T` when the program calls one, or "" when it calls none (its
+// source is then the one it always was)
+static std::string pw_helper_declarations(const tsde_pointwise& in, const char* T) {
+  bool any = false;
+  for (int i = 0; i < in.n_instr; ++i) any = any || pw_transcendental(in.instr[i].op);
+  if (!any) return "";
+  std::string o = "namespace tsde {  // kPwHelpers, linked in\n";
+  for (int op = TSDE_PW_EXP; op <= TSDE_PW_SIGMOID_BACKWARD; ++op)
+    o += std::string("__device__ ") + T + " pw_" + kPwHelperNames[op - TSDE_PW_EXP] + "(" + T +
+         (pw_unary(op) ? "" : std::string(", ") + T) + ");\n";
+  return o + "}  // namespace tsde\n\n";
+}
+
 // The translation unit of a program that passed pw_valid_tables and pw_valid_milstein, for dtype `f64`: the kernels
 // of consecutive steps (single, multi), or with `adaptive` the kernel of an adaptive solve's proposal
 // (tsde_pw_milstein_adaptive, a translation unit of its own).
@@ -444,6 +510,7 @@ static std::string pw_milstein_source(const tsde_pointwise& in, bool f64, bool a
     const std::string a = src(x.a), b = pw_unary(x.op) ? a : src(x.b), d = "r" + num(x.dst) + "[j]";
     const std::string f = f64 ? "" : "f";
     std::string e;
+    if (pw_transcendental(x.op)) return "      " + d + " = " + pw_helper_call(x.op, a, b) + ";\n";
     switch (x.op) {
       case TSDE_PW_MUL: e = a + " * " + b; break;
       case TSDE_PW_ADD: e = a + " + " + b; break;
@@ -498,6 +565,7 @@ static std::string pw_milstein_source(const tsde_pointwise& in, bool f64, bool a
   };
   std::string o = "// A Milstein program of torchsde_b200, generated by pw_milstein_source\n"
                   "#include \"pw_device.cuh\"\n\n";
+  o += pw_helper_declarations(in, T);
   o += "namespace tsde {\nnamespace {\ntypedef " + std::string(T) + " T;\n\nstruct Prog {\n";
   for (int r = 0; r < in.n_regs; ++r) o += "  T r" + num(r) + "[4];\n";
   for (int k = 0; k < in.n_operands; ++k) {
@@ -595,8 +663,9 @@ std::string pw_compile_error() {
   return g_pw_error;
 }
 
-// The sm_90a cubin of `source`, or TSDE_ECOMPILE with the compiler's log
-static int pw_nvrtc(const std::string& source, std::string& cubin) {
+// The sm_90a cubin of `source`, or TSDE_ECOMPILE with the compiler's log.  `rdc`: a relocatable cubin, for nvJitLink;
+// `fmad`: FMA contraction on (kPwHelpers only)
+static int pw_nvrtc(const std::string& source, std::string& cubin, bool rdc = false, bool fmad = false) {
   const Nvrtc* nv = nvrtc();
   if (!nv) return pw_compile_failed("libnvrtc.so.12 (NVRTC) was not found");
   const char* names[kPwHeaderCount + 1];
@@ -612,9 +681,9 @@ static int pw_nvrtc(const std::string& source, std::string& cubin) {
   if (r != NVRTC_SUCCESS) return pw_compile_failed(nv->error(r));
   // straight to SASS (no PTX for the driver to JIT); the public header's declarations are host functions, which NVRTC
   // refuses unless unannotated functions are taken as device ones
-  const char* opts[] = {"-arch=sm_90a", "-std=c++17", "-fmad=false", "-prec-div=true", "-prec-sqrt=true",
-                        "-ftz=false", "-default-device"};
-  r = nv->compile(prog, (int)(sizeof(opts) / sizeof(opts[0])), opts);
+  const char* opts[] = {"-arch=sm_90a", "-std=c++17", fmad ? "-fmad=true" : "-fmad=false", "-prec-div=true",
+                        "-prec-sqrt=true", "-ftz=false", "-default-device", "-rdc=true"};
+  r = nv->compile(prog, (int)(sizeof(opts) / sizeof(opts[0])) - (rdc ? 0 : 1), opts);
   std::string log;
   size_t n = 0;
   if (nv->log_size(prog, &n) == NVRTC_SUCCESS && n > 1) {
@@ -631,6 +700,80 @@ static int pw_nvrtc(const std::string& source, std::string& cubin) {
   return 0;
 }
 
+// nvJitLink, opened like NVRTC when the first program with a transcendental op is linked (torchsde_b200/_cabi.py's
+// nvjitlink() preloads it from the nvidia-nvjitlink package PyTorch installs when such an op is recorded).  Its entry points are versioned; the 12.0 ones are in
+// every CUDA 12 release.
+struct NvJitLink {
+  typedef int (*Create)(void** h, uint32_t n, const char** opts);
+  typedef int (*AddData)(void* h, int kind, const void* data, size_t size, const char* name);
+  typedef int (*Handle)(void* h);
+  typedef int (*Size)(void* h, size_t* n);
+  typedef int (*Get)(void* h, void* out);
+  typedef int (*Destroy)(void** h);
+  Create create;
+  AddData add;
+  Handle complete;
+  Size cubin_size, log_size;
+  Get cubin, log;
+  Destroy destroy;
+};
+
+static const NvJitLink* nvjitlink() {
+  static const NvJitLink* api = []() -> const NvJitLink* {
+    void* h = dlopen("libnvJitLink.so.12", RTLD_NOW | RTLD_GLOBAL);
+    if (!h) return nullptr;
+    static NvJitLink n;
+    bool ok = true;
+    auto sym = [&](auto& fn, const char* name) {
+      fn = reinterpret_cast<std::remove_reference_t<decltype(fn)>>(dlsym(h, name));
+      ok = ok && fn;
+    };
+    sym(n.create, "__nvJitLinkCreate_12_0");
+    sym(n.add, "__nvJitLinkAddData_12_0");
+    sym(n.complete, "__nvJitLinkComplete_12_0");
+    sym(n.cubin_size, "__nvJitLinkGetLinkedCubinSize_12_0");
+    sym(n.cubin, "__nvJitLinkGetLinkedCubin_12_0");
+    sym(n.log_size, "__nvJitLinkGetErrorLogSize_12_0");
+    sym(n.log, "__nvJitLinkGetErrorLog_12_0");
+    sym(n.destroy, "__nvJitLinkDestroy_12_0");
+    return ok ? &n : nullptr;
+  }();
+  return api;
+}
+
+// The sm_90a cubin of program `source`, which calls kPwHelpers: both compiled relocatable and linked without LTO.
+static int pw_nvrtc_linked(const std::string& source, std::string& cubin) {
+  static std::string helpers;  // (compiled once; callers hold pw_loaded's lock)
+  if (helpers.empty())
+    if (int e = pw_nvrtc(kPwHelpers, helpers, true, true)) return e;
+  std::string prog;
+  if (int e = pw_nvrtc(source, prog, true)) return e;
+  const NvJitLink* nj = nvjitlink();
+  if (!nj) return pw_compile_failed("libnvJitLink.so.12 (nvJitLink) was not found");
+  const int kCubin = 1;  // NVJITLINK_INPUT_CUBIN
+  const char* opts[] = {"-arch=sm_90a"};
+  void* h = nullptr;
+  if (nj->create(&h, 1, opts) != 0) return pw_compile_failed("nvJitLinkCreate failed");
+  int r = nj->add(h, kCubin, prog.data(), prog.size(), "program");
+  if (r == 0) r = nj->add(h, kCubin, helpers.data(), helpers.size(), "helpers");
+  if (r == 0) r = nj->complete(h);
+  size_t n = 0;
+  if (r == 0) r = nj->cubin_size(h, &n);
+  if (r == 0) {
+    cubin.resize(n);
+    r = nj->cubin(h, &cubin[0]);
+  }
+  std::string log;
+  if (r != 0 && nj->log_size(h, &n) == 0 && n > 1) {
+    log.resize(n);
+    nj->log(h, &log[0]);
+    log.resize(n - 1);
+  }
+  nj->destroy(&h);
+  if (r != 0) return pw_compile_failed("nvJitLink error " + num(r) + "\n" + log);
+  return 0;
+}
+
 struct PwCompiled {
   // one Brownian cell per step, several cells merged (kSrcCounterMulti); adaptive: kernel[0]; a general-noise program:
   // Euler's two, then midpoint's two
@@ -638,8 +781,10 @@ struct PwCompiled {
 };
 
 // The kernels `names` of `source` (kernel[i] for names[i]; a null name takes the kernel before it), compiled and loaded
-// on first use.  Libraries are context-independent: one entry serves every device.
-static int pw_loaded(std::string source, std::initializer_list<const char*> names, PwCompiled& out) {
+// on first use.  Libraries are context-independent: one entry serves every device.  A program of `prog` with a
+// transcendental op is linked with kPwHelpers.
+static int pw_loaded(const tsde_pointwise& prog, std::string source, std::initializer_list<const char*> names,
+                     PwCompiled& out) {
   static std::mutex mu;
   static std::map<std::string, PwCompiled> cache;
   std::lock_guard<std::mutex> lock(mu);
@@ -648,8 +793,10 @@ static int pw_loaded(std::string source, std::initializer_list<const char*> name
     out = it->second;
     return 0;
   }
+  bool link = false;
+  for (int i = 0; i < prog.n_instr; ++i) link = link || pw_transcendental(prog.instr[i].op);
   std::string cubin;
-  if (int e = pw_nvrtc(source, cubin)) return e;
+  if (int e = link ? pw_nvrtc_linked(source, cubin) : pw_nvrtc(source, cubin)) return e;
   cudaLibrary_t lib;
   cudaError_t e = cudaLibraryLoadData(&lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0);
   int i = 0;
@@ -673,16 +820,17 @@ static int pw_loaded(std::string source, std::initializer_list<const char*> name
 // The loaded kernels of a Milstein program that passed validation, compiled on first use.
 static int pw_compiled(const tsde_pointwise& prog, bool f64, PwCompiled& out, bool adaptive = false) {
   std::string source = pw_milstein_source(prog, f64, adaptive);
-  return adaptive ? pw_loaded(std::move(source), {"tsde_pw_milstein_adaptive", nullptr}, out)
-                  : pw_loaded(std::move(source), {"tsde_pw_milstein_single", "tsde_pw_milstein_multi"}, out);
+  return adaptive ? pw_loaded(prog, std::move(source), {"tsde_pw_milstein_adaptive", nullptr}, out)
+                  : pw_loaded(prog, std::move(source), {"tsde_pw_milstein_single", "tsde_pw_milstein_multi"}, out);
 }
 
 // The Milstein layout, in the order the kernel reads it: go exists from the vjp part on, registers carry over.
 static bool pw_valid_milstein(const tsde_pointwise& pg) {
   uint64_t written = 0;
-  return pw_valid_range(pg, 0, pg.n_fg, false, written) &&
+  return pw_valid_range(pg, 0, pg.n_fg, false, written, true) &&
          pw_valid_source(pg, pg.f_src, false, written) && pw_valid_source(pg, pg.g_src, false, written) &&
-         pw_valid_range(pg, pg.n_fg, pg.n_instr, true, written) && pw_valid_source(pg, pg.gdg_src, true, written);
+         pw_valid_range(pg, pg.n_fg, pg.n_instr, true, written, true) &&
+         pw_valid_source(pg, pg.gdg_src, true, written);
 }
 
 // ---- a whole SRK step (tsde_step_srk_diag_pointwise) ----------------------------------------------------------------
@@ -828,14 +976,16 @@ pw_srk_ext_kernel(const __grid_constant__ PwProg<T> pg, const PwSrkP<T> p, const
 
 // The two-program layout (SRK, predictor-corrector): an f program and a g program that each start with no register
 // defined; go is never a source.  At most MAX_REGS registers: SRK keeps the ones past TSDE_PW_SRK_MAX_REGS for its
-// stash.
-template <int MAX_REGS>
+// stash.  COMPILED: the layout's kernels are compiled (the general layouts), not interpreted.
+template <int MAX_REGS, bool COMPILED = false>
 static bool pw_valid_two(const tsde_pointwise& pg) {
   if (pg.n_regs > MAX_REGS) return false;
   uint64_t written = 0;
-  if (!pw_valid_range(pg, 0, pg.n_fg, false, written) || !pw_valid_source(pg, pg.f_src, false, written)) return false;
+  if (!pw_valid_range(pg, 0, pg.n_fg, false, written, COMPILED) || !pw_valid_source(pg, pg.f_src, false, written))
+    return false;
   written = 0;
-  return pw_valid_range(pg, pg.n_fg, pg.n_instr, false, written) && pw_valid_source(pg, pg.g_src, false, written);
+  return pw_valid_range(pg, pg.n_fg, pg.n_instr, false, written, COMPILED) &&
+         pw_valid_source(pg, pg.g_src, false, written);
 }
 
 // ---- a whole Heun, midpoint or Euler-Heun step (tsde_step_predictor_corrector_pointwise) ----------------------------
@@ -1536,7 +1686,7 @@ static bool pw_per_channel_kind(int kind) { return kind == TSDE_PW_DM || kind ==
 
 // The general layout (tagged TSDE_PW_LAYOUT_GENERAL): the two-program layout with DM / M operands read by g only.
 static bool pw_valid_general(const tsde_pointwise& pg) {
-  if (!pw_valid_two<TSDE_PW_MAX_REGS>(pg)) return false;
+  if (!pw_valid_two<TSDE_PW_MAX_REGS, true>(pg)) return false;
   auto per_channel = [&](uint8_t s) {
     return s >= TSDE_PW_OPERAND(0) && s != TSDE_PW_SRC_Y && s != TSDE_PW_SRC_GO &&
            pw_per_channel_kind(pg.operand[s - TSDE_PW_OPERAND(0)].kind);
@@ -1596,6 +1746,7 @@ static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t
   // the expression of instruction x with sources a, b and destination (SEL's condition) d, as pw_loop's case
   auto expression = [&](const tsde_pw_instr& x, const std::string& a, const std::string& b,
                         const std::string& d) -> const std::string {
+    if (pw_transcendental(x.op)) return pw_helper_call(x.op, a, b);
     switch (x.op) {
       case TSDE_PW_MUL: return a + " * " + b;
       case TSDE_PW_ADD: return a + " + " + b;
@@ -1618,6 +1769,7 @@ static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t
   };
   std::string o = "// An element-wise general-noise program of torchsde_b200, generated by pw_general_source\n"
                   "#include \"pw_device.cuh\"\n\n";
+  o += pw_helper_declarations(in, T);
   o += "namespace tsde {\nnamespace {\ntypedef " + std::string(T) + " T;\n\nstruct Prog {\n";
   o += "  static constexpr int MQ = " + num(mq) + ";\n";
   for (int k = 0; k < in.n_operands; ++k) {
@@ -1754,8 +1906,8 @@ static int pw_general_compiled(const tsde_launch* L, const tsde_pointwise* prog,
   if (!pw_general_program(L, prog, sizeof(T), route, layout)) return TSDE_EINVAL;
   std::string src = pw_general_source(*prog, sizeof(T) == 8, L->m, route, layout);
   if (layout == TSDE_PW_LAYOUT_GENERAL_SRA)
-    return pw_loaded(std::move(src), {"tsde_pw_general_sra1_single", "tsde_pw_general_sra1_multi"}, kc);
-  return pw_loaded(std::move(src),
+    return pw_loaded(*prog, std::move(src), {"tsde_pw_general_sra1_single", "tsde_pw_general_sra1_multi"}, kc);
+  return pw_loaded(*prog, std::move(src),
                    {"tsde_pw_general_euler_single", "tsde_pw_general_euler_multi", "tsde_pw_general_midpoint_single",
                     "tsde_pw_general_midpoint_multi"},
                    kc);
