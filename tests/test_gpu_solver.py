@@ -6,6 +6,8 @@
 * counter path: sdeint with this repo's BrownianInterval (increments regenerated in registers)
   vs the numpy oracle integrating the same Philox-defined path.
 """
+import warnings
+
 import numpy as np
 import pytest
 import torch
@@ -384,6 +386,40 @@ def test_row_split_graph_is_bit_identical():
     for opts in ({}, {'cuda_graph': True, 'row_split': 2}, {'cuda_graph': True, 'row_split': 3}):
         bm = tsde.BrownianInterval(0.0, 0.5, size=(B, d), dtype=torch.float32, device=dev, entropy=21)
         outs.append(tsde.sdeint(sde, y0, ts, bm=bm, method='milstein', dt=2.0 ** -4, options=opts).clone())
+    assert torch.equal(outs[0], outs[1]) and torch.equal(outs[0], outs[2])
+
+
+class _HostConstant(torch.nn.Module):
+    """f copies a CPU tensor to the device at every call: a stream capture cannot record that copy."""
+    noise_type, sde_type = 'diagonal', 'ito'
+
+    def __init__(self, d):
+        super().__init__()
+        self.k = torch.tensor(0.7)
+        self.sigma = torch.nn.Parameter(torch.linspace(0.1, 0.4, d))
+
+    def f(self, t, y):
+        return -y * self.k.to(y.device)
+
+    def g(self, t, y):
+        return self.sigma * y
+
+
+def test_row_split_graph_of_an_uncapturable_sde_falls_back_to_the_eager_loop():
+    """As an unsplit graph solve does: a warning, and the eager solve's bits (a row-split capture used to raise)."""
+    tsde = _tsde()
+    dev = torch.device('cuda')
+    B, d = 99, 8
+    sde = _HostConstant(d).to(dev)
+    ts = torch.tensor([0.0, 0.25, 0.5], device=dev)
+    y0 = torch.rand(B, d, device=dev) + 0.1
+    outs = []
+    for opts in ({}, {'cuda_graph': True}, {'cuda_graph': True, 'row_split': 3}):
+        bm = tsde.BrownianInterval(0.0, 0.5, size=(B, d), dtype=torch.float32, device=dev, entropy=21)
+        with warnings.catch_warnings(record=True) as caught:
+            warnings.simplefilter('always')
+            outs.append(tsde.sdeint(sde, y0, ts, bm=bm, method='euler', dt=2.0 ** -4, options=opts).clone())
+        assert bool(opts) == any('cannot be captured' in str(w.message) for w in caught), opts
     assert torch.equal(outs[0], outs[1]) and torch.equal(outs[0], outs[2])
 
 

@@ -254,9 +254,7 @@ def _capture(solver, sched, binding, y0, ts, extra0):
 # next one ramps up, the other chain's kernel keeps the SMs busy (per-kernel fixed cost ~3 us on 16 MiB tensors).
 # Requires f/g to act row-wise on (t, y) — true for any SDE whose trajectories are independent.
 def _integrate_captured_split(solver, y0, ts, static_ok=False):
-    import copy
     global LAST_PLAN
-    from .. import _cabi
     k = int(solver.options['row_split'])
     sde_obj, _ = cache_owner(solver.sde)
     sched = schedule_lib.get_schedule(ts, solver.dt)
@@ -273,68 +271,88 @@ def _integrate_captured_split(solver, y0, ts, static_ok=False):
     if plans is None:
         return solver.integrate(y0, ts, ())
     plan = plans.get(key)
-    if plan is None:
-        plan = _Plan()
-        dev = y0.device
-        B = y0.shape[0]
-        plan.binding = binding
-        plan.y0 = y0.clone()
-        plan.key = binding.interval.key_tensor().clone()
-        T = ts.numel()
-        # (k, T, rows_i, d) blocks so that every chain writes contiguous rows; returned as one (T, B, d) view
-        plan.ys = torch.empty((T, B, solver.d), dtype=solver.dtype, device=dev)
-        bounds = [(B * i) // k for i in range(k + 1)]
-        subs = []
-        for i in range(k):
-            sub = copy.copy(solver)
-            sub._side_streams = []
-            sub._err_buf = None
-            lo, hi = bounds[i], bounds[i + 1]
-            sub._prepare(plan.y0[lo:hi])
-            feed = base_solver.NoiseFeed(sub, solver.bm, binding)
-            feed._key_ptr = plan.key.data_ptr()
-            feed._row_offset = binding.interval._row_offset + lo
-            sub._feed = feed
-            sub_ctxs = sub._contexts(sched, ts)
-            subs.append((sub, sub_ctxs, lo, hi))
-        plan.time_table = [getattr(sub, '_time_table', None) for sub, _, _, _ in subs]  # (no reference to the sub-solvers / the SDE)
-        streams = [torch.cuda.Stream(device=dev) for _ in range(k - 1)]
-
-        def body(n_steps=None):
-            main = torch.cuda.current_stream(dev)
-            plan.ys[0].copy_(plan.y0)
-            for j, (sub, sub_ctxs, lo, hi) in enumerate(subs):
-                st = main if j == 0 else streams[j - 1]
-                if st is not main:
-                    st.wait_stream(main)
-                with torch.cuda.stream(st):
-                    view = plan.ys[:, lo:hi]
-                    if n_steps is None:
-                        sub._run(sched, sub_ctxs, view, ())
-                    else:
-                        class _Few:
-                            aligned_row = staticmethod(lambda kk: None)
-                            outputs_after = {}
-                        sub._run(_Few, sub_ctxs[:n_steps], view, ())
-            for st in streams:
-                main.wait_stream(st)
-
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side), torch.no_grad(), uncached_autocast():
-            body(min(3, sched.n_steps))
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        graph = torch.cuda.CUDAGraph()
-        launches0 = _cabi.LAUNCHES
-        with no_gc(), torch.no_grad(), torch.cuda.graph(graph), uncached_autocast():
-            body()
-        plan.abi_launches = _cabi.LAUNCHES - launches0
-        plan.graph = graph
-        plan.extra_out = ()
+    if plan is None and key not in plans:
+        plan = _capture_split(solver, sched, binding, y0, ts, k)
         _remember(plans, key, plan)
+    if plan is None:  # (f / g cannot be captured: the ordinary eager loop, as integrate_captured falls back)
+        return solver.integrate(y0, ts, ())
     plan.y0.copy_(y0)
     plan.key.copy_(binding.interval.key_tensor())
     plan.graph.replay()
     LAST_PLAN = plan
     return _hand_out(plan, solver, static_ok)
+
+
+def _capture_split(solver, sched, binding, y0, ts, k):
+    """The plan of a row-split solve: k row blocks captured as k chains of one graph; None (with a warning) when f / g
+    do something a stream capture cannot record, as `integrate_captured` does for an unsplit solve."""
+    import copy
+    from .. import _cabi
+    plan = _Plan()
+    dev = y0.device
+    B = y0.shape[0]
+    plan.binding = binding
+    plan.y0 = y0.clone()
+    plan.key = binding.interval.key_tensor().clone()
+    T = ts.numel()
+    # (k, T, rows_i, d) blocks so that every chain writes contiguous rows; returned as one (T, B, d) view
+    plan.ys = torch.empty((T, B, solver.d), dtype=solver.dtype, device=dev)
+    bounds = [(B * i) // k for i in range(k + 1)]
+    subs = []
+    for i in range(k):
+        sub = copy.copy(solver)
+        sub._side_streams = []
+        sub._err_buf = None
+        lo, hi = bounds[i], bounds[i + 1]
+        sub._prepare(plan.y0[lo:hi])
+        feed = base_solver.NoiseFeed(sub, solver.bm, binding)
+        feed._key_ptr = plan.key.data_ptr()
+        feed._row_offset = binding.interval._row_offset + lo
+        sub._feed = feed
+        sub_ctxs = sub._contexts(sched, ts)
+        subs.append((sub, sub_ctxs, lo, hi))
+    plan.time_table = [getattr(sub, '_time_table', None) for sub, _, _, _ in subs]  # (no reference to the sub-solvers / the SDE)
+    streams = [torch.cuda.Stream(device=dev) for _ in range(k - 1)]
+
+    def body(n_steps=None):
+        main = torch.cuda.current_stream(dev)
+        plan.ys[0].copy_(plan.y0)
+        for j, (sub, sub_ctxs, lo, hi) in enumerate(subs):
+            st = main if j == 0 else streams[j - 1]
+            if st is not main:
+                st.wait_stream(main)
+            with torch.cuda.stream(st):
+                view = plan.ys[:, lo:hi]
+                if n_steps is None:
+                    sub._run(sched, sub_ctxs, view, ())
+                else:
+                    class _Few:
+                        aligned_row = staticmethod(lambda kk: None)
+                        outputs_after = {}
+                    sub._run(_Few, sub_ctxs[:n_steps], view, ())
+        for st in streams:
+            main.wait_stream(st)
+
+    side = torch.cuda.Stream(device=dev)
+    side.wait_stream(torch.cuda.current_stream(dev))
+    with torch.cuda.stream(side), torch.no_grad(), uncached_autocast():
+        body(min(3, sched.n_steps))
+    torch.cuda.current_stream(dev).wait_stream(side)
+    torch.cuda.synchronize(dev)
+    graph = torch.cuda.CUDAGraph()
+    launches0 = _cabi.LAUNCHES
+    try:
+        with no_gc(), torch.no_grad(), torch.cuda.graph(graph), uncached_autocast():
+            body()
+    except RuntimeError as e:
+        if 'captur' not in str(e).lower():
+            raise
+        import warnings
+        warnings.warn("torchsde_b200: this SDE's f/g cannot be captured into a CUDA graph "
+                      f"({str(e).splitlines()[0][:160]}); falling back to the eager time loop.")
+        torch.cuda.synchronize(dev)
+        return None
+    plan.abi_launches = _cabi.LAUNCHES - launches0
+    plan.graph = graph
+    plan.extra_out = ()
+    return plan
