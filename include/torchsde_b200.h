@@ -138,10 +138,11 @@ const char* tsde_error_string(int code);
                                      tsde_solve_reversible_heun_pointwise)                                      */
 #define TSDE_KERNEL_PW_ADAPTIVE 7 /* an adaptive solve's proposal with an element-wise SDE, the full step and both
                                      half steps in one launch (tsde_adaptive_proposal_pointwise)                */
-#define TSDE_KERNEL_PW_GENERAL 8  /* general / additive-noise Euler steps, a midpoint step or an additive-noise
-                                     SRK step with an element-wise SDE (GENERAL launches of
-                                     tsde_solve_euler_pointwise, tsde_step_predictor_corrector_pointwise and
-                                     tsde_step_srk_diag_pointwise)                                               */
+#define TSDE_KERNEL_PW_GENERAL 8  /* general / additive-noise Euler or reversible-Heun steps, a midpoint or
+                                     Euler-Heun step or an additive-noise SRK step with an element-wise SDE
+                                     (GENERAL launches of tsde_solve_euler_pointwise,
+                                     tsde_solve_reversible_heun_pointwise, tsde_step_predictor_corrector_pointwise
+                                     and tsde_step_srk_diag_pointwise)                                           */
 int64_t tsde_kernel_launches(int32_t family);
 
 
@@ -278,8 +279,8 @@ int tsde_step_milstein(const tsde_launch* L, const tsde_noise* nz, const void* y
  *   SEL  dst = dst != 0 ? a : b: the condition is the destination register itself, which must have been written
  *        (torch.where, masked_fill).
  * Transcendental opcodes (16 and up), valid only in the programs the library compiles (this Milstein layout, its
- * adaptive proposal, and the general layouts TSDE_PW_LAYOUT_GENERAL and TSDE_PW_LAYOUT_GENERAL_SRA); the interpreted
- * entry points refuse them.  Each is the lambda of the ATen CUDA kernel it restates, in T, compiled apart from the
+ * adaptive proposal, and the general layouts TSDE_PW_LAYOUT_GENERAL, _SRA, _EULER_HEUN and _REVERSIBLE_HEUN); the
+ * interpreted entry points refuse them.  Each is the lambda of the ATen CUDA kernel it restates, in T, compiled apart from the
  * program with FMA contraction on, as ATen's kernels are (libdevice's exp, log, ... of T):
  *   EXP exp(a)   LOG log(a)   SIN sin(a)   COS cos(a)   TANH tanh(a)   LOG1P log1p(a)   EXPM1 expm1(a)
  *   RSQRT rsqrt(a)   SIGMOID 1 / (1 + exp(-a))   (unary: b unused)
@@ -536,6 +537,27 @@ enum { TSDE_PW_DM = 5, TSDE_PW_M = 6 };
  * the SRA tag and null times.  The Euler and midpoint GENERAL launches refuse an SRA-tagged program.
  */
 #define TSDE_PW_LAYOUT_GENERAL_SRA 2 /* tsde_pointwise.reserved of a general-layout program for the sra1 step */
+
+/*
+ * General and additive noise, Stratonovich Euler-Heun and reversible Heun.  Two more tags of the general layout, each
+ * compiled into a translation unit of its own by tsde_pointwise_compile and written out by tsde_pointwise_source:
+ *   tsde_step_predictor_corrector_pointwise with TSDE_PC_EULER_HEUN on a GENERAL launch, for a program tagged
+ *     TSDE_PW_LAYOUT_GENERAL_EULER_HEUN: one Euler-Heun step, f and g.dW at (t0, y0), y' as tsde_euler_heun_predict,
+ *     g'.dW at (t_p, y') and y1 as tsde_step_euler_heun (dt);
+ *   tsde_solve_reversible_heun_pointwise on a GENERAL launch, for a program tagged
+ *     TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN: consecutive reversible-Heun steps as for diagonal noise, with g0 and g1
+ *     the (rows, d, m) state (contiguous, not overlapping); each thread keeps its lanes' m values of g in registers.
+ * Each contraction sums in the order the unfused launch takes, as above.  Euler-Heun's two launches see the same g
+ * operand, so they take one order.  The reversible-Heun pair always reads a dense g (it refuses launch flags), so its
+ * order is that of a contiguous aligned g, whatever the program's g source.  Every stored value equals the unfused
+ * steps' bit for bit (reversible Heun: under the half-step condition of the diagonal chunk).  The launches count under
+ * TSDE_KERNEL_PW_GENERAL.  TSDE_EINVAL, before anything is compiled or launched: a program with another tag (the
+ * Euler / midpoint and sra1 programs among them), other predictor-corrector methods, m outside
+ * [1, TSDE_PW_GENERAL_MAX_M], noise other than counter noise, launch flags, null times or state pointers, and what
+ * the diagonal entry points refuse.
+ */
+#define TSDE_PW_LAYOUT_GENERAL_EULER_HEUN 3      /* tsde_pointwise.reserved for the general Euler-Heun step     */
+#define TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN 4 /* tsde_pointwise.reserved for general reversible-Heun chunks */
 
 /* derivative-free Milstein, predictor: y' = y0 + (Ito ? dt*f : 0) + g*sqrt_dt
  * methods/milstein.py:58-63,83-84,93-94.  g is (rows,d) also for scalar noise (squeezed). */

@@ -74,7 +74,8 @@ def general_pointwise_source(prog, dtype, d, m):
 
 def compile_general_pointwise(prog, dtype, d, m):
     """tsde_pointwise_compile on a GENERAL launch: compile and load the Euler and midpoint kernels of general-noise
-    program `prog` (the sra1 kernels if it is tagged PW_LAYOUT_GENERAL_SRA); 0 or an error code."""
+    program `prog` (the sra1, Euler-Heun or reversible-Heun kernels if it is tagged PW_LAYOUT_GENERAL_SRA, _EULER_HEUN
+    or _REVERSIBLE_HEUN); 0 or an error code."""
     return lib().tsde_pointwise_compile(ctypes.byref(_general_launch(dtype, d, m)), ctypes.byref(prog))
 
 
@@ -118,6 +119,8 @@ KERNEL_PW_GENERAL = 8  # TSDE_KERNEL_PW_GENERAL
 PW_GENERAL_MAX_M = 32  # TSDE_PW_GENERAL_MAX_M
 PW_LAYOUT_GENERAL = 1  # TSDE_PW_LAYOUT_GENERAL: Pointwise.reserved of a general-noise program
 PW_LAYOUT_GENERAL_SRA = 2  # TSDE_PW_LAYOUT_GENERAL_SRA: Pointwise.reserved of a general-noise program of an sra1 step
+PW_LAYOUT_GENERAL_EULER_HEUN = 3  # TSDE_PW_LAYOUT_GENERAL_EULER_HEUN: ... of a general-noise Euler-Heun step
+PW_LAYOUT_GENERAL_REVERSIBLE_HEUN = 4  # TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN: ... of general reversible-Heun chunks
 # TSDE_PROPOSAL_*: the method of tsde_adaptive_proposal_pointwise
 (PROPOSAL_EULER, PROPOSAL_MILSTEIN_ITO, PROPOSAL_MILSTEIN_STRATONOVICH, PROPOSAL_SRK, PROPOSAL_HEUN, PROPOSAL_MIDPOINT,
  PROPOSAL_EULER_HEUN) = range(7)

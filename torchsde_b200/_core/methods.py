@@ -99,6 +99,7 @@ class Euler(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
 
     _pw_method = 'euler'
     _pw_general = True  # general / additive noise fuses too (pointwise.general)
+    _pw_layout = _cabi.PW_LAYOUT_GENERAL
 
     def __init__(self, sde, **kwargs):
         self.strong_order = 1.0 if sde.noise_type == NOISE_TYPES.additive else 0.5
@@ -277,6 +278,7 @@ class Midpoint(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
     levy_area_approximations = LEVY_AREA_APPROXIMATIONS.all()
 
     _pw_general = True  # general / additive noise fuses too (pointwise.general)
+    _pw_layout = _cabi.PW_LAYOUT_GENERAL
 
     def __init__(self, sde, **kwargs):
         self.strong_order = 0.5 if sde.noise_type == NOISE_TYPES.general else 1.0
@@ -316,6 +318,9 @@ class EulerHeun(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
     noise_types = NOISE_TYPES.all()
     levy_area_approximations = LEVY_AREA_APPROXIMATIONS.all()
 
+    _pw_general = True  # general / additive noise fuses too (pointwise.general)
+    _pw_layout = _cabi.PW_LAYOUT_GENERAL_EULER_HEUN
+
     def __init__(self, sde, **kwargs):
         self.strong_order = 0.5 if sde.noise_type == NOISE_TYPES.general else 1.0
         super(EulerHeun, self).__init__(sde=sde, **kwargs)
@@ -324,7 +329,8 @@ class EulerHeun(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
     def _step(self, c, y0, extra0, out):
         sde = self.sde
         if pointwise.ready(self):
-            # f and g were recorded as element-wise programs (pointwise.py): the whole step is one kernel
+            # f and g were recorded as element-wise programs (pointwise.py): the whole step is one kernel (for
+            # general / additive noise, on the solver's GENERAL launch)
             return pointwise.launch(self, 'tsde_step_predictor_corrector_pointwise', self._feed.get(c), y0,
                                     (c.t0.data_ptr(), c.t1.data_ptr(), _cabi.PC_EULER_HEUN, c.dt, 0.0), out), ()
         # the first step of an eligible solve runs as always, with the user's three evaluations recorded
@@ -353,7 +359,9 @@ class EulerHeun(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
             L2, nz2, gp = self._LU, self._feed.unit(), _contig(gp)
         else:
             L2, nz2, gp = self._g_prod(c, c.t1, yp, rec)
-        if rec is not None:
+        if isinstance(rec, pointwise.GeneralRecorder):
+            self._pw = pointwise.compile_general(self, rec, rec.finish()) or False
+        elif rec is not None:
             self._pw = rec.finish() or False
         return self._k('tsde_step_euler_heun', L2, nz2, (y0, f, g, gp), (c.dt,), out), ()
 
@@ -366,6 +374,8 @@ class ReversibleHeun(base_solver.BaseSDESolver):
     levy_area_approximations = LEVY_AREA_APPROXIMATIONS.all()
 
     _pw_method = 'reversible_heun'
+    _pw_general = True  # general / additive noise fuses too (pointwise.general)
+    _pw_layout = _cabi.PW_LAYOUT_GENERAL_REVERSIBLE_HEUN
 
     def __init__(self, sde, **kwargs):
         self.strong_order = 1.0 if sde.noise_type == NOISE_TYPES.additive else 0.5
@@ -397,7 +407,9 @@ class ReversibleHeun(base_solver.BaseSDESolver):
                 y1, extra0 = self._unfused_step(c, y1, extra0, out)
             return y1, extra0
         if self._pw_state is None:
-            self._pw_state = [tuple(torch.empty_like(y0) for _ in range(3)) for _ in range(2)]
+            # (f, g, z); a general- or additive-noise g is (rows, d, m)
+            g_shape = tuple(state[1].shape)
+            self._pw_state = [(torch.empty_like(y0), y0.new_empty(g_shape), torch.empty_like(y0)) for _ in range(2)]
         # the recorded element-wise programs (pointwise.py), several steps per kernel with y, z, f and g in registers;
         # the chunk stores its state to the set it does not read
         a, b = self._pw_state
@@ -423,7 +435,10 @@ class ReversibleHeun(base_solver.BaseSDESolver):
         if rec is not None:
             f1, g1 = self._fork(lambda: rec.evaluation('f', lambda: sde.f(c.t1, z1), c.t1, z1),
                                 lambda: rec.evaluation('g', lambda: sde.g(c.t1, z1), c.t1, z1))
-            self._pw = rec.finish() or False
+            if isinstance(rec, pointwise.GeneralRecorder):
+                self._pw = pointwise.compile_general(self, rec, rec.finish()) or False
+            else:
+                self._pw = rec.finish() or False
         else:
             f1, g1 = self._f_and_g(c.t1, z1)
         f1, g1 = _contig(f1), _contig(g1)
@@ -444,6 +459,7 @@ class SRK(_ProposalMixin, base_solver.BaseSDESolver):
                                 LEVY_AREA_APPROXIMATIONS.foster)
     want_u = True
     _pw_general = True  # additive noise fuses too (pointwise.general)
+    _pw_layout = _cabi.PW_LAYOUT_GENERAL_SRA
 
     def __init__(self, sde, **kwargs):
         if getattr(sde, 'is_adjoint_sde', False):

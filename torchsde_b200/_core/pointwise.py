@@ -41,7 +41,7 @@ Transcendental ops, with options={'transcendental': True} only (`Recorder.transc
 They are libdevice code, not correctly rounded, and ATen's kernels contract their arithmetic into FMAs: the library
 compiles each as a function of its own with ATen's lambda as its body and FMA contraction on, and links it to the
 program (csrc/pointwise.cu, kPwHelpers), so only the compiled layouts take them: Milstein (fixed-step and adaptive)
-and the general / additive-noise Euler, midpoint and sra1 kernels.  The interpreted ones (`SrkRecorder` on diagonal
+and the general / additive-noise Euler, midpoint, sra1, Euler-Heun and reversible-Heun kernels.  The interpreted ones (`SrkRecorder` on diagonal
 noise: SRK, Heun, midpoint, Euler-Heun, Euler, reversible Heun) reject such a tape with the reason.  So does every
 recorder when the NVRTC the library compiles with is not the CUDA release PyTorch was built with (`nvrtc_mismatch`),
 or when there is no nvJitLink to link with (loaded only then, `_cabi.nvjitlink`).
@@ -90,7 +90,8 @@ tsde_solve_reversible_heun_pointwise).  Both evaluate f and g once per step: Eul
 up to TSDE_PW_MAX_STEPS steps per launch once the batch fills the GPU, a single step being a chunk of one.
 Reversible Heun's solver state (f, g, z) stays in registers inside a chunk and is stored at its end, alternately to
 two sets of solver-owned buffers; its half step T(0.5) * T(dt) must equal the unfused step's half_dt at every step
-(`halves_exactly`), and the state it starts from must be (rows, d) tensors of the state dtype (`state_fits`), else
+(`halves_exactly`), and the state it starts from must be tensors of the state dtype of the shapes the kernel reads
+(`state_fits`), else
 the solve keeps the ordinary step.  `sdeint_adjoint`'s forward solve is a no-grad solve, so the reversible pair's
 forward steps fuse too.
 
@@ -116,7 +117,12 @@ they run on the solver's GENERAL launch of tsde_solve_euler_pointwise (chunks, a
 tsde_step_predictor_corrector_pointwise (midpoint).  A fixed-step additive-noise SRK solve (sra1) records its step's
 four evaluations f0, gA, gB, f1 the same way (pattern 'fggf'); its program is tagged PW_LAYOUT_GENERAL_SRA and every
 later step is one launch of tsde_step_srk_diag_pointwise on the solver's GENERAL launch, which draws W and U and
-contracts g three times, with the weights of the unfused stage and final launches.  Every other method keeps diagonal-only tapes.
+contracts g three times, with the weights of the unfused stage and final launches.  Fixed-step Euler-Heun ('fgg') and
+reversible Heun ('fg' at (t1, z1)) record the same way; their programs are tagged PW_LAYOUT_GENERAL_EULER_HEUN and
+_REVERSIBLE_HEUN (the solver's `_pw_layout`: reversible Heun's pattern is Euler's) and run as one launch of
+tsde_step_predictor_corrector_pointwise per Euler-Heun step, and as chunks of tsde_solve_reversible_heun_pointwise whose
+solver state holds g as (rows, d, m), kept in registers within a chunk; `sdeint_adjoint`'s forward solve fuses too.
+Heun and every other method keep diagonal-only tapes.
 """
 import ctypes
 import numbers
@@ -761,13 +767,17 @@ class GeneralRecorder(SrkRecorder):
         an (m,) row (M), a dense (d, m) block (DM); a (rows, d, m) tensor from outside the tape rejects it.
     f must be of the (rows, d) class; g must have the shape (rows, d, m) and may be any of those (an operand's
     `expand` is additive noise).  The kernel derives which instructions are per channel from their sources alone.  The
-    program is tagged with its step's layout: PW_LAYOUT_GENERAL_SRA for SRK's pattern, else PW_LAYOUT_GENERAL.  Its
+    program is tagged with its step's layout `layout`, the solver's `_pw_layout` (Euler's and reversible Heun's
+    pattern 'fg' is the same); without one, PW_LAYOUT_GENERAL_SRA for SRK's pattern, else PW_LAYOUT_GENERAL.  Its
     kernels are compiled, so with `transcendental` it takes the transcendental ops."""
 
     compiled = True
 
-    def __init__(self, y, t, pattern, m, transcendental=False):
+    def __init__(self, y, t, pattern, m, transcendental=False, layout=None):
         self.m = m
+        if layout is None:
+            layout = _cabi.PW_LAYOUT_GENERAL_SRA if pattern == SRA_PATTERN else _cabi.PW_LAYOUT_GENERAL
+        self.layout = layout
         self._wide = set()     # the per-channel values
         self._lifted = set()   # id() of (rows, d)-class tensors viewed as (..., 1)
         self._w3 = False       # the op being recorded is per channel
@@ -878,7 +888,7 @@ class GeneralRecorder(SrkRecorder):
 
     def _program(self, code, n_fg, results, n_regs, max_regs):
         prog, keep = super()._program(code, n_fg, results, n_regs, max_regs)
-        prog.reserved = _cabi.PW_LAYOUT_GENERAL_SRA if self.pattern == SRA_PATTERN else _cabi.PW_LAYOUT_GENERAL
+        prog.reserved = self.layout
         return prog, keep
 
     def _step_result(self, t, allow_go=False):
@@ -905,8 +915,8 @@ def recording(solver):
 
 def general(solver):
     """Whether `solver` runs general- or additive-noise steps that the element-wise general kernels serve: a fixed-step
-    Euler, midpoint or (additive-noise) SRK solve (`_pw_general`) with 1 <= m <= TSDE_PW_GENERAL_MAX_M Brownian
-    channels."""
+    Euler, midpoint, Euler-Heun, reversible-Heun or (additive-noise) SRK solve (`_pw_general`, whose kernels are those
+    of its `_pw_layout`) with 1 <= m <= TSDE_PW_GENERAL_MAX_M Brownian channels."""
     return (getattr(solver, '_pw_general', False) and not solver.adaptive
             and solver.sde.noise_type in (NOISE_TYPES.general, NOISE_TYPES.additive)
             and 1 <= solver.m <= _cabi.PW_GENERAL_MAX_M)
@@ -922,13 +932,13 @@ def pc_recorder(solver, y, t, pattern):
             or getattr(sde, 'user_f_and_g', True) or getattr(sde, 'is_adjoint_sde', False)):
         return None
     if sde.noise_type != NOISE_TYPES.diagonal:
-        return GeneralRecorder(y, t, pattern, solver.m, transcendental(solver))
+        return GeneralRecorder(y, t, pattern, solver.m, transcendental(solver), solver._pw_layout)
     return SrkRecorder(y, t, pattern, _cabi.PW_MAX_REGS, transcendental(solver))
 
 
 def compile_general(solver, rec, res):
-    """`res`, what a GeneralRecorder's `finish` returned, once the Euler and midpoint kernels of its program (the sra1
-    kernels of an SRK program) are compiled and loaded (tsde_pointwise_compile on the solver's GENERAL launch), on the
+    """`res`, what a GeneralRecorder's `finish` returned, once the Euler and midpoint kernels of its program (the sra1,
+    Euler-Heun or reversible-Heun kernels of a program with that tag) are compiled and loaded (tsde_pointwise_compile on the solver's GENERAL launch), on the
     recording step as for
     `compile_milstein`; None if `res` is, or if the library refuses or cannot compile the program (the tape is then
     rejected with the reason)."""
@@ -978,8 +988,10 @@ def plan_chunks(first, n_steps, interpolated=(), multi_cell=(), max_steps=_cabi.
 # Resident CTAs (256 threads) per SM of each chunked kernel, (float32, float64), from its registers (-Xptxas -v,
 # sm_90a: 64 K registers per SM): Milstein's compiled kernels are pinned there by their launch bounds (256, 4) and
 # (256, 2) (cfg2's program: 41 registers in fp32); Euler at 54 and 88-96; reversible Heun at 72 and 110-120.
-# The compiled general-noise Euler kernels are bounded at (256, 1): at least one resident CTA, whatever m.
-_RESIDENT_CTAS = {'milstein': (4, 2), 'euler': (4, 2), 'reversible_heun': (3, 2), 'euler_general': (1, 1)}
+# The compiled general-noise Euler and reversible-Heun kernels are bounded at (256, 1): at least one resident CTA,
+# whatever m.
+_RESIDENT_CTAS = {'milstein': (4, 2), 'euler': (4, 2), 'reversible_heun': (3, 2), 'euler_general': (1, 1),
+                  'reversible_heun_general': (1, 1)}
 
 
 def chunk_length(solver):
@@ -1036,10 +1048,15 @@ def halves_exactly(dtype, ctxs):
 
 
 def state_fits(solver, tensors):
-    """Whether solver-state tensors (reversible Heun's f, g, z) are what a chunk kernel reads: contiguous (rows, d)
-    tensors of the state dtype on the state's device."""
-    return all(torch.is_tensor(x) and tuple(x.shape) == (solver.rows, solver.d) and x.dtype == solver.dtype
-               and x.device == solver.device and x.is_contiguous() for x in tensors)
+    """Whether reversible Heun's solver state (f, g, z) is what a chunk kernel reads: contiguous tensors of the state
+    dtype on the state's device, of shape (rows, d), except a general- or additive-noise g, of shape (rows, d, m) and
+    16-byte aligned (the unfused pair reads such a g as quads: the summation order the kernel was compiled for)."""
+    rows_d = (solver.rows, solver.d)
+    general = solver.sde.noise_type != NOISE_TYPES.diagonal
+    shapes = (rows_d, rows_d + (solver.m,) if general else rows_d, rows_d)
+    return len(tensors) == 3 and all(
+        torch.is_tensor(x) and tuple(x.shape) == shape and x.dtype == solver.dtype and x.device == solver.device
+        and x.is_contiguous() for x, shape in zip(tensors, shapes)) and (not general or tensors[1].data_ptr() % 16 == 0)
 
 
 def eligible(solver):

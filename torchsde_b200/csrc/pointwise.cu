@@ -1368,14 +1368,18 @@ static int pw_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_point
                       p, np, p.base.nquads, slots, TSDE_KERNEL_PW_CHUNK, st);
 }
 
-// GENERAL launches of tsde_solve_euler_pointwise, tsde_step_predictor_corrector_pointwise,
-// tsde_step_srk_diag_pointwise, tsde_pointwise_compile and tsde_pointwise_source (general / additive noise; defined
-// with the general-noise code generator below)
+// GENERAL launches of tsde_solve_euler_pointwise, tsde_solve_reversible_heun_pointwise,
+// tsde_step_predictor_corrector_pointwise, tsde_step_srk_diag_pointwise, tsde_pointwise_compile and
+// tsde_pointwise_source (general / additive noise; defined with the general-noise code generator below)
 template <typename T>
 static int pw_general_euler(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
                             const tsde_pw_step* steps, int32_t n_steps);
 template <typename T>
-static int pw_general_midpoint_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+static int pw_general_reversible_heun(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                      const void* y0, const void* const (&in)[3], const tsde_pw_step* steps,
+                                      int32_t n_steps, void* const (&out)[3]);
+template <typename T>
+static int pw_general_pc_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
                                     const void* y0, const void* t0, const void* t_p, int32_t method, double dt,
                                     double half_dt, void* y1);
 template <typename T>
@@ -1403,9 +1407,13 @@ TSDE_EXPORT int tsde_solve_reversible_heun_pointwise(const tsde_launch* L, const
                                                      const tsde_pointwise* prog, const void* y0, const void* z0,
                                                      const void* f0, const void* g0, const tsde_pw_step* steps,
                                                      int32_t n_steps, void* z1, void* f1, void* g1) {
-  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
   const void* const in[3] = {z0, f0, g0};
   void* const out[3] = {z1, f1, g1};
+  if (valid_launch(L) && L->noise_type == TSDE_NOISE_GENERAL)
+    return dispatch(L, [&](auto t) -> int {
+      return pw_general_reversible_heun<decltype(t)>(L, nz, prog, y0, in, steps, n_steps, out);
+    });
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
   return dispatch(L, [&](auto t) -> int {
     return pw_chunk<decltype(t), kPwReversibleHeun>(L, nz, prog, y0, steps, n_steps, in, out);
   });
@@ -1469,7 +1477,7 @@ TSDE_EXPORT int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, co
                                                         void* y1) {
   if (valid_launch(L) && L->noise_type == TSDE_NOISE_GENERAL)
     return dispatch(L, [&](auto t) -> int {
-      return pw_general_midpoint_step<decltype(t)>(L, nz, prog, y0, t0, t_p, method, dt, half_dt, y1);
+      return pw_general_pc_step<decltype(t)>(L, nz, prog, y0, t0, t_p, method, dt, half_dt, y1);
     });
   if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
   return dispatch(L, [&](auto t) -> int {
@@ -1659,8 +1667,9 @@ TSDE_EXPORT int tsde_adaptive_pointwise_compile(const tsde_launch* L, const tsde
 // ---- general / additive noise (GENERAL launches) -------------------------------------------------------------------
 // The two-program layout with per-channel values.  A g program runs m times per output, so it is compiled, never
 // interpreted (an interpreted instruction costs about 30 SASS instructions, DESIGN §4): pw_general_source writes it
-// out as a `Prog` for pw_general_euler_steps / pw_general_midpoint, or for pw_general_sra1 when the program is tagged
-// TSDE_PW_LAYOUT_GENERAL_SRA (pw_device.cuh), with the IEEE options and the cache of the Milstein kernels.  A g
+// out as a `Prog` for pw_general_euler_steps / pw_general_midpoint, or, by the program's tag, for pw_general_sra1
+// (TSDE_PW_LAYOUT_GENERAL_SRA), pw_general_euler_heun (_EULER_HEUN) or pw_general_reversible_heun_steps
+// (_REVERSIBLE_HEUN) (pw_device.cuh), with the IEEE options and the cache of the Milstein kernels.  A g
 // instruction is per channel when one of its sources is (a DM or M operand, or a per-channel value); the others are
 // per (row, d) element, evaluated once per lane before the channel loop.  The contraction of each lane's m values with
 // the increments is written out for the route the unfused step takes (gen_route), as that kernel sums:
@@ -1681,6 +1690,10 @@ static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralMidP<double>) + sizeo
               "the compiled general midpoint kernel's parameters fit the 4 KiB parameter space");
 static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralSraP<double>) + sizeof(NoiseP<double>) <= 4096,
               "the compiled sra1 kernel's parameters fit the 4 KiB parameter space");
+static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralRevHeunP<double>) + sizeof(NoiseP<double>) +
+                      sizeof(PwSteps<double>) <=
+                  4096,
+              "the compiled general reversible-Heun kernel's parameters fit the 4 KiB parameter space");
 
 static bool pw_per_channel_kind(int kind) { return kind == TSDE_PW_DM || kind == TSDE_PW_M; }
 
@@ -1705,11 +1718,12 @@ static bool pw_general_program(const tsde_launch* L, const tsde_pointwise* prog,
     return false;
   bool vec = true;
   if (!pw_valid_tables(*prog, &vec, TSDE_PW_M) || !pw_valid_general(*prog)) return false;
-  // the unfused step's g is a new contiguous tensor (aligned), or the user's (d, m) block itself when g is a DM operand
+  // the unfused step's g is a new contiguous tensor (aligned), or the user's (d, m) block itself when g is a DM operand;
+  // the reversible-Heun pair densifies every g it reads (its solver state)
   bool quads = true;
   const uint8_t g = prog->g_src;
-  if (g >= TSDE_PW_OPERAND(0) && g != TSDE_PW_SRC_Y && g != TSDE_PW_SRC_GO &&
-      prog->operand[g - TSDE_PW_OPERAND(0)].kind == TSDE_PW_DM)
+  if (layout != TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN && g >= TSDE_PW_OPERAND(0) && g != TSDE_PW_SRC_Y &&
+      g != TSDE_PW_SRC_GO && prog->operand[g - TSDE_PW_OPERAND(0)].kind == TSDE_PW_DM)
     quads = aligned16(prog->operand[g - TSDE_PW_OPERAND(0)].ptr);
   if (layout == TSDE_PW_LAYOUT_GENERAL_SRA) {
     // the sra1 launches call launch_gen directly, which stages U too, and take gen_kernel where cabi.cu would take the
@@ -1772,6 +1786,7 @@ static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t
   o += pw_helper_declarations(in, T);
   o += "namespace tsde {\nnamespace {\ntypedef " + std::string(T) + " T;\n\nstruct Prog {\n";
   o += "  static constexpr int MQ = " + num(mq) + ";\n";
+  if (layout == TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN) o += "  static constexpr int M = " + M + ";\n";
   for (int k = 0; k < in.n_operands; ++k) {
     const std::string n = num(k);
     if (in.operand[k].kind == TSDE_PW_SCALAR) o += "  T u" + n + ";\n";
@@ -1829,41 +1844,81 @@ static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t
       narrow += "      n" + num(i) + "[j] = " + expression(x, a, b, d) + ";\n";
     def[x.dst] = i;
   }
-  o += "  __device__ __forceinline__ void gp(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
-       "                                     const T (&w)[4 * MQ], T (&out)[4]) {\n    const T t0 = *tp;\n"
-       "    (void)t0;\n";
+  // the g program at (*tp, y), up to lane j's channel values G(k)
+  std::string g_head = "    const T t0 = *tp;\n    (void)t0;\n";
   for (int i = in.n_fg; i < in.n_instr; ++i)
-    if (!wide[i]) o += "    T n" + num(i) + "[4];\n";
-  o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n" + narrow + "    }\n";
-  o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n"
-       "      const int64_t i = c.chan + (j < c.nvalid ? j : 0);  // (the d index of the lane; padding lanes read lane 0's)\n"
-       "      (void)i;\n      auto G = [&](int k) -> T {\n        (void)k;\n" +
-       per_channel + "        return " + gsrc(in.g_src) + ";\n      };\n";
+    if (!wide[i]) g_head += "    T n" + num(i) + "[4];\n";
+  g_head += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
+  g_head += narrow;
+  g_head += "    }\n#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n"
+            "      const int64_t i = c.chan + (j < c.nvalid ? j : 0);  // (the d index of the lane; padding lanes read lane 0's)\n"
+            "      (void)i;\n      auto G = [&](int k) -> T {\n        (void)k;\n";
+  g_head += per_channel;
+  g_head += "        return ";
+  g_head += gsrc(in.g_src);
+  g_head += ";\n      };\n";
+  // lane j's acc: the values val(k) contracted with the weights w[k] in the route's order; pre(k) / post(k) are the
+  // statements before / after channel k's term.  (Built by appending: a sum of two temporaries would instantiate a
+  // std::operator+ that the library might export.)
+  auto cat = [](std::initializer_list<std::string> parts) {
+    std::string s;
+    for (const std::string& x : parts) s += x;
+    return s;
+  };
   const std::string fma = "fma" + fs;
-  if (route == TSDE_GEN_ROWWISE) {
-    o += "      const T acc = G(0) * w[0];\n";
-  } else if (route == TSDE_GEN_GENERIC) {
-    o += "      T acc = T(0);\n";
-    for (int k = 0; k < m; ++k) o += "      acc = acc + G(" + num(k) + ") * w[" + num(k) + "];\n";
-  } else {
-    std::string level[TSDE_PW_GENERAL_MAX_M / 4];  // the partial sums of the tree's current level
-    for (int q = 0; q < mq; ++q) {
-      const std::string s = "s" + num(q);
-      o += "      T " + s + " = " + fma + "(G(" + num(4 * q) + "), w[" + num(4 * q) + "], T(0));\n";
-      for (int j = 1; j < 4; ++j)
-        o += "      " + s + " = " + fma + "(G(" + num(4 * q + j) + "), w[" + num(4 * q + j) + "], " + s + ");\n";
-      level[q] = s;
-    }
-    for (int l = 0, n = mq; n > 1; ++l, n /= 2) {
-      for (int p = 0; p < n; p += 2) {
-        const std::string s = "a" + num(l) + "_" + num(p / 2);
-        o += "      const T " + s + " = " + level[p] + " + " + level[p + 1] + ";\n";
-        level[p / 2] = s;
+  auto contraction = [&](auto val, auto pre, auto post) {
+    std::string s;
+    if (route == TSDE_GEN_ROWWISE) {
+      s += cat({pre(0), "      const T acc = ", val(0), " * w[0];\n", post(0)});
+    } else if (route == TSDE_GEN_GENERIC) {
+      s += "      T acc = T(0);\n";
+      for (int k = 0; k < m; ++k) s += cat({pre(k), "      acc = acc + ", val(k), " * w[", num(k), "];\n", post(k)});
+    } else {
+      std::string level[TSDE_PW_GENERAL_MAX_M / 4];  // the partial sums of the tree's current level
+      for (int q = 0; q < mq; ++q) {
+        const std::string sq = cat({"s", num(q)});
+        const int k0 = 4 * q;
+        s += cat({pre(k0), "      T ", sq, " = ", fma, "(", val(k0), ", w[", num(k0), "], T(0));\n", post(k0)});
+        for (int j = 1; j < 4; ++j)
+          s += cat({pre(k0 + j), "      ", sq, " = ", fma, "(", val(k0 + j), ", w[", num(k0 + j), "], ", sq, ");\n",
+                    post(k0 + j)});
+        level[q] = sq;
       }
+      for (int l = 0, n = mq; n > 1; ++l, n /= 2) {
+        for (int p = 0; p < n; p += 2) {
+          const std::string a = cat({"a", num(l), "_", num(p / 2)});
+          s += cat({"      const T ", a, " = ", level[p], " + ", level[p + 1], ";\n"});
+          level[p / 2] = a;
+        }
+      }
+      s += cat({"      const T acc = ", level[0], ";\n"});
     }
-    o += "      const T acc = " + level[0] + ";\n";
+    s += "      out[j] = acc;\n    }\n  }\n";
+    return s;
+  };
+  auto none = [](int) { return std::string(); };
+  if (layout == TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN) {
+    // the state's g values gs[j][k] stay in registers: z's contraction reads them, y's contracts (gs + g1) and leaves
+    // g1 in their place (pw_general_reversible_heun_steps)
+    o += "  template <typename Op>\n"
+         "  __device__ __forceinline__ void dot(const Op& op, const T (&gs)[4][M], const T (&w)[4 * MQ], T (&out)[4]) {\n"
+         "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
+    o += contraction([&](int k) { return cat({"op.gval(0, {gs[j][", num(k), "]})"}); }, none, none);
+    o += "  template <typename Op>\n"
+         "  __device__ __forceinline__ void gstep(const PwOperands<T>& ops, const PwQuad& c, const T* tp,\n"
+         "                                        const T (&y)[4], const Op& op, const T (&w)[4 * MQ], T (&gs)[4][M],\n"
+         "                                        T (&out)[4]) {\n";
+    o += g_head;
+    o += contraction([&](int k) { return cat({"op.gval(0, {gs[j][", num(k), "], h", num(k), "})"}); },
+                     [&](int k) { return cat({"      const T h", num(k), " = G(", num(k), ");\n"}); },
+                     [&](int k) { return cat({"      gs[j][", num(k), "] = h", num(k), ";\n"}); });
+  } else {
+    o += "  __device__ __forceinline__ void gp(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
+         "                                     const T (&w)[4 * MQ], T (&out)[4]) {\n";
+    o += g_head;
+    o += contraction([&](int k) { return cat({"G(", num(k), ")"}); }, none, none);
   }
-  o += "      out[j] = acc;\n    }\n  }\n};\n}  // namespace\n}  // namespace tsde\n";
+  o += "};\n}  // namespace\n}  // namespace tsde\n";
   const std::string bounds = "__launch_bounds__(" + num(kThreads) + ", 1)";
   if (layout == TSDE_PW_LAYOUT_GENERAL_SRA) {
     for (const char* v : {"single", "multi"}) {
@@ -1872,6 +1927,27 @@ static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t
            "(const __grid_constant__ tsde::PwOperands<tsde::T> ops,\n"
            "    const __grid_constant__ tsde::PwGeneralSraP<tsde::T> p, const tsde::NoiseP<tsde::T> nz) {\n"
            "  tsde::pw_general_sra1<tsde::T, " + src + ", tsde::Prog>(ops, p, nz);\n}\n";
+    }
+    return o;
+  }
+  if (layout == TSDE_PW_LAYOUT_GENERAL_EULER_HEUN) {
+    for (const char* v : {"single", "multi"}) {
+      const std::string src = v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti";
+      o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_general_euler_heun_" + v +
+           "(const __grid_constant__ tsde::PwOperands<tsde::T> ops,\n"
+           "    const tsde::PwGeneralMidP<tsde::T> p, const tsde::NoiseP<tsde::T> nz) {\n"
+           "  tsde::pw_general_euler_heun<tsde::T, " + src + ", tsde::Prog>(ops, p, nz);\n}\n";
+    }
+    return o;
+  }
+  if (layout == TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN) {
+    for (const char* v : {"single", "multi"}) {
+      const std::string src = v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti";
+      o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_general_reversible_heun_" + v +
+           "(const __grid_constant__ tsde::PwOperands<tsde::T> ops,\n"
+           "    const tsde::PwGeneralRevHeunP<tsde::T> p, const tsde::NoiseP<tsde::T> nz,\n"
+           "    const __grid_constant__ tsde::PwSteps<tsde::T> st) {\n"
+           "  tsde::pw_general_reversible_heun_steps<tsde::T, " + src + ", tsde::Prog>(ops, p, nz, st);\n}\n";
     }
     return o;
   }
@@ -1892,13 +1968,22 @@ static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t
   return o;
 }
 
-// The layout a GENERAL launch of tsde_pointwise_compile / tsde_pointwise_source serves `prog` in: the sra1 unit for an
-// SRA-tagged program, else the Euler / midpoint unit (which refuses every other tag).
+// The layout a GENERAL launch of tsde_pointwise_compile / tsde_pointwise_source serves `prog` in: the unit of its
+// SRA, EULER_HEUN or REVERSIBLE_HEUN tag, else the Euler / midpoint unit (which refuses every other tag).
 static int pw_general_layout(const tsde_pointwise* prog) {
-  return prog && prog->reserved == TSDE_PW_LAYOUT_GENERAL_SRA ? TSDE_PW_LAYOUT_GENERAL_SRA : TSDE_PW_LAYOUT_GENERAL;
+  if (!prog) return TSDE_PW_LAYOUT_GENERAL;
+  switch (prog->reserved) {
+    case TSDE_PW_LAYOUT_GENERAL_SRA:
+    case TSDE_PW_LAYOUT_GENERAL_EULER_HEUN:
+    case TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN:
+      return prog->reserved;
+    default:
+      return TSDE_PW_LAYOUT_GENERAL;
+  }
 }
 
-// The loaded kernels of a general-layout program: Euler's two, then midpoint's two; of an SRA-tagged one, sra1's two.
+// The loaded kernels of a general-layout program: Euler's two, then midpoint's two; of a tagged one, the two of its
+// unit (single cell, then multi-cell).
 template <typename T>
 static int pw_general_compiled(const tsde_launch* L, const tsde_pointwise* prog, PwCompiled& kc) {
   int route;
@@ -1907,6 +1992,12 @@ static int pw_general_compiled(const tsde_launch* L, const tsde_pointwise* prog,
   std::string src = pw_general_source(*prog, sizeof(T) == 8, L->m, route, layout);
   if (layout == TSDE_PW_LAYOUT_GENERAL_SRA)
     return pw_loaded(*prog, std::move(src), {"tsde_pw_general_sra1_single", "tsde_pw_general_sra1_multi"}, kc);
+  if (layout == TSDE_PW_LAYOUT_GENERAL_EULER_HEUN)
+    return pw_loaded(*prog, std::move(src), {"tsde_pw_general_euler_heun_single", "tsde_pw_general_euler_heun_multi"},
+                     kc);
+  if (layout == TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN)
+    return pw_loaded(*prog, std::move(src),
+                     {"tsde_pw_general_reversible_heun_single", "tsde_pw_general_reversible_heun_multi"}, kc);
   return pw_loaded(*prog, std::move(src),
                    {"tsde_pw_general_euler_single", "tsde_pw_general_euler_multi", "tsde_pw_general_midpoint_single",
                     "tsde_pw_general_midpoint_multi"},
@@ -1961,14 +2052,17 @@ static int pw_general_euler(const tsde_launch* L, const tsde_noise* nz, const ts
 }
 
 // tsde_step_predictor_corrector_pointwise for a GENERAL launch: one midpoint step as one launch of the program's
-// compiled midpoint kernel.
+// compiled midpoint kernel, or one Euler-Heun step of an EULER_HEUN-tagged program.
 template <typename T>
-static int pw_general_midpoint_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
-                                    const void* y0, const void* t0, const void* t_p, int32_t method, double dt,
-                                    double half_dt, void* y1) {
+static int pw_general_pc_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                              const void* y0, const void* t0, const void* t_p, int32_t method, double dt,
+                              double half_dt, void* y1) {
   int route;
-  if (method != TSDE_PC_MIDPOINT || !t0 || !t_p || !y0 || !y1 || !nz || nz->source != TSDE_SRC_COUNTER ||
-      nz->flags || !pw_general_program(L, prog, sizeof(T), route))
+  const bool euler_heun = method == TSDE_PC_EULER_HEUN;
+  if ((method != TSDE_PC_MIDPOINT && !euler_heun) || !t0 || !t_p || !y0 || !y1 || !nz ||
+      nz->source != TSDE_SRC_COUNTER || nz->flags ||
+      !pw_general_program(L, prog, sizeof(T), route,
+                          euler_heun ? TSDE_PW_LAYOUT_GENERAL_EULER_HEUN : TSDE_PW_LAYOUT_GENERAL))
     return TSDE_EINVAL;
   bool vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y1);
   pw_valid_tables(*prog, &vec, TSDE_PW_M);
@@ -1987,7 +2081,61 @@ static int pw_general_midpoint_step(const tsde_launch* L, const tsde_noise* nz, 
   p.t_p = static_cast<const T*>(t_p);
   p.half_dt = (T)half_dt;
   void* args[] = {&ops, &p, &np};
-  const int e = launch_kernel_handle(kc.kernel[np.n_cells > 1 ? 3 : 2], (p.base.nquads + kThreads - 1) / kThreads,
+  const int first = euler_heun ? 0 : 2;  // (the Euler-Heun unit's kernels, or the midpoint ones after Euler's)
+  const int e = launch_kernel_handle(kc.kernel[first + (np.n_cells > 1 ? 1 : 0)],
+                                     (p.base.nquads + kThreads - 1) / kThreads, kThreads,
+                                     reinterpret_cast<cudaStream_t>(L->stream), args);
+  if (e == 0) g_launches[TSDE_KERNEL_PW_GENERAL].fetch_add(1, std::memory_order_relaxed);
+  return e;
+}
+
+// tsde_solve_reversible_heun_pointwise for a GENERAL launch: the chunk `steps[0, n_steps)` from y0 and the solver state
+// in[] = z0, f0, g0 (g of shape (rows, d, m)), left in out[] = z1, f1, g1, as one launch of the REVERSIBLE_HEUN-tagged
+// program's compiled kernel, under the rules of pw_general_euler.
+template <typename T>
+static int pw_general_reversible_heun(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                                      const void* y0, const void* const (&in)[3], const tsde_pw_step* steps,
+                                      int32_t n_steps, void* const (&out)[3]) {
+  int route;
+  if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
+  if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !y0 ||
+      !pw_general_program(L, prog, sizeof(T), route, TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN))
+    return TSDE_EINVAL;
+  for (int i = 0; i < 3; ++i)
+    if (!in[i] || !out[i]) return TSDE_EINVAL;
+  bool vec = L->d % 4 == 0 && aligned16(y0);
+  for (int i = 0; i < 2; ++i) vec = vec && aligned16(in[i]) && aligned16(out[i]);  // z, f
+  pw_valid_tables(*prog, &vec, TSDE_PW_M);
+  NoiseP<T> np;
+  if (int e = fill_noise<T>(L, nz, false, np)) return e;
+  if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
+  PwSteps<T> st{};
+  st.n = n_steps;
+  for (int j = 0; j < n_steps; ++j) {
+    const tsde_pw_step& s = steps[j];
+    if (!s.t0) return TSDE_EINVAL;
+    if (s.y1 && !aligned16(s.y1)) vec = false;
+    st.s[j] = PwStep<T>{s.cell_id, static_cast<const T*>(s.t0), static_cast<T*>(s.y1), (T)sqrt(s.h), (T)s.dt};
+  }
+  PwCompiled kc;
+  if (int e = pw_general_compiled<T>(L, prog, kc)) return e;
+  PwOperands<T> ops = pw_operands<T>(prog);
+  PwGeneralRevHeunP<T> p{};
+  p.base.y0 = static_cast<const T*>(y0);
+  fill_quad_map(L->rows, L->d, p.base);
+  p.base.vec = vec ? 1 : 0;
+  p.z0 = static_cast<const T*>(in[0]);
+  p.f0 = static_cast<const T*>(in[1]);
+  p.g0 = static_cast<const T*>(in[2]);
+  p.z1 = static_cast<T*>(out[0]);
+  p.f1 = static_cast<T*>(out[1]);
+  p.g1 = static_cast<T*>(out[2]);
+  p.gvec = L->m % 4 == 0 && aligned16(in[2]) && aligned16(out[2]) ? 1 : 0;
+  // (the multi-cell merge reads the first cell and the uniform length from the noise descriptor)
+  np.cell_id = steps[0].cell_id;
+  np.h = steps[0].h;
+  void* args[] = {&ops, &p, &np, &st};
+  const int e = launch_kernel_handle(kc.kernel[np.n_cells > 1 ? 1 : 0], (p.base.nquads + kThreads - 1) / kThreads,
                                      kThreads, reinterpret_cast<cudaStream_t>(L->stream), args);
   if (e == 0) g_launches[TSDE_KERNEL_PW_GENERAL].fetch_add(1, std::memory_order_relaxed);
   return e;

@@ -436,6 +436,60 @@ struct GSraFinalOp {
     o[0] = y1;
   }
 };
+// y' = y0 + g.dW                                                                 methods/euler_heun.py:36
+template <typename T>
+struct GEulerHeunPredictOp {
+  static constexpr int NE = 1, NG = 1, NP = 1, NO = 1;
+  static constexpr bool WANT_U = false;
+  __device__ __forceinline__ T gval(int, const T (&g)[1]) const { return g[0]; }
+  __device__ __forceinline__ T weight(int, T w, T) const { return w; }
+  __device__ __forceinline__ void combine(const T (&e)[1], const T (&gp)[1], T (&o)[1]) const {
+    o[0] = e[0] + gp[0];
+  }
+};
+// y1 = y0 + dt*f + (g.dW + g'.dW)*0.5                                            methods/euler_heun.py:40
+template <typename T>
+struct GEulerHeunOp {
+  static constexpr int NE = 2, NG = 2, NP = 2, NO = 1;
+  static constexpr bool WANT_U = false;
+  static constexpr bool STREAM_INPUTS = true;  // last kernel of the step: the g tiles are dead afterwards
+  T dt;
+  __device__ __forceinline__ T gval(int p, const T (&g)[2]) const { return g[p]; }
+  __device__ __forceinline__ T weight(int, T w, T) const { return w; }
+  __device__ __forceinline__ void combine(const T (&e)[2], const T (&gp)[2], T (&o)[1]) const {
+    o[0] = (e[0] + dt * e[1]) + (gp[0] + gp[1]) * T(0.5);
+  }
+};
+// z1 = 2*y0 - z0 + f0*dt + g0.dW                                                 reversible_heun.py:69
+// sign = -1 gives the adjoint's reconstruction z1 = 2*y0 - z0 - f0*dt - g0.dW    reversible_heun.py:109
+template <typename T>
+struct GRevHeunZOp {
+  static constexpr int NE = 3, NG = 1, NP = 1, NO = 1;
+  static constexpr bool WANT_U = false;
+  T dt;
+  int backward;
+  __device__ __forceinline__ T gval(int, const T (&g)[1]) const { return g[0]; }
+  __device__ __forceinline__ T weight(int, T w, T) const { return w; }
+  __device__ __forceinline__ void combine(const T (&e)[3], const T (&gp)[1], T (&o)[1]) const {
+    const T a = T(2) * e[0] - e[1];
+    o[0] = backward ? ((a - e[2] * dt) - gp[0]) : ((a + e[2] * dt) + gp[0]);
+  }
+};
+// y1 = y0 + (f0+f1)*half_dt + (g0+g1).(0.5*dW)                                   reversible_heun.py:71
+// backward: y1 = y0 - (f0+f1)*half_dt - (g0+g1).half_dW                          reversible_heun.py:134-135
+template <typename T>
+struct GRevHeunOp {
+  static constexpr int NE = 3, NG = 2, NP = 1, NO = 1;
+  static constexpr bool WANT_U = false;
+  T half_dt;
+  int backward;
+  __device__ __forceinline__ T gval(int, const T (&g)[2]) const { return g[0] + g[1]; }
+  __device__ __forceinline__ T weight(int, T w, T) const { return T(0.5) * w; }
+  __device__ __forceinline__ void combine(const T (&e)[3], const T (&gp)[1], T (&o)[1]) const {
+    const T fd = (e[1] + e[2]) * half_dt;
+    o[0] = backward ? ((e[0] - fd) - gp[0]) : ((e[0] + fd) + gp[0]);
+  }
+};
 
 // ---- general / additive noise with an element-wise f and g (tsde_solve_euler_general_pointwise, ...) ---------------
 // One thread per (row, quad of d), as above.  The thread draws all m increments of its row (MQ channel quads on the
@@ -445,6 +499,10 @@ struct GSraFinalOp {
 //   load(ops, c)                  the operands kept in registers, after the dependency wait
 //   f(ops, c, t, y, f)            the f program at (*t, y)
 //   gp(ops, c, t, y, w, gp)       the g program at (*t, y), contracted with w[0, 4 MQ)
+// and, in the reversible-Heun unit, whose g values stay in registers (gs[j][k]: lane j, channel k < M):
+//   dot(op, gs, w, gp)                  op.gval(0, {gs_k}) contracted with w
+//   gstep(ops, c, t, y, op, w, gs, gp)  the g program at (*t, y), g1_k; op.gval(0, {gs_k, g1_k}) contracted with w,
+//                                       and gs_k <- g1_k
 
 // The increments of this thread's row: channel k in w[k], and with WANT_U its U in u[k]
 template <typename T, int SRC, int MQ, bool WANT_U>
@@ -605,6 +663,161 @@ __device__ __forceinline__ void pw_general_sra1(const PwOperands<T>& ops, const 
     h[i] = o[0];
   }
   store_quad(p.base.y1, c.base, c.vec, c.nvalid, h);
+}
+
+// One Euler-Heun step (methods/euler_heun.py:34-40), with the parameters of a midpoint step (half_dt unused):
+// f = f(t0, y0) and g.dW at (t0, y0); y' = GEulerHeunPredictOp on (y0, g.dW); g'.dW at (t_p, y');
+// y1 = GEulerHeunOp{dt} on (y0, f, g.dW, g'.dW).  The unfused predict launch and the final one see the same g operand
+// (g and g' come from one program: both dense, or both the user's DM block) and stage m increments per row, so their
+// routes are one and the predictor's g.dW is the final launch's first product.
+template <typename T, int SRC, typename Prog>
+__device__ __forceinline__ void pw_general_euler_heun(const PwOperands<T>& ops, const PwGeneralMidP<T>& p,
+                                                      const NoiseP<T>& nz) {
+  PwQuad c;
+  int64_t Q, row, q;
+  pw_locate(p.base, c, Q, row, q);
+  T w[4 * Prog::MQ];
+  pw_general_noise<T, SRC, Prog::MQ>(nz, load_key(nz.key), row, w);
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (Q >= p.base.nquads) return;
+  Prog prog;
+  T y0[4], yp[4], f[4], gp[4], gq[4];
+  load_quad(p.base.y0, c.base, c.vec, c.nvalid, y0);
+  prog.load(ops, c);
+  prog.f(ops, c, p.base.t0, y0, f);
+  prog.gp(ops, c, p.base.t0, y0, w, gp);
+  const GEulerHeunPredictOp<T> predict{};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const T e[1] = {y0[i]}, g1[1] = {gp[i]};
+    T o[1];
+    predict.combine(e, g1, o);
+    yp[i] = o[0];
+  }
+  prog.gp(ops, c, p.t_p, yp, w, gq);
+  const GEulerHeunOp<T> step{p.base.dt};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const T e[2] = {y0[i], f[i]}, g2[2] = {gp[i], gq[i]};
+    T o[1];
+    step.combine(e, g2, o);
+    yp[i] = o[0];
+  }
+  store_quad(p.base.y1, c.base, c.vec, c.nvalid, yp);
+}
+
+template <typename T>
+struct PwGeneralRevHeunP {
+  PwP<T> base;            // y0, the quad mapping (base.y1, t0, dt and ito unused: the step table has them)
+  const T *z0, *f0, *g0;  // the solver state the chunk starts from: z and f (rows, d), g (rows, d, m)
+  T *z1, *f1, *g1;        // and where the chunk leaves it
+  int32_t gvec;           // m % 4 == 0 and g0, g1 16-byte aligned: g moves as quads
+};
+
+// This thread's values of a (rows, d, m) tensor: lane j's run of M channels at (c.base + j) * M, a padding lane
+// reading lane 0's (as Prog's G does)
+template <typename T, int M>
+__device__ __forceinline__ void pw_load_g(const T* g, const PwQuad& c, bool vec, T (&gs)[4][M]) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int64_t base = (c.base + (j < c.nvalid ? j : 0)) * M;
+    if (M % 4 == 0 && vec) {
+#pragma unroll
+      for (int q = 0; q < M / 4; ++q) {
+        T v[4];
+        ld4(g + base + 4 * q, v);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) gs[j][4 * q + i] = v[i];
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < M; ++k) gs[j][k] = g[base + k];
+    }
+  }
+}
+template <typename T, int M>
+__device__ __forceinline__ void pw_store_g(T* g, const PwQuad& c, bool vec, const T (&gs)[4][M]) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    if (j >= c.nvalid) continue;
+    const int64_t base = (c.base + j) * M;
+    if (M % 4 == 0 && vec) {
+#pragma unroll
+      for (int q = 0; q < M / 4; ++q) {
+        const T v[4] = {gs[j][4 * q], gs[j][4 * q + 1], gs[j][4 * q + 2], gs[j][4 * q + 3]};
+        st4(g + base + 4 * q, v);
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < M; ++k) g[base + k] = gs[j][k];
+    }
+  }
+}
+
+// Consecutive reversible-Heun steps, as pw_general_euler_steps (reversible_heun.py:64-73); st.s[j].t0 is the step's t1:
+//   z1 = GRevHeunZOp{dt} on (y, z, f, g.dW);  f1 at (t1, z1);
+//   g1 at (t1, z1), channel by channel, contracted as GRevHeunOp's (g + g1) . (0.5 dW) and left in place of g;
+//   y1 = GRevHeunOp{T(0.5) * dt} on (y, f, f1, that product);  (y, z, f) <- (y1, z1, f1)
+// The solver state (z, f, g) is read once at the chunk's start and stored once at its end, to pointers the chunk does
+// not read; each lane's m values of g stay in registers in between.  Both contractions take the weights the unfused
+// launches form (the op's weight per channel) and the route of their dense g operands (Prog, pw_general_source).
+// With its 4 M values of g, this kernel holds the most registers of the general ones; m = 32 spills (DESIGN §4).
+template <typename T, int SRC, typename Prog>
+__device__ __forceinline__ void pw_general_reversible_heun_steps(const PwOperands<T>& ops,
+                                                                 const PwGeneralRevHeunP<T>& p, const NoiseP<T>& nz,
+                                                                 const PwSteps<T>& st) {
+  PwQuad c;
+  int64_t Q, row, q;
+  pw_locate(p.base, c, Q, row, q);
+  const Key key = load_key(nz.key);
+  Prog prog;
+  T y[4], z[4], f[4], g[4][Prog::M];
+  for (int j = 0; j < st.n; ++j) {
+    const PwStep<T>& s = st.s[j];
+    NoiseP<T> n = nz;  // this step's cell
+    n.cell_id = s.cell;
+    n.sqrt_h = s.sqrt_h;
+    T w[4 * Prog::MQ], wt[4 * Prog::MQ];
+    pw_general_noise<T, SRC, Prog::MQ>(n, key, row, w);
+    if (j == 0) {  // the first increments are drawn while the previous kernel drains; the rest is read after the wait
+      asm volatile("griddepcontrol.wait;" ::: "memory");
+      if (Q >= p.base.nquads) return;
+      load_quad(p.base.y0, c.base, c.vec, c.nvalid, y);
+      load_quad(p.z0, c.base, c.vec, c.nvalid, z);
+      load_quad(p.f0, c.base, c.vec, c.nvalid, f);
+      pw_load_g<T, Prog::M>(p.g0, c, p.gvec != 0, g);
+      prog.load(ops, c);
+    }
+    T gp[4], f1[4];
+    const GRevHeunZOp<T> zop{s.dt, 0};
+#pragma unroll
+    for (int k = 0; k < 4 * Prog::MQ; ++k) wt[k] = zop.weight(0, w[k], T(0));
+    prog.dot(zop, g, wt, gp);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const T e[3] = {y[i], z[i], f[i]}, g1[1] = {gp[i]};
+      T o[1];
+      zop.combine(e, g1, o);
+      z[i] = o[0];
+    }
+    prog.f(ops, c, s.t0, z, f1);
+    const GRevHeunOp<T> step{T(0.5) * s.dt, 0};
+#pragma unroll
+    for (int k = 0; k < 4 * Prog::MQ; ++k) wt[k] = step.weight(0, w[k], T(0));
+    prog.gstep(ops, c, s.t0, z, step, wt, g, gp);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const T e[3] = {y[i], f[i], f1[i]}, g1[1] = {gp[i]};
+      T o[1];
+      step.combine(e, g1, o);
+      y[i] = o[0];
+      f[i] = f1[i];
+    }
+    if (s.y1) store_quad(s.y1, c.base, c.vec, c.nvalid, y);
+  }
+  store_quad(p.z1, c.base, c.vec, c.nvalid, z);
+  store_quad(p.f1, c.base, c.vec, c.nvalid, f);
+  pw_store_g<T, Prog::M>(p.g1, c, p.gvec != 0, g);
 }
 
 }  // namespace tsde

@@ -883,8 +883,8 @@ static int launch_gen_fmt(const tsde_launch* L, const tsde_noise* nz, std::initi
 }
 
 // ---- ops ---------------------------------------------------------------------------------------
-// (GEulerOp, GMidpointPredictOp, GSraStageOp and GSraFinalOp: pw_device.cuh, which the run-time compiled general-noise
-// kernels include too)
+// (GEulerOp, GMidpointPredictOp, GSraStageOp, GSraFinalOp, GEulerHeunPredictOp, GEulerHeunOp, GRevHeunZOp and
+// GRevHeunOp: pw_device.cuh, which the run-time compiled general-noise kernels include too)
 // y1 = y0 + (dt*(f+f') + g.dW + g'.dW) * 0.5                                     methods/heun.py:46
 template <typename T>
 struct GHeunOp {
@@ -896,60 +896,6 @@ struct GHeunOp {
   __device__ __forceinline__ T weight(int, T w, T) const { return w; }
   __device__ __forceinline__ void combine(const T (&e)[3], const T (&gp)[2], T (&o)[1]) const {
     o[0] = e[0] + ((dt * (e[1] + e[2]) + gp[0]) + gp[1]) * T(0.5);
-  }
-};
-// y' = y0 + g.dW                                                                 methods/euler_heun.py:36
-template <typename T>
-struct GEulerHeunPredictOp {
-  static constexpr int NE = 1, NG = 1, NP = 1, NO = 1;
-  static constexpr bool WANT_U = false;
-  __device__ __forceinline__ T gval(int, const T (&g)[1]) const { return g[0]; }
-  __device__ __forceinline__ T weight(int, T w, T) const { return w; }
-  __device__ __forceinline__ void combine(const T (&e)[1], const T (&gp)[1], T (&o)[1]) const {
-    o[0] = e[0] + gp[0];
-  }
-};
-// y1 = y0 + dt*f + (g.dW + g'.dW)*0.5                                            methods/euler_heun.py:40
-template <typename T>
-struct GEulerHeunOp {
-  static constexpr int NE = 2, NG = 2, NP = 2, NO = 1;
-  static constexpr bool WANT_U = false;
-  static constexpr bool STREAM_INPUTS = true;  // last kernel of the step: the g tiles are dead afterwards
-  T dt;
-  __device__ __forceinline__ T gval(int p, const T (&g)[2]) const { return g[p]; }
-  __device__ __forceinline__ T weight(int, T w, T) const { return w; }
-  __device__ __forceinline__ void combine(const T (&e)[2], const T (&gp)[2], T (&o)[1]) const {
-    o[0] = (e[0] + dt * e[1]) + (gp[0] + gp[1]) * T(0.5);
-  }
-};
-// z1 = 2*y0 - z0 + f0*dt + g0.dW                                                 reversible_heun.py:69
-// sign = -1 gives the adjoint's reconstruction z1 = 2*y0 - z0 - f0*dt - g0.dW    reversible_heun.py:109
-template <typename T>
-struct GRevHeunZOp {
-  static constexpr int NE = 3, NG = 1, NP = 1, NO = 1;
-  static constexpr bool WANT_U = false;
-  T dt;
-  int backward;
-  __device__ __forceinline__ T gval(int, const T (&g)[1]) const { return g[0]; }
-  __device__ __forceinline__ T weight(int, T w, T) const { return w; }
-  __device__ __forceinline__ void combine(const T (&e)[3], const T (&gp)[1], T (&o)[1]) const {
-    const T a = T(2) * e[0] - e[1];
-    o[0] = backward ? ((a - e[2] * dt) - gp[0]) : ((a + e[2] * dt) + gp[0]);
-  }
-};
-// y1 = y0 + (f0+f1)*half_dt + (g0+g1).(0.5*dW)                                   reversible_heun.py:71
-// backward: y1 = y0 - (f0+f1)*half_dt - (g0+g1).half_dW                          reversible_heun.py:134-135
-template <typename T>
-struct GRevHeunOp {
-  static constexpr int NE = 3, NG = 2, NP = 1, NO = 1;
-  static constexpr bool WANT_U = false;
-  T half_dt;
-  int backward;
-  __device__ __forceinline__ T gval(int, const T (&g)[2]) const { return g[0] + g[1]; }
-  __device__ __forceinline__ T weight(int, T w, T) const { return T(0.5) * w; }
-  __device__ __forceinline__ void combine(const T (&e)[3], const T (&gp)[1], T (&o)[1]) const {
-    const T fd = (e[1] + e[2]) * half_dt;
-    o[0] = backward ? ((e[0] - fd) - gp[0]) : ((e[0] + fd) + gp[0]);
   }
 };
 // ---- outer-product bookkeeping of the reversible-Heun adjoint (g-shaped element-wise) ----------
