@@ -12,10 +12,10 @@ from torchsde_b200._core import pointwise
 B, D = 6, 8
 
 
-def record(f, g, m, pattern='fg', dtype=torch.float32):
+def record(f, g, m, pattern='fg', dtype=torch.float32, layout=None):
     y = torch.rand(B, D, dtype=dtype) + 0.1
     t = torch.tensor(0.25, dtype=dtype)
-    rec = pointwise.GeneralRecorder(y, t, pattern, m)
+    rec = pointwise.GeneralRecorder(y, t, pattern, m, layout=layout)
     for kind in pattern:
         rec.evaluation(kind, (lambda: f(t, y)) if kind == 'f' else (lambda: g(t, y)), t, y)
     return rec, rec.finish()

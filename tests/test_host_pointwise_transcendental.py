@@ -3,8 +3,9 @@ sigmoid, a general power and the tanh / sigmoid backward ops, which the tapes ta
 options={'transcendental': True} and only in the layouts the library compiles (Milstein, its adaptive proposal, and
 the general / additive-noise Euler, midpoint and sra1 kernels).  Here: which recorders accept them, the opcodes they
 record (the vjp's backward ops, the pow ladder), the NVRTC version guard, the generated sources (calls of the helper
-functions, and the unchanged sources of programs without them), the refusal of the interpreted entry points, and the
-helper and program translation units compiled and linked as the library links them, with their registers and stack."""
+functions, and the digests that pin every generator's text, with and without them), the refusal of the interpreted
+entry points, and the helper and program translation units compiled and linked as the library links them, with their
+registers and stack."""
 import ctypes
 import hashlib
 import re
@@ -42,13 +43,13 @@ def _milstein(op, where, transcendental=True, dtype=torch.float32):
     return rec, res
 
 
-def _general(op, pattern='fg', transcendental=True, m=4, dtype=torch.float32):
+def _general(op, pattern='fg', transcendental=True, m=4, dtype=torch.float32, layout=None):
     """A general-noise tape whose g is op(y)[..., None] * S (TanhGeneral's shape)."""
     fn = OPS[op][0]
     mu, S, _ = general.params(m, dtype)
     y = torch.rand(general.B, general.D, dtype=dtype) + 0.1
     t = torch.tensor(0.25, dtype=dtype)
-    rec = pointwise.GeneralRecorder(y, t, pattern, m, transcendental)
+    rec = pointwise.GeneralRecorder(y, t, pattern, m, transcendental, layout)
     for kind in pattern:
         fg = (lambda: mu * y) if kind == 'f' else (lambda: fn(y)[..., None] * S)
         rec.evaluation(kind, fg, t, y)
@@ -185,8 +186,11 @@ def test_generated_sources_call_the_helpers(op, dtype):
     assert re.search(rf'n\d+\[j\] = pw_{name}\(y\[j\]', narrow)
 
 
-# sha256 of the generated sources of the existing tests' programs, in the order below: the sources of programs without
-# transcendental ops, written by the generators before the ops existed
+# sha256 of the generated sources of the programs below, in the order below.  host, select and general-fg / -fggf:
+# the existing tests' programs, written by the generators before the transcendental ops existed.  general-eulerheun /
+# -revheun: those programs under the Euler-Heun and reversible-Heun tags.  widths: every tagged unit at Brownian
+# widths around each route's edges, with g also the user's (d, m) block, 16-byte aligned or not (so the row-wise,
+# tile and generic contractions all appear).  transcendental: a program per op, Milstein and every general unit.
 SOURCES = {
     'host-float32': 'c47308dbab452dbf4772981850f754c9b50c0e3389e088f2b07ac335c19dbf6a',
     'host-float64': '60dca03978eff78bc00df009e8bd6b62b72ab41c552bded8e6925ae02713474d',
@@ -196,26 +200,71 @@ SOURCES = {
     'general-fg-float64': '9670665a269f1c6499ce1e367a503e3db2a37af3405c24370f84c5f3612fd627',
     'general-fggf-float32': '0f8938695716053e0b5267b10c235906d18e53f7de2f34fae0b60f39daf89698',
     'general-fggf-float64': 'cf34954570a1b377e0eaa00f46b381969773ceb6929fadf14372bd10729b819b',
+    'general-eulerheun-float32': 'c0ea862bdce9217b9ad7f2126e2e03d9184f1c9107e4a965bc4c857df0cbf9ba',
+    'general-eulerheun-float64': 'ce98b518dbcc370cc58850544d04e55904811d65af5b057dfe638b5a0cf5122d',
+    'general-revheun-float32': '4cf36b5a13b3ee199589bb9a571076aa7bab818028105aae6359358cb4aef2fa',
+    'general-revheun-float64': '92bb442f095a45fab2217ad58ceffedcc12e840a235f2261290b0aab3773e29b',
+    'widths-float32': 'd9e0b58f710d5af3ec61647161ce1b42e77c2ff3b0c215fe171723105b7c7bf4',
+    'widths-float64': '08e074cfd1cb32269ba0170d736e266470d1086a508b403e8b22376ecfc94ddf',
+    'transcendental-float32': '80be0f6f672771e5e71b2d23809664bbe3707e97b096db25d11b4948b82e712c',
+    'transcendental-float64': '6ed18d3ca8a7f4d7b030aedb0f77636d58597f2262a483271e76ec91193ce0fb',
 }
 
+# the general units: (evaluation pattern, layout tag)
+UNITS = {'fg': ('fg', _cabi.PW_LAYOUT_GENERAL), 'fggf': ('fggf', _cabi.PW_LAYOUT_GENERAL_SRA),
+         'eulerheun': ('fgg', _cabi.PW_LAYOUT_GENERAL_EULER_HEUN),
+         'revheun': ('fg', _cabi.PW_LAYOUT_GENERAL_REVERSIBLE_HEUN)}
+WIDTHS = (1, 2, 4, 5, 8, 17, 32)
 
-@pytest.mark.parametrize('key', sorted(SOURCES))
-def test_the_sources_of_programs_without_the_ops_are_unchanged(key):
-    h = hashlib.sha256()
+
+def _sources(key):
+    """The generated sources that `key`'s digest covers, in order."""
     parts = key.split('-')
     dtype = getattr(torch, parts[-1])
     if parts[0] in ('host', 'select'):
         table = milstein.ACCEPTED if parts[0] == 'host' else select.ACCEPTED
         for name in sorted(table):
             _, res, _, _ = milstein._record(*table[name], dtype)
-            h.update(_cabi.pointwise_source(res[0], dtype).encode())
-    else:
+            yield _cabi.pointwise_source(res[0], dtype)
+    elif parts[0] == 'general':
+        pattern, layout = UNITS[parts[1]]
         for m in (1, 3, 16):
             acc = general.accepted(m, dtype)
             for name in sorted(acc):
-                _, res = general.record(*acc[name], m, parts[1], dtype)
+                _, res = general.record(*acc[name], m, pattern, dtype, layout)
                 if res is not None:
-                    h.update(_cabi.general_pointwise_source(res[0], dtype, general.D, m).encode())
+                    yield _cabi.general_pointwise_source(res[0], dtype, general.D, m)
+    elif parts[0] == 'widths':
+        for m in WIDTHS:
+            store = torch.zeros(general.D * m + 1, dtype=dtype)
+            blocks = (torch.rand(general.D, m, dtype=dtype), store[1:].view(general.D, m))
+            for unit in sorted(UNITS):
+                pattern, layout = UNITS[unit]
+                acc = general.accepted(m, dtype)
+                fgs = [acc[name] for name in sorted(acc)]
+                fgs += [(lambda t, y: -y, lambda t, y, S=S: S.expand(general.B, general.D, m)) for S in blocks]
+                for f, g in fgs:
+                    rec, res = general.record(f, g, m, pattern, dtype, layout)
+                    assert res is not None, rec.reason
+                    yield _cabi.general_pointwise_source(res[0], dtype, general.D, m)
+    else:
+        for op in sorted(OPS):
+            for where in 'fg':
+                yield _cabi.pointwise_source(_milstein(op, where, dtype=dtype)[1][0], dtype)
+            for unit in sorted(UNITS):
+                pattern, layout = UNITS[unit]
+                for m in (1, 4, 5):
+                    rec, res = _general(op, pattern, m=m, dtype=dtype, layout=layout)
+                    assert res is not None, rec.reason
+                    yield _cabi.general_pointwise_source(res[0], dtype, general.D, m)
+
+
+@pytest.mark.parametrize('key', sorted(SOURCES))
+def test_the_sources_of_programs_without_the_ops_are_unchanged(key):
+    h = hashlib.sha256()
+    for src in _sources(key):
+        assert src is not None
+        h.update(src.encode())
     assert h.hexdigest() == SOURCES[key]
 
 

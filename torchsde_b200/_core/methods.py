@@ -120,10 +120,8 @@ class Euler(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
         # the first step of an eligible solve runs as always, with the user's two evaluations recorded
         rec = pointwise.pc_recorder(self, y0, c.t0, 'fg')
         L, nz, f, g = self._f_and_g_prod(c, c.t0, y0, rec)
-        if isinstance(rec, pointwise.GeneralRecorder):
-            self._pw = pointwise.compile_general(self, rec, rec.finish()) or False
-        elif rec is not None:
-            self._pw = rec.finish() or False
+        if rec is not None:
+            self._pw = pointwise.finish(self, rec)
         return self._k('tsde_step_euler', L, nz, (y0, f, g), (c.dt,), out), ()
 
 
@@ -265,7 +263,7 @@ class Heun(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
         yp = self._k('tsde_step_euler', L, nz, (y0, f, g), (c.dt,), None)
         L, nz, fp, gp = self._f_and_g_prod(c, c.t1, yp, rec)
         if rec is not None:
-            self._pw = rec.finish() or False
+            self._pw = pointwise.finish(self, rec)
         return self._k('tsde_step_heun', L, nz, (y0, f, fp, g, gp), (c.dt,), out), ()
 
 
@@ -303,10 +301,8 @@ class Midpoint(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
         L, nz, f, g = self._f_and_g_prod(c, c.t0, y0, rec)
         yp = self._k('tsde_midpoint_predict', L, nz, (y0, f, g), (c.scalars['half_dt'],), None)
         L, nz, fp, gp = self._f_and_g_prod(c, c.aux_t[0], yp, rec)
-        if isinstance(rec, pointwise.GeneralRecorder):
-            self._pw = pointwise.compile_general(self, rec, rec.finish()) or False
-        elif rec is not None:
-            self._pw = rec.finish() or False
+        if rec is not None:
+            self._pw = pointwise.finish(self, rec)
         return self._k('tsde_step_euler', L, nz, (y0, fp, gp), (c.dt,), out), ()
 
 
@@ -359,10 +355,8 @@ class EulerHeun(_ProposalMixin, _ProdMixin, base_solver.BaseSDESolver):
             L2, nz2, gp = self._LU, self._feed.unit(), _contig(gp)
         else:
             L2, nz2, gp = self._g_prod(c, c.t1, yp, rec)
-        if isinstance(rec, pointwise.GeneralRecorder):
-            self._pw = pointwise.compile_general(self, rec, rec.finish()) or False
-        elif rec is not None:
-            self._pw = rec.finish() or False
+        if rec is not None:
+            self._pw = pointwise.finish(self, rec)
         return self._k('tsde_step_euler_heun', L2, nz2, (y0, f, g, gp), (c.dt,), out), ()
 
 
@@ -435,10 +429,7 @@ class ReversibleHeun(base_solver.BaseSDESolver):
         if rec is not None:
             f1, g1 = self._fork(lambda: rec.evaluation('f', lambda: sde.f(c.t1, z1), c.t1, z1),
                                 lambda: rec.evaluation('g', lambda: sde.g(c.t1, z1), c.t1, z1))
-            if isinstance(rec, pointwise.GeneralRecorder):
-                self._pw = pointwise.compile_general(self, rec, rec.finish()) or False
-            else:
-                self._pw = rec.finish() or False
+            self._pw = pointwise.finish(self, rec)
         else:
             f1, g1 = self._f_and_g(c.t1, z1)
         f1, g1 = _contig(f1), _contig(g1)
@@ -569,7 +560,7 @@ class SRK(_ProposalMixin, base_solver.BaseSDESolver):
         h1_3 = self._k('tsde_srk_diag_stage3', LU, None, (y0, g0, g1, f2, g2), (c.dt, s['sqrt_dt']), None)
         g3 = g(t_q, h1_3)
         if rec is not None:
-            self._pw = rec.finish() or False
+            self._pw = pointwise.finish(self, rec)
         return self._k('tsde_step_srk_diag', L, self._feed.get(c, True), (y0, f0, f1, f2, g0, g1, g2, g3),
                        (c.dt, s['rdt'], s['sqrt_dt'], s['three_dt']), out)
 
@@ -598,7 +589,7 @@ class SRK(_ProposalMixin, base_solver.BaseSDESolver):
                        None)
         f1 = f(t_34, h0_1)
         if rec is not None:
-            self._pw = pointwise.compile_general(self, rec, rec.finish()) or False
+            self._pw = pointwise.finish(self, rec)
         return self._k('tsde_step_srk_additive', self._L, self._feed.get(c, True), (y0, f0, f1, ga, gb),
                        (c.dt, s['rdt']), out)
 

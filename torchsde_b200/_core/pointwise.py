@@ -953,6 +953,14 @@ def compile_general(solver, rec, res):
     return res
 
 
+def finish(solver, rec):
+    """The end of a recording step of `solver` other than Milstein's: what becomes its `_pw`, the program of `rec`'s
+    tape (a GeneralRecorder's once `compile_general` has compiled it), or False if the tape was rejected."""
+    if isinstance(rec, GeneralRecorder):
+        return compile_general(solver, rec, rec.finish()) or False
+    return rec.finish() or False
+
+
 def ready(solver):
     """Whether `solver` has a program and the counter noise its kernel draws from."""
     return bool(solver._pw) and solver._feed.binding is not None

@@ -8,11 +8,13 @@
 // The SDE's f and g (and for Milstein the vjp of g) arrive as a small program of element-wise instructions.  The SRK,
 // predictor-corrector and Euler / reversible-Heun kernels interpret it between the unfused step's own ops
 // (tableau_diag_ops.cuh), one IEEE rounding per element (this translation unit is compiled with -fmad=false, as the
-// tableaus are), so a fused step equals the unfused one bit for bit.  A Milstein program is compiled instead, at run
-// time, into a kernel of its own with the same roundings (pw_milstein_source, NVRTC).  The file holds, in this order:
-// the decoded program, its register file and interpreter, the validation every program passes before a launch and the
-// decoding that follows it, the prologue the kernels share, the Milstein code generator and its kernel cache, the
-// interpreting kernels with the layout each accepts, and the launches.
+// tableaus are), so a fused step equals the unfused one bit for bit.  A Milstein program, and a general-noise one, is
+// compiled instead, at run time, into a kernel of its own with the same roundings (pw_milstein_source,
+// pw_general_source, NVRTC).  The file holds, in this order: the decoded program, its register file and interpreter,
+// the validation every program passes before a launch and the decoding that follows it, the prologue the kernels
+// share, the program emitter the two code generators share, the compiled units (kPwUnits) and their kernel cache, the
+// interpreting kernels with the layout each accepts, the host steps every launch shares (pw_fill, pw_steps,
+// pw_launch, pw_launch_compiled), and the launches.
 //
 // One thread per quad, as ew_fast_kernel.  The program's registers live in shared memory as 16-byte vectors laid
 // out [reg][plane][thread] (a float quad is one plane, a double quad two): a warp's 128-bit access is 512 contiguous
@@ -396,16 +398,17 @@ __device__ __forceinline__ bool pw_begin(const PwProg<T>& pg, const PwP<T>& p, c
   return true;
 }
 
-// ---- consecutive Milstein steps, compiled (tsde_solve_milstein_pointwise, tsde_step_milstein_pointwise) -----------
+// ---- compiled programs (tsde_solve_milstein_pointwise, tsde_step_milstein_pointwise, GENERAL launches) -------------
 // A Milstein program is not interpreted: once validated, it is written out as one CUDA translation unit
 // (pw_milstein_source) whose kernels run pw_milstein_steps (pw_device.cuh) with the program inlined as straight-line
 // register code, compiled at run time by NVRTC to an sm_90a cubin and loaded as a CUDA library.  Each instruction is
-// the expression of the matching `case` of pw_loop, one statement per lane, and the translation unit is compiled with
-// the library's IEEE options (-fmad=false, NVRTC's default -prec-div=true, -prec-sqrt=true, -ftz=false), so a compiled
-// step equals the unfused one bit for bit.  Operand values and addresses are not in the source: IMM values and
-// SCALAR / CHANNEL / ROW pointers are the kernel's PwOperands parameter, so the source is a function of the program's
-// structure alone (instruction words, n_regs, n_fg, result sources, operand kinds, dtype), and it is the key of the
-// process-wide cache of loaded kernels: SDEs that differ only in parameter values share one compiled kernel.
+// the expression of the matching `case` of pw_loop (pw_expression), one statement per lane, and the translation unit
+// is compiled with the library's IEEE options (-fmad=false, NVRTC's default -prec-div=true, -prec-sqrt=true,
+// -ftz=false), so a compiled step equals the unfused one bit for bit.  Operand values and addresses are not in the
+// source: IMM values and SCALAR / CHANNEL / ROW pointers are the kernel's PwOperands parameter, so the source is a
+// function of the program's structure alone (instruction words, n_regs, n_fg, result sources, operand kinds, dtype),
+// and it is the key of the process-wide cache of loaded kernels: SDEs that differ only in parameter values share one
+// compiled kernel.  The general-noise programs (pw_general_source) are written out from the same parts.
 
 // CHANNEL / ROW operand quads a compiled program keeps in registers for the whole chunk (loaded once per launch after
 // the dependency wait); any past these are loaded again at every step.  Within the launch bounds below, cfg2's program
@@ -416,16 +419,19 @@ constexpr int kPwJitHoistQuads[2] = {4, 2};  // float, double
 // 88-92 in fp64): pointwise.py's _RESIDENT_CTAS and chunk_length count on it.
 constexpr int kPwJitCtas[2] = {4, 2};
 
-static_assert(sizeof(PwOperands<double>) + sizeof(PwP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <=
-                  4096,
-              "the compiled Milstein kernel's parameters fit the 4 KiB parameter space");
-
 // (const: concatenating two temporaries would instantiate std::operator+(string&&, string&&) out of line, an exported
 // symbol of the library)
 static const std::string num(int x) {
   char b[16];
   snprintf(b, sizeof(b), "%d", x);
   return b;
+}
+
+// The concatenation of `parts` (built by appending, for the reason above)
+static std::string pw_cat(std::initializer_list<std::string> parts) {
+  std::string s;
+  for (const std::string& x : parts) s += x;
+  return s;
 }
 
 // ---- the transcendental ops (TSDE_PW_EXP .. TSDE_PW_SIGMOID_BACKWARD) -----------------------------------------------
@@ -482,56 +488,194 @@ static std::string pw_helper_declarations(const tsde_pointwise& in, const char* 
   return o + "}  // namespace tsde\n\n";
 }
 
-// The translation unit of a program that passed pw_valid_tables and pw_valid_milstein, for dtype `f64`: the kernels
-// of consecutive steps (single, multi), or with `adaptive` the kernel of an adaptive solve's proposal
-// (tsde_pw_milstein_adaptive, a translation unit of its own).
-static std::string pw_milstein_source(const tsde_pointwise& in, bool f64, bool adaptive = false) {
+// ---- the program emitter --------------------------------------------------------------------------------------------
+// The expression of instruction x on sources a and b in dtype f64 / float, as pw_loop's case of its opcode (a
+// transcendental op: the call of its helper).  d is the destination, SEL's condition.
+static const std::string pw_expression(const tsde_pw_instr& x, const std::string& a, const std::string& b,
+                                       const std::string& d, bool f64) {
+  if (pw_transcendental(x.op)) return pw_helper_call(x.op, a, b);
+  const char* f = f64 ? "" : "f";
+  switch (x.op) {
+    case TSDE_PW_MUL: return a + " * " + b;
+    case TSDE_PW_ADD: return a + " + " + b;
+    case TSDE_PW_SUB: return a + " - " + b;
+    case TSDE_PW_DIV: return a + " / " + b;
+    case TSDE_PW_NEG: return "-" + a;
+    case TSDE_PW_SQRT: return pw_cat({"sqrt", f, "(", a, ")"});
+    case TSDE_PW_LT: return a + " < " + b + " ? T(1) : T(0)";
+    case TSDE_PW_LE: return a + " <= " + b + " ? T(1) : T(0)";
+    case TSDE_PW_EQ: return a + " == " + b + " ? T(1) : T(0)";
+    case TSDE_PW_MAXIMUM:  // maximum_kernel_cuda (::max is fmax)
+      return pw_cat({a, " != ", a, " ? ", a, " : ", b, " != ", b, " ? ", b, " : fmax", f, "(", a, ", ", b, ")"});
+    case TSDE_PW_MINIMUM:  // minimum_kernel_cuda (::min is fmin)
+      return pw_cat({a, " != ", a, " ? ", a, " : ", b, " != ", b, " ? ", b, " : fmin", f, "(", a, ", ", b, ")"});
+    case TSDE_PW_ABS: return pw_cat({"fabs", f, "(", a, ")"});
+    default: return d + " != T(0) ? " + a + " : " + b;  // TSDE_PW_SEL: the condition is the destination
+  }
+}
+
+static bool pw_per_channel_kind(int kind) { return kind == TSDE_PW_DM || kind == TSDE_PW_M; }
+
+// Source s names an operand (not y, go or a register)
+static bool pw_operand_source(uint8_t s) {
+  return s >= TSDE_PW_OPERAND(0) && s != TSDE_PW_SRC_Y && s != TSDE_PW_SRC_GO;
+}
+
+// The CHANNEL / ROW operands a unit keeps in its Prog (k<k>[4], loaded once per launch): the first `max` of them.  A
+// part loads the others where it reads them (x<k>[4]).
+static void pw_hoist(const tsde_pointwise& in, int max, bool (&hoisted)[TSDE_PW_MAX_OPERANDS]) {
+  for (int k = 0, n = 0; k < in.n_operands; ++k) {
+    const int kind = in.operand[k].kind;
+    hoisted[k] = (kind == TSDE_PW_CHANNEL || kind == TSDE_PW_ROW) && n++ < max;
+  }
+}
+
+// The value of source s in lane j: y, go, register s, or an operand (a DM or M operand at channel k of the lane's d
+// index i, for m channels)
+static const std::string pw_value(const tsde_pointwise& in, uint8_t s, const bool (&hoisted)[TSDE_PW_MAX_OPERANDS],
+                                  int64_t m = 0) {
+  if (s == TSDE_PW_SRC_Y) return "y[j]";
+  if (s == TSDE_PW_SRC_GO) return "go[j]";
+  if (!pw_operand_source(s)) return pw_cat({"r", num(s), "[j]"});
+  const int k = s - TSDE_PW_OPERAND(0);
+  const std::string n = num(k);
+  switch (in.operand[k].kind) {
+    case TSDE_PW_IMM: return pw_cat({"ops.k[", n, "].imm"});
+    case TSDE_PW_T0: return "t0";
+    case TSDE_PW_SCALAR: return "u" + n;
+    case TSDE_PW_DM: return pw_cat({"ops.k[", n, "].ptr[i * ", num((int)m), " + k]"});
+    case TSDE_PW_M: return pw_cat({"ops.k[", n, "].ptr[k]"});
+    default: return pw_cat({hoisted[k] ? "k" : "x", n, "[j]"});
+  }
+}
+
+// The statement that loads this thread's quad of CHANNEL / ROW operand k into <var>k
+static std::string pw_load_operand(const tsde_pointwise& in, int k, const char* var) {
+  const std::string n = num(k);
+  return pw_cat({"    load_quad(ops.k[", n, "].ptr, c.", in.operand[k].kind == TSDE_PW_ROW ? "base" : "chan",
+                 ", c.vec, c.nvalid, ", var, n, ");\n"});
+}
+
+// A unit's text up to its Prog's members: the `title` comment, the helper declarations, and `struct Prog {` with
+// `members` (the layout's own), each SCALAR operand's value u<k>, the `hoisted` quads k<k>[4], and load(), which
+// fills them after the dependency wait.
+static std::string pw_prog_head(const tsde_pointwise& in, bool f64, const char* title, const std::string& members,
+                                const bool (&hoisted)[TSDE_PW_MAX_OPERANDS]) {
   const char* T = f64 ? "double" : "float";
-  bool hoisted[TSDE_PW_MAX_OPERANDS] = {};
-  for (int k = 0, n = 0; k < in.n_operands; ++k)
-    if (in.operand[k].kind >= TSDE_PW_CHANNEL) hoisted[k] = n++ < kPwJitHoistQuads[f64];
-  auto operand = [&](uint8_t s) { return s >= TSDE_PW_OPERAND(0) && s != TSDE_PW_SRC_Y && s != TSDE_PW_SRC_GO; };
-  // the value of source s in lane j
-  auto src = [&](uint8_t s) -> std::string {
-    if (s == TSDE_PW_SRC_Y) return "y[j]";
-    if (s == TSDE_PW_SRC_GO) return "go[j]";
-    if (!operand(s)) return "r" + num(s) + "[j]";
-    const int k = s - TSDE_PW_OPERAND(0);
-    const std::string n = num(k);
-    switch (in.operand[k].kind) {
-      case TSDE_PW_IMM: return "ops.k[" + n + "].imm";
-      case TSDE_PW_T0: return "t0";
-      case TSDE_PW_SCALAR: return "u" + n;
-      default: return (hoisted[k] ? "k" : "x") + n + "[j]";
-    }
-  };
-  // instruction i, as pw_loop's case of its opcode
-  auto statement = [&](const tsde_pw_instr& x) -> std::string {
-    const std::string a = src(x.a), b = pw_unary(x.op) ? a : src(x.b), d = "r" + num(x.dst) + "[j]";
-    const std::string f = f64 ? "" : "f";
-    std::string e;
-    if (pw_transcendental(x.op)) return "      " + d + " = " + pw_helper_call(x.op, a, b) + ";\n";
-    switch (x.op) {
-      case TSDE_PW_MUL: e = a + " * " + b; break;
-      case TSDE_PW_ADD: e = a + " + " + b; break;
-      case TSDE_PW_SUB: e = a + " - " + b; break;
-      case TSDE_PW_DIV: e = a + " / " + b; break;
-      case TSDE_PW_NEG: e = "-" + a; break;
-      case TSDE_PW_SQRT: e = "sqrt" + f + "(" + a + ")"; break;
-      case TSDE_PW_LT: e = a + " < " + b + " ? T(1) : T(0)"; break;
-      case TSDE_PW_LE: e = a + " <= " + b + " ? T(1) : T(0)"; break;
-      case TSDE_PW_EQ: e = a + " == " + b + " ? T(1) : T(0)"; break;
-      case TSDE_PW_MAXIMUM:  // maximum_kernel_cuda (::max is fmax)
-        e = a + " != " + a + " ? " + a + " : " + b + " != " + b + " ? " + b + " : fmax" + f + "(" + a + ", " + b + ")";
-        break;
-      case TSDE_PW_MINIMUM:  // minimum_kernel_cuda (::min is fmin)
-        e = a + " != " + a + " ? " + a + " : " + b + " != " + b + " ? " + b + " : fmin" + f + "(" + a + ", " + b + ")";
-        break;
-      case TSDE_PW_ABS: e = "fabs" + f + "(" + a + ")"; break;
-      default: e = d + " != T(0) ? " + a + " : " + b; break;  // TSDE_PW_SEL: the condition is the destination
-    }
-    return "      " + d + " = " + e + ";\n";
-  };
+  std::string o = title;
+  o += "#include \"pw_device.cuh\"\n\n";
+  o += pw_helper_declarations(in, T);
+  o += pw_cat({"namespace tsde {\nnamespace {\ntypedef ", T, " T;\n\nstruct Prog {\n", members});
+  for (int k = 0; k < in.n_operands; ++k) {
+    if (in.operand[k].kind == TSDE_PW_SCALAR) o += pw_cat({"  T u", num(k), ";\n"});
+    if (hoisted[k]) o += pw_cat({"  T k", num(k), "[4];\n"});
+  }
+  o += "  __device__ __forceinline__ void load(const PwOperands<T>& ops, const PwQuad& c) {\n";
+  for (int k = 0; k < in.n_operands; ++k) {
+    if (in.operand[k].kind == TSDE_PW_SCALAR) o += pw_cat({"    u", num(k), " = *ops.k[", num(k), "].ptr;\n"});
+    if (hoisted[k]) o += pw_load_operand(in, k, "k");
+  }
+  return o + "  }\n";
+}
+
+// ---- the compiled units ---------------------------------------------------------------------------------------------
+// Each unit's extern "C" kernels, as its source spells them and as pw_loaded looks them up.  A kernel with `cells` has
+// two: <name>_single draws each step from one Brownian cell (TSDE_SRC_COUNTER), <name>_multi sums the cells of a step
+// that spans several (kSrcCounterMulti).
+struct PwKernelText {
+  const char* name;
+  bool cells;
+  const char* params;  // the wrapper's parameter list, as written
+  const char* driver;  // the pw_device.cuh function it calls, with
+  const char* args;    // these arguments
+};
+
+struct PwUnit {
+  bool jit_ctas;           // launch bounds (kThreads, kPwJitCtas[f64]); else (kThreads, 1)
+  PwKernelText kernel[2];  // (a unit of one kernel: the second has no name)
+};
+
+// The units, by index: Milstein, the four general ones by their layout tag, and the Milstein adaptive proposal
+enum { kPwUnitMilstein = 0, kPwUnitAdaptive = TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN + 1 };
+static_assert(TSDE_PW_LAYOUT_GENERAL == 1 && TSDE_PW_LAYOUT_GENERAL_SRA == 2 &&
+                  TSDE_PW_LAYOUT_GENERAL_EULER_HEUN == 3 && TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN == 4,
+              "a general unit's index is its layout tag");
+enum { kPwGeneralEuler = 0, kPwGeneralMidpoint = 1 };  // the kernels of the TSDE_PW_LAYOUT_GENERAL unit
+
+static const PwUnit kPwUnits[] = {
+    {true,
+     {{"tsde_pw_milstein", true,
+       "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwP<tsde::T> p,\n"
+       "    const tsde::NoiseP<tsde::T> nz, const __grid_constant__ tsde::PwSteps<tsde::T> st) {\n",
+       "pw_milstein_steps", "(ops, p, nz, st)"}}},
+    {false,
+     {{"tsde_pw_general_euler", true,
+       "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwP<tsde::T> p,\n"
+       "    const tsde::NoiseP<tsde::T> nz, const __grid_constant__ tsde::PwSteps<tsde::T> st) {\n",
+       "pw_general_euler_steps", "(ops, p, nz, st)"},
+      {"tsde_pw_general_midpoint", true,
+       "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwGeneralMidP<tsde::T> p,\n"
+       "    const tsde::NoiseP<tsde::T> nz) {\n",
+       "pw_general_midpoint", "(ops, p, nz)"}}},
+    {false,
+     {{"tsde_pw_general_sra1", true,
+       "(const __grid_constant__ tsde::PwOperands<tsde::T> ops,\n"
+       "    const __grid_constant__ tsde::PwGeneralSraP<tsde::T> p, const tsde::NoiseP<tsde::T> nz) {\n",
+       "pw_general_sra1", "(ops, p, nz)"}}},
+    {false,
+     {{"tsde_pw_general_euler_heun", true,
+       "(const __grid_constant__ tsde::PwOperands<tsde::T> ops,\n"
+       "    const tsde::PwGeneralMidP<tsde::T> p, const tsde::NoiseP<tsde::T> nz) {\n",
+       "pw_general_euler_heun", "(ops, p, nz)"}}},
+    {false,
+     {{"tsde_pw_general_reversible_heun", true,
+       "(const __grid_constant__ tsde::PwOperands<tsde::T> ops,\n"
+       "    const tsde::PwGeneralRevHeunP<tsde::T> p, const tsde::NoiseP<tsde::T> nz,\n"
+       "    const __grid_constant__ tsde::PwSteps<tsde::T> st) {\n",
+       "pw_general_reversible_heun_steps", "(ops, p, nz, st)"}}},
+    {true,
+     {{"tsde_pw_milstein_adaptive", false,
+       "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwP<tsde::T> p,\n"
+       "    tsde::T* y_next, const __grid_constant__ tsde::PwSubs<tsde::T> st) {\n",
+       "pw_milstein_proposal", "(ops, p, y_next, st)"}}},
+};
+
+static const char* const kPwCellSuffix[2] = {"_single", "_multi"};
+
+// (the general kernels' launch bounds: one resident CTA per SM at least, so that ptxas never spills the increments;
+// pointwise.py's _RESIDENT_CTAS counts on one)
+static_assert(sizeof(PwOperands<double>) + sizeof(PwP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <=
+                  4096,
+              "the compiled Milstein and general Euler kernels' parameters fit the 4 KiB parameter space");
+static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralMidP<double>) + sizeof(NoiseP<double>) <= 4096,
+              "the compiled general midpoint and Euler-Heun kernels' parameters fit the 4 KiB parameter space");
+static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralSraP<double>) + sizeof(NoiseP<double>) <= 4096,
+              "the compiled sra1 kernel's parameters fit the 4 KiB parameter space");
+static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralRevHeunP<double>) + sizeof(NoiseP<double>) +
+                      sizeof(PwSteps<double>) <=
+                  4096,
+              "the compiled general reversible-Heun kernel's parameters fit the 4 KiB parameter space");
+
+// The end of unit `unit`'s source: the close of its Prog and namespaces, then its kernels
+static std::string pw_unit_tail(int unit, bool f64) {
+  const PwUnit& u = kPwUnits[unit];
+  const std::string bounds = pw_cat({"__launch_bounds__(", num(kThreads), ", ", num(u.jit_ctas ? kPwJitCtas[f64] : 1),
+                                     ")"});
+  std::string o = "};\n}  // namespace\n}  // namespace tsde\n";
+  for (const PwKernelText& k : u.kernel)
+    for (int multi = 0; k.name && multi < (k.cells ? 2 : 1); ++multi)
+      o += pw_cat({"\nextern \"C\" __global__ void ", bounds, "\n", k.name, k.cells ? kPwCellSuffix[multi] : "",
+                   k.params, "  tsde::", k.driver, "<tsde::T, ",
+                   k.cells ? (multi ? "tsde::kSrcCounterMulti, " : "TSDE_SRC_COUNTER, ") : "", "tsde::Prog>", k.args,
+                   ";\n}\n"});
+  return o;
+}
+
+// The translation unit of a program that passed pw_valid_tables and pw_valid_milstein, for dtype `f64`: the Milstein
+// unit (the kernels of consecutive steps) or the adaptive one (the kernel of an adaptive solve's proposal).
+static std::string pw_milstein_source(const tsde_pointwise& in, bool f64, int unit = kPwUnitMilstein) {
+  bool hoisted[TSDE_PW_MAX_OPERANDS];
+  pw_hoist(in, kPwJitHoistQuads[f64], hoisted);
   // instructions [i0, i1) and then `results` (name = source); the time and the operands not kept in registers that
   // they read are loaded first
   auto part = [&](int i0, int i1, std::initializer_list<std::pair<const char*, uint8_t>> results) {
@@ -546,61 +690,178 @@ static std::string pw_milstein_source(const tsde_pointwise& in, bool f64, bool a
     bool t0 = false, x[TSDE_PW_MAX_OPERANDS] = {};
     for (int i = 0; i < n; ++i) {
       const uint8_t s = reads[i];
-      if (!operand(s)) continue;
+      if (!pw_operand_source(s)) continue;
       const int k = s - TSDE_PW_OPERAND(0), kind = in.operand[k].kind;
       if (kind == TSDE_PW_T0 && !t0) {
         t0 = true;
         o += "    const T t0 = *s.t0;\n";
       } else if (kind >= TSDE_PW_CHANNEL && !hoisted[k] && !x[k]) {
         x[k] = true;
-        const std::string n = num(k);
-        o += "    T x" + n + "[4];\n    load_quad(ops.k[" + n + "].ptr, c." + (kind == TSDE_PW_ROW ? "base" : "chan") +
-             ", c.vec, c.nvalid, x" + n + ");\n";
+        o += pw_cat({"    T x", num(k), "[4];\n"});
+        o += pw_load_operand(in, k, "x");
       }
     }
     o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
-    for (int i = i0; i < i1; ++i) o += statement(in.instr[i]);
-    for (const auto& r : results) o += std::string("      ") + r.first + "[j] = " + src(r.second) + ";\n";
+    for (int i = i0; i < i1; ++i) {
+      const tsde_pw_instr& ins = in.instr[i];
+      const std::string a = pw_value(in, ins.a, hoisted), b = pw_unary(ins.op) ? a : pw_value(in, ins.b, hoisted);
+      const std::string d = pw_cat({"r", num(ins.dst), "[j]"});
+      o += pw_cat({"      ", d, " = ", pw_expression(ins, a, b, d, f64), ";\n"});
+    }
+    for (const auto& r : results) o += pw_cat({"      ", r.first, "[j] = ", pw_value(in, r.second, hoisted), ";\n"});
     return o + "    }\n";
   };
-  std::string o = "// A Milstein program of torchsde_b200, generated by pw_milstein_source\n"
-                  "#include \"pw_device.cuh\"\n\n";
-  o += pw_helper_declarations(in, T);
-  o += "namespace tsde {\nnamespace {\ntypedef " + std::string(T) + " T;\n\nstruct Prog {\n";
-  for (int r = 0; r < in.n_regs; ++r) o += "  T r" + num(r) + "[4];\n";
-  for (int k = 0; k < in.n_operands; ++k) {
-    const std::string n = num(k);
-    if (in.operand[k].kind == TSDE_PW_SCALAR) o += "  T u" + n + ";\n";
-    if (hoisted[k]) o += "  T k" + n + "[4];\n";
-  }
-  o += "  __device__ __forceinline__ void load(const PwOperands<T>& ops, const PwQuad& c) {\n";
-  for (int k = 0; k < in.n_operands; ++k) {
-    const std::string n = num(k);
-    if (in.operand[k].kind == TSDE_PW_SCALAR) o += "    u" + n + " = *ops.k[" + n + "].ptr;\n";
-    if (hoisted[k])
-      o += "    load_quad(ops.k[" + n + "].ptr, c." + (in.operand[k].kind == TSDE_PW_ROW ? "base" : "chan") +
-           ", c.vec, c.nvalid, k" + n + ");\n";
-  }
-  o += "  }\n  __device__ __forceinline__ void fg(const PwOperands<T>& ops, const PwQuad& c, const PwStep<T>& s,\n"
+  std::string regs;
+  for (int r = 0; r < in.n_regs; ++r) regs += pw_cat({"  T r", num(r), "[4];\n"});
+  std::string o = pw_prog_head(in, f64, "// A Milstein program of torchsde_b200, generated by pw_milstein_source\n",
+                               regs, hoisted);
+  o += "  __device__ __forceinline__ void fg(const PwOperands<T>& ops, const PwQuad& c, const PwStep<T>& s,\n"
        "                                     const T (&y)[4], T (&f)[4], T (&g)[4]) {\n";
   o += part(0, in.n_fg, {{"f", in.f_src}, {"g", in.g_src}});
   o += "  }\n  __device__ __forceinline__ void vjp(const PwOperands<T>& ops, const PwQuad& c, const PwStep<T>& s,\n"
        "                                      const T (&y)[4], const T (&go)[4], T (&gdg)[4]) {\n";
   o += part(in.n_fg, in.n_instr, {{"gdg", in.gdg_src}});
-  o += "  }\n};\n}  // namespace\n}  // namespace tsde\n";
-  const std::string bounds = "__launch_bounds__(" + num(kThreads) + ", " + num(kPwJitCtas[f64]) + ")";
-  if (adaptive)
-    return o + "\nextern \"C\" __global__ void " + bounds +
-           "\ntsde_pw_milstein_adaptive(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwP<tsde::T> p,\n"
-           "    tsde::T* y_next, const __grid_constant__ tsde::PwSubs<tsde::T> st) {\n"
-           "  tsde::pw_milstein_proposal<tsde::T, tsde::Prog>(ops, p, y_next, st);\n}\n";
-  for (const char* v : {"single", "multi"}) {
-    o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_milstein_" + v +
-         "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwP<tsde::T> p,\n"
-         "    const tsde::NoiseP<tsde::T> nz, const __grid_constant__ tsde::PwSteps<tsde::T> st) {\n"
-         "  tsde::pw_milstein_steps<tsde::T, " + (v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti") +
-         ", tsde::Prog>(ops, p, nz, st);\n}\n";
+  o += "  }\n";
+  o += pw_unit_tail(unit, f64);
+  return o;
+}
+
+// ---- the general-noise programs (GENERAL launches) ------------------------------------------------------------------
+// The two-program layout with per-channel values.  A g program runs m times per output, so it is compiled, never
+// interpreted (an interpreted instruction costs about 30 SASS instructions, DESIGN §4): pw_general_source writes it
+// out as a `Prog` for pw_general_euler_steps / pw_general_midpoint, or, by the program's tag, for pw_general_sra1
+// (TSDE_PW_LAYOUT_GENERAL_SRA), pw_general_euler_heun (_EULER_HEUN) or pw_general_reversible_heun_steps
+// (_REVERSIBLE_HEUN) (pw_device.cuh), with the IEEE options and the cache of the Milstein kernels.  A g
+// instruction is per channel when one of its sources is (a DM or M operand, or a per-channel value); the others are
+// per (row, d) element, evaluated once per lane before the channel loop.  The contraction of each lane's m values with
+// the increments is written out for the route the unfused step takes (gen_route), as that kernel sums:
+//   TSDE_GEN_ROWWISE   g * w                                       (the row-wise kernels' single product)
+//   TSDE_GEN_TILE      per channel quad an fma chain from 0; the quad sums as the xor-butterfly adds them, a pairwise
+//                      tree in natural order                       (gen_cta_kernel, gen_tma_kernel)
+//   TSDE_GEN_GENERIC   left to right from 0, a rounded multiply and a rounded add per channel    (gen_kernel)
+// (the sra1 launches never take the row-wise kernels: their m == 1 route is TSDE_GEN_GENERIC, pw_general_program).
+// Register use stays bounded: m <= TSDE_PW_GENERAL_MAX_M increments per thread, and the tree keeps at most
+// log2(m / 4) + 1 partial sums.
+
+// The translation unit of a program that passed pw_general_program, for m channels and contraction `route`: the
+// unit of its layout tag `layout` (Euler and midpoint kernels for TSDE_PW_LAYOUT_GENERAL).
+static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t m, int route, int layout) {
+  const std::string fs = f64 ? "" : "f", M = num((int)m);
+  const int mq = (int)((m + 3) / 4);
+  bool hoisted[TSDE_PW_MAX_OPERANDS];
+  pw_hoist(in, TSDE_PW_MAX_OPERANDS, hoisted);
+  std::string members = pw_cat({"  static constexpr int MQ = ", num(mq), ";\n"});
+  if (layout == TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN) members += pw_cat({"  static constexpr int M = ", M, ";\n"});
+  std::string o = pw_prog_head(
+      in, f64, "// An element-wise general-noise program of torchsde_b200, generated by pw_general_source\n", members,
+      hoisted);
+  // f: instructions [0, n_fg) on registers r<n>[4], as the Milstein kernels run them
+  o += "  __device__ __forceinline__ void f(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
+       "                                    T (&out)[4]) {\n    const T t0 = *tp;\n    (void)t0;\n";
+  for (int r = 0; r < in.n_regs; ++r) o += pw_cat({"    T r", num(r), "[4];\n"});
+  o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
+  for (int i = 0; i < in.n_fg; ++i) {
+    const tsde_pw_instr& x = in.instr[i];
+    const std::string a = pw_value(in, x.a, hoisted, m), b = pw_unary(x.op) ? a : pw_value(in, x.b, hoisted, m);
+    const std::string d = pw_cat({"r", num(x.dst), "[j]"});
+    o += pw_cat({"      ", d, " = ", pw_expression(x, a, b, d, f64), ";\n"});
   }
+  o += pw_cat({"      out[j] = ", pw_value(in, in.f_src, hoisted, m), ";\n    }\n  }\n"});
+  // g: instruction i is n<i>[4] (per element, before the channel loop) or v<i> (per channel, inside G(k)); a register
+  // names the instruction that last wrote it
+  int def[TSDE_PW_MAX_REGS];
+  bool wide[TSDE_PW_MAX_INSTR] = {};
+  for (int r = 0; r < TSDE_PW_MAX_REGS; ++r) def[r] = -1;
+  auto is_wide = [&](uint8_t s) {
+    if (s == TSDE_PW_SRC_Y) return false;
+    if (pw_operand_source(s)) return pw_per_channel_kind(in.operand[s - TSDE_PW_OPERAND(0)].kind);
+    return wide[def[s]];
+  };
+  auto gsrc = [&](uint8_t s) -> std::string {
+    if (s == TSDE_PW_SRC_Y || pw_operand_source(s)) return pw_value(in, s, hoisted, m);
+    return wide[def[s]] ? "v" + num(def[s]) : pw_cat({"n", num(def[s]), "[j]"});
+  };
+  std::string narrow, per_channel;
+  for (int i = in.n_fg; i < in.n_instr; ++i) {
+    const tsde_pw_instr& x = in.instr[i];
+    const bool sel = x.op == TSDE_PW_SEL;
+    wide[i] = is_wide(x.a) || (!pw_unary(x.op) && is_wide(x.b)) || (sel && is_wide(x.dst));
+    const std::string a = gsrc(x.a), b = pw_unary(x.op) ? a : gsrc(x.b), d = sel ? gsrc(x.dst) : "";
+    if (wide[i])
+      per_channel += pw_cat({"        const T v", num(i), " = ", pw_expression(x, a, b, d, f64), ";\n"});
+    else
+      narrow += pw_cat({"      n", num(i), "[j] = ", pw_expression(x, a, b, d, f64), ";\n"});
+    def[x.dst] = i;
+  }
+  // the g program at (*tp, y), up to lane j's channel values G(k)
+  std::string g_head = "    const T t0 = *tp;\n    (void)t0;\n";
+  for (int i = in.n_fg; i < in.n_instr; ++i)
+    if (!wide[i]) g_head += "    T n" + num(i) + "[4];\n";
+  g_head += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
+  g_head += narrow;
+  g_head += "    }\n#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n"
+            "      const int64_t i = c.chan + (j < c.nvalid ? j : 0);  // (the d index of the lane; padding lanes read lane 0's)\n"
+            "      (void)i;\n      auto G = [&](int k) -> T {\n        (void)k;\n";
+  g_head += per_channel;
+  g_head += "        return ";
+  g_head += gsrc(in.g_src);
+  g_head += ";\n      };\n";
+  // lane j's acc: the values val(k) contracted with the weights w[k] in the route's order; pre(k) / post(k) are the
+  // statements before / after channel k's term
+  const std::string fma = "fma" + fs;
+  auto contraction = [&](auto val, auto pre, auto post) {
+    std::string s;
+    if (route == TSDE_GEN_ROWWISE) {
+      s += pw_cat({pre(0), "      const T acc = ", val(0), " * w[0];\n", post(0)});
+    } else if (route == TSDE_GEN_GENERIC) {
+      s += "      T acc = T(0);\n";
+      for (int k = 0; k < m; ++k) s += pw_cat({pre(k), "      acc = acc + ", val(k), " * w[", num(k), "];\n", post(k)});
+    } else {
+      std::string level[TSDE_PW_GENERAL_MAX_M / 4];  // the partial sums of the tree's current level
+      for (int q = 0; q < mq; ++q) {
+        const std::string sq = pw_cat({"s", num(q)});
+        const int k0 = 4 * q;
+        s += pw_cat({pre(k0), "      T ", sq, " = ", fma, "(", val(k0), ", w[", num(k0), "], T(0));\n", post(k0)});
+        for (int j = 1; j < 4; ++j)
+          s += pw_cat({pre(k0 + j), "      ", sq, " = ", fma, "(", val(k0 + j), ", w[", num(k0 + j), "], ", sq, ");\n",
+                       post(k0 + j)});
+        level[q] = sq;
+      }
+      for (int l = 0, n = mq; n > 1; ++l, n /= 2) {
+        for (int p = 0; p < n; p += 2) {
+          const std::string a = pw_cat({"a", num(l), "_", num(p / 2)});
+          s += pw_cat({"      const T ", a, " = ", level[p], " + ", level[p + 1], ";\n"});
+          level[p / 2] = a;
+        }
+      }
+      s += pw_cat({"      const T acc = ", level[0], ";\n"});
+    }
+    s += "      out[j] = acc;\n    }\n  }\n";
+    return s;
+  };
+  auto none = [](int) { return std::string(); };
+  if (layout == TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN) {
+    // the state's g values gs[j][k] stay in registers: z's contraction reads them, y's contracts (gs + g1) and leaves
+    // g1 in their place (pw_general_reversible_heun_steps)
+    o += "  template <typename Op>\n"
+         "  __device__ __forceinline__ void dot(const Op& op, const T (&gs)[4][M], const T (&w)[4 * MQ], T (&out)[4]) {\n"
+         "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
+    o += contraction([&](int k) { return pw_cat({"op.gval(0, {gs[j][", num(k), "]})"}); }, none, none);
+    o += "  template <typename Op>\n"
+         "  __device__ __forceinline__ void gstep(const PwOperands<T>& ops, const PwQuad& c, const T* tp,\n"
+         "                                        const T (&y)[4], const Op& op, const T (&w)[4 * MQ], T (&gs)[4][M],\n"
+         "                                        T (&out)[4]) {\n";
+    o += g_head;
+    o += contraction([&](int k) { return pw_cat({"op.gval(0, {gs[j][", num(k), "], h", num(k), "})"}); },
+                     [&](int k) { return pw_cat({"      const T h", num(k), " = G(", num(k), ");\n"}); },
+                     [&](int k) { return pw_cat({"      gs[j][", num(k), "] = h", num(k), ";\n"}); });
+  } else {
+    o += "  __device__ __forceinline__ void gp(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
+         "                                     const T (&w)[4 * MQ], T (&out)[4]) {\n";
+    o += g_head;
+    o += contraction([&](int k) { return pw_cat({"G(", num(k), ")"}); }, none, none);
+  }
+  o += pw_unit_tail(layout, f64);
   return o;
 }
 
@@ -775,16 +1036,12 @@ static int pw_nvrtc_linked(const std::string& source, std::string& cubin) {
 }
 
 struct PwCompiled {
-  // one Brownian cell per step, several cells merged (kSrcCounterMulti); adaptive: kernel[0]; a general-noise program:
-  // Euler's two, then midpoint's two
-  cudaKernel_t kernel[4];
+  cudaKernel_t kernel[2][2];  // [the unit's kernel][its multi-cell variant] (kPwUnits; a kernel without: [k][0])
 };
 
-// The kernels `names` of `source` (kernel[i] for names[i]; a null name takes the kernel before it), compiled and loaded
-// on first use.  Libraries are context-independent: one entry serves every device.  A program of `prog` with a
-// transcendental op is linked with kPwHelpers.
-static int pw_loaded(const tsde_pointwise& prog, std::string source, std::initializer_list<const char*> names,
-                     PwCompiled& out) {
+// The kernels of unit `unit` of `source`, compiled and loaded on first use.  Libraries are context-independent: one
+// entry serves every device.  A program of `prog` with a transcendental op is linked with kPwHelpers.
+static int pw_loaded(const tsde_pointwise& prog, int unit, std::string source, PwCompiled& out) {
   static std::mutex mu;
   static std::map<std::string, PwCompiled> cache;
   std::lock_guard<std::mutex> lock(mu);
@@ -799,29 +1056,20 @@ static int pw_loaded(const tsde_pointwise& prog, std::string source, std::initia
   if (int e = link ? pw_nvrtc_linked(source, cubin) : pw_nvrtc(source, cubin)) return e;
   cudaLibrary_t lib;
   cudaError_t e = cudaLibraryLoadData(&lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0);
-  int i = 0;
-  for (const char* name : names) {
-    if (e != cudaSuccess) break;
-    if (name)
-      e = cudaLibraryGetKernel(&out.kernel[i], lib, name);
-    else
-      out.kernel[i] = out.kernel[i - 1];
-    ++i;
+  const bool loaded = e == cudaSuccess;
+  for (int i = 0; i < 2; ++i) {
+    const PwKernelText& k = kPwUnits[unit].kernel[i];
+    for (int multi = 0; k.name && multi < (k.cells ? 2 : 1) && e == cudaSuccess; ++multi)
+      e = cudaLibraryGetKernel(&out.kernel[i][multi], lib,
+                               (std::string(k.name) + (k.cells ? kPwCellSuffix[multi] : "")).c_str());
   }
-  if (e != cudaSuccess && i > 0) cudaLibraryUnload(lib);
+  if (e != cudaSuccess && loaded) cudaLibraryUnload(lib);
   if (e != cudaSuccess) {
     cudaGetLastError();
     return (int)e;
   }
   cache.emplace(std::move(source), out);
   return 0;
-}
-
-// The loaded kernels of a Milstein program that passed validation, compiled on first use.
-static int pw_compiled(const tsde_pointwise& prog, bool f64, PwCompiled& out, bool adaptive = false) {
-  std::string source = pw_milstein_source(prog, f64, adaptive);
-  return adaptive ? pw_loaded(prog, std::move(source), {"tsde_pw_milstein_adaptive", nullptr}, out)
-                  : pw_loaded(prog, std::move(source), {"tsde_pw_milstein_single", "tsde_pw_milstein_multi"}, out);
 }
 
 // The Milstein layout, in the order the kernel reads it: go exists from the vjp part on, registers carry over.
@@ -1242,17 +1490,17 @@ static_assert(sizeof(PwProg<double>) + sizeof(PwProposalP<double>) <= 4096,
               "the proposal kernel's parameters fit the 4 KiB parameter space");
 
 // ---- launch ---------------------------------------------------------------------------------------------------------
-// The noise, the decoded program `pg` with the shared-memory slots its launch takes (`extra` past its layout), and the part of the kernel parameters every pointwise step has (y0, y1, the
-// quad mapping, vec) for a program that passes `layout`; TSDE_EINVAL for a launch the kernels cannot serve.
+// What every launch of a step program checks and fills before anything is compiled or launched: counter noise without
+// flags (np), y0, and the part of the kernel parameters every pointwise step has (y0, y1, the quad mapping, vec for
+// y0, y1 and the program's CHANNEL / ROW operands).  y1 is null for a chunk, whose step table holds the destinations
+// (pw_steps).  `prog` has passed its layout's validation.
 template <typename T>
-static int pw_prepare(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
-                      void* y1, bool (*layout)(const tsde_pointwise&), int extra, PwProg<T>& pg, int& slots,
-                      PwP<T>& p, NoiseP<T>& np) {
-  if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !prog || !y0 || !y1) return TSDE_EINVAL;
-  bool vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y1);
-  if (!pw_valid_tables(*prog, &vec) || !layout(*prog)) return TSDE_EINVAL;
+static int pw_fill(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise& prog, const void* y0, void* y1,
+                   PwP<T>& p, NoiseP<T>& np) {
+  if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !y0) return TSDE_EINVAL;
+  bool vec = L->d % 4 == 0 && aligned16(y0) && (!y1 || aligned16(y1));
+  pw_valid_tables(prog, &vec, TSDE_PW_M);
   if (int e = fill_noise<T>(L, nz, false, np)) return e;
-  slots = pw_decode<T>(*prog, extra, pg);
   p = PwP<T>{};
   p.y0 = static_cast<const T*>(y0);
   p.y1 = static_cast<T*>(y1);
@@ -1260,6 +1508,62 @@ static int pw_prepare(const tsde_launch* L, const tsde_noise* nz, const tsde_poi
   p.vec = vec ? 1 : 0;
   return 0;
 }
+
+// The step table of the chunk steps[0, n_steps), after pw_fill: 1 to kPwMaxSteps steps, each with its time, the last
+// with a destination.  A step that merges several Brownian cells (np.n_cells > 1) runs alone, in the kSrcCounterMulti
+// kernel, which reads the first cell and the uniform length from the noise descriptor.  Clears p.vec for a destination
+// that is not 16-byte aligned.
+template <typename T>
+static int pw_steps(const tsde_pw_step* steps, int32_t n_steps, PwP<T>& p, NoiseP<T>& np, PwSteps<T>& st) {
+  if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
+  if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
+  st = PwSteps<T>{};
+  st.n = n_steps;
+  for (int j = 0; j < n_steps; ++j) {
+    const tsde_pw_step& s = steps[j];
+    if (!s.t0) return TSDE_EINVAL;
+    if (s.y1 && !aligned16(s.y1)) p.vec = 0;
+    st.s[j] = PwStep<T>{s.cell_id, static_cast<const T*>(s.t0), static_cast<T*>(s.y1), (T)sqrt(s.h), (T)s.dt};
+  }
+  np.cell_id = steps[0].cell_id;
+  np.h = steps[0].h;
+  return 0;
+}
+
+// The decoded program `pg` of an interpreted launch, with the shared-memory slots it takes (`extra` past its layout),
+// and pw_fill's parameters, for a program that passes `layout`; TSDE_EINVAL for a launch the kernels cannot serve.
+template <typename T>
+static int pw_prepare(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
+                      void* y1, bool (*layout)(const tsde_pointwise&), int extra, PwProg<T>& pg, int& slots,
+                      PwP<T>& p, NoiseP<T>& np) {
+  bool vec = true;
+  if (!prog || !pw_valid_tables(*prog, &vec) || !layout(*prog)) return TSDE_EINVAL;
+  if (int e = pw_fill<T>(L, nz, *prog, y0, y1, p, np)) return e;
+  slots = pw_decode<T>(*prog, extra, pg);
+  return 0;
+}
+
+// f(std::integral_constant<int, M>{}) for the M of METHODS that `method` is (the caller has checked that one is)
+template <int... METHODS, typename F>
+static int pw_method(int method, F&& f) {
+  int e = TSDE_EINVAL;
+  (void)((method == METHODS && ((e = f(std::integral_constant<int, METHODS>{})), true)) || ...);
+  return e;
+}
+
+// f(std::true_type{}) for a program with comparison and selection ops (PwProg::ext), else f(std::false_type{})
+template <typename F>
+static int pw_ext(bool ext, F&& f) {
+  return ext ? f(std::true_type{}) : f(std::false_type{});
+}
+
+// The interpreted kernels of a program with comparison and selection ops (EXT) or without, for Brownian source SRC
+template <typename T, int SRC, bool EXT>
+constexpr auto pw_srk_of = EXT ? pw_srk_ext_kernel<T, SRC> : pw_srk_kernel<T, SRC>;
+template <typename T, int SRC, int METHOD, bool EXT>
+constexpr auto pw_pc_of = EXT ? pw_pc_ext_kernel<T, SRC, METHOD> : pw_pc_kernel<T, SRC, METHOD>;
+template <typename T, int SRC, int METHOD, bool EXT>
+constexpr auto pw_chunk_of = EXT ? pw_chunk_ext_kernel<T, SRC, METHOD> : pw_chunk_kernel<T, SRC, METHOD>;
 
 // One thread per quad, `slots` shared-memory registers per thread; `single` draws from one Brownian cell, `multi` sums
 // the cells of a step that spans several.  `x` are the kernel's parameters past the noise (a chunk's step table).
@@ -1278,49 +1582,67 @@ static int pw_launch(const tsde_launch* L, const PwProg<T>& prog,
   return e;
 }
 
+// The PwOperands parameter of a compiled kernel: the IMM values and device pointers of `prog`'s operands
+template <typename T>
+static PwOperands<T> pw_operands(const tsde_pointwise* prog) {
+  PwOperands<T> ops{};
+  for (int k = 0; k < prog->n_operands; ++k)
+    ops.k[k] = PwOperand<T>{static_cast<const T*>(prog->operand[k].ptr), (T)prog->operand[k].imm};
+  return ops;
+}
+
+// One launch of kernel `entry` of unit `unit` of `source` (compiled here if this is the first launch of its
+// structure), its multi-cell variant for a step of several Brownian cells, with parameters (the operands of `prog`,
+// x...), one thread per quad of `nquads`, counted under `family`
+template <typename T, typename... X>
+static int pw_launch_compiled(const tsde_launch* L, const tsde_pointwise* prog, int unit, std::string source,
+                              int entry, bool multi, int64_t nquads, int family, X&... x) {
+  PwCompiled kc;
+  if (int e = pw_loaded(*prog, unit, std::move(source), kc)) return e;
+  PwOperands<T> ops = pw_operands<T>(prog);
+  void* args[] = {&ops, &x...};
+  const int e = launch_kernel_handle(kc.kernel[entry][multi], (nquads + kThreads - 1) / kThreads, kThreads,
+                                     reinterpret_cast<cudaStream_t>(L->stream), args);
+  if (e == 0) g_launches[family].fetch_add(1, std::memory_order_relaxed);
+  return e;
+}
+
+// tsde_pointwise_source's result: `src` copied into the caller's buffer (at most size - 1 bytes and a NUL), and its
+// length
+static int64_t pw_copy_source(const std::string& src, char* buf, int64_t size) {
+  if (buf && size > 0) {
+    const size_t n = std::min(src.size(), (size_t)size - 1);
+    memcpy(buf, src.data(), n);
+    buf[n] = 0;
+  }
+  return (int64_t)src.size();
+}
+
 }  // namespace tsde
 
 using namespace tsde;
 
+// A Milstein program the launches `L` may run (tsde_solve_milstein_pointwise's checks of L and prog)
+static bool pw_milstein_program(const tsde_launch* L, const tsde_pointwise* prog) {
+  bool vec = true;
+  return L->noise_type == TSDE_NOISE_DIAGONAL && L->m == L->d && prog && pw_valid_tables(*prog, &vec) &&
+         pw_valid_milstein(*prog);
+}
+
 // The chunk `steps[0, n_steps)` from y0 (both entry points): one launch of the program's compiled kernel (compiled
-// here if this is the first launch of its structure).  A step that merges several Brownian cells (nz->n_cells > 1)
-// runs alone, in the kSrcCounterMulti kernel.
+// here if this is the first launch of its structure).
 template <typename T>
 static int pw_milstein_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
                              const tsde_pw_step* steps, int32_t n_steps, int32_t ito) {
-  if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
-  if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !prog || !y0) return TSDE_EINVAL;
-  bool vec = L->d % 4 == 0 && aligned16(y0);
-  if (!pw_valid_tables(*prog, &vec) || !pw_valid_milstein(*prog)) return TSDE_EINVAL;
+  PwP<T> p;
   NoiseP<T> np;
-  if (int e = fill_noise<T>(L, nz, false, np)) return e;
-  if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
-  PwSteps<T> st{};
-  st.n = n_steps;
-  for (int j = 0; j < n_steps; ++j) {
-    const tsde_pw_step& s = steps[j];
-    if (!s.t0) return TSDE_EINVAL;
-    if (s.y1 && !aligned16(s.y1)) vec = false;
-    st.s[j] = PwStep<T>{s.cell_id, static_cast<const T*>(s.t0), static_cast<T*>(s.y1), (T)sqrt(s.h), (T)s.dt};
-  }
-  PwCompiled kc;
-  if (int e = pw_compiled(*prog, sizeof(T) == 8, kc)) return e;
-  PwOperands<T> ops{};
-  for (int k = 0; k < prog->n_operands; ++k)
-    ops.k[k] = PwOperand<T>{static_cast<const T*>(prog->operand[k].ptr), (T)prog->operand[k].imm};
-  PwP<T> p{};
-  p.y0 = static_cast<const T*>(y0);
-  fill_quad_map(L->rows, L->d, p);
-  p.vec = vec ? 1 : 0;
+  PwSteps<T> st;
+  if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
+  if (int e = pw_fill<T>(L, nz, *prog, y0, nullptr, p, np)) return e;
+  if (int e = pw_steps<T>(steps, n_steps, p, np, st)) return e;
   p.ito = ito;
-  // (the multi-cell merge reads the first cell and the uniform length from the noise descriptor)
-  np.cell_id = steps[0].cell_id;
-  np.h = steps[0].h;
-  void* args[] = {&ops, &p, &np, &st};
-  const int e = launch_kernel_handle(kc.kernel[np.n_cells > 1], (p.nquads + kThreads - 1) / kThreads, kThreads,
-                                     reinterpret_cast<cudaStream_t>(L->stream), args);
-  if (e == 0) g_launches[TSDE_KERNEL_PW_MILSTEIN].fetch_add(1, std::memory_order_relaxed);
-  return e;
+  return pw_launch_compiled<T>(L, prog, kPwUnitMilstein, pw_milstein_source(*prog, sizeof(T) == 8), 0,
+                               np.n_cells > 1, p.nquads, TSDE_KERNEL_PW_MILSTEIN, p, np, st);
 }
 
 // The chunk `steps[0, n_steps)` of Euler or reversible Heun from y0 (and, for reversible Heun, from the solver state
@@ -1329,15 +1651,14 @@ static int pw_milstein_chunk(const tsde_launch* L, const tsde_noise* nz, const t
 template <typename T, int METHOD>
 static int pw_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
                     const tsde_pw_step* steps, int32_t n_steps, const void* const (&in)[3], void* const (&out)[3]) {
-  if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
   PwProg<T> pg;
   int slots;
   PwChunkP<T> p{};
   NoiseP<T> np;
-  if (int e = pw_prepare<T>(L, nz, prog, y0, steps[n_steps - 1].y1, pw_valid_two<TSDE_PW_MAX_REGS>, 0, pg,
-                            slots, p.base, np))
+  PwSteps<T> st;
+  if (int e = pw_prepare<T>(L, nz, prog, y0, nullptr, pw_valid_two<TSDE_PW_MAX_REGS>, 0, pg, slots, p.base, np))
     return e;
-  if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
+  if (int e = pw_steps<T>(steps, n_steps, p.base, np, st)) return e;
   if constexpr (METHOD == kPwReversibleHeun) {
     for (int i = 0; i < 3; ++i) {
       if (!in[i] || !out[i]) return TSDE_EINVAL;
@@ -1350,47 +1671,164 @@ static int pw_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_point
     p.f1 = static_cast<T*>(out[1]);
     p.g1 = static_cast<T*>(out[2]);
   }
-  PwSteps<T> st{};
-  st.n = n_steps;
-  for (int j = 0; j < n_steps; ++j) {
-    const tsde_pw_step& s = steps[j];
-    if (!s.t0) return TSDE_EINVAL;
-    if (s.y1 && !aligned16(s.y1)) p.base.vec = 0;
-    st.s[j] = PwStep<T>{s.cell_id, static_cast<const T*>(s.t0), static_cast<T*>(s.y1), (T)sqrt(s.h), (T)s.dt};
-  }
-  np.cell_id = steps[0].cell_id;
-  np.h = steps[0].h;
-  if (pg.ext)
-    return pw_launch<T>(L, pg, pw_chunk_ext_kernel<T, TSDE_SRC_COUNTER, METHOD>,
-                        pw_chunk_ext_kernel<T, kSrcCounterMulti, METHOD>, p, np, p.base.nquads, slots,
+  return pw_ext(pg.ext, [&](auto ext) {
+    return pw_launch<T>(L, pg, pw_chunk_of<T, TSDE_SRC_COUNTER, METHOD, decltype(ext)::value>,
+                        pw_chunk_of<T, kSrcCounterMulti, METHOD, decltype(ext)::value>, p, np, p.base.nquads, slots,
                         TSDE_KERNEL_PW_CHUNK, st);
-  return pw_launch<T>(L, pg, pw_chunk_kernel<T, TSDE_SRC_COUNTER, METHOD>, pw_chunk_kernel<T, kSrcCounterMulti, METHOD>,
-                      p, np, p.base.nquads, slots, TSDE_KERNEL_PW_CHUNK, st);
+  });
 }
 
-// GENERAL launches of tsde_solve_euler_pointwise, tsde_solve_reversible_heun_pointwise,
-// tsde_step_predictor_corrector_pointwise, tsde_step_srk_diag_pointwise, tsde_pointwise_compile and
-// tsde_pointwise_source (general / additive noise; defined with the general-noise code generator below)
+// ---- general / additive noise (GENERAL launches) -------------------------------------------------------------------
+// The general layout (tagged TSDE_PW_LAYOUT_GENERAL): the two-program layout with DM / M operands read by g only.
+static bool pw_valid_general(const tsde_pointwise& pg) {
+  if (!pw_valid_two<TSDE_PW_MAX_REGS, true>(pg)) return false;
+  auto per_channel = [&](uint8_t s) {
+    return pw_operand_source(s) && pw_per_channel_kind(pg.operand[s - TSDE_PW_OPERAND(0)].kind);
+  };
+  for (int i = 0; i < pg.n_fg; ++i)
+    if (per_channel(pg.instr[i].a) || (!pw_unary(pg.instr[i].op) && per_channel(pg.instr[i].b))) return false;
+  return !per_channel(pg.f_src);
+}
+
+// A launch and program of layout tag `layout` the general kernels serve; `route` is the contraction order (gen_route)
+// for dtype size `s`.
+static bool pw_general_program(const tsde_launch* L, const tsde_pointwise* prog, int64_t s, int& route,
+                               int layout = TSDE_PW_LAYOUT_GENERAL) {
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_GENERAL || L->m > TSDE_PW_GENERAL_MAX_M || !prog ||
+      prog->reserved != layout)
+    return false;
+  bool vec = true;
+  if (!pw_valid_tables(*prog, &vec, TSDE_PW_M) || !pw_valid_general(*prog)) return false;
+  // the unfused step's g is a new contiguous tensor (aligned), or the user's (d, m) block itself when g is a DM operand;
+  // the reversible-Heun pair densifies every g it reads (its solver state)
+  bool quads = true;
+  const uint8_t g = prog->g_src;
+  if (layout != TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN && g >= TSDE_PW_OPERAND(0) && g != TSDE_PW_SRC_Y &&
+      g != TSDE_PW_SRC_GO && prog->operand[g - TSDE_PW_OPERAND(0)].kind == TSDE_PW_DM)
+    quads = aligned16(prog->operand[g - TSDE_PW_OPERAND(0)].ptr);
+  if (layout == TSDE_PW_LAYOUT_GENERAL_SRA) {
+    // the sra1 launches call launch_gen directly, which stages U too, and take gen_kernel where cabi.cu would take the
+    // row-wise kernels (m == 1: the sum 0 + g * w, which turns a -0 product into +0)
+    route = gen_route(L->m, quads, 2 * L->m * s);
+    if (route == TSDE_GEN_ROWWISE) route = TSDE_GEN_GENERIC;
+  } else {
+    route = gen_route(L->m, quads, L->m * s);
+  }
+  return route != TSDE_GEN_WIDE;
+}
+
+// pw_launch_compiled of kernel `entry` of a general program that passed pw_general_program with contraction `route`
+// and tag `layout`
+template <typename T, typename... X>
+static int pw_general_launch(const tsde_launch* L, const tsde_pointwise* prog, int route, int layout, int entry,
+                             const NoiseP<T>& np, int64_t nquads, X&... x) {
+  return pw_launch_compiled<T>(L, prog, layout, pw_general_source(*prog, sizeof(T) == 8, L->m, route, layout), entry,
+                               np.n_cells > 1, nquads, TSDE_KERNEL_PW_GENERAL, x...);
+}
+
+// tsde_solve_euler_pointwise for a GENERAL launch: the chunk `steps[0, n_steps)` from y0 as one launch of the
+// program's compiled Euler kernel, under the rules of pw_milstein_chunk.
 template <typename T>
 static int pw_general_euler(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
-                            const tsde_pw_step* steps, int32_t n_steps);
+                            const tsde_pw_step* steps, int32_t n_steps) {
+  int route;
+  PwP<T> p;
+  NoiseP<T> np;
+  PwSteps<T> st;
+  if (!pw_general_program(L, prog, sizeof(T), route)) return TSDE_EINVAL;
+  if (int e = pw_fill<T>(L, nz, *prog, y0, nullptr, p, np)) return e;
+  if (int e = pw_steps<T>(steps, n_steps, p, np, st)) return e;
+  return pw_general_launch<T>(L, prog, route, TSDE_PW_LAYOUT_GENERAL, kPwGeneralEuler, np, p.nquads, p, np, st);
+}
+
+// tsde_step_predictor_corrector_pointwise for a GENERAL launch: one midpoint step as one launch of the program's
+// compiled midpoint kernel, or one Euler-Heun step of an EULER_HEUN-tagged program.
+template <typename T>
+static int pw_general_pc_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
+                              const void* y0, const void* t0, const void* t_p, int32_t method, double dt,
+                              double half_dt, void* y1) {
+  int route;
+  const bool euler_heun = method == TSDE_PC_EULER_HEUN;
+  const int layout = euler_heun ? TSDE_PW_LAYOUT_GENERAL_EULER_HEUN : TSDE_PW_LAYOUT_GENERAL;
+  PwGeneralMidP<T> p{};
+  NoiseP<T> np;
+  if ((method != TSDE_PC_MIDPOINT && !euler_heun) || !t0 || !t_p || !y1 ||
+      !pw_general_program(L, prog, sizeof(T), route, layout))
+    return TSDE_EINVAL;
+  if (int e = pw_fill<T>(L, nz, *prog, y0, y1, p.base, np)) return e;
+  p.base.t0 = static_cast<const T*>(t0);
+  p.base.dt = (T)dt;
+  p.t_p = static_cast<const T*>(t_p);
+  p.half_dt = (T)half_dt;
+  // (the Euler-Heun unit's one kernel, or the general unit's midpoint kernel)
+  return pw_general_launch<T>(L, prog, route, layout, euler_heun ? 0 : kPwGeneralMidpoint, np, p.base.nquads, p, np);
+}
+
+// tsde_solve_reversible_heun_pointwise for a GENERAL launch: the chunk `steps[0, n_steps)` from y0 and the solver state
+// in[] = z0, f0, g0 (g of shape (rows, d, m)), left in out[] = z1, f1, g1, as one launch of the REVERSIBLE_HEUN-tagged
+// program's compiled kernel, under the rules of pw_general_euler.
 template <typename T>
 static int pw_general_reversible_heun(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
                                       const void* y0, const void* const (&in)[3], const tsde_pw_step* steps,
-                                      int32_t n_steps, void* const (&out)[3]);
-template <typename T>
-static int pw_general_pc_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
-                                    const void* y0, const void* t0, const void* t_p, int32_t method, double dt,
-                                    double half_dt, void* y1);
-template <typename T>
-static int pw_general_compiled(const tsde_launch* L, const tsde_pointwise* prog, PwCompiled& kc);
+                                      int32_t n_steps, void* const (&out)[3]) {
+  int route;
+  PwGeneralRevHeunP<T> p{};
+  NoiseP<T> np;
+  PwSteps<T> st;
+  if (!pw_general_program(L, prog, sizeof(T), route, TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN)) return TSDE_EINVAL;
+  for (int i = 0; i < 3; ++i)
+    if (!in[i] || !out[i]) return TSDE_EINVAL;
+  if (int e = pw_fill<T>(L, nz, *prog, y0, nullptr, p.base, np)) return e;
+  if (int e = pw_steps<T>(steps, n_steps, p.base, np, st)) return e;
+  for (int i = 0; i < 2; ++i)  // z, f
+    if (!aligned16(in[i]) || !aligned16(out[i])) p.base.vec = 0;
+  p.z0 = static_cast<const T*>(in[0]);
+  p.f0 = static_cast<const T*>(in[1]);
+  p.g0 = static_cast<const T*>(in[2]);
+  p.z1 = static_cast<T*>(out[0]);
+  p.f1 = static_cast<T*>(out[1]);
+  p.g1 = static_cast<T*>(out[2]);
+  p.gvec = L->m % 4 == 0 && aligned16(in[2]) && aligned16(out[2]) ? 1 : 0;
+  return pw_general_launch<T>(L, prog, route, TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN, 0, np, p.base.nquads, p, np,
+                              st);
+}
+
+// tsde_step_srk_diag_pointwise for a GENERAL launch: one sra1 step as one launch of the SRA-tagged program's
+// compiled kernel.
 template <typename T>
 static int pw_general_sra1_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
                                 const void* y0, const void* t_1, const void* t_34, const void* t_00, double dt,
-                                double rdt, void* y1);
-template <typename T>
-static int64_t pw_general_source_of(const tsde_launch* L, const tsde_pointwise* prog, char* buf, int64_t size);
+                                double rdt, void* y1) {
+  int route;
+  PwGeneralSraP<T> p{};
+  NoiseP<T> np;
+  if (!t_1 || !t_34 || !t_00 || !y1 || !pw_general_program(L, prog, sizeof(T), route, TSDE_PW_LAYOUT_GENERAL_SRA))
+    return TSDE_EINVAL;
+  if (int e = pw_fill<T>(L, nz, *prog, y0, y1, p.base, np)) return e;
+  p.base.t0 = static_cast<const T*>(t_00);
+  p.base.dt = (T)dt;
+  p.t_1 = static_cast<const T*>(t_1);
+  p.t_34 = static_cast<const T*>(t_34);
+  p.stage = GSraStageOp<T>{(T)dt, (T)rdt};
+  p.final_op = GSraFinalOp<T>{(T)dt, (T)rdt, (T)(1.0 / 3), (T)(2.0 / 3)};
+  return pw_general_launch<T>(L, prog, route, TSDE_PW_LAYOUT_GENERAL_SRA, 0, np, p.base.nquads, p, np);
+}
 
+// The unit (its layout tag) and source a GENERAL launch of tsde_pointwise_compile / tsde_pointwise_source serves
+// `prog` with: that of its SRA, EULER_HEUN or REVERSIBLE_HEUN tag, else the Euler / midpoint unit (which refuses every
+// other tag); false if the general kernels cannot serve it.
+template <typename T>
+static bool pw_general_unit(const tsde_launch* L, const tsde_pointwise* prog, int& layout, std::string& source) {
+  int route;
+  const int tag = prog ? prog->reserved : 0;
+  layout = tag >= TSDE_PW_LAYOUT_GENERAL_SRA && tag <= TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN ? tag
+                                                                                              : TSDE_PW_LAYOUT_GENERAL;
+  if (!pw_general_program(L, prog, sizeof(T), route, layout)) return false;
+  source = pw_general_source(*prog, sizeof(T) == 8, L->m, route, layout);
+  return true;
+}
+
+// ---- the entry points -----------------------------------------------------------------------------------------------
 TSDE_EXPORT int tsde_solve_euler_pointwise(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
                                            const void* y0, const tsde_pw_step* steps, int32_t n_steps) {
   if (valid_launch(L) && L->noise_type == TSDE_NOISE_GENERAL)
@@ -1448,7 +1886,7 @@ TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_no
   if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
   return dispatch(L, [&](auto t) -> int {
     using T = decltype(t);
-    if (!t_0 || !t_1 || !t_q || !t_h) return TSDE_EINVAL;
+    if (!t_0 || !t_1 || !t_q || !t_h || !y1) return TSDE_EINVAL;
     PwProg<T> pg;
     int slots;
     PwSrkP<T> p;
@@ -1463,11 +1901,11 @@ TSDE_EXPORT int tsde_step_srk_diag_pointwise(const tsde_launch* L, const tsde_no
     p.s2 = SrkDiagStage2Op<T>{(T)dt, (T)rdt, (T)sqrt_dt};
     p.s3 = SrkDiagStage3Op<T>{(T)dt, (T)sqrt_dt};
     p.fin = make_srk_final<T>(dt, rdt, sqrt_dt, three_dt);
-    if (pg.ext)
-      return pw_launch<T>(L, pg, pw_srk_ext_kernel<T, TSDE_SRC_COUNTER>, pw_srk_ext_kernel<T, kSrcCounterMulti>, p, np,
-                          p.base.nquads, slots, TSDE_KERNEL_PW_SRK);
-    return pw_launch<T>(L, pg, pw_srk_kernel<T, TSDE_SRC_COUNTER>, pw_srk_kernel<T, kSrcCounterMulti>, p, np,
-                        p.base.nquads, slots, TSDE_KERNEL_PW_SRK);
+    return pw_ext(pg.ext, [&](auto ext) {
+      return pw_launch<T>(L, pg, pw_srk_of<T, TSDE_SRC_COUNTER, decltype(ext)::value>,
+                          pw_srk_of<T, kSrcCounterMulti, decltype(ext)::value>, p, np, p.base.nquads, slots,
+                          TSDE_KERNEL_PW_SRK);
+    });
   });
 }
 
@@ -1482,7 +1920,7 @@ TSDE_EXPORT int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, co
   if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
   return dispatch(L, [&](auto t) -> int {
     using T = decltype(t);
-    if (!t0 || !t_p || method < TSDE_PC_HEUN || method > TSDE_PC_EULER_HEUN) return TSDE_EINVAL;
+    if (!t0 || !t_p || !y1 || method < TSDE_PC_HEUN || method > TSDE_PC_EULER_HEUN) return TSDE_EINVAL;
     PwProg<T> pg;
     int slots;
     PwPcP<T> p;
@@ -1493,62 +1931,41 @@ TSDE_EXPORT int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, co
     p.base.dt = (T)dt;
     p.t_p = static_cast<const T*>(t_p);
     p.half_dt = (T)half_dt;
-    auto go = [&](auto single, auto multi) {
-      return pw_launch<T>(L, pg, single, multi, p, np, p.base.nquads, slots, TSDE_KERNEL_PW_PC);
-    };
-    if (pg.ext) {
-      switch (method) {
-        case TSDE_PC_HEUN:
-          return go(pw_pc_ext_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_HEUN>,
-                    pw_pc_ext_kernel<T, kSrcCounterMulti, TSDE_PC_HEUN>);
-        case TSDE_PC_MIDPOINT:
-          return go(pw_pc_ext_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_MIDPOINT>,
-                    pw_pc_ext_kernel<T, kSrcCounterMulti, TSDE_PC_MIDPOINT>);
-        default:
-          return go(pw_pc_ext_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_EULER_HEUN>,
-                    pw_pc_ext_kernel<T, kSrcCounterMulti, TSDE_PC_EULER_HEUN>);
-      }
-    }
-    switch (method) {
-      case TSDE_PC_HEUN:
-        return go(pw_pc_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_HEUN>, pw_pc_kernel<T, kSrcCounterMulti, TSDE_PC_HEUN>);
-      case TSDE_PC_MIDPOINT:
-        return go(pw_pc_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_MIDPOINT>,
-                  pw_pc_kernel<T, kSrcCounterMulti, TSDE_PC_MIDPOINT>);
-      default:
-        return go(pw_pc_kernel<T, TSDE_SRC_COUNTER, TSDE_PC_EULER_HEUN>,
-                  pw_pc_kernel<T, kSrcCounterMulti, TSDE_PC_EULER_HEUN>);
-    }
+    return pw_method<TSDE_PC_HEUN, TSDE_PC_MIDPOINT, TSDE_PC_EULER_HEUN>(method, [&](auto m) {
+      return pw_ext(pg.ext, [&](auto ext) {
+        constexpr int M = decltype(m)::value;
+        constexpr bool X = decltype(ext)::value;
+        return pw_launch<T>(L, pg, pw_pc_of<T, TSDE_SRC_COUNTER, M, X>, pw_pc_of<T, kSrcCounterMulti, M, X>, p, np,
+                            p.base.nquads, slots, TSDE_KERNEL_PW_PC);
+      });
+    });
   });
-}
-
-// A Milstein program the launches `L` may run (tsde_solve_milstein_pointwise's checks of L and prog)
-static bool pw_milstein_program(const tsde_launch* L, const tsde_pointwise* prog) {
-  bool vec = true;
-  return L->noise_type == TSDE_NOISE_DIAGONAL && L->m == L->d && prog && pw_valid_tables(*prog, &vec) &&
-         pw_valid_milstein(*prog);
 }
 
 TSDE_EXPORT int tsde_pointwise_compile(const tsde_launch* L, const tsde_pointwise* prog) {
   return dispatch(L, [&](auto t) -> int {
     PwCompiled kc;
-    if (L->noise_type == TSDE_NOISE_GENERAL) return pw_general_compiled<decltype(t)>(L, prog, kc);
+    if (L->noise_type == TSDE_NOISE_GENERAL) {
+      int layout;
+      std::string source;
+      if (!pw_general_unit<decltype(t)>(L, prog, layout, source)) return TSDE_EINVAL;
+      return pw_loaded(*prog, layout, std::move(source), kc);
+    }
     if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
-    return pw_compiled(*prog, sizeof(t) == 8, kc);
+    return pw_loaded(*prog, kPwUnitMilstein, pw_milstein_source(*prog, sizeof(t) == 8), kc);
   });
 }
 
 TSDE_EXPORT int64_t tsde_pointwise_source(const tsde_launch* L, const tsde_pointwise* prog, char* buf, int64_t size) {
   return dispatch(L, [&](auto t) -> int64_t {
-    if (L->noise_type == TSDE_NOISE_GENERAL) return pw_general_source_of<decltype(t)>(L, prog, buf, size);
-    if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
-    const std::string src = pw_milstein_source(*prog, sizeof(t) == 8);
-    if (buf && size > 0) {
-      const size_t n = std::min(src.size(), (size_t)size - 1);
-      memcpy(buf, src.data(), n);
-      buf[n] = 0;
+    if (L->noise_type == TSDE_NOISE_GENERAL) {
+      int layout;
+      std::string source;
+      if (!pw_general_unit<decltype(t)>(L, prog, layout, source)) return TSDE_EINVAL;
+      return pw_copy_source(source, buf, size);
     }
-    return (int64_t)src.size();
+    if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
+    return pw_copy_source(pw_milstein_source(*prog, sizeof(t) == 8), buf, size);
   });
 }
 
@@ -1596,18 +2013,10 @@ static int pw_proposal_launch(const tsde_launch* L, const tsde_pointwise* prog, 
   fill_quad_map(L->rows, L->d, p.base);
   p.base.vec = vec ? 1 : 0;
   p.y_next = static_cast<T*>(y_next);
-  const int64_t grid = (p.base.nquads + kThreads - 1) / kThreads;
   if (method == TSDE_PROPOSAL_MILSTEIN_ITO || method == TSDE_PROPOSAL_MILSTEIN_STRATONOVICH) {
-    PwCompiled kc;
-    if (int e = pw_compiled(*prog, sizeof(T) == 8, kc, true)) return e;
-    PwOperands<T> ops{};
-    for (int k = 0; k < prog->n_operands; ++k)
-      ops.k[k] = PwOperand<T>{static_cast<const T*>(prog->operand[k].ptr), (T)prog->operand[k].imm};
     p.base.ito = method == TSDE_PROPOSAL_MILSTEIN_ITO ? 1 : 0;
-    void* args[] = {&ops, &p.base, &p.y_next, &p.st};
-    const int e = launch_kernel_handle(kc.kernel[0], grid, kThreads, reinterpret_cast<cudaStream_t>(L->stream), args);
-    if (e == 0) g_launches[TSDE_KERNEL_PW_ADAPTIVE].fetch_add(1, std::memory_order_relaxed);
-    return e;
+    return pw_launch_compiled<T>(L, prog, kPwUnitAdaptive, pw_milstein_source(*prog, sizeof(T) == 8, kPwUnitAdaptive),
+                                 0, false, p.base.nquads, TSDE_KERNEL_PW_ADAPTIVE, p.base, p.y_next, p.st);
   }
   if (method == TSDE_PROPOSAL_SRK) {
     for (int k = 0; k < 3; ++k) {
@@ -1620,31 +2029,18 @@ static int pw_proposal_launch(const tsde_launch* L, const tsde_pointwise* prog, 
   }
   PwProg<T> pg;
   const int slots = pw_decode<T>(*prog, method == TSDE_PROPOSAL_SRK && PwSrkStash<T>::kShared ? kPwSrkStash : 0, pg);
-  void (*kernel)(PwProg<T>, PwProposalP<T>) = nullptr;
-  auto pick = [&](auto plain, auto ext) { kernel = pg.ext ? ext : plain; };
-  switch (method) {
-    case TSDE_PROPOSAL_EULER:
-      pick(pw_proposal_kernel<T, TSDE_PROPOSAL_EULER, false>, pw_proposal_kernel<T, TSDE_PROPOSAL_EULER, true>);
-      break;
-    case TSDE_PROPOSAL_SRK:
-      pick(pw_proposal_kernel<T, TSDE_PROPOSAL_SRK, false>, pw_proposal_kernel<T, TSDE_PROPOSAL_SRK, true>);
-      break;
-    case TSDE_PROPOSAL_HEUN:
-      pick(pw_proposal_kernel<T, TSDE_PROPOSAL_HEUN, false>, pw_proposal_kernel<T, TSDE_PROPOSAL_HEUN, true>);
-      break;
-    case TSDE_PROPOSAL_MIDPOINT:
-      pick(pw_proposal_kernel<T, TSDE_PROPOSAL_MIDPOINT, false>, pw_proposal_kernel<T, TSDE_PROPOSAL_MIDPOINT, true>);
-      break;
-    default:
-      pick(pw_proposal_kernel<T, TSDE_PROPOSAL_EULER_HEUN, false>,
-           pw_proposal_kernel<T, TSDE_PROPOSAL_EULER_HEUN, true>);
-      break;
-  }
   const size_t smem = (size_t)slots * kThreads * 4 * sizeof(T);
-  if (resident_ctas(reinterpret_cast<const void*>(kernel), kThreads, smem) < 1) return TSDE_EINVAL;
-  const int e = launch_kernel(kernel, grid, kThreads, smem, reinterpret_cast<cudaStream_t>(L->stream), true, pg, p);
-  if (e == 0) g_launches[TSDE_KERNEL_PW_ADAPTIVE].fetch_add(1, std::memory_order_relaxed);
-  return e;
+  return pw_method<TSDE_PROPOSAL_EULER, TSDE_PROPOSAL_SRK, TSDE_PROPOSAL_HEUN, TSDE_PROPOSAL_MIDPOINT,
+                   TSDE_PROPOSAL_EULER_HEUN>(method, [&](auto m) {
+    return pw_ext(pg.ext, [&](auto ext) {
+      auto kernel = pw_proposal_kernel<T, decltype(m)::value, decltype(ext)::value>;
+      if (resident_ctas(reinterpret_cast<const void*>(kernel), kThreads, smem) < 1) return TSDE_EINVAL;
+      const int e = launch_kernel(kernel, (p.base.nquads + kThreads - 1) / kThreads, kThreads, smem,
+                                  reinterpret_cast<cudaStream_t>(L->stream), true, pg, p);
+      if (e == 0) g_launches[TSDE_KERNEL_PW_ADAPTIVE].fetch_add(1, std::memory_order_relaxed);
+      return e;
+    });
+  });
 }
 
 TSDE_EXPORT int tsde_adaptive_proposal_pointwise(const tsde_launch* L, const tsde_pointwise* prog, int32_t method,
@@ -1660,533 +2056,7 @@ TSDE_EXPORT int tsde_adaptive_pointwise_compile(const tsde_launch* L, const tsde
   return dispatch(L, [&](auto t) -> int {
     if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
     PwCompiled kc;
-    return pw_compiled(*prog, sizeof(t) == 8, kc, true);
+    return pw_loaded(*prog, kPwUnitAdaptive, pw_milstein_source(*prog, sizeof(t) == 8, kPwUnitAdaptive), kc);
   });
 }
 
-// ---- general / additive noise (GENERAL launches) -------------------------------------------------------------------
-// The two-program layout with per-channel values.  A g program runs m times per output, so it is compiled, never
-// interpreted (an interpreted instruction costs about 30 SASS instructions, DESIGN §4): pw_general_source writes it
-// out as a `Prog` for pw_general_euler_steps / pw_general_midpoint, or, by the program's tag, for pw_general_sra1
-// (TSDE_PW_LAYOUT_GENERAL_SRA), pw_general_euler_heun (_EULER_HEUN) or pw_general_reversible_heun_steps
-// (_REVERSIBLE_HEUN) (pw_device.cuh), with the IEEE options and the cache of the Milstein kernels.  A g
-// instruction is per channel when one of its sources is (a DM or M operand, or a per-channel value); the others are
-// per (row, d) element, evaluated once per lane before the channel loop.  The contraction of each lane's m values with
-// the increments is written out for the route the unfused step takes (gen_route), as that kernel sums:
-//   TSDE_GEN_ROWWISE   g * w                                       (the row-wise kernels' single product)
-//   TSDE_GEN_TILE      per channel quad an fma chain from 0; the quad sums as the xor-butterfly adds them, a pairwise
-//                      tree in natural order                       (gen_cta_kernel, gen_tma_kernel)
-//   TSDE_GEN_GENERIC   left to right from 0, a rounded multiply and a rounded add per channel    (gen_kernel)
-// (the sra1 launches never take the row-wise kernels: their m == 1 route is TSDE_GEN_GENERIC, pw_general_program).
-// Register use stays bounded: m <= TSDE_PW_GENERAL_MAX_M increments per thread, and the tree keeps at most
-// log2(m / 4) + 1 partial sums.
-
-// The launch bounds of the compiled general kernels: one resident CTA per SM at least, so that ptxas never spills the
-// increments (pointwise.py's _RESIDENT_CTAS counts on one).
-static_assert(sizeof(PwOperands<double>) + sizeof(PwP<double>) + sizeof(NoiseP<double>) + sizeof(PwSteps<double>) <=
-                  4096,
-              "the compiled general Euler kernel's parameters fit the 4 KiB parameter space");
-static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralMidP<double>) + sizeof(NoiseP<double>) <= 4096,
-              "the compiled general midpoint kernel's parameters fit the 4 KiB parameter space");
-static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralSraP<double>) + sizeof(NoiseP<double>) <= 4096,
-              "the compiled sra1 kernel's parameters fit the 4 KiB parameter space");
-static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralRevHeunP<double>) + sizeof(NoiseP<double>) +
-                      sizeof(PwSteps<double>) <=
-                  4096,
-              "the compiled general reversible-Heun kernel's parameters fit the 4 KiB parameter space");
-
-static bool pw_per_channel_kind(int kind) { return kind == TSDE_PW_DM || kind == TSDE_PW_M; }
-
-// The general layout (tagged TSDE_PW_LAYOUT_GENERAL): the two-program layout with DM / M operands read by g only.
-static bool pw_valid_general(const tsde_pointwise& pg) {
-  if (!pw_valid_two<TSDE_PW_MAX_REGS, true>(pg)) return false;
-  auto per_channel = [&](uint8_t s) {
-    return s >= TSDE_PW_OPERAND(0) && s != TSDE_PW_SRC_Y && s != TSDE_PW_SRC_GO &&
-           pw_per_channel_kind(pg.operand[s - TSDE_PW_OPERAND(0)].kind);
-  };
-  for (int i = 0; i < pg.n_fg; ++i)
-    if (per_channel(pg.instr[i].a) || (!pw_unary(pg.instr[i].op) && per_channel(pg.instr[i].b))) return false;
-  return !per_channel(pg.f_src);
-}
-
-// A launch and program of layout tag `layout` the general kernels serve; `route` is the contraction order (gen_route)
-// for dtype size `s`.
-static bool pw_general_program(const tsde_launch* L, const tsde_pointwise* prog, int64_t s, int& route,
-                               int layout = TSDE_PW_LAYOUT_GENERAL) {
-  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_GENERAL || L->m > TSDE_PW_GENERAL_MAX_M || !prog ||
-      prog->reserved != layout)
-    return false;
-  bool vec = true;
-  if (!pw_valid_tables(*prog, &vec, TSDE_PW_M) || !pw_valid_general(*prog)) return false;
-  // the unfused step's g is a new contiguous tensor (aligned), or the user's (d, m) block itself when g is a DM operand;
-  // the reversible-Heun pair densifies every g it reads (its solver state)
-  bool quads = true;
-  const uint8_t g = prog->g_src;
-  if (layout != TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN && g >= TSDE_PW_OPERAND(0) && g != TSDE_PW_SRC_Y &&
-      g != TSDE_PW_SRC_GO && prog->operand[g - TSDE_PW_OPERAND(0)].kind == TSDE_PW_DM)
-    quads = aligned16(prog->operand[g - TSDE_PW_OPERAND(0)].ptr);
-  if (layout == TSDE_PW_LAYOUT_GENERAL_SRA) {
-    // the sra1 launches call launch_gen directly, which stages U too, and take gen_kernel where cabi.cu would take the
-    // row-wise kernels (m == 1: the sum 0 + g * w, which turns a -0 product into +0)
-    route = gen_route(L->m, quads, 2 * L->m * s);
-    if (route == TSDE_GEN_ROWWISE) route = TSDE_GEN_GENERIC;
-  } else {
-    route = gen_route(L->m, quads, L->m * s);
-  }
-  return route != TSDE_GEN_WIDE;
-}
-
-// The translation unit of a program that passed pw_general_program, for m channels and contraction `route`: the
-// kernels of Euler chunks and of a midpoint step, or for an SRA-tagged program (`layout`) those of an sra1 step.
-static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t m, int route,
-                                     int layout = TSDE_PW_LAYOUT_GENERAL) {
-  const char* T = f64 ? "double" : "float";
-  const std::string fs = f64 ? "" : "f", M = num((int)m);
-  const int mq = (int)((m + 3) / 4);
-  auto operand = [&](uint8_t s) { return s >= TSDE_PW_OPERAND(0) && s != TSDE_PW_SRC_Y && s != TSDE_PW_SRC_GO; };
-  auto kind = [&](uint8_t s) { return in.operand[s - TSDE_PW_OPERAND(0)].kind; };
-  // an operand's value in lane j (channel k for DM / M; i is the lane's d index)
-  auto operand_value = [&](uint8_t s) -> std::string {
-    const std::string n = num(s - TSDE_PW_OPERAND(0));
-    switch (kind(s)) {
-      case TSDE_PW_IMM: return "ops.k[" + n + "].imm";
-      case TSDE_PW_T0: return "t0";
-      case TSDE_PW_SCALAR: return "u" + n;
-      case TSDE_PW_DM: return "ops.k[" + n + "].ptr[i * " + M + " + k]";
-      case TSDE_PW_M: return "ops.k[" + n + "].ptr[k]";
-      default: return "k" + n + "[j]";
-    }
-  };
-  // the expression of instruction x with sources a, b and destination (SEL's condition) d, as pw_loop's case
-  auto expression = [&](const tsde_pw_instr& x, const std::string& a, const std::string& b,
-                        const std::string& d) -> const std::string {
-    if (pw_transcendental(x.op)) return pw_helper_call(x.op, a, b);
-    switch (x.op) {
-      case TSDE_PW_MUL: return a + " * " + b;
-      case TSDE_PW_ADD: return a + " + " + b;
-      case TSDE_PW_SUB: return a + " - " + b;
-      case TSDE_PW_DIV: return a + " / " + b;
-      case TSDE_PW_NEG: return "-" + a;
-      case TSDE_PW_SQRT: return "sqrt" + fs + "(" + a + ")";
-      case TSDE_PW_LT: return a + " < " + b + " ? T(1) : T(0)";
-      case TSDE_PW_LE: return a + " <= " + b + " ? T(1) : T(0)";
-      case TSDE_PW_EQ: return a + " == " + b + " ? T(1) : T(0)";
-      case TSDE_PW_MAXIMUM:  // maximum_kernel_cuda (::max is fmax)
-        return a + " != " + a + " ? " + a + " : " + b + " != " + b + " ? " + b + " : fmax" + fs + "(" + a + ", " + b +
-               ")";
-      case TSDE_PW_MINIMUM:  // minimum_kernel_cuda (::min is fmin)
-        return a + " != " + a + " ? " + a + " : " + b + " != " + b + " ? " + b + " : fmin" + fs + "(" + a + ", " + b +
-               ")";
-      case TSDE_PW_ABS: return "fabs" + fs + "(" + a + ")";
-      default: return d + " != T(0) ? " + a + " : " + b;  // TSDE_PW_SEL: the condition is the destination
-    }
-  };
-  std::string o = "// An element-wise general-noise program of torchsde_b200, generated by pw_general_source\n"
-                  "#include \"pw_device.cuh\"\n\n";
-  o += pw_helper_declarations(in, T);
-  o += "namespace tsde {\nnamespace {\ntypedef " + std::string(T) + " T;\n\nstruct Prog {\n";
-  o += "  static constexpr int MQ = " + num(mq) + ";\n";
-  if (layout == TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN) o += "  static constexpr int M = " + M + ";\n";
-  for (int k = 0; k < in.n_operands; ++k) {
-    const std::string n = num(k);
-    if (in.operand[k].kind == TSDE_PW_SCALAR) o += "  T u" + n + ";\n";
-    if (in.operand[k].kind == TSDE_PW_CHANNEL || in.operand[k].kind == TSDE_PW_ROW) o += "  T k" + n + "[4];\n";
-  }
-  o += "  __device__ __forceinline__ void load(const PwOperands<T>& ops, const PwQuad& c) {\n";
-  for (int k = 0; k < in.n_operands; ++k) {
-    const std::string n = num(k);
-    const int kd = in.operand[k].kind;
-    if (kd == TSDE_PW_SCALAR) o += "    u" + n + " = *ops.k[" + n + "].ptr;\n";
-    if (kd == TSDE_PW_CHANNEL || kd == TSDE_PW_ROW)
-      o += "    load_quad(ops.k[" + n + "].ptr, c." + (kd == TSDE_PW_ROW ? "base" : "chan") + ", c.vec, c.nvalid, k" +
-           n + ");\n";
-  }
-  o += "  }\n";
-  // f: instructions [0, n_fg) on registers r<n>[4], as the Milstein kernels run them
-  o += "  __device__ __forceinline__ void f(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
-       "                                    T (&out)[4]) {\n    const T t0 = *tp;\n    (void)t0;\n";
-  for (int r = 0; r < in.n_regs; ++r) o += "    T r" + num(r) + "[4];\n";
-  auto fsrc = [&](uint8_t s) -> std::string {
-    if (s == TSDE_PW_SRC_Y) return "y[j]";
-    return operand(s) ? operand_value(s) : "r" + num(s) + "[j]";
-  };
-  o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
-  for (int i = 0; i < in.n_fg; ++i) {
-    const tsde_pw_instr& x = in.instr[i];
-    const std::string a = fsrc(x.a), b = pw_unary(x.op) ? a : fsrc(x.b), d = "r" + num(x.dst) + "[j]";
-    o += "      " + d + " = " + expression(x, a, b, d) + ";\n";
-  }
-  o += "      out[j] = " + fsrc(in.f_src) + ";\n    }\n  }\n";
-  // g: instruction i is n<i>[4] (per element, before the channel loop) or v<i> (per channel, inside G(k)); a register
-  // names the instruction that last wrote it
-  int def[TSDE_PW_MAX_REGS];
-  bool wide[TSDE_PW_MAX_INSTR] = {};
-  for (int r = 0; r < TSDE_PW_MAX_REGS; ++r) def[r] = -1;
-  auto is_wide = [&](uint8_t s) {
-    if (s == TSDE_PW_SRC_Y) return false;
-    if (operand(s)) return pw_per_channel_kind(kind(s));
-    return wide[def[s]];
-  };
-  auto gsrc = [&](uint8_t s) -> std::string {
-    if (s == TSDE_PW_SRC_Y) return "y[j]";
-    if (operand(s)) return operand_value(s);
-    return wide[def[s]] ? "v" + num(def[s]) : "n" + num(def[s]) + "[j]";
-  };
-  std::string narrow, per_channel;
-  for (int i = in.n_fg; i < in.n_instr; ++i) {
-    const tsde_pw_instr& x = in.instr[i];
-    const bool sel = x.op == TSDE_PW_SEL;
-    wide[i] = is_wide(x.a) || (!pw_unary(x.op) && is_wide(x.b)) || (sel && is_wide(x.dst));
-    const std::string a = gsrc(x.a), b = pw_unary(x.op) ? a : gsrc(x.b), d = sel ? gsrc(x.dst) : "";
-    if (wide[i])
-      per_channel += "        const T v" + num(i) + " = " + expression(x, a, b, d) + ";\n";
-    else
-      narrow += "      n" + num(i) + "[j] = " + expression(x, a, b, d) + ";\n";
-    def[x.dst] = i;
-  }
-  // the g program at (*tp, y), up to lane j's channel values G(k)
-  std::string g_head = "    const T t0 = *tp;\n    (void)t0;\n";
-  for (int i = in.n_fg; i < in.n_instr; ++i)
-    if (!wide[i]) g_head += "    T n" + num(i) + "[4];\n";
-  g_head += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
-  g_head += narrow;
-  g_head += "    }\n#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n"
-            "      const int64_t i = c.chan + (j < c.nvalid ? j : 0);  // (the d index of the lane; padding lanes read lane 0's)\n"
-            "      (void)i;\n      auto G = [&](int k) -> T {\n        (void)k;\n";
-  g_head += per_channel;
-  g_head += "        return ";
-  g_head += gsrc(in.g_src);
-  g_head += ";\n      };\n";
-  // lane j's acc: the values val(k) contracted with the weights w[k] in the route's order; pre(k) / post(k) are the
-  // statements before / after channel k's term.  (Built by appending: a sum of two temporaries would instantiate a
-  // std::operator+ that the library might export.)
-  auto cat = [](std::initializer_list<std::string> parts) {
-    std::string s;
-    for (const std::string& x : parts) s += x;
-    return s;
-  };
-  const std::string fma = "fma" + fs;
-  auto contraction = [&](auto val, auto pre, auto post) {
-    std::string s;
-    if (route == TSDE_GEN_ROWWISE) {
-      s += cat({pre(0), "      const T acc = ", val(0), " * w[0];\n", post(0)});
-    } else if (route == TSDE_GEN_GENERIC) {
-      s += "      T acc = T(0);\n";
-      for (int k = 0; k < m; ++k) s += cat({pre(k), "      acc = acc + ", val(k), " * w[", num(k), "];\n", post(k)});
-    } else {
-      std::string level[TSDE_PW_GENERAL_MAX_M / 4];  // the partial sums of the tree's current level
-      for (int q = 0; q < mq; ++q) {
-        const std::string sq = cat({"s", num(q)});
-        const int k0 = 4 * q;
-        s += cat({pre(k0), "      T ", sq, " = ", fma, "(", val(k0), ", w[", num(k0), "], T(0));\n", post(k0)});
-        for (int j = 1; j < 4; ++j)
-          s += cat({pre(k0 + j), "      ", sq, " = ", fma, "(", val(k0 + j), ", w[", num(k0 + j), "], ", sq, ");\n",
-                    post(k0 + j)});
-        level[q] = sq;
-      }
-      for (int l = 0, n = mq; n > 1; ++l, n /= 2) {
-        for (int p = 0; p < n; p += 2) {
-          const std::string a = cat({"a", num(l), "_", num(p / 2)});
-          s += cat({"      const T ", a, " = ", level[p], " + ", level[p + 1], ";\n"});
-          level[p / 2] = a;
-        }
-      }
-      s += cat({"      const T acc = ", level[0], ";\n"});
-    }
-    s += "      out[j] = acc;\n    }\n  }\n";
-    return s;
-  };
-  auto none = [](int) { return std::string(); };
-  if (layout == TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN) {
-    // the state's g values gs[j][k] stay in registers: z's contraction reads them, y's contracts (gs + g1) and leaves
-    // g1 in their place (pw_general_reversible_heun_steps)
-    o += "  template <typename Op>\n"
-         "  __device__ __forceinline__ void dot(const Op& op, const T (&gs)[4][M], const T (&w)[4 * MQ], T (&out)[4]) {\n"
-         "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
-    o += contraction([&](int k) { return cat({"op.gval(0, {gs[j][", num(k), "]})"}); }, none, none);
-    o += "  template <typename Op>\n"
-         "  __device__ __forceinline__ void gstep(const PwOperands<T>& ops, const PwQuad& c, const T* tp,\n"
-         "                                        const T (&y)[4], const Op& op, const T (&w)[4 * MQ], T (&gs)[4][M],\n"
-         "                                        T (&out)[4]) {\n";
-    o += g_head;
-    o += contraction([&](int k) { return cat({"op.gval(0, {gs[j][", num(k), "], h", num(k), "})"}); },
-                     [&](int k) { return cat({"      const T h", num(k), " = G(", num(k), ");\n"}); },
-                     [&](int k) { return cat({"      gs[j][", num(k), "] = h", num(k), ";\n"}); });
-  } else {
-    o += "  __device__ __forceinline__ void gp(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
-         "                                     const T (&w)[4 * MQ], T (&out)[4]) {\n";
-    o += g_head;
-    o += contraction([&](int k) { return cat({"G(", num(k), ")"}); }, none, none);
-  }
-  o += "};\n}  // namespace\n}  // namespace tsde\n";
-  const std::string bounds = "__launch_bounds__(" + num(kThreads) + ", 1)";
-  if (layout == TSDE_PW_LAYOUT_GENERAL_SRA) {
-    for (const char* v : {"single", "multi"}) {
-      const std::string src = v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti";
-      o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_general_sra1_" + v +
-           "(const __grid_constant__ tsde::PwOperands<tsde::T> ops,\n"
-           "    const __grid_constant__ tsde::PwGeneralSraP<tsde::T> p, const tsde::NoiseP<tsde::T> nz) {\n"
-           "  tsde::pw_general_sra1<tsde::T, " + src + ", tsde::Prog>(ops, p, nz);\n}\n";
-    }
-    return o;
-  }
-  if (layout == TSDE_PW_LAYOUT_GENERAL_EULER_HEUN) {
-    for (const char* v : {"single", "multi"}) {
-      const std::string src = v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti";
-      o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_general_euler_heun_" + v +
-           "(const __grid_constant__ tsde::PwOperands<tsde::T> ops,\n"
-           "    const tsde::PwGeneralMidP<tsde::T> p, const tsde::NoiseP<tsde::T> nz) {\n"
-           "  tsde::pw_general_euler_heun<tsde::T, " + src + ", tsde::Prog>(ops, p, nz);\n}\n";
-    }
-    return o;
-  }
-  if (layout == TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN) {
-    for (const char* v : {"single", "multi"}) {
-      const std::string src = v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti";
-      o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_general_reversible_heun_" + v +
-           "(const __grid_constant__ tsde::PwOperands<tsde::T> ops,\n"
-           "    const tsde::PwGeneralRevHeunP<tsde::T> p, const tsde::NoiseP<tsde::T> nz,\n"
-           "    const __grid_constant__ tsde::PwSteps<tsde::T> st) {\n"
-           "  tsde::pw_general_reversible_heun_steps<tsde::T, " + src + ", tsde::Prog>(ops, p, nz, st);\n}\n";
-    }
-    return o;
-  }
-  for (const char* v : {"single", "multi"}) {
-    const std::string src = v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti";
-    o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_general_euler_" + v +
-           "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwP<tsde::T> p,\n"
-           "    const tsde::NoiseP<tsde::T> nz, const __grid_constant__ tsde::PwSteps<tsde::T> st) {\n"
-           "  tsde::pw_general_euler_steps<tsde::T, " + src + ", tsde::Prog>(ops, p, nz, st);\n}\n";
-  }
-  for (const char* v : {"single", "multi"}) {
-    const std::string src = v[0] == 's' ? "TSDE_SRC_COUNTER" : "tsde::kSrcCounterMulti";
-    o += std::string("\nextern \"C\" __global__ void ") + bounds + "\ntsde_pw_general_midpoint_" + v +
-           "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwGeneralMidP<tsde::T> p,\n"
-           "    const tsde::NoiseP<tsde::T> nz) {\n"
-           "  tsde::pw_general_midpoint<tsde::T, " + src + ", tsde::Prog>(ops, p, nz);\n}\n";
-  }
-  return o;
-}
-
-// The layout a GENERAL launch of tsde_pointwise_compile / tsde_pointwise_source serves `prog` in: the unit of its
-// SRA, EULER_HEUN or REVERSIBLE_HEUN tag, else the Euler / midpoint unit (which refuses every other tag).
-static int pw_general_layout(const tsde_pointwise* prog) {
-  if (!prog) return TSDE_PW_LAYOUT_GENERAL;
-  switch (prog->reserved) {
-    case TSDE_PW_LAYOUT_GENERAL_SRA:
-    case TSDE_PW_LAYOUT_GENERAL_EULER_HEUN:
-    case TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN:
-      return prog->reserved;
-    default:
-      return TSDE_PW_LAYOUT_GENERAL;
-  }
-}
-
-// The loaded kernels of a general-layout program: Euler's two, then midpoint's two; of a tagged one, the two of its
-// unit (single cell, then multi-cell).
-template <typename T>
-static int pw_general_compiled(const tsde_launch* L, const tsde_pointwise* prog, PwCompiled& kc) {
-  int route;
-  const int layout = pw_general_layout(prog);
-  if (!pw_general_program(L, prog, sizeof(T), route, layout)) return TSDE_EINVAL;
-  std::string src = pw_general_source(*prog, sizeof(T) == 8, L->m, route, layout);
-  if (layout == TSDE_PW_LAYOUT_GENERAL_SRA)
-    return pw_loaded(*prog, std::move(src), {"tsde_pw_general_sra1_single", "tsde_pw_general_sra1_multi"}, kc);
-  if (layout == TSDE_PW_LAYOUT_GENERAL_EULER_HEUN)
-    return pw_loaded(*prog, std::move(src), {"tsde_pw_general_euler_heun_single", "tsde_pw_general_euler_heun_multi"},
-                     kc);
-  if (layout == TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN)
-    return pw_loaded(*prog, std::move(src),
-                     {"tsde_pw_general_reversible_heun_single", "tsde_pw_general_reversible_heun_multi"}, kc);
-  return pw_loaded(*prog, std::move(src),
-                   {"tsde_pw_general_euler_single", "tsde_pw_general_euler_multi", "tsde_pw_general_midpoint_single",
-                    "tsde_pw_general_midpoint_multi"},
-                   kc);
-}
-
-template <typename T>
-static PwOperands<T> pw_operands(const tsde_pointwise* prog) {
-  PwOperands<T> ops{};
-  for (int k = 0; k < prog->n_operands; ++k)
-    ops.k[k] = PwOperand<T>{static_cast<const T*>(prog->operand[k].ptr), (T)prog->operand[k].imm};
-  return ops;
-}
-
-// tsde_solve_euler_pointwise for a GENERAL launch: the chunk `steps[0, n_steps)` from y0 as one launch of the
-// program's compiled Euler kernel, under the rules of pw_milstein_chunk.
-template <typename T>
-static int pw_general_euler(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog, const void* y0,
-                            const tsde_pw_step* steps, int32_t n_steps) {
-  int route;
-  if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
-  if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !y0 || !pw_general_program(L, prog, sizeof(T), route))
-    return TSDE_EINVAL;
-  bool vec = L->d % 4 == 0 && aligned16(y0);
-  pw_valid_tables(*prog, &vec, TSDE_PW_M);
-  NoiseP<T> np;
-  if (int e = fill_noise<T>(L, nz, false, np)) return e;
-  if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
-  PwSteps<T> st{};
-  st.n = n_steps;
-  for (int j = 0; j < n_steps; ++j) {
-    const tsde_pw_step& s = steps[j];
-    if (!s.t0) return TSDE_EINVAL;
-    if (s.y1 && !aligned16(s.y1)) vec = false;
-    st.s[j] = PwStep<T>{s.cell_id, static_cast<const T*>(s.t0), static_cast<T*>(s.y1), (T)sqrt(s.h), (T)s.dt};
-  }
-  PwCompiled kc;
-  if (int e = pw_general_compiled<T>(L, prog, kc)) return e;
-  PwOperands<T> ops = pw_operands<T>(prog);
-  PwP<T> p{};
-  p.y0 = static_cast<const T*>(y0);
-  fill_quad_map(L->rows, L->d, p);
-  p.vec = vec ? 1 : 0;
-  // (the multi-cell merge reads the first cell and the uniform length from the noise descriptor)
-  np.cell_id = steps[0].cell_id;
-  np.h = steps[0].h;
-  void* args[] = {&ops, &p, &np, &st};
-  const int e = launch_kernel_handle(kc.kernel[np.n_cells > 1 ? 1 : 0], (p.nquads + kThreads - 1) / kThreads,
-                                     kThreads, reinterpret_cast<cudaStream_t>(L->stream), args);
-  if (e == 0) g_launches[TSDE_KERNEL_PW_GENERAL].fetch_add(1, std::memory_order_relaxed);
-  return e;
-}
-
-// tsde_step_predictor_corrector_pointwise for a GENERAL launch: one midpoint step as one launch of the program's
-// compiled midpoint kernel, or one Euler-Heun step of an EULER_HEUN-tagged program.
-template <typename T>
-static int pw_general_pc_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
-                              const void* y0, const void* t0, const void* t_p, int32_t method, double dt,
-                              double half_dt, void* y1) {
-  int route;
-  const bool euler_heun = method == TSDE_PC_EULER_HEUN;
-  if ((method != TSDE_PC_MIDPOINT && !euler_heun) || !t0 || !t_p || !y0 || !y1 || !nz ||
-      nz->source != TSDE_SRC_COUNTER || nz->flags ||
-      !pw_general_program(L, prog, sizeof(T), route,
-                          euler_heun ? TSDE_PW_LAYOUT_GENERAL_EULER_HEUN : TSDE_PW_LAYOUT_GENERAL))
-    return TSDE_EINVAL;
-  bool vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y1);
-  pw_valid_tables(*prog, &vec, TSDE_PW_M);
-  NoiseP<T> np;
-  if (int e = fill_noise<T>(L, nz, false, np)) return e;
-  PwCompiled kc;
-  if (int e = pw_general_compiled<T>(L, prog, kc)) return e;
-  PwOperands<T> ops = pw_operands<T>(prog);
-  PwGeneralMidP<T> p{};
-  p.base.y0 = static_cast<const T*>(y0);
-  p.base.y1 = static_cast<T*>(y1);
-  p.base.t0 = static_cast<const T*>(t0);
-  p.base.dt = (T)dt;
-  fill_quad_map(L->rows, L->d, p.base);
-  p.base.vec = vec ? 1 : 0;
-  p.t_p = static_cast<const T*>(t_p);
-  p.half_dt = (T)half_dt;
-  void* args[] = {&ops, &p, &np};
-  const int first = euler_heun ? 0 : 2;  // (the Euler-Heun unit's kernels, or the midpoint ones after Euler's)
-  const int e = launch_kernel_handle(kc.kernel[first + (np.n_cells > 1 ? 1 : 0)],
-                                     (p.base.nquads + kThreads - 1) / kThreads, kThreads,
-                                     reinterpret_cast<cudaStream_t>(L->stream), args);
-  if (e == 0) g_launches[TSDE_KERNEL_PW_GENERAL].fetch_add(1, std::memory_order_relaxed);
-  return e;
-}
-
-// tsde_solve_reversible_heun_pointwise for a GENERAL launch: the chunk `steps[0, n_steps)` from y0 and the solver state
-// in[] = z0, f0, g0 (g of shape (rows, d, m)), left in out[] = z1, f1, g1, as one launch of the REVERSIBLE_HEUN-tagged
-// program's compiled kernel, under the rules of pw_general_euler.
-template <typename T>
-static int pw_general_reversible_heun(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
-                                      const void* y0, const void* const (&in)[3], const tsde_pw_step* steps,
-                                      int32_t n_steps, void* const (&out)[3]) {
-  int route;
-  if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || !steps[n_steps - 1].y1) return TSDE_EINVAL;
-  if (!nz || nz->source != TSDE_SRC_COUNTER || nz->flags || !y0 ||
-      !pw_general_program(L, prog, sizeof(T), route, TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN))
-    return TSDE_EINVAL;
-  for (int i = 0; i < 3; ++i)
-    if (!in[i] || !out[i]) return TSDE_EINVAL;
-  bool vec = L->d % 4 == 0 && aligned16(y0);
-  for (int i = 0; i < 2; ++i) vec = vec && aligned16(in[i]) && aligned16(out[i]);  // z, f
-  pw_valid_tables(*prog, &vec, TSDE_PW_M);
-  NoiseP<T> np;
-  if (int e = fill_noise<T>(L, nz, false, np)) return e;
-  if (np.n_cells > 1 && n_steps > 1) return TSDE_EINVAL;
-  PwSteps<T> st{};
-  st.n = n_steps;
-  for (int j = 0; j < n_steps; ++j) {
-    const tsde_pw_step& s = steps[j];
-    if (!s.t0) return TSDE_EINVAL;
-    if (s.y1 && !aligned16(s.y1)) vec = false;
-    st.s[j] = PwStep<T>{s.cell_id, static_cast<const T*>(s.t0), static_cast<T*>(s.y1), (T)sqrt(s.h), (T)s.dt};
-  }
-  PwCompiled kc;
-  if (int e = pw_general_compiled<T>(L, prog, kc)) return e;
-  PwOperands<T> ops = pw_operands<T>(prog);
-  PwGeneralRevHeunP<T> p{};
-  p.base.y0 = static_cast<const T*>(y0);
-  fill_quad_map(L->rows, L->d, p.base);
-  p.base.vec = vec ? 1 : 0;
-  p.z0 = static_cast<const T*>(in[0]);
-  p.f0 = static_cast<const T*>(in[1]);
-  p.g0 = static_cast<const T*>(in[2]);
-  p.z1 = static_cast<T*>(out[0]);
-  p.f1 = static_cast<T*>(out[1]);
-  p.g1 = static_cast<T*>(out[2]);
-  p.gvec = L->m % 4 == 0 && aligned16(in[2]) && aligned16(out[2]) ? 1 : 0;
-  // (the multi-cell merge reads the first cell and the uniform length from the noise descriptor)
-  np.cell_id = steps[0].cell_id;
-  np.h = steps[0].h;
-  void* args[] = {&ops, &p, &np, &st};
-  const int e = launch_kernel_handle(kc.kernel[np.n_cells > 1 ? 1 : 0], (p.base.nquads + kThreads - 1) / kThreads,
-                                     kThreads, reinterpret_cast<cudaStream_t>(L->stream), args);
-  if (e == 0) g_launches[TSDE_KERNEL_PW_GENERAL].fetch_add(1, std::memory_order_relaxed);
-  return e;
-}
-
-// tsde_step_srk_diag_pointwise for a GENERAL launch: one sra1 step as one launch of the SRA-tagged program's
-// compiled kernel.
-template <typename T>
-static int pw_general_sra1_step(const tsde_launch* L, const tsde_noise* nz, const tsde_pointwise* prog,
-                                const void* y0, const void* t_1, const void* t_34, const void* t_00, double dt,
-                                double rdt, void* y1) {
-  int route;
-  if (!t_1 || !t_34 || !t_00 || !y0 || !y1 || !nz || nz->source != TSDE_SRC_COUNTER || nz->flags ||
-      !pw_general_program(L, prog, sizeof(T), route, TSDE_PW_LAYOUT_GENERAL_SRA))
-    return TSDE_EINVAL;
-  bool vec = L->d % 4 == 0 && aligned16(y0) && aligned16(y1);
-  pw_valid_tables(*prog, &vec, TSDE_PW_M);
-  NoiseP<T> np;
-  if (int e = fill_noise<T>(L, nz, false, np)) return e;
-  PwCompiled kc;
-  if (int e = pw_general_compiled<T>(L, prog, kc)) return e;
-  PwOperands<T> ops = pw_operands<T>(prog);
-  PwGeneralSraP<T> p{};
-  p.base.y0 = static_cast<const T*>(y0);
-  p.base.y1 = static_cast<T*>(y1);
-  p.base.t0 = static_cast<const T*>(t_00);
-  p.base.dt = (T)dt;
-  fill_quad_map(L->rows, L->d, p.base);
-  p.base.vec = vec ? 1 : 0;
-  p.t_1 = static_cast<const T*>(t_1);
-  p.t_34 = static_cast<const T*>(t_34);
-  p.stage = GSraStageOp<T>{(T)dt, (T)rdt};
-  p.final_op = GSraFinalOp<T>{(T)dt, (T)rdt, (T)(1.0 / 3), (T)(2.0 / 3)};
-  void* args[] = {&ops, &p, &np};
-  const int e = launch_kernel_handle(kc.kernel[np.n_cells > 1 ? 1 : 0], (p.base.nquads + kThreads - 1) / kThreads,
-                                     kThreads, reinterpret_cast<cudaStream_t>(L->stream), args);
-  if (e == 0) g_launches[TSDE_KERNEL_PW_GENERAL].fetch_add(1, std::memory_order_relaxed);
-  return e;
-}
-
-// tsde_pointwise_source for a GENERAL launch
-template <typename T>
-static int64_t pw_general_source_of(const tsde_launch* L, const tsde_pointwise* prog, char* buf, int64_t size) {
-  int route;
-  const int layout = pw_general_layout(prog);
-  if (!pw_general_program(L, prog, sizeof(T), route, layout)) return TSDE_EINVAL;
-  const std::string src = pw_general_source(*prog, sizeof(T) == 8, L->m, route, layout);
-  if (buf && size > 0) {
-    const size_t n = std::min(src.size(), (size_t)size - 1);
-    memcpy(buf, src.data(), n);
-    buf[n] = 0;
-  }
-  return (int64_t)src.size();
-}

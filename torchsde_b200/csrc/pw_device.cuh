@@ -306,7 +306,7 @@ __device__ __forceinline__ void pw_milstein_step(Prog& prog, const PwOperands<T>
 // gives it a destination (an output row, the chunk's last state).  The unfused step moves 13 tensors; a chunk moves one
 // read and the stores it is asked for.
 //
-// `Prog` is the program, generated by the library as straight-line code (pw_codegen in pointwise.cu):
+// `Prog` is the program, generated by the library as straight-line code (pw_milstein_source in pointwise.cu):
 //   load(ops, c)                    its operands, after the dependency wait (CHANNEL / ROW quads it keeps in registers)
 //   fg(ops, c, s, y, f, g)          instructions [0, n_fg) at (s.t0, y), and the f and g results
 //   vjp(ops, c, s, y, go, gdg)      instructions [n_fg, n_instr), and the gdg result
