@@ -100,6 +100,7 @@ OLD_BMM_SHAPES = [(8192, 32, 16), (257, 5, 3), (64, 7, 8), (33, 4, 2), (100, 40,
 
 
 BMM_GROUPS = [str(m) for m in ref.TILE_M] + ['generic', 'unaligned', 'old']
+TRACE_ATTEMPTS = 5   # traces of the same launches taken before a short one counts as a missing kernel
 
 
 def _bmm_cases(dtype, group):
@@ -161,12 +162,15 @@ def test_bmm_ga_routes_vs_exact(dtype, group):
     names = _bmm_kernels(run)
     codes = [code for code, _ in results]
     assert codes == [0] * len(expect), codes
-    if len(names) != len(expect):
-        # every launch returned 0, but the trace holds fewer kernel records than launches: capture the same launches
-        # once more (their outputs are checked below either way)
+    counts = [len(names)]
+    while len(names) != len(expect) and len(counts) < TRACE_ATTEMPTS:
+        # every launch returned 0, but the trace holds fewer kernel records than launches (the profiler now and then
+        # loses a few records of a busy process, and can lose them in consecutive traces): capture the same launches
+        # again (their outputs are checked below either way)
         names = _bmm_kernels(run)
+        counts.append(len(names))
         assert [code for code, _ in results] == [0] * len(expect)
-    assert len(names) == len(expect), (len(names), len(expect))
+    assert len(names) == len(expect), f'{len(expect)} launches; kernel records per trace: {counts}'
     wrong = [(i, n, e) for i, (n, e) in enumerate(zip(names, expect)) if ref.bmm_kernel_name(e, TAG[dtype]) not in n]
     assert not wrong, wrong[:5]
     bad, it = [], iter(results)
