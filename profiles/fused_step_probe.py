@@ -13,7 +13,12 @@ The program is the one the solver records for cfg2's SDE (f = mu*y, g = sigma*y,
            every step), in situ (the next launch starts from the last row) and cold (y0 from the rotating sets);
            microseconds per step and the achieved write bandwidth.  K = 128 does not fit the step table
            (TSDE_PW_MAX_STEPS = 64, bounded by the 4 KiB parameter space) and is reported as such.  The write bandwidth is also
-           given as a share of the H100 SXM data sheet's 3.35 TB/s, the floor of a step being its y1 store.
+           given as a share of the H100 SXM data sheet's 3.35 TB/s and of the measured fill floor, the floor of a step
+           being its y1 store.  Each chunk runs on a uniform grid (consecutive cells: the kernel's loop of one back-edge,
+           PwSteps::uniform) and, as chunk_K_table_*, on cells two apart, which the kernel runs through its step table
+           (the general loop) with the same work per step.
+  fill     torch's fill_ of the 64 rows of one output series (64 x 16 MiB at cfg2), in microseconds per row: the store
+           floor of a step as this card reaches it.
   compile  the one-time cost of the program's kernels: tsde_pointwise_compile (NVRTC to an sm_90a cubin, then the
            library load) in a process that has not compiled the program yet, in ms.  The solver pays it on the recording
            step, outside bench.py's timed region; a later program of the same structure pays nothing.
@@ -80,21 +85,29 @@ def fused(s_in, s_out):
 series = [torch.empty(_cabi.PW_MAX_STEPS, B, D, device=dev) for _ in range(2)]
 
 
-def chunk(k, y0, rows):
+def chunk(k, y0, rows, cell_step=1):
     steps = (_cabi.PwStep * k)()
     for j, st in enumerate(steps):
-        st.cell_id, st.h, st.dt, st.t0, st.y1 = 7 + j, dt, dt, P(t0), P(rows[j])
+        st.cell_id, st.h, st.dt, st.t0, st.y1 = 7 + cell_step * j, dt, dt, P(t0), P(rows[j])
     _cabi.check(lib.tsde_solve_milstein_pointwise(ctypes.byref(L), ctypes.byref(nz), ctypes.byref(prog), P(y0), steps,
                                                   k, 1), 'chunk')
 
 
-def timed_chunk(k, chained):
+def timed_chunk(k, chained, cell_step=1):
     """Microseconds per launch of a k-step chunk, graph-captured."""
     def issue():
         for i in range(REPS):
             src, dst = series[i % 2], series[(i + 1) % 2]
-            chunk(k, src[k - 1] if chained else sets[i % NSET]['y0'], dst)
+            chunk(k, src[k - 1] if chained else sets[i % NSET]['y0'], dst, cell_step)
     return timed_issue(issue)
+
+
+def timed_fill():
+    """Microseconds per 16 MiB row of torch's fill_ of one whole output series."""
+    def issue():
+        for i in range(REPS):
+            series[i % 2].fill_(float(i))
+    return timed_issue(issue) / _cabi.PW_MAX_STEPS
 
 
 def seed(s_in, s_out):
@@ -154,13 +167,20 @@ DATASHEET_GBPS = 3350.0
 for name, launch, chained in (('fused_cold', fused, False), ('fused_in_situ', fused, True), ('seed_cold', seed, False)):
     us = timed(launch, chained)
     out[name] = {'us': round(us, 2), 'GBps': round(nbytes / (us * 1e-6) / 1e9, 1)}
-for k in (1, 8, 32, 64, 128):
+fill_us = timed_fill()
+fill_gbps = B * D * 4 / (fill_us * 1e-6) / 1e9
+out['fill'] = {'us_per_row': round(fill_us, 2), 'GBps': round(fill_gbps, 1)}
+for k in (1, 8, 16, 32, 64, 128):
     if k > _cabi.PW_MAX_STEPS:
         out[f'chunk_{k}'] = 'exceeds TSDE_PW_MAX_STEPS'
         continue
-    for mode, chained in (('in_situ', True), ('cold', False)):
-        us = timed_chunk(k, chained)
-        gbps = k * B * D * 4 / (us * 1e-6) / 1e9
-        out[f'chunk_{k}_{mode}'] = {'us_per_step': round(us / k, 2), 'write_GBps': round(gbps, 1),
-                                    'of_datasheet': round(gbps / DATASHEET_GBPS, 3)}
+    for grid, cell_step in (('', 1), ('table_', 2)):
+        if grid and k == 1:  # (a one-step chunk is always uniform)
+            continue
+        for mode, chained in (('in_situ', True), ('cold', False)):
+            us = timed_chunk(k, chained, cell_step)
+            gbps = k * B * D * 4 / (us * 1e-6) / 1e9
+            out[f'chunk_{k}_{grid}{mode}'] = {'us_per_step': round(us / k, 2), 'write_GBps': round(gbps, 1),
+                                              'of_datasheet': round(gbps / DATASHEET_GBPS, 3),
+                                              'of_fill': round(gbps / fill_gbps, 3)}
 print(json.dumps(out), flush=True)

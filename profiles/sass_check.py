@@ -7,7 +7,10 @@ load and store the shared-memory register file): the loop that runs programs who
 reads no global memory (LDG) and decodes no byte fields from the parameter space (LDC.U8).  Milstein programs are not
 interpreted but compiled at run time (NVRTC): it writes cfg2's program out (tsde_pointwise_source), compiles it as the
 library does and checks that the compiled kernel's step loop touches no shared memory (LDS / STS), no local memory
-(LDL / STL, spills) and reads no instruction word from the parameter space (an indexed LDC); exit status 1 otherwise.
+(LDL / STL, spills) and reads no instruction word from the parameter space (an indexed LDC).  Its loops for a uniform
+grid (PwSteps::uniform, one per `ito`) each have one back-edge, no indexed LDC / ULDC, no LDL / STL and at most
+UNIFORM_MAX instructions, and the kernel at most 64 registers (its launch bounds, 256 threads x 4 CTAs); exit status 1
+otherwise.
 
     python profiles/sass_check.py > out/sass_evidence.txt
 """
@@ -48,6 +51,7 @@ PICK = [  # (label, regex on the demangled kernel name)
     ('logqp KL-integrand augmentation, fp32', r'logqp_augment_kernel<float>'),
 ]
 INTERPRETED = [r'pw_chunk_kernel<float, 1, 0>', r'pw_chunk_kernel<double, 1, 0>', r'pw_chunk_kernel<float, 1, 1>', r'pw_chunk_kernel<double, 1, 1>']
+UNIFORM_MAX = 150  # instructions per step of the uniform-grid loop (one back-edge: the static count is the dynamic one)
 COUNT = ['LDG.E.128', 'LDG.E.EF.128', 'STG.E.128', 'LDS.128', 'UBLKCP', 'SYNCS', 'MUFU', 'FFMA', 'FMUL', 'FADD', 'DFMA',
          'SHFL', 'BAR.SYNC', 'LDL', 'STL', 'IMAD.WIDE']
 
@@ -107,15 +111,26 @@ def compiled_milstein():
     back = [(int(re.search(r'0x([0-9a-f]+)', op.split('BRA')[1]).group(1), 16), addr) for addr, op in ins
             if re.search(r'\bBRA\b', op) and re.search(r'0x([0-9a-f]+)', op.split('BRA')[1])
             and int(re.search(r'0x([0-9a-f]+)', op.split('BRA')[1]).group(1), 16) < addr]
-    a, b = max(back, key=lambda x: x[1] - x[0])  # the step loop: the outermost backward branch
+    a, b = max(back, key=lambda x: x[1] - x[0])  # the step table's loop: the outermost backward branch
     loop = [op for addr, op in ins if a <= addr <= b]
     bad = [o for o in loop if re.search(r'\bLDS|\bSTS|\bLDL|\bSTL|LDC[.\w]*\s+\S+,\s*c\[0x0\]\[R', o)]
     cnt = {k: sum(1 for o in loop if re.search(r'\b' + re.escape(k) + r'\b', o)) for k in COUNT}
     print(f"## cfg2's Milstein program, compiled at run time (NVRTC), fp32, one cell per step\n"
-          f"   REG {reg}  STACK {stack}  SHARED {shared}  LOCAL {local}  step loop: {len(loop)} instructions\n   " +
+          f"   REG {reg}  STACK {stack}  SHARED {shared}  LOCAL {local}  step-table loop: {len(loop)} instructions\n   " +
           '  '.join(f"{k}={v}" for k, v in cnt.items() if v) +
-          f"\n   shared / local memory or indexed parameter reads in the step loop: {len(bad)}\n")
-    return not bad and not stack and not local
+          f"\n   shared / local memory or indexed parameter reads in the step-table loop: {len(bad)}")
+    # the uniform-grid loops: the loops whose only branch is their back-edge
+    uniform = [[op for addr, op in ins if x <= addr <= y] for x, y in back]
+    uniform = [u for u in uniform if sum(1 for o in u if re.search(r'\bBRA\b', o)) == 1]
+    ok = len(uniform) == 2 and reg <= 64
+    for u in uniform:
+        ubad = [o for o in u if re.search(r'\bLDL|\bSTL|U?LDC[.\w]*\s+\S+,\s*c\[0x0\]\[U?R', o)]
+        ok = ok and not ubad and len(u) <= UNIFORM_MAX
+        cnt = {k: sum(1 for o in u if re.search(r'\b' + re.escape(k) + r'\b', o)) for k in COUNT}
+        print(f"   uniform-grid loop: {len(u)} instructions (at most {UNIFORM_MAX}), indexed parameter reads or local"
+              f" memory: {len(ubad)}\n   " + '  '.join(f"{k}={v}" for k, v in cnt.items() if v))
+    print(f"   uniform-grid loops: {len(uniform)} (one per ito), registers {reg} (at most 64)\n")
+    return ok and not bad and not stack and not local
 
 
 def main():

@@ -995,7 +995,7 @@ def plan_chunks(first, n_steps, interpolated=(), multi_cell=(), max_steps=_cabi.
 
 # Resident CTAs (256 threads) per SM of each chunked kernel, (float32, float64), from its registers (-Xptxas -v,
 # sm_90a: 64 K registers per SM): Milstein's compiled kernels are pinned there by their launch bounds (256, 4) and
-# (256, 2) (cfg2's program: 41 registers in fp32); Euler at 54 and 88-96; reversible Heun at 72 and 110-120.
+# (256, 2) (cfg2's program: 54 registers in fp32); Euler at 54 and 88-96; reversible Heun at 72 and 110-120.
 # The compiled general-noise Euler and reversible-Heun kernels are bounded at (256, 1): at least one resident CTA,
 # whatever m.
 _RESIDENT_CTAS = {'milstein': (4, 2), 'euler': (4, 2), 'reversible_heun': (3, 2), 'euler_general': (1, 1),

@@ -41,17 +41,55 @@ struct Key {
   uint32_t lo, hi;
 };
 
+constexpr uint32_t kPhiloxM0 = 0xD2511F53u, kPhiloxM1 = 0xCD9E8D57u;  // round multipliers
+constexpr uint32_t kPhiloxW0 = 0x9E3779B9u, kPhiloxW1 = 0xBB67AE85u;  // key increments (Weyl sequence)
+
+__device__ __forceinline__ uint4 philox_round(uint4 c, uint32_t k0, uint32_t k1) {
+  const uint32_t hi0 = __umulhi(kPhiloxM0, c.x), lo0 = kPhiloxM0 * c.x;
+  const uint32_t hi1 = __umulhi(kPhiloxM1, c.z), lo1 = kPhiloxM1 * c.z;
+  return make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+}
+
+// (round i XORs in the key words (k0 + i W0, k1 + i W1))
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
-  constexpr uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
-  constexpr uint32_t W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
 #pragma unroll
   for (int i = 0; i < 10; ++i) {
-    const uint32_t hi0 = __umulhi(M0, c.x), lo0 = M0 * c.x;
-    const uint32_t hi1 = __umulhi(M1, c.z), lo1 = M1 * c.z;
-    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-    k0 += W0;
-    k1 += W1;
+    c = philox_round(c, k0, k1);
+    k0 += kPhiloxW0;
+    k1 += kPhiloxW1;
   }
+  return c;
+}
+
+// Philox4x32-10 of the counters (x, y, z, w) of one thread that share words x and y: its draws of one stream and row
+// on successive cells.  The key schedule and the part of round 0 that reads x and y alone are formed once
+// (philox_xy); each draw (philox_zw) forms the rest.  XOR is associative, so the words are philox4x32_10's.
+struct PhiloxXY {
+  uint32_t k0[10], k1[10];  // the key words of each round
+  uint32_t yk;              // y ^ k0[0]:               round 0's first word is umulhi(M1, z) ^ yk
+  uint32_t hx;              // umulhi(M0, x) ^ k1[0]:   its third is hx ^ w
+  uint32_t lx;              // M0 x:                    its fourth
+};
+
+__device__ __forceinline__ PhiloxXY philox_xy(uint32_t x, uint32_t y, uint32_t k0, uint32_t k1) {
+  PhiloxXY s;
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    s.k0[i] = k0;
+    s.k1[i] = k1;
+    k0 += kPhiloxW0;
+    k1 += kPhiloxW1;
+  }
+  s.yk = y ^ s.k0[0];
+  s.hx = __umulhi(kPhiloxM0, x) ^ s.k1[0];
+  s.lx = kPhiloxM0 * x;
+  return s;
+}
+
+__device__ __forceinline__ uint4 philox_zw(const PhiloxXY& s, uint32_t z, uint32_t w) {
+  uint4 c = make_uint4(__umulhi(kPhiloxM1, z) ^ s.yk, kPhiloxM1 * z, s.hx ^ w, s.lx);
+#pragma unroll
+  for (int i = 1; i < 10; ++i) c = philox_round(c, s.k0[i], s.k1[i]);
   return c;
 }
 

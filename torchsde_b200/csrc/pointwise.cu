@@ -412,7 +412,7 @@ __device__ __forceinline__ bool pw_begin(const PwProg<T>& pg, const PwP<T>& p, c
 
 // CHANNEL / ROW operand quads a compiled program keeps in registers for the whole chunk (loaded once per launch after
 // the dependency wait); any past these are loaded again at every step.  Within the launch bounds below, cfg2's program
-// (two CHANNEL operands) takes 41 registers in fp32.
+// (two CHANNEL operands) takes 54 registers in fp32.
 constexpr int kPwJitHoistQuads[2] = {4, 2};  // float, double
 
 // The compiled kernels run at the resident CTAs per SM the interpreted Milstein kernel had (58-59 registers in fp32,
@@ -1525,6 +1525,22 @@ static int pw_steps(const tsde_pw_step* steps, int32_t n_steps, PwP<T>& p, Noise
     if (s.y1 && !aligned16(s.y1)) p.vec = 0;
     st.s[j] = PwStep<T>{s.cell_id, static_cast<const T*>(s.t0), static_cast<T*>(s.y1), (T)sqrt(s.h), (T)s.dt};
   }
+  // a uniform grid (PwSteps::uniform): consecutive cells, one sqrt_h and dt, and evenly spaced times and
+  // destinations, every step stored
+  const tsde_pw_step& s0 = steps[0];
+  const auto at = [](const void* x) { return (intptr_t)x; };
+  const intptr_t dy = n_steps > 1 ? at(steps[1].y1) - at(s0.y1) : 0, dt0 = n_steps > 1 ? at(steps[1].t0) - at(s0.t0) : 0;
+  bool uniform = np.n_cells == 1 && !np.bcast && p.vec && dy % (intptr_t)sizeof(T) == 0 &&
+                 dt0 % (intptr_t)sizeof(T) == 0;
+  for (int j = 0; j < n_steps && uniform; ++j) {
+    const tsde_pw_step& s = steps[j];
+    uniform = s.y1 && s.cell_id == s0.cell_id + (uint64_t)j && !memcmp(&st.s[j].sqrt_h, &st.s[0].sqrt_h, sizeof(T)) &&
+              !memcmp(&st.s[j].dt, &st.s[0].dt, sizeof(T)) && at(s.y1) == at(s0.y1) + j * dy &&
+              at(s.t0) == at(s0.t0) + j * dt0;
+  }
+  st.uniform = uniform ? 1 : 0;
+  st.y1_stride = dy / (intptr_t)sizeof(T);
+  st.t0_stride = dt0 / (intptr_t)sizeof(T);
   np.cell_id = steps[0].cell_id;
   np.h = steps[0].h;
   return 0;

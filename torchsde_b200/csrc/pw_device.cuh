@@ -267,6 +267,11 @@ template <typename T>
 struct PwSteps {  // by value: a captured launch carries the whole table
   int32_t n;
   PwStep<T> s[kPwMaxSteps];
+  // A uniform grid (pw_steps): every step drawn from one Brownian cell, cell s[0].cell + j, stored to
+  // s[0].y1 + j y1_stride, run at s[0].t0 + j t0_stride, with s[0]'s sqrt_h and dt; the noise is not broadcast and
+  // every quad is whole (p.vec).  pw_milstein_steps runs such a chunk without reading the table step by step.
+  int32_t uniform;
+  int64_t y1_stride, t0_stride;  // in elements
 };
 
 // ---- consecutive Milstein steps of a compiled program ----------------------------------------
@@ -301,6 +306,58 @@ __device__ __forceinline__ void pw_milstein_step(Prog& prog, const PwOperands<T>
   }
 }
 
+// A program compiled as relocatable device code calls its transcendental ops out of line (pointwise.cu, kPwHelpers),
+// and every register live across a call is saved to the stack around it: a second step loop, with the Philox
+// schedule live across the calls, would grow its kernels' call frame.  Its chunks all run through the step table.
+#ifdef __CUDACC_RDC__
+constexpr bool kPwCalls = true;
+#else
+constexpr bool kPwCalls = false;
+#endif
+
+// pw_milstein_steps on a uniform grid (st.uniform), with `ito` fixed: the launch constants are read once, and the loop
+// has one back-edge, no per-step branch and no indexed read of the step table.  Step j's PwStep is built in registers
+// (the program reads it as it reads a table entry) and its increment is drawn as counter_noise draws it; in fp32 on a
+// Philox whose key schedule and the counter words fixed for the thread are formed once (philox_xy).
+template <typename T, typename Prog, int ITO>
+__device__ __forceinline__ void pw_milstein_uniform(const PwOperands<T>& ops, const PwP<T>& p, const NoiseP<T>& nz,
+                                                    const PwSteps<T>& st) {
+  PwQuad c;
+  int64_t Q, row, q;
+  pw_locate(p, c, Q, row, q);
+  c.vec = true;
+  const Key key = load_key(nz.key);
+  const uint32_t grow = (uint32_t)(row + nz.row_offset);
+  const PhiloxXY ph = philox_xy((uint32_t)q | (STREAM_W << 24), grow, key.lo, key.hi);
+  PwStep<T> s = st.s[0];
+  T w[4], y[4];
+  auto draw = [&]() {
+    T n[4];
+    if constexpr (sizeof(T) == 4)
+      box_muller4(philox_zw(ph, (uint32_t)s.cell, (uint32_t)(s.cell >> 32)), n);
+    else  // (fp64 draws two counters per quad, which differ in word x)
+      normal4(key, s.cell, STREAM_W, grow, (uint32_t)q, n);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) w[i] = n[i] * s.sqrt_h;
+  };
+  draw();  // the first increment is drawn while the previous kernel drains
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  if (Q >= p.nquads) return;
+  Prog prog;
+  ld4(p.y0 + c.base, y);
+  prog.load(ops, c);
+  T* y1 = s.y1 + c.base;
+  for (int j = 1;; ++j) {
+    pw_milstein_step<T>(prog, ops, c, s, ITO, w, y);
+    st4(y1, y);
+    if (j == st.n) break;
+    ++s.cell;
+    s.t0 += st.t0_stride;
+    y1 += st.y1_stride;
+    draw();
+  }
+}
+
 // Per step: pw_milstein_step on the state the step before left in registers.  A quad's trajectory depends on nothing but its own state (element-wise SDE, diagonal noise), so one thread runs the
 // whole chunk: y0 is read once, y stays in registers from one step to the next and is stored only where the step table
 // gives it a destination (an output row, the chunk's last state).  The unfused step moves 13 tensors; a chunk moves one
@@ -314,6 +371,13 @@ __device__ __forceinline__ void pw_milstein_step(Prog& prog, const PwOperands<T>
 template <typename T, int SRC, typename Prog>
 __device__ __forceinline__ void pw_milstein_steps(const PwOperands<T>& ops, const PwP<T>& p, const NoiseP<T>& nz,
                                                   const PwSteps<T>& st) {
+  if (SRC == TSDE_SRC_COUNTER && !kPwCalls && st.uniform) {
+    if (p.ito)
+      pw_milstein_uniform<T, Prog, 1>(ops, p, nz, st);
+    else
+      pw_milstein_uniform<T, Prog, 0>(ops, p, nz, st);
+    return;
+  }
   PwQuad c;
   int64_t Q, row, q;
   pw_locate(p, c, Q, row, q);
