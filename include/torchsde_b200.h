@@ -143,6 +143,9 @@ const char* tsde_error_string(int code);
                                      (GENERAL launches of tsde_solve_euler_pointwise,
                                      tsde_solve_reversible_heun_pointwise, tsde_step_predictor_corrector_pointwise
                                      and tsde_step_srk_diag_pointwise)                                           */
+#define TSDE_KERNEL_PW_ADJOINT 9  /* backward steps of the reversible-Heun adjoint with an element-wise SDE, up to
+                                     TSDE_PW_MAX_STEPS per launch (tsde_solve_reversible_heun_pointwise with a
+                                     TSDE_PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN program)                            */
 int64_t tsde_kernel_launches(int32_t family);
 
 
@@ -558,6 +561,70 @@ enum { TSDE_PW_DM = 5, TSDE_PW_M = 6 };
  */
 #define TSDE_PW_LAYOUT_GENERAL_EULER_HEUN 3      /* tsde_pointwise.reserved for the general Euler-Heun step     */
 #define TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN 4 /* tsde_pointwise.reserved for general reversible-Heun chunks */
+
+/*
+ * The backward sweep of the reversible-Heun adjoint (reversible_heun.py:98-144, adjoint.py:97-119) for a diagonal-noise
+ * SDE whose f(t, y) and g(t, y) are element-wise programs.  tsde_solve_reversible_heun_pointwise on a DIAGONAL launch,
+ * for a program tagged reserved = TSDE_PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN (the `prog` member of a tsde_pw_adjoint, whose
+ * other members it reads), runs `n_steps` consecutive backward steps as one launch.  Each thread reads its quad of the
+ * augmented state once, (y, z, f, g) from y0, z0, f0, g0 and (adj_y, adj_f, adj_g, adj_z) from adj_in[], and per
+ * step, in reversed time,
+ *     z1, adj_f_mid, adj_g_mid as tsde_adjoint_reversible_heun_a (dt, half_dt);
+ *     vjp_z and one contribution per parameter: the program's vjp with seeds (adj_f_mid, adj_g_mid) of f and g at the
+ *       state z the step starts from (evaluated at (steps[j-1].t0, z), or (t0, z) for the chunk's first step);
+ *     f1, g1 at (steps[j].t0, z1): steps[j].t0 is the forward time of the step's end;
+ *     y, adj_y, adj_z, adj_f, adj_g as tsde_adjoint_reversible_heun_b (dt, half_dt); (z, f, g) <- (z1, f1, g1);
+ *     when steps[j].y1 is not NULL (the step ends an output interval; it points at row k of ys, ys + k rows d):
+ *       y <- ys[k], adj_y <- adj_y + grad_ys[k]
+ * in registers, with half_dt = 0.5 * dt rounded once to the state dtype.  The state after the last step is stored
+ * once, to y1, z1, f1, g1 and adj_out[], which must not overlap what the chunk reads.  Every stored value equals the
+ * unfused sweep's (kernels A and B around the user's f, g and torch.autograd.grad) bit for bit when (state dtype) 0.5 *
+ * (state dtype) dt is the unfused step's half_dt, which holds unless it is subnormal.  Parameter gradients are not
+ * formed here: the chunk sums each parameter's contributions over its steps in registers, in step order, and adds that
+ * sum to partial[k], a (rows, d) tensor, once, element-wise; the caller reduces each partial over the batch once per
+ * sweep.  Nothing is accumulated with atomics, so every result is the same from run to run.  ys and grad_ys are
+ * contiguous (n_out, rows, d) series of the state dtype.  The noise is that of tsde_solve_milstein_pointwise
+ * (steps[j].cell_id, h; a step spanning several cells runs alone), on the global row (nz->row_offset).  The launches
+ * count under TSDE_KERNEL_PW_ADJOINT.
+ *
+ * Program: prog holds f and g in [0, n_fg) with results f_src and g_src, as the Milstein layout; [n_fg, n_instr) is the
+ * vjp, whose seeds are TSDE_PW_SRC_GO (f's cotangent) and TSDE_PW_SRC_GO2 (g's), with vjp_z in gdg_src and parameter
+ * k's contribution in param_src[k] (0 <= n_params <= TSDE_PW_ADJ_MAX_PARAMS).  A contribution is the (rows, d) value
+ * whose batch reduction is that parameter's gradient: the value itself for a (rows, d) parameter.  The program is
+ * compiled at run time into a kernel of its own, as the Milstein programs are (one translation unit per structure,
+ * n_params and dtype), with the library's IEEE options; tsde_pointwise_compile compiles and loads it for a DIAGONAL
+ * launch without launching (call it before a stream capture) and tsde_pointwise_source writes out its source.
+ *
+ * Launch: 256 threads per CTA, bounded at one resident CTA per SM (__launch_bounds__(256, 1)), no shared memory.  The
+ * kernel holds 8 state quads, the program's registers and one accumulator quad per parameter.  Measured on sm_90a
+ * (ptxas of CUDA 12.9 on the generated source, DESIGN section 3): the program of profiles/adjoint_pointwise_probe.py
+ * (f = mu*y - sigma*(sigma*(0.5*y)), g = sigma*y, (d,) mu and sigma) takes 121 / 102 registers (single- / multi-cell
+ * kernel) in fp32 and 198 / 190 in fp64, with no spills.
+ * TSDE_EINVAL, before anything is compiled or launched: a launch that is not DIAGONAL with m == d, noise other than
+ * counter noise or with flags, 16-bit formats, an invalid program (tsde_pointwise_compile's checks with the second
+ * seed, a bad n_params or param_src), n_steps outside [1, TSDE_PW_MAX_STEPS], a step spanning several cells in a chunk
+ * of more than one, a null t0, steps[j].t0, state pointer, ys, grad_ys or partial[k], and a steps[j].y1 that is not one
+ * of the n_out rows of ys.  The tag is valid only on the `prog` member of a tsde_pw_adjoint: the library reads the
+ * whole struct behind a program so tagged.  An empty batch is a no-op.
+ */
+#define TSDE_PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN 5 /* tsde_pointwise.reserved of a tsde_pw_adjoint's program */
+#define TSDE_PW_ADJ_MAX_PARAMS 8
+#define TSDE_PW_SRC_GO2 0xFD
+typedef struct tsde_pw_adjoint {
+  tsde_pointwise prog;
+  int32_t n_params;
+  int32_t reserved;
+  uint8_t param_src[TSDE_PW_ADJ_MAX_PARAMS];
+  /* DEVICE buffers of a launch */
+  const void* t0;                             /* 0-d forward time of the chunk's first forward values (state dtype) */
+  const void* adj_in[4];                      /* adj_y, adj_f, adj_g, adj_z the chunk starts from                   */
+  void*       y1;                             /* where the chunk leaves y                                           */
+  void*       adj_out[4];                     /* and adj_y, adj_f, adj_g, adj_z                                     */
+  const void* ys;                             /* the output series and its cotangent, (n_out, rows, d)              */
+  const void* grad_ys;
+  int64_t     n_out;
+  void*       partial[TSDE_PW_ADJ_MAX_PARAMS];
+} tsde_pw_adjoint;
 
 /* derivative-free Milstein, predictor: y' = y0 + (Ito ? dt*f : 0) + g*sqrt_dt
  * methods/milstein.py:58-63,83-84,93-94.  g is (rows,d) also for scalar noise (squeezed). */

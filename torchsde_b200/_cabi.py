@@ -116,6 +116,7 @@ KERNEL_PW_PC = 5  # TSDE_KERNEL_PW_PC
 KERNEL_PW_CHUNK = 6  # TSDE_KERNEL_PW_CHUNK
 KERNEL_PW_ADAPTIVE = 7  # TSDE_KERNEL_PW_ADAPTIVE
 KERNEL_PW_GENERAL = 8  # TSDE_KERNEL_PW_GENERAL
+KERNEL_PW_ADJOINT = 9  # TSDE_KERNEL_PW_ADJOINT
 PW_GENERAL_MAX_M = 32  # TSDE_PW_GENERAL_MAX_M
 PW_LAYOUT_GENERAL = 1  # TSDE_PW_LAYOUT_GENERAL: Pointwise.reserved of a general-noise program
 PW_LAYOUT_GENERAL_SRA = 2  # TSDE_PW_LAYOUT_GENERAL_SRA: Pointwise.reserved of a general-noise program of an sra1 step
@@ -126,6 +127,9 @@ PW_LAYOUT_GENERAL_REVERSIBLE_HEUN = 4  # TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN:
  PROPOSAL_EULER_HEUN) = range(7)
 PC_HEUN, PC_MIDPOINT, PC_EULER_HEUN = range(3)  # TSDE_PC_*
 PW_MAX_STEPS = 64  # TSDE_PW_MAX_STEPS
+PW_ADJ_MAX_PARAMS = 8  # TSDE_PW_ADJ_MAX_PARAMS
+PW_SRC_GO2 = 0xFD  # TSDE_PW_SRC_GO2: the adjoint layout's second vjp seed (g's cotangent)
+PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN = 5  # TSDE_PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN: ... of a PwAdjoint's program
 
 
 class PwInstr(ctypes.Structure):
@@ -147,6 +151,16 @@ class Pointwise(ctypes.Structure):
 class PwStep(ctypes.Structure):
     _fields_ = [('cell_id', ctypes.c_uint64), ('h', ctypes.c_double), ('dt', ctypes.c_double), ('t0', ctypes.c_void_p),
                 ('y1', ctypes.c_void_p)]
+
+
+class PwAdjoint(ctypes.Structure):
+    """tsde_pw_adjoint: a program tagged PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN and the buffers of one launch (the entry
+    points take `prog`, the first member)."""
+    _fields_ = [('prog', Pointwise), ('n_params', ctypes.c_int32), ('reserved', ctypes.c_int32),
+                ('param_src', ctypes.c_uint8 * PW_ADJ_MAX_PARAMS), ('t0', ctypes.c_void_p),
+                ('adj_in', ctypes.c_void_p * 4), ('y1', ctypes.c_void_p), ('adj_out', ctypes.c_void_p * 4),
+                ('ys', ctypes.c_void_p), ('grad_ys', ctypes.c_void_p), ('n_out', ctypes.c_int64),
+                ('partial', ctypes.c_void_p * PW_ADJ_MAX_PARAMS)]
 
 
 class PwSubstep(ctypes.Structure):

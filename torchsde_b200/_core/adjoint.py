@@ -16,7 +16,10 @@ _core/adjoint_sde.py (the augmented backward SDE).
   with the Brownian increment of the step regenerated from the Philox counter in both kernels (the same cells the
   forward pass consumed, addressed in reverse: `ReverseBrownian` semantics, _brownian/derived.py:27-30).  The sweep
   can be captured as a CUDA graph (`adjoint_options={'cuda_graph': True}`); with `adjoint_adaptive=True` it runs the
-  reference's adaptive controller on the augmented state (`_BackwardEngine.run_adaptive`).
+  reference's adaptive controller on the augmented state (`_BackwardEngine.run_adaptive`).  With
+  `adjoint_options={'fused_backward': True}` and an element-wise diagonal-noise SDE, the first step is recorded
+  (pointwise.AdjointRecorder) and the whole sweep runs as chunks of up to TSDE_PW_MAX_STEPS steps per kernel
+  (`_BackwardEngine._fused_sweep`).
 * Every other pair: the generic `AdjointSDE` (adjoint_sde.py) integrated backwards by the ordinary solvers on the flat
   augmented state (`_generic_backward`).
 * Double backward (create_graph=True): the generic path re-enters `_SdeintAdjointMethod.apply` per interval exactly
@@ -31,6 +34,7 @@ from torch import nn
 
 from . import base_solver
 from . import methods
+from . import pointwise
 from . import schedule as schedule_lib
 from . import sdeint as sdeint_mod
 from .base_sde import widen
@@ -75,10 +79,14 @@ class _BackwardEngine(base_solver.BaseSDESolver):
     noise_types = NOISE_TYPES.all()
     levy_area_approximations = LEVY_AREA_APPROXIMATIONS.all()
 
-    def __init__(self, sde, bm, dt, params):
+    _pw_method = 'adjoint_reversible_heun'  # (pointwise.chunk_length)
+
+    def __init__(self, sde, bm, dt, params, adjoint_options=None):
         super(_BackwardEngine, self).__init__(sde=sde, bm=bm, dt=dt, adaptive=False, rtol=None, atol=None,
                                               dt_min=None, options={})
         self.params = list(params)
+        self.adjoint_options = adjoint_options or {}
+        self._pw = None  # the fused sweep's program (pointwise.AdjointRecorder.finish), False when it cannot fuse
 
     def aux_times(self, t0, t1, dt):
         return [-t0, -t1]  # forward-time arguments of f_and_g (reversible_heun.py:122,133)
@@ -139,6 +147,10 @@ class _BackwardEngine(base_solver.BaseSDESolver):
 
     def _sweep(self, ys, grad_ys, extras, grad_extras, params):
         self._refresh_stream()
+        if self.adjoint_options.get('fused_backward', False) and self._pw is not False:
+            out = self._fused_sweep(ys, grad_ys, extras, grad_extras, params)
+            if out is not None:
+                return out
         L = self._L
         T = self.T
         y = _contig(ys[-1])
@@ -205,6 +217,84 @@ class _BackwardEngine(base_solver.BaseSDESolver):
             y = _contig(ys[i - 1])
             adj_y = adj_y + grad_ys[i - 1]
         return adj_y, (adj_f, adj_g, adj_z), adj_params
+
+    # ---- the fused sweep (adjoint_options={'fused_backward': True}) -------------------------------------------
+    def _record(self, ys, grad_ys, extras, grad_extras, params):
+        """The first backward step, run the ordinary way (kernel A, f and g, the vjp, f and g again) under an
+        AdjointRecorder; its results are discarded: the chunks start from the same state."""
+        c = self.ctxs[0]
+        y = _contig(ys[-1])
+        f0, g0, z0 = (_contig(x.detach()) for x in extras)
+        adj_f, adj_g, _ = (_contig(x) for x in grad_extras)
+        z1, adj_f_mid, adj_g_mid = torch.empty_like(y), torch.empty_like(adj_f), torch.empty_like(adj_g)
+        self._half('tsde_adjoint_reversible_heun_a', self._L, self._feed.get(c),
+                   (y, z0, f0, g0, _contig(grad_ys[-1]), adj_f, adj_g), (c.dt, c.scalars['half_dt']),
+                   (z1, adj_f_mid, adj_g_mid))
+        t_fwd0, t_fwd1 = c.aux_t
+        sde = self.sde
+        with torch.enable_grad():
+            z0r = z0.detach().requires_grad_()
+            rec = pointwise.AdjointRecorder(z0r, t_fwd0, len(params),
+                                            bool(self.adjoint_options.get('transcendental', False)))
+            re_f0, re_g0 = rec.forward(lambda: sde.f_and_g(t_fwd0, z0r))
+            pairs = [(o, go) for o, go in ((re_f0, adj_f_mid), (re_g0, adj_g_mid)) if o.requires_grad]
+            if not pairs:
+                rec.reject("f and g depend on neither the state nor a parameter")
+                return rec
+            rec.vjp(lambda: torch.autograd.grad([widen(o, go.dtype) for o, go in pairs], [z0r] + list(params),
+                                                [go.view_as(o) for o, go in pairs], allow_unused=True),
+                    adj_f_mid, adj_g_mid, params)
+            z1r = z1.detach().requires_grad_()
+            rec.again(lambda: sde.f_and_g(t_fwd1, z1r), t_fwd1, z1r)
+        return rec
+
+    def _fused_sweep(self, ys, grad_ys, extras, grad_extras, params):
+        """The sweep as chunks of the adjoint program (tsde_solve_reversible_heun_pointwise), or None (after a warning
+        with the reason) when it cannot fuse.  Records and compiles the program on first use: under graph capture that
+        is the warm-up sweep (_backward_plan), and the captured sweep only launches chunks and the final reductions."""
+        y = _contig(ys[-1])
+        state = [y] + [_contig(x.detach()) for x in (extras[2], extras[0], extras[1])] + \
+            [_contig(grad_ys[-1])] + [_contig(x) for x in grad_extras]   # y, z, f, g, adj_y, adj_f, adj_g, adj_z
+        if self._pw is None:
+            reason = pointwise.adjoint_refusal(self, self.adjoint_options)
+            if reason is None and not pointwise.state_fits(self, state[2:4] + state[1:2]):
+                reason = "the solver state (f0, g0, z0) is not made of (rows, d) tensors of the state dtype"
+            if reason is None and any(s.n_steps == 0 for s in self.scheds):
+                reason = "an output interval without steps"
+            res = None
+            if reason is None:
+                rec = self._record(ys, grad_ys, extras, grad_extras, params)
+                res = pointwise.compile_adjoint(rec, rec.finish())
+                reason = rec.reason
+            self._pw = res or False
+            if not res:
+                warn_unfused(reason)
+                return None
+        self._out = []  # per step: the output index whose row the step ends on, or -1
+        for n, sched in enumerate(self.scheds):
+            self._out += [-1] * (sched.n_steps - 1) + [self.T - 2 - n]
+        n_steps = len(self._out)
+        kinds = self._pw[2]
+        partials = [torch.zeros_like(y) for kind in kinds if kind is not None]
+        ys_c, gys_c = _contig(ys), _contig(grad_ys)
+        multi = [k for k in range(n_steps) if self.binding.cell(self.ctxs[k].k)[2] > 1]
+        chunks = pointwise.plan_chunks(0, n_steps, multi_cell=multi, max_steps=pointwise.chunk_length(self))
+        # a chunk stores its state to the set it did not read: the caller's tensors are read once, so a sweep of one
+        # chunk needs one set, any other two
+        sets = [[torch.empty_like(y) for _ in state] for _ in range(min(len(chunks), 2))]
+        for j, (k0, k1) in enumerate(chunks):
+            t0 = self.ctxs[0].aux_t[0] if k0 == 0 else self.ctxs[k0 - 1].aux_t[1]
+            pointwise.solve_adjoint_chunk(self, range(k0, k1), t0, state, sets[j % 2], ys_c, gys_c, partials)
+            state = sets[j % 2]
+        # each parameter's contributions, reduced once over the batch as autograd's sum_to reduces one step's
+        adj_params = [torch.zeros_like(p) for p in params]
+        live = iter(partials)
+        for ap, kind in zip(adj_params, kinds):
+            if kind is not None:
+                part = next(live)
+                ap.add_((part.sum(0) if kind == pointwise.REDUCE_ROWS else
+                         part.sum() if kind == pointwise.REDUCE_ALL else part).view_as(ap))
+        return state[4], (state[5], state[6], state[7]), adj_params
 
     def run(self, ys, ts, grad_ys, extras, grad_extras):
         self.plan(ys, ts)
@@ -312,6 +402,15 @@ class _BackwardEngine(base_solver.BaseSDESolver):
 
 
 _BWD_PLANS = __import__('weakref').WeakKeyDictionary()
+_WARNED = set()
+
+
+def warn_unfused(reason):
+    """adjoint_options={'fused_backward': True} was given, but the sweep keeps its unfused steps: say why, once per
+    reason."""
+    if reason not in _WARNED:
+        _WARNED.add(reason)
+        warnings.warn(f"sdeint_adjoint: the backward sweep keeps its unfused steps ({reason}).")
 
 
 def drop_plans(sde):
@@ -336,8 +435,11 @@ def _backward_plan(engine, ys, ts, extras):
     if binding is None or names is None:
         return None
     sde_obj, _ = graph_mod.cache_owner(engine.sde)
+    # (the adjoint options decide what the sweep launches: a plan captured with fused_backward must not serve a solve
+    # without it, nor the other way round)
     key = ('bwd',) + graph_mod._plan_key(engine, ys[0], ts, tuple(extras), binding) + (
-        tuple(tuple(p.shape) for p in engine.params),)
+        tuple(tuple(p.shape) for p in engine.params),
+        tuple(sorted((k, repr(v)) for k, v in engine.adjoint_options.items() if k != 'cuda_graph')))
     plans = graph_mod.plans_of(_BWD_PLANS, sde_obj)
     if plans is None:
         return None
@@ -516,7 +618,7 @@ class _SdeintAdjointMethod(torch.autograd.Function):
         ctx.bwd_plan = None
         if adjoint_options.get('cuda_graph', False) and isinstance(bm, BrownianInterval) \
                 and adjoint_options_reversible(adjoint_options) and adjoint_options.get('_adaptive') is None:
-            engine = _BackwardEngine(sde, ReverseBrownian(bm), dt, params)
+            engine = _BackwardEngine(sde, ReverseBrownian(bm), dt, params, adjoint_options)
             ctx.bwd_plan = _backward_plan(engine, ys, ts, extras_out)
         # (y0 and the initial solver state are saved as well: the differentiable backward of the reversible pair
         # re-runs the solve from the Function's INPUTS, see _reversible_backward_differentiable)
@@ -548,6 +650,9 @@ class _SdeintAdjointMethod(torch.autograd.Function):
             return (None, None, None, None, None, None, None, None, adj_y, *([None] * ctx.n_extras), *adj_params)
         # (the adjoint state is kept in the state dtype also for 16-bit solver state (f0, g0))
         grad_extras = [widen(torch.zeros_like(e) if g is None else g, ys.dtype) for g, e in zip(grad_extras, extras)]
+        if ctx.adjoint_options.get('fused_backward', False) and (differentiable or
+                                                                 ctx.adjoint_options.get('_adaptive') is not None):
+            warn_unfused("create_graph (double backward)" if differentiable else "adjoint_adaptive")
         if differentiable:
             adj_y, adj_extras, adj_params = _reversible_backward_differentiable(
                 ctx.sde, ctx.bm, ctx.dt, ts, y0_in, extras_in, list(params), grad_ys, grad_extras)
@@ -561,7 +666,7 @@ class _SdeintAdjointMethod(torch.autograd.Function):
                 adj_y, adj_extras, adj_params = _replay_backward(ctx.bwd_plan, ctx.bm, ys, grad_ys, extras,
                                                                  grad_extras)
             else:
-                engine = _BackwardEngine(ctx.sde, ReverseBrownian(ctx.bm), ctx.dt, params)
+                engine = _BackwardEngine(ctx.sde, ReverseBrownian(ctx.bm), ctx.dt, params, ctx.adjoint_options)
                 adj_y, adj_extras, adj_params = engine.run(ys, ts, grad_ys, extras, grad_extras)
         return (None, None, None, None, None, None, None, None, adj_y, *adj_extras, *adj_params)
 

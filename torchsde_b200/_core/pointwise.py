@@ -123,6 +123,19 @@ _REVERSIBLE_HEUN (the solver's `_pw_layout`: reversible Heun's pattern is Euler'
 tsde_step_predictor_corrector_pointwise per Euler-Heun step, and as chunks of tsde_solve_reversible_heun_pointwise whose
 solver state holds g as (rows, d, m), kept in registers within a chunk; `sdeint_adjoint`'s forward solve fuses too.
 Heun and every other method keep diagonal-only tapes.
+
+The reversible adjoint's backward sweep (`AdjointRecorder`, `compile_adjoint`, `solve_adjoint_chunk`), with
+`sdeint_adjoint(..., adjoint_options={'fused_backward': True})`.  Its first backward step runs the ordinary way under
+the recorder in three segments: f and g at (t0, z0); torch.autograd.grad of both with respect to z0 and the parameters
+with two seeds (GO, f's cotangent, and GO2, g's); f and g at (t1, z1), which must be the first segment's program.  The
+program's results are f, g, vjp_z and one contribution per parameter: the (rows, d) value whose batch reduction autograd
+returns as that parameter's gradient (on a parameter's path the tape holds autograd's sum_to reductions, views and the
+`add` of two of them, nothing else).  It is tagged PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN, compiled right after recording,
+and every step of the sweep then runs in chunks of tsde_solve_reversible_heun_pointwise, each contribution summed in
+registers and added once per chunk to a (rows, d) partial that the sweep reduces over the batch once at its end
+(adjoint._BackwardEngine._fused_sweep).  y, the adjoint state and y0's gradient are the unfused sweep's bits; parameter
+gradients differ by summation order only.  Only diagonal noise on a bound grid, without logqp, autocast, overlap=False,
+adjoint_adaptive, create_graph or a user f_and_g (`adjoint_refusal`); anything else keeps the unfused sweep and warns.
 """
 import ctypes
 import numbers
@@ -174,7 +187,7 @@ _BACKWARD = {aten.tanh_backward.default: _cabi.PW_TANH_BACKWARD,
 _ALIAS = {aten.view.default, aten._unsafe_view.default, aten.expand.default, aten.unsqueeze.default,
           aten.detach.default, aten.alias.default}
 
-Y, GO, T0 = ('y',), ('go',), ('t0',)
+Y, GO, GO2, T0 = ('y',), ('go',), ('go2',), ('t0',)
 STALE = ('stale',)  # a tensor whose storage was written in place through another tensor
 FOREIGN = ('foreign',)  # a value bound by an earlier evaluation of an SRK step
 
@@ -236,6 +249,8 @@ def _allocate(instrs, reads):
             return _cabi.PW_SRC_Y
         if s == GO:
             return _cabi.PW_SRC_GO
+        if s == GO2:
+            return _cabi.PW_SRC_GO2
         if s[0] == 'k':
             return _cabi.PW_OPERAND0 + s[1]
         return reg[s]
@@ -321,6 +336,17 @@ class Recorder(TorchDispatchMode):
     def reject(self, reason):
         if self.ok:
             self.ok, self.reason = False, reason
+
+    def _isolate(self):
+        """Make every value bound so far (a state, a time, an intermediate) foreign to what is recorded next; a view of
+        an operand is an operand again."""
+        for table in (self._by_obj, self._by_addr):
+            for key, src in list(table.items()):
+                if src[0] == 'k':
+                    del table[key]
+                    self._storage.pop(key, None)
+                else:
+                    table[key] = FOREIGN
 
     def __torch_dispatch__(self, func, types, args=(), kwargs=None):
         kwargs = kwargs or {}
@@ -601,7 +627,7 @@ class Recorder(TorchDispatchMode):
         if not torch.is_tensor(t) or tuple(t.shape) != (self.rows, self.d) or t.dtype != self.dtype:
             raise Reject("a result is not a (rows, d) tensor of the state dtype")
         src = self._source(t)
-        if src[0] == 'k' or src == GO and not allow_go:
+        if src[0] == 'k' or src in (GO, GO2) and not allow_go:
             raise Reject("a result is not computed from the state")
         return src
 
@@ -696,13 +722,7 @@ class SrkRecorder(Recorder):
         """fn(), the SDE's f (`kind` 'f') or g ('g') at (t, y), with its ATen ops recorded.  Every value bound by an
         earlier evaluation (its state, its time, its intermediates) is foreign to this one; a view of an operand is
         an operand again."""
-        for table in (self._by_obj, self._by_addr):
-            for key, src in list(table.items()):
-                if src[0] == 'k':
-                    del table[key]
-                    self._storage.pop(key, None)
-                else:
-                    table[key] = FOREIGN
+        self._isolate()
         start = len(self.instrs)
         out = self._run(fn, y, t)
         if self.ok:
@@ -997,9 +1017,9 @@ def plan_chunks(first, n_steps, interpolated=(), multi_cell=(), max_steps=_cabi.
 # sm_90a: 64 K registers per SM): Milstein's compiled kernels are pinned there by their launch bounds (256, 4) and
 # (256, 2) (cfg2's program: 54 registers in fp32); Euler at 54 and 88-96; reversible Heun at 72 and 110-120.
 # The compiled general-noise Euler and reversible-Heun kernels are bounded at (256, 1): at least one resident CTA,
-# whatever m.
+# whatever m; so is the reversible-Heun adjoint's backward-step kernel, whatever its parameters.
 _RESIDENT_CTAS = {'milstein': (4, 2), 'euler': (4, 2), 'reversible_heun': (3, 2), 'euler_general': (1, 1),
-                  'reversible_heun_general': (1, 1)}
+                  'reversible_heun_general': (1, 1), 'adjoint_reversible_heun': (1, 1)}
 
 
 def chunk_length(solver):
@@ -1131,3 +1151,272 @@ def propose(solver, method, curr_t, next_t, midpoint_t, y0):
                                                              subs, y_full.data_ptr(), y_next.data_ptr()),
                 "tsde_adaptive_proposal_pointwise")
     return y_full, y_next
+
+
+# ---- the reversible-Heun adjoint's backward sweep --------------------------------------------------------------------
+# How a parameter's gradient leaves the vjp: reduced over the rows (a (d,) parameter), over everything (one element),
+# or not at all (a (rows, d) parameter)
+REDUCE_ROWS, REDUCE_ALL, REDUCE_NONE = 'rows', 'all', 'none'
+_SUMS = (aten.sum.dim_IntList, aten.sum.default)
+
+
+class AdjointRecorder(Recorder):
+    """Records the first backward step of `sdeint_adjoint`'s reversible pair (adjoint._BackwardEngine) in three
+    segments: f and g at (t0, z0) (`forward`); torch.autograd.grad of [f, g] with respect to [z0] + params with seeds
+    GO (f's) and GO2 (g's) (`vjp`); f and g at (t1, z1) (`again`), which must be the first segment's program.  The
+    program is the first two: its results are f, g, vjp_z and one contribution per parameter, the (rows, d) value whose
+    batch reduction autograd returns as that parameter's gradient.  On a parameter's path the tape accepts only
+      * sum.dim_IntList / sum.default of a (rows, d) value over the rows or over everything (autograd's sum_to of a
+        (d,) or one-element parameter's gradient), views of that reduction, and `add` of two such reductions (a
+        parameter used twice), which becomes the element-wise sum of their contributions;
+      * a (rows, d) value itself, the gradient of a (rows, d) parameter;
+      * None, a parameter the step does not reach: no contribution.
+    Any other op on a reduced value (a parameter transformed before it is broadcast), more than
+    TSDE_PW_ADJ_MAX_PARAMS parameters, or anything the Milstein recorder rejects, rejects the tape."""
+
+    def __init__(self, z0, t0, n_params, transcendental=False):
+        super().__init__(z0, t0, transcendental)
+        self.reduced = []      # ('r', j) -> (kind, [contribution sources])
+        self.fg = self.fg3 = self.results = None
+        self._in_vjp = False   # a sum is a parameter's batch reduction only in the vjp segment
+        if n_params > _cabi.PW_ADJ_MAX_PARAMS:
+            self.reject(f"{n_params} parameters: at most {_cabi.PW_ADJ_MAX_PARAMS} are fused")
+
+    # -- the three segments ---------------------------------------------------------------------------------------
+    def _results(self, tensors):
+        try:
+            return [self._step_result(t) for t in tensors]
+        except Exception as e:
+            self.reject(f"{type(e).__name__}: {e}")
+            return None
+
+    def forward(self, fn):
+        """fn() = (f, g) at the state and time the recorder was made with."""
+        out = self._run(fn)
+        if self.ok:
+            self.fg = self._results(out)
+        self.n_fg = len(self.instrs)
+        return out
+
+    def vjp(self, fn, go, go2, params):
+        """fn() = autograd's gradients of [z0] + `params`, with seeds go and go2."""
+        for t, src in ((go, GO), (go2, GO2)):
+            self._bind(t, src)
+        self._in_vjp = True
+        try:
+            grads = self._run(fn)
+        finally:
+            self._in_vjp = False
+        if self.ok:
+            try:
+                self.results = self._contributions(grads, params)
+            except Exception as e:
+                self.reject(f"{type(e).__name__}: {e}")
+        self.n_vjp = len(self.instrs)
+        return grads
+
+    def again(self, fn, t1, z1):
+        """fn() = (f, g) at (t1, z1), with every value of the first two segments foreign."""
+        self._isolate()
+        self.start3 = len(self.instrs)
+        self._at(z1, t1)
+        out = self._run(fn)
+        if self.ok:
+            self.fg3 = self._results(out)
+        return out
+
+    def _contributions(self, grads, params):
+        """(vjp_z's source, [(reduction, contribution source) or None per parameter]); a parameter with several
+        contributions gets their sum, appended to the tape."""
+        vz = grads[0]
+        vz = self._operand(_cabi.PW_IMM, None, 0.0) if vz is None else self._step_result(vz, allow_go=True)
+        out = []
+        for p, gp in zip(params, grads[1:]):
+            if gp is None:
+                out.append(None)
+                continue
+            src = self._lookup(gp)
+            if src is not None and src[0] == 'r':
+                kind, srcs = self.reduced[src[1]]
+            elif tuple(gp.shape) == (self.rows, self.d) and tuple(p.shape) == (self.rows, self.d):
+                kind, srcs = REDUCE_NONE, [self._step_result(gp, allow_go=True)]
+            else:
+                raise Reject(f"the gradient of a {tuple(p.shape)} parameter is not a batch reduction of the tape")
+            acc = srcs[0]
+            for s in srcs[1:]:
+                acc = self._value(_cabi.PW_ADD, acc, s)
+            out.append((kind, acc))
+        return vz, out
+
+    # -- the ops on a parameter's path ----------------------------------------------------------------------------
+    def _lookup(self, x):
+        if not torch.is_tensor(x):
+            return None
+        src = self._by_obj.get(id(x))
+        return src if src is not None else self._by_addr.get(self._addr(x))
+
+    def _source(self, x):
+        src = super()._source(x)
+        if src == FOREIGN:
+            raise Reject("a value of another evaluation is read")
+        if src[0] == 'r':
+            raise Reject("a parameter's gradient is transformed after its batch reduction")
+        return src
+
+    def _record(self, func, args, kwargs, out):
+        if func in _SUMS and self._in_vjp:  # (a sum in f or g is rejected as any other reduction is)
+            self._reduce(args, kwargs, out)
+            return
+        tensors = [a for a in list(args) + list(kwargs.values()) if torch.is_tensor(a)]
+        reds = [self._lookup(a) for a in tensors]
+        reds = [r for r in reds if r is not None and r[0] == 'r']
+        if not reds:
+            return super()._record(func, args, kwargs, out)
+        if func in _ALIAS:
+            self._bind(out, reds[0])
+            return
+        alpha = kwargs.get('alpha', args[2] if len(args) > 2 else 1)
+        if func in (aten.add.Tensor, aten.add_.Tensor) and len(reds) == 2 == len(tensors) and alpha == 1 \
+                and not isinstance(alpha, bool):
+            (ka, a), (kb, b) = (self.reduced[r[1]] for r in reds)
+            if ka != kb:
+                raise Reject("two reductions of one parameter's gradient differ")
+            self.reduced.append((ka, a + b))
+            v = ('r', len(self.reduced) - 1)
+            if func is aten.add_.Tensor:
+                self._written(args[0])
+                self._bind(args[0], v)
+            self._bind(out, v)
+            return
+        raise Reject("a parameter's gradient is transformed after its batch reduction")
+
+    def _reduce(self, args, kwargs, out):
+        x = args[0]
+        if kwargs.get('dtype') is not None:
+            raise Reject("a reduction with a dtype")
+        src = self._number(x)
+        if tuple(x.shape) != (self.rows, self.d):
+            raise Reject(f"a reduction of a {tuple(x.shape)} value")
+        if out.numel() == 1:
+            kind = REDUCE_ALL
+        elif len(args) > 1 and sorted(int(k) % 2 for k in args[1]) == [0] and out.numel() == self.d:
+            kind = REDUCE_ROWS
+        else:
+            raise Reject(f"a reduction to {tuple(out.shape)}")
+        self._keep.append(out)
+        self.reduced.append((kind, [src]))
+        self._bind(out, ('r', len(self.reduced) - 1))
+
+    # -- the program -----------------------------------------------------------------------------------------------
+    def finish(self):
+        """(the tsde_pw_adjoint program, the tensors it reads, each parameter's reduction or None), or None if the tape
+        was rejected."""
+        if self.ok and (self.fg is None or self.results is None or self.fg3 is None):
+            self.reject("not the three segments of a backward step")
+        if not self.ok:
+            return None
+        try:
+            def rel(src, start):
+                return ('v', src[1] - start) if src is not None and src[0] == 'v' else src
+
+            def tape(start, end):
+                return [(op, *(rel(x, start) for x in srcs)) for op, *srcs in self.instrs[start:end]]
+            if tape(0, self.n_fg) != tape(self.start3, len(self.instrs)) or \
+                    [rel(x, 0) for x in self.fg] != [rel(x, self.start3) for x in self.fg3]:
+                raise Reject("the evaluations at (t0, z0) and (t1, z1) differ")
+            vz, contribs = self.results
+            live = [c for c in contribs if c is not None]
+            reads = [(self.n_fg, self.fg[0]), (self.n_fg, self.fg[1]), (self.n_vjp, vz)] + \
+                [(self.n_vjp, src) for _, src in live]
+            code, results, n_regs = _allocate(self.instrs[:self.n_vjp], reads)
+            n_fg = sum(1 for c in code if c[0] < self.n_fg)
+            prog, keep = self._program(code, n_fg, results[:3], n_regs, _cabi.PW_MAX_REGS)
+            ad = _cabi.PwAdjoint()
+            ad.prog = prog
+            ad.prog.reserved = _cabi.PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN
+            ad.n_params = len(live)
+            for k, src in enumerate(results[3:]):
+                ad.param_src[k] = src
+            return ad, keep, [None if c is None else c[0] for c in contribs]
+        except Exception as e:
+            self.reject(f"{type(e).__name__}: {e}")
+            return None
+
+
+def compile_adjoint(rec, res):
+    """`res`, what `rec.finish` returned, once its backward-step kernels are compiled and loaded
+    (tsde_pointwise_compile of the tagged program), on the recording step as for `compile_milstein`; None if `res` is,
+    or if the library refuses or cannot compile the program (the tape is then rejected with the reason)."""
+    global COMPILES
+    if res is None:
+        return None
+    ad = res[0]
+    src = _cabi.pointwise_source(ad.prog, rec.dtype)
+    if src is None:
+        rec.reject("the library refuses the program")
+        return None
+    done = _COMPILED.setdefault(_cabi.lib(), set())
+    if ('adjoint', src) not in done:
+        err = _cabi.compile_pointwise(ad.prog, rec.dtype)
+        if err != 0:
+            rec.reject(_cabi.lib().tsde_error_string(err).decode())
+            return None
+        done.add(('adjoint', src))
+        COMPILES += 1
+    return res
+
+
+def adjoint_refusal(engine, options, differentiable=False, adaptive=False):
+    """Why the backward sweep of `engine` (adjoint._BackwardEngine) with adjoint_options `options` keeps its unfused
+    steps although options={'fused_backward': True} asks for chunks, or None if it may record its first step."""
+    from .base_sde import SDELogqp
+    sde = engine.sde
+    obj = sde
+    while hasattr(obj, '_base_sde'):
+        obj = obj._base_sde
+        if isinstance(obj, SDELogqp):
+            return "logqp"
+    if differentiable:
+        return "create_graph (double backward)"
+    if adaptive:
+        return "adjoint_adaptive"
+    if sde.noise_type != NOISE_TYPES.diagonal:
+        return f"{sde.noise_type} noise (diagonal only)"
+    if getattr(engine, 'binding', None) is None:
+        return "the Brownian motion is not a BrownianInterval bound to the solver grid"
+    if options.get('overlap') is not None and not options['overlap']:
+        return "overlap=False"
+    if torch.is_autocast_enabled('cuda'):
+        return "autocast"
+    if sde.f_and_g_prod_mode != 'fused' or sde.g_prod_mode != 'fused' or getattr(sde, 'user_f_and_g', True):
+        return "f and g are not two separate callables (a user f_and_g, g_prod or f_and_g_prod)"
+    if not halves_exactly(engine.dtype, engine.ctxs):
+        return "a half step is subnormal in the state dtype"
+    return None
+
+
+def solve_adjoint_chunk(engine, ks, t0, state_in, state_out, ys, grad_ys, partials):
+    """Backward steps `ks` (consecutive, single-cell unless alone) of `engine` as one launch of
+    tsde_solve_reversible_heun_pointwise on its adjoint program, from the forward values at (t0, z); step k ends on
+    output row engine._out[k] (-1: none).  `state_in` / `state_out` are (y, z, f, g, adj_y, adj_f, adj_g, adj_z)."""
+    ad = engine._pw[0]
+    feed = engine._feed
+    nz = feed.get(engine.ctxs[ks[0]])
+    feed._nz.flags = 0
+    steps = (_cabi.PwStep * len(ks))()
+    row = ys.stride(0) * ys.element_size()  # (ys is contiguous: output k starts k rows of bytes past ys)
+    for s, k in zip(steps, ks):
+        c = engine.ctxs[k]
+        s.cell_id, s.h, _ = feed.binding.cell(c.k)
+        s.dt, s.t0 = c.dt, c.aux_t[1].data_ptr()
+        s.y1 = None if engine._out[k] < 0 else ys.data_ptr() + engine._out[k] * row
+    ad.t0, ad.ys, ad.grad_ys, ad.n_out = t0.data_ptr(), ys.data_ptr(), grad_ys.data_ptr(), ys.shape[0]
+    ad.y1 = state_out[0].data_ptr()
+    for i in range(4):
+        ad.adj_in[i], ad.adj_out[i] = state_in[4 + i].data_ptr(), state_out[4 + i].data_ptr()
+    for i, x in enumerate(partials):
+        ad.partial[i] = x.data_ptr()
+    y, z, f, g = (x.data_ptr() for x in state_in[:4])
+    _cabi.check(engine._lib.tsde_solve_reversible_heun_pointwise(
+        engine._L, nz, ctypes.byref(ad.prog), y, z, f, g, steps, len(ks),
+        *(x.data_ptr() for x in state_out[1:4])), 'tsde_solve_reversible_heun_pointwise')

@@ -27,7 +27,7 @@ constexpr int64_t kMaxGlobalRows = 0xFFFFFFFFll;
 constexpr int64_t kMaxCounterChannels = 1ll << 26;
 
 // Launches issued per kernel family (TSDE_KERNEL_*), read by tsde_kernel_launches.
-constexpr int kKernelFamilies = 9;
+constexpr int kKernelFamilies = 10;
 inline std::atomic<int64_t> g_launches[kKernelFamilies];
 
 // The contraction of a GENERAL-noise launch with m channels: cabi.cu sends m == 1 to the row-wise kernels (one product

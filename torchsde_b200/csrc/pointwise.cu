@@ -265,10 +265,12 @@ static bool pw_valid_tables(const tsde_pointwise& pg, bool* vec, int max_kind = 
   return true;
 }
 
-// a source that can be read when the registers in `written` are defined
-static bool pw_valid_source(const tsde_pointwise& pg, uint32_t s, bool allow_go, uint64_t written) {
+// a source that can be read when the registers in `written` are defined and `seeds` seeds exist (1: go; 2: go and
+// go2, the adjoint layout's vjp part)
+static bool pw_valid_source(const tsde_pointwise& pg, uint32_t s, int seeds, uint64_t written) {
   if (s == TSDE_PW_SRC_Y) return true;
-  if (s == TSDE_PW_SRC_GO) return allow_go;
+  if (s == TSDE_PW_SRC_GO) return seeds >= 1;
+  if (s == TSDE_PW_SRC_GO2) return seeds >= 2;
   if (s >= (uint32_t)TSDE_PW_OPERAND(0)) return (int)(s - TSDE_PW_OPERAND(0)) < pg.n_operands;
   return (int)s < pg.n_regs && ((written >> s) & 1u);
 }
@@ -283,16 +285,16 @@ static bool pw_unary(int op) {
 
 // instructions [i0, i1), run in order from the registers in `written`, which gains the ones they define; `compiled`:
 // the layout is compiled, so the transcendental opcodes are valid too (POW's exponent an IMM operand)
-static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, bool allow_go, uint64_t& written,
+static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, int seeds, uint64_t& written,
                            bool compiled = false) {
   for (int i = i0; i < i1; ++i) {
     const tsde_pw_instr& in = pg.instr[i];
     if (!(compiled && pw_transcendental(in.op)) &&
         ((in.op > TSDE_PW_SQRT && in.op < TSDE_PW_LT) || in.op > TSDE_PW_SEL))
       return false;
-    if ((int)in.dst >= pg.n_regs || !pw_valid_source(pg, in.a, allow_go, written)) return false;
-    if (!pw_unary(in.op) && !pw_valid_source(pg, in.b, allow_go, written)) return false;
-    if (in.op == TSDE_PW_POW && (in.b < TSDE_PW_OPERAND(0) || in.b == TSDE_PW_SRC_Y || in.b == TSDE_PW_SRC_GO ||
+    if ((int)in.dst >= pg.n_regs || !pw_valid_source(pg, in.a, seeds, written)) return false;
+    if (!pw_unary(in.op) && !pw_valid_source(pg, in.b, seeds, written)) return false;
+    if (in.op == TSDE_PW_POW && (in.b < TSDE_PW_OPERAND(0) || in.b >= TSDE_PW_SRC_GO2 ||
                                  pg.operand[in.b - TSDE_PW_OPERAND(0)].kind != TSDE_PW_IMM))
       return false;
     if (in.op == TSDE_PW_SEL && !((written >> in.dst) & 1u)) return false;  // the condition
@@ -516,9 +518,9 @@ static const std::string pw_expression(const tsde_pw_instr& x, const std::string
 
 static bool pw_per_channel_kind(int kind) { return kind == TSDE_PW_DM || kind == TSDE_PW_M; }
 
-// Source s names an operand (not y, go or a register)
+// Source s names an operand (not y, a seed or a register)
 static bool pw_operand_source(uint8_t s) {
-  return s >= TSDE_PW_OPERAND(0) && s != TSDE_PW_SRC_Y && s != TSDE_PW_SRC_GO;
+  return s >= TSDE_PW_OPERAND(0) && s != TSDE_PW_SRC_Y && s != TSDE_PW_SRC_GO && s != TSDE_PW_SRC_GO2;
 }
 
 // The CHANNEL / ROW operands a unit keeps in its Prog (k<k>[4], loaded once per launch): the first `max` of them.  A
@@ -536,6 +538,7 @@ static const std::string pw_value(const tsde_pointwise& in, uint8_t s, const boo
                                   int64_t m = 0) {
   if (s == TSDE_PW_SRC_Y) return "y[j]";
   if (s == TSDE_PW_SRC_GO) return "go[j]";
+  if (s == TSDE_PW_SRC_GO2) return "go2[j]";
   if (!pw_operand_source(s)) return pw_cat({"r", num(s), "[j]"});
   const int k = s - TSDE_PW_OPERAND(0);
   const std::string n = num(k);
@@ -595,8 +598,9 @@ struct PwUnit {
   PwKernelText kernel[2];  // (a unit of one kernel: the second has no name)
 };
 
-// The units, by index: Milstein, the four general ones by their layout tag, and the Milstein adaptive proposal
-enum { kPwUnitMilstein = 0, kPwUnitAdaptive = TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN + 1 };
+// The units, by index: Milstein, the four general ones by their layout tag, the Milstein adaptive proposal and the
+// reversible-Heun adjoint's backward steps
+enum { kPwUnitMilstein = 0, kPwUnitAdaptive = TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN + 1, kPwUnitAdjoint };
 static_assert(TSDE_PW_LAYOUT_GENERAL == 1 && TSDE_PW_LAYOUT_GENERAL_SRA == 2 &&
                   TSDE_PW_LAYOUT_GENERAL_EULER_HEUN == 3 && TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN == 4,
               "a general unit's index is its layout tag");
@@ -638,6 +642,11 @@ static const PwUnit kPwUnits[] = {
        "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const tsde::PwP<tsde::T> p,\n"
        "    tsde::T* y_next, const __grid_constant__ tsde::PwSubs<tsde::T> st) {\n",
        "pw_milstein_proposal", "(ops, p, y_next, st)"}}},
+    {false,
+     {{"tsde_pw_adjoint_reversible_heun", true,
+       "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const __grid_constant__ tsde::PwAdjP<tsde::T> p,\n"
+       "    const tsde::NoiseP<tsde::T> nz, const __grid_constant__ tsde::PwAdjSteps<tsde::T> st) {\n",
+       "pw_adjoint_reversible_heun_steps", "(ops, p, nz, st)"}}},
 };
 
 static const char* const kPwCellSuffix[2] = {"_single", "_multi"};
@@ -655,6 +664,10 @@ static_assert(sizeof(PwOperands<double>) + sizeof(PwGeneralRevHeunP<double>) + s
                       sizeof(PwSteps<double>) <=
                   4096,
               "the compiled general reversible-Heun kernel's parameters fit the 4 KiB parameter space");
+static_assert(sizeof(PwOperands<double>) + sizeof(PwAdjP<double>) + sizeof(NoiseP<double>) +
+                      sizeof(PwAdjSteps<double>) <=
+                  4096,
+              "the compiled adjoint kernel's parameters fit the 4 KiB parameter space");
 
 // The end of unit `unit`'s source: the close of its Prog and namespaces, then its kernels
 static std::string pw_unit_tail(int unit, bool f64) {
@@ -671,58 +684,92 @@ static std::string pw_unit_tail(int unit, bool f64) {
   return o;
 }
 
+// The body of a compiled program's part: instructions [i0, i1) and then `results`, each a statement `prefix` followed
+// by the value of its source; the time (*`time`) and the operands not kept in registers (`hoisted`) that they read
+// are loaded first.
+static std::string pw_part(const tsde_pointwise& in, bool f64, const bool (&hoisted)[TSDE_PW_MAX_OPERANDS], int i0,
+                           int i1, const std::pair<std::string, uint8_t>* results, int n_results, const char* time) {
+  uint8_t reads[2 * TSDE_PW_MAX_INSTR + 2 + TSDE_PW_ADJ_MAX_PARAMS];
+  int n = 0;
+  for (int i = i0; i < i1; ++i) {
+    reads[n++] = in.instr[i].a;
+    if (!pw_unary(in.instr[i].op)) reads[n++] = in.instr[i].b;
+  }
+  for (int r = 0; r < n_results; ++r) reads[n++] = results[r].second;
+  std::string o;
+  bool t0 = false, x[TSDE_PW_MAX_OPERANDS] = {};
+  for (int i = 0; i < n; ++i) {
+    const uint8_t s = reads[i];
+    if (!pw_operand_source(s)) continue;
+    const int k = s - TSDE_PW_OPERAND(0), kind = in.operand[k].kind;
+    if (kind == TSDE_PW_T0 && !t0) {
+      t0 = true;
+      o += pw_cat({"    const T t0 = *", time, ";\n"});
+    } else if (kind >= TSDE_PW_CHANNEL && !hoisted[k] && !x[k]) {
+      x[k] = true;
+      o += pw_cat({"    T x", num(k), "[4];\n"});
+      o += pw_load_operand(in, k, "x");
+    }
+  }
+  o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
+  for (int i = i0; i < i1; ++i) {
+    const tsde_pw_instr& ins = in.instr[i];
+    const std::string a = pw_value(in, ins.a, hoisted), b = pw_unary(ins.op) ? a : pw_value(in, ins.b, hoisted);
+    const std::string d = pw_cat({"r", num(ins.dst), "[j]"});
+    o += pw_cat({"      ", d, " = ", pw_expression(ins, a, b, d, f64), ";\n"});
+  }
+  for (int r = 0; r < n_results; ++r)
+    o += pw_cat({"      ", results[r].first, pw_value(in, results[r].second, hoisted), ";\n"});
+  return o + "    }\n";
+}
+
 // The translation unit of a program that passed pw_valid_tables and pw_valid_milstein, for dtype `f64`: the Milstein
 // unit (the kernels of consecutive steps) or the adaptive one (the kernel of an adaptive solve's proposal).
 static std::string pw_milstein_source(const tsde_pointwise& in, bool f64, int unit = kPwUnitMilstein) {
   bool hoisted[TSDE_PW_MAX_OPERANDS];
   pw_hoist(in, kPwJitHoistQuads[f64], hoisted);
-  // instructions [i0, i1) and then `results` (name = source); the time and the operands not kept in registers that
-  // they read are loaded first
-  auto part = [&](int i0, int i1, std::initializer_list<std::pair<const char*, uint8_t>> results) {
-    uint8_t reads[2 * TSDE_PW_MAX_INSTR + 2];
-    int n = 0;
-    for (int i = i0; i < i1; ++i) {
-      reads[n++] = in.instr[i].a;
-      if (!pw_unary(in.instr[i].op)) reads[n++] = in.instr[i].b;
-    }
-    for (const auto& r : results) reads[n++] = r.second;
-    std::string o;
-    bool t0 = false, x[TSDE_PW_MAX_OPERANDS] = {};
-    for (int i = 0; i < n; ++i) {
-      const uint8_t s = reads[i];
-      if (!pw_operand_source(s)) continue;
-      const int k = s - TSDE_PW_OPERAND(0), kind = in.operand[k].kind;
-      if (kind == TSDE_PW_T0 && !t0) {
-        t0 = true;
-        o += "    const T t0 = *s.t0;\n";
-      } else if (kind >= TSDE_PW_CHANNEL && !hoisted[k] && !x[k]) {
-        x[k] = true;
-        o += pw_cat({"    T x", num(k), "[4];\n"});
-        o += pw_load_operand(in, k, "x");
-      }
-    }
-    o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
-    for (int i = i0; i < i1; ++i) {
-      const tsde_pw_instr& ins = in.instr[i];
-      const std::string a = pw_value(in, ins.a, hoisted), b = pw_unary(ins.op) ? a : pw_value(in, ins.b, hoisted);
-      const std::string d = pw_cat({"r", num(ins.dst), "[j]"});
-      o += pw_cat({"      ", d, " = ", pw_expression(ins, a, b, d, f64), ";\n"});
-    }
-    for (const auto& r : results) o += pw_cat({"      ", r.first, "[j] = ", pw_value(in, r.second, hoisted), ";\n"});
-    return o + "    }\n";
-  };
   std::string regs;
   for (int r = 0; r < in.n_regs; ++r) regs += pw_cat({"  T r", num(r), "[4];\n"});
   std::string o = pw_prog_head(in, f64, "// A Milstein program of torchsde_b200, generated by pw_milstein_source\n",
                                regs, hoisted);
   o += "  __device__ __forceinline__ void fg(const PwOperands<T>& ops, const PwQuad& c, const PwStep<T>& s,\n"
        "                                     const T (&y)[4], T (&f)[4], T (&g)[4]) {\n";
-  o += part(0, in.n_fg, {{"f", in.f_src}, {"g", in.g_src}});
+  const std::pair<std::string, uint8_t> fg[2] = {{"f[j] = ", in.f_src}, {"g[j] = ", in.g_src}};
+  o += pw_part(in, f64, hoisted, 0, in.n_fg, fg, 2, "s.t0");
   o += "  }\n  __device__ __forceinline__ void vjp(const PwOperands<T>& ops, const PwQuad& c, const PwStep<T>& s,\n"
        "                                      const T (&y)[4], const T (&go)[4], T (&gdg)[4]) {\n";
-  o += part(in.n_fg, in.n_instr, {{"gdg", in.gdg_src}});
+  const std::pair<std::string, uint8_t> gdg[1] = {{"gdg[j] = ", in.gdg_src}};
+  o += pw_part(in, f64, hoisted, in.n_fg, in.n_instr, gdg, 1, "s.t0");
   o += "  }\n";
   o += pw_unit_tail(unit, f64);
+  return o;
+}
+
+// The translation unit of an adjoint program that passed pw_valid_adjoint, for dtype `f64`: the Milstein layout's f / g
+// part at a time pointer, and a vjp part with two seeds whose results are vjp_z and the contributions, each added to
+// its accumulator (pw_adjoint_reversible_heun_steps).  The CHANNEL / ROW operands stay in registers as Milstein's do.
+static std::string pw_adjoint_source(const tsde_pw_adjoint& ad, bool f64) {
+  const tsde_pointwise& in = ad.prog;
+  bool hoisted[TSDE_PW_MAX_OPERANDS];
+  pw_hoist(in, kPwJitHoistQuads[f64], hoisted);
+  std::string members = pw_cat({"  static constexpr int NP = ", num(ad.n_params > 0 ? ad.n_params : 1), ";\n"});
+  for (int r = 0; r < in.n_regs; ++r) members += pw_cat({"  T r", num(r), "[4];\n"});
+  std::string o = pw_prog_head(
+      in, f64, "// A reversible-Heun adjoint program of torchsde_b200, generated by pw_adjoint_source\n", members,
+      hoisted);
+  o += "  __device__ __forceinline__ void fg(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
+       "                                     T (&f)[4], T (&g)[4]) {\n";
+  const std::pair<std::string, uint8_t> fg[2] = {{"f[j] = ", in.f_src}, {"g[j] = ", in.g_src}};
+  o += pw_part(in, f64, hoisted, 0, in.n_fg, fg, 2, "tp");
+  o += "  }\n  __device__ __forceinline__ void vjp(const PwOperands<T>& ops, const PwQuad& c, const T* tp,\n"
+       "                                      const T (&y)[4], const T (&go)[4], const T (&go2)[4], T (&vz)[4],\n"
+       "                                      T (&acc)[NP][4]) {\n";
+  std::pair<std::string, uint8_t> results[1 + TSDE_PW_ADJ_MAX_PARAMS] = {{"vz[j] = ", in.gdg_src}};
+  for (int k = 0; k < ad.n_params; ++k)
+    results[1 + k] = {pw_cat({"acc[", num(k), "][j] = acc[", num(k), "][j] + "}), ad.param_src[k]};
+  o += pw_part(in, f64, hoisted, in.n_fg, in.n_instr, results, 1 + ad.n_params, "tp");
+  o += "  }\n";
+  o += pw_unit_tail(kPwUnitAdjoint, f64);
   return o;
 }
 
@@ -1661,6 +1708,86 @@ static int pw_milstein_chunk(const tsde_launch* L, const tsde_noise* nz, const t
                                np.n_cells > 1, p.nquads, TSDE_KERNEL_PW_MILSTEIN, p, np, st);
 }
 
+// ---- the reversible-Heun adjoint's backward sweep (TSDE_PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN) -----------------------
+// An adjoint program the launches `L` may run: tagged TSDE_PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN, the Milstein layout's
+// checks, with two seeds in the vjp part, vjp_z in gdg_src and each parameter's contribution read at the end
+static bool pw_adjoint_program(const tsde_launch* L, const tsde_pw_adjoint* ad) {
+  bool vec = true;
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d || !ad ||
+      ad->prog.reserved != TSDE_PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN || ad->n_params < 0 ||
+      ad->n_params > TSDE_PW_ADJ_MAX_PARAMS || !pw_valid_tables(ad->prog, &vec))
+    return false;
+  const tsde_pointwise& pg = ad->prog;
+  uint64_t written = 0;
+  if (!pw_valid_range(pg, 0, pg.n_fg, 0, written, true) || !pw_valid_source(pg, pg.f_src, 0, written) ||
+      !pw_valid_source(pg, pg.g_src, 0, written) || !pw_valid_range(pg, pg.n_fg, pg.n_instr, 2, written, true) ||
+      !pw_valid_source(pg, pg.gdg_src, 2, written))
+    return false;
+  for (int k = 0; k < ad->n_params; ++k)
+    if (!pw_valid_source(pg, ad->param_src[k], 2, written)) return false;
+  return true;
+}
+
+// tsde_solve_reversible_heun_pointwise for an adjoint program: the chunk steps[0, n_steps) from the state (y, z, f, g)
+// of the arguments and (adj_y, adj_f, adj_g, adj_z) of the program's launch buffers, as one launch of its compiled
+// kernel (compiled here if this is the first launch of its structure)
+template <typename T>
+static int pw_adjoint_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_pw_adjoint* ad,
+                            const void* const (&in4)[4], const tsde_pw_step* steps, int32_t n_steps,
+                            void* const (&out3)[3]) {
+  if (!pw_adjoint_program(L, ad) || !ad->t0 || !ad->y1 || !ad->ys || !ad->grad_ys) return TSDE_EINVAL;
+  const void* const in[kAdjState] = {in4[0], in4[1], in4[2], in4[3], ad->adj_in[0], ad->adj_in[1], ad->adj_in[2],
+                                     ad->adj_in[3]};
+  void* const out[kAdjState] = {ad->y1, out3[0], out3[1], out3[2], ad->adj_out[0], ad->adj_out[1], ad->adj_out[2],
+                                ad->adj_out[3]};
+  PwAdjP<T> p{};
+  NoiseP<T> np;
+  if (int e = pw_fill<T>(L, nz, ad->prog, in[0], nullptr, p.base, np)) return e;
+  p.base.t0 = static_cast<const T*>(ad->t0);
+  bool vec = p.base.vec != 0 && aligned16(ad->ys) && aligned16(ad->grad_ys);
+  for (int k = 0; k < kAdjState; ++k) {
+    if (!in[k] || !out[k]) return TSDE_EINVAL;
+    vec = vec && aligned16(in[k]) && aligned16(out[k]);
+    p.in[k] = static_cast<const T*>(in[k]);
+    p.out[k] = static_cast<T*>(out[k]);
+  }
+  for (int k = 0; k < ad->n_params; ++k) {
+    if (!ad->partial[k]) return TSDE_EINVAL;
+    vec = vec && aligned16(ad->partial[k]);
+    p.part[k] = static_cast<T*>(ad->partial[k]);
+  }
+  p.base.vec = vec ? 1 : 0;
+  p.ys = static_cast<const T*>(ad->ys);
+  p.gys = static_cast<const T*>(ad->grad_ys);
+  p.plane = L->rows * L->d;
+  if (!steps || n_steps < 1 || n_steps > kPwMaxSteps || (np.n_cells > 1 && n_steps > 1)) return TSDE_EINVAL;
+  PwAdjSteps<T> st{};
+  st.n = n_steps;
+  const intptr_t plane = (intptr_t)(p.plane * (int64_t)sizeof(T));
+  for (int j = 0; j < n_steps; ++j) {
+    const tsde_pw_step& s = steps[j];
+    int64_t row = -1;  // the output the step ends on: steps[j].y1 = ys + row * rows * d
+    if (s.y1) {
+      const intptr_t off = (intptr_t)s.y1 - (intptr_t)ad->ys;
+      if (off < 0 || off % plane || off / plane >= ad->n_out) return TSDE_EINVAL;
+      row = off / plane;
+    }
+    if (!s.t0) return TSDE_EINVAL;
+    st.s[j] = PwAdjStep<T>{s.cell_id, static_cast<const T*>(s.t0), row, (T)sqrt(s.h), (T)s.dt};
+  }
+  np.cell_id = steps[0].cell_id;
+  np.h = steps[0].h;
+  return pw_launch_compiled<T>(L, &ad->prog, kPwUnitAdjoint, pw_adjoint_source(*ad, sizeof(T) == 8), 0,
+                               np.n_cells > 1, p.base.nquads, TSDE_KERNEL_PW_ADJOINT, p, np, st);
+}
+
+// The adjoint program of a tagged tsde_pointwise (the first member of its tsde_pw_adjoint), or null
+static const tsde_pw_adjoint* pw_adjoint_of(const tsde_pointwise* prog) {
+  return prog && prog->reserved == TSDE_PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN
+             ? reinterpret_cast<const tsde_pw_adjoint*>(prog)
+             : nullptr;
+}
+
 // The chunk `steps[0, n_steps)` of Euler or reversible Heun from y0 (and, for reversible Heun, from the solver state
 // in[] = z0, f0, g0, left in out[] = z1, f1, g1): one launch of pw_chunk_kernel, under the rules of
 // pw_milstein_chunk.
@@ -1868,6 +1995,12 @@ TSDE_EXPORT int tsde_solve_reversible_heun_pointwise(const tsde_launch* L, const
       return pw_general_reversible_heun<decltype(t)>(L, nz, prog, y0, in, steps, n_steps, out);
     });
   if (!valid_launch(L) || L->noise_type != TSDE_NOISE_DIAGONAL || L->m != L->d) return TSDE_EINVAL;
+  if (const tsde_pw_adjoint* ad = pw_adjoint_of(prog)) {
+    const void* const in4[4] = {y0, z0, f0, g0};
+    return dispatch(L, [&](auto t) -> int {
+      return pw_adjoint_chunk<decltype(t)>(L, nz, ad, in4, steps, n_steps, out);
+    });
+  }
   return dispatch(L, [&](auto t) -> int {
     return pw_chunk<decltype(t), kPwReversibleHeun>(L, nz, prog, y0, steps, n_steps, in, out);
   });
@@ -1967,6 +2100,10 @@ TSDE_EXPORT int tsde_pointwise_compile(const tsde_launch* L, const tsde_pointwis
       if (!pw_general_unit<decltype(t)>(L, prog, layout, source)) return TSDE_EINVAL;
       return pw_loaded(*prog, layout, std::move(source), kc);
     }
+    if (const tsde_pw_adjoint* ad = pw_adjoint_of(prog)) {
+      if (!pw_adjoint_program(L, ad)) return TSDE_EINVAL;
+      return pw_loaded(*prog, kPwUnitAdjoint, pw_adjoint_source(*ad, sizeof(t) == 8), kc);
+    }
     if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
     return pw_loaded(*prog, kPwUnitMilstein, pw_milstein_source(*prog, sizeof(t) == 8), kc);
   });
@@ -1979,6 +2116,10 @@ TSDE_EXPORT int64_t tsde_pointwise_source(const tsde_launch* L, const tsde_point
       std::string source;
       if (!pw_general_unit<decltype(t)>(L, prog, layout, source)) return TSDE_EINVAL;
       return pw_copy_source(source, buf, size);
+    }
+    if (const tsde_pw_adjoint* ad = pw_adjoint_of(prog)) {
+      if (!pw_adjoint_program(L, ad)) return TSDE_EINVAL;
+      return pw_copy_source(pw_adjoint_source(*ad, sizeof(t) == 8), buf, size);
     }
     if (!pw_milstein_program(L, prog)) return TSDE_EINVAL;
     return pw_copy_source(pw_milstein_source(*prog, sizeof(t) == 8), buf, size);

@@ -203,6 +203,39 @@ struct MilsteinOp {
   }
 };
 
+// ---- reversible-Heun adjoint, diagonal noise                     methods/reversible_heun.py:98-144
+template <typename T>
+struct AdjRevHeunAOp {
+  static constexpr int NIN = 7, NOUT = 3;
+  static constexpr bool USES_NOISE = true, WANT_U = false;
+  T dt, half_dt;
+  __device__ __forceinline__ void operator()(const T (&in)[7], T w, T, T (&out)[3]) const {
+    const T y0 = in[0], z0 = in[1], f0 = in[2], g0 = in[3];
+    const T adj_y0 = in[4], adj_f0 = in[5], adj_g0 = in[6];
+    const T half_dw = T(0.5) * w;                                   // :102
+    out[0] = ((T(2) * y0 - z0) - f0 * dt) - g0 * w;                  // :109
+    out[1] = adj_f0 + adj_y0 * half_dt;                              // :104,113
+    out[2] = adj_g0 + adj_y0 * half_dw;                              // :105,115
+  }
+};
+template <typename T>
+struct AdjRevHeunBOp {
+  static constexpr int NIN = 8, NOUT = 5;
+  static constexpr bool USES_NOISE = true, WANT_U = false;
+  T dt, half_dt;
+  __device__ __forceinline__ void operator()(const T (&in)[8], T w, T, T (&out)[5]) const {
+    const T y0 = in[0], f0 = in[1], f1 = in[2], g0 = in[3], g1 = in[4];
+    const T adj_y0 = in[5], adj_z0_in = in[6], vjp_z = in[7];
+    const T half_dw = T(0.5) * w;
+    const T adj_z0 = adj_z0_in + vjp_z;                              // :130
+    out[0] = (y0 - (f0 + f1) * half_dt) - (g0 + g1) * half_dw;       // :134-135
+    out[1] = adj_y0 + T(2) * adj_z0;                                 // :137
+    out[2] = -adj_z0;                                                // :138
+    out[3] = adj_y0 * half_dt + adj_z0 * dt;                         // :112,139
+    out[4] = adj_y0 * half_dw + adj_z0 * w;                          // :114,140
+  }
+};
+
 // ---- the whole-step kernels' parameters (pointwise.cu) --------------------------------------
 template <typename T>
 struct PwP {
@@ -882,6 +915,127 @@ __device__ __forceinline__ void pw_general_reversible_heun_steps(const PwOperand
   store_quad(p.z1, c.base, c.vec, c.nvalid, z);
   store_quad(p.f1, c.base, c.vec, c.nvalid, f);
   pw_store_g<T, Prog::M>(p.g1, c, p.gvec != 0, g);
+}
+
+// ---- the reversible-Heun adjoint's backward sweep (TSDE_PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN) -----------------------
+// The augmented state of a backward step, in the order of the entry point's state_in / state_out
+enum { kAdjY = 0, kAdjZ, kAdjF, kAdjG, kAdjAdjY, kAdjAdjF, kAdjAdjG, kAdjAdjZ, kAdjState };
+
+template <typename T>
+struct PwAdjStep {  // one backward step, from tsde_pw_step with its scalars rounded to T on the host
+  uint64_t cell;    // Brownian cell
+  const T* t1;      // forward time of the step's end: f and g run at (t1, z1)
+  int64_t out;      // >= 0: the step ends an output interval (y <- ys[out], adj_y <- adj_y + grad_ys[out]); else -1
+  T sqrt_h, dt;
+};
+template <typename T>
+struct PwAdjSteps {  // by value: a captured launch carries the whole table
+  int32_t n;
+  PwAdjStep<T> s[kPwMaxSteps];
+};
+template <typename T>
+struct PwAdjP {
+  PwP<T> base;                          // the quad mapping; base.t0 the time of the first step's forward values
+  const T* in[kAdjState];               // the state the chunk starts from
+  T* out[kAdjState];                    // where it leaves it (no pointer of in[])
+  const T *ys, *gys;                    // the output series and its cotangent, (n_out, rows, d)
+  int64_t plane;                        // rows * d
+  T* part[TSDE_PW_ADJ_MAX_PARAMS];      // each parameter's (rows, d) partial sum of contributions
+};
+
+// Consecutive backward steps of AdjointReversibleHeun (reversible_heun.py:98-144) in reversed time, one thread per
+// quad, in the order of the unfused sweep (_BackwardEngine._sweep):
+//   z1, adj_f_mid, adj_g_mid = AdjRevHeunAOp (y, z, f, g, adj_y, adj_f, adj_g);
+//   vjp_z and the contributions = the vjp with seeds (adj_f_mid, adj_g_mid) of the forward values at z;
+//   f1, g1 at (t1, z1);  y, adj_y, adj_z, adj_f, adj_g = AdjRevHeunBOp (y, f, f1, g, g1, adj_y, adj_z, vjp_z);
+// and, at an output interval's end, y <- ys[out], adj_y <- adj_y + grad_ys[out].  The forward values the vjp
+// differentiates are the program's registers: the evaluation at (t1, z1) of one step is the next step's (the unfused
+// sweep keeps that graph as `pending`), and the chunk's first step evaluates them at (base.t0, z).  Each contribution
+// is summed over the chunk's steps in a register accumulator and added to its partial once, at the end.
+// `Prog` (pw_adjoint_source in pointwise.cu):
+//   load(ops, c)                                  the operands kept in registers, after the dependency wait
+//   fg(ops, c, t, y, f, g)                        instructions [0, n_fg) at (*t, y), and the f and g results
+//   vjp(ops, c, t, y, go, go2, vz, acc)           instructions [n_fg, n_instr) with seeds go (f) and go2 (g), vjp_z
+//                                                 into vz, each contribution added to acc[k]
+template <typename T, int SRC, typename Prog>
+__device__ __forceinline__ void pw_adjoint_reversible_heun_steps(const PwOperands<T>& ops, const PwAdjP<T>& p,
+                                                                 const NoiseP<T>& nz, const PwAdjSteps<T>& st) {
+  PwQuad c;
+  int64_t Q, row, q;
+  pw_locate(p.base, c, Q, row, q);
+  const Key key = load_key(nz.key);
+  Prog prog;
+  T x[kAdjState][4], acc[Prog::NP][4];
+  const T* tv = p.base.t0;  // the time of the forward values in the program's registers
+  for (int j = 0; j < st.n; ++j) {
+    const PwAdjStep<T>& s = st.s[j];
+    T w[4], u[4];
+    NoiseP<T> n = nz;  // this step's cell
+    n.cell_id = s.cell;
+    n.sqrt_h = s.sqrt_h;
+    quad_noise<T, SRC, false>(n, key, row, q, c.vec, c.nvalid, w, u);
+    if (j == 0) {  // the first increment is drawn while the previous kernel drains; the rest is read after the wait
+      asm volatile("griddepcontrol.wait;" ::: "memory");
+      if (Q >= p.base.nquads) return;
+#pragma unroll
+      for (int k = 0; k < kAdjState; ++k) load_quad(p.in[k], c.base, c.vec, c.nvalid, x[k]);
+      prog.load(ops, c);
+      T f0[4], g0[4];
+      prog.fg(ops, c, tv, x[kAdjZ], f0, g0);
+#pragma unroll
+      for (int k = 0; k < Prog::NP; ++k)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) acc[k][i] = T(0);
+    }
+    const T dt = s.dt, half_dt = T(0.5) * dt;
+    T z1[4], afm[4], agm[4];
+    const AdjRevHeunAOp<T> a{dt, half_dt};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      T o[3];
+      a({x[kAdjY][i], x[kAdjZ][i], x[kAdjF][i], x[kAdjG][i], x[kAdjAdjY][i], x[kAdjAdjF][i], x[kAdjAdjG][i]}, w[i],
+        T(0), o);
+      z1[i] = o[0];
+      afm[i] = o[1];
+      agm[i] = o[2];
+    }
+    T vz[4], f1[4], g1[4];
+    prog.vjp(ops, c, tv, x[kAdjZ], afm, agm, vz, acc);
+    prog.fg(ops, c, s.t1, z1, f1, g1);
+    tv = s.t1;
+    const AdjRevHeunBOp<T> b{dt, half_dt};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      T o[5];
+      b({x[kAdjY][i], x[kAdjF][i], f1[i], x[kAdjG][i], g1[i], x[kAdjAdjY][i], x[kAdjAdjZ][i], vz[i]}, w[i], T(0), o);
+      x[kAdjY][i] = o[0];
+      x[kAdjAdjY][i] = o[1];
+      x[kAdjAdjZ][i] = o[2];
+      x[kAdjAdjF][i] = o[3];
+      x[kAdjAdjG][i] = o[4];
+      x[kAdjZ][i] = z1[i];
+      x[kAdjF][i] = f1[i];
+      x[kAdjG][i] = g1[i];
+    }
+    if (s.out >= 0) {  // adjoint.py:114-116
+      T gy[4];
+      load_quad(p.ys + s.out * p.plane, c.base, c.vec, c.nvalid, x[kAdjY]);
+      load_quad(p.gys + s.out * p.plane, c.base, c.vec, c.nvalid, gy);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) x[kAdjAdjY][i] = x[kAdjAdjY][i] + gy[i];
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < kAdjState; ++k) store_quad(p.out[k], c.base, c.vec, c.nvalid, x[k]);
+#pragma unroll
+  for (int k = 0; k < Prog::NP; ++k) {
+    if (!p.part[k]) continue;  // (NP is 1 for a program without parameters)
+    T v[4];
+    load_quad(p.part[k], c.base, c.vec, c.nvalid, v);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) v[i] = v[i] + acc[k][i];
+    store_quad(p.part[k], c.base, c.vec, c.nvalid, v);
+  }
 }
 
 }  // namespace tsde

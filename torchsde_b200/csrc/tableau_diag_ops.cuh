@@ -208,38 +208,7 @@ struct LerpOp {
   }
 };
 
-// ---- reversible-Heun adjoint, diagonal noise                     methods/reversible_heun.py:98-144
-template <typename T>
-struct AdjRevHeunAOp {
-  static constexpr int NIN = 7, NOUT = 3;
-  static constexpr bool USES_NOISE = true, WANT_U = false;
-  T dt, half_dt;
-  __device__ __forceinline__ void operator()(const T (&in)[7], T w, T, T (&out)[3]) const {
-    const T y0 = in[0], z0 = in[1], f0 = in[2], g0 = in[3];
-    const T adj_y0 = in[4], adj_f0 = in[5], adj_g0 = in[6];
-    const T half_dw = T(0.5) * w;                                   // :102
-    out[0] = ((T(2) * y0 - z0) - f0 * dt) - g0 * w;                  // :109
-    out[1] = adj_f0 + adj_y0 * half_dt;                              // :104,113
-    out[2] = adj_g0 + adj_y0 * half_dw;                              // :105,115
-  }
-};
-template <typename T>
-struct AdjRevHeunBOp {
-  static constexpr int NIN = 8, NOUT = 5;
-  static constexpr bool USES_NOISE = true, WANT_U = false;
-  T dt, half_dt;
-  __device__ __forceinline__ void operator()(const T (&in)[8], T w, T, T (&out)[5]) const {
-    const T y0 = in[0], f0 = in[1], f1 = in[2], g0 = in[3], g1 = in[4];
-    const T adj_y0 = in[5], adj_z0_in = in[6], vjp_z = in[7];
-    const T half_dw = T(0.5) * w;
-    const T adj_z0 = adj_z0_in + vjp_z;                              // :130
-    out[0] = (y0 - (f0 + f1) * half_dt) - (g0 + g1) * half_dw;       // :134-135
-    out[1] = adj_y0 + T(2) * adj_z0;                                 // :137
-    out[2] = -adj_z0;                                                // :138
-    out[3] = adj_y0 * half_dt + adj_z0 * dt;                         // :112,139
-    out[4] = adj_y0 * half_dw + adj_z0 * w;                          // :114,140
-  }
-};
+// (AdjRevHeunAOp, AdjRevHeunBOp: pw_device.cuh, which the run-time compiled adjoint kernels include too)
 
 template <typename T>
 static SrkDiagFinalOp<T> make_srk_final(double dt, double rdt, double sqrt_dt, double three_dt) {
