@@ -610,6 +610,32 @@ enum { TSDE_PW_DM = 5, TSDE_PW_M = 6 };
 #define TSDE_PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN 5 /* tsde_pointwise.reserved of a tsde_pw_adjoint's program */
 #define TSDE_PW_ADJ_MAX_PARAMS 8
 #define TSDE_PW_SRC_GO2 0xFD
+/*
+ * General and additive noise.  tsde_solve_reversible_heun_pointwise on a GENERAL launch with 2 <= L->m <=
+ * TSDE_PW_GENERAL_MAX_M, for the `prog` member of a tsde_pw_adjoint tagged reserved =
+ * TSDE_PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN, runs the same backward steps with g, adj_g and their kernels A and B
+ * as tsde_adjoint_reversible_heun_a / _b take them on a GENERAL launch: g0 (the g argument) and adj_in[2] are
+ * (rows, d, m), and so are the chunk's g1 and adj_out[2] (contiguous, 16-byte aligned, not overlapping).  Each thread
+ * runs one quad of d and keeps no (d, m) block in registers: g at (t, z) is re-evaluated channel by channel from the
+ * program, and adj_g is carried in kernel B's rank-2 form (adj_y and adj_z per lane, the step's m increments per
+ * thread); only the chunk's first step reads g0 and adj_in[2].  Each contraction with the increments sums in the order
+ * of the unfused launch's route, and vjp_z's channel sums in the order of ATen's CUDA sum over the last dimension, so
+ * every stored value equals the unfused sweep's bit for bit under the half-step condition above.
+ *
+ * Program: the general layout's f and g in [0, n_fg) (g per channel, with DM and M operands), and the vjp in
+ * [n_fg, n_instr) with seeds TSDE_PW_SRC_GO ((rows, d)) and TSDE_PW_SRC_GO2 (per channel, adj_g_mid).  An instruction
+ * is per channel when one of its sources is; TSDE_PW_CSUM (source a only, valid in this layout only) is the channel
+ * sum of a per-channel value, a (rows, d) value.  A per-channel instruction may not read a value computed from a
+ * channel sum.  f_src and gdg_src (vjp_z) are (rows, d) values; param_src[k] may be either: a (rows, d) contribution is
+ * summed over the chunk in registers and added to partial[k], (rows, d), once; a per-channel one is added to
+ * partial[k], (rows, d, m), at every step, element by element, by the thread that owns the element.  The launches count
+ * under TSDE_KERNEL_PW_ADJOINT; tsde_pointwise_compile and tsde_pointwise_source compile and write out the program on
+ * a GENERAL launch.  TSDE_EINVAL, before anything is compiled or launched: m outside [2, TSDE_PW_GENERAL_MAX_M], noise
+ * other than counter noise or with flags, an invalid program, and what the diagonal tag refuses.
+ */
+#define TSDE_PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN 6 /* ... of a general-noise tsde_pw_adjoint's program */
+enum { TSDE_PW_CSUM = 28 };
+
 typedef struct tsde_pw_adjoint {
   tsde_pointwise prog;
   int32_t n_params;

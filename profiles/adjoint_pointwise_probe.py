@@ -2,6 +2,7 @@
 alternated in one process.
 
     python profiles/adjoint_pointwise_probe.py [--reps 3] [--solves 5] [--steps 200] [--batch 65536] [--dim 64]
+                                               [--sde gbm|corr_gbm|mf_ou] [--m 16]
 
 cfg2's SDE in Stratonovich form (GBM, diagonal noise, fp32, B = 65536, d = 64, dt = 2^-10), 200 steps of
 `sdeint_adjoint` with the reversible pair, the loss sum(w * ys).  The drift is written with sigma broadcast before it is
@@ -13,6 +14,9 @@ passes: CUDA events around sdeint_adjoint (forward) and around backward() (the b
 captured).  ys, y0's gradient and the extra-state gradients of fused and unfused must be byte-identical, and the
 parameter gradients close (their largest relative difference is printed).  Prints one JSON line with the card's name,
 power limit and SM clock (read after the timed solves), the median times in ms and the compiled kernel's launches.
+
+--sde corr_gbm and mf_ou run general noise with --m Brownian channels instead: correlated GBM (f = mu*y,
+g = y.unsqueeze(-1) * S) and multi-factor OU (f = kappa*(theta - y), g = S.expand(B, d, m)), S a (d, m) parameter.
 """
 import argparse
 import json
@@ -48,9 +52,30 @@ class GBM(nn.Module):
         return self.sigma * y
 
 
+class General(nn.Module):
+    sde_type, noise_type = 'stratonovich', 'general'
+
+    def __init__(self, kind, d, m):
+        super().__init__()
+        gen = torch.Generator().manual_seed(0)
+        self.kind = kind
+        if kind == 'mf_ou':
+            self.kappa, self.theta = nn.Parameter(torch.ones(1)), nn.Parameter(torch.full((1,), 0.1))
+        else:
+            self.mu = nn.Parameter(torch.rand(d, generator=gen) * 0.1)
+        self.S = nn.Parameter((torch.rand(d, m, generator=gen) - 0.5) * (0.5 / m ** 0.5))
+
+    def f(self, t, y):
+        return self.kappa * (self.theta - y) if self.kind == 'mf_ou' else self.mu * y
+
+    def g(self, t, y):
+        return self.S.expand(y.shape[0], *self.S.shape) if self.kind == 'mf_ou' else y.unsqueeze(-1) * self.S
+
+
 def run(args, fused, graphs, timed):
     B, d, T, dt = args.batch, args.dim, args.steps, 2.0 ** -10
-    sde = GBM(d).to(DEV)
+    sde = (GBM(d) if args.sde == 'gbm' else General(args.sde, d, args.m)).to(DEV)
+    m = d if args.sde == 'gbm' else args.m
     ts = torch.arange(T + 1, device=DEV, dtype=torch.float32) * dt
     y0 = torch.full((B, d), 0.1, device=DEV, requires_grad=True)
     w = torch.linspace(-1, 1, (T + 1) * B * d, device=DEV).view(T + 1, B, d)
@@ -65,7 +90,7 @@ def run(args, fused, graphs, timed):
         y0.grad = None
         for p in sde.parameters():
             p.grad = None
-        bm = tsde.BrownianInterval(0.0, float(ts[-1]), size=(B, d), device=DEV, entropy=1)
+        bm = tsde.BrownianInterval(0.0, float(ts[-1]), size=(B, m), device=DEV, entropy=1)
         e = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
         e[0].record()
         ys = tsde.sdeint_adjoint(sde, y0, ts, bm=bm, method='reversible_heun', dt=dt, adjoint_options=dict(opts))
@@ -89,6 +114,8 @@ def main():
     ap.add_argument('--steps', type=int, default=200)
     ap.add_argument('--batch', type=int, default=65536)
     ap.add_argument('--dim', type=int, default=64)
+    ap.add_argument('--sde', choices=['gbm', 'corr_gbm', 'mf_ou'], default='gbm')
+    ap.add_argument('--m', type=int, default=16)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("adjoint_pointwise_probe: no CUDA device; nothing is measured")
@@ -112,7 +139,8 @@ def main():
                          capture_output=True, text=True).stdout.strip()
     name = {(False, False): 'unfused_eager', (True, False): 'fused_eager', (False, True): 'unfused_graph',
             (True, True): 'fused_graph'}
-    res = {'gpu': smi, 'B': args.batch, 'd': args.dim, 'steps': args.steps, 'reps': args.reps,
+    res = {'gpu': smi, 'sde': args.sde, 'B': args.batch, 'd': args.dim,
+           'm': args.dim if args.sde == 'gbm' else args.m, 'steps': args.steps, 'reps': args.reps,
            'solves': args.solves, 'ys_and_y0_grad_identical': same, 'param_grad_max_rel_diff': rel,
            'fused_kernel_launches': fused_launches}
     for v in variants:

@@ -133,6 +133,69 @@ def compiled_milstein():
     return ok and not bad and not stack and not local
 
 
+# The general-noise adjoint kernel (pw_general_adjoint_reversible_heun_steps) of correlated GBM (f = mu*y,
+# g = y.unsqueeze(-1) * S): (m, dtype) -> the most spill memory (bytes per thread, STACK + LOCAL of cuobjdump
+# -res-usage) its single- and multi-cell kernels may use, as measured with CUDA 12.9.  It keeps no (d, m) block in registers, but the four lanes' channel passes,
+# the step's increments w and the previous step's wp stay live together; past m = 8 in fp32 and m = 4 in fp64 the
+# 255 registers of its launch bounds (256, 1) do not hold them (DESIGN section 3).
+GENERAL_ADJOINT_SPILL = {(4, 'float32'): 0, (16, 'float32'): 8, (32, 'float32'): 8,
+                         (4, 'float64'): 0, (16, 'float64'): 64, (32, 'float64'): 832}
+
+
+def _nvrtc_usage(src, kernels):
+    """{kernel: (REG, STACK, LOCAL)} of `src` compiled as the library compiles a program (NVRTC, its options)."""
+    import ctypes
+    import tempfile
+    from tests.test_host_pointwise_compile import OPTIONS, HEADERS, STDINT
+    nv = ctypes.CDLL('libnvrtc.so.12')
+    arr = lambda xs: (ctypes.c_char_p * len(xs))(*[x.encode() for x in xs])  # noqa: E731
+    prog = ctypes.c_void_p()
+    names = list(HEADERS) + ['stdint.h']
+    nv.nvrtcCreateProgram(ctypes.byref(prog), src.encode(), b'prog.cu', len(names),
+                          arr([open(p).read() for p in HEADERS.values()] + [STDINT]), arr(names))
+    assert nv.nvrtcCompileProgram(prog, len(OPTIONS), arr(OPTIONS)) == 0
+    n = ctypes.c_size_t()
+    nv.nvrtcGetCUBINSize(prog, ctypes.byref(n))
+    cubin = ctypes.create_string_buffer(n.value)
+    nv.nvrtcGetCUBIN(prog, cubin)
+    with tempfile.NamedTemporaryFile(suffix='.cubin') as f:
+        f.write(cubin.raw)
+        f.flush()
+        res = subprocess.run(['cuobjdump', '-res-usage', f.name], capture_output=True, text=True).stdout
+    out = {}
+    for k in kernels:
+        m = re.search(r'Function ' + k + r':\n\s*REG:(\d+) STACK:(\d+) SHARED:(\d+) LOCAL:(\d+)', res)
+        out[k] = (int(m.group(1)), int(m.group(2)), int(m.group(4)))
+    return out
+
+
+def compiled_general_adjoint():
+    """Registers and local memory of the general-noise adjoint kernels at m = 4, 16, 32 in fp32 and fp64, against
+    GENERAL_ADJOINT_SPILL; False if one spills more than it states."""
+    sys.path.insert(0, ROOT)
+    import torch
+    from tests import test_host_pointwise_adjoint_general as gen
+    from torchsde_b200 import _cabi
+    ok = True
+    print("## the general-noise adjoint's backward-step kernel (correlated GBM), compiled at run time (NVRTC)\n"
+          "   m  dtype     single: REG STACK LOCAL   multi: REG STACK LOCAL   (STACK + LOCAL at most)")
+    for dtype in (torch.float32, torch.float64):
+        for m in (4, 16, 32):
+            mu = gen.P(gen.D).detach().to(dtype).requires_grad_()
+            S = gen.P(gen.D, m).detach().to(dtype).requires_grad_()
+            rec, res = gen.record(lambda t, y: mu * y, lambda t, y: y.unsqueeze(-1) * S, [mu, S], m=m, dtype=dtype)
+            src = _cabi.general_pointwise_source(res[0].prog, dtype, gen.D, m)
+            names = ['tsde_pw_general_adjoint_reversible_heun_single', 'tsde_pw_general_adjoint_reversible_heun_multi']
+            u = _nvrtc_usage(src, names)
+            name = str(dtype).split('.')[-1]
+            most = GENERAL_ADJOINT_SPILL[(m, name)]
+            ok = ok and all(v[1] + v[2] <= most for v in u.values())
+            print(f"   {m:2d} {name}   {u[names[0]][0]:3d} {u[names[0]][1]:5d} {u[names[0]][2]:5d}           "
+                  f"{u[names[1]][0]:3d} {u[names[1]][1]:5d} {u[names[1]][2]:5d}   ({most})")
+    print()
+    return ok
+
+
 def main():
     if not os.path.exists(LIB):
         sys.exit("build the library first: python -c 'import __graft_entry__ as g; g.build()'")
@@ -168,6 +231,7 @@ def main():
         cnt = {k: sum(1 for o in ops if re.search(r'\b' + re.escape(k) + r'\b', o)) for k in COUNT}
         print('   ' + '  '.join(f"{k}={v}" for k, v in cnt.items() if v) + '\n')
     bad = 0 if compiled_milstein() else 1
+    bad += 0 if compiled_general_adjoint() else 1
     for pat in INTERPRETED:
         hit = [n for n, d in zip(names, dem) if re.search(pat, d)]
         sass = subprocess.run(['cuobjdump', '-sass', '-fun', hit[0], LIB], capture_output=True, text=True).stdout

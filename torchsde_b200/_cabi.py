@@ -130,6 +130,8 @@ PW_MAX_STEPS = 64  # TSDE_PW_MAX_STEPS
 PW_ADJ_MAX_PARAMS = 8  # TSDE_PW_ADJ_MAX_PARAMS
 PW_SRC_GO2 = 0xFD  # TSDE_PW_SRC_GO2: the adjoint layout's second vjp seed (g's cotangent)
 PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN = 5  # TSDE_PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN: ... of a PwAdjoint's program
+PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN = 6  # TSDE_PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN: ... general noise
+PW_CSUM = 28  # TSDE_PW_CSUM: the channel sum of a per-channel value (the general adjoint's vjp part only)
 
 
 class PwInstr(ctypes.Structure):

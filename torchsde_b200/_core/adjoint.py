@@ -234,8 +234,11 @@ class _BackwardEngine(base_solver.BaseSDESolver):
         sde = self.sde
         with torch.enable_grad():
             z0r = z0.detach().requires_grad_()
-            rec = pointwise.AdjointRecorder(z0r, t_fwd0, len(params),
-                                            bool(self.adjoint_options.get('transcendental', False)))
+            transcendental = bool(self.adjoint_options.get('transcendental', False))
+            if sde.noise_type == NOISE_TYPES.diagonal:
+                rec = pointwise.AdjointRecorder(z0r, t_fwd0, len(params), transcendental)
+            else:
+                rec = pointwise.GeneralAdjointRecorder(z0r, t_fwd0, len(params), self.m, transcendental)
             re_f0, re_g0 = rec.forward(lambda: sde.f_and_g(t_fwd0, z0r))
             pairs = [(o, go) for o, go in ((re_f0, adj_f_mid), (re_g0, adj_g_mid)) if o.requires_grad]
             if not pairs:
@@ -259,6 +262,10 @@ class _BackwardEngine(base_solver.BaseSDESolver):
             reason = pointwise.adjoint_refusal(self, self.adjoint_options)
             if reason is None and not pointwise.state_fits(self, state[2:4] + state[1:2]):
                 reason = "the solver state (f0, g0, z0) is not made of (rows, d) tensors of the state dtype"
+            # (general noise: the kernel reads adj_g as (rows, d, m), which autograd need not give it)
+            if reason is None and self.sde.noise_type != NOISE_TYPES.diagonal and \
+                    not pointwise.state_fits(self, state[5:7] + state[7:8]):
+                reason = "the cotangent of (f0, g0, z0) is not made of tensors of the state dtype and shapes"
             if reason is None and any(s.n_steps == 0 for s in self.scheds):
                 reason = "an output interval without steps"
             res = None
@@ -275,13 +282,15 @@ class _BackwardEngine(base_solver.BaseSDESolver):
             self._out += [-1] * (sched.n_steps - 1) + [self.T - 2 - n]
         n_steps = len(self._out)
         kinds = self._pw[2]
-        partials = [torch.zeros_like(y) for kind in kinds if kind is not None]
+        wide = y.shape + (self.m,)  # (a general-noise g, adj_g and per-channel partial)
+        partials = [y.new_zeros(wide if kind in pointwise.PER_CHANNEL else y.shape) for kind in kinds
+                    if kind is not None]
         ys_c, gys_c = _contig(ys), _contig(grad_ys)
         multi = [k for k in range(n_steps) if self.binding.cell(self.ctxs[k].k)[2] > 1]
         chunks = pointwise.plan_chunks(0, n_steps, multi_cell=multi, max_steps=pointwise.chunk_length(self))
         # a chunk stores its state to the set it did not read: the caller's tensors are read once, so a sweep of one
         # chunk needs one set, any other two
-        sets = [[torch.empty_like(y) for _ in state] for _ in range(min(len(chunks), 2))]
+        sets = [[torch.empty_like(x) for x in state] for _ in range(min(len(chunks), 2))]
         for j, (k0, k1) in enumerate(chunks):
             t0 = self.ctxs[0].aux_t[0] if k0 == 0 else self.ctxs[k0 - 1].aux_t[1]
             pointwise.solve_adjoint_chunk(self, range(k0, k1), t0, state, sets[j % 2], ys_c, gys_c, partials)
@@ -292,8 +301,8 @@ class _BackwardEngine(base_solver.BaseSDESolver):
         for ap, kind in zip(adj_params, kinds):
             if kind is not None:
                 part = next(live)
-                ap.add_((part.sum(0) if kind == pointwise.REDUCE_ROWS else
-                         part.sum() if kind == pointwise.REDUCE_ALL else part).view_as(ap))
+                dims = pointwise.REDUCE_DIMS[kind]
+                ap.add_((part.sum() if dims is None else part.sum(dims) if dims else part).view_as(ap))
         return state[4], (state[5], state[6], state[7]), adj_params
 
     def run(self, ys, ts, grad_ys, extras, grad_extras):

@@ -134,8 +134,11 @@ returns as that parameter's gradient (on a parameter's path the tape holds autog
 and every step of the sweep then runs in chunks of tsde_solve_reversible_heun_pointwise, each contribution summed in
 registers and added once per chunk to a (rows, d) partial that the sweep reduces over the batch once at its end
 (adjoint._BackwardEngine._fused_sweep).  y, the adjoint state and y0's gradient are the unfused sweep's bits; parameter
-gradients differ by summation order only.  Only diagonal noise on a bound grid, without logqp, autocast, overlap=False,
-adjoint_adaptive, create_graph or a user f_and_g (`adjoint_refusal`); anything else keeps the unfused sweep and warns.
+gradients differ by summation order only.  General and additive noise with 2 <= m <= TSDE_PW_GENERAL_MAX_M record
+under `GeneralAdjointRecorder` (g per channel, vjp_z's channel sums as CSUM instructions, per-channel contributions
+with (rows, d, m) partials) into a PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN program run on the GENERAL launch.  Only a
+bound grid, without logqp, autocast, overlap=False, adjoint_adaptive, create_graph or a user f_and_g
+(`adjoint_refusal`); anything else keeps the unfused sweep and warns.
 """
 import ctypes
 import numbers
@@ -1017,9 +1020,10 @@ def plan_chunks(first, n_steps, interpolated=(), multi_cell=(), max_steps=_cabi.
 # sm_90a: 64 K registers per SM): Milstein's compiled kernels are pinned there by their launch bounds (256, 4) and
 # (256, 2) (cfg2's program: 54 registers in fp32); Euler at 54 and 88-96; reversible Heun at 72 and 110-120.
 # The compiled general-noise Euler and reversible-Heun kernels are bounded at (256, 1): at least one resident CTA,
-# whatever m; so is the reversible-Heun adjoint's backward-step kernel, whatever its parameters.
+# whatever m; so are the reversible-Heun adjoint's backward-step kernels, whatever their parameters and m.
 _RESIDENT_CTAS = {'milstein': (4, 2), 'euler': (4, 2), 'reversible_heun': (3, 2), 'euler_general': (1, 1),
-                  'reversible_heun_general': (1, 1), 'adjoint_reversible_heun': (1, 1)}
+                  'reversible_heun_general': (1, 1), 'adjoint_reversible_heun': (1, 1),
+                  'adjoint_reversible_heun_general': (1, 1)}
 
 
 def chunk_length(solver):
@@ -1157,7 +1161,15 @@ def propose(solver, method, curr_t, next_t, midpoint_t, y0):
 # How a parameter's gradient leaves the vjp: reduced over the rows (a (d,) parameter), over everything (one element),
 # or not at all (a (rows, d) parameter)
 REDUCE_ROWS, REDUCE_ALL, REDUCE_NONE = 'rows', 'all', 'none'
+# and, for general and additive noise (GeneralAdjointRecorder), of a per-channel contribution, whose partial is
+# (rows, d, m): over the rows (a (d, m) parameter), over the rows and d (an (m,) parameter), over everything
+REDUCE_CHANNEL_ROWS, REDUCE_CHANNEL_ROWS_D, REDUCE_CHANNEL_ALL = 'channel_rows', 'channel_rows_d', 'channel_all'
+PER_CHANNEL = (REDUCE_CHANNEL_ROWS, REDUCE_CHANNEL_ROWS_D, REDUCE_CHANNEL_ALL)
+# each kind's partial reduced as autograd's sum_to reduces one step's gradient: the dims summed (None: all)
+REDUCE_DIMS = {REDUCE_ROWS: (0,), REDUCE_ALL: None, REDUCE_NONE: (), REDUCE_CHANNEL_ROWS: (0,),
+               REDUCE_CHANNEL_ROWS_D: (0, 1), REDUCE_CHANNEL_ALL: None}
 _SUMS = (aten.sum.dim_IntList, aten.sum.default)
+_SQUEEZE = (aten.squeeze.dim, aten.squeeze.dims, aten.squeeze.default)
 
 
 class AdjointRecorder(Recorder):
@@ -1173,6 +1185,8 @@ class AdjointRecorder(Recorder):
       * None, a parameter the step does not reach: no contribution.
     Any other op on a reduced value (a parameter transformed before it is broadcast), more than
     TSDE_PW_ADJ_MAX_PARAMS parameters, or anything the Milstein recorder rejects, rejects the tape."""
+
+    layout = _cabi.PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN
 
     def __init__(self, z0, t0, n_params, transcendental=False):
         super().__init__(z0, t0, transcendental)
@@ -1333,7 +1347,7 @@ class AdjointRecorder(Recorder):
             prog, keep = self._program(code, n_fg, results[:3], n_regs, _cabi.PW_MAX_REGS)
             ad = _cabi.PwAdjoint()
             ad.prog = prog
-            ad.prog.reserved = _cabi.PW_LAYOUT_ADJOINT_REVERSIBLE_HEUN
+            ad.prog.reserved = self.layout
             ad.n_params = len(live)
             for k, src in enumerate(results[3:]):
                 ad.param_src[k] = src
@@ -1341,6 +1355,124 @@ class AdjointRecorder(Recorder):
         except Exception as e:
             self.reject(f"{type(e).__name__}: {e}")
             return None
+
+
+class GeneralAdjointRecorder(AdjointRecorder, GeneralRecorder):
+    """The AdjointRecorder of a general- or additive-noise SDE with 2 <= m <= TSDE_PW_GENERAL_MAX_M Brownian channels:
+    f and g as the GeneralRecorder takes them (g a (rows, d, m) value, per-channel values and DM / M operands), and a vjp
+    whose seed GO2 is per channel.  In the vjp segment a sum of a per-channel value is either
+      * over the channels, (rows, d, m) -> (rows, d, 1), autograd's sum_to of a lifted (rows, d) value's gradient: the
+        tape's CSUM, a (rows, d) value that further ops may read (and `squeeze` to (rows, d)); the kernel sums it in the
+        order of ATen's CUDA reduction;
+      * a parameter's batch reduction, over the rows (a (d, m) parameter), the rows and d (an (m,) one) or everything (a
+        one-element one): a per-channel contribution (REDUCE_CHANNEL_*), whose partial is (rows, d, m);
+    any other sum, or anything either recorder rejects, rejects the tape.  The program is tagged
+    PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN and compiled on a GENERAL launch."""
+
+    def __init__(self, z0, t0, n_params, m, transcendental=False):
+        GeneralRecorder.__init__(self, z0, t0, 'fg', m, transcendental,
+                                 _cabi.PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN)
+        self.reduced = []
+        self.fg = self.fg3 = self.results = None
+        self._in_vjp = False
+        if not 2 <= m <= _cabi.PW_GENERAL_MAX_M:
+            self.reject(f"general noise with m = {m} Brownian channels: 2 to {_cabi.PW_GENERAL_MAX_M} are fused")
+        if n_params > _cabi.PW_ADJ_MAX_PARAMS:
+            self.reject(f"{n_params} parameters: at most {_cabi.PW_ADJ_MAX_PARAMS} are fused")
+
+    def vjp(self, fn, go, go2, params):
+        self._wide.add(GO2)
+        return super().vjp(fn, go, go2, params)
+
+    def _step_result(self, t, allow_go=False):
+        if torch.is_tensor(t) and t.dim() == 3:
+            self._kind = 'g'
+            return GeneralRecorder._step_result(self, t)
+        self._kind, self._w3 = 'f', False
+        src = Recorder._step_result(self, t, allow_go)
+        if src in self._wide:
+            raise Reject("f or vjp_z is computed per channel")
+        return src
+
+    def _record(self, func, args, kwargs, out):
+        if func in _SQUEEZE and self._in_vjp:  # (the squeeze that ends sum_to of a lifted value's gradient)
+            src = self._lookup(args[0])
+            if src is not None and src[0] == 'v' and src not in self._wide and \
+                    tuple(out.shape) == (self.rows, self.d):
+                self._bind(out, src)
+                return
+        super()._record(func, args, kwargs, out)
+
+    def _operand3(self, x):
+        # (a view of a leaf parameter, S.expand(rows, d, m), has a grad_fn: it is still the parameter's storage)
+        if x.grad_fn is not None and x._is_view() and x._base.grad_fn is None:
+            x = x.detach()
+        return super()._operand3(x)
+
+    def _reduce(self, args, kwargs, out):
+        x = args[0]
+        if x.dim() != 3:
+            self._w3 = False
+            return super()._reduce(args, kwargs, out)
+        if kwargs.get('dtype') is not None:
+            raise Reject("a reduction with a dtype")
+        self._w3 = True
+        src = self._source(x)
+        if tuple(x.shape) != (self.rows, self.d, self.m) or src not in self._wide:
+            raise Reject(f"a reduction of a {tuple(x.shape)} value")
+        dims = tuple(sorted(int(k) % 3 for k in args[1])) if len(args) > 1 and args[1] else (0, 1, 2)
+        if dims == (2,):
+            if tuple(out.shape) != (self.rows, self.d, 1):
+                raise Reject(f"a channel sum to {tuple(out.shape)}")
+            self._w3 = False
+            v = self._value(_cabi.PW_CSUM, src)
+            self._bind(out, v)
+            self._lifted.add(id(out))
+            return
+        kind = {(0,): REDUCE_CHANNEL_ROWS, (0, 1): REDUCE_CHANNEL_ROWS_D, (0, 1, 2): REDUCE_CHANNEL_ALL}.get(dims)
+        if kind is None:
+            raise Reject(f"a reduction over dims {dims} of a per-channel value")
+        self._keep.append(out)
+        self.reduced.append((kind, [src]))
+        self._bind(out, ('r', len(self.reduced) - 1))
+
+
+def channel_sum(x):
+    """ATen's CUDA sum(x, -1, keepdim=True) of a contiguous (..., m) x, 2 <= m <= TSDE_PW_GENERAL_MAX_M, op by op in the
+    order the general adjoint kernel sums vjp_z's channels (TSDE_PW_CSUM, pw_general_adjoint_source; Reduce.cuh of
+    PyTorch 2.11 for CUDA): P = the largest power of two <= m threads, thread j holding (0 + x_j) + (0 + x_{j+P}) (or
+    0 + x_j), then the shfl_down butterfly with offsets P/2, P/4, ..., 1, thread j adding thread j + offset."""
+    m = x.shape[-1]
+    P = 1 << (m.bit_length() - 1)
+    zero = torch.zeros((), dtype=x.dtype, device=x.device)
+    level = [zero + x[..., j] for j in range(P)]
+    for j in range(P, m):
+        level[j - P] = level[j - P] + (zero + x[..., j])
+    while len(level) > 1:
+        half = len(level) // 2
+        level = [level[i] + level[i + half] for i in range(half)]
+    return level[0].unsqueeze(-1)
+
+
+_SUM_ORDER = {}  # (m, dtype, device) -> whether this PyTorch's CUDA channel sum adds in channel_sum's order
+
+
+def sums_in_order(m, dtype, device):
+    """Whether torch.sum(x, -1, keepdim=True) on `device` adds m values in the order of `channel_sum`, checked once per
+    (m, dtype, device) on values whose sum depends on the order (mixed magnitudes, cancellation, signed zeros).  The
+    order is ATen's and can differ between PyTorch releases and builds (ROCm and older releases add the butterfly's
+    offsets in increasing order)."""
+    key = (m, dtype, str(device))
+    if key not in _SUM_ORDER:
+        gen = torch.Generator(device=device).manual_seed(5)
+        mag = torch.exp2(torch.randint(-30, 30, (4096, m), generator=gen, device=device).to(dtype))
+        x = (torch.rand(4096, m, generator=gen, dtype=dtype, device=device) - 0.5) * mag
+        x[:2048, 1::2] = -x[:2048, 0::2][:, :m // 2]
+        x[0] = -0.0
+        got, want = channel_sum(x), torch.sum(x, -1, keepdim=True)
+        _SUM_ORDER[key] = bool(torch.equal(got.view(torch.int64 if dtype == torch.float64 else torch.int32),
+                                           want.view(torch.int64 if dtype == torch.float64 else torch.int32)))
+    return _SUM_ORDER[key]
 
 
 def compile_adjoint(rec, res):
@@ -1351,13 +1483,21 @@ def compile_adjoint(rec, res):
     if res is None:
         return None
     ad = res[0]
-    src = _cabi.pointwise_source(ad.prog, rec.dtype)
+    general = isinstance(rec, GeneralAdjointRecorder)
+    if general and rec.device.type == 'cuda' and any(ad.prog.instr[i].op == _cabi.PW_CSUM
+                                                     for i in range(ad.prog.n_instr)) and \
+            not sums_in_order(rec.m, rec.dtype, rec.device):
+        rec.reject(f"this PyTorch's CUDA sum over {rec.m} channels does not add in the order the kernel restates")
+        return None
+    src = (_cabi.general_pointwise_source(ad.prog, rec.dtype, rec.d, rec.m) if general else
+           _cabi.pointwise_source(ad.prog, rec.dtype))
     if src is None:
         rec.reject("the library refuses the program")
         return None
     done = _COMPILED.setdefault(_cabi.lib(), set())
     if ('adjoint', src) not in done:
-        err = _cabi.compile_pointwise(ad.prog, rec.dtype)
+        err = (_cabi.compile_general_pointwise(ad.prog, rec.dtype, rec.d, rec.m) if general else
+               _cabi.compile_pointwise(ad.prog, rec.dtype))
         if err != 0:
             rec.reject(_cabi.lib().tsde_error_string(err).decode())
             return None
@@ -1380,8 +1520,11 @@ def adjoint_refusal(engine, options, differentiable=False, adaptive=False):
         return "create_graph (double backward)"
     if adaptive:
         return "adjoint_adaptive"
-    if sde.noise_type != NOISE_TYPES.diagonal:
-        return f"{sde.noise_type} noise (diagonal only)"
+    if sde.noise_type not in (NOISE_TYPES.diagonal, NOISE_TYPES.general, NOISE_TYPES.additive):
+        return f"{sde.noise_type} noise (diagonal, general or additive only)"
+    if sde.noise_type != NOISE_TYPES.diagonal and not 2 <= engine.m <= _cabi.PW_GENERAL_MAX_M:
+        return (f"{sde.noise_type} noise with m = {engine.m} Brownian channels (2 to {_cabi.PW_GENERAL_MAX_M} are "
+                f"fused)")
     if getattr(engine, 'binding', None) is None:
         return "the Brownian motion is not a BrownianInterval bound to the solver grid"
     if options.get('overlap') is not None and not options['overlap']:

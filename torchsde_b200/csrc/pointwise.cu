@@ -25,6 +25,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
+#include <functional>
 #include <string>
 #include <type_traits>
 
@@ -284,16 +286,18 @@ static bool pw_unary(int op) {
 }
 
 // instructions [i0, i1), run in order from the registers in `written`, which gains the ones they define; `compiled`:
-// the layout is compiled, so the transcendental opcodes are valid too (POW's exponent an IMM operand)
+// the layout is compiled, so the transcendental opcodes are valid too (POW's exponent an IMM operand); `csum`: the
+// general adjoint's vjp part, where CSUM (source a only) is valid too
 static bool pw_valid_range(const tsde_pointwise& pg, int i0, int i1, int seeds, uint64_t& written,
-                           bool compiled = false) {
+                           bool compiled = false, bool csum = false) {
   for (int i = i0; i < i1; ++i) {
     const tsde_pw_instr& in = pg.instr[i];
-    if (!(compiled && pw_transcendental(in.op)) &&
+    const bool sum = csum && in.op == TSDE_PW_CSUM;
+    if (!(compiled && pw_transcendental(in.op)) && !sum &&
         ((in.op > TSDE_PW_SQRT && in.op < TSDE_PW_LT) || in.op > TSDE_PW_SEL))
       return false;
     if ((int)in.dst >= pg.n_regs || !pw_valid_source(pg, in.a, seeds, written)) return false;
-    if (!pw_unary(in.op) && !pw_valid_source(pg, in.b, seeds, written)) return false;
+    if (!pw_unary(in.op) && !sum && !pw_valid_source(pg, in.b, seeds, written)) return false;
     if (in.op == TSDE_PW_POW && (in.b < TSDE_PW_OPERAND(0) || in.b >= TSDE_PW_SRC_GO2 ||
                                  pg.operand[in.b - TSDE_PW_OPERAND(0)].kind != TSDE_PW_IMM))
       return false;
@@ -599,8 +603,9 @@ struct PwUnit {
 };
 
 // The units, by index: Milstein, the four general ones by their layout tag, the Milstein adaptive proposal and the
-// reversible-Heun adjoint's backward steps
-enum { kPwUnitMilstein = 0, kPwUnitAdaptive = TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN + 1, kPwUnitAdjoint };
+// reversible-Heun adjoint's backward steps, of diagonal and of general noise
+enum { kPwUnitMilstein = 0, kPwUnitAdaptive = TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN + 1, kPwUnitAdjoint,
+       kPwUnitGeneralAdjoint };
 static_assert(TSDE_PW_LAYOUT_GENERAL == 1 && TSDE_PW_LAYOUT_GENERAL_SRA == 2 &&
                   TSDE_PW_LAYOUT_GENERAL_EULER_HEUN == 3 && TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN == 4,
               "a general unit's index is its layout tag");
@@ -647,6 +652,11 @@ static const PwUnit kPwUnits[] = {
        "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const __grid_constant__ tsde::PwAdjP<tsde::T> p,\n"
        "    const tsde::NoiseP<tsde::T> nz, const __grid_constant__ tsde::PwAdjSteps<tsde::T> st) {\n",
        "pw_adjoint_reversible_heun_steps", "(ops, p, nz, st)"}}},
+    {false,
+     {{"tsde_pw_general_adjoint_reversible_heun", true,
+       "(const __grid_constant__ tsde::PwOperands<tsde::T> ops, const __grid_constant__ tsde::PwAdjP<tsde::T> p,\n"
+       "    const tsde::NoiseP<tsde::T> nz, const __grid_constant__ tsde::PwAdjSteps<tsde::T> st) {\n",
+       "pw_general_adjoint_reversible_heun_steps", "(ops, p, nz, st)"}}},
 };
 
 static const char* const kPwCellSuffix[2] = {"_single", "_multi"};
@@ -790,10 +800,46 @@ static std::string pw_adjoint_source(const tsde_pw_adjoint& ad, bool f64) {
 // Register use stays bounded: m <= TSDE_PW_GENERAL_MAX_M increments per thread, and the tree keeps at most
 // log2(m / 4) + 1 partial sums.
 
+// Lane j's `acc`: the values val(k) of m channels contracted with the weights w[k] in the order of route `route`;
+// pre(k) / post(k) are the statements before / after channel k's term.
+static std::string pw_contraction(int route, int64_t m, bool f64, const std::function<std::string(int)>& val,
+                                  const std::function<std::string(int)>& pre,
+                                  const std::function<std::string(int)>& post) {
+  const std::string fma = f64 ? "fma" : "fmaf";
+  const int mq = (int)((m + 3) / 4);
+  std::string s;
+  if (route == TSDE_GEN_ROWWISE) {
+    s += pw_cat({pre(0), "      const T acc = ", val(0), " * w[0];\n", post(0)});
+  } else if (route == TSDE_GEN_GENERIC) {
+    s += "      T acc = T(0);\n";
+    for (int k = 0; k < m; ++k) s += pw_cat({pre(k), "      acc = acc + ", val(k), " * w[", num(k), "];\n", post(k)});
+  } else {
+    std::string level[TSDE_PW_GENERAL_MAX_M / 4];  // the partial sums of the tree's current level
+    for (int q = 0; q < mq; ++q) {
+      const std::string sq = pw_cat({"s", num(q)});
+      const int k0 = 4 * q;
+      s += pw_cat({pre(k0), "      T ", sq, " = ", fma, "(", val(k0), ", w[", num(k0), "], T(0));\n", post(k0)});
+      for (int j = 1; j < 4; ++j)
+        s += pw_cat({pre(k0 + j), "      ", sq, " = ", fma, "(", val(k0 + j), ", w[", num(k0 + j), "], ", sq, ");\n",
+                     post(k0 + j)});
+      level[q] = sq;
+    }
+    for (int l = 0, n = mq; n > 1; ++l, n /= 2) {
+      for (int p = 0; p < n; p += 2) {
+        const std::string a = pw_cat({"a", num(l), "_", num(p / 2)});
+        s += pw_cat({"      const T ", a, " = ", level[p], " + ", level[p + 1], ";\n"});
+        level[p / 2] = a;
+      }
+    }
+    s += pw_cat({"      const T acc = ", level[0], ";\n"});
+  }
+  return s;
+}
+
 // The translation unit of a program that passed pw_general_program, for m channels and contraction `route`: the
 // unit of its layout tag `layout` (Euler and midpoint kernels for TSDE_PW_LAYOUT_GENERAL).
 static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t m, int route, int layout) {
-  const std::string fs = f64 ? "" : "f", M = num((int)m);
+  const std::string M = num((int)m);
   const int mq = (int)((m + 3) / 4);
   bool hoisted[TSDE_PW_MAX_OPERANDS];
   pw_hoist(in, TSDE_PW_MAX_OPERANDS, hoisted);
@@ -853,38 +899,8 @@ static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t
   g_head += "        return ";
   g_head += gsrc(in.g_src);
   g_head += ";\n      };\n";
-  // lane j's acc: the values val(k) contracted with the weights w[k] in the route's order; pre(k) / post(k) are the
-  // statements before / after channel k's term
-  const std::string fma = "fma" + fs;
   auto contraction = [&](auto val, auto pre, auto post) {
-    std::string s;
-    if (route == TSDE_GEN_ROWWISE) {
-      s += pw_cat({pre(0), "      const T acc = ", val(0), " * w[0];\n", post(0)});
-    } else if (route == TSDE_GEN_GENERIC) {
-      s += "      T acc = T(0);\n";
-      for (int k = 0; k < m; ++k) s += pw_cat({pre(k), "      acc = acc + ", val(k), " * w[", num(k), "];\n", post(k)});
-    } else {
-      std::string level[TSDE_PW_GENERAL_MAX_M / 4];  // the partial sums of the tree's current level
-      for (int q = 0; q < mq; ++q) {
-        const std::string sq = pw_cat({"s", num(q)});
-        const int k0 = 4 * q;
-        s += pw_cat({pre(k0), "      T ", sq, " = ", fma, "(", val(k0), ", w[", num(k0), "], T(0));\n", post(k0)});
-        for (int j = 1; j < 4; ++j)
-          s += pw_cat({pre(k0 + j), "      ", sq, " = ", fma, "(", val(k0 + j), ", w[", num(k0 + j), "], ", sq, ");\n",
-                       post(k0 + j)});
-        level[q] = sq;
-      }
-      for (int l = 0, n = mq; n > 1; ++l, n /= 2) {
-        for (int p = 0; p < n; p += 2) {
-          const std::string a = pw_cat({"a", num(l), "_", num(p / 2)});
-          s += pw_cat({"      const T ", a, " = ", level[p], " + ", level[p + 1], ";\n"});
-          level[p / 2] = a;
-        }
-      }
-      s += pw_cat({"      const T acc = ", level[0], ";\n"});
-    }
-    s += "      out[j] = acc;\n    }\n  }\n";
-    return s;
+    return pw_contraction(route, m, f64, val, pre, post) + "      out[j] = acc;\n    }\n  }\n";
   };
   auto none = [](int) { return std::string(); };
   if (layout == TSDE_PW_LAYOUT_GENERAL_REVERSIBLE_HEUN) {
@@ -909,6 +925,239 @@ static std::string pw_general_source(const tsde_pointwise& in, bool f64, int64_t
     o += contraction([&](int k) { return pw_cat({"G(", num(k), ")"}); }, none, none);
   }
   o += pw_unit_tail(layout, f64);
+  return o;
+}
+
+// ---- the general-noise adjoint (TSDE_PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN) --------------------------------------
+// What each instruction of a general adjoint program is, derived from its sources alone: per channel (`wide`: a DM or M
+// operand, GO2 or a per-channel value is a source; a CSUM never is), and for a (rows, d) instruction of the vjp part,
+// `late` when it reads a channel sum (it runs after the channel loop).  def_*: the instruction that last wrote a
+// register source when the instruction runs (-1: not a register), dst_def that of SEL's condition; nidx: a forward
+// (rows, d) instruction's index in the Prog's nn[][4] values.  res_def: the instruction of each result's register.
+struct PwGAdjShape {
+  int def_a[TSDE_PW_MAX_INSTR], def_b[TSDE_PW_MAX_INSTR], dst_def[TSDE_PW_MAX_INSTR], nidx[TSDE_PW_MAX_INSTR];
+  bool wide[TSDE_PW_MAX_INSTR], late[TSDE_PW_MAX_INSTR];
+  int nn;
+  int f_def, g_def, vz_def, p_def[TSDE_PW_ADJ_MAX_PARAMS];
+};
+
+// (a range-for over a [begin, end) pair)
+template <typename I>
+struct PwRange {
+  I b, e;
+  I begin() const { return b; }
+  I end() const { return e; }
+};
+template <typename I>
+static PwRange<I> range(std::pair<I, I> p) {
+  return {p.first, p.second};
+}
+
+// The shape of a program whose tables and ranges are valid; false if the layout cannot run it: a CSUM of a (rows, d)
+// value or in the forward part, a per-channel instruction that reads a channel sum, f or vjp_z per channel.
+static bool pw_gadj_shape(const tsde_pw_adjoint& ad, PwGAdjShape& sh) {
+  const tsde_pointwise& in = ad.prog;
+  int def[TSDE_PW_MAX_REGS];
+  for (int r = 0; r < TSDE_PW_MAX_REGS; ++r) def[r] = -1;
+  auto reg = [&](uint8_t s) { return s < TSDE_PW_MAX_REGS ? def[s] : -1; };
+  auto wide = [&](uint8_t s, int d) {
+    if (s == TSDE_PW_SRC_GO2) return true;
+    if (pw_operand_source(s)) return pw_per_channel_kind(in.operand[s - TSDE_PW_OPERAND(0)].kind);
+    return d >= 0 && sh.wide[d];
+  };
+  auto late = [&](int d) { return d >= 0 && sh.late[d]; };
+  sh.nn = 0;
+  for (int i = 0; i < in.n_instr; ++i) {
+    const tsde_pw_instr& x = in.instr[i];
+    const bool un = pw_unary(x.op) || x.op == TSDE_PW_CSUM, sel = x.op == TSDE_PW_SEL;
+    sh.def_a[i] = reg(x.a);
+    sh.def_b[i] = un ? -1 : reg(x.b);
+    sh.dst_def[i] = sel ? def[x.dst] : -1;
+    const bool wa = wide(x.a, sh.def_a[i]), wb = !un && wide(x.b, sh.def_b[i]), wc = sel && wide(x.dst, sh.dst_def[i]);
+    const bool la = late(sh.def_a[i]), lb = late(sh.def_b[i]), lc = late(sh.dst_def[i]);
+    if (x.op == TSDE_PW_CSUM) {
+      if (i < in.n_fg || !wa) return false;
+      sh.wide[i] = false;
+      sh.late[i] = true;
+    } else {
+      sh.wide[i] = wa || wb || wc;
+      if (sh.wide[i] && (la || lb || lc)) return false;
+      sh.late[i] = !sh.wide[i] && (la || lb || lc);
+    }
+    sh.nidx[i] = i < in.n_fg && !sh.wide[i] ? sh.nn++ : -1;
+    def[x.dst] = i;
+    if (i + 1 == in.n_fg) {
+      sh.f_def = reg(in.f_src);
+      sh.g_def = reg(in.g_src);
+    }
+  }
+  if (in.n_fg == 0) sh.f_def = sh.g_def = -1;
+  sh.vz_def = reg(in.gdg_src);
+  for (int k = 0; k < ad.n_params; ++k) sh.p_def[k] = reg(ad.param_src[k]);
+  return !wide(in.f_src, sh.f_def) && !wide(in.gdg_src, sh.vz_def);
+}
+
+// The translation unit of a general adjoint program that passed pw_general_adjoint_program, for m channels and the
+// contraction order `route` of the unfused kernels A and B.  Its Prog, for pw_general_adjoint_reversible_heun_steps:
+//   fwd(ops, c, tp, y, nn, f)    the forward (rows, d) values at (*tp, y) into nn, and f
+//   gk(ops, c, t0, y, nn, j, k)  g's channel k of lane j at (t0, y), from the (rows, d) values nn
+//   vjp(...)                     kernel A's g0.dW and adj_g_mid, and the vjp, in one pass over the channels
+//   ystep(...)                   kernel B's (g0 + g1).(0.5 dW), g0 at (t0, y0) and g1 at (t1, y1)
+//   gstore(ops, c, tp, y, nn, g) g at (*tp, y), stored
+// and pc(k): whether parameter k's contribution is per channel.
+static std::string pw_general_adjoint_source(const tsde_pw_adjoint& ad, bool f64, int64_t m, int route) {
+  const tsde_pointwise& in = ad.prog;
+  PwGAdjShape sh;
+  pw_gadj_shape(ad, sh);
+  const std::string M = num((int)m);
+  const int mq = (int)((m + 3) / 4), P = (int)(m >= 32 ? 32 : m >= 16 ? 16 : m >= 8 ? 8 : m >= 4 ? 4 : 2);
+  bool hoisted[TSDE_PW_MAX_OPERANDS];
+  pw_hoist(in, TSDE_PW_MAX_OPERANDS, hoisted);
+  std::string members = pw_cat({"  static constexpr int M = ", M, ", MQ = ", num(mq), ", NN = ", num(sh.nn > 0 ? sh.nn : 1),
+                                ", NP = ", num(ad.n_params > 0 ? ad.n_params : 1), ";\n"});
+  // a contribution is per channel when its source is: a per-channel value, GO2 (a parameter that g broadcasts as it
+  // is, S.expand) or a DM / M operand
+  auto per_channel = [&](int p) {
+    const uint8_t s = ad.param_src[p];
+    if (s == TSDE_PW_SRC_GO2) return true;
+    if (pw_operand_source(s)) return pw_per_channel_kind(in.operand[s - TSDE_PW_OPERAND(0)].kind);
+    return sh.p_def[p] >= 0 && sh.wide[sh.p_def[p]];
+  };
+  std::string pc = "false";
+  for (int k = 0; k < ad.n_params; ++k)
+    if (per_channel(k)) pc += pw_cat({" || k == ", num(k)});
+  members += pw_cat({"  __host__ __device__ static constexpr bool pc(int k) { return ", pc, "; }\n"});
+  std::string o = pw_prog_head(
+      in, f64, "// A general-noise reversible-Heun adjoint program of torchsde_b200, generated by pw_general_adjoint_source\n",
+      members, hoisted);
+  // source s (last written by instruction d) in lane j: a per-channel value v<d>, a forward (rows, d) value nn[][j], a
+  // vjp one e<d>[j], the seeds, y or an operand (a DM / M one at the lane's d index i and channel k)
+  auto src = [&](uint8_t s, int d) -> std::string {
+    if (s == TSDE_PW_SRC_GO2) return "agm";
+    if (s == TSDE_PW_SRC_Y || s == TSDE_PW_SRC_GO || pw_operand_source(s)) return pw_value(in, s, hoisted, m);
+    if (sh.wide[d]) return "v" + num(d);
+    if (d < in.n_fg) return pw_cat({"nn[", num(sh.nidx[d]), "][j]"});
+    return pw_cat({"e", num(d), "[j]"});
+  };
+  auto expr = [&](int i) {
+    const tsde_pw_instr& x = in.instr[i];
+    const std::string a = src(x.a, sh.def_a[i]);
+    const std::string b = pw_unary(x.op) ? a : src(x.b, sh.def_b[i]);
+    return pw_expression(x, a, b, x.op == TSDE_PW_SEL ? src(x.dst, sh.dst_def[i]) : "", f64);
+  };
+  const std::string lane = "      const int64_t i = c.chan + (j < c.nvalid ? j : 0);  // (padding lanes read lane 0's)\n"
+                           "      (void)i;\n";
+  const std::string own = "(c.base + (j < c.nvalid ? j : 0)) * M + k";
+  // per-channel forward values of channel k (in a scope that defines k)
+  std::string fwd_wide;
+  for (int i = 0; i < in.n_fg; ++i)
+    if (sh.wide[i]) fwd_wide += pw_cat({"        const T v", num(i), " = ", expr(i), ";\n"});
+  const std::string gval = src(in.g_src, sh.g_def);
+  // fwd
+  o += "  __device__ __forceinline__ void fwd(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
+       "                                      T (&nn)[NN][4], T (&f)[4]) {\n    const T t0 = *tp;\n    (void)t0;\n"
+       "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
+  for (int i = 0; i < in.n_fg; ++i)
+    if (!sh.wide[i]) o += pw_cat({"      nn[", num(sh.nidx[i]), "][j] = ", expr(i), ";\n"});
+  o += pw_cat({"      f[j] = ", src(in.f_src, sh.f_def), ";\n    }\n  }\n"});
+  // gk
+  o += "  __device__ __forceinline__ T gk(const PwOperands<T>& ops, const PwQuad& c, const T t0, const T (&y)[4],\n"
+       "                                  const T (&nn)[NN][4], const int j, const int k) {\n    (void)t0;\n"
+       "    const int64_t i = c.chan + (j < c.nvalid ? j : 0);\n    (void)i;\n";
+  o += fwd_wide;
+  o += pw_cat({"    return ", gval, ";\n  }\n"});
+  // vjp: per lane, the early (rows, d) ops, then the channels (A's contraction, adj_g_mid, the per-channel vjp ops,
+  // the channel sums in ATen's order and the per-channel contributions), then the late (rows, d) ops
+  o += "  __device__ __forceinline__ void vjp(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
+       "                                      const T (&nn)[NN][4], const T (&w)[4 * MQ], const T (&wp)[4 * MQ],\n"
+       "                                      const bool first, const T* gin, const T* ain, const T (&ay)[4],\n"
+       "                                      const T (&ra)[4], const T (&rb)[4], const T (&go)[4], T (&zc)[4],\n"
+       "                                      T (&vz)[4], T (&pacc)[NP][4], T* const (&part)[TSDE_PW_ADJ_MAX_PARAMS]) {\n"
+       "    const T t0 = *tp;\n    (void)t0;\n";
+  int csum_at[TSDE_PW_MAX_INSTR], n_csum = 0;
+  for (int i = in.n_fg; i < in.n_instr; ++i) {
+    if (!sh.wide[i]) o += pw_cat({"    T e", num(i), "[4];\n"});
+    if (in.instr[i].op == TSDE_PW_CSUM) csum_at[n_csum++] = i;
+  }
+  const auto csums = [&]() { return std::pair<const int*, const int*>(csum_at, csum_at + n_csum); };
+  o += "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n" + lane;
+  for (int i = in.n_fg; i < in.n_instr; ++i)
+    if (!sh.wide[i] && !sh.late[i]) o += pw_cat({"      e", num(i), "[j] = ", expr(i), ";\n"});
+  for (int cs : range(csums()))
+    for (int x = 0; x < P; ++x) o += pw_cat({"      T q", num(cs), "_0_", num(x), ";\n"});
+  // ATen's sum over the last dimension (Reduce.cuh, for m <= 32 values per output): P = the largest power of two <= m
+  // threads, thread x summing (0 + v_x) + (0 + v_{x+P}) (or 0 + v_x), the P sums then added as the shfl_down
+  // butterfly adds them (offsets P/2, P/4, ..., 1: node (l, x) = (l-1, x) + (l-1, x + P/2^l)); emitted as each node
+  // completes
+  auto leaf_done = [&](int x) { return x + P < m ? x + P : x; };
+  auto pre = [&](int k) {
+    std::string s = pw_cat({"      T h", num(k), ";\n      {\n        const int k = ", num(k), ";\n"});
+    s += fwd_wide;
+    s += pw_cat({"        const T g0 = first ? gin[", own, "] : ", gval, ";\n"});
+    s += pw_cat({"        const T adg = first ? ain[", own, "] : ra[j] * (T(0.5) * wp[", num(k), "]) + rb[j] * (T(-1) * wp[",
+                 num(k), "]);\n"});
+    s += pw_cat({"        const T agm = adg + ay[j] * (T(0.5) * w[", num(k), "]);\n        (void)agm;\n"});
+    for (int i = in.n_fg; i < in.n_instr; ++i)
+      if (sh.wide[i]) s += pw_cat({"        const T v", num(i), " = ", expr(i), ";\n"});
+    for (int cs : range(csums())) {
+      const std::string v = src(in.instr[cs].a, sh.def_a[cs]);
+      if (k < P)
+        s += pw_cat({"        q", num(cs), "_0_", num(k), " = T(0) + ", v, ";\n"});
+      else
+        s += pw_cat({"        q", num(cs), "_0_", num(k - P), " = q", num(cs), "_0_", num(k - P), " + (T(0) + ", v, ");\n"});
+    }
+    for (int p = 0; p < ad.n_params; ++p)
+      if (per_channel(p))
+        s += pw_cat({"        if (j < c.nvalid) {\n          T* const pp = part[", num(p), "] + (c.base + j) * M + k;\n"
+                     "          *pp = *pp + ", src(ad.param_src[p], sh.p_def[p]), ";\n        }\n"});
+    return s + pw_cat({"        h", num(k), " = g0;\n      }\n"});
+  };
+  auto post = [&](int k) {
+    std::string s;
+    for (int l = 1, n = P / 2; n >= 1; ++l, n /= 2)
+      for (int x = 0; x < n; ++x) {
+        int last = 0;  // (the node sums leaves x + i n, i < 2^l)
+        for (int leaf = x; leaf < P; leaf += n) last = std::max(last, leaf_done(leaf));
+        if (last != k) continue;
+        for (int cs : range(csums()))
+          s += pw_cat({"      const T q", num(cs), "_", num(l), "_", num(x), " = q", num(cs), "_", num(l - 1), "_",
+                       num(x), " + q", num(cs), "_", num(l - 1), "_", num(x + n), ";\n"});
+      }
+    return s;
+  };
+  o += pw_contraction(route, m, f64, [&](int k) { return "h" + num(k); }, pre, post);
+  o += "      zc[j] = acc;\n";
+  int levels = 0;
+  while ((1 << levels) < P) ++levels;
+  for (int cs : range(csums())) o += pw_cat({"      e", num(cs), "[j] = q", num(cs), "_", num(levels), "_0;\n"});
+  for (int i = in.n_fg; i < in.n_instr; ++i)
+    if (sh.late[i] && in.instr[i].op != TSDE_PW_CSUM) o += pw_cat({"      e", num(i), "[j] = ", expr(i), ";\n"});
+  o += pw_cat({"      vz[j] = ", src(in.gdg_src, sh.vz_def), ";\n"});
+  for (int p = 0; p < ad.n_params; ++p)
+    if (!per_channel(p))
+      o += pw_cat({"      pacc[", num(p), "][j] = pacc[", num(p), "][j] + ", src(ad.param_src[p], sh.p_def[p]), ";\n"});
+  o += "    }\n  }\n";
+  // ystep
+  o += "  __device__ __forceinline__ void ystep(const PwOperands<T>& ops, const PwQuad& c, const T* tp0, const T (&y0)[4],\n"
+       "                                        const T (&n0)[NN][4], const T* tp1, const T (&y1)[4], const T (&n1)[NN][4],\n"
+       "                                        const T (&w)[4 * MQ], const bool first, const T* gin, T (&out)[4]) {\n"
+       "    const T ta = *tp0, tb = *tp1;\n#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n";
+  o += pw_contraction(
+      route, m, f64, [&](int k) { return "h" + num(k); },
+      [&](int k) {
+        const std::string K = num(k);
+        return pw_cat({"      const T h", K, " = (first ? gin[(c.base + (j < c.nvalid ? j : 0)) * M + ", K,
+                       "] : gk(ops, c, ta, y0, n0, j, ", K, ")) + gk(ops, c, tb, y1, n1, j, ", K, ");\n"});
+      },
+      [](int) { return std::string(); });
+  o += "      out[j] = acc;\n    }\n  }\n";
+  // gstore
+  o += "  __device__ __forceinline__ void gstore(const PwOperands<T>& ops, const PwQuad& c, const T* tp, const T (&y)[4],\n"
+       "                                         const T (&nn)[NN][4], T* g) {\n    const T t0 = *tp;\n"
+       "#pragma unroll\n    for (int j = 0; j < 4; ++j) {\n      if (j >= c.nvalid) continue;\n"
+       "#pragma unroll\n      for (int k = 0; k < M; ++k) g[(c.base + j) * M + k] = gk(ops, c, t0, y, nn, j, k);\n"
+       "    }\n  }\n";
+  o += pw_unit_tail(kPwUnitGeneralAdjoint, f64);
   return o;
 }
 
@@ -1728,14 +1977,50 @@ static bool pw_adjoint_program(const tsde_launch* L, const tsde_pw_adjoint* ad) 
   return true;
 }
 
+// ---- the general-noise adjoint (TSDE_PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN) --------------------------------------
+// A general adjoint program the GENERAL launches `L` may run, with `route` the contraction order of the unfused kernels
+// A and B (dense aligned g, gen_route) for dtype size `s`: the general layout's tables and f / g part, the vjp part with
+// two seeds and CSUM, 2 <= m <= TSDE_PW_GENERAL_MAX_M, and a shape pw_gadj_shape accepts.
+static bool pw_general_adjoint_program(const tsde_launch* L, const tsde_pw_adjoint* ad, int64_t s, int& route) {
+  bool vec = true;
+  if (!valid_launch(L) || L->noise_type != TSDE_NOISE_GENERAL || L->m < 2 || L->m > TSDE_PW_GENERAL_MAX_M || !ad ||
+      ad->prog.reserved != TSDE_PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN || ad->n_params < 0 ||
+      ad->n_params > TSDE_PW_ADJ_MAX_PARAMS || !pw_valid_tables(ad->prog, &vec, TSDE_PW_M))
+    return false;
+  const tsde_pointwise& pg = ad->prog;
+  uint64_t written = 0;
+  if (!pw_valid_range(pg, 0, pg.n_fg, 0, written, true) || !pw_valid_source(pg, pg.f_src, 0, written) ||
+      !pw_valid_source(pg, pg.g_src, 0, written) || !pw_valid_range(pg, pg.n_fg, pg.n_instr, 2, written, true, true) ||
+      !pw_valid_source(pg, pg.gdg_src, 2, written))
+    return false;
+  for (int k = 0; k < ad->n_params; ++k)
+    if (!pw_valid_source(pg, ad->param_src[k], 2, written)) return false;
+  PwGAdjShape sh;
+  if (!pw_gadj_shape(*ad, sh)) return false;
+  route = gen_route(L->m, true, L->m * s);
+  return route == TSDE_GEN_TILE || route == TSDE_GEN_GENERIC;
+}
+
+// The general adjoint program of a tagged tsde_pointwise (the first member of its tsde_pw_adjoint), or null
+static const tsde_pw_adjoint* pw_general_adjoint_of(const tsde_pointwise* prog) {
+  return prog && prog->reserved == TSDE_PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN
+             ? reinterpret_cast<const tsde_pw_adjoint*>(prog)
+             : nullptr;
+}
+
 // tsde_solve_reversible_heun_pointwise for an adjoint program: the chunk steps[0, n_steps) from the state (y, z, f, g)
 // of the arguments and (adj_y, adj_f, adj_g, adj_z) of the program's launch buffers, as one launch of its compiled
-// kernel (compiled here if this is the first launch of its structure)
+// kernel (compiled here if this is the first launch of its structure).  `general`: a general adjoint program on a
+// GENERAL launch, whose g and adj_g (in and out) are (rows, d, m) and read element by element, as is a per-channel
+// parameter's partial.
 template <typename T>
 static int pw_adjoint_chunk(const tsde_launch* L, const tsde_noise* nz, const tsde_pw_adjoint* ad,
                             const void* const (&in4)[4], const tsde_pw_step* steps, int32_t n_steps,
-                            void* const (&out3)[3]) {
-  if (!pw_adjoint_program(L, ad) || !ad->t0 || !ad->y1 || !ad->ys || !ad->grad_ys) return TSDE_EINVAL;
+                            void* const (&out3)[3], bool general = false) {
+  int route = 0;
+  if (!(general ? pw_general_adjoint_program(L, ad, sizeof(T), route) : pw_adjoint_program(L, ad)) || !ad->t0 ||
+      !ad->y1 || !ad->ys || !ad->grad_ys)
+    return TSDE_EINVAL;
   const void* const in[kAdjState] = {in4[0], in4[1], in4[2], in4[3], ad->adj_in[0], ad->adj_in[1], ad->adj_in[2],
                                      ad->adj_in[3]};
   void* const out[kAdjState] = {ad->y1, out3[0], out3[1], out3[2], ad->adj_out[0], ad->adj_out[1], ad->adj_out[2],
@@ -1747,7 +2032,7 @@ static int pw_adjoint_chunk(const tsde_launch* L, const tsde_noise* nz, const ts
   bool vec = p.base.vec != 0 && aligned16(ad->ys) && aligned16(ad->grad_ys);
   for (int k = 0; k < kAdjState; ++k) {
     if (!in[k] || !out[k]) return TSDE_EINVAL;
-    vec = vec && aligned16(in[k]) && aligned16(out[k]);
+    if (!general || (k != kAdjG && k != kAdjAdjG)) vec = vec && aligned16(in[k]) && aligned16(out[k]);
     p.in[k] = static_cast<const T*>(in[k]);
     p.out[k] = static_cast<T*>(out[k]);
   }
@@ -1777,6 +2062,10 @@ static int pw_adjoint_chunk(const tsde_launch* L, const tsde_noise* nz, const ts
   }
   np.cell_id = steps[0].cell_id;
   np.h = steps[0].h;
+  if (general)
+    return pw_launch_compiled<T>(L, &ad->prog, kPwUnitGeneralAdjoint,
+                                 pw_general_adjoint_source(*ad, sizeof(T) == 8, L->m, route), 0, np.n_cells > 1,
+                                 p.base.nquads, TSDE_KERNEL_PW_ADJOINT, p, np, st);
   return pw_launch_compiled<T>(L, &ad->prog, kPwUnitAdjoint, pw_adjoint_source(*ad, sizeof(T) == 8), 0,
                                np.n_cells > 1, p.base.nquads, TSDE_KERNEL_PW_ADJOINT, p, np, st);
 }
@@ -1990,6 +2279,13 @@ TSDE_EXPORT int tsde_solve_reversible_heun_pointwise(const tsde_launch* L, const
                                                      int32_t n_steps, void* z1, void* f1, void* g1) {
   const void* const in[3] = {z0, f0, g0};
   void* const out[3] = {z1, f1, g1};
+  if (valid_launch(L) && L->noise_type == TSDE_NOISE_GENERAL && pw_general_adjoint_of(prog)) {
+    const tsde_pw_adjoint* ad = pw_general_adjoint_of(prog);
+    const void* const in4[4] = {y0, z0, f0, g0};
+    return dispatch(L, [&](auto t) -> int {
+      return pw_adjoint_chunk<decltype(t)>(L, nz, ad, in4, steps, n_steps, out, true);
+    });
+  }
   if (valid_launch(L) && L->noise_type == TSDE_NOISE_GENERAL)
     return dispatch(L, [&](auto t) -> int {
       return pw_general_reversible_heun<decltype(t)>(L, nz, prog, y0, in, steps, n_steps, out);
@@ -2094,6 +2390,12 @@ TSDE_EXPORT int tsde_step_predictor_corrector_pointwise(const tsde_launch* L, co
 TSDE_EXPORT int tsde_pointwise_compile(const tsde_launch* L, const tsde_pointwise* prog) {
   return dispatch(L, [&](auto t) -> int {
     PwCompiled kc;
+    if (L->noise_type == TSDE_NOISE_GENERAL && pw_general_adjoint_of(prog)) {
+      int route;
+      const tsde_pw_adjoint* ad = pw_general_adjoint_of(prog);
+      if (!pw_general_adjoint_program(L, ad, sizeof(t), route)) return TSDE_EINVAL;
+      return pw_loaded(*prog, kPwUnitGeneralAdjoint, pw_general_adjoint_source(*ad, sizeof(t) == 8, L->m, route), kc);
+    }
     if (L->noise_type == TSDE_NOISE_GENERAL) {
       int layout;
       std::string source;
@@ -2111,6 +2413,12 @@ TSDE_EXPORT int tsde_pointwise_compile(const tsde_launch* L, const tsde_pointwis
 
 TSDE_EXPORT int64_t tsde_pointwise_source(const tsde_launch* L, const tsde_pointwise* prog, char* buf, int64_t size) {
   return dispatch(L, [&](auto t) -> int64_t {
+    if (L->noise_type == TSDE_NOISE_GENERAL && pw_general_adjoint_of(prog)) {
+      int route;
+      const tsde_pw_adjoint* ad = pw_general_adjoint_of(prog);
+      if (!pw_general_adjoint_program(L, ad, sizeof(t), route)) return TSDE_EINVAL;
+      return pw_copy_source(pw_general_adjoint_source(*ad, sizeof(t) == 8, L->m, route), buf, size);
+    }
     if (L->noise_type == TSDE_NOISE_GENERAL) {
       int layout;
       std::string source;

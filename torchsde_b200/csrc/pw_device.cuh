@@ -1038,4 +1038,130 @@ __device__ __forceinline__ void pw_adjoint_reversible_heun_steps(const PwOperand
   }
 }
 
+// Consecutive backward steps of a general- or additive-noise SDE (TSDE_PW_LAYOUT_GENERAL_ADJOINT_REVERSIBLE_HEUN), in
+// the order of the unfused sweep with kernels A and B on a GENERAL launch (general_adjoint_reversible_heun_a / _b):
+//   z1 = GRevHeunZOp{dt, backward} on (y, z, f, g0.dW);  adj_f_mid = adj_f + adj_y * half_dt;
+//   adj_g_mid_k = adj_g_k + adj_y * (0.5 dW_k), and the vjp with seeds (adj_f_mid, adj_g_mid) at (tv, z);
+//   f1, g1 at (t1, z1);  y1 = GRevHeunOp{half_dt, backward} on (y, f, f1, (g0 + g1).(0.5 dW));
+//   adj_z' = adj_z + vjp_z; adj_y1 = adj_y + 2 adj_z'; adj_z1 = -adj_z'; adj_f1 = adj_y * half_dt + adj_z' * dt;
+//   adj_g1_k = adj_y * (0.5 dW_k) + adj_z1 * (-1 dW_k)
+// No (d, m) block stays in registers: g_k at (t, z) is re-evaluated from the program whenever it is read (it is
+// deterministic, so it equals the g the unfused step stored), and adj_g is carried as kernel B's rank-2 form: per lane
+// (ra, rb) = (adj_y, adj_z1) of the previous step, per thread its increments wp.  Only the chunk's first step reads g0
+// and adj_g from memory; the chunk stores both once at its end.  `Prog` (pw_general_adjoint_source in pointwise.cu)
+// runs each channel pass.  A per-channel contribution is added to its (rows, d, m) partial at every step by the thread
+// that owns the element; a (rows, d) one is summed in registers and added to its partial once, as for diagonal noise.
+template <typename T, int SRC, typename Prog>
+__device__ __forceinline__ void pw_general_adjoint_reversible_heun_steps(const PwOperands<T>& ops, const PwAdjP<T>& p,
+                                                                         const NoiseP<T>& nz,
+                                                                         const PwAdjSteps<T>& st) {
+  PwQuad c;
+  int64_t Q, row, q;
+  pw_locate(p.base, c, Q, row, q);
+  const Key key = load_key(nz.key);
+  Prog prog;
+  T y[4], z[4], f[4], ay[4], af[4], az[4], ra[4], rb[4], acc[Prog::NP][4], nn[Prog::NN][4], wp[4 * Prog::MQ];
+  const T* tv = p.base.t0;  // the time of z, at which nn holds the forward (rows, d) values
+  for (int j = 0; j < st.n; ++j) {
+    const PwAdjStep<T>& s = st.s[j];
+    NoiseP<T> n = nz;  // this step's cell
+    n.cell_id = s.cell;
+    n.sqrt_h = s.sqrt_h;
+    T w[4 * Prog::MQ];
+    pw_general_noise<T, SRC, Prog::MQ>(n, key, row, w);
+    if (j == 0) {  // the first increments are drawn while the previous kernel drains; the rest is read after the wait
+      asm volatile("griddepcontrol.wait;" ::: "memory");
+      if (Q >= p.base.nquads) return;
+      load_quad(p.in[kAdjY], c.base, c.vec, c.nvalid, y);
+      load_quad(p.in[kAdjZ], c.base, c.vec, c.nvalid, z);
+      load_quad(p.in[kAdjF], c.base, c.vec, c.nvalid, f);
+      load_quad(p.in[kAdjAdjY], c.base, c.vec, c.nvalid, ay);
+      load_quad(p.in[kAdjAdjF], c.base, c.vec, c.nvalid, af);
+      load_quad(p.in[kAdjAdjZ], c.base, c.vec, c.nvalid, az);
+      prog.load(ops, c);
+      T f0[4];
+      prog.fwd(ops, c, tv, z, nn, f0);
+#pragma unroll
+      for (int k = 0; k < Prog::NP; ++k)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) acc[k][i] = T(0);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) ra[i] = rb[i] = T(0);
+#pragma unroll
+      for (int k = 0; k < 4 * Prog::MQ; ++k) wp[k] = T(0);
+    }
+    const bool first = j == 0;
+    const T dt = s.dt, half_dt = T(0.5) * dt;
+    T afm[4], zc[4], vz[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) afm[i] = af[i] + ay[i] * half_dt;  // AdjAElemOp
+    prog.vjp(ops, c, tv, z, nn, w, wp, first, p.in[kAdjG], p.in[kAdjAdjG], ay, ra, rb, afm, zc, vz, acc, p.part);
+    T z1[4], f1[4], nn1[Prog::NN][4];
+    const GRevHeunZOp<T> zop{dt, 1};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const T e[3] = {y[i], z[i], f[i]}, g1[1] = {zc[i]};
+      T o[1];
+      zop.combine(e, g1, o);
+      z1[i] = o[0];
+    }
+    prog.fwd(ops, c, s.t1, z1, nn1, f1);
+    const GRevHeunOp<T> yop{half_dt, 1};
+    T wt[4 * Prog::MQ], yc[4];
+#pragma unroll
+    for (int k = 0; k < 4 * Prog::MQ; ++k) wt[k] = yop.weight(0, w[k], T(0));
+    prog.ystep(ops, c, tv, z, nn, s.t1, z1, nn1, wt, first, p.in[kAdjG], yc);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const T e[3] = {y[i], f[i], f1[i]}, g1[1] = {yc[i]};
+      T o[1];
+      yop.combine(e, g1, o);
+      y[i] = o[0];
+      const T adj_z0 = az[i] + vz[i];  // AdjBElemOp
+      ra[i] = ay[i];
+      af[i] = ay[i] * half_dt + adj_z0 * dt;
+      ay[i] = ay[i] + T(2) * adj_z0;
+      az[i] = -adj_z0;
+      rb[i] = az[i];
+      z[i] = z1[i];
+      f[i] = f1[i];
+#pragma unroll
+      for (int k = 0; k < Prog::NN; ++k) nn[k][i] = nn1[k][i];
+    }
+#pragma unroll
+    for (int k = 0; k < 4 * Prog::MQ; ++k) wp[k] = w[k];
+    tv = s.t1;
+    if (s.out >= 0) {  // adjoint.py:114-116
+      T gy[4];
+      load_quad(p.ys + s.out * p.plane, c.base, c.vec, c.nvalid, y);
+      load_quad(p.gys + s.out * p.plane, c.base, c.vec, c.nvalid, gy);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) ay[i] = ay[i] + gy[i];
+    }
+  }
+  store_quad(p.out[kAdjY], c.base, c.vec, c.nvalid, y);
+  store_quad(p.out[kAdjZ], c.base, c.vec, c.nvalid, z);
+  store_quad(p.out[kAdjF], c.base, c.vec, c.nvalid, f);
+  store_quad(p.out[kAdjAdjY], c.base, c.vec, c.nvalid, ay);
+  store_quad(p.out[kAdjAdjF], c.base, c.vec, c.nvalid, af);
+  store_quad(p.out[kAdjAdjZ], c.base, c.vec, c.nvalid, az);
+  prog.gstore(ops, c, tv, z, nn, p.out[kAdjG]);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    if (j >= c.nvalid) continue;
+#pragma unroll
+    for (int k = 0; k < Prog::M; ++k)  // launch_outer (tableau_general.cu): adj_y (x) (0.5 dW) + adj_z1 (x) (-1 dW)
+      p.out[kAdjAdjG][(c.base + j) * Prog::M + k] = ra[j] * (T(0.5) * wp[k]) + rb[j] * (T(-1) * wp[k]);
+  }
+#pragma unroll
+  for (int k = 0; k < Prog::NP; ++k) {
+    if (!p.part[k] || Prog::pc(k)) continue;  // (NP is 1 for a program without parameters)
+    T v[4];
+    load_quad(p.part[k], c.base, c.vec, c.nvalid, v);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) v[i] = v[i] + acc[k][i];
+    store_quad(p.part[k], c.base, c.vec, c.nvalid, v);
+  }
+}
+
 }  // namespace tsde
